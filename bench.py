@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- keyframes/sec of the loop-closure front-end and pose-graph solve ms on B200.
+"""bench.py -- keyframes/sec of the loop-closure front-end and pose-graph solve ms on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one batch of KF_PER_STEP = 10 four-view fisheye keyframes through the hot path (BASELINE.json config C3 per
@@ -19,6 +19,10 @@ timed once per run on every rank and reported as `solve_ms`.
 `--impl reference`: the reference's CPU path restated by oracle/ (torch CPU SuperPoint/NetVLAD with all host threads,
 numpy scan, cross-check matcher, scipy sparse LM) -- the reference itself cannot be built here (DESIGN.md).  With
 --gpus N it runs N CPU drones side by side (N processes sharing the host threads), the same weak-scaling workload.
+`--dump-outputs DIR`: after the timed steps, the keyframe records and loop results the resident path produced in its last
+step (the structs a caller of osb_frontend_extract / osb_frontend_query receives, one row per keyframe of the step) as
+DIR/<struct>_<field>.npy, float32 where the field is float32, float64 otherwise.  Inputs are seeded: two builds run with the
+same arguments can be compared output for output.
 `trt_like_baseline` (N = 1, in the main line): baseline/trt_like.py, the reference's TensorRT structure with the engines
 replaced by PyTorch/cuDNN fp16 -- batch 1, H2D + enqueue + D2H of every binding + synchronize per image, CPU
 post-processing -- timed on the same GPU and host.
@@ -72,6 +76,8 @@ def parse():
     p.add_argument("--no-trt-like", action="store_true")
     p.add_argument("--blocking-exchange", action="store_true",
                    help="N > 1: all-gather of round i between extract and ingest of round i (the r01 pipeline), for A/B")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the records / loop results of the last timed step as DIR/<name>.npy")
     p.add_argument("--cpu-drone", type=int, default=-1, help=argparse.SUPPRESS)      # internal: one CPU drone of --impl reference
     p.add_argument("--cpu-threads", type=int, default=0, help=argparse.SUPPRESS)
     return p.parse_args()
@@ -83,11 +89,12 @@ def peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # H100 SXM datasheet values (dense bf16); the sustained rate is not measured here, so it is the datasheet rate too
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM datasheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -302,7 +309,7 @@ def workload_config(args, world, keyframes_per_step=KF_PER_STEP):
             "keyframes_per_step": keyframes_per_step, "distinct_keyframes": POOL,
             "images_per_keyframe": 2 * N_DIRS, "db_rows": args.db_rows, "max_kpts": MAX_NUM, "sp_thres": 0.015,
             "parallelism": f"drone-per-GPU x{world}" + (" + 1 NCCL all-gather of the keyframe record per step" if world > 1 else ""),
-            "l2_note": "per-step working set (activations ~1.3 GB + DB 164 MB) exceeds the 126 MB L2; no explicit flush"}
+            "l2_note": "per-step working set (activations ~1.3 GB + DB 164 MB) exceeds the 50 MB L2; no explicit flush"}
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -386,17 +393,28 @@ def run_ours(args):
         sw.exchange_async(rec.data_ptr(), gath2[b].data_ptr(), st)
         pending[0] = True
 
-    def keyframe_resident(i):
+    # the resident path writes keyframe k of a step into slot k of a ring of records and loop results, so that after the
+    # timed region the ring holds what the last step computed (--dump-outputs) without any extra work inside it.  N > 1
+    # keeps its two exchange buffers; there --dump-outputs copies the record after each keyframe of the last step.
+    last_step = args.warmup + args.steps - 1
+    rec_ring = torch.zeros((KF_PER_STEP, lib.RECORD_BYTES), dtype=torch.uint8, device="cuda")
+    res_ring = torch.zeros((KF_PER_STEP, lib.RESULT_BYTES), dtype=torch.uint8, device="cuda")
+
+    def keyframe_resident(i, capture=False):
         j = i % POOL
+        res = res_ring[i % KF_PER_STEP]
         if world > 1:
             rec = rec2[i & 1]
             fe.extract(dev_up[j].data_ptr(), dev_dn[j].data_ptr(), i, rec.data_ptr(), st, device_images=True)
             swarm_round(i, rec)
-            fe.query(rec.data_ptr(), res_dev.data_ptr(), st)
+            fe.query(rec.data_ptr(), res.data_ptr(), st)
+            if capture and args.dump_outputs:
+                rec_ring[i % KF_PER_STEP].copy_(rec)
         else:
-            fe.extract(dev_up[j].data_ptr(), dev_dn[j].data_ptr(), i, rec_dev.data_ptr(), st, device_images=True)
-            fe.ingest_own(rec_dev.data_ptr(), st)
-            fe.query(rec_dev.data_ptr(), res_dev.data_ptr(), st)
+            rec = rec_ring[i % KF_PER_STEP]
+            fe.extract(dev_up[j].data_ptr(), dev_dn[j].data_ptr(), i, rec.data_ptr(), st, device_images=True)
+            fe.ingest_own(rec.data_ptr(), st)
+            fe.query(rec.data_ptr(), res.data_ptr(), st)
 
     def keyframe_e2e(i):
         j = i % POOL
@@ -412,7 +430,7 @@ def run_ours(args):
 
     def step_resident(i):                 # one step = one batch of KF_PER_STEP keyframes
         for k in range(KF_PER_STEP):
-            keyframe_resident(i * KF_PER_STEP + k)
+            keyframe_resident(i * KF_PER_STEP + k, capture=i == last_step)
 
     def step_e2e(i):
         for k in range(KF_PER_STEP):
@@ -452,6 +470,8 @@ def run_ours(args):
     sampler = ClockSampler(local_rank)
     sampler.start()
     ms_total, launches = timed(step_resident, args.steps, args.warmup, 0, sampler)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, lib, rec_ring.cpu().numpy(), res_ring.cpu().numpy())
     # host cost of ENQUEUEING a keyframe with an empty launch queue (8 keyframes right after a synchronisation: no back-pressure)
     fe.finish(st); barrier()
     th = time.perf_counter()
@@ -521,7 +541,7 @@ def run_ours(args):
                     "api": "osb_swarm_* (C ABI; exchange_us times the blocking ncclAllGather form)"}
 
     # ---- rooflines ----
-    # dominant kernel: the conv1b launch of conv_umma_kernel<64> (43 % of the network's FLOPs).  Its own duration comes
+    # dominant kernel: the conv1b launch of conv_umma_kernel<64> (43 % of the network's FLOPs; conv1a is fused into it).  Its own duration comes
     # from CUDA events recorded around every layer launch on the library's stream (osb_superpoint_layer_ms).
     GMAC = {"conv1a": 0.17695, "conv1b+pool": 11.3246, "conv2a": 2.83116, "conv2b+pool": 2.83116, "conv3a": 1.41558,
             "conv3b+pool": 2.83116, "conv4a": 0.70779, "conv4b": 0.70779, "convPa": 1.41558, "convPb": 0.07987,
@@ -537,22 +557,17 @@ def run_ours(args):
     layer_tflops = {k: (2 * GMAC[k] * 2 * N_DIRS / v if v > 0 else None) for k, v in layer_ms.items()}
     conv_ms = float(sum(layer_ms.values()))      # the 12 conv launches of a standalone handle (no overlapped work)
     conv_tflops = 2 * N_DIRS * SP_GFLOP_PER_IMAGE / conv_ms  # GFLOP / ms = TFLOP/s
-    dom = "conv1b+pool"        # with the default fused first layers this launch is conv1a + conv1b + pool
+    dom = "conv1b+pool"        # with OSB_SP_FUSE1=1 this launch is conv1a + conv1b + pool
     dom_gmac = GMAC["conv1a"] + GMAC["conv1b+pool"] if layer_ms["conv1a"] < 0.02 else GMAC["conv1b+pool"]
     dom_tflops = 2 * dom_gmac * 2 * N_DIRS / layer_ms[dom]
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath))
     scan_ms = stages["db_scan"]
     scan_bytes = (db_rows_now + db_rows_remote) * 4096 * 4.0        # local + remote database, each row read once
     scan_gbs = scan_bytes / scan_ms / 1e6
-    roofline = {"kernel": "conv1_fused_kernel (conv1a 1->64 computed in the SM by 6 producer warps (lane = pixel, constant-bank weights, FFMA2) + conv1b 64->64 3x3 @640x480 on "
-                          "tcgen05 from ONE shared-memory halo copy (9 descriptor views) + fused 2x2 max-pool; split-fp16: hi*hi + "
-                          "hi*lo as one MMA of width 128, lo*hi as one of width 64 per K step)",
+    roofline = {"kernel": "conv_umma_kernel<64, RES> (conv1b 64->64 3x3 @640x480 on wgmma, weights resident, fused 2x2 max-pool; "
+                          "with OSB_SP_FUSE1=1 conv1a is computed in the same launch; split-fp16: hi*hi, hi*lo and lo*hi as three "
+                          "MMAs of width 64 per K step)",
                 "bound": "tensor", "achieved": dom_tflops, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                 "frac": dom_tflops / pk["bf16_tflops_sustained"],
-                "traffic": (traffic or {}).get("conv1_fused_dram_bytes_per_launch"),
                 "algorithmic": f"{2 * N_DIRS} images x {2 * dom_gmac:.3f} GFLOP (conv1a + conv1b, fp32-equivalent MACs x 2); the "
                                "tensor pipes execute 3x conv1b's share as fp16 MACs for fp32-level accuracy",
                 "algorithmic_dram_bytes": 2 * N_DIRS * (W * H + (W // 2) * (H // 2) * 64 * 4),
@@ -562,10 +577,10 @@ def run_ours(args):
     roofline_stack = {"what": "whole SuperPoint conv stack (12 conv launches, per-layer CUDA-event times of a standalone handle)", "achieved": conv_tflops,
                       "unit": "TFLOP/s", "frac": conv_tflops / pk["bf16_tflops_sustained"], "ms": conv_ms,
                       "layer_ms": layer_ms, "layer_tflops": layer_tflops, "keypoint_counts_image0": kp_counts}
-    scan_kernel = "db_scan_coop_kernel<1>" if db_rows_now <= 2 * 148 * 64 else "db_scan_kernel<1,4>"
+    n_sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
+    scan_kernel = "db_scan_coop_kernel<1>" if db_rows_now <= 2 * n_sms * 64 else "db_scan_kernel<1,4>"
     roofline_match = {"kernel": scan_kernel, "bound": "hbm", "achieved": scan_gbs, "peak": pk["hbm_gbs"],
                       "unit": "GB/s", "frac": scan_gbs / pk["hbm_gbs"],
-                      "traffic": (traffic or {}).get("db_scan_dram_bytes_per_launch"),
                       "algorithmic": f"({db_rows_now} local + {db_rows_remote} remote) rows x 16384 B", "ms": scan_ms,
                       "peak_source": pk["source"],
                       "note": "ms = the db_scan stage of a keyframe: the remote-database and the local-database scan launches "
@@ -594,7 +609,7 @@ def run_ours(args):
             gbs = rows * 16384 / ms / 1e6
             match_sweep.append({"db_rows": rows, "ms_per_search": ms, "achieved_gbs": gbs, "frac_of_hbm_peak": gbs / pk["hbm_gbs"],
                                 "note": "scan + merge launches, 1 query, k = 10; "
-                                        + ("164 MB > 126 MB L2" if rows == 10_000 else "819 MB >> L2")})
+                                        + ("164 MB > 50 MB L2" if rows == 10_000 else "819 MB >> L2")})
             idx.close(); del blk
 
     # ---- config C2: one pinhole stream, the reference's own call pattern (one synchronous inference() per image,
@@ -729,7 +744,7 @@ def run_ours(args):
                 state["solves"] += 1; state["solve_ms"].append(sm.solve_ms)
 
         fe.finish(st); barrier()
-        L.osb_set_sm_budget(148 - 16)                # the solve's cluster holds 16 SMs: keep the persistent conv grids off them
+        L.osb_set_sm_budget(torch.cuda.get_device_properties(local_rank).multi_processor_count - 16)   # the solve's cluster holds 16 SMs: keep the persistent conv grids off them
         th = threading.Thread(target=solver_loop); th.start()
         n_kf = REPLAY_KF
         t0r = time.perf_counter()
@@ -846,7 +861,7 @@ def run_ours(args):
         c1 = {"graph": f"C1: {g1['n_nodes']} nodes / {len(g1['ftype'])} factors", "solve_ms": float(np.median(c1_t)),
               "solve_wall_ms": float(np.median(c1_w)), "iterations": int(s1.iterations), "pcg_iterations": int(s1.pcg_iterations)}
         # "replicas only": R independent C5 windows solved CONCURRENTLY on one GPU, one 16-CTA cluster each (a solve uses
-        # 16 of the 148 SMs), one handle + host thread per window -- what a ground station solving for the whole swarm does
+        # 16 of the 132 SMs), one handle + host thread per window -- what a ground station solving for the whole swarm does
         replicas = None
         try:
             R = 8
@@ -930,6 +945,20 @@ def run_ours(args):
         dist.barrier()
         sw.close()
         dist.destroy_process_group()
+
+
+def dump_outputs(d: str, lib, rec_bytes: np.ndarray, res_bytes: np.ndarray):
+    """--dump-outputs: every field of the KF_PER_STEP keyframe records and loop results as DIR/<struct>_<field>.npy, one row
+    per keyframe (float32 fields stay float32, integer and double fields become float64, both exact)"""
+    os.makedirs(d, exist_ok=True)
+    for prefix, cls, raw in (("record", lib.KeyframeRecord, rec_bytes), ("loop", lib.LoopResult, res_bytes)):
+        structs = [cls.from_buffer_copy(r.tobytes()) for r in raw]
+        for name, _ in cls._fields_:
+            if name == "reserved":
+                continue
+            a = np.stack([np.ctypeslib.as_array(v) if isinstance(v, C.Array) else np.asarray(v)
+                          for v in (getattr(s, name) for s in structs)])
+            np.save(os.path.join(d, f"{prefix}_{name}.npy"), a if a.dtype == np.float32 else a.astype(np.float64))
 
 
 def _emit(line: dict):

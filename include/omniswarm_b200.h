@@ -1,7 +1,7 @@
 /*
  * omniswarm_b200.h -- C ABI of libomniswarm_b200.so
  *
- * B200-native (sm_100a) replacement for the ONE compute-heavy path of HKUST-Aerial-Robotics/Omni-swarm:
+ * H100-native (sm_90a) replacement for the ONE compute-heavy path of HKUST-Aerial-Robotics/Omni-swarm:
  * the swarm_loop keyframe front-end and the swarm_localization pose-graph solve.  The reference has no
  * plugin ABI for this path (the boundary is C++ member calls inside one process, SURVEY.md section 8b);
  * every entry point below names the reference call site it replaces (paths relative to /root/reference).
@@ -54,7 +54,7 @@ int osb_device_count(void);                /* 0 when no CUDA device is visible *
  * `weights`: float32 blob, for each layer of swarm_loop/superpoint.ipynb:143-158 in definition order
  *            (conv1a,conv1b,conv2a,conv2b,conv3a,conv3b,conv4a,conv4b,convPa,convPb,convDa,convDb):
  *            weight in PyTorch OIHW order, then bias.  1 300 865 floats.  (Replaces the .trt engine path:
- *            TensorRT engine binaries are device-specific and unusable on B200.)
+ *            TensorRT engine binaries are device-specific and not portable.)
  * `pca_comp` [64][256] row-major = components_.csv, `pca_mean` [256] = mean_.csv (superpoint_tensorrt.cpp:110-111).
  * infer():   images  [batch][height][width] uint8 (the reference asserts the size, superpoint_tensorrt.cpp:122)
  *            n_kpts  [batch]                          number of keypoints per image (<= max_num)
@@ -76,9 +76,7 @@ osb_status osb_superpoint_infer_dev(osb_superpoint* h, const uint8_t* images_dev
  *               outputs, superpoint_tensorrt.cpp:139-140) and run ONLY getKeyPoints+NMS2+computeDescriptors.
  *  read:        copy an intermediate of the last infer() back: what = 0 semi [H][W], 1 desc [256][H/8][W/8],
  *               2 confidences of the returned keypoints [max_num], 3 NMS survivor plane as float [H][W],
- *               4 keypoint kernel counters [8]: candidates, survivors, NMS rounds, 0, SM cycles of its 4 phases,
- *               5 cycle counters [16] of the fused conv1a+conv1b kernel's CTA 0 from the last infer() with profiling on
- *                 (producer wait / compute / wait, loop total, MMA wait TMEM / wait tile / issue, epilogue wait / work, tiles). */
+ *               4 keypoint kernel counters [8]: candidates, survivors, NMS rounds, 0, SM cycles of its 4 phases. */
 osb_status osb_superpoint_postprocess(osb_superpoint* h, const float* semi, const float* desc_nchw, int batch,
                                       int32_t* n_kpts, float* kpts, float* desc);
 osb_status osb_superpoint_read(osb_superpoint* h, int what, int image, float* out, size_t n_floats);

@@ -8,7 +8,7 @@ std::atomic<int> g_sm_budget{0};
 }  // namespace osb
 
 extern "C" const char* osb_last_error(void) { return osb::g_last_error.c_str(); }
-extern "C" const char* osb_version(void) { return "omniswarm_b200 0.2.0 (sm_100a)"; }
+extern "C" const char* osb_version(void) { return "omniswarm_b200 0.3.0 (sm_90a)"; }
 extern "C" int osb_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

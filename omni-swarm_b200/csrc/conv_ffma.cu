@@ -2,7 +2,7 @@
 //
 // These are the full-precision implicit-GEMM kernels of the SuperPoint / NetVLAD networks
 // (network definition: swarm_loop/superpoint.ipynb:135-205 of the reference).  They accumulate in fp32 with FFMA
-// and are what the parity tests pin the tensor-core path against; conv_umma.cu holds the tcgen05 kernels.
+// and are what the parity tests pin the tensor-core path against; conv_umma.cu holds the tensor-core (wgmma) kernels.
 #include "common.cuh"
 #include "kernels.cuh"
 

@@ -1,27 +1,33 @@
-// conv_umma.cu -- SuperPoint convolutions on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// conv_umma.cu -- SuperPoint / NetVLAD convolutions on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // Layers: swarm_loop/superpoint.ipynb:143-158 of the reference (3x3 pad 1 and 1x1 convolutions, NHWC here).
 //
-// Implicit GEMM, one CTA tile = 8 x 16 output pixels (M = 128) x all output channels (N = Cout, 64..256):
-//   * A operand: for every filter tap (ky,kx) and every 64-channel slab, ONE TMA box {64 ch, 16 x, 8 y, 1 image}
-//     fetched at the tap-shifted coordinate; out-of-image elements are zero-filled by the TMA unit, which is the
-//     convolution's zero padding.  The box lands in shared memory as 128 rows x 128 B with the 128-byte swizzle,
-//     i.e. exactly the canonical K-major SWIZZLE_128B UMMA layout (im2col staging is done by the copy engine).
+// Implicit GEMM, one CTA tile = 8 x 16 output pixels (M = 128) x N output channels (N = 64, 80 or 128; layers of 256 / 512
+// channels run as 2 / 4 work items of 128 channels per tile):
+//   * A operand: for every horizontal filter tap kx and every 64-channel slab, ONE TMA box {64 ch, 16 x, 8 + 2 y, 1 image}
+//     fetched at the kx-shifted coordinate; out-of-image elements are zero-filled by the TMA unit, which is the
+//     convolution's zero padding.  The box lands in shared memory as one 128-byte row per pixel with the 128-byte swizzle,
+//     i.e. exactly the canonical K-major SWIZZLE_128B wgmma layout (im2col staging is done by the copy engine).  The three
+//     vertical taps ky read the same box from pixel row ky on: + ky * 2048 bytes, a multiple of the 1024-byte swizzle atom.
 //   * B operand: the weight slab [N][64] of the same tap, K-major SWIZZLE_128B, by TMA.
-//   * D: fp32 accumulators in TMEM (128 lanes x N columns), double buffered so the epilogue of tile t overlaps
-//     the MMAs of tile t+1.
+//   * D: fp32 accumulators in the registers of two consumer warpgroups, 64 pixels each.  Warpgroup g reads the 8-pixel core
+//     matrices at columns 8g .. 8g+7 of the eight tile rows (descriptor stride = one pixel row), so the two accumulator
+//     rows a thread holds are vertically adjacent pixels of one column: the fused 2x2 max-pool is one max in the thread
+//     and one shuffle.
 // Precision: parity with the fp32 oracle needs ~1e-6 relative error, which fp16/bf16 operands cannot give.  Every
 // fp32 operand x is carried as TWO fp16 planes  hi = fp16(s*x), lo = fp16(s*x - hi)  (s a power of two, exact), and
 // each K step computes the three products  hi*hi + lo*hi + hi*lo  (the dropped lo*lo term is 2^-22 relative): hi*hi goes
-// to a MAIN accumulator, the two cross products to a CROSS accumulator (see the truncation note at the MMA issuer), and
-// for 2N <= 256 one MMA of width 2N covers hi*hi and hi*lo at once.  Both planes together are 4 bytes per element -- the
-// same HBM/L2 footprint as fp32 activations -- and the fp16 MACs cost 1.5x one TF32 MMA.  Measured against the oracle:
-// see tests/test_gpu_superpoint.py.
-// Warp roles (384 threads): warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane each), warp 2 = TMEM
-// allocator, warps 4-11 = epilogue (tcgen05.ld -> bias/ReLU -> re-split -> NHWC stores; two warps per TMEM lane quarter).
-// Persistent over tiles.
+// to a MAIN accumulator, the two cross products to a CROSS accumulator whose magnitude -- and rounding error -- is 2^-11
+// of the main one; the epilogue adds them in fp32.  The weight slot is [W_hi (N rows) | W_lo (N rows)]; per K step three
+// MMAs of width N write two register fragments of the same shape (hi*hi -> main, hi*lo and lo*hi -> cross), disjoint so
+// that the compiler keeps the wgmma pipeline asynchronous.  Both planes together are 4 bytes per element -- the same
+// HBM/L2 footprint as fp32 activations.  Measured against the oracle: see tests/test_gpu_superpoint.py.
+// Warp roles (384 threads): warpgroups 0-1 = MMA + epilogue, warpgroup 2 = producer (one elected thread issues the TMA
+// copies; in the first-layers form, FIRST below, its 128 threads compute conv1a into the A slots instead).  Persistent over
+// tiles; the producer runs up to two A boxes and the weight ring ahead of the MMAs.
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <type_traits>
 #include "common.cuh"
 #include "kernels.cuh"
 #include "conv_umma.cuh"
@@ -31,28 +37,31 @@ namespace osb {
 
 constexpr int UM_TH = 8, UM_TW = 16;            // output tile (pixels)
 constexpr int UM_KC = 64;                       // fp16 channels per K slab (= 128 bytes = one swizzle row)
+constexpr int UM_ROW = UM_TW * 128;             // bytes of one pixel row of an A box (2 swizzle atoms)
 
-// Shared-memory plan.  For a 3x3 layer ONE A box per (kx, 64-channel slab) carries 10 rows (tile + vertical halo):
-// the three vertical taps ky = 0,1,2 read it at row offsets ky*16 rows = ky*2048 bytes -- a multiple of the 1024-byte
-// swizzle atom, so the same SWIZZLE_128B descriptor applies with only the start address moved.  That cuts the
-// activation traffic from 9 to 3.75 tile-loads per tile (L2 -> shared memory is what bounds this kernel).
-// The weights of each tap stream through their own ring.
-constexpr int UM_A_SLOT = (UM_TH + 2) * UM_TW * 128;   // 20 KB per plane: 10 rows x 16 px x 128 B
+// Shared-memory plan.  For a 3x3 layer ONE A box per (kx, 64-channel slab) carries 10 rows (tile + vertical halo), read
+// by the three vertical taps; that cuts the activation traffic from 9 to 3.75 tile-loads per tile.  The weights of each
+// tap stream through their own ring.
+constexpr int UM_A_SLOT = (UM_TH + 2) * UM_ROW;        // 20 KB per plane: 10 rows x 16 px x 128 B
 constexpr int UM_A_SLOTS = 2;
-constexpr int UM_THREADS = 384;                 // 12 warps: TMA, MMA, TMEM allocator, (idle), 8 x epilogue
+// threads: warpgroups 0 and 1 issue the MMAs and run the epilogue, warpgroup 2 is the producer.  Launched at 168 registers
+// per thread; the producer hands registers to the MMA warpgroups with setmaxnreg (TMA producer 40 -> consumers 232; conv1a
+// producers 96 -> consumers 200), so that a 128-register accumulator fragment fits with the MMA pipeline in flight.
+constexpr int UM_CONSUMERS = 256;
+constexpr int um_threads(bool) { return UM_CONSUMERS + 128; }
+template <bool FIRST> struct UmRegs { static constexpr int PRODUCER = FIRST ? 96 : 40, CONSUMER = FIRST ? 200 : 232; };
+static_assert(128 * UmRegs<false>::PRODUCER + 256 * UmRegs<false>::CONSUMER <= 65536, "register file");
+static_assert(128 * UmRegs<true>::PRODUCER + 256 * UmRegs<true>::CONSUMER <= 65536, "register file");
 // RES = true (64 -> 64 channel 3x3 layers: conv1b, conv2a, conv2b = 65 % of the network's FLOPs): the 9 taps' weight
-// planes (144 KB) stay resident in shared memory for the CTA's whole life instead of streaming through a ring, which
-// removes more than half of the remaining L2 -> shared-memory traffic.
+// planes (144 KB) stay resident in shared memory for the CTA's whole life instead of streaming through a ring.
 template <int N, bool RES>
 struct UmmaCfg {
   static constexpr int B_BYTES = N * 128;                        // one weight plane of one tap / slab
   static constexpr int B_SLOT = 2 * B_BYTES;                     // hi + lo
-  static constexpr int B_SLOTS = RES ? 9 : (N <= 64) ? 6 : (N <= 80) ? 5 : (N <= 128) ? 4 : 2;
+  static constexpr int B_SLOTS = RES ? 9 : (N <= 64) ? 6 : (N <= 80) ? 5 : 4;
   static constexpr int A_RING = UM_A_SLOTS * 2 * UM_A_SLOT;      // 80 KB
-  // two fp32 accumulators per tile (see the precision note in the kernel): 2N TMEM columns per buffer
-  static constexpr int NBUF = (4 * N <= 512) ? 2 : 1;
-  static constexpr int TMEM_COLS = (2 * N * NBUF <= 128) ? 128 : (2 * N * NBUF <= 256) ? 256 : 512;
   static constexpr int SMEM_BYTES = A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
 };
 
 struct UmmaArgs {
@@ -68,19 +77,33 @@ struct UmmaArgs {
   float inv_scale;         // 1 / (act_scale * w_scale)
   float out_scale;         // scale of the stored fp16 planes
   int relu;                // 0 none, 1 ReLU, 2 ReLU6
-  int n_off;               // first output channel of this launch (Cout > 256 runs as several N <= 256 passes)
+  int n_off;               // first output channel of this launch
   int pool;                // 1: fused 2x2 max-pool, the planes written are [B][H/2][W/2][C]
   int n_split;             // a layer wider than the kernel's N runs as n_split work items per tile (N channels each)
   int epi;                 // 0: bias/act/pool + store; 1: detector head -- softmax over 65 logits, drop the dustbin,
                            //    8x8 pixel shuffle straight into the heat map `out_f32` ([B][8H][8W])
+  const uint8_t* img;      // FIRST only: u8 images [B][H][W]
+  float alpha;             // FIRST only: (float)(1/255), u8 -> f32 as cv::Mat::convertTo does (superpoint_tensorrt.cpp:127)
 };
+struct NoConv1a {};
 
-template <int N, bool RES, bool SPLIT>
-__global__ void __launch_bounds__(UM_THREADS, 1)
+__device__ __forceinline__ void st_shared_128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+
+// FIRST = true: SuperPoint's first two layers in one kernel.  The A slots are not loaded but COMPUTED: the producer
+// warpgroup evaluates conv1a (1 -> 64, 3x3, ReLU) from the u8 image for the 10 x 16 pixels of each kx-shifted box and writes
+// them, split and swizzled, where TMA would have put conv1a's planes; conv1a's output never reaches HBM.  Lane = pixel, so
+// every lane of a warp uses the same weight: the 576 weights + 64 biases are a kernel parameter read through the constant
+// bank.  The fp32 FMAs run in the order of conv_first_split_kernel, so the fused and unfused paths are bit-identical.
+template <int N, bool RES, bool SPLIT, bool FIRST>
+__global__ void __launch_bounds__(um_threads(FIRST), 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-                 const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
+                 const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P,
+                 const __grid_constant__ typename std::conditional<FIRST, Conv1aW, NoConv1a>::type W1) {
   using Cfg = UmmaCfg<N, RES>;
-  constexpr int AS = UM_A_SLOTS, BS = Cfg::B_SLOTS, NBUF = Cfg::NBUF;
+  constexpr int AS = UM_A_SLOTS, BS = Cfg::B_SLOTS;
+  static_assert(!FIRST || (N == 64 && RES && !SPLIT), "the first-layers form is the 64 -> 64 3x3 layer");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t b_base = smem_base + Cfg::A_RING;
@@ -89,44 +112,31 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
   auto a_empty = [&](int s) { return bar_base + 8u * (AS + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (2 * AS + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (2 * AS + BS + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * AS + 2 * BS + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * AS + 2 * BS + 2 + a); };
-  __shared__ uint32_t tmem_base_slot;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
   const int n_tiles = P.B * tiles_x * tiles_y;
   // work item = (tile, channel block): items of one tile are adjacent, so concurrent CTAs share its activations in L2
   const int n_split = SPLIT ? P.n_split : 1;          // compile-time 1 for ordinary layers: no div / mod per item
   const int n_items = n_tiles * n_split;
   const int halo = P.ks / 2;
-  const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_TW * 128;   // bytes of one A plane box
+  const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_ROW;   // bytes of one A plane box
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < AS; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < BS; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
-    // (with NBUF == 1 only index 0 is used; with RES the b_full barriers are filled once and b_empty stays unused)
+    // the empty barriers count one arrival per consumer warpgroup; with RES the b_full barriers are filled once
+    for (int s = 0; s < AS; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 2); }
+    for (int s = 0; s < BS; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                 "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
   // programmatic dependent launch: the next layer's CTAs may be scheduled as ours retire (they still wait for this whole
   // grid in their own griddepcontrol.wait before touching activations)
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0 && elect_one()) {
-    // ===================== TMA producer =====================
-    int as = 0; uint32_t aph = 0;
-    int bs = 0; uint32_t bph = 0;
-    if (RES) {
+  if (threadIdx.x >= UM_CONSUMERS) {
+    const int pt = threadIdx.x - UM_CONSUMERS;             // producer thread
+    setmaxnreg_dec<UmRegs<FIRST>::PRODUCER>();
+    if (RES && pt < 32 && elect_one()) {
       // all 9 taps (one 64-channel slab) once: slot t holds tap t.  Issued BEFORE the dependency wait: weights are
       // constants, so under programmatic dependent launch they stream in while the previous layer is still draining.
       for (int t = 0; t < 9; ++t) {
@@ -138,230 +148,245 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
     }
     // the activations are the previous kernel's output: wait for the whole grid we depend on (no-op without PDL)
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
-      const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
-      const int x0 = tx * UM_TW, y0 = ty * UM_TH;
-      for (int kx = 0; kx < P.ks; ++kx) {
-        for (int cs = 0; cs < P.cin_slabs; ++cs) {
-          // activation box: tile rows + vertical halo at the kx-shifted column, shared by the ks vertical taps
+    if constexpr (FIRST) {
+      // ===================== conv1a producers (128 threads, thread = pixel of the box) =====================
+      const int tid = pt;
+      int as = 0; uint32_t aph = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+        const uint8_t* ib = P.img + (size_t)b * P.H * P.W;
+        for (int kx = 0; kx < 3; ++kx) {
           mbar_wait(a_empty(as), aph ^ 1);
           const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
-          mbar_expect_tx(a_full(as), 2 * a_box_bytes);
-          tma_load_4d(sa, &tm_a_hi, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
-          tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
+          for (int p = tid; p < (UM_TH + 2) * UM_TW; p += 128) {
+            // box pixel p = conv1b input pixel (iy, ix); outside the image it is conv1b's zero padding
+            const int iy = ty * UM_TH - 1 + p / UM_TW, ix = tx * UM_TW + kx - 1 + p % UM_TW;
+            const bool valid = iy >= 0 && iy < P.H && ix >= 0 && ix < P.W;
+            float in[9];
+#pragma unroll
+            for (int t = 0; t < 9; ++t) {
+              const int gy = iy + t / 3 - 1, gx = ix + t % 3 - 1;
+              in[t] = (valid && gy >= 0 && gy < P.H && gx >= 0 && gx < P.W)
+                          ? __fmul_rn(__uint2float_rn((uint32_t)__ldg(ib + (size_t)gy * P.W + gx)), P.alpha) : 0.f;
+            }
+            const uint32_t row_hi = sa + (uint32_t)p * 128u, row_lo = row_hi + UM_A_SLOT;
+            const uint32_t ph = (uint32_t)p & 7u;                  // swizzle phase of the row (slots are 1024-aligned)
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+              uint32_t h[4], l[4];
+#pragma unroll
+              for (int j2 = 0; j2 < 4; ++j2) {
+                const int c = g * 8 + 2 * j2;
+                float a0 = W1.b[c], a1 = W1.b[c + 1];              // bias first: 9 taps accumulate onto it
+#pragma unroll
+                for (int t = 0; t < 9; ++t) {
+                  a0 = fmaf(in[t], W1.w[t][c], a0);
+                  a1 = fmaf(in[t], W1.w[t][c + 1], a1);
+                }
+                const float s0 = fmaxf(a0, 0.f), s1 = fmaxf(a1, 0.f);
+                const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
+                const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
+                h[j2] = valid ? ((uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16)) : 0u;
+                l[j2] = valid ? ((uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16)) : 0u;
+              }
+              st_shared_128(row_hi + (((uint32_t)g ^ ph) << 4), h[0], h[1], h[2], h[3]);
+              st_shared_128(row_lo + (((uint32_t)g ^ ph) << 4), l[0], l[1], l[2], l[3]);
+            }
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
+          asm volatile("bar.sync 1, 128;" ::: "memory");
+          if (tid == 0) mbar_arrive(a_full(as));
           if (++as == AS) { as = 0; aph ^= 1; }
-          for (int ky = 0; ky < P.ks && !RES; ++ky) {
-            mbar_wait(b_empty(bs), bph ^ 1);
-            const uint32_t sb = b_base + bs * Cfg::B_SLOT;
-            mbar_expect_tx(b_full(bs), Cfg::B_SLOT);
-            tma_load_3d(sb, &tm_w_hi, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
-            tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
-            if (++bs == BS) { bs = 0; bph ^= 1; }
+        }
+      }
+    } else if (pt < 32 && elect_one()) {
+      // ===================== TMA producer =====================
+      int as = 0; uint32_t aph = 0;
+      int bs = 0; uint32_t bph = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
+        const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+        const int x0 = tx * UM_TW, y0 = ty * UM_TH;
+        for (int kx = 0; kx < P.ks; ++kx) {
+          for (int cs = 0; cs < P.cin_slabs; ++cs) {
+            // activation box: tile rows + vertical halo at the kx-shifted column, shared by the ks vertical taps
+            mbar_wait(a_empty(as), aph ^ 1);
+            const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+            mbar_expect_tx(a_full(as), 2 * a_box_bytes);
+            tma_load_4d(sa, &tm_a_hi, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
+            tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
+            if (++as == AS) { as = 0; aph ^= 1; }
+            for (int ky = 0; ky < P.ks && !RES; ++ky) {
+              mbar_wait(b_empty(bs), bph ^ 1);
+              const uint32_t sb = b_base + bs * Cfg::B_SLOT;
+              mbar_expect_tx(b_full(bs), Cfg::B_SLOT);
+              tma_load_3d(sb, &tm_w_hi, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
+              tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
+              if (++bs == BS) { bs = 0; bph ^= 1; }
+            }
           }
         }
       }
     }
-  } else if (warp == 1 && elect_one()) {
-    // ===================== MMA issuer =====================
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D = f32 (1 << 4), A = B = f16 (0), K-major both,
-    // N >> 3 at bit 17, M >> 4 at bit 24
-    constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    constexpr bool WIDE = (2 * N <= 256);
-    constexpr uint32_t idesc2 = (1u << 4) | ((uint32_t)((2 * N) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    // Precision: the tensor core TRUNCATES its fp32 accumulator after every MMA (measured: ~1e-5 relative per layer when
-    // all three products of the split share one accumulator).  The exact-in-fp32 hi*hi products therefore go to a MAIN
-    // accumulator (one truncation per K=16 step) and the two small cross products lo*hi, hi*lo to a second, CROSS
-    // accumulator whose magnitude -- and truncation error -- is 2^-11 of the main one; the epilogue adds them in fp32.
+  } else {
+    // ===================== MMA + epilogue (two warpgroups, 64 pixels each) =====================
+    setmaxnreg_inc<UmRegs<FIRST>::CONSUMER>();
+    const int cw = threadIdx.x >> 7;                         // warpgroup: tile columns 8cw .. 8cw+7
+    const int wq = (threadIdx.x >> 5) & 3;                   // warp of the warpgroup: tile rows 2wq, 2wq+1
+    const int col = lane >> 2, t4 = lane & 3;                // pixel column in the core matrix, channel pair in a group of 8
+    const bool signaller = (threadIdx.x & 127) == 0;
     int as = 0; uint32_t aph = 0;
     int bs = 0; uint32_t bph = 0;
-    int acc = 0; uint32_t acc_phase = 0;
     if (RES)
       for (int t = 0; t < 9; ++t) mbar_wait(b_full(t), 0);
+    // buffers are released once the MMAs that read them have retired: one warpgroup arrival on each empty barrier.  The MMAs
+    // of one vertical tap form one commit group, and a group's buffers (its weight slot; the A box after its last tap) are
+    // released when the NEXT group has been issued and this one has completed -- so a warpgroup holds at most two weight
+    // slots and two A boxes at any time, whatever the ring sizes.
+    auto release = [&](int a_slot, int b_slot) {
+      if (!signaller) return;
+      if (a_slot >= 0) mbar_arrive(a_empty(a_slot));
+      if (b_slot >= 0) mbar_arrive(b_empty(b_slot));
+    };
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_main = tmem_base + (uint32_t)(acc * 2 * N);
-      const uint32_t d_cross = d_main + (uint32_t)N;
-      uint32_t first = 1;
+      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
+      // two fragments of the same shape (N/2 registers each): main = hi*hi, cross = hi*lo + lo*hi.  Disjoint register sets --
+      // an MMA into part of another MMA's fragment would make the compiler serialize the wgmma pipeline
+      float acc[N / 2], cross[N / 2];
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) { acc[i] = 0.f; cross[i] = 0.f; }
+      uint32_t scale_d = 0;
+      int pend_a = -1, pend_b = -1;                          // buffers of the last committed group
       for (int kx = 0; kx < P.ks; ++kx) {
         for (int cs = 0; cs < P.cin_slabs; ++cs) {
           mbar_wait(a_full(as), aph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+          const uint32_t sa = smem_base + as * (2 * UM_A_SLOT) + cw * 1024;
           for (int ky = 0; ky < P.ks; ++ky) {
             uint32_t sb;
+            int b_slot = -1;
             if (RES) {
               sb = b_base + (ky * 3 + kx) * Cfg::B_SLOT;
             } else {
               mbar_wait(b_full(bs), bph);
-              tc_fence_after();
               sb = b_base + bs * Cfg::B_SLOT;
+              b_slot = bs;
+              if (++bs == BS) { bs = 0; bph ^= 1; }
             }
-            // vertical tap ky reads the box from tile row ky on: + ky * 16 px * 128 B = ky * 2048 B (2 swizzle atoms)
-            const uint64_t a_hi = umma_desc_sw128(sa + ky * (UM_TW * 128));
-            const uint64_t a_lo = umma_desc_sw128(sa + UM_A_SLOT + ky * (UM_TW * 128));
-            const uint64_t b_hi = umma_desc_sw128(sb), b_lo = umma_desc_sw128(sb + Cfg::B_BYTES);
+            // vertical tap ky reads the box from pixel row ky on; core matrices one pixel row (2048 B) apart
+            const uint64_t a_hi = wgmma_desc_sw128(sa + ky * UM_ROW, UM_ROW);
+            const uint64_t a_lo = wgmma_desc_sw128(sa + UM_A_SLOT + ky * UM_ROW, UM_ROW);
+            const uint64_t b_hi = wgmma_desc_sw128(sb, 1024), b_lo = wgmma_desc_sw128(sb + Cfg::B_BYTES, 1024);
+            // the warpgroup is converged again after the barrier waits: fence the accumulators here, right before the
+            // tap's MMAs, so that no compiler-inserted fence lands on a divergent path and serializes the MMA pipeline
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+            wgmma_fence();
 #pragma unroll
             for (int k = 0; k < UM_KC / 16; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);     // advance 16 fp16 = 32 bytes inside the swizzle row
-              const uint32_t accum = (first && k == 0) ? 0u : 1u;
-              if (WIDE) {
-                // the weight slot is [W_hi (N rows) | W_lo (N rows)] and the accumulators are [main (N cols) | cross (N cols)]:
-                // ONE MMA of width 2N computes hi*hi -> main and hi*lo -> cross, fetching the activation operand once
-                // (at N = 64 the instruction is bound by shared-memory operand bandwidth, not by the tensor pipe)
-                umma_f16(d_main, a_hi + adv, b_hi + adv, idesc2, accum);
-                umma_f16(d_cross, a_lo + adv, b_hi + adv, idesc, 1u);
-              } else {
-                umma_f16(d_main, a_hi + adv, b_hi + adv, idesc, accum);
-                umma_f16(d_cross, a_lo + adv, b_hi + adv, idesc, accum);
-                umma_f16(d_cross, a_hi + adv, b_lo + adv, idesc, 1u);
-              }
+              Wgmma<N>::mma(acc, a_hi + adv, b_hi + adv, scale_d);        // hi*hi -> main
+              Wgmma<N>::mma(cross, a_hi + adv, b_lo + adv, scale_d);      // hi*lo -> cross
+              Wgmma<N>::mma(cross, a_lo + adv, b_hi + adv, 1u);           // lo*hi -> cross
+              scale_d = 1;
             }
-            first = 0;
-            if (!RES) {
-              umma_commit(b_empty(bs));                          // weight slot free when these MMAs retire
-              if (++bs == BS) { bs = 0; bph ^= 1; }
-            }
+            wgmma_commit();
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+            wgmma_wait<1>();                                 // the previous group has retired
+            release(pend_a, pend_b);
+            pend_a = (ky == P.ks - 1) ? as : -1;
+            pend_b = b_slot;
           }
-          umma_commit(a_empty(as));                              // activation box free after its last vertical tap
           if (++as == AS) { as = 0; aph ^= 1; }
         }
       }
-      umma_commit(tfull_bar(acc));                               // accumulators complete -> epilogue
-      if (++acc == NBUF) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    // eight warps: two per TMEM lane quarter, which take the 16-column chunks alternately -- one warp per quarter leaves
-    // the epilogue, not the MMAs, as the pace of the 64-channel layers (a chunk is a long dependent chain: TMEM load,
-    // arithmetic, conversions, stores)
-    const int q = warp & 3;                                    // TMEM lane quarter this warp may access
-    const int eset = (warp - 4) >> 2;                          // 0 / 1: which chunks of the quarter
-    const int m = q * 32 + lane;                               // output pixel within the tile
-    const int r = m / UM_TW, c = m % UM_TW;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
+      wgmma_wait<0>();
+      release(pend_a, pend_b);
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+
+      // ---- epilogue: registers [4j, 4j+1] hold channels 8j + 2*t4 + {0,1} of pixel (y, x), [4j+2, 4j+3] of (y+1, x) ----
       const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
-      const int y = ty * UM_TH + r, x = tx * UM_TW + c;
-      const bool inside = (y < P.H) && (x < P.W);
-      const size_t pix = ((size_t)b * P.H + y) * P.W + x;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 2 * N);
-      // fused 2x2 max-pool: the warp owns tile rows 2q, 2q+1 (lane = (row & 1) * 16 + col); the pooled pixel of
-      // (even row, even col) is the max over lanes l, l+1, l+16, l+17 -> two shuffle steps, writer lanes l < 16, l even
-      const int py = ty * (UM_TH / 2) + q, px = tx * (UM_TW / 2) + (lane >> 1);
-      const bool pool_writer = P.pool && lane < 16 && !(lane & 1) && py < (P.H >> 1) && px < (P.W >> 1);
-      const size_t ppix = ((size_t)b * (P.H >> 1) + py) * (P.W >> 1) + px;
+      const int x = tx * UM_TW + cw * 8 + col, y = ty * UM_TH + 2 * wq;
+      const bool in0 = y < P.H && x < P.W, in1 = y + 1 < P.H && x < P.W;
+      const size_t pix0 = ((size_t)b * P.H + y) * P.W + x, pix1 = pix0 + P.W;
+      auto value = [&](int r, int c) {                       // r = register index of the main accumulator
+        return fmaf(acc[r] + cross[r], P.inv_scale, __ldg(P.bias + n_off + c));
+      };
       if (P.epi == 1) {
-        if (eset == 0) {
-        // fused detector head (superpoint.ipynb:190-198): the thread holds one cell's 65 logits in TMEM.  Three passes over
-        // the columns (max, sum in channel order, normalise + pixel shuffle) -- the arithmetic of sp_softmax_shuffle_kernel,
-        // so the heat map is bit-identical to the two-kernel path.
-        auto logit = [&](uint32_t a, uint32_t c, int ch) {
-          return fmaf(__uint_as_float(a) + __uint_as_float(c), P.inv_scale, __ldg(P.bias + ch));
-        };
-        float mx = -INFINITY;
-#pragma unroll 1
-        for (int n0 = 0; n0 < 80; n0 += 16) {
-          uint32_t v[16], vc[16];
-          tmem_ld16(t_row + n0, v);
-          tmem_ld16(t_row + N + n0, vc);
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (n0 + i < 65) mx = fmaxf(mx, logit(v[i], vc[i], n0 + i));
-        }
-        float sum = 0.f;
-#pragma unroll 1
-        for (int n0 = 0; n0 < 80; n0 += 16) {
-          uint32_t v[16], vc[16];
-          tmem_ld16(t_row + n0, v);
-          tmem_ld16(t_row + N + n0, vc);
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (n0 + i < 65) sum += expf(logit(v[i], vc[i], n0 + i) - mx);
-        }
+        // fused detector head (superpoint.ipynb:190-198): softmax over the 65 logits of a cell, which four lanes of a quad
+        // hold, then the dustbin is dropped and the 64 probabilities are pixel-shuffled into the heat map
         const int W8 = P.W * 8;
-        float* out = P.out_f32 + ((size_t)b * P.H * 8 + (size_t)y * 8) * W8 + (size_t)x * 8;
-#pragma unroll 1
-        for (int n0 = 0; n0 < 64; n0 += 16) {
-          uint32_t v[16], vc[16];
-          tmem_ld16(t_row + n0, v);
-          tmem_ld16(t_row + N + n0, vc);
-          if (!inside) continue;
-          float e[16];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) e[i] = expf(logit(v[i], vc[i], n0 + i) - mx) / sum;
+        for (int r = 0; r < 2; ++r) {
+          float mx = -INFINITY;
 #pragma unroll
-          for (int r2 = 0; r2 < 2; ++r2) {
-            float4* dst = reinterpret_cast<float4*>(out + (size_t)(n0 / 8 + r2) * W8);
-            dst[0] = make_float4(e[8 * r2], e[8 * r2 + 1], e[8 * r2 + 2], e[8 * r2 + 3]);
-            dst[1] = make_float4(e[8 * r2 + 4], e[8 * r2 + 5], e[8 * r2 + 6], e[8 * r2 + 7]);
+          for (int j = 0; j < 9; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (8 * j + 2 * t4 + e < 65) mx = fmaxf(mx, value(4 * j + 2 * r + e, 8 * j + 2 * t4 + e));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          float sum = 0.f;
+#pragma unroll
+          for (int j = 0; j < 9; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (8 * j + 2 * t4 + e < 65) sum += expf(value(4 * j + 2 * r + e, 8 * j + 2 * t4 + e) - mx);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          if (!(r ? in1 : in0)) continue;
+          float* out = P.out_f32 + ((size_t)b * P.H * 8 + (size_t)(y + r) * 8) * W8 + (size_t)x * 8 + 2 * t4;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float e0 = expf(value(4 * j + 2 * r, 8 * j + 2 * t4) - mx) / sum;
+            const float e1 = expf(value(4 * j + 2 * r + 1, 8 * j + 2 * t4 + 1) - mx) / sum;
+            *reinterpret_cast<float2*>(out + (size_t)j * W8) = make_float2(e0, e1);
           }
         }
-        }      // (the second warp of the quarter has nothing to do for this head: it only releases the accumulator)
-      } else
-#pragma unroll 1
-      for (int n0 = eset * 16; n0 < N; n0 += 32) {
-        uint32_t v[16], vc[16];
-        tmem_ld16(t_row + n0, v);
-        tmem_ld16(t_row + N + n0, vc);
-        if (n_off - P.n_off + n0 >= P.out_c) continue;              // warp-uniform
-        float f[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float a = fmaf(__uint_as_float(v[i]) + __uint_as_float(vc[i]), P.inv_scale, __ldg(P.bias + n_off + n0 + i));
-          if (P.relu) a = fmaxf(a, 0.f);
-          if (P.relu == 2) a = fminf(a, 6.f);
-          f[i] = a;
-        }
-        bool store = inside;
-        size_t opix = pix;
-        if (P.pool) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            f[i] = fmaxf(f[i], __shfl_down_sync(0xffffffffu, f[i], 1));
-            f[i] = fmaxf(f[i], __shfl_down_sync(0xffffffffu, f[i], 16));
-          }
-          store = pool_writer; opix = ppix;
-        }
-        if (!store) continue;
-        if (P.out_f32) {
-          float* dst = P.out_f32 + opix * P.out_cstride + n_off + n0;
-#pragma unroll
-          for (int i = 0; i < 2; ++i)
-            st_global_256(dst + 8 * i, __float_as_uint(f[8 * i]), __float_as_uint(f[8 * i + 1]), __float_as_uint(f[8 * i + 2]),
-                          __float_as_uint(f[8 * i + 3]), __float_as_uint(f[8 * i + 4]), __float_as_uint(f[8 * i + 5]),
-                          __float_as_uint(f[8 * i + 6]), __float_as_uint(f[8 * i + 7]));
-        } else {
-          uint32_t hi[8], lo[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float s0 = f[2 * i] * P.out_scale, s1 = f[2 * i + 1] * P.out_scale;
-            // packed conversions (cvt.rn.f16x2.f32: the roundings of two scalar conversions, off the slow F2F pipe)
+      } else {
+        // fused 2x2 max-pool: the pooled pixel of (even y, even x) is the max over this thread's two rows and the lane
+        // holding column x + 1 (lane + 4); writer lanes hold even columns
+        const int py = ty * (UM_TH / 2) + wq, px = tx * (UM_TW / 2) + cw * 4 + (col >> 1);
+        const bool pool_writer = !(col & 1) && py < (P.H >> 1) && px < (P.W >> 1);
+        const size_t ppix = ((size_t)b * (P.H >> 1) + py) * (P.W >> 1) + px;
+        auto store = [&](size_t pix, int c, float v0, float v1) {
+          if (P.out_f32) {
+            *reinterpret_cast<float2*>(P.out_f32 + pix * P.out_cstride + n_off + c) = make_float2(v0, v1);
+          } else {
+            const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
+            // packed conversions (cvt.rn.f16x2.f32: the roundings of two scalar conversions)
             const __half2 hp = __floats2half2_rn(s0, s1);
             const float2 hf = __half22float2(hp);
             const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
-            hi[i] = *reinterpret_cast<const uint32_t*>(&hp);
-            lo[i] = *reinterpret_cast<const uint32_t*>(&lp);
+            *reinterpret_cast<__half2*>(P.out_hi + pix * P.out_cstride + n_off + c) = hp;
+            *reinterpret_cast<__half2*>(P.out_lo + pix * P.out_cstride + n_off + c) = lp;
           }
-          st_global_256(P.out_hi + opix * P.out_cstride + n_off + n0, hi[0], hi[1], hi[2], hi[3], hi[4], hi[5], hi[6], hi[7]);
-          st_global_256(P.out_lo + opix * P.out_cstride + n_off + n0, lo[0], lo[1], lo[2], lo[3], lo[4], lo[5], lo[6], lo[7]);
+        };
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          if (n_off - P.n_off + 8 * j >= P.out_c) continue;            // warp-uniform
+          const int c = 8 * j + 2 * t4;
+          float f[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            float a = value(4 * j + i, c + (i & 1));
+            if (P.relu) a = fmaxf(a, 0.f);
+            if (P.relu == 2) a = fminf(a, 6.f);
+            f[i] = a;
+          }
+          if (P.pool) {
+            float m0 = fmaxf(f[0], f[2]), m1 = fmaxf(f[1], f[3]);
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 4));
+            m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 4));
+            if (pool_writer) store(ppix, c, m0, m1);
+          } else {
+            if (in0) store(pix0, c, f[0], f[1]);
+            if (in1) store(pix1, c, f[2], f[3]);
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));              // 8 epilogue warps -> count 8
-      if (++acc == NBUF) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS) : "memory");
   }
 }
 
@@ -495,7 +520,7 @@ osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bia
                              float w_scale) {
   L->cin = cin; L->cout = cout; L->ks = ks; L->taps = ks * ks; L->w_scale = w_scale;
   L->n_pad = (cout <= 64) ? 64 : (cout <= 80) ? 80 : (cout <= 128) ? 128 : (cout <= 256) ? 256 : 512;
-  OSB_REQUIRE(cin % UM_KC == 0 && cout <= 512, "tcgen05 conv: Cin must be a multiple of 64 and Cout <= 512");
+  OSB_REQUIRE(cin % UM_KC == 0 && cout <= 512, "tensor-core conv: Cin must be a multiple of 64 and Cout <= 512");
   const size_t n = (size_t)L->taps * L->n_pad * cin;
   std::vector<__half> hi(n, __float2half(0.f)), lo(n, __float2half(0.f));
   std::vector<float> bp(L->n_pad, 0.f);
@@ -522,10 +547,6 @@ osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bia
   osb_status s;
   if ((s = umma_make_tmap(&L->tm_hi, L->w_hi, 3, dims, strides, box)) != OSB_OK) return s;
   if ((s = umma_make_tmap(&L->tm_lo, L->w_lo, 3, dims, strides, box)) != OSB_OK) return s;
-  if (L->n_pad == 64) {
-    const uint32_t box32[3] = {UM_KC, 32, 1};
-    if ((s = umma_make_tmap(&L->tm_hi32, L->w_hi, 3, dims, strides, box32)) != OSB_OK) return s;
-  }
   if (L->n_pad >= 256) {                       // 128-row boxes: the layer as n_pad / 128 work items per tile
     const uint32_t box128[3] = {UM_KC, 128, 1};
     if ((s = umma_make_tmap(&L->tm_hi128, L->w_hi, 3, dims, strides, box128)) != OSB_OK) return s;
@@ -550,30 +571,27 @@ osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half*
   return umma_make_tmap(lo, p_lo, 4, dims, strides, box);
 }
 
-// OSB_CONV_PDL=1 launches the convolutions with programmatic dependent launch.  Off by default: measured (r01f) it
-// costs throughput here -- the dependent layer's CTAs take the SMs the concurrent NetVLAD stream was filling
-// (2.10 ms per keyframe with it, 1.93 ms without).
+// OSB_CONV_PDL=1 launches the convolutions with programmatic dependent launch.  Off by default: the dependent layer's CTAs
+// take the SMs the concurrent NetVLAD stream of the front-end would otherwise fill.
 static const bool g_conv_pdl = [] { const char* e = getenv("OSB_CONV_PDL"); return e && atoi(e) != 0; }();
 
-// OSB_CONV_NSPLIT=0: layers of 256 / 512 output channels run through the N = 256 kernel (A/B switch)
-static const bool g_conv_nsplit = [] { const char* e = getenv("OSB_CONV_NSPLIT"); return !(e && atoi(e) == 0); }();
-
-template <int N, bool RES, bool SPLIT = false>
+template <int N, bool RES, bool SPLIT = false, bool FIRST = false>
 static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
-                              cudaStream_t st, int max_ctas, bool box128 = false) {
+                              cudaStream_t st, int max_ctas, bool box128 = false,
+                              const typename std::conditional<FIRST, Conv1aW, NoConv1a>::type& W1 = {}) {
   using Cfg = UmmaCfg<N, RES>;
-  OSB_SMEM_OPT_IN((conv_umma_kernel<N, RES, SPLIT>), Cfg::SMEM_BYTES);
+  OSB_SMEM_OPT_IN((conv_umma_kernel<N, RES, SPLIT, FIRST>), Cfg::SMEM_BYTES);
   const int tiles = P.B * cdiv(P.W, UM_TW) * cdiv(P.H, UM_TH) * P.n_split;
   // persistent CTAs, one per SM; `max_ctas` leaves SMs free for a kernel running beside this one on another stream
   const int grid = std::min(tiles, persistent_ctas(max_ctas));
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(UM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = st;
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(um_threads(FIRST)); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = st;
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = g_conv_pdl ? 1 : 0;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  OSB_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<N, RES, SPLIT>, a_hi, a_lo, box128 ? L.tm_hi128 : L.tm_hi,
-                              box128 ? L.tm_lo128 : L.tm_lo, P));
+  OSB_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<N, RES, SPLIT, FIRST>, a_hi, a_lo, box128 ? L.tm_hi128 : L.tm_hi,
+                              box128 ? L.tm_lo128 : L.tm_lo, P, W1));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return OSB_OK;
 }
@@ -581,14 +599,14 @@ static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, 
 osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                              float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
                              float out_scale, int relu, int pool, cudaStream_t st, int max_ctas) {
-  UmmaArgs P;
+  UmmaArgs P = {};
   P.pool = pool;
   OSB_REQUIRE(!pool || (H % 2 == 0 && W % 2 == 0), "fused max-pool needs even H and W");
   P.bias = L.bias; P.out_hi = out_hi; P.out_lo = out_lo; P.out_f32 = out_f32;
   P.H = H; P.W = W; P.B = B; P.ks = L.ks; P.cin_slabs = L.cin / UM_KC;
   P.out_c = out_c; P.out_cstride = out_cstride;
   P.inv_scale = 1.0f / (act_scale * L.w_scale); P.out_scale = out_scale; P.relu = relu;
-  OSB_REQUIRE(out_c % 16 == 0 && out_c <= L.n_pad && out_cstride % 8 == 0, "tcgen05 conv: bad output channel layout");
+  OSB_REQUIRE(out_c % 16 == 0 && out_c <= L.n_pad && out_cstride % 8 == 0, "tensor-core conv: bad output channel layout");
   P.n_off = 0; P.n_split = 1; P.epi = 0;
   switch (L.n_pad) {
     case 64:
@@ -596,24 +614,10 @@ osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const 
       return launch_umma<64, false>(a_hi, a_lo, L, P, st, max_ctas);
     case 80: return launch_umma<80, false>(a_hi, a_lo, L, P, st, max_ctas);
     case 128: return launch_umma<128, false>(a_hi, a_lo, L, P, st, max_ctas);
-    case 256:
-      if (g_conv_nsplit) {                        // 2 items of 128 channels per tile: TMEM double-buffered (the N = 256
-        P.n_split = 2;                            // kernel is single-buffered), finer work items for the 320-tile layers
-        return launch_umma<128, false, true>(a_hi, a_lo, L, P, st, max_ctas, true);
-      }
-      return launch_umma<256, false>(a_hi, a_lo, L, P, st, max_ctas);
-    case 512: {
-      if (g_conv_nsplit) {
-        P.n_split = 4;
-        return launch_umma<128, false, true>(a_hi, a_lo, L, P, st, max_ctas, true);
-      }
-      // two N = 256 passes over the same activations
-      P.out_c = 256;
-      osb_status s = launch_umma<256, false>(a_hi, a_lo, L, P, st, max_ctas);
-      if (s != OSB_OK) return s;
-      P.n_off = 256;
-      return launch_umma<256, false>(a_hi, a_lo, L, P, st, max_ctas);
-    }
+    case 256:                                     // 2 / 4 items of 128 channels per tile (a 256-wide accumulator pair
+    case 512:                                     // would not fit a warpgroup's registers)
+      P.n_split = L.n_pad / 128;
+      return launch_umma<128, false, true>(a_hi, a_lo, L, P, st, max_ctas, true);
   }
   set_error("umma_conv_forward", "unsupported N");
   return OSB_ERR_INVALID;
@@ -624,7 +628,7 @@ osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const 
 osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                                      float act_scale, float* semi, cudaStream_t st, int max_ctas) {
   OSB_REQUIRE(L.n_pad == 80 && L.cout == 65 && L.ks == 1, "fused detector head expects the 65-logit 1x1 layer");
-  UmmaArgs P;
+  UmmaArgs P = {};
   P.pool = 0; P.bias = L.bias; P.out_hi = nullptr; P.out_lo = nullptr; P.out_f32 = semi;
   P.H = H; P.W = W; P.B = B; P.ks = L.ks; P.cin_slabs = L.cin / UM_KC;
   P.out_c = 80; P.out_cstride = 80;
@@ -633,8 +637,30 @@ osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi
   return launch_umma<80, false>(a_hi, a_lo, L, P, st, max_ctas);
 }
 
+// conv1a + ReLU + conv1b + ReLU + 2x2 max-pool: u8 images -> the split planes conv2a reads.  L1b = conv1b's weights
+// (n_pad 64, Cin 64, 3x3) as uploaded by umma_layer_upload; w1a [tap][64], b1a [64] fp32.
+osb_status umma_conv1_fused_forward(const UmmaLayer& L1b, const float* w1a_host, const float* b1a_host, const uint8_t* img, int B,
+                                    int H, int W, float act_scale, __half* out_hi, __half* out_lo, float out_scale, cudaStream_t st,
+                                    int max_ctas) {
+  OSB_REQUIRE(L1b.n_pad == 64 && L1b.cin == 64 && L1b.ks == 3, "fused first layers expect the 64 -> 64 3x3 layer");
+  OSB_REQUIRE(H % 2 == 0 && W % 2 == 0, "fused max-pool needs even H and W");
+  UmmaArgs P = {};
+  P.bias = L1b.bias; P.out_hi = out_hi; P.out_lo = out_lo; P.out_f32 = nullptr;
+  P.H = H; P.W = W; P.B = B; P.ks = 3; P.cin_slabs = 1;
+  P.out_c = 64; P.out_cstride = 64;
+  P.inv_scale = 1.0f / (act_scale * L1b.w_scale); P.out_scale = out_scale; P.relu = 1; P.pool = 1;
+  P.n_off = 0; P.n_split = 1; P.epi = 0;
+  P.img = img; P.alpha = (float)(1.0 / 255.0);
+  Conv1aW W1;                                             // the plane scale is a power of two: the products are exact
+  for (int t = 0; t < 9; ++t)
+    for (int c = 0; c < 64; ++c) W1.w[t][c] = w1a_host[t * 64 + c] * act_scale;
+  for (int c = 0; c < 64; ++c) W1.b[c] = b1a_host[c] * act_scale;
+  // (the activation maps are unused by the FIRST form: the weight maps stand in)
+  return launch_umma<64, true, false, true>(L1b.tm_hi, L1b.tm_lo, L1b, P, st, max_ctas, false, W1);
+}
+
 // depthwise 3x3 (pad 1, stride s) + bias + ReLU6 on fp32 NHWC input, output as split fp16 planes for the pointwise
-// tcgen05 conv that follows; one thread per (output pixel, 8 channels)
+// tensor-core conv that follows; one thread per (output pixel, 8 channels)
 __global__ void dwconv3x3_split_kernel(const float* __restrict__ w, const float* __restrict__ bias,
                                        const float* __restrict__ x, __half* __restrict__ out_hi,
                                        __half* __restrict__ out_lo, int H, int W, int Ho, int Wo, int C, int stride,

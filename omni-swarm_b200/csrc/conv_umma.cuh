@@ -1,4 +1,4 @@
-// conv_umma.cuh -- host-side interface of the tcgen05 convolution path (conv_umma.cu)
+// conv_umma.cuh -- host-side interface of the tensor-core (wgmma) convolution path (conv_umma.cu)
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -14,7 +14,6 @@ struct UmmaLayer {
   float* bias = nullptr;
   CUtensorMap tm_hi, tm_lo;
   CUtensorMap tm_hi128, tm_lo128;     // same planes with 128-row boxes (n_pad >= 256 only)
-  CUtensorMap tm_hi32;                // W_hi with 32-row boxes (n_pad == 64: the CTA-pair kernel's half of the N = 64 operand)
 };
 
 osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks,
@@ -32,36 +31,17 @@ osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi
                                      float act_scale, float* semi, cudaStream_t st, int max_ctas = 0);
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
                               __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st);
-// conv1a + ReLU + conv1b + ReLU + 2x2 max-pool in one kernel (conv1_fused.cu): u8 images -> pooled split planes
+// conv1a + ReLU + conv1b + ReLU + 2x2 max-pool in one kernel (conv_umma.cu, FIRST form): u8 images -> pooled split planes.
 // conv1a's weights and bias, pre-multiplied by the plane scale, as a KERNEL PARAMETER: with lane = pixel every FFMA of a warp
-// uses the same weight, so it comes from the constant bank through a uniform register (LDCU.128 + FFMA2 R, R.F32, UR, R)
-// instead of occupying 72 registers per thread
+// uses the same weight, so it comes from the constant bank instead of occupying 72 registers per thread
 struct Conv1aW { float w[9][64]; float b[64]; };
 
 osb_status umma_conv1_fused_forward(const UmmaLayer& L1b, const float* w1a, const float* b1a, const uint8_t* img, int B, int H,
                                     int W, float act_scale, __half* out_hi, __half* out_lo, float out_scale, cudaStream_t st,
-                                    int max_ctas = 0, unsigned long long* dbg = nullptr);
-// dbg (optional, [16] device words): SM-clock cycles of CTA 0 summed over its tiles -- [0] producer wait (window free),
-// [1] producer compute + stores, [2] producer wait (shared rows), [3] producer loop total, [4] MMA issuer wait (TMEM free),
-// [5] wait (halo tile full), [6] issue, [7] epilogue wait, [8] epilogue work, [9] tiles of CTA 0
-// halo-window form of the 64 -> 64 3x3 layers (conv1_fused.cu, FIRST = false): one halo tile per output tile instead of
-// three kx-shifted boxes
-struct HaloMaps { CUtensorMap a15_hi, a15_lo, a3_hi, a3_lo; };
-osb_status umma_halo_maps(HaloMaps* M, __half* p_hi, __half* p_lo, int B, int H, int W);
-osb_status umma_conv64_halo_forward(const UmmaLayer& L, const HaloMaps& M, int B, int H, int W, float act_scale, __half* out_hi,
-                                    __half* out_lo, float out_scale, int pool, cudaStream_t st, int max_ctas = 0,
-                                    unsigned long long* dbg = nullptr);
+                                    int max_ctas = 0);
 osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
-// CTA-pair form (conv64_pair.cu: tcgen05.mma.cta_group::2, M = 256, weights split across the pair, two full halo windows)
-osb_status umma_pair_first_forward(const UmmaLayer& L1b, const float* w1a_host, const float* b1a_host, const uint8_t* img, int B, int H,
-                                   int W, float act_scale, __half* out_hi, __half* out_lo, float out_scale, cudaStream_t st,
-                                   int max_ctas = 0, unsigned long long* dbg = nullptr);
-osb_status umma_pair_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half* p_lo, int B, int H, int W);
-osb_status umma_pair_conv64_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
-                                    float act_scale, __half* out_hi, __half* out_lo, float out_scale, int pool, cudaStream_t st,
-                                    int max_ctas = 0, unsigned long long* dbg = nullptr);
-// depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tcgen05 conv)
+// depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv)
 osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const float* x, __half* out_hi, __half* out_lo,
                                int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st);
 }  // namespace osb

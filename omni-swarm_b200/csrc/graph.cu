@@ -178,8 +178,7 @@ __device__ __forceinline__ double factor_sqnorm(int type, const double* __restri
 // chain factorisation -- runs in fp32 when the requested pcg_tolerance allows (>= 1e-4); residuals, costs, the gradient
 // J^T r, the diagonal, the poses and every LM decision stay fp64.  fp32 halves what bounds a CG iteration here: the
 // 32-bit shuffles of the preconditioner sweeps, the bytes of every cross-thread gather through L2, the shared-memory
-// footprint of the Jacobians (96 KB instead of 192 KB) and the live registers.  (It is NOT an fp64-throughput issue:
-// scripts/microbench/fp64_rate.cu measures 62 DFMA lanes/clk/SM against 117 FFMA lanes/clk/SM on this B200.)  A numpy
+// footprint of the Jacobians (96 KB instead of 192 KB) and the live registers.  A numpy
 // emulation of the same loop gives the same iteration counts and poses within 1e-8 of the all-fp64 solve (DESIGN.md);
 // tests/test_gpu_solver.py checks it on the GPU.  T = double is kept for tight tolerances (parity tests).
 struct SolverDev {

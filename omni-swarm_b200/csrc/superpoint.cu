@@ -40,8 +40,6 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
   if (const char* e = getenv("OSB_SP_OVERLAP")) overlap_kp = atoi(e) != 0;
   if (const char* e = getenv("OSB_SP_FUSED_SOFTMAX")) fused_softmax = atoi(e) != 0;
   if (const char* e = getenv("OSB_SP_FUSE1")) fuse_first = atoi(e) != 0;
-  if (const char* e = getenv("OSB_SP_HALO64")) halo64 = atoi(e) != 0;
-  if (const char* e = getenv("OSB_SP_PAIR")) { pair64 = atoi(e) != 0; pair_first = atoi(e) == 1; pair_2a = atoi(e) != 3; }
   // ---- weights ----
   const float* p = weights;
   {
@@ -58,7 +56,7 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
     p += 64 * 9 + 64;
   }
   {
-    // OSB_SP_CONV=ffma selects the fp32 CUDA-core convolutions (debug / A-B parity); default = tcgen05 path
+    // OSB_SP_CONV=ffma selects the fp32 CUDA-core convolutions (debug / A-B parity); default = tensor-core path
     const char* e = getenv("OSB_SP_CONV");
     use_umma = !(e && strcmp(e, "ffma") == 0);
   }
@@ -110,16 +108,8 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
       in_lo[i] = base + (size_t)max_batch * h * w * c;
       osb_status s = umma_act_maps(&tmA[i], &tmB[i], in_hi[i], in_lo[i], max_batch, h, w, c, SP_KS[i]);
       if (s != OSB_OK) return s;
-      if (i == 2 || i == 3) {
-        s = umma_halo_maps(&halo[i], in_hi[i], in_lo[i], max_batch, h, w);
-        if (s != OSB_OK) return s;
-        s = umma_pair_maps(&pairA[i], &pairB[i], in_hi[i], in_lo[i], max_batch, h, w);
-        if (s != OSB_OK) return s;
-      }
     }
   }
-  OSB_CUDA(cudaMalloc(&d_f1dbg, 16 * sizeof(unsigned long long)));
-  OSB_CUDA(cudaMemset(d_f1dbg, 0, 16 * sizeof(unsigned long long)));
   OSB_CUDA(cudaMalloc(&d_semi, B * HW * sizeof(float)));
   OSB_CUDA(cudaMalloc(&d_desc, B * Hc * Wc * 256 * sizeof(float)));
   OSB_CUDA(cudaMalloc(&ks.state, B * HW));
@@ -144,7 +134,7 @@ void SuperPoint::release() {
   for (int i = 0; i < 20; ++i) if (lev[i]) cudaEventDestroy(lev[i]);
   cudaFree(d_img); cudaFree(actA); cudaFree(actB); cudaFree(d_logits); cudaFree(d_semi); cudaFree(d_desc);
   cudaFree(ks.state); cudaFree(ks.surv); cudaFree(ks.cand); cudaFree(ks.skey); cudaFree(ks.cmask); cudaFree(ks.counts); cudaFree(ks.cnorm);
-  cudaFree(d_nk); cudaFree(d_kpts); cudaFree(d_conf); cudaFree(d_out); cudaFree(d_f1dbg);
+  cudaFree(d_nk); cudaFree(d_kpts); cudaFree(d_conf); cudaFree(d_out);
   if (stream) cudaStreamDestroy(stream);
   if (kp_stream) cudaStreamDestroy(kp_stream);
   if (ev_semi) cudaEventDestroy(ev_semi);
@@ -165,48 +155,20 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
     return umma_conv_forward(UL[i], tmA[i], tmB[i], B, h, w, SA, in_hi[out_layer], in_lo[out_layer], nullptr,
                              SP_COUT[i], SP_COUT[i], SA, 1, pool, st);
   };
-  // cycle counters of the 64 -> 64 kernels (osb_superpoint_read what = 5): OSB_F1_DEBUG=<1|2|3> selects conv1 / conv2a / conv2b;
-  // off by default because the clock reads cost a few percent of the kernel
-  static const int dbg_layer = [] { const char* e = getenv("OSB_F1_DEBUG"); return e ? atoi(e) : 0; }();
-  if (fuse_first && pair64 && pair_first) {
-    mark(st);
-    RUN(umma_pair_first_forward(UL[1], w1a_host.data(), b1a_host.data(), img_dev, B, H, W, SA, in_hi[2], in_lo[2], SA, st, 0,
-                                (layer_prof && dbg_layer == 1) ? d_f1dbg : nullptr));     // conv1a+conv1b+pool -> B
-    mark(st);
-  } else if (fuse_first) {
+  if (fuse_first) {
     mark(st);                                                                             // (conv1a has no launch of its own)
-    RUN(umma_conv1_fused_forward(UL[1], w1a_host.data(), b1a_host.data(), img_dev, B, H, W, SA, in_hi[2], in_lo[2], SA, st, 0,
-                                 (layer_prof && dbg_layer == 1) ? d_f1dbg : nullptr));   // conv1a+conv1b+pool -> B
-    mark(st);
+    RUN(umma_conv1_fused_forward(UL[1], w1a_host.data(), b1a_host.data(), img_dev, B, H, W, SA, in_hi[2], in_lo[2], SA, st));
+    mark(st);                                                                             // conv1a+conv1b+pool -> B
   } else {
     RUN(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st)); // conv1a            -> A
     mark(st);
     RUN(conv(1, H, W, 2, 1));                                                             // conv1b + pool     -> B
     mark(st);
   }
-  if (pair64) {
-    if (pair_2a)
-      RUN(umma_pair_conv64_forward(UL[2], pairA[2], pairB[2], B, H / 2, W / 2, SA, in_hi[3], in_lo[3], SA, 0, st, 0,
-                                   (layer_prof && dbg_layer == 2) ? d_f1dbg : nullptr));                // conv2a   -> A
-    else
-      RUN(conv(2, H / 2, W / 2, 3, 0));
-    mark(st);
-    RUN(umma_pair_conv64_forward(UL[3], pairA[3], pairB[3], B, H / 2, W / 2, SA, in_hi[4], in_lo[4], SA, 1, st, 0,
-                                 (layer_prof && dbg_layer == 3) ? d_f1dbg : nullptr));                  // conv2b + pool -> B
-    mark(st);
-  } else if (halo64) {
-    RUN(umma_conv64_halo_forward(UL[2], halo[2], B, H / 2, W / 2, SA, in_hi[3], in_lo[3], SA, 0, st, 0,
-                                 (layer_prof && dbg_layer == 2) ? d_f1dbg : nullptr));                  // conv2a   -> A
-    mark(st);
-    RUN(umma_conv64_halo_forward(UL[3], halo[3], B, H / 2, W / 2, SA, in_hi[4], in_lo[4], SA, 1, st, 0,
-                                 (layer_prof && dbg_layer == 3) ? d_f1dbg : nullptr));                  // conv2b + pool -> B
-    mark(st);
-  } else {
-    RUN(conv(2, H / 2, W / 2, 3, 0));                                                     // conv2a            -> A
-    mark(st);
-    RUN(conv(3, H / 2, W / 2, 4, 1));                                                     // conv2b + pool     -> B
-    mark(st);
-  }
+  RUN(conv(2, H / 2, W / 2, 3, 0));                                                       // conv2a            -> A
+  mark(st);
+  RUN(conv(3, H / 2, W / 2, 4, 1));                                                       // conv2b + pool     -> B
+  mark(st);
   RUN(conv(4, H / 4, W / 4, 5, 0));                                                       // conv3a            -> A
   mark(st);
   RUN(conv(5, H / 4, W / 4, 6, 1));                                                       // conv3b + pool     -> B
@@ -440,13 +402,6 @@ extern "C" osb_status osb_superpoint_read(osb_superpoint* h, int what, int image
     OSB_CUDA(cudaMemcpyAsync(c, sp.ks.counts + image * 8, sizeof(c), cudaMemcpyDeviceToHost, st));
     OSB_CUDA(cudaStreamSynchronize(st));
     for (int i = 0; i < 8; ++i) out[i] = (float)c[i];
-    return OSB_OK;
-  } else if (what == 5) {
-    OSB_REQUIRE(n_floats == 16, "fused-kernel counters need 16 floats");
-    unsigned long long c[16];
-    OSB_CUDA(cudaMemcpyAsync(c, sp.d_f1dbg, sizeof(c), cudaMemcpyDeviceToHost, st));
-    OSB_CUDA(cudaStreamSynchronize(st));
-    for (int i = 0; i < 16; ++i) out[i] = (float)c[i];
     return OSB_OK;
   } else {
     set_error("osb_superpoint_read", "unknown `what`");

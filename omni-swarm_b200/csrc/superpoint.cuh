@@ -44,18 +44,10 @@ struct SuperPoint {
   cudaStream_t kp_stream = nullptr;
   cudaEvent_t ev_semi = nullptr, ev_kp = nullptr;
   bool overlap_kp = true;
-  unsigned long long* d_f1dbg = nullptr;   // cycle counters of the fused first-layers kernel (filled while layer_prof is on)
-  CUtensorMap pairA[4], pairB[4]; // [2], [3]: conv2a / conv2b inputs for the CTA-pair kernel (one 18-row box per plane)
-  bool pair_first = false;        // OSB_SP_PAIR=1: the first layers on CTA pairs too; =2: only conv2a / conv2b; =3: only conv2b
-  bool pair_2a = true;
-  bool pair64 = false;            // OSB_SP_PAIR=1: conv1a+1b, conv2a, conv2b on CTA pairs (conv64_pair.cu, tcgen05.mma.cta_group::2).
-                                  // Bit-identical, measured SLOWER than the single-CTA kernels (r02: conv1 0.57 vs 0.47 ms, conv2a
-                                  // 0.120 vs 0.116 ms; the pair's MMA stream ran at 134 cycles per K step against 114) -- kept as a switch
-  HaloMaps halo[4];               // [2], [3]: conv2a / conv2b inputs for the halo-window kernel
-  bool halo64 = false;            // OSB_SP_HALO64=1: conv2a / conv2b through conv64_halo_kernel<false> (one TMA halo window per tile:
-                                  // 2.6x less activation traffic, but the 3 rows the two windows share are loaded after the previous
-                                  // tile's MMAs and cost a ~1200-cycle bubble per tile: 0.118 vs 0.116 ms, r02) -- kept as a switch
-  bool fuse_first = true;          // conv1a computed inside conv1b's kernel (conv1_fused.cu; OSB_SP_FUSE1=0: two kernels)
+  bool fuse_first = false;         // OSB_SP_FUSE1=1: conv1a computed inside conv1b's kernel (conv_umma.cu, FIRST form).  Off by
+                                   // default: on an H100 (80GB HBM3, 400 W power limit) conv1a+conv1b+pool of 8 images at 640x480
+                                   // took 5.44 ms fused against 1.28 ms as two kernels -- the producer warpgroup computes each conv1a
+                                   // pixel three times (once per kx-shifted box) and cannot keep up with the MMAs
   bool fused_softmax = true;       // detector-head softmax + pixel shuffle in convPb's epilogue (OSB_SP_FUSED_SOFTMAX=0: two kernels)
   osb_status network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp = nullptr);
   osb_status network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp);

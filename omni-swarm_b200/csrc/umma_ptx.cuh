@@ -1,5 +1,5 @@
-// umma_ptx.cuh -- inline-PTX helpers shared by the tcgen05 convolution kernels (mbarrier, TMA, tcgen05.mma / ld / commit,
-// shared-memory matrix descriptors).  sm_100a only.
+// umma_ptx.cuh -- inline-PTX helpers shared by the tensor-core convolution kernels on Hopper (sm_90a): mbarrier, TMA,
+// warpgroup MMA (wgmma.mma_async) and its shared-memory matrix descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -23,8 +23,17 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   do {
     asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
                  : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    // a pipeline bug must surface as a launch failure, never as a hung GPU (try_wait itself blocks for a while)
+    // a pipeline bug must surface as a launch failure, never as a hung GPU (try_wait itself blocks for a while).
+    // Debug builds (make EXTRA=-DOSB_MBAR_DEBUG) report the stalled barrier and let the kernel drain instead.
+#ifdef OSB_MBAR_DEBUG
+    if (!done && ++spins > (1u << 22)) {
+      if (blockIdx.x == 0 && (threadIdx.x & 31) == 0)
+        printf("mbar_wait stalled: block %d thread %d barrier +%u parity %u\n", blockIdx.x, threadIdx.x, bar & 0xFFFFu, parity);
+      return;
+    }
+#else
     if (!done && ++spins > (1u << 24)) __trap();
+#endif
   } while (!done);
 }
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
@@ -35,47 +44,56 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// packed fp32 pairs (sm_100: FFMA2 / FADD2 -- one issue slot for two IEEE fp32 operations; the producers are issue bound)
-__device__ __forceinline__ uint64_t pk2(float a, float b) { uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d;
-}
-__device__ __forceinline__ uint64_t sub2(uint64_t a, uint64_t b) { uint64_t d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
 // one lane of a CONVERGED warp (elect.sync): unlike `lane == 0`, the compiler knows that exactly one thread runs the guarded
-// code, so tcgen05.mma's operands are uniform by construction and no per-thread election loop is emitted around each MMA
+// code and emits no per-thread election loop around it
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+
+// K-major SWIZZLE_128B shared-memory matrix descriptor of wgmma: start >> 4 | LBO (unused for this layout) = 1 << 16 |
+// SBO (byte distance between consecutive 8-row core-matrix groups) >> 4 << 32 | layout SWIZZLE_128B (1) << 62.
+// The start must sit on a 1024-byte swizzle atom; moving it by 32 bytes selects the next K = 16 slice of a 128-byte row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO(16B units)=1 <<16 |
-// SBO = 1024 B (8 rows x 128 B) <<32 | version 1 <<46 | layout SWIZZLE_128B (2) <<61
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// 256-bit global store (STG.256, sm_100): the epilogue's stores have one lane per pixel, so every store instruction
-// touches 32 different lines whatever its width -- 32 bytes per lane halves the instruction (and LSU line) count
-__device__ __forceinline__ void st_global_256(void* p, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4,
-                                              uint32_t r5, uint32_t r6, uint32_t r7) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(r4),
-               "r"(r5), "r"(r6), "r"(r7) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                 "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// register budget of a warpgroup (all four of its warps execute it): the producer warpgroup gives registers to the MMA ones
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across the asynchronous MMAs that own it
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// D[64 x W] (+)= A[64 x 16] * B[W x 16]^T, f16 operands from shared memory (K-major descriptors), f32 accumulators in
+// registers (W / 2 per thread).  scale_d = 0 overwrites D.
+template <int W> struct Wgmma;
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<80> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+                 : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+
 
 }  // namespace osb

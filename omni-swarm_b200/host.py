@@ -85,7 +85,7 @@ class SuperPoint:
     def read(self, what: str, image: int = 0) -> np.ndarray:
         H, W = self.height, self.width
         shapes = {"semi": (0, (H, W)), "desc": (1, (256, H // 8, W // 8)), "conf": (2, (self.max_num,)),
-                  "survivors": (3, (H, W)), "counts": (4, (8,)), "fused1_cycles": (5, (16,))}
+                  "survivors": (3, (H, W)), "counts": (4, (8,))}
         code, shape = shapes[what]
         out = np.zeros(shape, np.float32)
         _l.check(self._lib.osb_superpoint_read(self._h, code, image, _l.ptr(out), out.size))

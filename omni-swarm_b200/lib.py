@@ -181,7 +181,7 @@ _lib = None
 
 
 def build(verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into csrc/libomniswarm_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into csrc/libomniswarm_b200.so (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout[-4000:])

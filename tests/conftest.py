@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _has_gpu():
@@ -25,7 +25,7 @@ def gpu():
     """GPU tests must FAIL (not skip) when the CUDA library is missing on a GPU box; they are only deselected by -m."""
     from omniswarm_b200 import lib
     L = lib.load()
-    assert L.osb_device_count() > 0, "no CUDA device visible: -m gpu tests need the B200"
+    assert L.osb_device_count() > 0, "no CUDA device visible: -m gpu tests need an H100"
     return L
 
 

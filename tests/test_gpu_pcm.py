@@ -1,10 +1,23 @@
-"""GPU parity of the PCM outlier rejection (osb_pcm: pairwise consistency + FMC::maxCliqueHeu) against oracle/pcm_ref.py."""
+"""GPU parity of the PCM outlier rejection (osb_pcm: pairwise consistency + FMC::maxCliqueHeu) against oracle/pcm_ref.py,
+and the clique against the reference's own maxCliqueHeu (tests/golden/ref_fmc.npz, written by tests/golden/make_ref_fmc.py
+from the library compiled out of the reference's sources)."""
+import os
+
 import numpy as np
 import pytest
 
+from conftest import GOLDEN
 from omniswarm_b200 import synth, host
 from oracle import pcm_ref as pr
 from oracle import fmc_ref
+
+_REF = np.load(os.path.join(GOLDEN, "ref_fmc.npz"))
+
+
+def ref_clique(case):
+    """the reference library's clique of PCM case `case` (0..3: test_pcm_matches_oracle's parameters, 4: the large graph)"""
+    v, o = _REF["pcm_verts"], _REF["pcm_offs"]
+    return v[o[case]:o[case + 1]].tolist()
 
 pytestmark = pytest.mark.gpu
 THRES, POS, ANG = 15.0, 1e-4, 1e-5
@@ -12,6 +25,7 @@ THRES, POS, ANG = 15.0, 1e-4, 1e-5
 
 @pytest.mark.parametrize("n,out,seed", [(60, 0.3, 0), (150, 0.5, 1), (33, 0.0, 2), (1, 0.0, 3)])
 def test_pcm_matches_oracle(gpu, n, out, seed):
+    case = [(60, 0.3, 0), (150, 0.5, 1), (33, 0.0, 2), (1, 0.0, 3)].index((n, out, seed))
     edges = synth.pcm_edges(n, out, seed, other_pair=3 if n > 1 else 0)
     clique, adj, smd = host.pcm_outlier_rejection(edges, THRES, POS, ANG, want_matrices=True)
     radj, rsmd = pr.consistency_matrix(edges, THRES, POS, ANG)
@@ -23,8 +37,9 @@ def test_pcm_matches_oracle(gpu, n, out, seed):
     assert np.array_equal(adj, radj)                                  # consistency graph bit-exact
     rclique, rsize = pr.max_clique_heu(radj)
     assert clique.tolist() == rclique                                 # same vertices in maxCliqueHeu's order
-    if fmc_ref.available():                                           # ... and in the order of the REFERENCE's own library
-        assert clique.tolist() == fmc_ref.max_clique_heu(radj)[0]     # (oracle/_ref/libfmc_ref.so, built from its sources)
+    assert clique.tolist() == ref_clique(case)                        # ... and in the order of the REFERENCE's own library
+    if fmc_ref.available():                                           # (oracle/_ref/libfmc_ref.so, built from its sources)
+        assert clique.tolist() == fmc_ref.max_clique_heu(radj)[0]
     if n > 30:
         assert all(edges[i]["inlier"] for i in clique) and len(clique) >= 0.4 * sum(e["inlier"] for e in edges)
 
@@ -45,6 +60,7 @@ def test_pcm_large_graph_bitmatrix_in_global_memory(gpu):
         assert adj[i, j] == (s < THRES)
     rclique, _ = pr.max_clique_heu(adj)
     assert clique.tolist() == rclique
+    assert clique.tolist() == ref_clique(4)                           # the reference library on the oracle's consistency graph
     if fmc_ref.available():
         assert clique.tolist() == fmc_ref.max_clique_heu(adj)[0]
     assert all(edges[i]["inlier"] for i in clique) and len(clique) > 100

@@ -190,7 +190,7 @@ def test_onboard_resolution_400x208(gpu):
 
 
 def test_tensor_core_path_vs_cuda_core_path(gpu):
-    """The tcgen05 convolutions (split-fp16, 3 MMAs per K step) and the fp32 FFMA convolutions are two
+    """The tensor-core convolutions (split-fp16, 3 products per K step) and the fp32 FFMA convolutions are two
     implementations of the same network: both must sit within 1e-4 of the fp32 oracle, and within 1e-5 of each other."""
     comp, mean = synth.pca_matrices(0)
     wts = synth.flatten_sp_weights(synth.superpoint_weights(0))
@@ -214,11 +214,11 @@ def test_tensor_core_path_vs_cuda_core_path(gpu):
 
 @pytest.mark.parametrize("size", [(640, 480), (400, 208), (96, 64), (200, 120)])
 def test_fused_first_layers_bit_identical(gpu, size):
-    """conv1a computed inside conv1b's kernel (conv1_fused.cu: one shared-memory copy of the halo tile, nine descriptor
-    views) and conv2a / conv2b through the same halo-window kernel fed by TMA, against the TMA-box kernels (conv1a planes
-    through HBM, three kx-shifted boxes per tile): same fp32 FMA order in conv1a, same MMA accumulation order in the 64 -> 64
-    layers, so heat-map and descriptor map must be BIT-identical -- including ragged tiles (208 = 13 x 16 rows, 200 x 120:
-    half tiles in both directions at every resolution) and the blanked bottom quarter."""
+    """conv1a computed inside conv1b's kernel (conv_umma.cu, FIRST form: the producer warpgroup writes conv1a's split planes
+    straight into the shared-memory A slots) against the two-kernel path (conv1a planes through HBM, then the TMA-box
+    kernel): same fp32 FMA order in conv1a, same MMA accumulation order in conv1b, so heat-map and descriptor map must be
+    BIT-identical -- including ragged tiles (208 = 13 x 16 rows, 200 x 120: half tiles in both directions at every
+    resolution) and the blanked bottom quarter."""
     W, H = size
     comp, mean = synth.pca_matrices(0)
     wts = synth.flatten_sp_weights(synth.superpoint_weights(0))
@@ -226,21 +226,40 @@ def test_fused_first_layers_bit_identical(gpu, size):
                      np.zeros((H, W), np.uint8)])
     imgs[2, ::7, ::5] = 255
     out = {}
-    # "pair": CTA-pair kernels (tcgen05.mma.cta_group::2) for conv1a+1b, conv2a, conv2b; "halo": their single-CTA forms;
-    # "box": conv1a through HBM + the TMA-box kernel for every layer
-    modes = {"pair": ("1", "1", "1"), "halo": ("1", "1", "0"), "box": ("0", "0", "0")}
-    for name, (f1, h64, pr) in modes.items():
-        os.environ["OSB_SP_FUSE1"], os.environ["OSB_SP_HALO64"], os.environ["OSB_SP_PAIR"] = f1, h64, pr
+    # "fused": conv1a + conv1b + pool in one kernel; "box": conv1a through HBM + the TMA-box kernel for every layer
+    for name, f1 in {"fused": "1", "box": "0"}.items():
+        os.environ["OSB_SP_FUSE1"] = f1
         sp = host.SuperPoint(wts, comp, mean, W, H, 0.015, 200, max_batch=3)
         res = sp.inference_batch(imgs)
         out[name] = [(sp.read("semi", b), sp.read("desc", b), res[b][0], res[b][1]) for b in range(3)]
         sp.close()
-    for k in ("OSB_SP_FUSE1", "OSB_SP_HALO64", "OSB_SP_PAIR"):
-        os.environ.pop(k)
+    os.environ.pop("OSB_SP_FUSE1")
     for b in range(3):
-        for name in ("pair", "halo"):
-            for a, c in zip(out[name][b], out["box"][b]):
-                assert np.array_equal(a, c, equal_nan=True), f"image {b}: the {name} kernels and the TMA-box kernels differ"
+        for a, c in zip(out["fused"][b], out["box"][b]):
+            assert np.array_equal(a, c, equal_nan=True), f"image {b}: the fused first layers and the two-kernel path differ"
+
+
+def test_fused_softmax_matches_two_kernel_softmax(gpu):
+    """The detector head's softmax + pixel shuffle fused into convPb's epilogue (default) against convPb writing its logits
+    and sp_softmax_shuffle_kernel (OSB_SP_FUSED_SOFTMAX=0).  Same logits; the fused form reduces max and sum over the four
+    lanes that hold a cell, the stand-alone kernel in channel order, so the heat maps agree to rounding, not bit for bit.
+    The descriptor head does not depend on the switch: bit-identical."""
+    W, H = 400, 208
+    comp, mean = synth.pca_matrices(0)
+    wts = synth.flatten_sp_weights(synth.superpoint_weights(0))
+    imgs = np.stack([synth.image(21, H, W), synth.image(22, H, W, zero_bottom_quarter=True)])
+    out = {}
+    for f in ("1", "0"):
+        os.environ["OSB_SP_FUSED_SOFTMAX"] = f
+        sp = host.SuperPoint(wts, comp, mean, W, H, 0.015, 200, max_batch=2)
+        sp.inference_batch(imgs)
+        out[f] = [(sp.read("semi", b), sp.read("desc", b)) for b in range(2)]
+        sp.close()
+    os.environ.pop("OSB_SP_FUSED_SOFTMAX")
+    for b in range(2):
+        (s1, d1), (s0, d0) = out["1"][b], out["0"][b]
+        assert np.abs(s1 - s0).max() < 1e-6 and rel_err(s1, s0) < 1e-6
+        assert np.array_equal(d1, d0)
 
 
 def test_network_vs_the_references_own_module(small_sp):
