@@ -86,6 +86,33 @@ osb_status osb_superpoint_read(osb_superpoint* h, int what, int image, float* ou
 osb_status osb_superpoint_set_profiling(osb_superpoint* h, int enable);
 osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int n);
 
+/* Convolution parity hooks (tests only): ONE layer of the tensor-core path, run by the same host functions and kernels
+ * as the SuperPoint / NetVLAD networks, on caller-supplied operands.  Weights and biases are HOST fp32, OIHW; activation
+ * operands are DEVICE pointers; every call synchronises `stream` (a cudaStream_t as void*, 0 = default stream).
+ * Split planes are fp16 NHWC [batch][H][W][C] pairs hi = fp16(s * x), lo = fp16(s * x - hi) with s a power of two.
+ *  conv_layer:  w [cout][cin][ks][ks] (cin a multiple of 64, cout <= 512, ks 1 or 3) split at w_scale (the networks use
+ *               1024); in_hi/in_lo the input planes at act_scale.  relu 0 none / 1 ReLU / 2 ReLU6, pool 1 = fused 2x2
+ *               max-pool (even H and W), out_c channels stored (a multiple of 16), max_ctas 0 = one CTA per SM.
+ *               mode 0: out_f32 [batch*Ho*Wo][out_cstride]; mode 1: planes out_hi/out_lo [batch][Ho][Wo][out_cstride] at
+ *               out_scale; mode 2: the detector head (cout 65, ks 1): softmax, dustbin dropped, 8x8 pixel shuffle into
+ *               out_f32 = heat map [batch][8H][8W].
+ *  conv_first:  SuperPoint conv1a (w1a [64][1][3][3]) + ReLU on u8 images [batch][H][W] (scaled by 1/255), planes at
+ *               act_scale: fused = 0 -> the conv1a planes [batch][H][W][64]; fused = 1 -> conv1a + conv1b (w1b
+ *               [64][64][3][3], weights at x1024) + ReLU + 2x2 max-pool in one kernel -> [batch][H/2][W/2][64].
+ *  dwconv:      depthwise 3x3 (w [C][1][3][3], pad 1, stride 1 or 2) + bias + ReLU6 on fp32 NHWC x [batch][H][W][C]
+ *               -> planes [batch][H/stride][W/stride][C] at out_scale; generic = 1 runs the one-pixel kernel at stride 1
+ *               instead of the four-pixel one. */
+osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
+                                 const void* in_hi, const void* in_lo, int batch, int height, int width, float act_scale,
+                                 int relu, int pool, int out_c, int out_cstride, int max_ctas, int mode, float* out_f32,
+                                 void* out_hi, void* out_lo, float out_scale, void* stream);
+osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const float* w1b, const float* b1b,
+                                 const uint8_t* images_dev, int batch, int height, int width, float act_scale, int fused,
+                                 void* out_hi, void* out_lo, int max_ctas, void* stream);
+osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
+                             int channels, int stride, int generic, float out_scale, void* out_hi, void* out_lo,
+                             void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * NetVLAD global descriptor -- replaces class MobileNetVLADTensorRT
  *   (swarm_loop/include/swarm_loop/mobilenetvlad_tensorrt.h:10-21, loop_cam.cpp:27 ctor, loop_cam.cpp:554 call).

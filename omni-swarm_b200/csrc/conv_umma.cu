@@ -27,6 +27,7 @@
 // tiles; the producer runs up to two A boxes and the weight ring ahead of the MMAs.
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <cmath>
 #include <type_traits>
 #include "common.cuh"
 #include "kernels.cuh"
@@ -530,6 +531,14 @@ osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bia
       for (int t = 0; t < L->taps; ++t) {
         const float s = w_oihw[((size_t)o * cin + c) * L->taps + t] * w_scale;
         const __half h = __float2half_rn(s);
+        if (!std::isfinite(__half2float(h))) {
+          char buf[192];
+          snprintf(buf, sizeof(buf), "weight %g (output %d, input %d, tap %d) is outside the split-fp16 range: "
+                   "|w| * %g must be below 65520", (double)w_oihw[((size_t)o * cin + c) * L->taps + t], o, c, t,
+                   (double)w_scale);
+          set_error("umma_layer_upload", buf);
+          return OSB_ERR_INVALID;
+        }
         const size_t idx = ((size_t)t * L->n_pad + o) * cin + c;
         hi[idx] = h;
         lo[idx] = __float2half_rn(s - __half2float(h));
@@ -762,9 +771,9 @@ __global__ void dwconv3x3_split_s1x4_kernel(const float* __restrict__ w, const f
 }
 
 osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const float* x, __half* out_hi, __half* out_lo,
-                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st) {
+                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4) {
   const int Ho = H / stride, Wo = W / stride;
-  if (stride == 1) {
+  if (stride == 1 && s1x4) {
     const int64_t total4 = (int64_t)B * H * ((W + 3) / 4) * (C / 8);
     OSB_LAUNCH(dwconv3x3_split_s1x4_kernel, (unsigned)cdiv64(total4, 128), 128, 0, st, w_tap_c, bias, x, out_hi, out_lo,
                H, W, C, out_scale, total4);
@@ -787,3 +796,111 @@ osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const 
 }
 
 }  // namespace osb
+
+// --------------------------------------------------------------------------------------------------------------
+// parity hooks: one layer of the networks' tensor-core path on caller-supplied operands (tests only)
+// --------------------------------------------------------------------------------------------------------------
+using namespace osb;
+
+namespace {
+// [cout][taps] (OIHW with one input channel) -> [tap][cout], on the device
+osb_status upload_tap_major(float** dst, const float* w_oihw, int cout) {
+  std::vector<float> t(9 * (size_t)cout);
+  for (int o = 0; o < cout; ++o)
+    for (int k = 0; k < 9; ++k) t[(size_t)k * cout + o] = w_oihw[(size_t)o * 9 + k];
+  OSB_CUDA(cudaMalloc(dst, t.size() * sizeof(float)));
+  OSB_CUDA(cudaMemcpy(*dst, t.data(), t.size() * sizeof(float), cudaMemcpyHostToDevice));
+  return OSB_OK;
+}
+osb_status upload_f32(float** dst, const float* src, size_t n) {
+  OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
+  OSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
+  return OSB_OK;
+}
+}  // namespace
+
+extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
+                                            const void* in_hi, const void* in_lo, int batch, int height, int width,
+                                            float act_scale, int relu, int pool, int out_c, int out_cstride, int max_ctas,
+                                            int mode, float* out_f32, void* out_hi, void* out_lo, float out_scale,
+                                            void* stream) {
+  OSB_REQUIRE(w && bias && in_hi && in_lo, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (ks == 1 || ks == 3), "bad geometry");
+  OSB_REQUIRE(relu >= 0 && relu <= 2 && mode >= 0 && mode <= 2, "relu must be 0..2, mode 0 (fp32), 1 (planes) or 2 (softmax)");
+  OSB_REQUIRE(mode == 1 ? (out_hi && out_lo) : (out_f32 != nullptr), "null output");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  UmmaLayer L;
+  CUtensorMap a_hi, a_lo;
+  s = umma_layer_upload(&L, w, bias, cin, cout, ks, w_scale);
+  if (s == OSB_OK)
+    s = umma_act_maps(&a_hi, &a_lo, (__half*)in_hi, (__half*)in_lo, batch, height, width, cin, ks);
+  if (s == OSB_OK && mode == 2)
+    s = umma_conv_softmax_forward(L, a_hi, a_lo, batch, height, width, act_scale, out_f32, st, max_ctas);
+  else if (s == OSB_OK)
+    s = umma_conv_forward(L, a_hi, a_lo, batch, height, width, act_scale, mode == 1 ? (__half*)out_hi : nullptr,
+                          mode == 1 ? (__half*)out_lo : nullptr, mode == 0 ? out_f32 : nullptr, out_c, out_cstride,
+                          out_scale, relu, pool, st, max_ctas);
+  const cudaError_t e = cudaStreamSynchronize(st);         // the weights are freed below
+  umma_layer_free(&L);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const float* w1b, const float* b1b,
+                                            const uint8_t* images_dev, int batch, int height, int width, float act_scale,
+                                            int fused, void* out_hi, void* out_lo, int max_ctas, void* stream) {
+  OSB_REQUIRE(w1a && b1a && images_dev && out_hi && out_lo && (!fused || (w1b && b1b)), "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (fused) {
+    std::vector<float> w9(9 * 64);
+    for (int o = 0; o < 64; ++o)
+      for (int t = 0; t < 9; ++t) w9[t * 64 + o] = w1a[o * 9 + t];
+    UmmaLayer L;
+    s = umma_layer_upload(&L, w1b, b1b, 64, 64, 3, 1024.f);
+    if (s == OSB_OK)
+      s = umma_conv1_fused_forward(L, w9.data(), b1a, images_dev, batch, height, width, act_scale, (__half*)out_hi,
+                                   (__half*)out_lo, act_scale, st, max_ctas);
+    const cudaError_t e = cudaStreamSynchronize(st);
+    umma_layer_free(&L);
+    if (s == OSB_OK) OSB_CUDA(e);
+    return s;
+  }
+  float *wd = nullptr, *bd = nullptr, *lut = nullptr;
+  std::vector<float> l(256);
+  for (int v = 0; v < 256; ++v) l[v] = (float)v * (float)(1.0 / 255.0);
+  s = upload_tap_major(&wd, w1a, 64);
+  if (s == OSB_OK) s = upload_f32(&bd, b1a, 64);
+  if (s == OSB_OK) s = upload_f32(&lut, l.data(), 256);
+  if (s == OSB_OK)
+    s = umma_first_forward(wd, bd, lut, images_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, act_scale, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(wd); cudaFree(bd); cudaFree(lut);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
+                                        int width, int channels, int stride, int generic, float out_scale, void* out_hi,
+                                        void* out_lo, void* stream) {
+  OSB_REQUIRE(w && bias && x_dev && out_hi && out_lo, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0 && (stride == 1 || stride == 2),
+              "bad geometry (channels must be a multiple of 8, stride 1 or 2)");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  float *wd = nullptr, *bd = nullptr;
+  s = upload_tap_major(&wd, w, channels);
+  if (s == OSB_OK) s = upload_f32(&bd, bias, channels);
+  if (s == OSB_OK)
+    s = umma_dwconv_forward(wd, bd, x_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, channels, stride,
+                            out_scale, st, !generic);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(wd); cudaFree(bd);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}

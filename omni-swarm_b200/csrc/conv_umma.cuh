@@ -6,6 +6,11 @@
 
 namespace osb {
 
+// Range of the split planes: an operand x is stored as hi = fp16(scale * x), lo = fp16(scale * x - hi), and fp16 rounds
+// |v| >= 65520 to infinity, so x is representable only for |x| < 65520 / scale: activations below 4095 at the networks'
+// x16, weights below 63.984375 at x1024.  umma_layer_upload rejects weights outside that range (OSB_ERR_INVALID).  An
+// ACTIVATION beyond it is written as hi = +-inf, lo = -+inf; the next layer's sums are then NaN, which a following ReLU
+// (fmaxf) or max-pool turns into a finite value, so that overflow is silent (pinned by tests/test_gpu_conv_layers.py).
 // weights of one conv layer as two fp16 planes [tap][n_pad][Cin] (K-major rows) + their TMA descriptors
 struct UmmaLayer {
   int cin = 0, cout = 0, n_pad = 0, ks = 1, taps = 1;
@@ -41,7 +46,8 @@ osb_status umma_conv1_fused_forward(const UmmaLayer& L1b, const float* w1a, cons
                                     int max_ctas = 0);
 osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
-// depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv)
+// depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv).  Stride 1 runs
+// the four-pixel kernel unless s1x4 = false (the generic kernel; the planes are bit-identical)
 osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const float* x, __half* out_hi, __half* out_lo,
-                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st);
+                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4 = true);
 }  // namespace osb

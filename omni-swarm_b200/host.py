@@ -576,5 +576,72 @@ class Swarm:
         _l.check(self._lib.osb_swarm_wait(self._h, C.c_void_p(stream)))
 
 
+def conv_layer_parity(w, bias, in_hi, in_lo, act_scale: float, *, w_scale: float = 1024.0, relu: int = 0, pool: int = 0,
+                      out_c: int | None = None, out_cstride: int | None = None, max_ctas: int = 0, mode: str = "f32",
+                      out_scale: float = 1.0):
+    """One tensor-core convolution layer (osb_conv_layer_parity).  w [cout,cin,ks,ks], bias [cout] float32 (numpy);
+    in_hi / in_lo: CUDA torch.float16 [B,H,W,cin] split planes at act_scale.  Outputs are CUDA tensors pre-filled with NaN,
+    so anything the kernel did not write stays NaN:  mode "f32" -> [B,Ho,Wo,out_cstride] float32; "planes" -> (hi, lo)
+    [B,Ho,Wo,out_cstride] float16 at out_scale; "softmax" (the 65-logit detector head) -> heat map [B,8H,8W] float32."""
+    import torch
+    w, b = _f32(w), _f32(bias)
+    cout, cin, ks = w.shape[0], w.shape[1], w.shape[2]
+    B, H, W, c = in_hi.shape
+    assert c == cin and in_hi.dtype == torch.float16 and in_lo.shape == in_hi.shape and in_hi.is_contiguous() \
+        and in_lo.is_contiguous()
+    n_pad = 64 if cout <= 64 else 80 if cout <= 80 else 128 if cout <= 128 else 256 if cout <= 256 else 512
+    out_c = n_pad if out_c is None else out_c
+    out_cstride = out_c if out_cstride is None else out_cstride
+    Ho, Wo = (H // 2, W // 2) if pool else (H, W)
+    dev = in_hi.device
+    f32 = hi = lo = None
+    if mode == "softmax":
+        f32 = torch.full((B, 8 * H, 8 * W), float("nan"), dtype=torch.float32, device=dev)
+    elif mode == "f32":
+        f32 = torch.full((B, Ho, Wo, out_cstride), float("nan"), dtype=torch.float32, device=dev)
+    else:
+        hi = torch.full((B, Ho, Wo, out_cstride), float("nan"), dtype=torch.float16, device=dev)
+        lo = torch.full_like(hi, float("nan"))
+    code = {"f32": 0, "planes": 1, "softmax": 2}[mode]
+    dp = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    _l.check(_l.load().osb_conv_layer_parity(
+        _l.ptr(w), _l.ptr(b), cin, cout, ks, float(w_scale), dp(in_hi), dp(in_lo), B, H, W, float(act_scale), int(relu),
+        int(pool), out_c, out_cstride, int(max_ctas), code, dp(f32), dp(hi), dp(lo), float(out_scale),
+        C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    return (hi, lo) if mode == "planes" else f32
+
+
+def conv_first_parity(w1a, b1a, images, act_scale: float, *, fused: bool = False, w1b=None, b1b=None, max_ctas: int = 0):
+    """SuperPoint's first layer(s) (osb_conv_first_parity): images CUDA torch.uint8 [B,H,W] -> (hi, lo) float16 planes at
+    act_scale: conv1a + ReLU [B,H,W,64], or with fused=True conv1a + conv1b + ReLU + 2x2 max-pool [B,H/2,W/2,64]."""
+    import torch
+    B, H, W = images.shape
+    shape = (B, H // 2, W // 2, 64) if fused else (B, H, W, 64)
+    hi = torch.full(shape, float("nan"), dtype=torch.float16, device=images.device)
+    lo = torch.full_like(hi, float("nan"))
+    w1a, b1a = _f32(w1a), _f32(b1a)
+    w1b = None if w1b is None else _f32(w1b)
+    b1b = None if b1b is None else _f32(b1b)
+    _l.check(_l.load().osb_conv_first_parity(
+        _l.ptr(w1a), _l.ptr(b1a), _l.ptr(w1b), _l.ptr(b1b), C.c_void_p(images.data_ptr()), B, H, W, float(act_scale),
+        int(fused), C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()), int(max_ctas),
+        C.c_void_p(torch.cuda.current_stream(images.device).cuda_stream)))
+    return hi, lo
+
+
+def dwconv_parity(w, bias, x, out_scale: float, *, stride: int = 1, generic: bool = False):
+    """Depthwise 3x3 + bias + ReLU6 into split planes (osb_dwconv_parity): w [C,1,3,3], x CUDA float32 [B,H,W,C] ->
+    (hi, lo) float16 [B,H/stride,W/stride,C] at out_scale; generic=True runs the one-pixel kernel at stride 1."""
+    import torch
+    B, H, W, Cn = x.shape
+    hi = torch.full((B, H // stride, W // stride, Cn), float("nan"), dtype=torch.float16, device=x.device)
+    lo = torch.full_like(hi, float("nan"))
+    w, b = _f32(w), _f32(bias)
+    _l.check(_l.load().osb_dwconv_parity(
+        _l.ptr(w), _l.ptr(b), C.c_void_p(x.data_ptr()), B, H, W, Cn, int(stride), int(generic), float(out_scale),
+        C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()), C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+    return hi, lo
+
+
 def launch_count() -> int:
     return int(_l.load().osb_launch_count())

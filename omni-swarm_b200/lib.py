@@ -105,6 +105,13 @@ _SIG = {
     "osb_superpoint_read": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t]),
     "osb_superpoint_set_profiling": (C.c_int, [_P, C.c_int]),
     "osb_superpoint_layer_ms": (C.c_int, [_P, _P, C.c_int]),
+    "osb_conv_layer_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int,
+                                        C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
+                                        C.c_float, _P]),
+    "osb_conv_first_parity": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P, _P,
+                                        C.c_int, _P]),
+    "osb_dwconv_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P,
+                                    _P]),
     "osb_netvlad_create": (C.c_int, [C.POINTER(_P), _P, C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "osb_netvlad_destroy": (C.c_int, [_P]),
     "osb_netvlad_infer": (C.c_int, [_P, _P, C.c_int, _P]),

@@ -35,10 +35,11 @@ SEARCH_NEAREST_NUM = 5             # loop_defines.h:32
 # ------------------------------------------------------------------------------------------------
 # SuperPoint network: superpoint.ipynb:135-205 (module), :345-352 (export; input already /255)
 # ------------------------------------------------------------------------------------------------
-def superpoint_net(img_u8: np.ndarray, w: dict, num_threads: int | None = None):
+def superpoint_net(img_u8: np.ndarray, w: dict, num_threads: int | None = None, trace: dict | None = None):
     """img_u8 [H,W] uint8 -> (semi [H,W] f32, desc [256,H/8,W/8] f32).
 
     Pre-processing u8 -> f32 * (1/255): superpoint_tensorrt.cpp:127.
+    `trace`, if given, receives {layer: (max |input|, max |weight|)} of every convolution.
     """
     if num_threads is not None:
         torch.set_num_threads(num_threads)
@@ -48,6 +49,8 @@ def superpoint_net(img_u8: np.ndarray, w: dict, num_threads: int | None = None):
     relu = F.relu
 
     def conv(x, n, pad):
+        if trace is not None:
+            trace[n] = (float(x.abs().max()), float(t[n + ".weight"].abs().max()))
         return F.conv2d(x, t[n + ".weight"], t[n + ".bias"], padding=pad)
 
     with torch.no_grad():
@@ -171,18 +174,25 @@ def superpoint_inference(img_u8, w, thres, max_num, pca_comp, pca_mean):
 # NetVLAD stand-in (I/O contract mobilenetvlad_tensorrt.cpp:4-15; architecture is OURS, pinned in
 # omniswarm_b200/synth.py::NV_BLOCKS and DESIGN.md)
 # ------------------------------------------------------------------------------------------------
-def netvlad_net(img_u8: np.ndarray, w: dict) -> np.ndarray:
+def netvlad_net(img_u8: np.ndarray, w: dict, trace: dict | None = None) -> np.ndarray:
+    """`trace`, if given, receives {layer: (max |input|, max |weight|)} of the pointwise convolutions and the projection."""
     from omniswarm_b200 import synth
     t = {k: torch.from_numpy(np.ascontiguousarray(v)) for k, v in w.items()}
     x = torch.from_numpy(img_u8.astype(np.float32))[None, None]      # u8 -> f32 UNSCALED (:8,:10)
     relu6 = lambda v: torch.clamp(v, 0.0, 6.0)
+
+    def pointwise(x, n):
+        if trace is not None:
+            trace[n] = (float(x.abs().max()), float(t[n + ".weight"].abs().max()))
+        return F.conv2d(x, t[n + ".weight"], t[n + ".bias"])
+
     with torch.no_grad():
         x = x * np.float32(synth.NV_INPUT_SCALE)
         x = relu6(F.conv2d(x, t["conv0.weight"], t["conv0.bias"], stride=2, padding=1))
         for i, (ci, co, s) in enumerate(synth.NV_BLOCKS):
             x = relu6(F.conv2d(x, t[f"b{i}.dw.weight"], t[f"b{i}.dw.bias"], stride=s, padding=1, groups=ci))
-            x = relu6(F.conv2d(x, t[f"b{i}.pw.weight"], t[f"b{i}.pw.bias"]))
-        x = F.conv2d(x, t["proj.weight"], t["proj.bias"])            # [1,D,h,w]
+            x = relu6(pointwise(x, f"b{i}.pw"))
+        x = pointwise(x, "proj")                                      # [1,D,h,w]
         x = x - x.mean(dim=(2, 3), keepdim=True)                      # per-image centring (makes random-weight
         x = x / torch.clamp(torch.norm(x, dim=1, keepdim=True), min=1e-12)   # descriptors image-specific); per-location L2
         a = torch.softmax(F.conv2d(x, t["assign.weight"], t["assign.bias"]), 1)   # [1,K,h,w]

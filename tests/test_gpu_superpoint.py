@@ -3,7 +3,8 @@
 Parity definition (SURVEY.md section 7 hard part 1 / section 8 item 7):
   * post-processing (threshold, NMS2, top-K, sampling, norm, PCA) given the SAME engine outputs:
     keypoints and their order bit-exact, descriptors <= 1e-4 relative;
-  * network outputs: semi / desc <= 1e-4 relative to the fp32 oracle;
+  * network outputs: semi <= 1e-4, desc and NetVLAD <= 1e-5 relative to the fp32 oracle (a few times what an H100
+    measures, DESIGN.md section 4; the kernels themselves are bounded layer by layer in test_gpu_conv_layers.py);
   * end to end: keypoints identical except where the oracle heat-map is within a margin of a decision boundary
     (threshold or a neighbour's confidence), which is reported and bounded.
 """
@@ -114,8 +115,9 @@ def full_sp(gpu):
 
 
 def test_network_full_size_vs_oracle(full_sp):
-    """640x480 (BASELINE config 2): semi / desc within 1e-4 rel of the fp32 oracle; stage-wise keypoint parity
-    bit-exact on the device's own heat-map; end-to-end keypoints equal up to decision-margin cases."""
+    """640x480 (BASELINE config 2): semi / desc against the fp32 oracle; stage-wise keypoint parity bit-exact on the
+    device's own heat-map; end-to-end keypoints equal up to decision-margin cases.  Tolerances: about 3x (heat-map) and
+    4x (descriptors) what an H100 measures on these images (DESIGN.md section 4)."""
     comp, mean = synth.pca_matrices(0)
     w = synth.superpoint_weights(0)
     imgs = np.stack([synth.image(0), synth.image(1, zero_bottom_quarter=True)])
@@ -123,8 +125,8 @@ def test_network_full_size_vs_oracle(full_sp):
     for b in range(2):
         semi_o, desc_o = fr.superpoint_net(imgs[b], w)
         semi, desc = full_sp.read("semi", b), full_sp.read("desc", b)
-        assert rel_err(semi, semi_o) < 1e-4 and rel_err(desc, desc_o) < 1e-4
-        assert np.abs(semi - semi_o).max() < 1e-4       # tensor-core accumulation truncates: ~6e-5 observed
+        assert rel_err(semi, semi_o) < 1e-4 and rel_err(desc, desc_o) < 1e-5      # measured 3.5e-5, 2.3e-6
+        assert np.abs(semi - semi_o).max() < 7.5e-5                                # measured 2.6e-5
         # stage-wise: oracle post-processing applied to the DEVICE heat-map must agree bit-exactly
         k, d = out[b]
         rk, rc = fr.get_keypoints(semi, 0.015, 200)
@@ -150,13 +152,14 @@ def test_netvlad_vs_oracle(gpu):
     z = np.load(os.path.join(GOLDEN, "netvlad.npz"))
     nv = host.NetVLAD(synth.flatten_nv_weights(nvw), W0, H0, max_batch=2)
     v = nv.inference(z["img"])
-    assert rel_err(v, z["out"]) < 1e-4 and abs(np.linalg.norm(v) - 1) < 1e-5
+    assert rel_err(v, z["out"]) < 1e-5 and abs(np.linalg.norm(v) - 1) < 1e-5
     nv.close()
     nv = host.NetVLAD(synth.flatten_nv_weights(nvw), 640, 480, max_batch=4)
     imgs = np.stack([synth.image(s) for s in range(3)])
     out = nv.inference_batch(imgs)
     for b in range(3):
-        assert rel_err(out[b], fr.netvlad_net(imgs[b], nvw)) < 1e-4
+        # an H100 measures at most 2.1e-6 (DESIGN.md section 4): about 5x margin
+        assert rel_err(out[b], fr.netvlad_net(imgs[b], nvw)) < 1e-5
     # distinct images give distinct descriptors; same image gives the same descriptor regardless of batch slot
     assert np.abs(out[0] @ out[1]) < 0.9999       # (random-weight stand-in: textures of one generator stay similar)
     assert np.array_equal(nv.inference(imgs[2]), out[2])
@@ -175,7 +178,7 @@ def test_onboard_resolution_400x208(gpu):
     for b in range(2):
         semi_o, desc_o = fr.superpoint_net(imgs[b], w)
         semi, desc = sp.read("semi", b), sp.read("desc", b)
-        assert rel_err(semi, semi_o) < 1e-4 and rel_err(desc, desc_o) < 1e-4
+        assert rel_err(semi, semi_o) < 1e-4 and rel_err(desc, desc_o) < 1e-5      # measured 3.4e-5, 2.2e-6
         k, d = out[b]
         rk, _ = fr.get_keypoints(semi, 0.015, 200)
         assert np.array_equal(k, rk)                      # bit-exact on the device's own heat-map
@@ -185,13 +188,14 @@ def test_onboard_resolution_400x208(gpu):
     nv = host.NetVLAD(synth.flatten_nv_weights(nvw), W, H, max_batch=2)
     v = nv.inference_batch(imgs)
     for b in range(2):
-        assert rel_err(v[b], fr.netvlad_net(imgs[b], nvw)) < 1e-4
+        assert rel_err(v[b], fr.netvlad_net(imgs[b], nvw)) < 1e-5                 # measured 1.7e-6
     nv.close()
 
 
 def test_tensor_core_path_vs_cuda_core_path(gpu):
     """The tensor-core convolutions (split-fp16, 3 products per K step) and the fp32 FFMA convolutions are two
-    implementations of the same network: both must sit within 1e-4 of the fp32 oracle, and within 1e-5 of each other."""
+    implementations of the same network, both compared with the fp32 oracle and with each other.  Tolerances: about 3x
+    what an H100 measures on these images (DESIGN.md section 4); the layer-level bound is tests/test_gpu_conv_layers.py."""
     comp, mean = synth.pca_matrices(0)
     wts = synth.flatten_sp_weights(synth.superpoint_weights(0))
     img = np.stack([synth.image(3), synth.image(4, zero_bottom_quarter=True)])
@@ -206,9 +210,11 @@ def test_tensor_core_path_vs_cuda_core_path(gpu):
     w = synth.superpoint_weights(0)
     for b in range(2):
         so, do = fr.superpoint_net(img[b], w)
-        for mode in ("umma", "ffma"):
-            assert rel_err(out[mode][b][0], so) < 1e-4 and rel_err(out[mode][b][1], do) < 1e-4, mode
-        assert np.abs(out["umma"][b][0] - out["ffma"][b][0]).max() < 1e-4
+        # measured: umma 3.5e-5 / 2.2e-6, ffma 5.4e-6 / 1.3e-6 (heat-map / descriptors, relative)
+        assert rel_err(out["umma"][b][0], so) < 1e-4 and rel_err(out["umma"][b][1], do) < 1e-5
+        assert rel_err(out["ffma"][b][0], so) < 2e-5 and rel_err(out["ffma"][b][1], do) < 5e-6
+        assert np.abs(out["umma"][b][0] - out["ffma"][b][0]).max() < 7.5e-5      # measured 2.5e-5
+        assert np.abs(out["umma"][b][1] - out["ffma"][b][1]).max() < 5e-6        # measured 1.1e-6
         print("rel err vs oracle (semi, desc):", {m: (rel_err(out[m][b][0], so), rel_err(out[m][b][1], do)) for m in out})
 
 
