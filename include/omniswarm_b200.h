@@ -228,6 +228,37 @@ osb_status osb_solver_destroy(osb_solver* h);
 osb_status osb_solver_solve(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed, int n_factors,
                             const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
                             const uint8_t* huber, const osb_solve_options* opt, osb_solve_summary* summary);
+/* Random-restart initialisation -- solve_with_multiple_init (swarm_localization_solver.cpp:781-845, called at :925):
+ * n_trials solves of the same graph, all in ONE launch (one thread-block cluster per trial when the graph fits the
+ * one-cluster path; otherwise the trials run one after another as cooperative grids).  Trial t starts from `poses` with
+ * every node whose init_mask[node] is set and that is not fixed scattered as random_init_pose (:204-216) does: x, y
+ * uniform in [-rand_xy, rand_xy), z in [-rand_z, rand_z), yaw kept (the adapter supplies the odometry yaw there, :212).
+ * The draws are a counter hash of (seed, t, node, component) (oracle/multistart_ref.py: multistart_initial_poses).
+ * Each trial runs exactly the arithmetic of osb_solver_solve from its starting poses.  Then, as :783-831:
+ *   equv_t = normalise ? sqrt(final_cost_t) / n_residuals / window_size : final_cost_t      (:1721-1725)
+ *   best = acpt_cost; trial t is chosen iff equv_t < best (strictly; the first of equal minima wins, NaN never does).
+ * poses is overwritten with the chosen trial's result; when no trial is accepted *chosen = -1 and poses is untouched.
+ * trial_summaries[t] is filled for every trial; their solve_ms is the device time of the whole batch.
+ * Unlike the reference, every trial starts from the caller's poses (its trial i starts from trial i-1's solution for the
+ * nodes it does not scatter), and the draws are hashed instead of rand().
+ * Memory: a per-handle arena, grown to the largest call and kept until osb_solver_destroy, of about
+ *   704 n + 512 m + 64 G + 48 bytes per trial (n nodes, m factors, G CTAs per solve: <= 16 on the cluster path, <= the
+ *   SM count otherwise), plus 128 m (fp32 inner) / 256 m (fp64) when the Jacobians do not fit shared memory, plus
+ *   40 n + 48 n_trials + 1 KB.  A failed allocation returns OSB_ERR_CUDA and leaves the handle usable. */
+typedef struct {
+  int32_t n_trials;      /* INIT_TRIAL = 3 (solver.cpp:54); 1 ... 256 */
+  int32_t normalise;     /* 1: equv_cost = sqrt(final_cost)/n_residuals/window_size (the reference's num_res_blks > 1) */
+  int32_t window_size;   /* sliding_window_size() (solver.cpp:1724); >= 1 when normalise */
+  uint64_t seed;
+  double rand_xy, rand_z;   /* RAND_INIT_XY = 5, RAND_INIT_Z = 1 (solver.cpp:51-52); finite, >= 0 */
+  double acpt_cost;         /* max_accept_cost (swarm_localization_node.cpp:470); not NaN */
+} osb_multistart_options;
+osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed,
+                                       const uint8_t* init_mask, int n_factors, const int32_t* type, const int32_t* ia,
+                                       const int32_t* ib, const double* payload, const uint8_t* huber,
+                                       const osb_solve_options* opt, const osb_multistart_options* ms,
+                                       osb_solve_summary* trial_summaries /*[n_trials]*/, double* equv_costs /*[n_trials]*/,
+                                       int32_t* chosen);
 /* Resident graph (SURVEY.md 8f-4): instead of re-flattening the whole window for every solve (the reference rebuilds its
  * ceres::Problem each time: setup_problem_with_sferror / _loops_and_detections / _ego_motion,
  * swarm_localization_solver.cpp:1064-1214), the adapter appends what add_new_swarm_frame / add_new_loop_connection

@@ -207,7 +207,33 @@ class FlatPoseGraph {
     for (int i = 0; i < n; ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
     return s;
   }
+  // random_init_pose (solver.cpp:204-216): the caller marks every pose block of the drones in ids_to_init except
+  // self_id, with the odometry yaw already in pose[3] (:212)
+  void mark_for_init(double* pose) {
+    const int id = node(pose);
+    if (init_mask_.size() <= (size_t)id) init_mask_.resize(id + 1, 0);
+    init_mask_[id] = 1;
+  }
+  // solve_with_multiple_init (:781-845): ms.n_trials solves from random restarts of the marked blocks, one launch.  The
+  // pose blocks are written back only when a trial got below ms.acpt_cost; returns that (cost_updated, :844).
+  bool solve_with_multiple_init(osb_solver* solver, const osb_multistart_options& ms, const osb_solve_options* opt = nullptr) {
+    const int n = (int)ptr_.size(), m = (int)type_.size();
+    std::vector<double> poses((size_t)n * 4);
+    for (int i = 0; i < n; ++i) for (int j = 0; j < 4; ++j) poses[4 * i + j] = ptr_[i][j];
+    init_mask_.resize(n, 0);
+    std::vector<osb_solve_summary> summaries(ms.n_trials > 0 ? ms.n_trials : 1);
+    std::vector<double> equv(summaries.size());
+    int32_t chosen = -1;
+    check(osb_solver_solve_multistart(solver, n, poses.data(), fixed_.data(), init_mask_.data(), m, type_.data(), ia_.data(),
+                                      ib_.data(), payload_.data(), huber_.data(), opt, &ms, summaries.data(), equv.data(),
+                                      &chosen), "osb_solver_solve_multistart");
+    if (chosen < 0) return false;
+    for (int i = 0; i < n; ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
+    cost_now = equv[chosen];
+    return true;
+  }
   int num_factors() const { return (int)type_.size(); }
+  double cost_now = 0.0;             // equv_cost of the trial solve_with_multiple_init accepted last (:809)
 
  private:
   void push(int type, double* pa, double* pb, const double* pl, bool huber) {
@@ -216,7 +242,7 @@ class FlatPoseGraph {
   }
   std::vector<double*> ptr_;
   std::unordered_map<double*, int> index_;
-  std::vector<uint8_t> fixed_, huber_;
+  std::vector<uint8_t> fixed_, huber_, init_mask_;
   std::vector<int32_t> type_, ia_, ib_;
   std::vector<double> payload_;
 };

@@ -19,7 +19,9 @@
 // are hardware cluster barriers instead of software grid barriers.
 #include <cooperative_groups.h>
 #include <algorithm>
+#include <cmath>
 #include <cstring>
+#include <type_traits>
 #include "common.cuh"
 
 namespace cg = cooperative_groups;
@@ -211,7 +213,40 @@ struct SolverDev {
   const int32_t* es_slot;  // [m] -1, or 2 * (index into es) + (1 if the factor's node a is the later node of the pair)
   double* es;              // [<= m][16] J_i^T J_{i-1} of the chain factors (written at every linearisation)
   double* En;              // [n][16] summed coupling block of node i with node i-1
+  // batched trials (osb_solver_solve_multistart): CTA b solves trial first_trial + b / ctas as CTA b % ctas of that
+  // solve.  Every state pointer above (x .. En) is trial 0's; trial t's lies t * tstride bytes further.  The graph
+  // tables (fixed .. slot_b, link, es_ptr, es_slot) are shared, and only trial 0 writes dbg.
+  int ctas;                // CTAs per solve (the cluster size on the cluster path)
+  int first_trial;
+  long long tstride;
 };
+
+// trial t's copy of a per-trial state pointer lies t * tstride bytes past trial 0's.  It is recomputed at every use from
+// the cluster id (a special register) rather than shifted once at the start: twenty shifted pointers held for the whole
+// solve would not fit beside the solver's working set, which already fills the 255 registers.  A cooperative launch
+// runs one trial, whose pointers the host has already shifted.
+// MULTI = false (one solve per launch) compiles this away: reading the cluster id at every use costs the latency-bound
+// CG loop about 10 % (measured on C5), so a single solve runs the graph_solve_kernel<T, false> instantiation.
+template <bool MULTI, typename Q>
+__device__ __forceinline__ Q* tp(const SolverDev& P, Q* p) {
+  if (!MULTI) return p;
+  unsigned c;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(c));
+  return reinterpret_cast<Q*>(reinterpret_cast<char*>(p) + (long long)c * P.tstride);
+}
+
+// this CTA's index inside its solve, and the solve's trial (a cooperative launch is one solve of `ctas` = gridDim CTAs)
+__device__ __forceinline__ int solve_rank(const SolverDev& P) {
+  unsigned r;
+  if (P.use_cluster) asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); else r = blockIdx.x;
+  return (int)r;
+}
+template <bool MULTI>
+__device__ __forceinline__ int solve_trial(const SolverDev& P) {
+  unsigned c = 0;
+  if (MULTI) asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(c));
+  return P.first_trial + (int)c;
+}
 
 __device__ __forceinline__ void all_sync(const SolverDev& P, cg::grid_group& grid) {
   if (P.use_cluster) cg::this_cluster().sync(); else grid.sync();
@@ -226,10 +261,10 @@ __device__ __forceinline__ double warp_sum_t(double v) { return warp_sum_d(v); }
 
 // grid-wide sums of K values.  The warp level runs in T (cheap in fp32), the 8 warp sums, the CTA partials and the final
 // sum are fp64 (a handful of instructions on warp 0 only).
-template <int K, typename T>
+template <int K, bool MT, typename T>
 __device__ void grid_reduce_sum(T (&vin)[K], double (&v)[K], const SolverDev& P, int parity, double* sh, cg::grid_group& grid) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = GS_THREADS / 32, G = gridDim.x;
-  double* pbuf = P.partial + (size_t)parity * 4 * G;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = GS_THREADS / 32, G = P.ctas;
+  double* pbuf = tp<MT>(P, P.partial) + (size_t)parity * 4 * G;
   __syncwarp();
 #pragma unroll
   for (int k = 0; k < K; ++k) {
@@ -242,7 +277,7 @@ __device__ void grid_reduce_sum(T (&vin)[K], double (&v)[K], const SolverDev& P,
     for (int k = 0; k < K; ++k) {
       double xv = (lane < nw) ? sh[k * 32 + lane] : 0.0;
       xv = warp_sum_d(xv);
-      if (lane == 0) __stcg(pbuf + k * G + blockIdx.x, xv);
+      if (lane == 0) __stcg(pbuf + k * G + solve_rank(P), xv);
     }
   }
   all_sync(P, grid);
@@ -261,19 +296,20 @@ __device__ void grid_reduce_sum(T (&vin)[K], double (&v)[K], const SolverDev& P,
   __syncthreads();
 }
 
+template <bool MT>
 __device__ double grid_reduce_max(double vmax, const SolverDev& P, int parity, double* sh, cg::grid_group& grid) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, G = gridDim.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, G = P.ctas;
   __syncwarp();
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) vmax = fmax(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
   if (lane == 0) sh[warp] = vmax;
   __syncthreads();
-  double* pbuf = P.partial + (size_t)parity * 4 * G;
+  double* pbuf = tp<MT>(P, P.partial) + (size_t)parity * 4 * G;
   if (warp == 0) {
     double xv = (lane < GS_THREADS / 32) ? sh[lane] : 0.0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) xv = fmax(xv, __shfl_xor_sync(0xffffffffu, xv, o));
-    if (lane == 0) __stcg(pbuf + blockIdx.x, xv);
+    if (lane == 0) __stcg(pbuf + solve_rank(P), xv);
   }
   all_sync(P, grid);
   if (warp == 0) {
@@ -407,10 +443,10 @@ __device__ __forceinline__ void chain_apply(const T (&Si)[16], const T (&L)[16],
 // Linearise every factor of this CTA at `xp` (fp64): robustified Jacobians -> J store (as T), gradient contributions
 // J^T r -> gs slots, diagonal-block contributions J^T J -> hs slots, chain couplings -> es.  Returns this thread's share
 // of the cost.
-template <typename T>
+template <bool MT, typename T>
 __device__ double factor_linearize(const SolverDev& P, const double* __restrict__ xp, const JStore<T>& J) {
   double cost = 0.0;
-  const int f0 = blockIdx.x * P.fpc, f1 = min(P.m, f0 + P.fpc);
+  const int f0 = solve_rank(P) * P.fpc, f1 = min(P.m, f0 + P.fpc);
   for (int f = f0 + threadIdx.x; f < f1; f += GS_THREADS) {
     const int li = f - f0;
     const int a = P.ia[f], b = P.ib[f];
@@ -436,7 +472,7 @@ __device__ double factor_linearize(const SolverDev& P, const double* __restrict_
       if (es >= 0) {                      // E = J_later^T J_earlier (rows: the later node of the pair)
         const double* Jl = (es & 1) ? Ja : Jb;
         const double* Je = (es & 1) ? Jb : Ja;
-        double* dst = P.es + 16 * (size_t)(es >> 1);
+        double* dst = tp<MT>(P, P.es) + 16 * (size_t)(es >> 1);
 #pragma unroll
         for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -448,10 +484,10 @@ __device__ double factor_linearize(const SolverDev& P, const double* __restrict_
           }
       }
     }
-    double* ga = P.gs + 4 * (size_t)P.slot_a[f];
-    double* gb = P.gs + 4 * (size_t)P.slot_b[f];
-    double* ha = P.hs + 16 * (size_t)P.slot_a[f];
-    double* hb = P.hs + 16 * (size_t)P.slot_b[f];
+    double* ga = tp<MT>(P, P.gs) + 4 * (size_t)P.slot_a[f];
+    double* gb = tp<MT>(P, P.gs) + 4 * (size_t)P.slot_b[f];
+    double* ha = tp<MT>(P, P.hs) + 16 * (size_t)P.slot_a[f];
+    double* hb = tp<MT>(P, P.hs) + 16 * (size_t)P.slot_b[f];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       double sa = 0.0, sb = 0.0;
@@ -471,10 +507,10 @@ __device__ double factor_linearize(const SolverDev& P, const double* __restrict_
 }
 
 // cost at the trial point `xn` (fp64) and this thread's share of |J_cur delta|^2 (model decrease, in T)
-template <typename T>
+template <bool MT, typename T>
 __device__ void factor_trial(const SolverDev& P, const double* __restrict__ xn, const JStore<T>& J, double& cost, double& jd) {
-  const int f0 = blockIdx.x * P.fpc, f1 = min(P.m, f0 + P.fpc);
-  const T* delta = static_cast<const T*>(P.delta);
+  const int f0 = solve_rank(P) * P.fpc, f1 = min(P.m, f0 + P.fpc);
+  const T* delta = static_cast<const T*>(tp<MT>(P, P.delta));
   T jdt = T(0);
   for (int f = f0 + threadIdx.x; f < f1; f += GS_THREADS) {
     const int li = f - f0;
@@ -497,28 +533,32 @@ __device__ void factor_trial(const SolverDev& P, const double* __restrict__ xn, 
   jd += (double)jdt;
 }
 
-template <typename T>
+template <typename T, bool MT>
 __global__ void __launch_bounds__(GS_THREADS, 1)
 graph_solve_kernel(SolverDev P) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* smem_j = reinterpret_cast<T*>(smem_raw);
   __shared__ double sh[4 * 32];
-  const int T_ = gridDim.x * GS_THREADS;
-  const int gtid = blockIdx.x * GS_THREADS + threadIdx.x;
+  // from here on "the grid" is this trial's solve: `ctas` CTAs, thread ids counted inside it
+  const int trial = solve_trial<MT>(P);
+  const bool dbg_trial = trial == 0;
+  const int T_ = P.ctas * GS_THREADS;
+  const int gtid = solve_rank(P) * GS_THREADS + threadIdx.x;
   JStore<T> J;
   if (P.j_in_smem) { J.base = smem_j; J.stride = P.fpc; J.off = 0; }
-  else { J.base = static_cast<T*>(P.Jg); J.stride = P.m; J.off = blockIdx.x * P.fpc; }
+  else { J.base = static_cast<T*>(tp<MT>(P, P.Jg)); J.stride = P.m; J.off = solve_rank(P) * P.fpc; }
   T* Ls = smem_j + (size_t)32 * P.fpc;          // [16][GS_THREADS]: L_i of the chain preconditioner (use_chain only)
-  T* const Pp = static_cast<T*>(P.p); T* const Pz = static_cast<T*>(P.z); T* const Pres = static_cast<T*>(P.res);
-  T* const PAp = static_cast<T*>(P.Ap); T* const Pdelta = static_cast<T*>(P.delta); T* const PMinv = static_cast<T*>(P.Minv);
-  T* const Pcs = static_cast<T*>(P.cs);
+  const auto Pp = [&] { return static_cast<T*>(tp<MT>(P, P.p)); }; const auto Pz = [&] { return static_cast<T*>(tp<MT>(P, P.z)); }; const auto Pres = [&] { return static_cast<T*>(tp<MT>(P, P.res)); };
+  const auto PAp = [&] { return static_cast<T*>(tp<MT>(P, P.Ap)); }; const auto Pdelta = [&] { return static_cast<T*>(tp<MT>(P, P.delta)); }; const auto PMinv = [&] { return static_cast<T*>(tp<MT>(P, P.Minv)); };
+  const auto Pcs = [&] { return static_cast<T*>(tp<MT>(P, P.cs)); };
   int parity = 0;
   unsigned long long t0 = 0;
   const long long k0 = clock64();
-  if (gtid == 0) {
+  if (gtid == 0) {                           // each trial's time limit counts from its own start
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t0));
-    for (int i = 0; i < 8 + GS_MAX_CLUSTER * (GS_THREADS / 32); ++i) P.dbg[i] = 0;
+    if (dbg_trial)
+      for (int i = 0; i < 8 + GS_MAX_CLUSTER * (GS_THREADS / 32); ++i) P.dbg[i] = 0;
   }
 
   int cur = 0;
@@ -527,12 +567,12 @@ graph_solve_kernel(SolverDev P) {
   int iters = 0, pcg_total = 0, termination = 3;
 
   // ---- initial linearisation ----
-  double v1[1], w1[1] = {factor_linearize(P, P.x[0], J)};
-  grid_reduce_sum<1>(w1, v1, P, parity, sh, grid); parity ^= 1;
+  double v1[1], w1[1] = {factor_linearize<MT>(P, tp<MT>(P, P.x[0]), J)};
+  grid_reduce_sum<1, MT>(w1, v1, P, parity, sh, grid); parity ^= 1;
   double cost = v1[0];
   const double initial_cost = cost;
   bool need_gradient = true;
-  const int f0 = blockIdx.x * P.fpc, f1 = min(P.m, f0 + P.fpc);
+  const int f0 = solve_rank(P) * P.fpc, f1 = min(P.m, f0 + P.fpc);
   // static per-thread data of the fast CG path
   const bool fast = (P.fpc <= GS_KF * GS_THREADS) && (P.n <= T_);
   int fa[GS_KF], fb[GS_KF], fsa[GS_KF], fsb[GS_KF];
@@ -562,31 +602,31 @@ graph_solve_kernel(SolverDev P) {
 #pragma unroll 2
           for (int sidx = s0; sidx < s1; ++sidx) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) gn[i] += __ldcg(P.gs + 4 * (size_t)sidx + i);
+            for (int i = 0; i < 4; ++i) gn[i] += __ldcg(tp<MT>(P, P.gs) + 4 * (size_t)sidx + i);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) Hn[i] += __ldcg(P.hs + 16 * (size_t)sidx + i);
+            for (int i = 0; i < 16; ++i) Hn[i] += __ldcg(tp<MT>(P, P.hs) + 16 * (size_t)sidx + i);
           }
         }
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          P.g[4 * n + i] = gn[i];
-          P.D[4 * n + i] = fmin(fmax(Hn[i * 5], 1e-6), 1e32);
+          tp<MT>(P, P.g)[4 * n + i] = gn[i];
+          tp<MT>(P, P.D)[4 * n + i] = fmin(fmax(Hn[i * 5], 1e-6), 1e32);
           vmax = fmax(vmax, fabs(gn[i]));
         }
 #pragma unroll
-        for (int i = 0; i < 16; ++i) P.Hnn[16 * n + i] = Hn[i];
+        for (int i = 0; i < 16; ++i) tp<MT>(P, P.Hnn)[16 * n + i] = Hn[i];
         if (P.use_chain) {
           double En[16];
 #pragma unroll
           for (int i = 0; i < 16; ++i) En[i] = 0.0;
           for (int e = P.es_ptr[n]; e < P.es_ptr[n + 1]; ++e)
 #pragma unroll
-            for (int i = 0; i < 16; ++i) En[i] += __ldcg(P.es + 16 * (size_t)e + i);
+            for (int i = 0; i < 16; ++i) En[i] += __ldcg(tp<MT>(P, P.es) + 16 * (size_t)e + i);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) P.En[16 * n + i] = En[i];
+          for (int i = 0; i < 16; ++i) tp<MT>(P, P.En)[16 * n + i] = En[i];
         }
       }
-      const double gmax = grid_reduce_max(vmax, P, parity, sh, grid); parity ^= 1;
+      const double gmax = grid_reduce_max<MT>(vmax, P, parity, sh, grid); parity ^= 1;
       need_gradient = false;
       if (gmax <= P.opt.gradient_tolerance) { termination = 1; break; }
     }
@@ -608,15 +648,15 @@ graph_solve_kernel(SolverDev P) {
       if (is_node) {
         double Md[16];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) Md[i] = P.Hnn[16 * gtid + i];
+        for (int i = 0; i < 16; ++i) Md[i] = tp<MT>(P, P.Hnn)[16 * gtid + i];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) { const double ld = lam * P.D[4 * gtid + i]; Dl[i] = (T)ld; Md[i * 5] += ld; }
+        for (int i = 0; i < 4; ++i) { const double ld = lam * tp<MT>(P, P.D)[4 * gtid + i]; Dl[i] = (T)ld; Md[i * 5] += ld; }
 #pragma unroll
         for (int i = 0; i < 16; ++i) M[i] = (T)Md[i];
         lk = P.link[gtid] != 0;
         if (lk) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) E[i] = (T)P.En[16 * gtid + i];
+          for (int i = 0; i < 16; ++i) E[i] = (T)tp<MT>(P, P.En)[16 * gtid + i];
         }
       }
       T Lr[16];
@@ -647,12 +687,12 @@ graph_solve_kernel(SolverDev P) {
       for (int i = 0; i < 16; ++i) Ls[i * GS_THREADS + threadIdx.x] = Lr[i];
       if (is_node) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rn[i] = (T)(-P.g[4 * gtid + i]);
+        for (int i = 0; i < 4; ++i) rn[i] = (T)(-tp<MT>(P, P.g)[4 * gtid + i]);
       }
       chain_apply(Mi, Lr, lk, sl, rn, zn);
       if (gtid < P.n) {
         const T zero4[4] = {T(0), T(0), T(0), T(0)};
-        st4(Pres + 4 * gtid, rn); st4(Pz + 4 * gtid, zn); st4(Pp + 4 * gtid, zero4); st4(Pdelta + 4 * gtid, zero4);
+        st4(Pres() + 4 * gtid, rn); st4(Pz() + 4 * gtid, zn); st4(Pp() + 4 * gtid, zero4); st4(Pdelta() + 4 * gtid, zero4);
       }
       if (is_node) {
 #pragma unroll
@@ -665,23 +705,23 @@ graph_solve_kernel(SolverDev P) {
           double Md[16];
           T M[16];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) Md[i] = P.Hnn[16 * n + i];
+          for (int i = 0; i < 16; ++i) Md[i] = tp<MT>(P, P.Hnn)[16 * n + i];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) { const double ld = lam * P.D[4 * n + i]; Dl[i] = (T)ld; Md[i * 5] += ld; }
+          for (int i = 0; i < 4; ++i) { const double ld = lam * tp<MT>(P, P.D)[4 * n + i]; Dl[i] = (T)ld; Md[i * 5] += ld; }
 #pragma unroll
           for (int i = 0; i < 16; ++i) M[i] = (T)Md[i];
           inv4(M, Mi);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) PMinv[16 * n + i] = Mi[i];
+          for (int i = 0; i < 16; ++i) PMinv()[16 * n + i] = Mi[i];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) rl[i] = (T)(-P.g[4 * n + i]);
+          for (int i = 0; i < 4; ++i) rl[i] = (T)(-tp<MT>(P, P.g)[4 * n + i]);
 #pragma unroll
           for (int i = 0; i < 4; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) zl[i] += Mi[i * 4 + j] * rl[j];
         }
         const T zero4[4] = {T(0), T(0), T(0), T(0)};
-        st4(Pres + 4 * n, rl); st4(Pz + 4 * n, zl); st4(Pp + 4 * n, zero4); st4(Pdelta + 4 * n, zero4);
+        st4(Pres() + 4 * n, rl); st4(Pz() + 4 * n, zl); st4(Pp() + 4 * n, zero4); st4(Pdelta() + 4 * n, zero4);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           v2[0] += rl[i] * zl[i]; v2[1] += rl[i] * rl[i];
@@ -690,7 +730,7 @@ graph_solve_kernel(SolverDev P) {
       }
     }
     double r2[2];
-    grid_reduce_sum<2>(v2, r2, P, parity, sh, grid); parity ^= 1;
+    grid_reduce_sum<2, MT>(v2, r2, P, parity, sh, grid); parity ^= 1;
     double rz = r2[0];
     const double rr0 = r2[1];
     T beta = T(0);
@@ -704,8 +744,8 @@ graph_solve_kernel(SolverDev P) {
         T zq[GS_KF][2][4], pq[GS_KF][2][4];
 #pragma unroll
         for (int k = 0; k < GS_KF; ++k) {
-          ld4(Pz + 4 * fa[k], zq[k][0]); ld4(Pz + 4 * fb[k], zq[k][1]);
-          ld4(Pp + 4 * fa[k], pq[k][0]); ld4(Pp + 4 * fb[k], pq[k][1]);
+          ld4(Pz() + 4 * fa[k], zq[k][0]); ld4(Pz() + 4 * fb[k], zq[k][1]);
+          ld4(Pp() + 4 * fa[k], pq[k][0]); ld4(Pp() + 4 * fb[k], pq[k][1]);
         }
 #pragma unroll
         for (int k = 0; k < GS_KF; ++k) {
@@ -729,15 +769,15 @@ graph_solve_kernel(SolverDev P) {
             for (int i = 0; i < 4; ++i) { sa += J.at(i * 4 + j, li) * t[i]; sb += J.at(16 + i * 4 + j, li) * t[i]; }
             ca[j] = sa; cb[j] = sb;
           }
-          st4(Pcs + 4 * (size_t)fsa[k], ca);
-          st4(Pcs + 4 * (size_t)fsb[k], cb);
+          st4(Pcs() + 4 * (size_t)fsa[k], ca);
+          st4(Pcs() + 4 * (size_t)fsb[k], cb);
         }
       } else {
         for (int f = f0 + threadIdx.x; f < f1; f += GS_THREADS) {
           const int li = f - f0;
           const int a = P.ia[f], b = P.ib[f];
           T za[4], zb[4], qa[4], qb[4], pa[4], pb[4], t[4];
-          ld4(Pz + 4 * a, za); ld4(Pz + 4 * b, zb); ld4(Pp + 4 * a, qa); ld4(Pp + 4 * b, qb);
+          ld4(Pz() + 4 * a, za); ld4(Pz() + 4 * b, zb); ld4(Pp() + 4 * a, qa); ld4(Pp() + 4 * b, qb);
 #pragma unroll
           for (int i = 0; i < 4; ++i) { pa[i] = za[i] + beta * qa[i]; pb[i] = zb[i] + beta * qb[i]; }
 #pragma unroll
@@ -755,8 +795,8 @@ graph_solve_kernel(SolverDev P) {
             for (int i = 0; i < 4; ++i) { sa += J.at(i * 4 + j, li) * t[i]; sb += J.at(16 + i * 4 + j, li) * t[i]; }
             ca[j] = sa; cb[j] = sb;
           }
-          st4(Pcs + 4 * (size_t)P.slot_a[f], ca);
-          st4(Pcs + 4 * (size_t)P.slot_b[f], cb);
+          st4(Pcs() + 4 * (size_t)P.slot_a[f], ca);
+          st4(Pcs() + 4 * (size_t)P.slot_b[f], cb);
         }
       }
       long long c1 = clock64();
@@ -769,11 +809,11 @@ graph_solve_kernel(SolverDev P) {
         if (is_node) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) { pn[i] = zn[i] + beta * pn[i]; apn[i] = Dl[i] * pn[i]; }
-          st4(Pp + 4 * gtid, pn);
+          st4(Pp() + 4 * gtid, pn);
           for (int s0 = ns0; s0 < ns1; s0 += 16) {         // 16 (fp32) / 32 (fp64) independent 16-byte loads in flight
             T c[16][4];                                    // per batch: one L2 round trip covers every node of degree <= 16
 #pragma unroll
-            for (int k = 0; k < 16; ++k) ld4(Pcs + 4 * (size_t)min(s0 + k, ns1 - 1), c[k]);
+            for (int k = 0; k < 16; ++k) ld4(Pcs() + 4 * (size_t)min(s0 + k, ns1 - 1), c[k]);
 #pragma unroll
             for (int k = 0; k < 16; ++k)
               if (s0 + k < ns1) { apn[0] += c[k][0]; apn[1] += c[k][1]; apn[2] += c[k][2]; apn[3] += c[k][3]; }
@@ -785,25 +825,25 @@ graph_solve_kernel(SolverDev P) {
         for (int n = gtid; n < P.n; n += T_) {
           if (P.fixed[n]) continue;
           T zl[4], ql[4], pl[4], ap[4];
-          ld4(Pz + 4 * n, zl); ld4(Pp + 4 * n, ql);
+          ld4(Pz() + 4 * n, zl); ld4(Pp() + 4 * n, ql);
 #pragma unroll
-          for (int i = 0; i < 4; ++i) { pl[i] = zl[i] + beta * ql[i]; ap[i] = (T)(lam * P.D[4 * n + i]) * pl[i]; }
+          for (int i = 0; i < 4; ++i) { pl[i] = zl[i] + beta * ql[i]; ap[i] = (T)(lam * tp<MT>(P, P.D)[4 * n + i]) * pl[i]; }
           const int s0 = P.node_ptr[n], s1 = P.node_ptr[n + 1];
 #pragma unroll 4
           for (int sidx = s0; sidx < s1; ++sidx) {
             T c[4];
-            ld4(Pcs + 4 * (size_t)sidx, c);
+            ld4(Pcs() + 4 * (size_t)sidx, c);
 #pragma unroll
             for (int i = 0; i < 4; ++i) ap[i] += c[i];
           }
-          st4(Pp + 4 * n, pl); st4(PAp + 4 * n, ap);
+          st4(Pp() + 4 * n, pl); st4(PAp() + 4 * n, ap);
 #pragma unroll
           for (int i = 0; i < 4; ++i) v1b[0] += pl[i] * ap[i];
         }
       }
       long long c3 = clock_after(v1b[0]);
       double r1[1];
-      grid_reduce_sum<1>(v1b, r1, P, parity, sh, grid); parity ^= 1;
+      grid_reduce_sum<1, MT>(v1b, r1, P, parity, sh, grid); parity ^= 1;
       long long c4 = clock64();
       const double pAp = r1[0];
       if (!(pAp > 0.0)) break;
@@ -822,7 +862,7 @@ graph_solve_kernel(SolverDev P) {
           const long long q0 = clock_after(rn[0] + Lr[15]);
           chain_apply(Mi, Lr, lk, sl, rn, zn);
           const long long q1 = clock_after(zn[0] + zn[3]);
-          if ((threadIdx.x & 31) == 0) P.dbg[8 + blockIdx.x * (GS_THREADS / 32) + (threadIdx.x >> 5)] += q1 - q0;
+          if (dbg_trial && (threadIdx.x & 31) == 0) P.dbg[8 + solve_rank(P) * (GS_THREADS / 32) + (threadIdx.x >> 5)] += q1 - q0;
         } else if (is_node) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -833,7 +873,7 @@ graph_solve_kernel(SolverDev P) {
           }
         }
         if (is_node) {
-          st4(Pz + 4 * gtid, zn);
+          st4(Pz() + 4 * gtid, zn);
 #pragma unroll
           for (int i = 0; i < 4; ++i) { v22[0] += rn[i] * zn[i]; v22[1] += rn[i] * rn[i]; }
         }
@@ -841,22 +881,22 @@ graph_solve_kernel(SolverDev P) {
         for (int n = gtid; n < P.n; n += T_) {
           if (P.fixed[n]) continue;
           T dl[4], pl[4], rl[4], al[4], zl[4] = {T(0), T(0), T(0), T(0)};
-          ld4(Pdelta + 4 * n, dl); ld4(Pp + 4 * n, pl); ld4(Pres + 4 * n, rl); ld4(PAp + 4 * n, al);
+          ld4(Pdelta() + 4 * n, dl); ld4(Pp() + 4 * n, pl); ld4(Pres() + 4 * n, rl); ld4(PAp() + 4 * n, al);
 #pragma unroll
           for (int i = 0; i < 4; ++i) { dl[i] += alpha * pl[i]; rl[i] -= alpha * al[i]; }
 #pragma unroll
           for (int i = 0; i < 4; ++i)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) zl[i] += PMinv[16 * n + i * 4 + j] * rl[j];
-          st4(Pdelta + 4 * n, dl); st4(Pres + 4 * n, rl); st4(Pz + 4 * n, zl);
+            for (int j = 0; j < 4; ++j) zl[i] += PMinv()[16 * n + i * 4 + j] * rl[j];
+          st4(Pdelta() + 4 * n, dl); st4(Pres() + 4 * n, rl); st4(Pz() + 4 * n, zl);
 #pragma unroll
           for (int i = 0; i < 4; ++i) { v22[0] += rl[i] * zl[i]; v22[1] += rl[i] * rl[i]; }
         }
       }
       long long c5 = clock_after(v22[0] + v22[1]);
       double r22[2];
-      grid_reduce_sum<2>(v22, r22, P, parity, sh, grid); parity ^= 1;
-      if (gtid == 0) {
+      grid_reduce_sum<2, MT>(v22, r22, P, parity, sh, grid); parity ^= 1;
+      if (dbg_trial && gtid == 0) {
         const long long c6 = clock64();
         P.dbg[0] += c1 - c0; P.dbg[1] += c2 - c1; P.dbg[2] += c3 - c2; P.dbg[3] += c4 - c3; P.dbg[4] += c5 - c4;
         P.dbg[5] += c6 - c5; P.dbg[6] += 1;
@@ -866,38 +906,38 @@ graph_solve_kernel(SolverDev P) {
       rz = r22[0];
       if (r22[1] <= P.opt.pcg_tolerance * P.opt.pcg_tolerance * rr0) break;
     }
-    if (fast && is_node) st4(Pdelta + 4 * gtid, dn);
+    if (fast && is_node) st4(Pdelta() + 4 * gtid, dn);
     pcg_total += it;
     ++iters;
 
     // ---- trial point (fp64): x_new = x + delta; g.delta, |delta|^2, |x|^2 ----
-    double* xc = P.x[cur];
-    double* xn = P.x[cur ^ 1];
+    double* xc = tp<MT>(P, cur ? P.x[1] : P.x[0]);
+    double* xn = tp<MT>(P, cur ? P.x[0] : P.x[1]);
     double v4[3] = {0.0, 0.0, 0.0}, r4[3];
     for (int n = gtid; n < P.n; n += T_) {
       T dl[4];
-      ld4(Pdelta + 4 * n, dl);
+      ld4(Pdelta() + 4 * n, dl);
       if (fast && n == gtid && is_node) { dl[0] = dn[0]; dl[1] = dn[1]; dl[2] = dn[2]; dl[3] = dn[3]; }   // (own store)
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const double d = P.fixed[n] ? 0.0 : (double)dl[i];
         const double xv = xc[4 * n + i];
         __stcg(xn + 4 * n + i, xv + d);
-        v4[0] += P.g[4 * n + i] * d; v4[1] += d * d;
+        v4[0] += tp<MT>(P, P.g)[4 * n + i] * d; v4[1] += d * d;
         if (!P.fixed[n]) v4[2] += xv * xv;
       }
-      if (P.fixed[n]) { const T zero4[4] = {T(0), T(0), T(0), T(0)}; st4(Pdelta + 4 * n, zero4); }
+      if (P.fixed[n]) { const T zero4[4] = {T(0), T(0), T(0), T(0)}; st4(Pdelta() + 4 * n, zero4); }
     }
-    grid_reduce_sum<3>(v4, r4, P, parity, sh, grid); parity ^= 1;
+    grid_reduce_sum<3, MT>(v4, r4, P, parity, sh, grid); parity ^= 1;
     // ---- evaluate trial, model decrease, elapsed time ----
     double v5[3] = {0.0, 0.0, 0.0}, r5[3];
-    factor_trial(P, xn, J, v5[0], v5[1]);
+    factor_trial<MT>(P, xn, J, v5[0], v5[1]);
     if (gtid == 0) {
       unsigned long long t1;
       asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t1));
       v5[2] = (double)(t1 - t0) * 1e-9;
     }
-    grid_reduce_sum<3>(v5, r5, P, parity, sh, grid); parity ^= 1;
+    grid_reduce_sum<3, MT>(v5, r5, P, parity, sh, grid); parity ^= 1;
     const double new_cost = r5[0];
     const double model = -r4[0] - 0.5 * r5[1];
     const double elapsed = r5[2];
@@ -917,8 +957,8 @@ graph_solve_kernel(SolverDev P) {
       if (small_step) { termination = 2; break; }
       if (P.opt.max_time_s > 0.0 && elapsed > P.opt.max_time_s) { termination = 4; break; }
       // re-linearise at the accepted point (the trial pass kept the old Jacobians for the model term)
-      double v1c[1], w1c[1] = {factor_linearize(P, P.x[cur], J)};
-      grid_reduce_sum<1>(w1c, v1c, P, parity, sh, grid); parity ^= 1;
+      double v1c[1], w1c[1] = {factor_linearize<MT>(P, tp<MT>(P, cur ? P.x[1] : P.x[0]), J)};
+      grid_reduce_sum<1, MT>(w1c, v1c, P, parity, sh, grid); parity ^= 1;
       need_gradient = true;
     } else {
       radius /= decrease;
@@ -930,15 +970,15 @@ graph_solve_kernel(SolverDev P) {
   }
 
   // ---- write back ----
-  const double* xf = P.x[cur];
-  for (int i = gtid; i < 4 * P.n; i += T_) P.poses_out[i] = __ldcg(xf + i);
+  const double* xf = tp<MT>(P, cur ? P.x[1] : P.x[0]);
+  for (int i = gtid; i < 4 * P.n; i += T_) tp<MT>(P, P.poses_out)[i] = __ldcg(xf + i);
   if (gtid == 0) {
-    P.summary->initial_cost = initial_cost;
-    P.summary->final_cost = cost;
-    P.summary->iterations = iters;
-    P.summary->pcg_iterations = pcg_total;
-    P.summary->termination = termination;
-    P.dbg[7] = clock64() - k0;
+    tp<MT>(P, P.summary)->initial_cost = initial_cost;
+    tp<MT>(P, P.summary)->final_cost = cost;
+    tp<MT>(P, P.summary)->iterations = iters;
+    tp<MT>(P, P.summary)->pcg_iterations = pcg_total;
+    tp<MT>(P, P.summary)->termination = termination;
+    if (dbg_trial) P.dbg[7] = clock64() - k0;
   }
 }
 
@@ -952,6 +992,68 @@ __global__ void graph_linearize_kernel(int m, const double* __restrict__ poses, 
   linearize_factor(ftype[f], poses + 4 * ia[f], poses + 4 * ib[f], payload + (size_t)f * OSB_PAYLOAD_LEN, rr, A, B);
   for (int i = 0; i < 4; ++i) r[(size_t)f * 4 + i] = rr[i];
   for (int i = 0; i < 16; ++i) { Ja[(size_t)f * 16 + i] = A[i]; Jb[(size_t)f * 16 + i] = B[i]; }
+}
+
+// ---- random-restart initialisation (osb_solver_solve_multistart) ----------------------------------------------------
+// Counter-based draws: a value depends only on (seed, trial, caller's node id, component), not on the launch shape, the
+// chain plan or the other nodes.  No FMA anywhere, so numpy restates it bit for bit (oracle/multistart_ref.py).
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ double multistart_draw(uint64_t seed, int trial, int node, int comp, double r) {
+  const uint64_t key = ((uint64_t)trial << 34) | ((uint64_t)(uint32_t)node << 2) | (uint64_t)comp;
+  const double u = (double)(splitmix64(seed ^ splitmix64(key)) >> 11) * 0x1p-53;   // [0, 1)
+  return __dadd_rn(__dmul_rn(2.0 * r, u), -r);                                      // [-r, r)
+}
+
+// trial t's starting poses, internal order: random_init_pose (solver.cpp:204-216) on the masked free nodes -- x, y in
+// +-rand_xy, z in +-rand_z, yaw kept -- and the caller's pose elsewhere.  base: the caller's poses in internal order.
+__global__ void multistart_init_kernel(int n, int n_trials, const double* __restrict__ base, const uint8_t* __restrict__ fixed,
+                                       const int32_t* __restrict__ order, const uint8_t* __restrict__ mask, uint64_t seed,
+                                       double rand_xy, double rand_z, double* x0, long long tstride) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * n_trials) return;
+  const int t = (int)(idx / n), i = (int)(idx - (long long)t * n);
+  const int node = order[i];
+  double* dst = reinterpret_cast<double*>(reinterpret_cast<char*>(x0) + t * tstride) + 4 * (size_t)i;
+  const double* src = base + 4 * (size_t)i;
+  if (mask[node] && !fixed[i]) {
+    dst[0] = multistart_draw(seed, t, node, 0, rand_xy);
+    dst[1] = multistart_draw(seed, t, node, 1, rand_xy);
+    dst[2] = multistart_draw(seed, t, node, 2, rand_z);
+    dst[3] = src[3];
+  } else {
+    for (int k = 0; k < 4; ++k) dst[k] = src[k];
+  }
+}
+
+// One warp.  equv_cost of every trial (solver.cpp:1721-1725), the acceptance walk of solve_with_multiple_init
+// (:783-831: best starts at acpt_cost, strictly lower wins, so the first of equal minima is kept and a NaN never is),
+// then the chosen trial's poses to `poses`.  Results: summaries [K], equv [K], chosen.
+__global__ void multistart_select_kernel(int n_trials, int n, const char* __restrict__ trials, long long tstride,
+                                         size_t summary_off, size_t out_off, int normalise, int n_res, int window,
+                                         double acpt_cost, double* __restrict__ poses, double* __restrict__ equv,
+                                         osb_solve_summary* __restrict__ summaries, int32_t* __restrict__ chosen) {
+  const int lane = threadIdx.x;
+  int c = -1;
+  if (lane == 0) {
+    double best = acpt_cost;
+    for (int t = 0; t < n_trials; ++t) {
+      const osb_solve_summary sm = *reinterpret_cast<const osb_solve_summary*>(trials + t * tstride + summary_off);
+      const double e = normalise ? sqrt(sm.final_cost) / (double)n_res / (double)window : sm.final_cost;
+      equv[t] = e;
+      summaries[t] = sm;
+      if (e < best) { best = e; c = t; }
+    }
+    *chosen = c;
+  }
+  c = __shfl_sync(0xffffffffu, c, 0);
+  if (c < 0) return;
+  const double* src = reinterpret_cast<const double*>(trials + c * tstride + out_off);
+  for (int i = lane; i < 4 * n; i += 32) poses[i] = src[i];
 }
 
 }  // namespace osb
@@ -995,6 +1097,11 @@ struct osb_solver {
   unsigned long long g_topo_version = 1, cached_topo = 0;
   std::vector<int32_t> cached_order;
   int cached_nres = 0;
+  // osb_solver_solve_multistart: per-call arena (grown on demand, kept until destroy) and pinned staging of its results
+  char* d_ms = nullptr;
+  size_t ms_bytes = 0;
+  char* h_ms = nullptr;
+  size_t h_ms_bytes = 0;
 };
 
 extern "C" void osb_solve_default_options(osb_solve_options* o) {
@@ -1021,10 +1128,10 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
   OSB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   OSB_CUDA(cudaEventCreate(&h->ev0));
   OSB_CUDA(cudaEventCreate(&h->ev1));
-  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
-  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
-  h->cluster_ok = cudaFuncSetAttribute(graph_solve_kernel<float>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
-                  cudaFuncSetAttribute(graph_solve_kernel<double>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
+  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<double, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
+  h->cluster_ok = cudaFuncSetAttribute(graph_solve_kernel<float, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
+                  cudaFuncSetAttribute(graph_solve_kernel<double, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
   cudaGetLastError();
   OSB_CUDA(cudaMalloc(&h->d_fixed, n));
   OSB_CUDA(cudaMalloc(&h->d_huber, m));
@@ -1069,6 +1176,8 @@ extern "C" osb_status osb_solver_destroy(osb_solver* h) {
   cudaFree(h->d_link); cudaFree(h->d_es_ptr); cudaFree(h->d_es_slot); cudaFree(h->d_es); cudaFree(h->d_En);
   if (h->h_x) cudaFreeHost(h->h_x);
   if (h->h_summary) cudaFreeHost(h->h_summary);
+  cudaFree(h->d_ms);
+  if (h->h_ms) cudaFreeHost(h->h_ms);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -1159,14 +1268,13 @@ static osb_status validate_graph(int n_nodes, int n_factors, const int32_t* type
   return OSB_OK;
 }
 
-// the solve proper.  upload_static: copy type / huber / payload to the device (one-shot entry point); the resident entry
-// point has already appended them.  The caller holds h->mu.
-static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed, int n_factors,
-                             const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
-                             const uint8_t* huber, bool upload_static, const osb_solve_options* opt,
-                             osb_solve_summary* summary, unsigned long long topo_key = 0) {
-  osb_solve_options o;
-  if (opt) o = *opt; else osb_solve_default_options(&o);
+// Upload the graph of one solve and the caller's poses: the chain plan, the internal numbering and the index tables
+// (unless the resident graph's topology is unchanged), the factor arrays when upload_static (the resident entry point has
+// already appended them), and the poses in internal order into d_x0.  n_res_out: the problem's residual count.
+// The caller holds h->mu.
+static osb_status upload_graph(osb_solver* h, int n_nodes, const double* poses, const uint8_t* fixed, int n_factors,
+                               const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
+                               const uint8_t* huber, bool upload_static, unsigned long long topo_key, int& n_res_out) {
   // Internal node numbering: the paths of the chain plan are runs of consecutive ids (fixed nodes last).  Everything on
   // the device uses the internal ids; poses are permuted on the way in and out.
   const size_t n = n_nodes, m = n_factors;
@@ -1174,7 +1282,6 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
   std::vector<double> x_p(4 * n);
   // resident graph with unchanged topology: plan, numbering and every index table are already on the device
   const bool reuse = topo_key != 0 && topo_key == h->cached_topo && h->cached_order.size() == n;
-  std::vector<int32_t> order_local;
   int n_res = 0;
   if (reuse) {
     for (size_t i = 0; i < n; ++i) {
@@ -1242,30 +1349,30 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
   h->cached_nres = n_res;
   h->cached_topo = topo_key;               // 0 (one-shot solve) never matches
   }
-  const std::vector<int32_t>& order = h->cached_order;
+  n_res_out = h->cached_nres;
+  return OSB_OK;
+}
 
-  SolverDev P;
-  P.n = n_nodes; P.m = n_factors;
-  P.fixed = h->d_fixed; P.ftype = h->d_type; P.ia = h->d_ia; P.ib = h->d_ib; P.huber = h->d_huber;
-  P.payload = h->d_payload; P.node_ptr = h->d_ptr; P.slot_a = h->d_slot_a; P.slot_b = h->d_slot_b;
-  P.x[0] = h->d_x0; P.x[1] = h->d_x1; P.Jg = h->d_Jg;
-  double* nv = h->d_nodevec;
-  const size_t N4 = 4 * (size_t)h->max_nodes, N16 = 16 * (size_t)h->max_nodes;
-  P.g = nv; P.D = nv + N4; P.p = nv + 2 * N4; P.z = nv + 3 * N4; P.res = nv + 4 * N4; P.Ap = nv + 5 * N4;
-  P.delta = nv + 6 * N4; P.Hnn = nv + 7 * N4; P.Minv = nv + 7 * N4 + N16;
-  P.cs = h->d_cs; P.gs = h->d_gs; P.hs = h->d_hs; P.partial = h->d_partial; P.opt = o; P.summary = h->d_summary; P.poses_out = h->d_out; P.dbg = h->d_dbg;
-  P.use_chain = 0; P.link = h->d_link; P.es_ptr = h->d_es_ptr; P.es_slot = h->d_es_slot; P.es = h->d_es; P.En = h->d_En;
+// Launch shape of one solve.  It depends on the graph's size and the options only, never on how many solves run at once,
+// so that a trial of osb_solver_solve_multistart runs exactly the arithmetic of osb_solver_solve.
+struct SolveShape {
+  bool f32;              // fp32 inner (PCG) arithmetic
+  const void* kern;      // one solve per launch
+  const void* kern_multi;  // several clusters per launch, one trial each (same resources, same arithmetic)
+  int cluster;           // 1: one thread-block cluster per solve (hardware barrier); 0: one cooperative grid per launch
+  int ctas, fpc, chain, jsmem;
+  size_t smem;           // dynamic shared memory per CTA
+};
 
+static osb_status solve_shape(const osb_solver* h, int n_nodes, int n_factors, const osb_solve_options& o, SolveShape& s) {
   // inner precision: fp32 PCG unless the caller asks for a tighter inner solve than fp32 can deliver
-  const bool f32 = o.inner_precision == OSB_INNER_FP32 || (o.inner_precision == OSB_INNER_AUTO && o.pcg_tolerance >= 1e-4);
-  const size_t tsz = f32 ? sizeof(float) : sizeof(double);
-  const void* kern = f32 ? (const void*)graph_solve_kernel<float> : (const void*)graph_solve_kernel<double>;
-  // launch shape: ONE thread-block cluster (hardware barrier, ~0.2 us) when the factor list fits 16 CTAs with their
-  // Jacobians in shared memory; otherwise a cooperative grid (software grid barrier).
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  cfg.blockDim = dim3(GS_THREADS); cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
-  bool launched_cluster = false;
+  s.f32 = o.inner_precision == OSB_INNER_FP32 || (o.inner_precision == OSB_INNER_AUTO && o.pcg_tolerance >= 1e-4);
+  const size_t tsz = s.f32 ? sizeof(float) : sizeof(double);
+  s.kern = s.f32 ? (const void*)graph_solve_kernel<float, false> : (const void*)graph_solve_kernel<double, false>;
+  s.kern_multi = s.f32 ? (const void*)graph_solve_kernel<float, true> : (const void*)graph_solve_kernel<double, true>;
+  s.chain = 0;
+  // ONE thread-block cluster (hardware barrier, ~0.2 us) when the factor list fits 16 CTAs with their Jacobians in
+  // shared memory; otherwise a cooperative grid (software grid barrier).
   {
     const int G = std::max(1, std::min(GS_MAX_CLUSTER, cdiv(std::max(n_nodes, n_factors), GS_THREADS)));
     const int fpc = cdiv(n_factors, G);
@@ -1274,51 +1381,143 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
       // chain preconditioner: needs the fast path (one thread per node, <= GS_KF factors per thread) and room for L
       const bool chain = o.preconditioner != OSB_PRECOND_BLOCK_JACOBI && fpc <= GS_KF * GS_THREADS &&
                          n_nodes <= G * GS_THREADS && jbytes + cbytes <= (size_t)GS_SMEM_DYN_MAX;
-      P.use_chain = chain ? 1 : 0;
-      cfg.gridDim = dim3(G); cfg.dynamicSmemBytes = jbytes + (chain ? cbytes : 0);
+      cudaLaunchConfig_t cfg = {};
+      cudaLaunchAttribute attr[1];
+      cfg.blockDim = dim3(GS_THREADS); cfg.gridDim = dim3(G); cfg.stream = h->stream; cfg.attrs = attr; cfg.numAttrs = 1;
+      cfg.dynamicSmemBytes = jbytes + (chain ? cbytes : 0);
       attr[0].id = cudaLaunchAttributeClusterDimension;
       attr[0].val.clusterDim.x = G; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
       int nclusters = 0;
-      if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cfg) == cudaSuccess && nclusters >= 1) {
-        P.fpc = fpc; P.use_cluster = 1; P.j_in_smem = 1;
-        launched_cluster = true;
-      } else {
-        cudaGetLastError();
-        P.use_chain = 0;
+      if (cudaOccupancyMaxActiveClusters(&nclusters, s.kern, &cfg) == cudaSuccess && nclusters >= 1) {
+        s.cluster = 1; s.ctas = G; s.fpc = fpc; s.chain = chain ? 1 : 0; s.jsmem = 1; s.smem = cfg.dynamicSmemBytes;
+        return OSB_OK;
       }
+      cudaGetLastError();
     }
   }
-  if (!launched_cluster) {
-    P.use_chain = 0;
-    int per_sm = 0;
-    const int G0 = std::max(1, std::min(num_sms(), cdiv(std::max(n_nodes, n_factors), GS_THREADS)));
-    int fpc = cdiv(n_factors, G0);
-    const size_t jbytes = (size_t)fpc * 32 * tsz;
-    P.j_in_smem = (jbytes <= (size_t)GS_SMEM_J_MAX) ? 1 : 0;
-    const size_t smem = P.j_in_smem ? jbytes : 0;
-    OSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GS_THREADS, smem));
-    if (per_sm < 1) { set_error("osb_solver_solve", "solve kernel cannot be made resident"); return OSB_ERR_CUDA; }
-    P.fpc = fpc; P.use_cluster = 0;
-    cfg.gridDim = dim3(G0); cfg.dynamicSmemBytes = smem;
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-  }
-  h->last_grid = (int)cfg.gridDim.x; h->last_cluster = P.use_cluster; h->last_jsmem = P.j_in_smem; h->last_chain = P.use_chain;
-  h->last_f32 = f32 ? 1 : 0;
-  OSB_CUDA(cudaEventRecord(h->ev0, st));
-  {
+  int per_sm = 0;
+  const int G0 = std::max(1, std::min(num_sms(), cdiv(std::max(n_nodes, n_factors), GS_THREADS)));
+  const int fpc = cdiv(n_factors, G0);
+  const size_t jbytes = (size_t)fpc * 32 * tsz;
+  s.jsmem = (jbytes <= (size_t)GS_SMEM_J_MAX) ? 1 : 0;
+  s.smem = s.jsmem ? jbytes : 0;
+  OSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, s.kern, GS_THREADS, s.smem));
+  if (per_sm < 1) { set_error("osb_solver_solve", "solve kernel cannot be made resident"); return OSB_ERR_CUDA; }
+  s.cluster = 0; s.ctas = G0; s.fpc = fpc;
+  return OSB_OK;
+}
+
+// the graph tables on the device (shared by every trial) and the solve's options
+static SolverDev graph_dev(const osb_solver* h, int n_nodes, int n_factors, const osb_solve_options& o) {
+  SolverDev P = {};
+  P.n = n_nodes; P.m = n_factors;
+  P.fixed = h->d_fixed; P.ftype = h->d_type; P.ia = h->d_ia; P.ib = h->d_ib; P.huber = h->d_huber;
+  P.payload = h->d_payload; P.node_ptr = h->d_ptr; P.slot_a = h->d_slot_a; P.slot_b = h->d_slot_b;
+  P.link = h->d_link; P.es_ptr = h->d_es_ptr; P.es_slot = h->d_es_slot;
+  P.opt = o; P.dbg = h->d_dbg;
+  return P;
+}
+
+// state of one solve inside a block of doubles laid out by trial_layout (per-trial buffers of the multistart arena)
+struct TrialLayout {
+  size_t x0, x1, out, nodevec, En, gs, cs, hs, es, Jg, partial, summary, bytes;
+};
+static TrialLayout trial_layout(int n_nodes, int n_factors, const SolveShape& s) {
+  const size_t n = n_nodes, m = n_factors;
+  TrialLayout L;
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t p = at; at += (bytes + 15) & ~(size_t)15; return p; };
+  L.x0 = take(4 * n * 8); L.x1 = take(4 * n * 8); L.out = take(4 * n * 8);
+  L.nodevec = take((7 * 4 + 2 * 16) * n * 8); L.En = take(16 * n * 8);
+  L.gs = take(8 * m * 8); L.cs = take(8 * m * 8); L.hs = take(32 * m * 8); L.es = take(16 * m * 8);
+  L.Jg = take(s.jsmem ? 0 : 32 * m * (s.f32 ? 4 : 8));
+  L.partial = take(2 * 4 * (size_t)s.ctas * 8);
+  L.summary = take(sizeof(osb_solve_summary));
+  L.bytes = at;
+  return L;
+}
+
+static void bind_nodevec(SolverDev& P, double* nv, size_t nodes) {
+  const size_t N4 = 4 * nodes, N16 = 16 * nodes;
+  P.g = nv; P.D = nv + N4; P.p = nv + 2 * N4; P.z = nv + 3 * N4; P.res = nv + 4 * N4; P.Ap = nv + 5 * N4;
+  P.delta = nv + 6 * N4; P.Hnn = nv + 7 * N4; P.Minv = nv + 7 * N4 + N16;
+}
+
+// every per-trial state pointer of P moved `o` bytes (host side: a cooperative launch runs one trial)
+static void shift_state(SolverDev& P, long long o) {
+  auto sh = [o](auto*& p) { p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<char*>(p) + o); };
+  sh(P.x[0]); sh(P.x[1]); sh(P.Jg); sh(P.g); sh(P.D); sh(P.Hnn); sh(P.Minv); sh(P.p); sh(P.z); sh(P.res); sh(P.Ap);
+  sh(P.delta); sh(P.gs); sh(P.cs); sh(P.hs); sh(P.partial); sh(P.summary); sh(P.poses_out); sh(P.es); sh(P.En);
+}
+
+// n_trials solves of one shape; trial t's state lies t * tstride bytes past P's.  Cluster path: ONE launch of n_trials
+// clusters (clusters do not wait for each other, so the grid may exceed what is resident).  Cooperative path: one grid
+// per trial, in order on the stream.
+static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s, int n_trials, long long tstride) {
+  P.fpc = s.fpc; P.use_cluster = s.cluster; P.j_in_smem = s.jsmem; P.use_chain = s.chain;
+  P.ctas = s.ctas; P.first_trial = 0; P.tstride = tstride;
+  h->last_grid = s.ctas; h->last_cluster = s.cluster; h->last_jsmem = s.jsmem; h->last_chain = s.chain;
+  h->last_f32 = s.f32 ? 1 : 0;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  cfg.blockDim = dim3(GS_THREADS); cfg.stream = h->stream; cfg.attrs = attr; cfg.numAttrs = 1;
+  cfg.dynamicSmemBytes = s.smem;
+  if (s.cluster) {
+    cfg.gridDim = dim3(n_trials * s.ctas);
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = s.ctas; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     void* kargs[1] = {&P};
-    OSB_CUDA(cudaLaunchKernelExC(&cfg, kern, kargs));
+    OSB_CUDA(cudaLaunchKernelExC(&cfg, n_trials > 1 ? s.kern_multi : s.kern, kargs));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return OSB_OK;
   }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cfg.gridDim = dim3(s.ctas);
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  for (int t = 0; t < n_trials; ++t) {
+    SolverDev Q = P;
+    Q.first_trial = t;
+    shift_state(Q, (long long)t * tstride);
+    void* kargs[1] = {&Q};
+    OSB_CUDA(cudaLaunchKernelExC(&cfg, s.kern, kargs));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+  }
+  return OSB_OK;
+}
+
+// the solve proper (K = 1 of launch_solves, in the handle's own buffers).  upload_static: see upload_graph.
+// The caller holds h->mu.
+static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed, int n_factors,
+                             const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
+                             const uint8_t* huber, bool upload_static, const osb_solve_options* opt,
+                             osb_solve_summary* summary, unsigned long long topo_key = 0) {
+  osb_solve_options o;
+  if (opt) o = *opt; else osb_solve_default_options(&o);
+  const size_t n = n_nodes;
+  cudaStream_t st = h->stream;
+  int n_res = 0;
+  osb_status s = upload_graph(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, upload_static, topo_key, n_res);
+  if (s != OSB_OK) return s;
+  const std::vector<int32_t>& order = h->cached_order;
+  SolveShape shape;
+  s = solve_shape(h, n_nodes, n_factors, o, shape);
+  if (s != OSB_OK) return s;
+
+  SolverDev P = graph_dev(h, n_nodes, n_factors, o);
+  P.x[0] = h->d_x0; P.x[1] = h->d_x1; P.Jg = h->d_Jg;
+  bind_nodevec(P, h->d_nodevec, h->max_nodes);
+  P.cs = h->d_cs; P.gs = h->d_gs; P.hs = h->d_hs; P.partial = h->d_partial; P.summary = h->d_summary; P.poses_out = h->d_out;
+  P.es = h->d_es; P.En = h->d_En;
+  OSB_CUDA(cudaEventRecord(h->ev0, st));
+  s = launch_solves(h, P, shape, 1, 0);
+  if (s != OSB_OK) return s;
   OSB_CUDA(cudaEventRecord(h->ev1, st));
   OSB_CUDA(cudaMemcpyAsync(h->h_x, h->d_out, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaMemcpyAsync(h->h_summary, h->d_summary, sizeof(osb_solve_summary), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
-  memcpy(x_p.data(), h->h_x, 4 * n * sizeof(double));
   *summary = *h->h_summary;
   for (size_t i = 0; i < n; ++i)
-    for (int k = 0; k < 4; ++k) poses[4 * (size_t)order[i] + k] = x_p[4 * i + k];
+    for (int k = 0; k < 4; ++k) poses[4 * (size_t)order[i] + k] = h->h_x[4 * i + k];
   float ms = 0.f;
   OSB_CUDA(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   summary->solve_ms = ms;
@@ -1340,6 +1539,109 @@ extern "C" osb_status osb_solver_solve(osb_solver* h, int n_nodes, double* poses
   h->g_static_valid = false;              // the device factor arrays now hold this graph, not the resident one
   h->cached_topo = 0;                     // ... and so do the index tables
   return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, opt, summary);
+}
+
+// ---- random-restart initialisation: solve_with_multiple_init (swarm_localization_solver.cpp:781-845) ----------------
+// Trials start from the caller's poses with the masked free nodes scattered (multistart_init_kernel), run as one launch
+// of n_trials solves of the osb_solver_solve shape, and are ranked on the device (multistart_select_kernel).
+// Arena: [order n x int32 | mask n | chosen poses 4n | equv K | summaries K | chosen] then K trial blocks (trial_layout).
+extern "C" osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed,
+                                                  const uint8_t* init_mask, int n_factors, const int32_t* type,
+                                                  const int32_t* ia, const int32_t* ib, const double* payload,
+                                                  const uint8_t* huber, const osb_solve_options* opt,
+                                                  const osb_multistart_options* ms, osb_solve_summary* trial_summaries,
+                                                  double* equv_costs, int32_t* chosen) {
+  OSB_REQUIRE(h && poses && fixed && init_mask && type && ia && ib && payload && huber && ms && trial_summaries &&
+              equv_costs && chosen, "null argument");
+  OSB_REQUIRE(ms->n_trials >= 1 && ms->n_trials <= 256, "n_trials must be 1 ... 256");
+  OSB_REQUIRE(!ms->normalise || ms->window_size >= 1, "window_size must be >= 1 when normalise is set");
+  OSB_REQUIRE(std::isfinite(ms->rand_xy) && ms->rand_xy >= 0.0 && std::isfinite(ms->rand_z) && ms->rand_z >= 0.0,
+              "rand_xy and rand_z must be finite and >= 0");
+  OSB_REQUIRE(!std::isnan(ms->acpt_cost), "acpt_cost is NaN");
+  OSB_REQUIRE(n_nodes > 0 && n_nodes <= h->max_nodes && n_factors > 0 && n_factors <= h->max_factors,
+              "graph larger than the solver capacity");
+  osb_status s = validate_graph(n_nodes, n_factors, type, ia, ib);
+  if (s != OSB_OK) return s;
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  h->g_static_valid = false;              // as osb_solver_solve: the device factor arrays and tables now hold this graph
+  h->cached_topo = 0;
+  for (const void* k : {(const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>}) {
+    OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
+    if (h->cluster_ok) OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  }
+  osb_solve_options o;
+  if (opt) o = *opt; else osb_solve_default_options(&o);
+  const int K = ms->n_trials;
+  const size_t n = n_nodes;
+  cudaStream_t st = h->stream;
+  int n_res = 0;
+  s = upload_graph(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, n_res);
+  if (s != OSB_OK) return s;
+  SolveShape shape;
+  s = solve_shape(h, n_nodes, n_factors, o, shape);
+  if (s != OSB_OK) return s;
+
+  const TrialLayout L = trial_layout(n_nodes, n_factors, shape);
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t o_order = 0, o_mask = al(4 * n), o_poses = o_mask + al(n), o_equv = o_poses + 4 * n * sizeof(double);
+  const size_t o_sum = o_equv + K * sizeof(double), o_chosen = o_sum + K * sizeof(osb_solve_summary);
+  const size_t res_bytes = o_chosen + sizeof(int32_t) - o_poses;
+  const size_t o_trials = al(o_chosen + sizeof(int32_t)), need = o_trials + K * L.bytes;
+  if (h->ms_bytes < need) {               // a failed allocation leaves no arena and the handle as it was otherwise
+    cudaFree(h->d_ms); h->d_ms = nullptr; h->ms_bytes = 0;
+    OSB_CUDA(cudaMalloc(&h->d_ms, need));
+    h->ms_bytes = need;
+  }
+  if (h->h_ms_bytes < res_bytes) {
+    if (h->h_ms) cudaFreeHost(h->h_ms);
+    h->h_ms = nullptr; h->h_ms_bytes = 0;
+    OSB_CUDA(cudaHostAlloc((void**)&h->h_ms, res_bytes, cudaHostAllocDefault));
+    h->h_ms_bytes = res_bytes;
+  }
+  char* A = h->d_ms;
+  char* T0 = A + o_trials;
+  OSB_CUDA(cudaMemcpyAsync(A + o_order, h->cached_order.data(), 4 * n, cudaMemcpyHostToDevice, st));
+  OSB_CUDA(cudaMemcpyAsync(A + o_mask, init_mask, n, cudaMemcpyHostToDevice, st));
+  const long long kn = (long long)K * n_nodes;
+  OSB_LAUNCH(multistart_init_kernel, (unsigned)((kn + 255) / 256), 256, 0, st, n_nodes, K, h->d_x0, h->d_fixed,
+             reinterpret_cast<const int32_t*>(A + o_order), reinterpret_cast<const uint8_t*>(A + o_mask), ms->seed,
+             ms->rand_xy, ms->rand_z, reinterpret_cast<double*>(T0 + L.x0), (long long)L.bytes);
+  OSB_CHECK_LAUNCH();
+
+  SolverDev P = graph_dev(h, n_nodes, n_factors, o);
+  P.x[0] = reinterpret_cast<double*>(T0 + L.x0); P.x[1] = reinterpret_cast<double*>(T0 + L.x1);
+  P.Jg = T0 + L.Jg;
+  bind_nodevec(P, reinterpret_cast<double*>(T0 + L.nodevec), n);
+  P.cs = T0 + L.cs; P.gs = reinterpret_cast<double*>(T0 + L.gs); P.hs = reinterpret_cast<double*>(T0 + L.hs);
+  P.partial = reinterpret_cast<double*>(T0 + L.partial); P.summary = reinterpret_cast<osb_solve_summary*>(T0 + L.summary);
+  P.poses_out = reinterpret_cast<double*>(T0 + L.out);
+  P.es = reinterpret_cast<double*>(T0 + L.es); P.En = reinterpret_cast<double*>(T0 + L.En);
+  OSB_CUDA(cudaEventRecord(h->ev0, st));
+  s = launch_solves(h, P, shape, K, (long long)L.bytes);
+  if (s != OSB_OK) return s;
+  OSB_CUDA(cudaEventRecord(h->ev1, st));
+  OSB_LAUNCH(multistart_select_kernel, 1, 32, 0, st, K, n_nodes, T0, (long long)L.bytes, L.summary, L.out,
+             ms->normalise ? 1 : 0, n_res, ms->window_size, ms->acpt_cost, reinterpret_cast<double*>(A + o_poses),
+             reinterpret_cast<double*>(A + o_equv), reinterpret_cast<osb_solve_summary*>(A + o_sum),
+             reinterpret_cast<int32_t*>(A + o_chosen));
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(cudaMemcpyAsync(h->h_ms, A + o_poses, res_bytes, cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  float msec = 0.f;
+  OSB_CUDA(cudaEventElapsedTime(&msec, h->ev0, h->ev1));
+  auto res = [&](size_t off) { return h->h_ms + (off - o_poses); };
+  std::memcpy(equv_costs, res(o_equv), K * sizeof(double));
+  std::memcpy(trial_summaries, res(o_sum), K * sizeof(osb_solve_summary));
+  for (int t = 0; t < K; ++t) { trial_summaries[t].solve_ms = msec; trial_summaries[t].n_residuals = n_res; }
+  std::memcpy(chosen, res(o_chosen), sizeof(int32_t));
+  if (*chosen >= 0) {
+    const double* xp = reinterpret_cast<const double*>(res(o_poses));
+    const std::vector<int32_t>& order = h->cached_order;
+    for (size_t i = 0; i < n; ++i)
+      for (int k = 0; k < 4; ++k) poses[4 * (size_t)order[i] + k] = xp[4 * i + k];
+  }
+  return OSB_OK;
 }
 
 // -------------------------------------------------------------------------------------------------------------

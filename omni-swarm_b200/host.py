@@ -257,6 +257,29 @@ class PoseGraphSolver:
                                             C.byref(opt), C.byref(summ)))
         return poses, summ
 
+    def solve_multistart(self, g: dict, init_mask: np.ndarray, n_trials: int, seed: int, window_size: int,
+                         acpt_cost: float, normalise: bool = True, options: _l.SolveOptions | None = None,
+                         rand_xy: float = 5.0, rand_z: float = 1.0, init: np.ndarray | None = None):
+        """SwarmLocalizationSolver::solve_with_multiple_init (solver.cpp:781-845): n_trials solves from random
+        restarts of the masked nodes, in one launch.  Returns (poses, chosen, summaries, equv): the chosen trial's poses
+        (the starting poses when chosen == -1, i.e. no trial got below acpt_cost), the trial index, the K summaries and
+        the K equv_costs."""
+        fixed, ftype, ia, ib, payload, huber = self._arrays(g)
+        poses = np.ascontiguousarray(g["init"] if init is None else init, np.float64).copy()
+        mask = np.ascontiguousarray(init_mask, np.uint8)
+        assert mask.shape == (poses.shape[0],)
+        opt = options if options is not None else self.default_options()
+        ms = _l.MultistartOptions(n_trials=n_trials, normalise=int(normalise), window_size=window_size, seed=seed,
+                                  rand_xy=rand_xy, rand_z=rand_z, acpt_cost=acpt_cost)
+        summ = (_l.SolveSummary * max(1, n_trials))()
+        equv = np.zeros(max(1, n_trials), np.float64)
+        chosen = C.c_int32(-2)
+        _l.check(self._lib.osb_solver_solve_multistart(self._h, poses.shape[0], _l.ptr(poses), _l.ptr(fixed),
+                                                       _l.ptr(mask), len(ftype), _l.ptr(ftype), _l.ptr(ia), _l.ptr(ib),
+                                                       _l.ptr(payload), _l.ptr(huber), C.byref(opt), C.byref(ms),
+                                                       C.cast(summ, C.c_void_p), _l.ptr(equv), C.byref(chosen)))
+        return poses, int(chosen.value), list(summ), equv
+
     # ---- resident graph (SURVEY 8f-4): the factor list stays on the device between solves ----
     def graph_clear(self):
         _l.check(self._lib.osb_solver_graph_clear(self._h))

@@ -39,6 +39,11 @@ class SolveSummary(C.Structure):
                 ("termination", C.c_int32)]
 
 
+class MultistartOptions(C.Structure):
+    _fields_ = [("n_trials", C.c_int32), ("normalise", C.c_int32), ("window_size", C.c_int32), ("seed", C.c_uint64),
+                ("rand_xy", C.c_double), ("rand_z", C.c_double), ("acpt_cost", C.c_double)]
+
+
 class KeyframeRecord(C.Structure):
     _fields_ = [("drone_id", C.c_int32), ("msg_id", C.c_int32), ("n_dirs", C.c_int32), ("reserved", C.c_int32),
                 ("n_kpts", C.c_int32 * MAX_DIRS), ("n_kpts_down", C.c_int32 * MAX_DIRS),
@@ -135,6 +140,9 @@ _SIG = {
     "osb_solver_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int]),
     "osb_solver_destroy": (C.c_int, [_P]),
     "osb_solver_solve": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P, C.POINTER(SolveOptions), C.POINTER(SolveSummary)]),
+    "osb_solver_solve_multistart": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, _P, _P,
+                                              C.POINTER(SolveOptions), C.POINTER(MultistartOptions), _P, _P,
+                                              C.POINTER(C.c_int32)]),
     "osb_solver_graph_clear": (C.c_int, [_P]),
     "osb_solver_graph_add_nodes": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int32)]),
     "osb_solver_graph_add_factors": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P]),

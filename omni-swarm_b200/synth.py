@@ -343,6 +343,60 @@ def pose_graph(n_drones: int = 5, n_frames: int = 100, n_uwb: int | None = None,
     )
 
 
+def init_graph(n_drones: int = 5, n_frames: int = 100, seed: int = 0) -> dict:
+    """The graph of the swarm's initialisation solve (solve_with_multiple_init, solver.cpp:781-845): odometry chains
+    and UWB ranges only (every drone to drone 0 and to the previous drone, every frame), before any loop or detection.  Each drone flies its
+    own circle (radius, phase, height), so the ranges change over time and fix the drones' offsets; in pose_graph()
+    all drones fly the same circle and constant ranges would leave them free.  `init`: drone 0 at ground truth
+    (its first pose constant), the others at the origin with their ground-truth (odometry) yaw; `mask` marks drones
+    1 ... n_drones-1 for random initialisation."""
+    rng = np.random.default_rng(seed + 9100)
+    nd, nf = n_drones, n_frames
+    n_nodes = nd * nf
+    t = np.arange(nf) * 0.5
+    gt = np.zeros((nf, nd, 4))
+    for i in range(nd):
+        r, ph, w = 1.0 + 0.2 * i, 1.3 * i, 2 * math.pi / (30.0 + 7.0 * i)
+        gt[:, i, 0] = r * np.cos(w * t + ph) + 4.0 * (i % 3)
+        gt[:, i, 1] = r * np.sin(w * t + ph) - 4.0 * (i // 3)
+        gt[:, i, 2] = 1.0 + 0.4 * i + 0.1 * np.sin(w * t * 2 + ph)
+        gt[:, i, 3] = _wrap(w * t + ph + math.pi / 2)
+    gt = gt.reshape(n_nodes, 4)
+    types, ia, ib, huber, payload = [], [], [], [], []
+
+    def add(tp, a, b, pl, hub):
+        types.append(tp); ia.append(a); ib.append(b); huber.append(hub)
+        p = np.zeros(PAYLOAD_LEN); p[:len(pl)] = pl
+        payload.append(p)
+
+    vo_cov_pos, vo_cov_yaw = 1e-4, 1e-5
+    for f in range(nf - 1):
+        for i in range(nd):
+            a, b = f * nd + i, (f + 1) * nd + i
+            step = max(np.linalg.norm(gt[b, :3] - gt[a, :3]), 0.05)
+            cov = np.diag([vo_cov_pos * step] * 3 + [vo_cov_yaw * step])
+            meas = _delta_pose(gt[a], gt[b]) + rng.standard_normal(4) * np.sqrt(np.diag(cov))
+            meas[3] = _wrap(meas[3])
+            add(FACTOR_RELPOSE, a, b, np.concatenate([meas, np.sqrt(np.abs(np.linalg.inv(cov))).reshape(-1)]), 0)
+    uwb_cov = 0.0014
+    for f in range(nf):
+        for i in range(1, nd):
+            for j in sorted({0, i - 1}):
+                a, b = f * nd + i, f * nd + j
+                d = np.linalg.norm(gt[a, :3] - gt[b, :3]) + rng.standard_normal() * math.sqrt(uwb_cov)
+                add(FACTOR_DISTANCE, a, b, [d, 1.0 / math.sqrt(uwb_cov)], 1)
+    drone = np.arange(n_nodes) % nd
+    init = gt.copy()
+    init[drone != 0, :3] = 0.0
+    fixed = np.zeros(n_nodes, np.uint8)
+    fixed[0] = 1
+    return dict(
+        n_nodes=n_nodes, gt=gt, init=init, fixed=fixed, mask=(drone != 0).astype(np.uint8),
+        ftype=np.array(types, np.int32), ia=np.array(ia, np.int32), ib=np.array(ib, np.int32),
+        huber=np.array(huber, np.uint8), payload=np.ascontiguousarray(np.array(payload, np.float64)),
+    )
+
+
 def pose_graph_c5(seed: int = 0) -> dict:
     """BASELINE.json C5 graph: 5 drones x 400 frames = 2000 nodes, 12 000 factors
     = 1995 ego + 4000 UWB + 4000 loop + 2005 detection-as-relative-pose."""
