@@ -241,10 +241,11 @@ osb_status osb_solver_solve(osb_solver* h, int n_nodes, double* poses, const uin
  * trial_summaries[t] is filled for every trial; their solve_ms is the device time of the whole batch.
  * Unlike the reference, every trial starts from the caller's poses (its trial i starts from trial i-1's solution for the
  * nodes it does not scatter), and the draws are hashed instead of rand().
- * Memory: a per-handle arena, grown to the largest call and kept until osb_solver_destroy, of about
- *   704 n + 512 m + 64 G + 48 bytes per trial (n nodes, m factors, G CTAs per solve: <= 16 on the cluster path, <= the
- *   SM count otherwise), plus 128 m (fp32 inner) / 256 m (fp64) when the Jacobians do not fit shared memory, plus
- *   40 n + 48 n_trials + 1 KB.  A failed allocation returns OSB_ERR_CUDA and leaves the handle usable. */
+ * Memory: the solves of a handle share one arena, which osb_solver_create sizes for one solve at the handle's capacity.
+ *   This call grows it to n_trials blocks of at most 704 n + 512 m + 64 G + 5 KB bytes (n nodes, m factors, G CTAs per
+ *   solve: <= 16 on the cluster path, <= the SM count otherwise), plus 128 m (fp32 inner) / 256 m (fp64) when the
+ *   Jacobians do not fit shared memory, and keeps it until osb_solver_destroy.  A failed allocation returns
+ *   OSB_ERR_CUDA and leaves the handle as it was. */
 typedef struct {
   int32_t n_trials;      /* INIT_TRIAL = 3 (solver.cpp:54); 1 ... 256 */
   int32_t normalise;     /* 1: equv_cost = sqrt(final_cost)/n_residuals/window_size (the reference's num_res_blks > 1) */

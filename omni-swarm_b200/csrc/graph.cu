@@ -214,8 +214,9 @@ struct SolverDev {
   double* es;              // [<= m][16] J_i^T J_{i-1} of the chain factors (written at every linearisation)
   double* En;              // [n][16] summed coupling block of node i with node i-1
   // batched trials (osb_solver_solve_multistart): CTA b solves trial first_trial + b / ctas as CTA b % ctas of that
-  // solve.  Every state pointer above (x .. En) is trial 0's; trial t's lies t * tstride bytes further.  The graph
-  // tables (fixed .. slot_b, link, es_ptr, es_slot) are shared, and only trial 0 writes dbg.
+  // solve.  The state pointers above (x .. En) point into trial 0's block of the handle's arena (trial_layout); trial t's
+  // block lies t * tstride bytes further.  The graph tables (fixed .. slot_b, link, es_ptr, es_slot) are shared, and
+  // only trial 0 writes dbg.
   int ctas;                // CTAs per solve (the cluster size on the cluster path)
   int first_trial;
   long long tstride;
@@ -224,7 +225,7 @@ struct SolverDev {
 // trial t's copy of a per-trial state pointer lies t * tstride bytes past trial 0's.  It is recomputed at every use from
 // the cluster id (a special register) rather than shifted once at the start: twenty shifted pointers held for the whole
 // solve would not fit beside the solver's working set, which already fills the 255 registers.  A cooperative launch
-// runs one trial, whose pointers the host has already shifted.
+// runs one trial, which the host binds at its own block of the arena.
 // MULTI = false (one solve per launch) compiles this away: reading the cluster id at every use costs the latency-bound
 // CG loop about 10 % (measured on C5), so a single solve runs the graph_solve_kernel<T, false> instantiation.
 template <bool MULTI, typename Q>
@@ -533,6 +534,27 @@ __device__ void factor_trial(const SolverDev& P, const double* __restrict__ xn, 
   jd += (double)jdt;
 }
 
+// factor phase of a PCG iteration for one factor: t = Ja p_a + Jb p_b and its two contributions ca = Ja^T t, cb = Jb^T t
+template <typename T>
+__device__ __forceinline__ void factor_apply(const JStore<T>& J, int li, const T (&pa)[4], const T (&pb)[4], T (&ca)[4],
+                                             T (&cb)[4]) {
+  T t[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    T acc = T(0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc += J.at(i * 4 + j, li) * pa[j] + J.at(16 + i * 4 + j, li) * pb[j];
+    t[i] = acc;
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T sa = T(0), sb = T(0);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { sa += J.at(i * 4 + j, li) * t[i]; sb += J.at(16 + i * 4 + j, li) * t[i]; }
+    ca[j] = sa; cb[j] = sb;
+  }
+}
+
 template <typename T, bool MT>
 __global__ void __launch_bounds__(GS_THREADS, 1)
 graph_solve_kernel(SolverDev P) {
@@ -750,51 +772,21 @@ graph_solve_kernel(SolverDev P) {
 #pragma unroll
         for (int k = 0; k < GS_KF; ++k) {
           if (!fvalid[k]) continue;
-          const int li = threadIdx.x + k * GS_THREADS;
-          T pa[4], pb[4], t[4];
+          T pa[4], pb[4], ca[4], cb[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i) { pa[i] = zq[k][0][i] + beta * pq[k][0][i]; pb[i] = zq[k][1][i] + beta * pq[k][1][i]; }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            T acc = T(0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc += J.at(i * 4 + j, li) * pa[j] + J.at(16 + i * 4 + j, li) * pb[j];
-            t[i] = acc;
-          }
-          T ca[4], cb[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            T sa = T(0), sb = T(0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { sa += J.at(i * 4 + j, li) * t[i]; sb += J.at(16 + i * 4 + j, li) * t[i]; }
-            ca[j] = sa; cb[j] = sb;
-          }
+          factor_apply(J, threadIdx.x + k * GS_THREADS, pa, pb, ca, cb);
           st4(Pcs() + 4 * (size_t)fsa[k], ca);
           st4(Pcs() + 4 * (size_t)fsb[k], cb);
         }
       } else {
         for (int f = f0 + threadIdx.x; f < f1; f += GS_THREADS) {
-          const int li = f - f0;
           const int a = P.ia[f], b = P.ib[f];
-          T za[4], zb[4], qa[4], qb[4], pa[4], pb[4], t[4];
+          T za[4], zb[4], qa[4], qb[4], pa[4], pb[4], ca[4], cb[4];
           ld4(Pz() + 4 * a, za); ld4(Pz() + 4 * b, zb); ld4(Pp() + 4 * a, qa); ld4(Pp() + 4 * b, qb);
 #pragma unroll
           for (int i = 0; i < 4; ++i) { pa[i] = za[i] + beta * qa[i]; pb[i] = zb[i] + beta * qb[i]; }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            T acc = T(0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc += J.at(i * 4 + j, li) * pa[j] + J.at(16 + i * 4 + j, li) * pb[j];
-            t[i] = acc;
-          }
-          T ca[4], cb[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            T sa = T(0), sb = T(0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { sa += J.at(i * 4 + j, li) * t[i]; sb += J.at(16 + i * 4 + j, li) * t[i]; }
-            ca[j] = sa; cb[j] = sb;
-          }
+          factor_apply(J, f - f0, pa, pb, ca, cb);
           st4(Pcs() + 4 * (size_t)P.slot_a[f], ca);
           st4(Pcs() + 4 * (size_t)P.slot_b[f], cb);
         }
@@ -1010,8 +1002,10 @@ __device__ __forceinline__ double multistart_draw(uint64_t seed, int trial, int 
 }
 
 // trial t's starting poses, internal order: random_init_pose (solver.cpp:204-216) on the masked free nodes -- x, y in
-// +-rand_xy, z in +-rand_z, yaw kept -- and the caller's pose elsewhere.  base: the caller's poses in internal order.
-__global__ void multistart_init_kernel(int n, int n_trials, const double* __restrict__ base, const uint8_t* __restrict__ fixed,
+// +-rand_xy, z in +-rand_z, yaw kept -- and the caller's pose elsewhere.  The caller's poses are trial 0's x0, which
+// this kernel rewrites in place.  That is race-free: in trial 0 it writes only x, y, z of the masked free nodes, and
+// the other trials read only the yaw of those nodes and the whole pose of the rest.
+__global__ void multistart_init_kernel(int n, int n_trials, const uint8_t* __restrict__ fixed,
                                        const int32_t* __restrict__ order, const uint8_t* __restrict__ mask, uint64_t seed,
                                        double rand_xy, double rand_z, double* x0, long long tstride) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1019,46 +1013,88 @@ __global__ void multistart_init_kernel(int n, int n_trials, const double* __rest
   const int t = (int)(idx / n), i = (int)(idx - (long long)t * n);
   const int node = order[i];
   double* dst = reinterpret_cast<double*>(reinterpret_cast<char*>(x0) + t * tstride) + 4 * (size_t)i;
-  const double* src = base + 4 * (size_t)i;
+  const double* src = x0 + 4 * (size_t)i;
   if (mask[node] && !fixed[i]) {
     dst[0] = multistart_draw(seed, t, node, 0, rand_xy);
     dst[1] = multistart_draw(seed, t, node, 1, rand_xy);
     dst[2] = multistart_draw(seed, t, node, 2, rand_z);
-    dst[3] = src[3];
-  } else {
+    if (t > 0) dst[3] = src[3];
+  } else if (t > 0) {
     for (int k = 0; k < 4; ++k) dst[k] = src[k];
   }
 }
 
+// What a call brings back to the host, followed by the poses [n][4] in internal order.  The selection kernel fills one
+// on the device and one copy moves it into the handle's pinned mirror; a single solve stages its poses (in and out) and
+// its summary in that mirror.
+constexpr int MS_MAX_TRIALS = 256;
+struct SolveResults {
+  int32_t chosen;
+  double equv[MS_MAX_TRIALS];
+  osb_solve_summary summaries[MS_MAX_TRIALS];
+  __host__ __device__ double* poses() { return reinterpret_cast<double*>(this + 1); }
+};
+
 // One warp.  equv_cost of every trial (solver.cpp:1721-1725), the acceptance walk of solve_with_multiple_init
 // (:783-831: best starts at acpt_cost, strictly lower wins, so the first of equal minima is kept and a NaN never is),
-// then the chosen trial's poses to `poses`.  Results: summaries [K], equv [K], chosen.
-__global__ void multistart_select_kernel(int n_trials, int n, const char* __restrict__ trials, long long tstride,
-                                         size_t summary_off, size_t out_off, int normalise, int n_res, int window,
-                                         double acpt_cost, double* __restrict__ poses, double* __restrict__ equv,
-                                         osb_solve_summary* __restrict__ summaries, int32_t* __restrict__ chosen) {
+// then the chosen trial's poses.  summary0 / out0: trial 0's summary and output poses, trial t's lie t * tstride further.
+__global__ void multistart_select_kernel(int n_trials, int n, const osb_solve_summary* __restrict__ summary0,
+                                         const double* __restrict__ out0, long long tstride, int normalise, int n_res,
+                                         int window, double acpt_cost, SolveResults* __restrict__ res) {
   const int lane = threadIdx.x;
   int c = -1;
   if (lane == 0) {
     double best = acpt_cost;
     for (int t = 0; t < n_trials; ++t) {
-      const osb_solve_summary sm = *reinterpret_cast<const osb_solve_summary*>(trials + t * tstride + summary_off);
+      const osb_solve_summary sm =
+          *reinterpret_cast<const osb_solve_summary*>(reinterpret_cast<const char*>(summary0) + t * tstride);
       const double e = normalise ? sqrt(sm.final_cost) / (double)n_res / (double)window : sm.final_cost;
-      equv[t] = e;
-      summaries[t] = sm;
+      res->equv[t] = e;
+      res->summaries[t] = sm;
       if (e < best) { best = e; c = t; }
     }
-    *chosen = c;
+    res->chosen = c;
   }
   c = __shfl_sync(0xffffffffu, c, 0);
   if (c < 0) return;
-  const double* src = reinterpret_cast<const double*>(trials + c * tstride + out_off);
-  for (int i = lane; i < 4 * n; i += 32) poses[i] = src[i];
+  const double* src = reinterpret_cast<const double*>(reinterpret_cast<const char*>(out0) + c * tstride);
+  for (int i = lane; i < 4 * n; i += 32) res->poses()[i] = src[i];
 }
 
 }  // namespace osb
 
 using namespace osb;
+
+// Launch shape of one solve.  It depends on the graph's size and the options only, never on how many solves run at once,
+// so that a trial of osb_solver_solve_multistart runs exactly the arithmetic of osb_solver_solve.
+struct SolveShape {
+  bool f32;              // fp32 inner (PCG) arithmetic
+  const void* kern;      // one solve per launch
+  const void* kern_multi;  // several clusters per launch, one trial each (same resources, same arithmetic)
+  int cluster;           // 1: one thread-block cluster per solve (hardware barrier); 0: one cooperative grid per launch
+  int ctas, fpc, chain, jsmem;
+  size_t smem;           // dynamic shared memory per CTA
+};
+
+// The state of one solve (SolverDev::x .. En) laid out from `base`: points P's state pointers into that block and returns
+// its bytes (base == nullptr: only the size).  Every buffer starts on a 256-byte boundary, as its own cudaMalloc would.
+static size_t trial_layout(SolverDev& P, char* base, size_t n, size_t m, const SolveShape& s) {
+  const size_t d = sizeof(double), tsz = s.f32 ? sizeof(float) : sizeof(double);
+  size_t at = 0;
+  auto take = [&](auto*& p, size_t bytes) {
+    p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + at);
+    at += (bytes + 255) & ~(size_t)255;
+  };
+  take(P.x[0], 4 * n * d); take(P.x[1], 4 * n * d); take(P.poses_out, 4 * n * d);
+  take(P.g, 4 * n * d); take(P.D, 4 * n * d); take(P.Hnn, 16 * n * d); take(P.En, 16 * n * d);
+  take(P.Minv, 16 * n * tsz); take(P.p, 4 * n * tsz); take(P.z, 4 * n * tsz); take(P.res, 4 * n * tsz);
+  take(P.Ap, 4 * n * tsz); take(P.delta, 4 * n * tsz);
+  take(P.gs, 8 * m * d); take(P.hs, 32 * m * d); take(P.es, 16 * m * d); take(P.cs, 8 * m * tsz);
+  take(P.Jg, s.jsmem ? 0 : 32 * m * tsz);
+  take(P.partial, 2 * 4 * (size_t)s.ctas * d);
+  take(P.summary, sizeof(osb_solve_summary));
+  return at;
+}
 
 struct osb_solver {
   int max_nodes = 0, max_factors = 0;
@@ -1066,25 +1102,29 @@ struct osb_solver {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::mutex mu;
-  // device
+  // device: the graph tables
   uint8_t *d_fixed = nullptr, *d_huber = nullptr;
   int32_t *d_type = nullptr, *d_ia = nullptr, *d_ib = nullptr, *d_ptr = nullptr, *d_slot_a = nullptr, *d_slot_b = nullptr;
-  double *d_payload = nullptr, *d_x0 = nullptr, *d_x1 = nullptr, *d_Jg = nullptr, *d_lin = nullptr;
-  double *d_nodevec = nullptr;   // g, D, p, z, res, Ap, delta (7 x 4n) + Hnn, Minv (2 x 16n)
-  double *d_cs = nullptr, *d_gs = nullptr, *d_hs = nullptr, *d_partial = nullptr, *d_out = nullptr;
-  osb_solve_summary* d_summary = nullptr;
-  long long* d_dbg = nullptr;
+  double* d_payload = nullptr;
   uint8_t* d_link = nullptr;
+  int32_t *d_es_ptr = nullptr, *d_es_slot = nullptr;
+  // the state of the solves: trial blocks of trial_layout, one after another.  osb_solver_create sizes it for one trial
+  // at the handle's capacity, so a single solve never allocates; osb_solver_solve_multistart grows it to K blocks.
+  char* d_arena = nullptr;
+  size_t arena_bytes = 0;
+  // osb_solver_solve_multistart's inputs (internal -> caller's node id, init mask) and results
+  int32_t* d_order = nullptr;
+  uint8_t* d_mask = nullptr;
+  SolveResults* d_res = nullptr;
+  double* d_lin = nullptr;        // osb_solver_linearize: poses [n][4], r [m][4], Ja, Jb [m][16]
+  long long* d_dbg = nullptr;
   // pinned staging for what crosses PCIe on EVERY solve (poses in, poses + summary out): a copy to / from pageable memory
   // blocks inside the driver until the stream reaches it -- for the results that is the whole solve, and other host threads
   // (the keyframe front-end of the same process) could not launch meanwhile (measured: 640 -> 57 keyframes/s beside a
   // back-to-back solver thread).  Pinned copies are asynchronous; the one wait is a cudaStreamSynchronize.
-  double* h_x = nullptr;
-  osb_solve_summary* h_summary = nullptr;
+  SolveResults* h_res = nullptr;
   int device = 0;
-  int32_t *d_es_ptr = nullptr, *d_es_slot = nullptr;
-  double *d_es = nullptr, *d_En = nullptr;
-  int last_grid = 0, last_cluster = 0, last_jsmem = 0, last_chain = 0, last_f32 = 0;
+  SolveShape last_shape = {};
   // resident graph (osb_solver_graph_*): host mirrors of what is already in device memory
   std::vector<double> g_poses, g_payload;
   std::vector<uint8_t> g_fixed, g_huber;
@@ -1097,11 +1137,6 @@ struct osb_solver {
   unsigned long long g_topo_version = 1, cached_topo = 0;
   std::vector<int32_t> cached_order;
   int cached_nres = 0;
-  // osb_solver_solve_multistart: per-call arena (grown on demand, kept until destroy) and pinned staging of its results
-  char* d_ms = nullptr;
-  size_t ms_bytes = 0;
-  char* h_ms = nullptr;
-  size_t h_ms_bytes = 0;
 };
 
 extern "C" void osb_solve_default_options(osb_solve_options* o) {
@@ -1128,10 +1163,12 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
   OSB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   OSB_CUDA(cudaEventCreate(&h->ev0));
   OSB_CUDA(cudaEventCreate(&h->ev1));
-  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
-  OSB_CUDA(cudaFuncSetAttribute(graph_solve_kernel<double, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
-  h->cluster_ok = cudaFuncSetAttribute(graph_solve_kernel<float, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
-                  cudaFuncSetAttribute(graph_solve_kernel<double, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+  h->cluster_ok = true;
+  for (const void* k : {(const void*)graph_solve_kernel<float, false>, (const void*)graph_solve_kernel<double, false>,
+                        (const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>}) {
+    OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
+    h->cluster_ok = h->cluster_ok && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+  }
   cudaGetLastError();
   OSB_CUDA(cudaMalloc(&h->d_fixed, n));
   OSB_CUDA(cudaMalloc(&h->d_huber, m));
@@ -1142,26 +1179,22 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
   OSB_CUDA(cudaMalloc(&h->d_slot_b, m * sizeof(int32_t)));
   OSB_CUDA(cudaMalloc(&h->d_ptr, (n + 1) * sizeof(int32_t)));
   OSB_CUDA(cudaMalloc(&h->d_payload, m * OSB_PAYLOAD_LEN * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_x0, 4 * n * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_x1, 4 * n * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_Jg, 32 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_lin, 36 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_nodevec, (7 * 4 + 2 * 16) * n * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_cs, 8 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_gs, 8 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_hs, 32 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_partial, 2 * 4 * (size_t)num_sms() * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_out, 4 * n * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_summary, sizeof(osb_solve_summary)));
-  OSB_CUDA(cudaMalloc(&h->d_dbg, (8 + 128) * sizeof(long long)));
-  OSB_CUDA(cudaMemset(h->d_dbg, 0, (8 + 128) * sizeof(long long)));
   OSB_CUDA(cudaMalloc(&h->d_link, n));
   OSB_CUDA(cudaMalloc(&h->d_es_ptr, (n + 1) * sizeof(int32_t)));
   OSB_CUDA(cudaMalloc(&h->d_es_slot, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_es, 16 * m * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_En, 16 * n * sizeof(double)));
-  OSB_CUDA(cudaHostAlloc((void**)&h->h_x, 4 * n * sizeof(double), cudaHostAllocDefault));
-  OSB_CUDA(cudaHostAlloc((void**)&h->h_summary, sizeof(osb_solve_summary), cudaHostAllocDefault));
+  // one trial of the worst shape: fp64 Jacobians in global memory, partials for a cooperative grid of every SM
+  SolveShape worst = {};
+  worst.ctas = num_sms();
+  SolverDev unbound = {};
+  h->arena_bytes = trial_layout(unbound, nullptr, n, m, worst);
+  OSB_CUDA(cudaMalloc(&h->d_arena, h->arena_bytes));
+  OSB_CUDA(cudaMalloc(&h->d_order, n * sizeof(int32_t)));
+  OSB_CUDA(cudaMalloc(&h->d_mask, n));
+  OSB_CUDA(cudaMalloc(&h->d_res, sizeof(SolveResults) + 4 * n * sizeof(double)));
+  OSB_CUDA(cudaHostAlloc((void**)&h->h_res, sizeof(SolveResults) + 4 * n * sizeof(double), cudaHostAllocDefault));
+  OSB_CUDA(cudaMalloc(&h->d_lin, (4 * n + 36 * m) * sizeof(double)));
+  OSB_CUDA(cudaMalloc(&h->d_dbg, (8 + 128) * sizeof(long long)));
+  OSB_CUDA(cudaMemset(h->d_dbg, 0, (8 + 128) * sizeof(long long)));
   h->device = current_device();
   *out = h;
   return OSB_OK;
@@ -1170,14 +1203,10 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
 extern "C" osb_status osb_solver_destroy(osb_solver* h) {
   if (!h) return OSB_OK;
   cudaFree(h->d_fixed); cudaFree(h->d_huber); cudaFree(h->d_type); cudaFree(h->d_ia); cudaFree(h->d_ib);
-  cudaFree(h->d_slot_a); cudaFree(h->d_slot_b); cudaFree(h->d_ptr); cudaFree(h->d_payload); cudaFree(h->d_x0);
-  cudaFree(h->d_x1); cudaFree(h->d_Jg); cudaFree(h->d_lin); cudaFree(h->d_nodevec); cudaFree(h->d_cs); cudaFree(h->d_gs); cudaFree(h->d_hs);
-  cudaFree(h->d_partial); cudaFree(h->d_out); cudaFree(h->d_summary); cudaFree(h->d_dbg);
-  cudaFree(h->d_link); cudaFree(h->d_es_ptr); cudaFree(h->d_es_slot); cudaFree(h->d_es); cudaFree(h->d_En);
-  if (h->h_x) cudaFreeHost(h->h_x);
-  if (h->h_summary) cudaFreeHost(h->h_summary);
-  cudaFree(h->d_ms);
-  if (h->h_ms) cudaFreeHost(h->h_ms);
+  cudaFree(h->d_slot_a); cudaFree(h->d_slot_b); cudaFree(h->d_ptr); cudaFree(h->d_payload);
+  cudaFree(h->d_link); cudaFree(h->d_es_ptr); cudaFree(h->d_es_slot);
+  cudaFree(h->d_arena); cudaFree(h->d_order); cudaFree(h->d_mask); cudaFree(h->d_res); cudaFree(h->d_lin); cudaFree(h->d_dbg);
+  if (h->h_res) cudaFreeHost(h->h_res);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -1270,99 +1299,76 @@ static osb_status validate_graph(int n_nodes, int n_factors, const int32_t* type
 
 // Upload the graph of one solve and the caller's poses: the chain plan, the internal numbering and the index tables
 // (unless the resident graph's topology is unchanged), the factor arrays when upload_static (the resident entry point has
-// already appended them), and the poses in internal order into d_x0.  n_res_out: the problem's residual count.
-// The caller holds h->mu.
+// already appended them), then the poses in internal order into x0 through the pinned staging.  The caller holds h->mu.
 static osb_status upload_graph(osb_solver* h, int n_nodes, const double* poses, const uint8_t* fixed, int n_factors,
                                const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
-                               const uint8_t* huber, bool upload_static, unsigned long long topo_key, int& n_res_out) {
+                               const uint8_t* huber, bool upload_static, unsigned long long topo_key, double* x0) {
   // Internal node numbering: the paths of the chain plan are runs of consecutive ids (fixed nodes last).  Everything on
   // the device uses the internal ids; poses are permuted on the way in and out.
   const size_t n = n_nodes, m = n_factors;
   cudaStream_t st = h->stream;
-  std::vector<double> x_p(4 * n);
   // resident graph with unchanged topology: plan, numbering and every index table are already on the device
   const bool reuse = topo_key != 0 && topo_key == h->cached_topo && h->cached_order.size() == n;
-  int n_res = 0;
-  if (reuse) {
-    for (size_t i = 0; i < n; ++i) {
-      const int o2 = h->cached_order[i];
-      for (int k = 0; k < 4; ++k) x_p[4 * i + k] = poses[4 * (size_t)o2 + k];
-    }
-    n_res = h->cached_nres;
-    memcpy(h->h_x, x_p.data(), 4 * n * sizeof(double));
-    OSB_CUDA(cudaMemcpyAsync(h->d_x0, h->h_x, 4 * n * sizeof(double), cudaMemcpyHostToDevice, st));
-  } else {
-  ChainPlan plan;
-  build_chain_plan(n_nodes, fixed, n_factors, type, ia, ib, payload, plan);
-  std::vector<int32_t> ia_p(m), ib_p(m);
-  std::vector<uint8_t> fixed_p(n);
-  for (size_t f = 0; f < m; ++f) { ia_p[f] = plan.inv[ia[f]]; ib_p[f] = plan.inv[ib[f]]; }
-  for (size_t i = 0; i < n; ++i) {
-    const int o = plan.order[i];
-    fixed_p[i] = fixed[o];
-    for (int k = 0; k < 4; ++k) x_p[4 * i + k] = poses[4 * (size_t)o + k];
-  }
-  // chain couplings: factor f couples node hi with hi-1 when its two nodes are consecutive and linked
-  std::vector<int32_t> es_ptr(n + 1, 0), es_slot(m, -1);
-  for (size_t f = 0; f < m; ++f) {
-    const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
-    if (std::abs(a - b) == 1 && plan.link[hi]) es_ptr[hi + 1]++;
-  }
-  for (size_t i = 0; i < n; ++i) es_ptr[i + 1] += es_ptr[i];
-  {
-    std::vector<int32_t> fill(es_ptr.begin(), es_ptr.end() - 1);
+  if (!reuse) {
+    ChainPlan plan;
+    build_chain_plan(n_nodes, fixed, n_factors, type, ia, ib, payload, plan);
+    std::vector<int32_t> ia_p(m), ib_p(m);
+    std::vector<uint8_t> fixed_p(n);
+    for (size_t f = 0; f < m; ++f) { ia_p[f] = plan.inv[ia[f]]; ib_p[f] = plan.inv[ib[f]]; }
+    for (size_t i = 0; i < n; ++i) fixed_p[i] = fixed[plan.order[i]];
+    // chain couplings: factor f couples node hi with hi-1 when its two nodes are consecutive and linked
+    std::vector<int32_t> es_ptr(n + 1, 0), es_slot(m, -1);
     for (size_t f = 0; f < m; ++f) {
       const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
-      if (std::abs(a - b) == 1 && plan.link[hi]) es_slot[f] = 2 * (fill[hi]++) + (a == hi ? 1 : 0);
+      if (std::abs(a - b) == 1 && plan.link[hi]) es_ptr[hi + 1]++;
     }
+    for (size_t i = 0; i < n; ++i) es_ptr[i + 1] += es_ptr[i];
+    {
+      std::vector<int32_t> fill(es_ptr.begin(), es_ptr.end() - 1);
+      for (size_t f = 0; f < m; ++f) {
+        const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
+        if (std::abs(a - b) == 1 && plan.link[hi]) es_slot[f] = 2 * (fill[hi]++) + (a == hi ? 1 : 0);
+      }
+    }
+    // CSR of contribution slots: node n owns slots [ptr[n], ptr[n+1]); factors in index order within a node, so the
+    // gather order -- and therefore every floating-point sum -- is fixed.
+    std::vector<int32_t> ptr(n + 1, 0), slot_a(m), slot_b(m);
+    for (size_t f = 0; f < m; ++f) { ptr[ia_p[f] + 1]++; ptr[ib_p[f] + 1]++; }
+    for (size_t i = 0; i < n; ++i) ptr[i + 1] += ptr[i];
+    {
+      std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
+      for (size_t f = 0; f < m; ++f) { slot_a[f] = fill[ia_p[f]]++; slot_b[f] = fill[ib_p[f]]++; }
+    }
+    int n_res = 0;
+    for (size_t f = 0; f < m; ++f)
+      n_res += type[f] == OSB_FACTOR_DISTANCE ? 1 : type[f] == OSB_FACTOR_RELPOSE ? 4
+               : (((int)payload[f * OSB_PAYLOAD_LEN + 10] & 1) ? 3 : 2);
+    OSB_CUDA(cudaMemcpyAsync(h->d_fixed, fixed_p.data(), n, cudaMemcpyHostToDevice, st));
+    if (upload_static) {
+      OSB_CUDA(cudaMemcpyAsync(h->d_huber, huber, m, cudaMemcpyHostToDevice, st));
+      OSB_CUDA(cudaMemcpyAsync(h->d_type, type, m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+      OSB_CUDA(cudaMemcpyAsync(h->d_payload, payload, m * OSB_PAYLOAD_LEN * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    OSB_CUDA(cudaMemcpyAsync(h->d_ia, ia_p.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_ib, ib_p.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_ptr, ptr.data(), (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_slot_a, slot_a.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_slot_b, slot_b.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_link, plan.link.data(), n, cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_es_ptr, es_ptr.data(), (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_es_slot, es_slot.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    // the staging vectors above die at the end of this block: the copies must have left them
+    OSB_CUDA(cudaStreamSynchronize(st));
+    h->cached_order = plan.order;
+    h->cached_nres = n_res;
+    h->cached_topo = topo_key;               // 0 (one-shot solve) never matches
   }
-  // CSR of contribution slots: node n owns slots [ptr[n], ptr[n+1]); factors in index order within a node, so the
-  // gather order -- and therefore every floating-point sum -- is fixed.
-  std::vector<int32_t> ptr(n + 1, 0), slot_a(m), slot_b(m);
-  for (size_t f = 0; f < m; ++f) { ptr[ia_p[f] + 1]++; ptr[ib_p[f] + 1]++; }
-  for (size_t i = 0; i < n; ++i) ptr[i + 1] += ptr[i];
-  {
-    std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
-    for (size_t f = 0; f < m; ++f) { slot_a[f] = fill[ia_p[f]]++; slot_b[f] = fill[ib_p[f]]++; }
-  }
-  for (size_t f = 0; f < m; ++f)
-    n_res += type[f] == OSB_FACTOR_DISTANCE ? 1 : type[f] == OSB_FACTOR_RELPOSE ? 4
-             : (((int)payload[f * OSB_PAYLOAD_LEN + 10] & 1) ? 3 : 2);
-  OSB_CUDA(cudaMemcpyAsync(h->d_fixed, fixed_p.data(), n, cudaMemcpyHostToDevice, st));
-  if (upload_static) {
-    OSB_CUDA(cudaMemcpyAsync(h->d_huber, huber, m, cudaMemcpyHostToDevice, st));
-    OSB_CUDA(cudaMemcpyAsync(h->d_type, type, m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    OSB_CUDA(cudaMemcpyAsync(h->d_payload, payload, m * OSB_PAYLOAD_LEN * sizeof(double), cudaMemcpyHostToDevice, st));
-  }
-  OSB_CUDA(cudaMemcpyAsync(h->d_ia, ia_p.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_ib, ib_p.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_ptr, ptr.data(), (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_slot_a, slot_a.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_slot_b, slot_b.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_x0, x_p.data(), 4 * n * sizeof(double), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_link, plan.link.data(), n, cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_es_ptr, es_ptr.data(), (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_es_slot, es_slot.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  // the staging vectors above die at the end of this block: the copies must have left them
-  OSB_CUDA(cudaStreamSynchronize(st));
-  h->cached_order = plan.order;
-  h->cached_nres = n_res;
-  h->cached_topo = topo_key;               // 0 (one-shot solve) never matches
-  }
-  n_res_out = h->cached_nres;
+  double* xs = h->h_res->poses();
+  for (size_t i = 0; i < n; ++i)
+    for (int k = 0; k < 4; ++k) xs[4 * i + k] = poses[4 * (size_t)h->cached_order[i] + k];
+  OSB_CUDA(cudaMemcpyAsync(x0, xs, 4 * n * sizeof(double), cudaMemcpyHostToDevice, st));
   return OSB_OK;
 }
-
-// Launch shape of one solve.  It depends on the graph's size and the options only, never on how many solves run at once,
-// so that a trial of osb_solver_solve_multistart runs exactly the arithmetic of osb_solver_solve.
-struct SolveShape {
-  bool f32;              // fp32 inner (PCG) arithmetic
-  const void* kern;      // one solve per launch
-  const void* kern_multi;  // several clusters per launch, one trial each (same resources, same arithmetic)
-  int cluster;           // 1: one thread-block cluster per solve (hardware barrier); 0: one cooperative grid per launch
-  int ctas, fpc, chain, jsmem;
-  size_t smem;           // dynamic shared memory per CTA
-};
 
 static osb_status solve_shape(const osb_solver* h, int n_nodes, int n_factors, const osb_solve_options& o, SolveShape& s) {
   // inner precision: fp32 PCG unless the caller asks for a tighter inner solve than fp32 can deliver
@@ -1418,46 +1424,13 @@ static SolverDev graph_dev(const osb_solver* h, int n_nodes, int n_factors, cons
   return P;
 }
 
-// state of one solve inside a block of doubles laid out by trial_layout (per-trial buffers of the multistart arena)
-struct TrialLayout {
-  size_t x0, x1, out, nodevec, En, gs, cs, hs, es, Jg, partial, summary, bytes;
-};
-static TrialLayout trial_layout(int n_nodes, int n_factors, const SolveShape& s) {
-  const size_t n = n_nodes, m = n_factors;
-  TrialLayout L;
-  size_t at = 0;
-  auto take = [&](size_t bytes) { const size_t p = at; at += (bytes + 15) & ~(size_t)15; return p; };
-  L.x0 = take(4 * n * 8); L.x1 = take(4 * n * 8); L.out = take(4 * n * 8);
-  L.nodevec = take((7 * 4 + 2 * 16) * n * 8); L.En = take(16 * n * 8);
-  L.gs = take(8 * m * 8); L.cs = take(8 * m * 8); L.hs = take(32 * m * 8); L.es = take(16 * m * 8);
-  L.Jg = take(s.jsmem ? 0 : 32 * m * (s.f32 ? 4 : 8));
-  L.partial = take(2 * 4 * (size_t)s.ctas * 8);
-  L.summary = take(sizeof(osb_solve_summary));
-  L.bytes = at;
-  return L;
-}
-
-static void bind_nodevec(SolverDev& P, double* nv, size_t nodes) {
-  const size_t N4 = 4 * nodes, N16 = 16 * nodes;
-  P.g = nv; P.D = nv + N4; P.p = nv + 2 * N4; P.z = nv + 3 * N4; P.res = nv + 4 * N4; P.Ap = nv + 5 * N4;
-  P.delta = nv + 6 * N4; P.Hnn = nv + 7 * N4; P.Minv = nv + 7 * N4 + N16;
-}
-
-// every per-trial state pointer of P moved `o` bytes (host side: a cooperative launch runs one trial)
-static void shift_state(SolverDev& P, long long o) {
-  auto sh = [o](auto*& p) { p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<char*>(p) + o); };
-  sh(P.x[0]); sh(P.x[1]); sh(P.Jg); sh(P.g); sh(P.D); sh(P.Hnn); sh(P.Minv); sh(P.p); sh(P.z); sh(P.res); sh(P.Ap);
-  sh(P.delta); sh(P.gs); sh(P.cs); sh(P.hs); sh(P.partial); sh(P.summary); sh(P.poses_out); sh(P.es); sh(P.En);
-}
-
-// n_trials solves of one shape; trial t's state lies t * tstride bytes past P's.  Cluster path: ONE launch of n_trials
-// clusters (clusters do not wait for each other, so the grid may exceed what is resident).  Cooperative path: one grid
-// per trial, in order on the stream.
+// n_trials solves of one shape, P bound at trial 0 = the start of the arena, trial t's block tstride bytes further.
+// Cluster path: ONE launch of n_trials clusters (clusters do not wait for each other, so the grid may exceed what is
+// resident).  Cooperative path: one grid per trial, in order on the stream.
 static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s, int n_trials, long long tstride) {
   P.fpc = s.fpc; P.use_cluster = s.cluster; P.j_in_smem = s.jsmem; P.use_chain = s.chain;
   P.ctas = s.ctas; P.first_trial = 0; P.tstride = tstride;
-  h->last_grid = s.ctas; h->last_cluster = s.cluster; h->last_jsmem = s.jsmem; h->last_chain = s.chain;
-  h->last_f32 = s.f32 ? 1 : 0;
+  h->last_shape = s;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   cfg.blockDim = dim3(GS_THREADS); cfg.stream = h->stream; cfg.attrs = attr; cfg.numAttrs = 1;
@@ -1477,7 +1450,7 @@ static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s,
   for (int t = 0; t < n_trials; ++t) {
     SolverDev Q = P;
     Q.first_trial = t;
-    shift_state(Q, (long long)t * tstride);
+    trial_layout(Q, h->d_arena + t * tstride, P.n, P.m, s);
     void* kargs[1] = {&Q};
     OSB_CUDA(cudaLaunchKernelExC(&cfg, s.kern, kargs));
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1485,43 +1458,73 @@ static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s,
   return OSB_OK;
 }
 
-// the solve proper (K = 1 of launch_solves, in the handle's own buffers).  upload_static: see upload_graph.
-// The caller holds h->mu.
+// One call of the solver, shared by every entry point: pick the shape, lay the trials out in the arena, upload the graph
+// and the caller's poses into trial 0's x0, launch, copy back, and return the poses in the caller's numbering.
+// ms == nullptr: one solve from the caller's poses, its summary in summaries[0].  Otherwise ms->n_trials random
+// restarts of the init_mask nodes, ranked on the device: summaries and equv [K], chosen, and the chosen trial's poses
+// (the caller's stay as they were when no trial is accepted).  upload_static: see upload_graph.  The caller holds h->mu.
 static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed, int n_factors,
                              const int32_t* type, const int32_t* ia, const int32_t* ib, const double* payload,
-                             const uint8_t* huber, bool upload_static, const osb_solve_options* opt,
-                             osb_solve_summary* summary, unsigned long long topo_key = 0) {
+                             const uint8_t* huber, bool upload_static, unsigned long long topo_key,
+                             const osb_solve_options* opt, const osb_multistart_options* ms, const uint8_t* init_mask,
+                             osb_solve_summary* summaries, double* equv = nullptr, int32_t* chosen = nullptr) {
   osb_solve_options o;
   if (opt) o = *opt; else osb_solve_default_options(&o);
+  const int K = ms ? ms->n_trials : 1;
   const size_t n = n_nodes;
   cudaStream_t st = h->stream;
-  int n_res = 0;
-  osb_status s = upload_graph(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, upload_static, topo_key, n_res);
-  if (s != OSB_OK) return s;
-  const std::vector<int32_t>& order = h->cached_order;
   SolveShape shape;
-  s = solve_shape(h, n_nodes, n_factors, o, shape);
+  osb_status s = solve_shape(h, n_nodes, n_factors, o, shape);
   if (s != OSB_OK) return s;
-
   SolverDev P = graph_dev(h, n_nodes, n_factors, o);
-  P.x[0] = h->d_x0; P.x[1] = h->d_x1; P.Jg = h->d_Jg;
-  bind_nodevec(P, h->d_nodevec, h->max_nodes);
-  P.cs = h->d_cs; P.gs = h->d_gs; P.hs = h->d_hs; P.partial = h->d_partial; P.summary = h->d_summary; P.poses_out = h->d_out;
-  P.es = h->d_es; P.En = h->d_En;
+  const size_t tstride = trial_layout(P, nullptr, n, n_factors, shape);
+  if (K * tstride > h->arena_bytes) {     // multistart only; a failed allocation leaves the old arena in place
+    char* grown = nullptr;
+    OSB_CUDA(cudaMalloc(&grown, K * tstride));
+    cudaFree(h->d_arena);
+    h->d_arena = grown;
+    h->arena_bytes = K * tstride;
+  }
+  trial_layout(P, h->d_arena, n, n_factors, shape);
+  s = upload_graph(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, upload_static, topo_key, P.x[0]);
+  if (s != OSB_OK) return s;
+  if (ms) {
+    OSB_CUDA(cudaMemcpyAsync(h->d_order, h->cached_order.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_mask, init_mask, n, cudaMemcpyHostToDevice, st));
+    const long long kn = (long long)K * n_nodes;
+    OSB_LAUNCH(multistart_init_kernel, (unsigned)((kn + 255) / 256), 256, 0, st, n_nodes, K, h->d_fixed, h->d_order,
+               h->d_mask, ms->seed, ms->rand_xy, ms->rand_z, P.x[0], (long long)tstride);
+    OSB_CHECK_LAUNCH();
+  }
   OSB_CUDA(cudaEventRecord(h->ev0, st));
-  s = launch_solves(h, P, shape, 1, 0);
+  s = launch_solves(h, P, shape, K, (long long)tstride);
   if (s != OSB_OK) return s;
   OSB_CUDA(cudaEventRecord(h->ev1, st));
-  OSB_CUDA(cudaMemcpyAsync(h->h_x, h->d_out, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, st));
-  OSB_CUDA(cudaMemcpyAsync(h->h_summary, h->d_summary, sizeof(osb_solve_summary), cudaMemcpyDeviceToHost, st));
+  SolveResults* r = h->h_res;
+  if (ms) {
+    OSB_LAUNCH(multistart_select_kernel, 1, 32, 0, st, K, n_nodes, P.summary, P.poses_out, (long long)tstride,
+               ms->normalise ? 1 : 0, h->cached_nres, ms->window_size, ms->acpt_cost, h->d_res);
+    OSB_CHECK_LAUNCH();
+    OSB_CUDA(cudaMemcpyAsync(r, h->d_res, sizeof(SolveResults) + 4 * n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  } else {
+    OSB_CUDA(cudaMemcpyAsync(r->poses(), P.poses_out, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaMemcpyAsync(&r->summaries[0], P.summary, sizeof(osb_solve_summary), cudaMemcpyDeviceToHost, st));
+  }
   OSB_CUDA(cudaStreamSynchronize(st));
-  *summary = *h->h_summary;
-  for (size_t i = 0; i < n; ++i)
-    for (int k = 0; k < 4; ++k) poses[4 * (size_t)order[i] + k] = h->h_x[4 * i + k];
-  float ms = 0.f;
-  OSB_CUDA(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-  summary->solve_ms = ms;
-  summary->n_residuals = n_res;
+  float msec = 0.f;
+  OSB_CUDA(cudaEventElapsedTime(&msec, h->ev0, h->ev1));
+  for (int t = 0; t < K; ++t) {
+    summaries[t] = r->summaries[t];
+    summaries[t].solve_ms = msec;
+    summaries[t].n_residuals = h->cached_nres;
+  }
+  if (ms) {
+    std::memcpy(equv, r->equv, K * sizeof(double));
+    *chosen = r->chosen;
+  }
+  if (!ms || r->chosen >= 0)
+    for (size_t i = 0; i < n; ++i)
+      for (int k = 0; k < 4; ++k) poses[4 * (size_t)h->cached_order[i] + k] = r->poses()[4 * i + k];
   return OSB_OK;
 }
 
@@ -1538,13 +1541,13 @@ extern "C" osb_status osb_solver_solve(osb_solver* h, int n_nodes, double* poses
   DeviceGuard dg(h->device);
   h->g_static_valid = false;              // the device factor arrays now hold this graph, not the resident one
   h->cached_topo = 0;                     // ... and so do the index tables
-  return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, opt, summary);
+  return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, opt, nullptr, nullptr,
+                    summary);
 }
 
 // ---- random-restart initialisation: solve_with_multiple_init (swarm_localization_solver.cpp:781-845) ----------------
 // Trials start from the caller's poses with the masked free nodes scattered (multistart_init_kernel), run as one launch
 // of n_trials solves of the osb_solver_solve shape, and are ranked on the device (multistart_select_kernel).
-// Arena: [order n x int32 | mask n | chosen poses 4n | equv K | summaries K | chosen] then K trial blocks (trial_layout).
 extern "C" osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, double* poses, const uint8_t* fixed,
                                                   const uint8_t* init_mask, int n_factors, const int32_t* type,
                                                   const int32_t* ia, const int32_t* ib, const double* payload,
@@ -1553,7 +1556,7 @@ extern "C" osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, do
                                                   double* equv_costs, int32_t* chosen) {
   OSB_REQUIRE(h && poses && fixed && init_mask && type && ia && ib && payload && huber && ms && trial_summaries &&
               equv_costs && chosen, "null argument");
-  OSB_REQUIRE(ms->n_trials >= 1 && ms->n_trials <= 256, "n_trials must be 1 ... 256");
+  OSB_REQUIRE(ms->n_trials >= 1 && ms->n_trials <= MS_MAX_TRIALS, "n_trials must be 1 ... 256");
   OSB_REQUIRE(!ms->normalise || ms->window_size >= 1, "window_size must be >= 1 when normalise is set");
   OSB_REQUIRE(std::isfinite(ms->rand_xy) && ms->rand_xy >= 0.0 && std::isfinite(ms->rand_z) && ms->rand_z >= 0.0,
               "rand_xy and rand_z must be finite and >= 0");
@@ -1566,82 +1569,8 @@ extern "C" osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, do
   DeviceGuard dg(h->device);
   h->g_static_valid = false;              // as osb_solver_solve: the device factor arrays and tables now hold this graph
   h->cached_topo = 0;
-  for (const void* k : {(const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>}) {
-    OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
-    if (h->cluster_ok) OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-  }
-  osb_solve_options o;
-  if (opt) o = *opt; else osb_solve_default_options(&o);
-  const int K = ms->n_trials;
-  const size_t n = n_nodes;
-  cudaStream_t st = h->stream;
-  int n_res = 0;
-  s = upload_graph(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, n_res);
-  if (s != OSB_OK) return s;
-  SolveShape shape;
-  s = solve_shape(h, n_nodes, n_factors, o, shape);
-  if (s != OSB_OK) return s;
-
-  const TrialLayout L = trial_layout(n_nodes, n_factors, shape);
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  const size_t o_order = 0, o_mask = al(4 * n), o_poses = o_mask + al(n), o_equv = o_poses + 4 * n * sizeof(double);
-  const size_t o_sum = o_equv + K * sizeof(double), o_chosen = o_sum + K * sizeof(osb_solve_summary);
-  const size_t res_bytes = o_chosen + sizeof(int32_t) - o_poses;
-  const size_t o_trials = al(o_chosen + sizeof(int32_t)), need = o_trials + K * L.bytes;
-  if (h->ms_bytes < need) {               // a failed allocation leaves no arena and the handle as it was otherwise
-    cudaFree(h->d_ms); h->d_ms = nullptr; h->ms_bytes = 0;
-    OSB_CUDA(cudaMalloc(&h->d_ms, need));
-    h->ms_bytes = need;
-  }
-  if (h->h_ms_bytes < res_bytes) {
-    if (h->h_ms) cudaFreeHost(h->h_ms);
-    h->h_ms = nullptr; h->h_ms_bytes = 0;
-    OSB_CUDA(cudaHostAlloc((void**)&h->h_ms, res_bytes, cudaHostAllocDefault));
-    h->h_ms_bytes = res_bytes;
-  }
-  char* A = h->d_ms;
-  char* T0 = A + o_trials;
-  OSB_CUDA(cudaMemcpyAsync(A + o_order, h->cached_order.data(), 4 * n, cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(A + o_mask, init_mask, n, cudaMemcpyHostToDevice, st));
-  const long long kn = (long long)K * n_nodes;
-  OSB_LAUNCH(multistart_init_kernel, (unsigned)((kn + 255) / 256), 256, 0, st, n_nodes, K, h->d_x0, h->d_fixed,
-             reinterpret_cast<const int32_t*>(A + o_order), reinterpret_cast<const uint8_t*>(A + o_mask), ms->seed,
-             ms->rand_xy, ms->rand_z, reinterpret_cast<double*>(T0 + L.x0), (long long)L.bytes);
-  OSB_CHECK_LAUNCH();
-
-  SolverDev P = graph_dev(h, n_nodes, n_factors, o);
-  P.x[0] = reinterpret_cast<double*>(T0 + L.x0); P.x[1] = reinterpret_cast<double*>(T0 + L.x1);
-  P.Jg = T0 + L.Jg;
-  bind_nodevec(P, reinterpret_cast<double*>(T0 + L.nodevec), n);
-  P.cs = T0 + L.cs; P.gs = reinterpret_cast<double*>(T0 + L.gs); P.hs = reinterpret_cast<double*>(T0 + L.hs);
-  P.partial = reinterpret_cast<double*>(T0 + L.partial); P.summary = reinterpret_cast<osb_solve_summary*>(T0 + L.summary);
-  P.poses_out = reinterpret_cast<double*>(T0 + L.out);
-  P.es = reinterpret_cast<double*>(T0 + L.es); P.En = reinterpret_cast<double*>(T0 + L.En);
-  OSB_CUDA(cudaEventRecord(h->ev0, st));
-  s = launch_solves(h, P, shape, K, (long long)L.bytes);
-  if (s != OSB_OK) return s;
-  OSB_CUDA(cudaEventRecord(h->ev1, st));
-  OSB_LAUNCH(multistart_select_kernel, 1, 32, 0, st, K, n_nodes, T0, (long long)L.bytes, L.summary, L.out,
-             ms->normalise ? 1 : 0, n_res, ms->window_size, ms->acpt_cost, reinterpret_cast<double*>(A + o_poses),
-             reinterpret_cast<double*>(A + o_equv), reinterpret_cast<osb_solve_summary*>(A + o_sum),
-             reinterpret_cast<int32_t*>(A + o_chosen));
-  OSB_CHECK_LAUNCH();
-  OSB_CUDA(cudaMemcpyAsync(h->h_ms, A + o_poses, res_bytes, cudaMemcpyDeviceToHost, st));
-  OSB_CUDA(cudaStreamSynchronize(st));
-  float msec = 0.f;
-  OSB_CUDA(cudaEventElapsedTime(&msec, h->ev0, h->ev1));
-  auto res = [&](size_t off) { return h->h_ms + (off - o_poses); };
-  std::memcpy(equv_costs, res(o_equv), K * sizeof(double));
-  std::memcpy(trial_summaries, res(o_sum), K * sizeof(osb_solve_summary));
-  for (int t = 0; t < K; ++t) { trial_summaries[t].solve_ms = msec; trial_summaries[t].n_residuals = n_res; }
-  std::memcpy(chosen, res(o_chosen), sizeof(int32_t));
-  if (*chosen >= 0) {
-    const double* xp = reinterpret_cast<const double*>(res(o_poses));
-    const std::vector<int32_t>& order = h->cached_order;
-    for (size_t i = 0; i < n; ++i)
-      for (int k = 0; k < 4; ++k) poses[4 * (size_t)order[i] + k] = xp[4 * i + k];
-  }
-  return OSB_OK;
+  return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, opt, ms, init_mask,
+                    trial_summaries, equv_costs, chosen);
 }
 
 // -------------------------------------------------------------------------------------------------------------
@@ -1773,7 +1702,8 @@ extern "C" osb_status osb_solver_solve_resident(osb_solver* h, const osb_solve_o
     h->g_uploaded = m;
   }
   return solver_run(h, (int)n, h->g_poses.data(), h->g_fixed.data(), (int)m, h->g_type.data(), h->g_ia.data(),
-                    h->g_ib.data(), h->g_payload.data(), h->g_huber.data(), false, opt, summary, h->g_topo_version);
+                    h->g_ib.data(), h->g_payload.data(), h->g_huber.data(), false, h->g_topo_version, opt, nullptr,
+                    nullptr, summary);
 }
 
 extern "C" osb_status osb_solver_phase_cycles(osb_solver* h, double* out12) {
@@ -1783,7 +1713,8 @@ extern "C" osb_status osb_solver_phase_cycles(osb_solver* h, double* out12) {
   long long c[8];
   OSB_CUDA(cudaMemcpy(c, h->d_dbg, sizeof(c), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 8; ++i) out12[i] = (double)c[i];
-  out12[8] = h->last_grid; out12[9] = h->last_cluster; out12[10] = h->last_jsmem + 2 * h->last_chain + 4 * h->last_f32; out12[11] = GS_THREADS;
+  const SolveShape& s = h->last_shape;
+  out12[8] = s.ctas; out12[9] = s.cluster; out12[10] = s.jsmem + 2 * s.chain + 4 * (s.f32 ? 1 : 0); out12[11] = GS_THREADS;
   return OSB_OK;
 }
 
@@ -1808,17 +1739,20 @@ extern "C" osb_status osb_solver_linearize(osb_solver* h, int n_nodes, const dou
   if (s != OSB_OK) return s;
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  h->g_static_valid = false;              // as osb_solver_solve: the device factor arrays and tables now hold this graph
+  h->cached_topo = 0;
   const size_t n = n_nodes, m = n_factors;
   cudaStream_t st = h->stream;
+  double* d_x = h->d_lin;             // [n][4]
+  double* d_r = d_x + 4 * n;          // [m][4]
+  double* d_ja = d_r + 4 * m;         // [m][16]
+  double* d_jb = d_ja + 16 * m;       // [m][16]
   OSB_CUDA(cudaMemcpyAsync(h->d_type, type, m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_ia, ia, m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_ib, ib, m * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_payload, payload, m * OSB_PAYLOAD_LEN * sizeof(double), cudaMemcpyHostToDevice, st));
-  OSB_CUDA(cudaMemcpyAsync(h->d_x0, poses, 4 * n * sizeof(double), cudaMemcpyHostToDevice, st));
-  double* d_r = h->d_lin;             // [m][4]
-  double* d_ja = h->d_lin + 4 * m;    // [m][16]
-  double* d_jb = h->d_lin + 20 * m;   // [m][16]
-  OSB_LAUNCH(graph_linearize_kernel, cdiv(n_factors, 128), 128, 0, st, n_factors, h->d_x0, h->d_type, h->d_ia, h->d_ib,
+  OSB_CUDA(cudaMemcpyAsync(d_x, poses, 4 * n * sizeof(double), cudaMemcpyHostToDevice, st));
+  OSB_LAUNCH(graph_linearize_kernel, cdiv(n_factors, 128), 128, 0, st, n_factors, d_x, h->d_type, h->d_ia, h->d_ib,
              h->d_payload, d_r, d_ja, d_jb);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(cudaMemcpyAsync(r, d_r, 4 * m * sizeof(double), cudaMemcpyDeviceToHost, st));

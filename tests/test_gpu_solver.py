@@ -201,6 +201,12 @@ def test_resident_graph_incremental_equals_one_shot(solver):
     solver.graph_set_poses(0, g["init"])
     s3 = solver.solve_resident()
     assert np.array_equal(solver.graph_get_poses(), ref_poses) and s3.final_cost == ref_s.final_cost
+    # ... and neither may a linearize of another graph, with the resident topology (and its cached tables) unchanged
+    solver.linearize(other, other["init"])
+    solver.graph_set_poses(0, g["init"])
+    s4 = solver.solve_resident()
+    assert np.array_equal(solver.graph_get_poses(), ref_poses) and s4.final_cost == ref_s.final_cost
+    assert s4.pcg_iterations == ref_s.pcg_iterations
 
 
 def test_resident_graph_sliding_window(solver):
