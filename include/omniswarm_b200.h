@@ -96,9 +96,8 @@ osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int n);
  *               mode 0: out_f32 [batch*Ho*Wo][out_cstride]; mode 1: planes out_hi/out_lo [batch][Ho][Wo][out_cstride] at
  *               out_scale; mode 2: the detector head (cout 65, ks 1): softmax, dustbin dropped, 8x8 pixel shuffle into
  *               out_f32 = heat map [batch][8H][8W].
- *  conv_first:  SuperPoint conv1a (w1a [64][1][3][3]) + ReLU on u8 images [batch][H][W] (scaled by 1/255), planes at
- *               act_scale: fused = 0 -> the conv1a planes [batch][H][W][64]; fused = 1 -> conv1a + conv1b (w1b
- *               [64][64][3][3], weights at x1024) + ReLU + 2x2 max-pool in one kernel -> [batch][H/2][W/2][64].
+ *  conv_first:  SuperPoint conv1a (w1a [64][1][3][3]) + ReLU on u8 images [batch][H][W] (scaled by 1/255) -> the conv1a
+ *               planes [batch][H][W][64] at act_scale.
  *  dwconv:      depthwise 3x3 (w [C][1][3][3], pad 1, stride 1 or 2) + bias + ReLU6 on fp32 NHWC x [batch][H][W][C]
  *               -> planes [batch][H/stride][W/stride][C] at out_scale; generic = 1 runs the one-pixel kernel at stride 1
  *               instead of the four-pixel one. */
@@ -106,9 +105,8 @@ osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int
                                  const void* in_hi, const void* in_lo, int batch, int height, int width, float act_scale,
                                  int relu, int pool, int out_c, int out_cstride, int max_ctas, int mode, float* out_f32,
                                  void* out_hi, void* out_lo, float out_scale, void* stream);
-osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const float* w1b, const float* b1b,
-                                 const uint8_t* images_dev, int batch, int height, int width, float act_scale, int fused,
-                                 void* out_hi, void* out_lo, int max_ctas, void* stream);
+osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch, int height,
+                                 int width, float act_scale, void* out_hi, void* out_lo, void* stream);
 osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
                              int channels, int stride, int generic, float out_scale, void* out_hi, void* out_lo,
                              void* stream);

@@ -36,14 +36,6 @@ osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi
                                      float act_scale, float* semi, cudaStream_t st, int max_ctas = 0);
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
                               __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st);
-// conv1a + ReLU + conv1b + ReLU + 2x2 max-pool in one kernel (conv_umma.cu, FIRST form): u8 images -> pooled split planes.
-// conv1a's weights and bias, pre-multiplied by the plane scale, as a KERNEL PARAMETER: with lane = pixel every FFMA of a warp
-// uses the same weight, so it comes from the constant bank instead of occupying 72 registers per thread
-struct Conv1aW { float w[9][64]; float b[64]; };
-
-osb_status umma_conv1_fused_forward(const UmmaLayer& L1b, const float* w1a, const float* b1a, const uint8_t* img, int B, int H,
-                                    int W, float act_scale, __half* out_hi, __half* out_lo, float out_scale, cudaStream_t st,
-                                    int max_ctas = 0);
 osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
 // depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv).  Stride 1 runs

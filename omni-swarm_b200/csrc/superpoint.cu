@@ -39,7 +39,6 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
   OSB_CUDA(cudaEventCreateWithFlags(&ev_kp, cudaEventDisableTiming));
   if (const char* e = getenv("OSB_SP_OVERLAP")) overlap_kp = atoi(e) != 0;
   if (const char* e = getenv("OSB_SP_FUSED_SOFTMAX")) fused_softmax = atoi(e) != 0;
-  if (const char* e = getenv("OSB_SP_FUSE1")) fuse_first = atoi(e) != 0;
   // ---- weights ----
   const float* p = weights;
   {
@@ -51,8 +50,6 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
     OSB_CUDA(cudaMalloc(&b1a, 64 * sizeof(float)));
     OSB_CUDA(cudaMemcpy(w1a, w9.data(), 9 * 64 * sizeof(float), cudaMemcpyHostToDevice));
     OSB_CUDA(cudaMemcpy(b1a, p + 64 * 9, 64 * sizeof(float), cudaMemcpyHostToDevice));
-    w1a_host = w9;
-    b1a_host.assign(p + 64 * 9, p + 64 * 9 + 64);
     p += 64 * 9 + 64;
   }
   {
@@ -155,16 +152,10 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
     return umma_conv_forward(UL[i], tmA[i], tmB[i], B, h, w, SA, in_hi[out_layer], in_lo[out_layer], nullptr,
                              SP_COUT[i], SP_COUT[i], SA, 1, pool, st);
   };
-  if (fuse_first) {
-    mark(st);                                                                             // (conv1a has no launch of its own)
-    RUN(umma_conv1_fused_forward(UL[1], w1a_host.data(), b1a_host.data(), img_dev, B, H, W, SA, in_hi[2], in_lo[2], SA, st));
-    mark(st);                                                                             // conv1a+conv1b+pool -> B
-  } else {
-    RUN(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st)); // conv1a            -> A
-    mark(st);
-    RUN(conv(1, H, W, 2, 1));                                                             // conv1b + pool     -> B
-    mark(st);
-  }
+  RUN(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st));   // conv1a            -> A
+  mark(st);
+  RUN(conv(1, H, W, 2, 1));                                                               // conv1b + pool     -> B
+  mark(st);
   RUN(conv(2, H / 2, W / 2, 3, 0));                                                       // conv2a            -> A
   mark(st);
   RUN(conv(3, H / 2, W / 2, 4, 1));                                                       // conv2b + pool     -> B

@@ -15,7 +15,6 @@ struct SuperPoint {
   cudaStream_t stream = nullptr;
   // weights
   float *w1a = nullptr, *b1a = nullptr, *lut = nullptr, *pca_compT = nullptr, *pca_mean_d = nullptr;
-  std::vector<float> w1a_host, b1a_host;          // conv1a [tap][64] and bias: the fused first-layers kernel takes them as a kernel parameter
   ConvLayer L[12];
   // activations / outputs (device)
   uint8_t* d_img = nullptr;
@@ -44,10 +43,6 @@ struct SuperPoint {
   cudaStream_t kp_stream = nullptr;
   cudaEvent_t ev_semi = nullptr, ev_kp = nullptr;
   bool overlap_kp = true;
-  bool fuse_first = false;         // OSB_SP_FUSE1=1: conv1a computed inside conv1b's kernel (conv_umma.cu, FIRST form).  Off by
-                                   // default: on an H100 (80GB HBM3, 400 W power limit) conv1a+conv1b+pool of 8 images at 640x480
-                                   // took 5.44 ms fused against 1.28 ms as two kernels -- the producer warpgroup computes each conv1a
-                                   // pixel three times (once per kx-shifted box) and cannot keep up with the MMAs
   bool fused_softmax = true;       // detector-head softmax + pixel shuffle in convPb's epilogue (OSB_SP_FUSED_SOFTMAX=0: two kernels)
   osb_status network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp = nullptr);
   osb_status network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp);

@@ -634,21 +634,17 @@ def conv_layer_parity(w, bias, in_hi, in_lo, act_scale: float, *, w_scale: float
     return (hi, lo) if mode == "planes" else f32
 
 
-def conv_first_parity(w1a, b1a, images, act_scale: float, *, fused: bool = False, w1b=None, b1b=None, max_ctas: int = 0):
-    """SuperPoint's first layer(s) (osb_conv_first_parity): images CUDA torch.uint8 [B,H,W] -> (hi, lo) float16 planes at
-    act_scale: conv1a + ReLU [B,H,W,64], or with fused=True conv1a + conv1b + ReLU + 2x2 max-pool [B,H/2,W/2,64]."""
+def conv_first_parity(w1a, b1a, images, act_scale: float):
+    """SuperPoint's first layer (osb_conv_first_parity): images CUDA torch.uint8 [B,H,W] -> conv1a + ReLU as (hi, lo)
+    float16 planes [B,H,W,64] at act_scale."""
     import torch
     B, H, W = images.shape
-    shape = (B, H // 2, W // 2, 64) if fused else (B, H, W, 64)
-    hi = torch.full(shape, float("nan"), dtype=torch.float16, device=images.device)
+    hi = torch.full((B, H, W, 64), float("nan"), dtype=torch.float16, device=images.device)
     lo = torch.full_like(hi, float("nan"))
     w1a, b1a = _f32(w1a), _f32(b1a)
-    w1b = None if w1b is None else _f32(w1b)
-    b1b = None if b1b is None else _f32(b1b)
     _l.check(_l.load().osb_conv_first_parity(
-        _l.ptr(w1a), _l.ptr(b1a), _l.ptr(w1b), _l.ptr(b1b), C.c_void_p(images.data_ptr()), B, H, W, float(act_scale),
-        int(fused), C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()), int(max_ctas),
-        C.c_void_p(torch.cuda.current_stream(images.device).cuda_stream)))
+        _l.ptr(w1a), _l.ptr(b1a), C.c_void_p(images.data_ptr()), B, H, W, float(act_scale), C.c_void_p(hi.data_ptr()),
+        C.c_void_p(lo.data_ptr()), C.c_void_p(torch.cuda.current_stream(images.device).cuda_stream)))
     return hi, lo
 
 

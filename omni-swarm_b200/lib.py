@@ -113,8 +113,7 @@ _SIG = {
     "osb_conv_layer_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int,
                                         C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                         C.c_float, _P]),
-    "osb_conv_first_parity": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P, _P,
-                                        C.c_int, _P]),
+    "osb_conv_first_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
     "osb_dwconv_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P,
                                     _P]),
     "osb_netvlad_create": (C.c_int, [C.POINTER(_P), _P, C.c_size_t, C.c_int, C.c_int, C.c_int]),

@@ -218,33 +218,6 @@ def test_tensor_core_path_vs_cuda_core_path(gpu):
         print("rel err vs oracle (semi, desc):", {m: (rel_err(out[m][b][0], so), rel_err(out[m][b][1], do)) for m in out})
 
 
-@pytest.mark.parametrize("size", [(640, 480), (400, 208), (96, 64), (200, 120)])
-def test_fused_first_layers_bit_identical(gpu, size):
-    """conv1a computed inside conv1b's kernel (conv_umma.cu, FIRST form: the producer warpgroup writes conv1a's split planes
-    straight into the shared-memory A slots) against the two-kernel path (conv1a planes through HBM, then the TMA-box
-    kernel): same fp32 FMA order in conv1a, same MMA accumulation order in conv1b, so heat-map and descriptor map must be
-    BIT-identical -- including ragged tiles (208 = 13 x 16 rows, 200 x 120: half tiles in both directions at every
-    resolution) and the blanked bottom quarter."""
-    W, H = size
-    comp, mean = synth.pca_matrices(0)
-    wts = synth.flatten_sp_weights(synth.superpoint_weights(0))
-    imgs = np.stack([synth.image(11, H, W), synth.image(12, H, W, zero_bottom_quarter=True),
-                     np.zeros((H, W), np.uint8)])
-    imgs[2, ::7, ::5] = 255
-    out = {}
-    # "fused": conv1a + conv1b + pool in one kernel; "box": conv1a through HBM + the TMA-box kernel for every layer
-    for name, f1 in {"fused": "1", "box": "0"}.items():
-        os.environ["OSB_SP_FUSE1"] = f1
-        sp = host.SuperPoint(wts, comp, mean, W, H, 0.015, 200, max_batch=3)
-        res = sp.inference_batch(imgs)
-        out[name] = [(sp.read("semi", b), sp.read("desc", b), res[b][0], res[b][1]) for b in range(3)]
-        sp.close()
-    os.environ.pop("OSB_SP_FUSE1")
-    for b in range(3):
-        for a, c in zip(out["fused"][b], out["box"][b]):
-            assert np.array_equal(a, c, equal_nan=True), f"image {b}: the fused first layers and the two-kernel path differ"
-
-
 def test_fused_softmax_matches_two_kernel_softmax(gpu):
     """The detector head's softmax + pixel shuffle fused into convPb's epilogue (default) against convPb writing its logits
     and sp_softmax_shuffle_kernel (OSB_SP_FUSED_SOFTMAX=0).  Same logits; the fused form reduces max and sum over the four
