@@ -533,6 +533,25 @@ osb_status osb_frontend_db_load(osb_frontend* h, int remote, int64_t n, const fl
 osb_status osb_frontend_set_cameras(osb_frontend* h, const double* intrinsics /*[4]*/, const double* left_extrinsics /*[n_dirs][7]*/,
                                     const double* right_extrinsics /*[n_dirs][7]*/, double triangle_thres);
 osb_status osb_frontend_set_drone_pose(osb_frontend* h, const double* pose_drone /*[7]*/);
+/* Depth-camera keyframes (PINHOLE_DEPTH, LoopCam::generate_gray_depth_image_descriptor, loop_cam.cpp:231-302): one gray
+ * image and one aligned 16-bit depth image (mm) per direction, both of the configured W x H.  extract_depth runs SuperPoint
+ * and NetVLAD on the n_dirs gray images (the bottom quarter is never blanked; zero_bottom_quarter is a STEREO_FISHEYE
+ * setting) and, when n_kpts > accept_min_3d_pts, lifts every keypoint through the depth look-up of osb_depth_lift with
+ * pose_cam = pose_drone * extrinsics[d] (pose_drone from osb_frontend_set_drone_pose): landmarks_flag = 1 iff
+ * near_thres < depth / 1000 < far_thres.  There is no stereo match: stereo_match = -1, n_kpts_down = 0.
+ * set_depth_camera takes the intrinsics fx fy cx cy of the distortion-free pinhole and allocates the handle's depth buffer;
+ * the extracts return OSB_ERR_INVALID until it has been called.  The stereo extract is unaffected by it. */
+osb_status osb_frontend_set_depth_camera(osb_frontend* h, const double* intrinsics /*[4]*/,
+                                         const double* extrinsics /*[n_dirs][7]*/, double near_thres, double far_thres);
+/* images [n_dirs][H][W] uint8 and depth_mm [n_dirs][H][W] uint16, HOST (pinned or pageable) -> record_dev, no synchronisation */
+osb_status osb_frontend_extract_depth(osb_frontend* h, const uint8_t* images, const uint16_t* depth_mm, int32_t msg_id,
+                                      osb_keyframe_record* record_dev, void* stream);
+/* same with images and depth already on the device */
+osb_status osb_frontend_extract_depth_dev(osb_frontend* h, const uint8_t* images_dev, const uint16_t* depth_mm_dev,
+                                          int32_t msg_id, osb_keyframe_record* record_dev, void* stream);
+/* osb_frontend_process for a depth keyframe: extract_depth + ingest(own) + query, one synchronisation at the end */
+osb_status osb_frontend_process_depth(osb_frontend* h, const uint8_t* images, const uint16_t* depth_mm, int32_t msg_id,
+                                      osb_keyframe_record* record_host, osb_loop_result* result_host);
 /* landmarks_2d [n][max_num][2] and stereo_match [n][max_num] (>= 0 <=> landmarks_flag) of rows loaded with
  * osb_frontend_db_load -- what the geometric filter reads when such a row is the loop hit */
 osb_status osb_frontend_db_set_geometry(osb_frontend* h, int remote, int64_t first_row, int64_t n, const float* kpts,
@@ -540,7 +559,7 @@ osb_status osb_frontend_db_set_geometry(osb_frontend* h, int remote, int64_t fir
 /* stage timing (CUDA events on the caller's stream, recorded only while enabled).  After a synchronising call
  * (process / finish) stage_ms returns the device time of the LAST extract+ingest+query sequence:
  * [0] SuperPoint network  [1] keypoints + descriptors (NetVLAD runs concurrently on a second stream)
- * [2] NetVLAD remainder not hidden behind [1]  [3] stereo match + record pack
+ * [2] NetVLAD remainder not hidden behind [1]  [3] stereo match + record pack (depth keyframes: depth lift + record pack)
  * [4] add_to_database  [5] database scans (remote + local)  [6] acceptance rule + per-direction match  [7] unused */
 osb_status osb_frontend_set_profiling(osb_frontend* h, int enable);
 osb_status osb_frontend_stage_ms(osb_frontend* h, float* ms8);

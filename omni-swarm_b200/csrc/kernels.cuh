@@ -74,6 +74,10 @@ osb_status stereo_lift_device(const float* kp_up, const float* kp_down, const in
                               const int32_t* n_down, int n_dirs, int max_n, const double* K, const double* pose_up,
                               const double* pose_down, double triangle_thres, int min_pts, float* pts3d, uint8_t* flag_up,
                               uint8_t* flag_down, cudaStream_t st);
+// depth look-up lift of the keypoints of n_dirs directions (lift.cu; loop_cam.cpp:276-302)
+osb_status depth_lift_device(const float* kp, const int32_t* n_kp, int n_dirs, int max_n, const uint16_t* depth_mm, int H,
+                             int W, const double* K, const double* pose_cam, double near_thres, double far_thres,
+                             int min_pts, float* pts3d, uint8_t* flag, cudaStream_t st);
 osb_status homography_ransac_device(const float* src_dev, const float* dst_dev, const int32_t* n_dev, int n_pairs, int max_n,
                                     float thresh, uint32_t seed, uint8_t* mask_dev, int32_t* n_inl_dev, int32_t* winner_dev,
                                     cudaStream_t st, unsigned int* scratch /* 2 * n_pairs words, zero between launches */);

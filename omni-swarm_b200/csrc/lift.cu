@@ -154,6 +154,16 @@ osb_status stereo_lift_device(const float* kp_up, const float* kp_down, const in
   return OSB_OK;
 }
 
+osb_status depth_lift_device(const float* kp, const int32_t* n_kp, int n_dirs, int max_n, const uint16_t* depth_mm, int H,
+                             int W, const double* K, const double* pose_cam, double near_thres, double far_thres,
+                             int min_pts, float* pts3d, uint8_t* flag, cudaStream_t st) {
+  const LiftCam cam{K[0], K[1], K[2], K[3]};
+  OSB_LAUNCH(depth_lift_kernel, dim3(cdiv(max_n, 64), n_dirs), 64, 0, st, kp, n_kp, max_n, depth_mm, H, W, cam, pose_cam,
+             near_thres, far_thres, min_pts, pts3d, flag);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -181,11 +191,8 @@ extern "C" osb_status osb_depth_lift_dev(const float* kp_dev, const int32_t* n_d
   OSB_REQUIRE(n_dirs > 0 && max_n > 0 && height > 0 && width > 0, "bad sizes");
   osb_status s = require_device();
   if (s != OSB_OK) return s;
-  const LiftCam cam{intrinsics[0], intrinsics[1], intrinsics[2], intrinsics[3]};
-  OSB_LAUNCH(depth_lift_kernel, dim3(cdiv(max_n, 64), n_dirs), 64, 0, (cudaStream_t)stream, kp_dev, n_dev, max_n, depth_mm_dev,
-             height, width, cam, pose_cam_dev, near_thres, far_thres, accept_min_3d_pts, pts3d_dev, flag_dev);
-  OSB_CHECK_LAUNCH();
-  return OSB_OK;
+  return depth_lift_device(kp_dev, n_dev, n_dirs, max_n, depth_mm_dev, height, width, intrinsics, pose_cam_dev, near_thres,
+                           far_thres, accept_min_3d_pts, pts3d_dev, flag_dev, (cudaStream_t)stream);
 }
 
 // host-buffer convenience forms (tests, small callers)

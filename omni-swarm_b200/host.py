@@ -450,6 +450,43 @@ class KeyframeFrontend:
         p = np.ascontiguousarray(pose_drone, np.float64)
         _l.check(self._lib.osb_frontend_set_drone_pose(self._h, _l.ptr(p)))
 
+    def set_depth_camera(self, intrinsics, extrinsics, near_thres=0.3, far_thres=10.0):
+        """PINHOLE_DEPTH keyframes (loop_cam.cpp:231-302): pinhole intrinsics fx fy cx cy, extrinsics [n_dirs,7],
+        DEPTH_NEAR_THRES / DEPTH_FAR_THRES in metres"""
+        K = np.ascontiguousarray(intrinsics, np.float64)
+        ext = np.ascontiguousarray(extrinsics, np.float64)
+        assert K.shape == (4,) and ext.shape == (self.cfg.n_dirs, 7)
+        _l.check(self._lib.osb_frontend_set_depth_camera(self._h, _l.ptr(K), _l.ptr(ext), float(near_thres), float(far_thres)))
+
+    def _depth_inputs(self, images, depth_mm):
+        img = np.ascontiguousarray(images, np.uint8); dep = np.ascontiguousarray(depth_mm, np.uint16)
+        shape = (self.cfg.n_dirs, self.cfg.height, self.cfg.width)
+        assert img.shape == shape and dep.shape == shape, "images and depth must be [n_dirs, H, W]"
+        return img, dep
+
+    def extract_depth(self, images, depth_mm, msg_id: int, record_dev: int, stream: int, device_images=False):
+        """gray images [n_dirs,H,W] u8 + depth [n_dirs,H,W] u16 mm -> record_dev, no synchronisation.  HOST numpy arrays, or
+        with device_images=True two device pointers (ints)."""
+        if device_images:
+            _l.check(self._lib.osb_frontend_extract_depth_dev(self._h, C.c_void_p(images), C.c_void_p(depth_mm), msg_id,
+                                                              C.c_void_p(record_dev), C.c_void_p(stream)))
+            return
+        img, dep = self._depth_inputs(images, depth_mm)
+        _l.check(self._lib.osb_frontend_extract_depth(self._h, _l.ptr(img), _l.ptr(dep), msg_id, C.c_void_p(record_dev),
+                                                      C.c_void_p(stream)))
+
+    def process_depth(self, images: np.ndarray, depth_mm: np.ndarray, msg_id: int):
+        """HOST gray images [n_dirs,H,W] u8 + depth [n_dirs,H,W] u16 mm -> (KeyframeRecord, LoopResult); one synchronisation."""
+        img, dep = self._depth_inputs(images, depth_mm)
+        rec, res = _l.KeyframeRecord(), _l.LoopResult()
+        _l.check(self._lib.osb_frontend_process_depth(self._h, _l.ptr(img), _l.ptr(dep), msg_id, C.byref(rec), C.byref(res)))
+        return rec, res
+
+    def process_depth_raw(self, img_ptr: int, depth_ptr: int, msg_id: int, rec_ptr: int, res_ptr: int):
+        """same, with raw HOST pointers (pinned buffers owned by the caller)."""
+        _l.check(self._lib.osb_frontend_process_depth(self._h, C.c_void_p(img_ptr), C.c_void_p(depth_ptr), msg_id,
+                                                      C.c_void_p(rec_ptr), C.c_void_p(res_ptr)))
+
     def db_size(self, remote=False) -> int:
         return int(self._lib.osb_frontend_db_size(self._h, int(remote)))
 

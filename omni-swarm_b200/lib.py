@@ -176,6 +176,10 @@ _SIG = {
     "osb_depth_lift_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_double, C.c_double, C.c_int, _P, _P, _P]),
     "osb_frontend_set_cameras": (C.c_int, [_P, _P, _P, _P, C.c_double]),
     "osb_frontend_set_drone_pose": (C.c_int, [_P, _P]),
+    "osb_frontend_set_depth_camera": (C.c_int, [_P, _P, _P, C.c_double, C.c_double]),
+    "osb_frontend_extract_depth": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
+    "osb_frontend_extract_depth_dev": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
+    "osb_frontend_process_depth": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
     "osb_pnp_ransac": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "osb_pnp_ransac_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "osb_pcm": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P]),

@@ -156,6 +156,29 @@ def image(seed: int, H: int = 480, W: int = 640, zero_bottom_quarter: bool = Fal
     return img
 
 
+def depth_image(seed: int, H: int = 480, W: int = 640, near: float = 0.3, far: float = 10.0) -> np.ndarray:
+    """Aligned 16-bit depth image in mm for a PINHOLE_DEPTH keyframe (loop_cam.cpp:231-302): a slanted plane inside
+    (near, far), with holes (0, no return), one patch beyond `far` and one below `near`, so that a keyframe's keypoints
+    fall on both valid and rejected depths."""
+    rng = np.random.default_rng(seed + 7000)
+    lo, hi = 1000.0 * near, 1000.0 * far
+    yy, xx = np.mgrid[0:H, 0:W]
+    a, b = rng.uniform(0.2, 0.8, 2)
+    plane = lo + (hi - lo) * (0.1 + 0.3 * a * xx / W + 0.5 * b * yy / H)          # stays within (near, far)
+    dep = np.round(plane).astype(np.uint16)
+
+    def patch():
+        h, w = max(1, H // 4), max(1, W // 4)
+        y0, x0 = int(rng.integers(0, H - h + 1)), int(rng.integers(0, W - w + 1))
+        return slice(y0, y0 + h), slice(x0, x0 + w)
+
+    dep[patch()] = np.uint16(min(65535, int(1.5 * hi)))                              # beyond DEPTH_FAR_THRES
+    dep[patch()] = np.uint16(0.5 * lo)                                               # below DEPTH_NEAR_THRES
+    dep[patch()] = 0                                                                 # a hole
+    dep[rng.uniform(size=(H, W)) < 0.1] = 0                                          # scattered missing returns
+    return dep
+
+
 def descriptor_db(n: int, dim: int = 4096, seed: int = 1) -> np.ndarray:
     """n unit-norm Gaussian rows, float32 (SURVEY.md section 8d C3)."""
     rng = np.random.default_rng(seed + 4000)
