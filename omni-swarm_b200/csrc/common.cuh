@@ -124,6 +124,22 @@ inline osb_status dmalloc(T** p, size_t n) {
   return OSB_OK;
 }
 
+// the device allocations of a handle: one cudaMalloc per buffer, every pointer remembered and freed together
+struct DeviceAllocs {
+  std::vector<void*> ptrs;
+  template <typename T>
+  osb_status alloc(T** p, size_t n) {        // n elements of T
+    OSB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
+    ptrs.push_back((void*)*p);
+    return OSB_OK;
+  }
+  void free_all() {
+    for (void* p : ptrs) cudaFree(p);
+    ptrs.clear();
+  }
+  ~DeviceAllocs() { free_all(); }
+};
+
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
