@@ -110,6 +110,24 @@ osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8
 osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
                              int channels, int stride, int generic, float out_scale, void* out_hi, void* out_lo,
                              void* stream);
+/* The same for the fp32 CUDA-core path (OSB_SP_CONV=ffma, and the layers both paths run in fp32); fp32 NHWC device
+ * operands, act 0 none / 1 ReLU / 2 ReLU6:
+ *  conv_ffma:       w [cout][cin][ks][ks] (cin a multiple of 8, ks 1 or 3), x [batch][H][W][cin] ->
+ *                   y [batch][H][W][out_cstride] (out_cstride a multiple of 8 in [cout, cout rounded up to 64]; the
+ *                   channels in [cout, out_cstride) are stored as 0).
+ *  conv_first_ffma: w [cout][1][3][3] (cout 32 or 64) on u8 images [batch][H][W] (scaled by 1/255), pad 1, stride 1 or 2
+ *                   -> y [batch][H/stride][W/stride][cout].
+ *  dwconv_ffma:     depthwise 3x3, w [C][1][3][3], pad 1, stride 1 or 2 -> y [batch][H/stride][W/stride][C].
+ *  maxpool:         2x2 max-pool, x [batch][H][W][C] (C a multiple of 4) -> y [batch][H/2][W/2][C]. */
+osb_status osb_conv_ffma_parity(const float* w, const float* bias, int cin, int cout, int ks, const float* x_dev,
+                                int batch, int height, int width, int act, int out_cstride, float* y_dev, void* stream);
+osb_status osb_conv_first_ffma_parity(const float* w, const float* bias, int cout, int stride, int act,
+                                      const uint8_t* images_dev, int batch, int height, int width, float* y_dev,
+                                      void* stream);
+osb_status osb_dwconv_ffma_parity(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
+                                  int channels, int stride, int act, float* y_dev, void* stream);
+osb_status osb_maxpool_parity(const float* x_dev, int batch, int height, int width, int channels, float* y_dev,
+                              void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * NetVLAD global descriptor -- replaces class MobileNetVLADTensorRT
@@ -124,6 +142,18 @@ osb_status osb_netvlad_create(osb_netvlad** out, const float* weights, size_t n_
 osb_status osb_netvlad_destroy(osb_netvlad* h);
 osb_status osb_netvlad_infer(osb_netvlad* h, const uint8_t* images, int batch, float* out);
 osb_status osb_netvlad_infer_dev(osb_netvlad* h, const uint8_t* images_dev, int batch, float* out_dev, void* stream);
+/* NetVLAD parity hooks (tests only): two parts of the network run by the host functions osb_netvlad_infer_dev calls,
+ * conventions as the convolution hooks above (host OIHW weights, device fp32 NHWC activations, one synchronise):
+ *  nv_block0: block 0 of the default path, depthwise 3x3 (dw_w [32][1][3][3]) + ReLU6 -> pointwise pw_w [64][32][1][1] +
+ *             ReLU6, x [batch][H][W][32] -> y [batch][H][W][64].
+ *  nv_head:   from the projected features x [batch][H][W][128]: mu [batch][128] (per-image mean), xn = (x - mu) / ||x - mu||
+ *             per location, logits [batch][H][W][32] of assign_w [32][128][1][1], their softmax `assign`, and the
+ *             4096-vector out [batch][32*128] (VLAD with centroids [32][128], intra- and global L2 normalisation). */
+osb_status osb_nv_block0_parity(const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_b,
+                                const float* x_dev, int batch, int height, int width, float* y_dev, void* stream);
+osb_status osb_nv_head_parity(const float* assign_w, const float* assign_b, const float* centroids, const float* x_dev,
+                              int batch, int height, int width, float* mu_dev, float* xn_dev, float* logits_dev,
+                              float* assign_dev, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Keyframe database -- replaces faiss::IndexFlatIP(4096) (swarm_loop/include/swarm_loop/loop_detector.h:27-29;

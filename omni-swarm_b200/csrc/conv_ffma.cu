@@ -137,6 +137,19 @@ void conv_layer_free(ConvLayer* L) {
   L->w = L->b = nullptr;
 }
 
+osb_status upload_f32(float** dst, const float* src, size_t n) {
+  OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
+  OSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
+  return OSB_OK;
+}
+
+osb_status upload_tap_major(float** dst, const float* w_oihw, int cout) {
+  std::vector<float> t(9 * (size_t)cout);
+  for (int o = 0; o < cout; ++o)
+    for (int k = 0; k < 9; ++k) t[(size_t)k * cout + o] = w_oihw[(size_t)o * 9 + k];
+  return upload_f32(dst, t.data(), t.size());
+}
+
 osb_status conv_forward(const ConvLayer& L, const float* x, float* y, int B, int H, int W, int out_cstride,
                         int act, cudaStream_t st) {
   OSB_REQUIRE(L.cin % CV_KC == 0 && out_cstride % 8 == 0 && out_cstride <= L.cout_pad && out_cstride >= L.cout,
@@ -296,3 +309,83 @@ osb_status dwconv3x3_forward(const float* w_tap_c, const float* bias, const floa
 }
 
 }  // namespace osb
+
+// --------------------------------------------------------------------------------------------------------------
+// parity hooks: one fp32 layer, run by the host functions above on caller-supplied operands (tests only)
+// --------------------------------------------------------------------------------------------------------------
+using namespace osb;
+
+extern "C" osb_status osb_conv_ffma_parity(const float* w, const float* bias, int cin, int cout, int ks,
+                                           const float* x_dev, int batch, int height, int width, int act,
+                                           int out_cstride, float* y_dev, void* stream) {
+  OSB_REQUIRE(w && bias && x_dev && y_dev, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && cin > 0 && cout > 0 && (ks == 1 || ks == 3) && act >= 0 &&
+              act <= 2, "bad geometry (ks 1 or 3, act 0..2)");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  ConvLayer L;
+  s = conv_layer_upload(&L, w, bias, cin, cout, ks);
+  if (s == OSB_OK) s = conv_forward(L, x_dev, y_dev, batch, height, width, out_cstride, act, st);
+  const cudaError_t e = cudaStreamSynchronize(st);         // the weights are freed below
+  conv_layer_free(&L);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_conv_first_ffma_parity(const float* w, const float* bias, int cout, int stride, int act,
+                                                 const uint8_t* images_dev, int batch, int height, int width,
+                                                 float* y_dev, void* stream) {
+  OSB_REQUIRE(w && bias && images_dev && y_dev, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (stride == 1 || stride == 2) && act >= 0 && act <= 2,
+              "bad geometry (stride 1 or 2, act 0..2)");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  float *wd = nullptr, *bd = nullptr, *lut = nullptr;
+  std::vector<float> l(256);
+  for (int v = 0; v < 256; ++v) l[v] = (float)v * (float)(1.0 / 255.0);
+  if (cout == 32 || cout == 64) {
+    s = upload_tap_major(&wd, w, cout);
+    if (s == OSB_OK) s = upload_f32(&bd, bias, cout);
+    if (s == OSB_OK) s = upload_f32(&lut, l.data(), 256);
+  }
+  if (s == OSB_OK) s = conv_first_forward(wd, bd, lut, images_dev, y_dev, batch, height, width, cout, stride, act, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(wd); cudaFree(bd); cudaFree(lut);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_dwconv_ffma_parity(const float* w, const float* bias, const float* x_dev, int batch,
+                                             int height, int width, int channels, int stride, int act, float* y_dev,
+                                             void* stream) {
+  OSB_REQUIRE(w && bias && x_dev && y_dev, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 4 == 0 && (stride == 1 || stride == 2) &&
+              act >= 0 && act <= 2, "bad geometry (channels a multiple of 4, stride 1 or 2, act 0..2)");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  float *wd = nullptr, *bd = nullptr;
+  s = upload_tap_major(&wd, w, channels);
+  if (s == OSB_OK) s = upload_f32(&bd, bias, channels);
+  if (s == OSB_OK) s = dwconv3x3_forward(wd, bd, x_dev, y_dev, batch, height, width, channels, stride, act, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  cudaFree(wd); cudaFree(bd);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_maxpool_parity(const float* x_dev, int batch, int height, int width, int channels,
+                                         float* y_dev, void* stream) {
+  OSB_REQUIRE(x_dev && y_dev, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 1 && width > 1 && channels > 0 && channels % 4 == 0,
+              "bad geometry (channels a multiple of 4)");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  s = maxpool2x2_forward(x_dev, y_dev, batch, height, width, channels, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}

@@ -711,23 +711,6 @@ osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const 
 // --------------------------------------------------------------------------------------------------------------
 using namespace osb;
 
-namespace {
-// [cout][taps] (OIHW with one input channel) -> [tap][cout], on the device
-osb_status upload_tap_major(float** dst, const float* w_oihw, int cout) {
-  std::vector<float> t(9 * (size_t)cout);
-  for (int o = 0; o < cout; ++o)
-    for (int k = 0; k < 9; ++k) t[(size_t)k * cout + o] = w_oihw[(size_t)o * 9 + k];
-  OSB_CUDA(cudaMalloc(dst, t.size() * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(*dst, t.data(), t.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return OSB_OK;
-}
-osb_status upload_f32(float** dst, const float* src, size_t n) {
-  OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
-  return OSB_OK;
-}
-}  // namespace
-
 extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
                                             const void* in_hi, const void* in_lo, int batch, int height, int width,
                                             float act_scale, int relu, int pool, int out_c, int out_cstride, int max_ctas,

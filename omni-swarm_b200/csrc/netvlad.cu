@@ -211,9 +211,51 @@ nv_block0_fused_kernel(const float* __restrict__ x, const float* __restrict__ dw
   }
 }
 
-static osb_status upload(float** dst, const float* src, size_t n) {
+static osb_status alloc(float** dst, size_t n) {
   OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
+  return OSB_OK;
+}
+
+static osb_status copy_dev(float* dst, const float* src, size_t n, cudaStream_t st) {
+  OSB_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return OSB_OK;
+}
+
+static osb_status nv_block0_prepare() {
+  OSB_CUDA(cudaFuncSetAttribute(nv_block0_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F0_SMEM));
+  return OSB_OK;
+}
+
+// block 0 of the tensor-core path: x fp32 [B][h][w][32] -> y fp32 [B][h][w][64]; dw_tap_c [9][32], pw_kc [32][64]
+static osb_status nv_block0_forward(const float* x, const float* dw_tap_c, const float* dw_b, const float* pw_kc,
+                                    const float* pw_b, float* y, int B, int h, int w, cudaStream_t st) {
+  dim3 grid(cdiv(w, F0_TW), cdiv(h, F0_TH), B);
+  OSB_LAUNCH(nv_block0_fused_kernel, grid, 256, F0_SMEM, st, x, dw_tap_c, dw_b, pw_kc, pw_b, y, h, w);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
+// The head, from the projected features x fp32 [B][h][w][D]: per-image mean mu [B][D]; x centred and L2-normalised per
+// location IN PLACE; soft-assignment a [B][h][w][K] (logits, then softmax in place; when logits_copy is not null the
+// logits are copied there first); VLAD partial sums part / psum, and the 4096-vector out [B][K*D].
+static osb_status nv_head_forward(const ConvLayer& assign, const float* centroids, float* x, int B, int h, int w,
+                                  float* mu, float* a, float* part, float* psum, float* out, cudaStream_t st,
+                                  float* logits_copy = nullptr) {
+  const int P = h * w;
+  const int64_t locs = (int64_t)B * P;
+  OSB_LAUNCH(nv_colmean_kernel, B, NV_D, 0, st, x, P, mu);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(nv_center_norm_kernel, (unsigned)cdiv64(locs * 32, 256), 256, 0, st, x, mu, P, locs);
+  OSB_CHECK_LAUNCH();
+  osb_status s = conv_forward(assign, x, a, B, h, w, NV_K, ACT_NONE, st);
+  if (s != OSB_OK) return s;
+  if (logits_copy && (s = copy_dev(logits_copy, a, (size_t)locs * NV_K, st)) != OSB_OK) return s;
+  OSB_LAUNCH(nv_softmax_kernel, (unsigned)cdiv64(locs, 128), 128, 0, st, a, locs);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(nv_vlad_partial_kernel, dim3(B, NV_SLICES), 1024, 0, st, x, a, P, part, psum);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(nv_vlad_final_kernel, B, 1024, 0, st, part, psum, centroids, out);
+  OSB_CHECK_LAUNCH();
   return OSB_OK;
 }
 
@@ -233,8 +275,8 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
     std::vector<float> w9(9 * 32);
     for (int o = 0; o < 32; ++o)
       for (int t = 0; t < 9; ++t) w9[t * 32 + o] = p[o * 9 + t];
-    if ((s = upload(&w0, w9.data(), 9 * 32)) != OSB_OK) return s;
-    if ((s = upload(&b0, p + 32 * 9, 32)) != OSB_OK) return s;
+    if ((s = upload_f32(&w0, w9.data(), 9 * 32)) != OSB_OK) return s;
+    if ((s = upload_f32(&b0, p + 32 * 9, 32)) != OSB_OK) return s;
     p += 32 * 9 + 32;
   }
   for (int i = 0; i < 7; ++i) {
@@ -243,18 +285,18 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
     std::vector<float> dw((size_t)9 * ci);
     for (int c = 0; c < ci; ++c)
       for (int t = 0; t < 9; ++t) dw[(size_t)t * ci + c] = p[(size_t)c * 9 + t];
-    if ((s = upload(&blk[i].dw, dw.data(), dw.size())) != OSB_OK) return s;
+    if ((s = upload_f32(&blk[i].dw, dw.data(), dw.size())) != OSB_OK) return s;
     p += (size_t)ci * 9;
-    if ((s = upload(&blk[i].dwb, p, ci)) != OSB_OK) return s;
+    if ((s = upload_f32(&blk[i].dwb, p, ci)) != OSB_OK) return s;
     p += ci;
     if ((s = conv_layer_upload(&blk[i].pw, p, p + (size_t)co * ci, ci, co, 1)) != OSB_OK) return s;
     if (i == 0) {                                  // block 0 fused kernel: pointwise weights as [k][oc]
       std::vector<float> kc((size_t)ci * co);
       for (int o = 0; o < co; ++o)
         for (int k = 0; k < ci; ++k) kc[(size_t)k * co + o] = p[(size_t)o * ci + k];
-      if ((s = upload(&pw0_kc, kc.data(), kc.size())) != OSB_OK) return s;
-      if ((s = upload(&pw0_b, p + (size_t)co * ci, co)) != OSB_OK) return s;
-      OSB_CUDA(cudaFuncSetAttribute(nv_block0_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F0_SMEM));
+      if ((s = upload_f32(&pw0_kc, kc.data(), kc.size())) != OSB_OK) return s;
+      if ((s = upload_f32(&pw0_b, p + (size_t)co * ci, co)) != OSB_OK) return s;
+      if ((s = nv_block0_prepare()) != OSB_OK) return s;
     }
     if (use_umma && i >= 1 && (s = umma_layer_upload(&upw[i], p, p + (size_t)co * ci, ci, co, 1, NV_W_SCALE)) != OSB_OK) return s;
     p += (size_t)co * ci + co;
@@ -264,14 +306,14 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
   p += (size_t)NV_D * 512 + NV_D;
   if ((s = conv_layer_upload(&assign, p, p + (size_t)NV_K * NV_D, NV_D, NV_K, 1)) != OSB_OK) return s;
   p += (size_t)NV_K * NV_D + NV_K;
-  if ((s = upload(&centroids, p, (size_t)NV_K * NV_D)) != OSB_OK) return s;
+  if ((s = upload_f32(&centroids, p, (size_t)NV_K * NV_D)) != OSB_OK) return s;
   {
     // engine input is the u8 image converted to float UNSCALED (mobilenetvlad_tensorrt.cpp:8-10); the stand-in
     // network's first op multiplies by 1/255 in f32.
     std::vector<float> l(256);
     const float sc = (float)(1.0 / 255.0);
     for (int v = 0; v < 256; ++v) l[v] = (float)v * sc;
-    if ((s = upload(&lut, l.data(), 256)) != OSB_OK) return s;
+    if ((s = upload_f32(&lut, l.data(), 256)) != OSB_OK) return s;
   }
   const size_t B = max_batch;
   const size_t act = B * (H / 2) * (W / 2) * 64;   // largest activation: block 0 output (64 ch at 1/2 res)
@@ -326,9 +368,7 @@ osb_status NetVLAD::infer_dev(const uint8_t* img_dev, int B, float* out_dev, cud
   float* cur = actA;                 // fp32 activations of the previous block
   for (int i = 0; i < 7; ++i) {
     if (use_umma && i == 0) {
-      dim3 grid(cdiv(w, F0_TW), cdiv(h, F0_TH), B);
-      OSB_LAUNCH(nv_block0_fused_kernel, grid, 256, F0_SMEM, st, cur, blk[0].dw, blk[0].dwb, pw0_kc, pw0_b, actB, h, w);
-      OSB_CHECK_LAUNCH();
+      RUN(nv_block0_forward(cur, blk[0].dw, blk[0].dwb, pw0_kc, pw0_b, actB, B, h, w, st));
       cur = actB;
     } else if (use_umma) {
       // depthwise (fp32 -> split planes) then pointwise on the tensor cores (planes -> fp32, or planes for the projection)
@@ -353,18 +393,7 @@ osb_status NetVLAD::infer_dev(const uint8_t* img_dev, int B, float* out_dev, cud
     RUN(umma_conv_forward(uproj, tmA[7], tmB[7], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actB, NV_D, NV_D, 1.f, 0, 0, st));
   else
     RUN(conv_forward(proj, actA, actB, B, h, w, NV_D, ACT_NONE, st));
-  const int64_t locs = (int64_t)B * h * w;
-  OSB_LAUNCH(nv_colmean_kernel, B, NV_D, 0, st, actB, h * w, d_mu);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(nv_center_norm_kernel, (unsigned)cdiv64(locs * 32, 256), 256, 0, st, actB, d_mu, h * w, locs);
-  OSB_CHECK_LAUNCH();
-  RUN(conv_forward(assign, actB, d_assign, B, h, w, NV_K, ACT_NONE, st));
-  OSB_LAUNCH(nv_softmax_kernel, (unsigned)cdiv64(locs, 128), 128, 0, st, d_assign, locs);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(nv_vlad_partial_kernel, dim3(B, NV_SLICES), 1024, 0, st, actB, d_assign, h * w, d_part, d_psum);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(nv_vlad_final_kernel, B, 1024, 0, st, d_part, d_psum, centroids, out_dev);
-  OSB_CHECK_LAUNCH();
+  RUN(nv_head_forward(assign, centroids, actB, B, h, w, d_mu, d_assign, d_part, d_psum, out_dev, st));
 #undef RUN
   return OSB_OK;
 }
@@ -420,4 +449,58 @@ extern "C" osb_status osb_netvlad_infer(osb_netvlad* h, const uint8_t* images, i
   OSB_CUDA(cudaMemcpyAsync(out, nv.d_out, (size_t)batch * NV_K * NV_D * sizeof(float), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
+}
+
+// --------------------------------------------------------------------------------------------------------------
+// parity hooks: block 0 and the head of the network, run by the host functions infer_dev calls (tests only)
+// --------------------------------------------------------------------------------------------------------------
+extern "C" osb_status osb_nv_block0_parity(const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_b,
+                                           const float* x_dev, int batch, int height, int width, float* y_dev,
+                                           void* stream) {
+  OSB_REQUIRE(dw_w && dw_b && pw_w && pw_b && x_dev && y_dev, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  std::vector<float> kc(F0_C * F0_OC);
+  for (int o = 0; o < F0_OC; ++o)
+    for (int k = 0; k < F0_C; ++k) kc[k * F0_OC + o] = pw_w[o * F0_C + k];
+  float *dwd = nullptr, *dbd = nullptr, *kcd = nullptr, *pbd = nullptr;
+  s = upload_tap_major(&dwd, dw_w, F0_C);
+  if (s == OSB_OK) s = upload_f32(&dbd, dw_b, F0_C);
+  if (s == OSB_OK) s = upload_f32(&kcd, kc.data(), kc.size());
+  if (s == OSB_OK) s = upload_f32(&pbd, pw_b, F0_OC);
+  if (s == OSB_OK) s = nv_block0_prepare();
+  if (s == OSB_OK) s = nv_block0_forward(x_dev, dwd, dbd, kcd, pbd, y_dev, batch, height, width, st);
+  const cudaError_t e = cudaStreamSynchronize(st);          // the weights are freed below
+  cudaFree(dwd); cudaFree(dbd); cudaFree(kcd); cudaFree(pbd);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
+}
+
+extern "C" osb_status osb_nv_head_parity(const float* assign_w, const float* assign_b, const float* centroids,
+                                         const float* x_dev, int batch, int height, int width, float* mu_dev,
+                                         float* xn_dev, float* logits_dev, float* assign_dev, float* out_dev,
+                                         void* stream) {
+  OSB_REQUIRE(assign_w && assign_b && centroids && x_dev && mu_dev && xn_dev && logits_dev && assign_dev && out_dev,
+              "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+  osb_status s = require_device();
+  if (s != OSB_OK) return s;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const size_t locs = (size_t)batch * height * width;
+  ConvLayer L;
+  float *cd = nullptr, *part = nullptr, *psum = nullptr;
+  s = conv_layer_upload(&L, assign_w, assign_b, NV_D, NV_K, 1);
+  if (s == OSB_OK) s = upload_f32(&cd, centroids, (size_t)NV_K * NV_D);
+  if (s == OSB_OK) s = alloc(&part, (size_t)batch * NV_SLICES * NV_K * NV_D);
+  if (s == OSB_OK) s = alloc(&psum, (size_t)batch * NV_SLICES * NV_K);
+  if (s == OSB_OK) s = copy_dev(xn_dev, x_dev, locs * NV_D, st);      // the head centres and normalises in place
+  if (s == OSB_OK)
+    s = nv_head_forward(L, cd, xn_dev, batch, height, width, mu_dev, assign_dev, part, psum, out_dev, st, logits_dev);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  conv_layer_free(&L);
+  cudaFree(cd); cudaFree(part); cudaFree(psum);
+  if (s == OSB_OK) OSB_CUDA(e);
+  return s;
 }

@@ -699,5 +699,94 @@ def dwconv_parity(w, bias, x, out_scale: float, *, stride: int = 1, generic: boo
     return hi, lo
 
 
+_GUARD = 64          # floats after an fp32 hook output, pre-filled with NaN like the output: a store past the end shows
+
+
+def _nan_out(shape, dev):
+    """a NaN-filled CUDA float32 tensor of `shape` followed by _GUARD NaN floats: (view, guard)"""
+    import torch
+    n = int(np.prod(shape))
+    buf = torch.full((n + _GUARD,), float("nan"), dtype=torch.float32, device=dev)
+    return buf[:n].view(shape), buf[n:]
+
+
+def _stream(dev):
+    import torch
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def conv_ffma_parity(w, bias, x, *, act: int = 0, out_cstride: int | None = None, guard: bool = False):
+    """One fp32 CUDA-core convolution (osb_conv_ffma_parity): w [cout,cin,ks,ks], bias [cout] float32 (numpy); x CUDA
+    float32 [B,H,W,cin] -> [B,H,W,out_cstride] float32, pre-filled with NaN (guard=True also returns the NaN-filled
+    floats behind it)."""
+    w, b = _f32(w), _f32(bias)
+    cout, cin, ks = w.shape[0], w.shape[1], w.shape[2]
+    B, H, W, c = x.shape
+    assert c == cin and x.is_contiguous()
+    out_cstride = cout if out_cstride is None else out_cstride
+    y, g = _nan_out((B, H, W, out_cstride), x.device)
+    _l.check(_l.load().osb_conv_ffma_parity(_l.ptr(w), _l.ptr(b), cin, cout, ks, C.c_void_p(x.data_ptr()), B, H, W,
+                                            int(act), out_cstride, C.c_void_p(y.data_ptr()), _stream(x.device)))
+    return (y, g) if guard else y
+
+
+def conv_first_ffma_parity(w, bias, images, *, stride: int, act: int):
+    """The fp32 first layer (osb_conv_first_ffma_parity): w [cout,1,3,3] (cout 32 or 64), images CUDA torch.uint8 [B,H,W]
+    -> [B,H/stride,W/stride,cout] float32."""
+    w, b = _f32(w), _f32(bias)
+    B, H, W = images.shape
+    cout = w.shape[0]
+    y, _ = _nan_out((B, H // stride, W // stride, cout), images.device)
+    _l.check(_l.load().osb_conv_first_ffma_parity(_l.ptr(w), _l.ptr(b), cout, int(stride), int(act),
+                                                  C.c_void_p(images.data_ptr()), B, H, W, C.c_void_p(y.data_ptr()),
+                                                  _stream(images.device)))
+    return y
+
+
+def dwconv_ffma_parity(w, bias, x, *, stride: int = 1, act: int = 2):
+    """fp32 depthwise 3x3 (osb_dwconv_ffma_parity): w [C,1,3,3], x CUDA float32 [B,H,W,C] -> [B,H/s,W/s,C] float32."""
+    w, b = _f32(w), _f32(bias)
+    B, H, W, Cn = x.shape
+    y, _ = _nan_out((B, H // stride, W // stride, Cn), x.device)
+    _l.check(_l.load().osb_dwconv_ffma_parity(_l.ptr(w), _l.ptr(b), C.c_void_p(x.data_ptr()), B, H, W, Cn, int(stride),
+                                              int(act), C.c_void_p(y.data_ptr()), _stream(x.device)))
+    return y
+
+
+def maxpool_parity(x):
+    """2x2 max-pool (osb_maxpool_parity): x CUDA float32 [B,H,W,C] -> [B,H/2,W/2,C] float32."""
+    B, H, W, Cn = x.shape
+    y, _ = _nan_out((B, H // 2, W // 2, Cn), x.device)
+    _l.check(_l.load().osb_maxpool_parity(C.c_void_p(x.data_ptr()), B, H, W, Cn, C.c_void_p(y.data_ptr()),
+                                          _stream(x.device)))
+    return y
+
+
+def nv_block0_parity(dw_w, dw_b, pw_w, pw_b, x):
+    """NetVLAD block 0 as the default path runs it, one fused kernel (osb_nv_block0_parity): dw_w [32,1,3,3], pw_w
+    [64,32,1,1]; x CUDA float32 [B,H,W,32] -> [B,H,W,64] float32."""
+    B, H, W, c = x.shape
+    assert c == 32 and x.is_contiguous()
+    y, _ = _nan_out((B, H, W, 64), x.device)
+    _l.check(_l.load().osb_nv_block0_parity(_l.ptr(_f32(dw_w)), _l.ptr(_f32(dw_b)), _l.ptr(_f32(pw_w)), _l.ptr(_f32(pw_b)),
+                                            C.c_void_p(x.data_ptr()), B, H, W, C.c_void_p(y.data_ptr()),
+                                            _stream(x.device)))
+    return y
+
+
+def nv_head_parity(assign_w, assign_b, centroids, x):
+    """The NetVLAD head (osb_nv_head_parity) on projected features x CUDA float32 [B,h,w,128] -> dict of CUDA float32
+    tensors: mu [B,128], xn [B,h,w,128] (centred, L2-normalised), logits and assign [B,h,w,32], out [B,4096]."""
+    B, h, w, c = x.shape
+    assert c == 128 and x.is_contiguous()
+    r = {"mu": _nan_out((B, 128), x.device)[0], "xn": _nan_out((B, h, w, 128), x.device)[0],
+         "logits": _nan_out((B, h, w, 32), x.device)[0], "assign": _nan_out((B, h, w, 32), x.device)[0],
+         "out": _nan_out((B, 4096), x.device)[0]}
+    _l.check(_l.load().osb_nv_head_parity(
+        _l.ptr(_f32(assign_w)), _l.ptr(_f32(assign_b)), _l.ptr(_f32(centroids)), C.c_void_p(x.data_ptr()), B, h, w,
+        *(C.c_void_p(r[k].data_ptr()) for k in ("mu", "xn", "logits", "assign", "out")), _stream(x.device)))
+    return r
+
+
 def launch_count() -> int:
     return int(_l.load().osb_launch_count())

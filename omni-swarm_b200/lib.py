@@ -120,6 +120,13 @@ _SIG = {
     "osb_netvlad_destroy": (C.c_int, [_P]),
     "osb_netvlad_infer": (C.c_int, [_P, _P, C.c_int, _P]),
     "osb_netvlad_infer_dev": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "osb_conv_ffma_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       _P, _P]),
+    "osb_conv_first_ffma_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "osb_dwconv_ffma_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "osb_maxpool_parity": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "osb_nv_block0_parity": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "osb_nv_head_parity": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "osb_db_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int64]),
     "osb_db_destroy": (C.c_int, [_P]),
     "osb_db_add": (C.c_int, [_P, C.c_int64, _P, C.POINTER(C.c_int64)]),
