@@ -1,9 +1,10 @@
-// abi.cu -- library-wide state of the C ABI (error text, version, launch accounting).
+// abi.cu -- library-wide state of the C ABI (error text, version, launch and resource accounting).
 #include "common.cuh"
 
 namespace osb {
 thread_local std::string g_last_error;
 std::atomic<long long> g_launches{0};
+std::atomic<long long> g_live_resources{0};
 std::atomic<int> g_sm_budget{0};
 }  // namespace osb
 
@@ -16,3 +17,4 @@ extern "C" int osb_device_count(void) {
 }
 extern "C" void osb_set_sm_budget(int n_sms) { osb::g_sm_budget.store(n_sms > 0 ? n_sms : 0); }
 extern "C" int64_t osb_launch_count(void) { return (int64_t)osb::g_launches.load(); }
+extern "C" int64_t osb_live_resources(void) { return (int64_t)osb::g_live_resources.load(); }

@@ -1,4 +1,5 @@
-// common.cuh -- shared plumbing of libomniswarm_b200 (error handling, launch accounting, small device helpers).
+// common.cuh -- shared plumbing of libomniswarm_b200 (error handling, launch accounting, resource ownership, small
+// device helpers).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,6 +7,7 @@
 #include <string.h>
 #include <algorithm>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -15,6 +17,7 @@ namespace osb {
 
 extern thread_local std::string g_last_error;
 extern std::atomic<long long> g_launches;
+extern std::atomic<long long> g_live_resources;    // held by every Resources of the process (osb_live_resources)
 
 inline void set_error(const char* where, const char* what) {
   g_last_error = std::string(where) + ": " + what;
@@ -47,6 +50,13 @@ inline void set_error(const char* where, const char* what) {
   } while (0)
 
 #define OSB_CHECK_LAUNCH() OSB_CUDA(cudaGetLastError())
+
+// returns the status of an internal call that failed (its error text is already set)
+#define OSB_TRY(expr)                                                                   \
+  do {                                                                                  \
+    const osb_status _s = (expr);                                                       \
+    if (_s != OSB_OK) return _s;                                                        \
+  } while (0)
 
 // Per-DEVICE (not per-process) state: a host process may open handles on several GPUs (one nodelet per drone on the
 // 8-GPU box), so "done once" flags and cached device attributes are keyed by the current device.
@@ -118,26 +128,81 @@ inline osb_status require_device() {
   return OSB_OK;
 }
 
-template <typename T>
-inline osb_status dmalloc(T** p, size_t n) {
-  OSB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-  return OSB_OK;
-}
-
-// the device allocations of a handle: one cudaMalloc per buffer, every pointer remembered and freed together
-struct DeviceAllocs {
-  std::vector<void*> ptrs;
+// The one owner of CUDA resources: every device buffer, pinned host buffer, stream and event of a handle (or of one call)
+// is acquired through it, and its destructor releases them all in reverse order of acquisition, on the device it was
+// created on.  An early return therefore frees whatever was acquired so far.  Not copyable: nothing is released twice.
+class Resources {
+ public:
+  Resources() = default;
+  Resources(const Resources&) = delete;
+  Resources& operator=(const Resources&) = delete;
+  ~Resources() {
+    if (items_.empty() && !sync_) return;
+    DeviceGuard dg(device_);
+    if (sync_) cudaStreamSynchronize(stream_);
+    for (size_t i = items_.size(); i-- > 0;) free_item(items_[i]);
+    g_live_resources.fetch_sub((long long)items_.size(), std::memory_order_relaxed);
+  }
   template <typename T>
-  osb_status alloc(T** p, size_t n) {        // n elements of T
+  osb_status alloc(T** p, size_t n) {        // n elements of T, one cudaMalloc
     OSB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-    ptrs.push_back((void*)*p);
+    hold(DEVICE, (void*)*p);
     return OSB_OK;
   }
-  void free_all() {
-    for (void* p : ptrs) cudaFree(p);
-    ptrs.clear();
+  template <typename T>
+  osb_status upload(T** p, const T* src, size_t n) {     // alloc + synchronous copy of n elements from the host
+    OSB_TRY(alloc(p, n));
+    OSB_CUDA(cudaMemcpy(*p, src, n * sizeof(T), cudaMemcpyHostToDevice));
+    return OSB_OK;
   }
-  ~DeviceAllocs() { free_all(); }
+  template <typename T>
+  osb_status host_alloc(T** p, size_t n, unsigned flags) {
+    OSB_CUDA(cudaHostAlloc((void**)p, n * sizeof(T), flags));
+    hold(PINNED, (void*)*p);
+    return OSB_OK;
+  }
+  osb_status stream(cudaStream_t* s, int priority = 0) {  // non-blocking
+    OSB_CUDA(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority));
+    hold(STREAM, *s);
+    return OSB_OK;
+  }
+  osb_status event(cudaEvent_t* e, unsigned flags = cudaEventDefault) {
+    OSB_CUDA(cudaEventCreateWithFlags(e, flags));
+    hold(EVENT, *e);
+    return OSB_OK;
+  }
+  // frees one device buffer before the owner goes (a buffer that is replaced by a larger one)
+  void release(void* p) {
+    for (size_t i = items_.size(); i-- > 0;)
+      if (items_[i].kind == DEVICE && items_[i].p == p) {
+        free_item(items_[i]);
+        items_.erase(items_.begin() + i);
+        g_live_resources.fetch_sub(1, std::memory_order_relaxed);
+        return;
+      }
+  }
+  // the destructor synchronises `st` before it releases anything: for operands of work launched on a caller's stream
+  void sync_before_release(cudaStream_t st) { stream_ = st; sync_ = true; }
+
+ private:
+  enum Kind { DEVICE, PINNED, STREAM, EVENT };
+  struct Item { Kind kind; void* p; };
+  std::vector<Item> items_;
+  int device_ = current_device();
+  bool sync_ = false;
+  cudaStream_t stream_ = nullptr;
+  void hold(Kind k, void* p) {
+    items_.push_back({k, p});
+    g_live_resources.fetch_add(1, std::memory_order_relaxed);
+  }
+  static void free_item(const Item& it) {
+    switch (it.kind) {
+      case DEVICE: cudaFree(it.p); break;
+      case PINNED: cudaFreeHost(it.p); break;
+      case STREAM: cudaStreamDestroy((cudaStream_t)it.p); break;
+      case EVENT: cudaEventDestroy((cudaEvent_t)it.p); break;
+    }
+  }
 };
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }

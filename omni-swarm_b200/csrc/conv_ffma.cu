@@ -115,7 +115,8 @@ conv_ffma_kernel(const float* __restrict__ x, const float* __restrict__ wp, cons
   }
 }
 
-osb_status conv_layer_upload(ConvLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks) {
+osb_status conv_layer_upload(Resources& res, ConvLayer* L, const float* w_oihw, const float* bias, int cin, int cout,
+                             int ks) {
   L->cin = cin; L->cout = cout; L->ks = ks;
   L->cout_pad = cdiv(cout, CV_TC) * CV_TC;
   const int taps = ks * ks;
@@ -125,29 +126,15 @@ osb_status conv_layer_upload(ConvLayer* L, const float* w_oihw, const float* bia
     for (int c = 0; c < cin; ++c)
       for (int t = 0; t < taps; ++t) wp[((size_t)t * cin + c) * L->cout_pad + o] = w_oihw[((size_t)o * cin + c) * taps + t];
   }
-  OSB_CUDA(cudaMalloc(&L->w, wp.size() * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&L->b, bp.size() * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(L->w, wp.data(), wp.size() * sizeof(float), cudaMemcpyHostToDevice));
-  OSB_CUDA(cudaMemcpy(L->b, bp.data(), bp.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return OSB_OK;
+  OSB_TRY(res.upload(&L->w, wp.data(), wp.size()));
+  return res.upload(&L->b, bp.data(), bp.size());
 }
 
-void conv_layer_free(ConvLayer* L) {
-  cudaFree(L->w); cudaFree(L->b);
-  L->w = L->b = nullptr;
-}
-
-osb_status upload_f32(float** dst, const float* src, size_t n) {
-  OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
-  return OSB_OK;
-}
-
-osb_status upload_tap_major(float** dst, const float* w_oihw, int cout) {
+osb_status upload_tap_major(Resources& res, float** dst, const float* w_oihw, int cout) {
   std::vector<float> t(9 * (size_t)cout);
   for (int o = 0; o < cout; ++o)
     for (int k = 0; k < 9; ++k) t[(size_t)k * cout + o] = w_oihw[(size_t)o * 9 + k];
-  return upload_f32(dst, t.data(), t.size());
+  return res.upload(dst, t.data(), t.size());
 }
 
 osb_status conv_forward(const ConvLayer& L, const float* x, float* y, int B, int H, int W, int out_cstride,
@@ -321,16 +308,15 @@ extern "C" osb_status osb_conv_ffma_parity(const float* w, const float* bias, in
   OSB_REQUIRE(w && bias && x_dev && y_dev, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && cin > 0 && cout > 0 && (ks == 1 || ks == 3) && act >= 0 &&
               act <= 2, "bad geometry (ks 1 or 3, act 0..2)");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   ConvLayer L;
-  s = conv_layer_upload(&L, w, bias, cin, cout, ks);
-  if (s == OSB_OK) s = conv_forward(L, x_dev, y_dev, batch, height, width, out_cstride, act, st);
-  const cudaError_t e = cudaStreamSynchronize(st);         // the weights are freed below
-  conv_layer_free(&L);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(conv_layer_upload(res, &L, w, bias, cin, cout, ks));
+  OSB_TRY(conv_forward(L, x_dev, y_dev, batch, height, width, out_cstride, act, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_conv_first_ffma_parity(const float* w, const float* bias, int cout, int stride, int act,
@@ -339,22 +325,21 @@ extern "C" osb_status osb_conv_first_ffma_parity(const float* w, const float* bi
   OSB_REQUIRE(w && bias && images_dev && y_dev, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (stride == 1 || stride == 2) && act >= 0 && act <= 2,
               "bad geometry (stride 1 or 2, act 0..2)");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   float *wd = nullptr, *bd = nullptr, *lut = nullptr;
   std::vector<float> l(256);
   for (int v = 0; v < 256; ++v) l[v] = (float)v * (float)(1.0 / 255.0);
   if (cout == 32 || cout == 64) {
-    s = upload_tap_major(&wd, w, cout);
-    if (s == OSB_OK) s = upload_f32(&bd, bias, cout);
-    if (s == OSB_OK) s = upload_f32(&lut, l.data(), 256);
+    OSB_TRY(upload_tap_major(res, &wd, w, cout));
+    OSB_TRY(res.upload(&bd, bias, cout));
+    OSB_TRY(res.upload(&lut, l.data(), 256));
   }
-  if (s == OSB_OK) s = conv_first_forward(wd, bd, lut, images_dev, y_dev, batch, height, width, cout, stride, act, st);
-  const cudaError_t e = cudaStreamSynchronize(st);
-  cudaFree(wd); cudaFree(bd); cudaFree(lut);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(conv_first_forward(wd, bd, lut, images_dev, y_dev, batch, height, width, cout, stride, act, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_dwconv_ffma_parity(const float* w, const float* bias, const float* x_dev, int batch,
@@ -363,17 +348,16 @@ extern "C" osb_status osb_dwconv_ffma_parity(const float* w, const float* bias, 
   OSB_REQUIRE(w && bias && x_dev && y_dev, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 4 == 0 && (stride == 1 || stride == 2) &&
               act >= 0 && act <= 2, "bad geometry (channels a multiple of 4, stride 1 or 2, act 0..2)");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   float *wd = nullptr, *bd = nullptr;
-  s = upload_tap_major(&wd, w, channels);
-  if (s == OSB_OK) s = upload_f32(&bd, bias, channels);
-  if (s == OSB_OK) s = dwconv3x3_forward(wd, bd, x_dev, y_dev, batch, height, width, channels, stride, act, st);
-  const cudaError_t e = cudaStreamSynchronize(st);
-  cudaFree(wd); cudaFree(bd);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(upload_tap_major(res, &wd, w, channels));
+  OSB_TRY(res.upload(&bd, bias, channels));
+  OSB_TRY(dwconv3x3_forward(wd, bd, x_dev, y_dev, batch, height, width, channels, stride, act, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_maxpool_parity(const float* x_dev, int batch, int height, int width, int channels,

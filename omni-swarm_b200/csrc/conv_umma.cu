@@ -449,8 +449,8 @@ osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t*
   return OSB_OK;
 }
 
-osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks,
-                             float w_scale) {
+osb_status umma_layer_upload(Resources& res, UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout,
+                             int ks, float w_scale) {
   L->cin = cin; L->cout = cout; L->ks = ks; L->taps = ks * ks; L->w_scale = w_scale;
   L->n_pad = (cout <= 64) ? 64 : (cout <= 80) ? 80 : (cout <= 128) ? 128 : (cout <= 256) ? 256 : 512;
   OSB_REQUIRE(cin % UM_KC == 0 && cout <= 512, "tensor-core conv: Cin must be a multiple of 64 and Cout <= 512");
@@ -476,29 +476,20 @@ osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bia
         lo[idx] = __float2half_rn(s - __half2float(h));
       }
   }
-  OSB_CUDA(cudaMalloc(&L->w_hi, n * sizeof(__half)));
-  OSB_CUDA(cudaMalloc(&L->w_lo, n * sizeof(__half)));
-  OSB_CUDA(cudaMalloc(&L->bias, L->n_pad * sizeof(float)));
-  OSB_CUDA(cudaMemcpy(L->w_hi, hi.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
-  OSB_CUDA(cudaMemcpy(L->w_lo, lo.data(), n * sizeof(__half), cudaMemcpyHostToDevice));
-  OSB_CUDA(cudaMemcpy(L->bias, bp.data(), L->n_pad * sizeof(float), cudaMemcpyHostToDevice));
+  OSB_TRY(res.upload(&L->w_hi, hi.data(), n));
+  OSB_TRY(res.upload(&L->w_lo, lo.data(), n));
+  OSB_TRY(res.upload(&L->bias, bp.data(), L->n_pad));
   const uint64_t dims[3] = {(uint64_t)cin, (uint64_t)L->n_pad, (uint64_t)L->taps};
   const uint64_t strides[2] = {(uint64_t)cin * 2, (uint64_t)cin * L->n_pad * 2};
   const uint32_t box[3] = {UM_KC, (uint32_t)std::min(L->n_pad, 256), 1};
-  osb_status s;
-  if ((s = umma_make_tmap(&L->tm_hi, L->w_hi, 3, dims, strides, box)) != OSB_OK) return s;
-  if ((s = umma_make_tmap(&L->tm_lo, L->w_lo, 3, dims, strides, box)) != OSB_OK) return s;
+  OSB_TRY(umma_make_tmap(&L->tm_hi, L->w_hi, 3, dims, strides, box));
+  OSB_TRY(umma_make_tmap(&L->tm_lo, L->w_lo, 3, dims, strides, box));
   if (L->n_pad >= 256) {                       // 128-row boxes: the layer as n_pad / 128 work items per tile
     const uint32_t box128[3] = {UM_KC, 128, 1};
-    if ((s = umma_make_tmap(&L->tm_hi128, L->w_hi, 3, dims, strides, box128)) != OSB_OK) return s;
-    if ((s = umma_make_tmap(&L->tm_lo128, L->w_lo, 3, dims, strides, box128)) != OSB_OK) return s;
+    OSB_TRY(umma_make_tmap(&L->tm_hi128, L->w_hi, 3, dims, strides, box128));
+    OSB_TRY(umma_make_tmap(&L->tm_lo128, L->w_lo, 3, dims, strides, box128));
   }
   return OSB_OK;
-}
-
-void umma_layer_free(UmmaLayer* L) {
-  cudaFree(L->w_hi); cudaFree(L->w_lo); cudaFree(L->bias);
-  L->w_hi = L->w_lo = nullptr; L->bias = nullptr;
 }
 
 osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half* p_lo, int B, int H, int W, int C,
@@ -720,24 +711,22 @@ extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, i
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (ks == 1 || ks == 3), "bad geometry");
   OSB_REQUIRE(relu >= 0 && relu <= 2 && mode >= 0 && mode <= 2, "relu must be 0..2, mode 0 (fp32), 1 (planes) or 2 (softmax)");
   OSB_REQUIRE(mode == 1 ? (out_hi && out_lo) : (out_f32 != nullptr), "null output");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   UmmaLayer L;
   CUtensorMap a_hi, a_lo;
-  s = umma_layer_upload(&L, w, bias, cin, cout, ks, w_scale);
-  if (s == OSB_OK)
-    s = umma_act_maps(&a_hi, &a_lo, (__half*)in_hi, (__half*)in_lo, batch, height, width, cin, ks);
-  if (s == OSB_OK && mode == 2)
-    s = umma_conv_softmax_forward(L, a_hi, a_lo, batch, height, width, act_scale, out_f32, st, max_ctas);
-  else if (s == OSB_OK)
-    s = umma_conv_forward(L, a_hi, a_lo, batch, height, width, act_scale, mode == 1 ? (__half*)out_hi : nullptr,
-                          mode == 1 ? (__half*)out_lo : nullptr, mode == 0 ? out_f32 : nullptr, out_c, out_cstride,
-                          out_scale, relu, pool, st, max_ctas);
-  const cudaError_t e = cudaStreamSynchronize(st);         // the weights are freed below
-  umma_layer_free(&L);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(umma_layer_upload(res, &L, w, bias, cin, cout, ks, w_scale));
+  OSB_TRY(umma_act_maps(&a_hi, &a_lo, (__half*)in_hi, (__half*)in_lo, batch, height, width, cin, ks));
+  if (mode == 2)
+    OSB_TRY(umma_conv_softmax_forward(L, a_hi, a_lo, batch, height, width, act_scale, out_f32, st, max_ctas));
+  else
+    OSB_TRY(umma_conv_forward(L, a_hi, a_lo, batch, height, width, act_scale, mode == 1 ? (__half*)out_hi : nullptr,
+                              mode == 1 ? (__half*)out_lo : nullptr, mode == 0 ? out_f32 : nullptr, out_c, out_cstride,
+                              out_scale, relu, pool, st, max_ctas));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch,
@@ -745,21 +734,19 @@ extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, 
                                             void* stream) {
   OSB_REQUIRE(w1a && b1a && images_dev && out_hi && out_lo, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   float *wd = nullptr, *bd = nullptr, *lut = nullptr;
   std::vector<float> l(256);
   for (int v = 0; v < 256; ++v) l[v] = (float)v * (float)(1.0 / 255.0);
-  s = upload_tap_major(&wd, w1a, 64);
-  if (s == OSB_OK) s = upload_f32(&bd, b1a, 64);
-  if (s == OSB_OK) s = upload_f32(&lut, l.data(), 256);
-  if (s == OSB_OK)
-    s = umma_first_forward(wd, bd, lut, images_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, act_scale, st);
-  const cudaError_t e = cudaStreamSynchronize(st);
-  cudaFree(wd); cudaFree(bd); cudaFree(lut);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(upload_tap_major(res, &wd, w1a, 64));
+  OSB_TRY(res.upload(&bd, b1a, 64));
+  OSB_TRY(res.upload(&lut, l.data(), 256));
+  OSB_TRY(umma_first_forward(wd, bd, lut, images_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, act_scale, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
@@ -768,17 +755,15 @@ extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const
   OSB_REQUIRE(w && bias && x_dev && out_hi && out_lo, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0 && (stride == 1 || stride == 2),
               "bad geometry (channels must be a multiple of 8, stride 1 or 2)");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   float *wd = nullptr, *bd = nullptr;
-  s = upload_tap_major(&wd, w, channels);
-  if (s == OSB_OK) s = upload_f32(&bd, bias, channels);
-  if (s == OSB_OK)
-    s = umma_dwconv_forward(wd, bd, x_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, channels, stride,
-                            out_scale, st, !generic);
-  const cudaError_t e = cudaStreamSynchronize(st);
-  cudaFree(wd); cudaFree(bd);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(upload_tap_major(res, &wd, w, channels));
+  OSB_TRY(res.upload(&bd, bias, channels));
+  OSB_TRY(umma_dwconv_forward(wd, bd, x_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, channels, stride,
+                              out_scale, st, !generic));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }

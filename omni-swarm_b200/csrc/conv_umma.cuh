@@ -21,9 +21,9 @@ struct UmmaLayer {
   CUtensorMap tm_hi128, tm_lo128;     // same planes with 128-row boxes (n_pad >= 256 only)
 };
 
-osb_status umma_layer_upload(UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks,
-                             float w_scale);
-void umma_layer_free(UmmaLayer* L);
+// the weight planes and bias belong to `res`
+osb_status umma_layer_upload(Resources& res, UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout,
+                             int ks, float w_scale);
 // TMA descriptors of an activation tensor stored as two fp16 NHWC planes [B][H][W][C]
 osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half* p_lo, int B, int H, int W, int C,
                          int ks);

@@ -198,10 +198,12 @@ extern "C" osb_status osb_homography_ransac_dev(const float* src_dev, const floa
   cudaStream_t st = (cudaStream_t)stream;
   unsigned int* scratch = nullptr;
   OSB_CUDA(cudaMallocAsync(&scratch, 2 * (size_t)n_pairs * sizeof(unsigned int), st));
-  OSB_CUDA(cudaMemsetAsync(scratch, 0, 2 * (size_t)n_pairs * sizeof(unsigned int), st));
-  s = homography_ransac_device(src_dev, dst_dev, n_dev, n_pairs, max_n, thresh, seed, mask_dev, n_inliers_dev, winner_dev, st,
-                               scratch);
+  const cudaError_t e = cudaMemsetAsync(scratch, 0, 2 * (size_t)n_pairs * sizeof(unsigned int), st);
+  if (e == cudaSuccess)
+    s = homography_ransac_device(src_dev, dst_dev, n_dev, n_pairs, max_n, thresh, seed, mask_dev, n_inliers_dev, winner_dev,
+                                 st, scratch);
   cudaFreeAsync(scratch, st);
+  OSB_CUDA(e);
   return s;
 }
 
@@ -210,30 +212,24 @@ extern "C" osb_status osb_homography_ransac(const float* src, const float* dst, 
                                             float thresh, uint32_t seed, uint8_t* mask, int32_t* n_inliers,
                                             int32_t* winner) {
   OSB_REQUIRE(src && dst && n && mask && n_inliers && n_pairs > 0 && max_n > 0, "bad argument");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const size_t pts = (size_t)n_pairs * max_n;
+  Resources res;
   float *d_src = nullptr, *d_dst = nullptr;
   unsigned int* d_scratch = nullptr;
   int32_t *d_n = nullptr, *d_inl = nullptr, *d_win = nullptr;
   uint8_t* d_mask = nullptr;
-  OSB_CUDA(cudaMalloc(&d_src, pts * 2 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_dst, pts * 2 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_n, n_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&d_inl, n_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&d_win, n_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&d_mask, pts));
-  OSB_CUDA(cudaMalloc(&d_scratch, 2 * (size_t)n_pairs * sizeof(unsigned int)));
+  OSB_TRY(res.upload(&d_src, src, pts * 2));
+  OSB_TRY(res.upload(&d_dst, dst, pts * 2));
+  OSB_TRY(res.upload(&d_n, n, n_pairs));
+  OSB_TRY(res.alloc(&d_inl, n_pairs));
+  OSB_TRY(res.alloc(&d_win, n_pairs));
+  OSB_TRY(res.alloc(&d_mask, pts));
+  OSB_TRY(res.alloc(&d_scratch, 2 * (size_t)n_pairs));
   OSB_CUDA(cudaMemset(d_scratch, 0, 2 * (size_t)n_pairs * sizeof(unsigned int)));
-  OSB_CUDA(cudaMemcpy(d_src, src, pts * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  OSB_CUDA(cudaMemcpy(d_dst, dst, pts * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  OSB_CUDA(cudaMemcpy(d_n, n, n_pairs * sizeof(int32_t), cudaMemcpyHostToDevice));
-  s = homography_ransac_device(d_src, d_dst, d_n, n_pairs, max_n, thresh, seed, d_mask, d_inl, d_win, nullptr, d_scratch);
-  if (s == OSB_OK) {
-    OSB_CUDA(cudaMemcpy(mask, d_mask, pts, cudaMemcpyDeviceToHost));
-    OSB_CUDA(cudaMemcpy(n_inliers, d_inl, n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    if (winner) OSB_CUDA(cudaMemcpy(winner, d_win, n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  }
-  cudaFree(d_src); cudaFree(d_dst); cudaFree(d_n); cudaFree(d_inl); cudaFree(d_win); cudaFree(d_mask); cudaFree(d_scratch);
-  return s;
+  OSB_TRY(homography_ransac_device(d_src, d_dst, d_n, n_pairs, max_n, thresh, seed, d_mask, d_inl, d_win, nullptr, d_scratch));
+  OSB_CUDA(cudaMemcpy(mask, d_mask, pts, cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(n_inliers, d_inl, n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (winner) OSB_CUDA(cudaMemcpy(winner, d_win, n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return OSB_OK;
 }

@@ -1097,6 +1097,7 @@ static size_t trial_layout(SolverDev& P, char* base, size_t n, size_t m, const S
 }
 
 struct osb_solver {
+  Resources res;
   int max_nodes = 0, max_factors = 0;
   bool cluster_ok = false;
   cudaStream_t stream = nullptr;
@@ -1155,14 +1156,13 @@ extern "C" void osb_solve_default_options(osb_solve_options* o) {
 
 extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max_factors) {
   OSB_REQUIRE(out != nullptr && max_nodes > 0 && max_factors > 0, "bad sizes");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_solver* h = new osb_solver();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_solver> h(new osb_solver());
   h->max_nodes = max_nodes; h->max_factors = max_factors;
   const size_t n = max_nodes, m = max_factors;
-  OSB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  OSB_CUDA(cudaEventCreate(&h->ev0));
-  OSB_CUDA(cudaEventCreate(&h->ev1));
+  OSB_TRY(h->res.stream(&h->stream));
+  OSB_TRY(h->res.event(&h->ev0));
+  OSB_TRY(h->res.event(&h->ev1));
   h->cluster_ok = true;
   for (const void* k : {(const void*)graph_solve_kernel<float, false>, (const void*)graph_solve_kernel<double, false>,
                         (const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>}) {
@@ -1170,46 +1170,37 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
     h->cluster_ok = h->cluster_ok && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
   }
   cudaGetLastError();
-  OSB_CUDA(cudaMalloc(&h->d_fixed, n));
-  OSB_CUDA(cudaMalloc(&h->d_huber, m));
-  OSB_CUDA(cudaMalloc(&h->d_type, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_ia, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_ib, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_slot_a, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_slot_b, m * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_ptr, (n + 1) * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_payload, m * OSB_PAYLOAD_LEN * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_link, n));
-  OSB_CUDA(cudaMalloc(&h->d_es_ptr, (n + 1) * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_es_slot, m * sizeof(int32_t)));
+  OSB_TRY(h->res.alloc(&h->d_fixed, n));
+  OSB_TRY(h->res.alloc(&h->d_huber, m));
+  OSB_TRY(h->res.alloc(&h->d_type, m));
+  OSB_TRY(h->res.alloc(&h->d_ia, m));
+  OSB_TRY(h->res.alloc(&h->d_ib, m));
+  OSB_TRY(h->res.alloc(&h->d_slot_a, m));
+  OSB_TRY(h->res.alloc(&h->d_slot_b, m));
+  OSB_TRY(h->res.alloc(&h->d_ptr, n + 1));
+  OSB_TRY(h->res.alloc(&h->d_payload, m * OSB_PAYLOAD_LEN));
+  OSB_TRY(h->res.alloc(&h->d_link, n));
+  OSB_TRY(h->res.alloc(&h->d_es_ptr, n + 1));
+  OSB_TRY(h->res.alloc(&h->d_es_slot, m));
   // one trial of the worst shape: fp64 Jacobians in global memory, partials for a cooperative grid of every SM
   SolveShape worst = {};
   worst.ctas = num_sms();
   SolverDev unbound = {};
   h->arena_bytes = trial_layout(unbound, nullptr, n, m, worst);
-  OSB_CUDA(cudaMalloc(&h->d_arena, h->arena_bytes));
-  OSB_CUDA(cudaMalloc(&h->d_order, n * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_mask, n));
-  OSB_CUDA(cudaMalloc(&h->d_res, sizeof(SolveResults) + 4 * n * sizeof(double)));
-  OSB_CUDA(cudaHostAlloc((void**)&h->h_res, sizeof(SolveResults) + 4 * n * sizeof(double), cudaHostAllocDefault));
-  OSB_CUDA(cudaMalloc(&h->d_lin, (4 * n + 36 * m) * sizeof(double)));
-  OSB_CUDA(cudaMalloc(&h->d_dbg, (8 + 128) * sizeof(long long)));
+  OSB_TRY(h->res.alloc(&h->d_arena, h->arena_bytes));
+  OSB_TRY(h->res.alloc(&h->d_order, n));
+  OSB_TRY(h->res.alloc(&h->d_mask, n));
+  OSB_TRY(h->res.alloc((char**)&h->d_res, sizeof(SolveResults) + 4 * n * sizeof(double)));
+  OSB_TRY(h->res.host_alloc((char**)&h->h_res, sizeof(SolveResults) + 4 * n * sizeof(double), cudaHostAllocDefault));
+  OSB_TRY(h->res.alloc(&h->d_lin, 4 * n + 36 * m));
+  OSB_TRY(h->res.alloc(&h->d_dbg, 8 + 128));
   OSB_CUDA(cudaMemset(h->d_dbg, 0, (8 + 128) * sizeof(long long)));
   h->device = current_device();
-  *out = h;
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_solver_destroy(osb_solver* h) {
-  if (!h) return OSB_OK;
-  cudaFree(h->d_fixed); cudaFree(h->d_huber); cudaFree(h->d_type); cudaFree(h->d_ia); cudaFree(h->d_ib);
-  cudaFree(h->d_slot_a); cudaFree(h->d_slot_b); cudaFree(h->d_ptr); cudaFree(h->d_payload);
-  cudaFree(h->d_link); cudaFree(h->d_es_ptr); cudaFree(h->d_es_slot);
-  cudaFree(h->d_arena); cudaFree(h->d_order); cudaFree(h->d_mask); cudaFree(h->d_res); cudaFree(h->d_lin); cudaFree(h->d_dbg);
-  if (h->h_res) cudaFreeHost(h->h_res);
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return OSB_OK;
 }
@@ -1480,8 +1471,8 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
   const size_t tstride = trial_layout(P, nullptr, n, n_factors, shape);
   if (K * tstride > h->arena_bytes) {     // multistart only; a failed allocation leaves the old arena in place
     char* grown = nullptr;
-    OSB_CUDA(cudaMalloc(&grown, K * tstride));
-    cudaFree(h->d_arena);
+    OSB_TRY(h->res.alloc(&grown, K * tstride));
+    h->res.release(h->d_arena);
     h->d_arena = grown;
     h->arena_bytes = K * tstride;
   }

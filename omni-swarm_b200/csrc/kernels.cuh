@@ -26,11 +26,10 @@ struct ConvLayer {
   float* w = nullptr;     // device
   float* b = nullptr;     // device
 };
-osb_status conv_layer_upload(ConvLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks);
-void conv_layer_free(ConvLayer* L);
-// host -> new device buffer: n floats as they are, or 3x3 one-input-channel weights [cout][9] (OIHW) as [9][cout]
-osb_status upload_f32(float** dst, const float* src, size_t n);
-osb_status upload_tap_major(float** dst, const float* w_oihw, int cout);
+// the weight buffers belong to `res`
+osb_status conv_layer_upload(Resources& res, ConvLayer* L, const float* w_oihw, const float* bias, int cin, int cout, int ks);
+// 3x3 one-input-channel weights [cout][9] (OIHW) -> new device buffer of `res` as [9][cout]
+osb_status upload_tap_major(Resources& res, float** dst, const float* w_oihw, int cout);
 
 // y[B][H][W][out_cstride] = act(conv_ks(x[B][H][W][Cin]) + b)   (NHWC, stride 1, "same" padding)
 osb_status conv_forward(const ConvLayer& L, const float* x, float* y, int B, int H, int W, int out_cstride,

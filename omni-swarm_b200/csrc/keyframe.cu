@@ -358,7 +358,7 @@ struct osb_frontend {
   cudaStream_t stream = nullptr;
   SuperPoint sp;
   NetVLAD nv;
-  DeviceAllocs mem;              // every device buffer of the handle
+  Resources res;                 // every buffer, stream and event of the handle (sp and nv own theirs)
   DbStore db[2];                 // 0 local, 1 remote
   uint8_t* d_img = nullptr;      // [2*n_dirs][H][W]
   // stereo matcher state
@@ -406,40 +406,37 @@ struct osb_frontend {
 
 static inline void fe_mark(osb_frontend* h, int i, cudaStream_t st) {
   if (!h->profiling) return;
-  if (!h->ev[i]) cudaEventCreate(&h->ev[i]);
+  if (!h->ev[i]) h->res.event(&h->ev[i]);
   cudaEventRecord(h->ev[i], st);
   h->ev_valid[i] = true;
 }
 
-static osb_status dbstore_alloc(DeviceAllocs& m, DbStore& s, int64_t cap, int max_num) {
+static osb_status dbstore_alloc(Resources& m, DbStore& s, int64_t cap, int max_num) {
   s.cap = cap; s.upper = 0;
   DbView& v = s.v;
   const size_t c = (size_t)cap, cn = c * max_num;
-  osb_status st;
-#define DB_TRY(x) do { if ((st = (x)) != OSB_OK) return st; } while (0)
-  DB_TRY(m.alloc(&v.dev, 1));
+  OSB_TRY(m.alloc(&v.dev, 1));
   OSB_CUDA(cudaMemset(v.dev, 0, sizeof(DbDev)));
-  DB_TRY(m.alloc(&v.rows, c * OSB_DEEP_DESC_SIZE));
-  DB_TRY(m.alloc(&v.ldesc, cn * OSB_FEATURE_DESC_SIZE));
-  DB_TRY(m.alloc(&v.kpts, cn * 2));
-  DB_TRY(m.alloc(&v.lflag, cn));
+  OSB_TRY(m.alloc(&v.rows, c * OSB_DEEP_DESC_SIZE));
+  OSB_TRY(m.alloc(&v.ldesc, cn * OSB_FEATURE_DESC_SIZE));
+  OSB_TRY(m.alloc(&v.kpts, cn * 2));
+  OSB_TRY(m.alloc(&v.lflag, cn));
   OSB_CUDA(cudaMemset(v.kpts, 0, cn * 2 * sizeof(float)));
   OSB_CUDA(cudaMemset(v.lflag, 1, cn * sizeof(int32_t)));   // rows loaded without geometry: every landmark flagged (non-zero)
-  DB_TRY(m.alloc(&v.nk, c));
-  DB_TRY(m.alloc(&v.row_frame, c));
-  DB_TRY(m.alloc(&v.row_dir, c));
-  DB_TRY(m.alloc(&v.frame_rows, c * OSB_MAX_DIRS));
-  DB_TRY(m.alloc(&v.frame_msg, c));
-  DB_TRY(m.alloc(&v.frame_drone, c));
+  OSB_TRY(m.alloc(&v.nk, c));
+  OSB_TRY(m.alloc(&v.row_frame, c));
+  OSB_TRY(m.alloc(&v.row_dir, c));
+  OSB_TRY(m.alloc(&v.frame_rows, c * OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&v.frame_msg, c));
+  OSB_TRY(m.alloc(&v.frame_drone, c));
   int64_t chunk;
   const int gmax = db_scan_grid(cap, &chunk);
-  DB_TRY(m.alloc(&s.part_scores, (size_t)8 * gmax * FE_KMAX));
-  DB_TRY(m.alloc(&s.part_ids, (size_t)8 * gmax * FE_KMAX));
-  DB_TRY(m.alloc(&s.done, 1));
+  OSB_TRY(m.alloc(&s.part_scores, (size_t)8 * gmax * FE_KMAX));
+  OSB_TRY(m.alloc(&s.part_ids, (size_t)8 * gmax * FE_KMAX));
+  OSB_TRY(m.alloc(&s.done, 1));
   OSB_CUDA(cudaMemset(s.done, 0, sizeof(unsigned int)));
-  DB_TRY(m.alloc(&v.top_scores, FE_KMAX));
-  DB_TRY(m.alloc(&v.top_ids, FE_KMAX));
-#undef DB_TRY
+  OSB_TRY(m.alloc(&v.top_scores, FE_KMAX));
+  OSB_TRY(m.alloc(&v.top_ids, FE_KMAX));
   OSB_CUDA(cudaMemset(v.top_ids, 0xFF, FE_KMAX * sizeof(int64_t)));     // "no result" (-1) until the first scan of this store
   return OSB_OK;
 }
@@ -455,82 +452,66 @@ extern "C" osb_status osb_frontend_create(osb_frontend** out, const osb_frontend
   OSB_REQUIRE(cfg->query_dir >= 0 && cfg->query_dir < cfg->n_dirs, "query_dir out of range");
   OSB_REQUIRE(cfg->db_capacity > 0 && cfg->db_capacity < (1 << 30), "bad db_capacity");
   OSB_REQUIRE(cfg->match_index_dist >= 1 && 5 + cfg->match_index_dist <= FE_KMAX, "bad match_index_dist");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_frontend* h = new osb_frontend();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_frontend> h(new osb_frontend());
   h->cfg = *cfg;
   h->device = current_device();
   const int nd = cfg->n_dirs, mn = cfg->max_num;
-#define FE_TRY(x) do { s = (x); if (s != OSB_OK) { osb_frontend_destroy(h); return s; } } while (0)
-#define FE_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { set_error("osb_frontend_create", cudaGetErrorString(e_)); osb_frontend_destroy(h); return OSB_ERR_CUDA; } } while (0)
-  FE_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  FE_CUDA(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
-  FE_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-  FE_CUDA(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
-  FE_CUDA(cudaEventCreateWithFlags(&h->ev_ingest, cudaEventDisableTiming));
-  FE_CUDA(cudaHostAlloc((void**)&h->h_cnt, 2 * sizeof(DbDev), cudaHostAllocDefault));
-  FE_CUDA(cudaHostAlloc((void**)&h->fb_host, sizeof(FeFeedback), cudaHostAllocMapped));
+  Resources& m = h->res;
+  OSB_TRY(m.stream(&h->stream));
+  OSB_TRY(m.stream(&h->stream2));
+  OSB_TRY(m.event(&h->ev_fork, cudaEventDisableTiming));
+  OSB_TRY(m.event(&h->ev_join, cudaEventDisableTiming));
+  OSB_TRY(m.event(&h->ev_ingest, cudaEventDisableTiming));
+  OSB_TRY(m.host_alloc(&h->h_cnt, 2, cudaHostAllocDefault));
+  OSB_TRY(m.host_alloc(&h->fb_host, 1, cudaHostAllocMapped));
   memset((void*)h->fb_host, 0, sizeof(FeFeedback));
-  FE_CUDA(cudaHostGetDevicePointer((void**)&h->fb_dev, (void*)h->fb_host, 0));
-  FE_TRY(h->sp.init(sp_weights, n_sp_weights, cfg->width, cfg->height, cfg->sp_thres, mn, pca_comp, pca_mean, 2 * nd));
+  OSB_CUDA(cudaHostGetDevicePointer((void**)&h->fb_dev, (void*)h->fb_host, 0));
+  OSB_TRY(h->sp.init(sp_weights, n_sp_weights, cfg->width, cfg->height, cfg->sp_thres, mn, pca_comp, pca_mean, 2 * nd));
   h->sp.ks.write_surv = false;       // the survivor plane is only a parity hook of the standalone SuperPoint handle
-  FE_TRY(h->nv.init(nv_weights, n_nv_weights, cfg->width, cfg->height, nd));
-  FE_TRY(dbstore_alloc(h->mem, h->db[0], cfg->db_capacity, mn));
-  FE_TRY(dbstore_alloc(h->mem, h->db[1], cfg->db_capacity, mn));
+  OSB_TRY(h->nv.init(nv_weights, n_nv_weights, cfg->width, cfg->height, nd));
+  OSB_TRY(dbstore_alloc(m, h->db[0], cfg->db_capacity, mn));
+  OSB_TRY(dbstore_alloc(m, h->db[1], cfg->db_capacity, mn));
   const size_t HW = (size_t)cfg->width * cfg->height, dk = (size_t)OSB_MAX_DIRS * OSB_MAX_KPTS, dm = (size_t)OSB_MAX_DIRS * mn;
-  DeviceAllocs& m = h->mem;
-  FE_TRY(m.alloc(&h->d_img, 2 * nd * HW));
-  FE_TRY(m.alloc(&h->d_st_pairs, 1));
-  FE_TRY(m.alloc(&h->d_q_pairs, 1));
-  FE_TRY(m.alloc(&h->d_st_qi, dm));
-  FE_TRY(m.alloc(&h->d_st_ti, dm));
-  FE_TRY(m.alloc(&h->d_st_map, dm));
-  FE_TRY(m.alloc(&h->d_st_n, OSB_MAX_DIRS));
-  FE_TRY(m.alloc(&h->d_st_dist, dm));
-  FE_TRY(m.alloc(&h->d_q_dist, dk));
-  FE_TRY(m.alloc(&h->d_g_src, dk * 2));
-  FE_TRY(m.alloc(&h->d_g_dst, dk * 2));
-  FE_TRY(m.alloc(&h->d_g_kept, dk));
-  FE_TRY(m.alloc(&h->d_g_nkept, OSB_MAX_DIRS));
-  FE_TRY(m.alloc(&h->d_g_ninl, OSB_MAX_DIRS));
-  FE_TRY(m.alloc(&h->d_g_win, OSB_MAX_DIRS));
-  FE_TRY(m.alloc(&h->d_g_mask, dk));
-  FE_TRY(m.alloc(&h->d_g_scratch, 2 * OSB_MAX_DIRS));
-  FE_CUDA(cudaMemset(h->d_g_scratch, 0, 2 * OSB_MAX_DIRS * sizeof(unsigned int)));
-  FE_TRY(m.alloc(&h->d_dist_scratch, dm * mn));
-  FE_TRY(m.alloc(&h->d_assign, (size_t)h->max_records * OSB_MAX_DIRS));
-  FE_TRY(m.alloc(&h->d_cam_pose, 2 * OSB_MAX_DIRS * 7));
-  FE_TRY(m.alloc(&h->d_l3d, dm * 3));
-  FE_TRY(m.alloc(&h->d_lflag_up, dm));
-  FE_TRY(m.alloc(&h->d_lflag_down, dm));
-  FE_TRY(m.alloc(&h->d_record, 1));
-  FE_TRY(m.alloc(&h->d_result, 1));
+  OSB_TRY(m.alloc(&h->d_img, 2 * nd * HW));
+  OSB_TRY(m.alloc(&h->d_st_pairs, 1));
+  OSB_TRY(m.alloc(&h->d_q_pairs, 1));
+  OSB_TRY(m.alloc(&h->d_st_qi, dm));
+  OSB_TRY(m.alloc(&h->d_st_ti, dm));
+  OSB_TRY(m.alloc(&h->d_st_map, dm));
+  OSB_TRY(m.alloc(&h->d_st_n, OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&h->d_st_dist, dm));
+  OSB_TRY(m.alloc(&h->d_q_dist, dk));
+  OSB_TRY(m.alloc(&h->d_g_src, dk * 2));
+  OSB_TRY(m.alloc(&h->d_g_dst, dk * 2));
+  OSB_TRY(m.alloc(&h->d_g_kept, dk));
+  OSB_TRY(m.alloc(&h->d_g_nkept, OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&h->d_g_ninl, OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&h->d_g_win, OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&h->d_g_mask, dk));
+  OSB_TRY(m.alloc(&h->d_g_scratch, 2 * OSB_MAX_DIRS));
+  OSB_CUDA(cudaMemset(h->d_g_scratch, 0, 2 * OSB_MAX_DIRS * sizeof(unsigned int)));
+  OSB_TRY(m.alloc(&h->d_dist_scratch, dm * mn));
+  OSB_TRY(m.alloc(&h->d_assign, (size_t)h->max_records * OSB_MAX_DIRS));
+  OSB_TRY(m.alloc(&h->d_cam_pose, 2 * OSB_MAX_DIRS * 7));
+  OSB_TRY(m.alloc(&h->d_l3d, dm * 3));
+  OSB_TRY(m.alloc(&h->d_lflag_up, dm));
+  OSB_TRY(m.alloc(&h->d_lflag_down, dm));
+  OSB_TRY(m.alloc(&h->d_record, 1));
+  OSB_TRY(m.alloc(&h->d_result, 1));
   {
     FePairs st{};                // the stereo match pairs up[d] with down[d]; its counts are sp.d_nk
     for (int d = 0; d < nd; ++d) {
       st.q[d] = h->sp.d_out + (size_t)d * mn * OSB_FEATURE_DESC_SIZE;
       st.t[d] = h->sp.d_out + (size_t)(nd + d) * mn * OSB_FEATURE_DESC_SIZE;
     }
-    FE_CUDA(cudaMemcpy(h->d_st_pairs, &st, sizeof(st), cudaMemcpyHostToDevice));
+    OSB_CUDA(cudaMemcpy(h->d_st_pairs, &st, sizeof(st), cudaMemcpyHostToDevice));
   }
-#undef FE_TRY
-#undef FE_CUDA
-  *out = h;
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_frontend_destroy(osb_frontend* h) {
-  if (!h) return OSB_OK;
-  h->sp.release(); h->nv.release();
-  h->mem.free_all();
-  for (int i = 0; i < 9; ++i) if (h->ev[i]) cudaEventDestroy(h->ev[i]);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->ev_ingest) cudaEventDestroy(h->ev_ingest);
-  if (h->h_cnt) cudaFreeHost(h->h_cnt);
-  if (h->fb_host) cudaFreeHost((void*)h->fb_host);
-  if (h->stream2) cudaStreamDestroy(h->stream2);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return OSB_OK;
 }
@@ -859,10 +840,7 @@ extern "C" osb_status osb_frontend_set_depth_camera(osb_frontend* h, const doubl
   OSB_REQUIRE(near_thres < far_thres, "near_thres must be below far_thres");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  if (!h->d_depth) {
-    const osb_status s = h->mem.alloc(&h->d_depth, (size_t)h->cfg.n_dirs * h->cfg.width * h->cfg.height);
-    if (s != OSB_OK) return s;
-  }
+  if (!h->d_depth) OSB_TRY(h->res.alloc(&h->d_depth, (size_t)h->cfg.n_dirs * h->cfg.width * h->cfg.height));
   for (int i = 0; i < 4; ++i) h->depth_K[i] = intrinsics[i];
   for (int d = 0; d < h->cfg.n_dirs; ++d)
     for (int i = 0; i < 7; ++i) h->depth_ext[d][i] = extrinsics[d * 7 + i];

@@ -202,65 +202,52 @@ extern "C" osb_status osb_stereo_lift(const float* kp_up, const float* kp_down, 
                                       int accept_min_3d_pts, float* pts3d, uint8_t* flag_up, uint8_t* flag_down) {
   OSB_REQUIRE(kp_up && kp_down && stereo_match && n_up && n_down && intrinsics && pose_up && pose_down && pts3d && flag_up &&
               flag_down, "null argument");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const size_t np = (size_t)n_dirs * max_n;
+  Resources res;
   float *d_u = nullptr, *d_d = nullptr, *d_p = nullptr;
   int32_t *d_m = nullptr, *d_nu = nullptr, *d_nd = nullptr;
   double *d_pu = nullptr, *d_pd = nullptr;
   uint8_t *d_fu = nullptr, *d_fd = nullptr;
-  auto cleanup = [&]() { cudaFree(d_u); cudaFree(d_d); cudaFree(d_p); cudaFree(d_m); cudaFree(d_nu); cudaFree(d_nd); cudaFree(d_pu); cudaFree(d_pd); cudaFree(d_fu); cudaFree(d_fd); };
-#define LF_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { set_error("osb_stereo_lift", cudaGetErrorString(e_)); cleanup(); return OSB_ERR_CUDA; } } while (0)
-  LF_CUDA(cudaMalloc(&d_u, np * 2 * sizeof(float))); LF_CUDA(cudaMalloc(&d_d, np * 2 * sizeof(float)));
-  LF_CUDA(cudaMalloc(&d_p, np * 3 * sizeof(float))); LF_CUDA(cudaMalloc(&d_m, np * sizeof(int32_t)));
-  LF_CUDA(cudaMalloc(&d_nu, n_dirs * sizeof(int32_t))); LF_CUDA(cudaMalloc(&d_nd, n_dirs * sizeof(int32_t)));
-  LF_CUDA(cudaMalloc(&d_pu, n_dirs * 7 * sizeof(double))); LF_CUDA(cudaMalloc(&d_pd, n_dirs * 7 * sizeof(double)));
-  LF_CUDA(cudaMalloc(&d_fu, np)); LF_CUDA(cudaMalloc(&d_fd, np));
-  LF_CUDA(cudaMemcpy(d_u, kp_up, np * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_d, kp_down, np * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_m, stereo_match, np * sizeof(int32_t), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_nu, n_up, n_dirs * sizeof(int32_t), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_nd, n_down, n_dirs * sizeof(int32_t), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_pu, pose_up, n_dirs * 7 * sizeof(double), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_pd, pose_down, n_dirs * 7 * sizeof(double), cudaMemcpyHostToDevice));
-  s = osb_stereo_lift_dev(d_u, d_d, d_m, d_nu, d_nd, n_dirs, max_n, intrinsics, d_pu, d_pd, triangle_thres, accept_min_3d_pts,
-                          d_p, d_fu, d_fd, nullptr);
-  if (s == OSB_OK) {
-    LF_CUDA(cudaMemcpy(pts3d, d_p, np * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-    LF_CUDA(cudaMemcpy(flag_up, d_fu, np, cudaMemcpyDeviceToHost));
-    LF_CUDA(cudaMemcpy(flag_down, d_fd, np, cudaMemcpyDeviceToHost));
-  }
-  cleanup();
-  return s;
+  OSB_TRY(res.upload(&d_u, kp_up, np * 2));
+  OSB_TRY(res.upload(&d_d, kp_down, np * 2));
+  OSB_TRY(res.alloc(&d_p, np * 3));
+  OSB_TRY(res.upload(&d_m, stereo_match, np));
+  OSB_TRY(res.upload(&d_nu, n_up, n_dirs));
+  OSB_TRY(res.upload(&d_nd, n_down, n_dirs));
+  OSB_TRY(res.upload(&d_pu, pose_up, n_dirs * 7));
+  OSB_TRY(res.upload(&d_pd, pose_down, n_dirs * 7));
+  OSB_TRY(res.alloc(&d_fu, np));
+  OSB_TRY(res.alloc(&d_fd, np));
+  OSB_TRY(osb_stereo_lift_dev(d_u, d_d, d_m, d_nu, d_nd, n_dirs, max_n, intrinsics, d_pu, d_pd, triangle_thres,
+                              accept_min_3d_pts, d_p, d_fu, d_fd, nullptr));
+  OSB_CUDA(cudaMemcpy(pts3d, d_p, np * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(flag_up, d_fu, np, cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(flag_down, d_fd, np, cudaMemcpyDeviceToHost));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_depth_lift(const float* kp, const int32_t* n, int n_dirs, int max_n, const uint16_t* depth_mm,
                                      int height, int width, const double* intrinsics, const double* pose_cam, double near_thres,
                                      double far_thres, int accept_min_3d_pts, float* pts3d, uint8_t* flag) {
   OSB_REQUIRE(kp && n && depth_mm && intrinsics && pose_cam && pts3d && flag, "null argument");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const size_t np = (size_t)n_dirs * max_n, nd = (size_t)n_dirs * height * width;
+  Resources res;
   float *d_k = nullptr, *d_p = nullptr;
   int32_t* d_n = nullptr;
   uint16_t* d_dep = nullptr;
   double* d_pc = nullptr;
   uint8_t* d_f = nullptr;
-  auto cleanup = [&]() { cudaFree(d_k); cudaFree(d_p); cudaFree(d_n); cudaFree(d_dep); cudaFree(d_pc); cudaFree(d_f); };
-  LF_CUDA(cudaMalloc(&d_k, np * 2 * sizeof(float))); LF_CUDA(cudaMalloc(&d_p, np * 3 * sizeof(float)));
-  LF_CUDA(cudaMalloc(&d_n, n_dirs * sizeof(int32_t))); LF_CUDA(cudaMalloc(&d_dep, nd * sizeof(uint16_t)));
-  LF_CUDA(cudaMalloc(&d_pc, n_dirs * 7 * sizeof(double))); LF_CUDA(cudaMalloc(&d_f, np));
-  LF_CUDA(cudaMemcpy(d_k, kp, np * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_n, n, n_dirs * sizeof(int32_t), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_dep, depth_mm, nd * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  LF_CUDA(cudaMemcpy(d_pc, pose_cam, n_dirs * 7 * sizeof(double), cudaMemcpyHostToDevice));
-  s = osb_depth_lift_dev(d_k, d_n, n_dirs, max_n, d_dep, height, width, intrinsics, d_pc, near_thres, far_thres,
-                         accept_min_3d_pts, d_p, d_f, nullptr);
-  if (s == OSB_OK) {
-    LF_CUDA(cudaMemcpy(pts3d, d_p, np * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-    LF_CUDA(cudaMemcpy(flag, d_f, np, cudaMemcpyDeviceToHost));
-  }
-#undef LF_CUDA
-  cleanup();
-  return s;
+  OSB_TRY(res.upload(&d_k, kp, np * 2));
+  OSB_TRY(res.alloc(&d_p, np * 3));
+  OSB_TRY(res.upload(&d_n, n, n_dirs));
+  OSB_TRY(res.upload(&d_dep, depth_mm, nd));
+  OSB_TRY(res.upload(&d_pc, pose_cam, n_dirs * 7));
+  OSB_TRY(res.alloc(&d_f, np));
+  OSB_TRY(osb_depth_lift_dev(d_k, d_n, n_dirs, max_n, d_dep, height, width, intrinsics, d_pc, near_thres, far_thres,
+                             accept_min_3d_pts, d_p, d_f, nullptr));
+  OSB_CUDA(cudaMemcpy(pts3d, d_p, np * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(flag, d_f, np, cudaMemcpyDeviceToHost));
+  return OSB_OK;
 }

@@ -506,6 +506,7 @@ osb_status bf_match_device(int n_pairs, int max_n, int out_stride, const float* 
 using namespace osb;
 
 struct osb_db {
+  Resources res;
   int device = 0;
   int dim = 0;
   int64_t cap = 0, ntotal = 0;
@@ -523,31 +524,26 @@ struct osb_db {
 
 extern "C" osb_status osb_db_create(osb_db** out, int dim, int64_t capacity) {
   OSB_REQUIRE(out != nullptr && dim > 0 && dim % 4 == 0 && dim <= 8192 && capacity > 0, "bad dim/capacity");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_db* h = new osb_db();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_db> h(new osb_db());
   h->device = current_device();
   h->dim = dim; h->cap = capacity;
   int64_t chunk;
   h->grid_max = db_scan_grid(capacity, &chunk);
-  OSB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  OSB_CUDA(cudaMalloc(&h->rows, (size_t)capacity * dim * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->part_scores, (size_t)8 * h->grid_max * h->kmax * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->part_ids, (size_t)8 * h->grid_max * h->kmax * sizeof(int64_t)));
-  OSB_CUDA(cudaMalloc(&h->done, sizeof(unsigned int)));
+  OSB_TRY(h->res.stream(&h->stream));
+  OSB_TRY(h->res.alloc(&h->rows, (size_t)capacity * dim));
+  OSB_TRY(h->res.alloc(&h->part_scores, (size_t)8 * h->grid_max * h->kmax));
+  OSB_TRY(h->res.alloc(&h->part_ids, (size_t)8 * h->grid_max * h->kmax));
+  OSB_TRY(h->res.alloc(&h->done, 1));
   OSB_CUDA(cudaMemset(h->done, 0, sizeof(unsigned int)));
-  OSB_CUDA(cudaMalloc(&h->d_q, (size_t)h->qmax * dim * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_scores, (size_t)h->qmax * h->kmax * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_ids, (size_t)h->qmax * h->kmax * sizeof(int64_t)));
-  *out = h;
+  OSB_TRY(h->res.alloc(&h->d_q, (size_t)h->qmax * dim));
+  OSB_TRY(h->res.alloc(&h->d_scores, (size_t)h->qmax * h->kmax));
+  OSB_TRY(h->res.alloc(&h->d_ids, (size_t)h->qmax * h->kmax));
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_db_destroy(osb_db* h) {
-  if (!h) return OSB_OK;
-  cudaFree(h->rows); cudaFree(h->part_scores); cudaFree(h->part_ids); cudaFree(h->done);
-  cudaFree(h->d_q); cudaFree(h->d_scores); cudaFree(h->d_ids);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return OSB_OK;
 }
@@ -655,6 +651,7 @@ extern "C" osb_status osb_db_search(osb_db* h, int64_t nq, const float* q, int k
 // C ABI: osb_matcher
 // =============================================================================================================
 struct osb_matcher {
+  Resources res;
   int device = 0;
   int max_pairs = 0, max_n = 0, dim = 0;
   float *d_q = nullptr, *d_t = nullptr, *d_dist = nullptr, *d_dout = nullptr;
@@ -678,32 +675,27 @@ static osb_status matcher_tables(osb_matcher* h, int n_pairs, const float* q, co
 extern "C" osb_status osb_matcher_create(osb_matcher** out, int max_pairs, int max_n, int dim) {
   OSB_REQUIRE(out != nullptr && max_pairs > 0 && max_n > 0 && max_n <= 256 && dim == BF_DIM,
               "max_n must be <= 256 and dim == 64");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_matcher* h = new osb_matcher();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_matcher> h(new osb_matcher());
   h->device = current_device();
   h->max_pairs = max_pairs; h->max_n = max_n; h->dim = dim;
   const size_t pn = (size_t)max_pairs * max_n;
-  OSB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  OSB_CUDA(cudaMalloc(&h->d_q, pn * dim * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_t, pn * dim * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_dist, pn * max_n * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_dout, pn * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&h->d_qi, pn * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_ti, pn * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_nq, max_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_nt, max_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_nout, max_pairs * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&h->d_ptrs, 2 * (size_t)max_pairs * sizeof(float*)));
-  *out = h;
+  OSB_TRY(h->res.stream(&h->stream));
+  OSB_TRY(h->res.alloc(&h->d_q, pn * dim));
+  OSB_TRY(h->res.alloc(&h->d_t, pn * dim));
+  OSB_TRY(h->res.alloc(&h->d_dist, pn * max_n));
+  OSB_TRY(h->res.alloc(&h->d_dout, pn));
+  OSB_TRY(h->res.alloc(&h->d_qi, pn));
+  OSB_TRY(h->res.alloc(&h->d_ti, pn));
+  OSB_TRY(h->res.alloc(&h->d_nq, max_pairs));
+  OSB_TRY(h->res.alloc(&h->d_nt, max_pairs));
+  OSB_TRY(h->res.alloc(&h->d_nout, max_pairs));
+  OSB_TRY(h->res.alloc(&h->d_ptrs, 2 * (size_t)max_pairs));
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_matcher_destroy(osb_matcher* h) {
-  if (!h) return OSB_OK;
-  cudaFree(h->d_q); cudaFree(h->d_t); cudaFree(h->d_dist); cudaFree(h->d_dout); cudaFree(h->d_qi);
-  cudaFree(h->d_ti); cudaFree(h->d_nq); cudaFree(h->d_nt); cudaFree(h->d_nout); cudaFree(h->d_ptrs);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return OSB_OK;
 }

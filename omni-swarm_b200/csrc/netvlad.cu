@@ -211,11 +211,6 @@ nv_block0_fused_kernel(const float* __restrict__ x, const float* __restrict__ dw
   }
 }
 
-static osb_status alloc(float** dst, size_t n) {
-  OSB_CUDA(cudaMalloc(dst, n * sizeof(float)));
-  return OSB_OK;
-}
-
 static osb_status copy_dev(float* dst, const float* src, size_t n, cudaStream_t st) {
   OSB_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return OSB_OK;
@@ -264,19 +259,18 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
   OSB_REQUIRE(n_weights == nv_expected_weights(), "weight blob has the wrong length (expected 607968 floats)");
   OSB_REQUIRE(width % 16 == 0 && height % 16 == 0 && width > 0 && height > 0, "width/height must be multiples of 16");
   W = width; H = height; max_batch = max_batch_;
-  OSB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  OSB_TRY(res.stream(&stream));
   {
     const char* e = getenv("OSB_SP_CONV");      // same debug switch as SuperPoint: ffma = fp32 CUDA-core pointwise convs
     use_umma = !(e && strcmp(e, "ffma") == 0);
   }
   const float* p = weights;
-  osb_status s;
   {
     std::vector<float> w9(9 * 32);
     for (int o = 0; o < 32; ++o)
       for (int t = 0; t < 9; ++t) w9[t * 32 + o] = p[o * 9 + t];
-    if ((s = upload_f32(&w0, w9.data(), 9 * 32)) != OSB_OK) return s;
-    if ((s = upload_f32(&b0, p + 32 * 9, 32)) != OSB_OK) return s;
+    OSB_TRY(res.upload(&w0, w9.data(), 9 * 32));
+    OSB_TRY(res.upload(&b0, p + 32 * 9, 32));
     p += 32 * 9 + 32;
   }
   for (int i = 0; i < 7; ++i) {
@@ -285,46 +279,46 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
     std::vector<float> dw((size_t)9 * ci);
     for (int c = 0; c < ci; ++c)
       for (int t = 0; t < 9; ++t) dw[(size_t)t * ci + c] = p[(size_t)c * 9 + t];
-    if ((s = upload_f32(&blk[i].dw, dw.data(), dw.size())) != OSB_OK) return s;
+    OSB_TRY(res.upload(&blk[i].dw, dw.data(), dw.size()));
     p += (size_t)ci * 9;
-    if ((s = upload_f32(&blk[i].dwb, p, ci)) != OSB_OK) return s;
+    OSB_TRY(res.upload(&blk[i].dwb, p, ci));
     p += ci;
-    if ((s = conv_layer_upload(&blk[i].pw, p, p + (size_t)co * ci, ci, co, 1)) != OSB_OK) return s;
+    OSB_TRY(conv_layer_upload(res, &blk[i].pw, p, p + (size_t)co * ci, ci, co, 1));
     if (i == 0) {                                  // block 0 fused kernel: pointwise weights as [k][oc]
       std::vector<float> kc((size_t)ci * co);
       for (int o = 0; o < co; ++o)
         for (int k = 0; k < ci; ++k) kc[(size_t)k * co + o] = p[(size_t)o * ci + k];
-      if ((s = upload_f32(&pw0_kc, kc.data(), kc.size())) != OSB_OK) return s;
-      if ((s = upload_f32(&pw0_b, p + (size_t)co * ci, co)) != OSB_OK) return s;
-      if ((s = nv_block0_prepare()) != OSB_OK) return s;
+      OSB_TRY(res.upload(&pw0_kc, kc.data(), kc.size()));
+      OSB_TRY(res.upload(&pw0_b, p + (size_t)co * ci, co));
+      OSB_TRY(nv_block0_prepare());
     }
-    if (use_umma && i >= 1 && (s = umma_layer_upload(&upw[i], p, p + (size_t)co * ci, ci, co, 1, NV_W_SCALE)) != OSB_OK) return s;
+    if (use_umma && i >= 1) OSB_TRY(umma_layer_upload(res, &upw[i], p, p + (size_t)co * ci, ci, co, 1, NV_W_SCALE));
     p += (size_t)co * ci + co;
   }
-  if ((s = conv_layer_upload(&proj, p, p + (size_t)NV_D * 512, 512, NV_D, 1)) != OSB_OK) return s;
-  if (use_umma && (s = umma_layer_upload(&uproj, p, p + (size_t)NV_D * 512, 512, NV_D, 1, NV_W_SCALE)) != OSB_OK) return s;
+  OSB_TRY(conv_layer_upload(res, &proj, p, p + (size_t)NV_D * 512, 512, NV_D, 1));
+  if (use_umma) OSB_TRY(umma_layer_upload(res, &uproj, p, p + (size_t)NV_D * 512, 512, NV_D, 1, NV_W_SCALE));
   p += (size_t)NV_D * 512 + NV_D;
-  if ((s = conv_layer_upload(&assign, p, p + (size_t)NV_K * NV_D, NV_D, NV_K, 1)) != OSB_OK) return s;
+  OSB_TRY(conv_layer_upload(res, &assign, p, p + (size_t)NV_K * NV_D, NV_D, NV_K, 1));
   p += (size_t)NV_K * NV_D + NV_K;
-  if ((s = upload_f32(&centroids, p, (size_t)NV_K * NV_D)) != OSB_OK) return s;
+  OSB_TRY(res.upload(&centroids, p, (size_t)NV_K * NV_D));
   {
     // engine input is the u8 image converted to float UNSCALED (mobilenetvlad_tensorrt.cpp:8-10); the stand-in
     // network's first op multiplies by 1/255 in f32.
     std::vector<float> l(256);
     const float sc = (float)(1.0 / 255.0);
     for (int v = 0; v < 256; ++v) l[v] = (float)v * sc;
-    if ((s = upload_f32(&lut, l.data(), 256)) != OSB_OK) return s;
+    OSB_TRY(res.upload(&lut, l.data(), 256));
   }
   const size_t B = max_batch;
   const size_t act = B * (H / 2) * (W / 2) * 64;   // largest activation: block 0 output (64 ch at 1/2 res)
-  OSB_CUDA(cudaMalloc(&d_img, B * H * W));
-  OSB_CUDA(cudaMalloc(&actA, act * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&actB, act * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_assign, B * (H / 16) * (W / 16) * NV_K * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_out, B * NV_K * NV_D * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_mu, B * NV_D * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_part, B * NV_SLICES * NV_K * NV_D * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_psum, B * NV_SLICES * NV_K * sizeof(float)));
+  OSB_TRY(res.alloc(&d_img, B * H * W));
+  OSB_TRY(res.alloc(&actA, act));
+  OSB_TRY(res.alloc(&actB, act));
+  OSB_TRY(res.alloc(&d_assign, B * (H / 16) * (W / 16) * NV_K));
+  OSB_TRY(res.alloc(&d_out, B * NV_K * NV_D));
+  OSB_TRY(res.alloc(&d_mu, B * NV_D));
+  OSB_TRY(res.alloc(&d_part, B * NV_SLICES * NV_K * NV_D));
+  OSB_TRY(res.alloc(&d_psum, B * NV_SLICES * NV_K));
   if (use_umma) {
     // planes of the pointwise inputs: blocks 1..6 (depthwise outputs) and the projection (block 6 output); all share
     // one buffer sized for the largest (they are live one at a time, except block 6 -> projection: two halves)
@@ -338,63 +332,49 @@ osb_status NetVLAD::init(const float* weights, size_t n_weights, int width, int 
     }
     gh[7] = h; gw[7] = w; gc[7] = 512;
     maxe = std::max(maxe, (size_t)B * h * w * 512);
-    OSB_CUDA(cudaMalloc(&planes, 4 * maxe * sizeof(__half)));          // two regions of (hi, lo)
+    OSB_TRY(res.alloc(&planes, 4 * maxe));      // two regions of (hi, lo)
     for (int i = 1; i < 8; ++i) {
       __half* base = planes + ((i & 1) ? 0 : 2 * maxe);                 // alternate regions: block 6 (even) vs proj (7, odd)
       pl_hi[i] = base; pl_lo[i] = base + (size_t)B * gh[i] * gw[i] * gc[i];
-      if ((s = umma_act_maps(&tmA[i], &tmB[i], pl_hi[i], pl_lo[i], (int)B, gh[i], gw[i], gc[i], 1)) != OSB_OK) return s;
+      OSB_TRY(umma_act_maps(&tmA[i], &tmB[i], pl_hi[i], pl_lo[i], (int)B, gh[i], gw[i], gc[i], 1));
     }
   }
   return OSB_OK;
 }
 
-void NetVLAD::release() {
-  cudaFree(w0); cudaFree(b0); cudaFree(lut); cudaFree(centroids); cudaFree(pw0_kc); cudaFree(pw0_b);
-  for (int i = 0; i < 7; ++i) { cudaFree(blk[i].dw); cudaFree(blk[i].dwb); conv_layer_free(&blk[i].pw); }
-  conv_layer_free(&proj); conv_layer_free(&assign);
-  cudaFree(d_img); cudaFree(actA); cudaFree(actB); cudaFree(d_assign); cudaFree(d_out);
-  cudaFree(d_mu); cudaFree(d_part); cudaFree(d_psum); cudaFree(planes);
-  for (int i = 0; i < 7; ++i) umma_layer_free(&upw[i]);
-  umma_layer_free(&uproj);
-  if (stream) cudaStreamDestroy(stream);
-}
-
 osb_status NetVLAD::infer_dev(const uint8_t* img_dev, int B, float* out_dev, cudaStream_t st) {
   OSB_REQUIRE(B > 0 && B <= max_batch, "batch out of range");
-  osb_status s;
-#define RUN(x) do { s = (x); if (s != OSB_OK) return s; } while (0)
   int h = H / 2, w = W / 2;
-  RUN(conv_first_forward(w0, b0, lut, img_dev, actA, B, H, W, 32, 2, ACT_RELU6, st));
+  OSB_TRY(conv_first_forward(w0, b0, lut, img_dev, actA, B, H, W, 32, 2, ACT_RELU6, st));
   float* cur = actA;                 // fp32 activations of the previous block
   for (int i = 0; i < 7; ++i) {
     if (use_umma && i == 0) {
-      RUN(nv_block0_forward(cur, blk[0].dw, blk[0].dwb, pw0_kc, pw0_b, actB, B, h, w, st));
+      OSB_TRY(nv_block0_forward(cur, blk[0].dw, blk[0].dwb, pw0_kc, pw0_b, actB, B, h, w, st));
       cur = actB;
     } else if (use_umma) {
       // depthwise (fp32 -> split planes) then pointwise on the tensor cores (planes -> fp32, or planes for the projection)
-      RUN(umma_dwconv_forward(blk[i].dw, blk[i].dwb, cur, pl_hi[i], pl_lo[i], B, h, w, blk[i].cin, blk[i].stride,
-                              NV_ACT_SCALE, st));
+      OSB_TRY(umma_dwconv_forward(blk[i].dw, blk[i].dwb, cur, pl_hi[i], pl_lo[i], B, h, w, blk[i].cin, blk[i].stride,
+                                  NV_ACT_SCALE, st));
       h /= blk[i].stride; w /= blk[i].stride;
       if (i < 6) {
-        RUN(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actA, blk[i].cout,
-                              blk[i].cout, 1.f, 2, 0, st));
+        OSB_TRY(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actA, blk[i].cout,
+                                  blk[i].cout, 1.f, 2, 0, st));
         cur = actA;
       } else {
-        RUN(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, pl_hi[7], pl_lo[7], nullptr, blk[i].cout,
-                              blk[i].cout, NV_ACT_SCALE, 2, 0, st));
+        OSB_TRY(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, pl_hi[7], pl_lo[7], nullptr, blk[i].cout,
+                                  blk[i].cout, NV_ACT_SCALE, 2, 0, st));
       }
     } else {
-      RUN(dwconv3x3_forward(blk[i].dw, blk[i].dwb, actA, actB, B, h, w, blk[i].cin, blk[i].stride, ACT_RELU6, st));
+      OSB_TRY(dwconv3x3_forward(blk[i].dw, blk[i].dwb, actA, actB, B, h, w, blk[i].cin, blk[i].stride, ACT_RELU6, st));
       h /= blk[i].stride; w /= blk[i].stride;
-      RUN(conv_forward(blk[i].pw, actB, actA, B, h, w, blk[i].cout, ACT_RELU6, st));
+      OSB_TRY(conv_forward(blk[i].pw, actB, actA, B, h, w, blk[i].cout, ACT_RELU6, st));
     }
   }
   if (use_umma)
-    RUN(umma_conv_forward(uproj, tmA[7], tmB[7], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actB, NV_D, NV_D, 1.f, 0, 0, st));
+    OSB_TRY(umma_conv_forward(uproj, tmA[7], tmB[7], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actB, NV_D, NV_D, 1.f, 0, 0, st));
   else
-    RUN(conv_forward(proj, actA, actB, B, h, w, NV_D, ACT_NONE, st));
-  RUN(nv_head_forward(assign, centroids, actB, B, h, w, d_mu, d_assign, d_part, d_psum, out_dev, st));
-#undef RUN
+    OSB_TRY(conv_forward(proj, actA, actB, B, h, w, NV_D, ACT_NONE, st));
+  OSB_TRY(nv_head_forward(assign, centroids, actB, B, h, w, d_mu, d_assign, d_part, d_psum, out_dev, st));
   return OSB_OK;
 }
 
@@ -411,19 +391,15 @@ struct osb_netvlad {
 extern "C" osb_status osb_netvlad_create(osb_netvlad** out, const float* weights, size_t n_weights, int width,
                                          int height, int max_batch) {
   OSB_REQUIRE(out != nullptr && max_batch > 0, "bad arguments");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_netvlad* h = new osb_netvlad();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_netvlad> h(new osb_netvlad());
   h->device = current_device();
-  s = h->nv.init(weights, n_weights, width, height, max_batch);
-  if (s != OSB_OK) { h->nv.release(); delete h; return s; }
-  *out = h;
+  OSB_TRY(h->nv.init(weights, n_weights, width, height, max_batch));
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_netvlad_destroy(osb_netvlad* h) {
-  if (!h) return OSB_OK;
-  h->nv.release();
   delete h;
   return OSB_OK;
 }
@@ -459,23 +435,22 @@ extern "C" osb_status osb_nv_block0_parity(const float* dw_w, const float* dw_b,
                                            void* stream) {
   OSB_REQUIRE(dw_w && dw_b && pw_w && pw_b && x_dev && y_dev, "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   std::vector<float> kc(F0_C * F0_OC);
   for (int o = 0; o < F0_OC; ++o)
     for (int k = 0; k < F0_C; ++k) kc[k * F0_OC + o] = pw_w[o * F0_C + k];
   float *dwd = nullptr, *dbd = nullptr, *kcd = nullptr, *pbd = nullptr;
-  s = upload_tap_major(&dwd, dw_w, F0_C);
-  if (s == OSB_OK) s = upload_f32(&dbd, dw_b, F0_C);
-  if (s == OSB_OK) s = upload_f32(&kcd, kc.data(), kc.size());
-  if (s == OSB_OK) s = upload_f32(&pbd, pw_b, F0_OC);
-  if (s == OSB_OK) s = nv_block0_prepare();
-  if (s == OSB_OK) s = nv_block0_forward(x_dev, dwd, dbd, kcd, pbd, y_dev, batch, height, width, st);
-  const cudaError_t e = cudaStreamSynchronize(st);          // the weights are freed below
-  cudaFree(dwd); cudaFree(dbd); cudaFree(kcd); cudaFree(pbd);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(upload_tap_major(res, &dwd, dw_w, F0_C));
+  OSB_TRY(res.upload(&dbd, dw_b, F0_C));
+  OSB_TRY(res.upload(&kcd, kc.data(), kc.size()));
+  OSB_TRY(res.upload(&pbd, pw_b, F0_OC));
+  OSB_TRY(nv_block0_prepare());
+  OSB_TRY(nv_block0_forward(x_dev, dwd, dbd, kcd, pbd, y_dev, batch, height, width, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_nv_head_parity(const float* assign_w, const float* assign_b, const float* centroids,
@@ -485,22 +460,19 @@ extern "C" osb_status osb_nv_head_parity(const float* assign_w, const float* ass
   OSB_REQUIRE(assign_w && assign_b && centroids && x_dev && mu_dev && xn_dev && logits_dev && assign_dev && out_dev,
               "null argument");
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
+  Resources res;
+  res.sync_before_release(st);
   const size_t locs = (size_t)batch * height * width;
   ConvLayer L;
   float *cd = nullptr, *part = nullptr, *psum = nullptr;
-  s = conv_layer_upload(&L, assign_w, assign_b, NV_D, NV_K, 1);
-  if (s == OSB_OK) s = upload_f32(&cd, centroids, (size_t)NV_K * NV_D);
-  if (s == OSB_OK) s = alloc(&part, (size_t)batch * NV_SLICES * NV_K * NV_D);
-  if (s == OSB_OK) s = alloc(&psum, (size_t)batch * NV_SLICES * NV_K);
-  if (s == OSB_OK) s = copy_dev(xn_dev, x_dev, locs * NV_D, st);      // the head centres and normalises in place
-  if (s == OSB_OK)
-    s = nv_head_forward(L, cd, xn_dev, batch, height, width, mu_dev, assign_dev, part, psum, out_dev, st, logits_dev);
-  const cudaError_t e = cudaStreamSynchronize(st);
-  conv_layer_free(&L);
-  cudaFree(cd); cudaFree(part); cudaFree(psum);
-  if (s == OSB_OK) OSB_CUDA(e);
-  return s;
+  OSB_TRY(conv_layer_upload(res, &L, assign_w, assign_b, NV_D, NV_K, 1));
+  OSB_TRY(res.upload(&cd, centroids, (size_t)NV_K * NV_D));
+  OSB_TRY(res.alloc(&part, (size_t)batch * NV_SLICES * NV_K * NV_D));
+  OSB_TRY(res.alloc(&psum, (size_t)batch * NV_SLICES * NV_K));
+  OSB_TRY(copy_dev(xn_dev, x_dev, locs * NV_D, st));  // the head centres and normalises in place
+  OSB_TRY(nv_head_forward(L, cd, xn_dev, batch, height, width, mu_dev, assign_dev, part, psum, out_dev, st, logits_dev));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
 }

@@ -194,11 +194,14 @@ extern "C" osb_status osb_pcm_dev(const osb_loop_edge* edges_dev, int n, double 
   uint32_t* bits = nullptr;
   int32_t* scratch = nullptr;
   OSB_CUDA(cudaMallocAsync(&bits, (size_t)n * W * sizeof(uint32_t), st));
-  OSB_CUDA(cudaMallocAsync(&scratch, (size_t)2 * n * sizeof(int32_t), st));
-  s = pcm_device(edges_dev, n, pcm_thres, odom_pos_cov_per_m, odom_ang_cov_per_m, bits, scratch, scratch + n, clique_dev,
-                 clique_size_dev, adj_dev, smd_dev, st);
+  const cudaError_t e = cudaMallocAsync(&scratch, (size_t)2 * n * sizeof(int32_t), st);
+  if (e == cudaSuccess) {
+    s = pcm_device(edges_dev, n, pcm_thres, odom_pos_cov_per_m, odom_ang_cov_per_m, bits, scratch, scratch + n, clique_dev,
+                   clique_size_dev, adj_dev, smd_dev, st);
+    cudaFreeAsync(scratch, st);
+  }
   cudaFreeAsync(bits, st);
-  cudaFreeAsync(scratch, st);
+  OSB_CUDA(e);
   return s;
 }
 
@@ -206,27 +209,20 @@ extern "C" osb_status osb_pcm(const osb_loop_edge* edges, int n, double pcm_thre
                               double odom_ang_cov_per_m, int32_t* clique, int32_t* clique_size, uint8_t* adj, double* smd) {
   OSB_REQUIRE(edges && clique && clique_size, "null argument");
   OSB_REQUIRE(n > 0 && n <= PCM_MAX_N, "number of loop edges must be in 1..4096");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
+  Resources res;
   osb_loop_edge* d_e = nullptr;
   int32_t* d_c = nullptr;
   uint8_t* d_adj = nullptr;
   double* d_smd = nullptr;
-  auto cleanup = [&]() { cudaFree(d_e); cudaFree(d_c); cudaFree(d_adj); cudaFree(d_smd); };
-#define PCM_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { set_error("osb_pcm", cudaGetErrorString(e_)); cleanup(); return OSB_ERR_CUDA; } } while (0)
-  PCM_CUDA(cudaMalloc(&d_e, (size_t)n * sizeof(osb_loop_edge)));
-  PCM_CUDA(cudaMalloc(&d_c, (size_t)(n + 1) * sizeof(int32_t)));
-  if (adj) PCM_CUDA(cudaMalloc(&d_adj, (size_t)n * n));
-  if (smd) PCM_CUDA(cudaMalloc(&d_smd, (size_t)n * n * sizeof(double)));
-  PCM_CUDA(cudaMemcpy(d_e, edges, (size_t)n * sizeof(osb_loop_edge), cudaMemcpyHostToDevice));
-  s = osb_pcm_dev(d_e, n, pcm_thres, odom_pos_cov_per_m, odom_ang_cov_per_m, d_c, d_c + n, d_adj, d_smd, nullptr);
-  if (s == OSB_OK) {
-    PCM_CUDA(cudaMemcpy(clique, d_c, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    PCM_CUDA(cudaMemcpy(clique_size, d_c + n, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    if (adj) PCM_CUDA(cudaMemcpy(adj, d_adj, (size_t)n * n, cudaMemcpyDeviceToHost));
-    if (smd) PCM_CUDA(cudaMemcpy(smd, d_smd, (size_t)n * n * sizeof(double), cudaMemcpyDeviceToHost));
-  }
-#undef PCM_CUDA
-  cleanup();
-  return s;
+  OSB_TRY(res.upload(&d_e, edges, n));
+  OSB_TRY(res.alloc(&d_c, (size_t)n + 1));
+  if (adj) OSB_TRY(res.alloc(&d_adj, (size_t)n * n));
+  if (smd) OSB_TRY(res.alloc(&d_smd, (size_t)n * n));
+  OSB_TRY(osb_pcm_dev(d_e, n, pcm_thres, odom_pos_cov_per_m, odom_ang_cov_per_m, d_c, d_c + n, d_adj, d_smd, nullptr));
+  OSB_CUDA(cudaMemcpy(clique, d_c, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(clique_size, d_c + n, sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (adj) OSB_CUDA(cudaMemcpy(adj, d_adj, (size_t)n * n, cudaMemcpyDeviceToHost));
+  if (smd) OSB_CUDA(cudaMemcpy(smd, d_smd, (size_t)n * n * sizeof(double), cudaMemcpyDeviceToHost));
+  return OSB_OK;
 }

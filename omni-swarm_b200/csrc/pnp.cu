@@ -351,32 +351,22 @@ extern "C" osb_status osb_pnp_ransac(const float* pts3d, const float* pts2d, con
                                      const osb_pnp_params* params, uint8_t* mask, osb_pnp_result* results) {
   OSB_REQUIRE(pts3d && pts2d && n && params && mask && results, "null argument");
   OSB_REQUIRE(n_cand > 0 && max_n > 0 && max_n <= PNP_MAXN, "max_n must be in 1..1024");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
+  OSB_TRY(require_device());
   const size_t np = (size_t)n_cand * max_n;
+  Resources res;
   float *d3 = nullptr, *d2 = nullptr;
   int32_t* dn = nullptr;
   osb_pnp_params* dp = nullptr;
   osb_pnp_result* dr = nullptr;
   uint8_t* dm = nullptr;
-  auto cleanup = [&]() { cudaFree(d3); cudaFree(d2); cudaFree(dn); cudaFree(dp); cudaFree(dr); cudaFree(dm); };
-#define PNP_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { set_error("osb_pnp_ransac", cudaGetErrorString(e_)); cleanup(); return OSB_ERR_CUDA; } } while (0)
-  PNP_CUDA(cudaMalloc(&d3, np * 3 * sizeof(float)));
-  PNP_CUDA(cudaMalloc(&d2, np * 2 * sizeof(float)));
-  PNP_CUDA(cudaMalloc(&dn, n_cand * sizeof(int32_t)));
-  PNP_CUDA(cudaMalloc(&dp, n_cand * sizeof(osb_pnp_params)));
-  PNP_CUDA(cudaMalloc(&dr, n_cand * sizeof(osb_pnp_result)));
-  PNP_CUDA(cudaMalloc(&dm, np));
-  PNP_CUDA(cudaMemcpy(d3, pts3d, np * 3 * sizeof(float), cudaMemcpyHostToDevice));
-  PNP_CUDA(cudaMemcpy(d2, pts2d, np * 2 * sizeof(float), cudaMemcpyHostToDevice));
-  PNP_CUDA(cudaMemcpy(dn, n, n_cand * sizeof(int32_t), cudaMemcpyHostToDevice));
-  PNP_CUDA(cudaMemcpy(dp, params, n_cand * sizeof(osb_pnp_params), cudaMemcpyHostToDevice));
-  s = osb_pnp_ransac_dev(d3, d2, dn, n_cand, max_n, dp, dm, dr, nullptr);
-  if (s == OSB_OK) {
-    PNP_CUDA(cudaMemcpy(mask, dm, np, cudaMemcpyDeviceToHost));
-    PNP_CUDA(cudaMemcpy(results, dr, n_cand * sizeof(osb_pnp_result), cudaMemcpyDeviceToHost));
-  }
-#undef PNP_CUDA
-  cleanup();
-  return s;
+  OSB_TRY(res.upload(&d3, pts3d, np * 3));
+  OSB_TRY(res.upload(&d2, pts2d, np * 2));
+  OSB_TRY(res.upload(&dn, n, n_cand));
+  OSB_TRY(res.upload(&dp, params, n_cand));
+  OSB_TRY(res.alloc(&dr, n_cand));
+  OSB_TRY(res.alloc(&dm, np));
+  OSB_TRY(osb_pnp_ransac_dev(d3, d2, dn, n_cand, max_n, dp, dm, dr, nullptr));
+  OSB_CUDA(cudaMemcpy(mask, dm, np, cudaMemcpyDeviceToHost));
+  OSB_CUDA(cudaMemcpy(results, dr, n_cand * sizeof(osb_pnp_result), cudaMemcpyDeviceToHost));
+  return OSB_OK;
 }

@@ -29,14 +29,14 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
   OSB_REQUIRE(max_num_ > 0 && max_num_ <= 8192 && max_batch_ > 0, "bad max_num / max_batch");
   W = width; H = height; thres = thres_; max_num = max_num_; max_batch = max_batch_;
   Hc = H / 8; Wc = W / 8;
-  OSB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  OSB_TRY(res.stream(&stream));
   {
     int least = 0, greatest = 0;
     OSB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-    OSB_CUDA(cudaStreamCreateWithPriority(&kp_stream, cudaStreamNonBlocking, greatest));
+    OSB_TRY(res.stream(&kp_stream, greatest));
   }
-  OSB_CUDA(cudaEventCreateWithFlags(&ev_semi, cudaEventDisableTiming));
-  OSB_CUDA(cudaEventCreateWithFlags(&ev_kp, cudaEventDisableTiming));
+  OSB_TRY(res.event(&ev_semi, cudaEventDisableTiming));
+  OSB_TRY(res.event(&ev_kp, cudaEventDisableTiming));
   if (const char* e = getenv("OSB_SP_OVERLAP")) overlap_kp = atoi(e) != 0;
   if (const char* e = getenv("OSB_SP_FUSED_SOFTMAX")) fused_softmax = atoi(e) != 0;
   // ---- weights ----
@@ -46,10 +46,8 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
     std::vector<float> w9(9 * 64);
     for (int o = 0; o < 64; ++o)
       for (int t = 0; t < 9; ++t) w9[t * 64 + o] = p[o * 9 + t];
-    OSB_CUDA(cudaMalloc(&w1a, 9 * 64 * sizeof(float)));
-    OSB_CUDA(cudaMalloc(&b1a, 64 * sizeof(float)));
-    OSB_CUDA(cudaMemcpy(w1a, w9.data(), 9 * 64 * sizeof(float), cudaMemcpyHostToDevice));
-    OSB_CUDA(cudaMemcpy(b1a, p + 64 * 9, 64 * sizeof(float), cudaMemcpyHostToDevice));
+    OSB_TRY(res.upload(&w1a, w9.data(), 9 * 64));
+    OSB_TRY(res.upload(&b1a, p + 64 * 9, 64));
     p += 64 * 9 + 64;
   }
   {
@@ -59,12 +57,8 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
   }
   for (int i = 1; i < 12; ++i) {
     const size_t nw = (size_t)SP_COUT[i] * SP_CIN[i] * SP_KS[i] * SP_KS[i];
-    osb_status s = conv_layer_upload(&L[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i]);
-    if (s != OSB_OK) return s;
-    if (use_umma) {
-      s = umma_layer_upload(&UL[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i], SP_W_SCALE);
-      if (s != OSB_OK) return s;
-    }
+    OSB_TRY(conv_layer_upload(res, &L[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i]));
+    if (use_umma) OSB_TRY(umma_layer_upload(res, &UL[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i], SP_W_SCALE));
     p += nw + SP_COUT[i];
   }
   {
@@ -73,24 +67,21 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
     std::vector<float> l(256);
     const float alpha = (float)(1.0 / 255.0);
     for (int v = 0; v < 256; ++v) l[v] = (float)v * alpha;
-    OSB_CUDA(cudaMalloc(&lut, 256 * sizeof(float)));
-    OSB_CUDA(cudaMemcpy(lut, l.data(), 256 * sizeof(float), cudaMemcpyHostToDevice));
+    OSB_TRY(res.upload(&lut, l.data(), 256));
   }
   {
     std::vector<float> ct(256 * 64);
     for (int o = 0; o < 64; ++o)
       for (int c = 0; c < 256; ++c) ct[c * 64 + o] = pca_comp[o * 256 + c];
-    OSB_CUDA(cudaMalloc(&pca_compT, 256 * 64 * sizeof(float)));
-    OSB_CUDA(cudaMalloc(&pca_mean_d, 256 * sizeof(float)));
-    OSB_CUDA(cudaMemcpy(pca_compT, ct.data(), 256 * 64 * sizeof(float), cudaMemcpyHostToDevice));
-    OSB_CUDA(cudaMemcpy(pca_mean_d, pca_mean, 256 * sizeof(float), cudaMemcpyHostToDevice));
+    OSB_TRY(res.upload(&pca_compT, ct.data(), 256 * 64));
+    OSB_TRY(res.upload(&pca_mean_d, pca_mean, 256));
   }
   // ---- activations ----
   const size_t B = max_batch, HW = (size_t)H * W;
-  OSB_CUDA(cudaMalloc(&d_img, B * HW));
-  OSB_CUDA(cudaMalloc(&actA, B * HW * 64 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&actB, B * HW * 64 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_logits, B * Hc * Wc * 80 * sizeof(float)));
+  OSB_TRY(res.alloc(&d_img, B * HW));
+  OSB_TRY(res.alloc(&actA, B * HW * 64));
+  OSB_TRY(res.alloc(&actB, B * HW * 64));
+  OSB_TRY(res.alloc(&d_logits, B * Hc * Wc * 80));
   if (use_umma) {
     // input geometry of every conv layer: which ping-pong buffer it reads and its [H][W][C]
     // (layer order: 1 conv1b 2 conv2a 3 conv2b 4 conv3a 5 conv3b 6 conv4a 7 conv4b 8 convPa 9 convPb 10 convDa 11 convDb)
@@ -103,46 +94,30 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
       __half* base = reinterpret_cast<__half*>(in_buf[i] == 0 ? actA : actB);
       in_hi[i] = base;
       in_lo[i] = base + (size_t)max_batch * h * w * c;
-      osb_status s = umma_act_maps(&tmA[i], &tmB[i], in_hi[i], in_lo[i], max_batch, h, w, c, SP_KS[i]);
-      if (s != OSB_OK) return s;
+      OSB_TRY(umma_act_maps(&tmA[i], &tmB[i], in_hi[i], in_lo[i], max_batch, h, w, c, SP_KS[i]));
     }
   }
-  OSB_CUDA(cudaMalloc(&d_semi, B * HW * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_desc, B * Hc * Wc * 256 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&ks.state, B * HW));
-  OSB_CUDA(cudaMalloc(&ks.surv, B * HW));
-  OSB_CUDA(cudaMalloc(&ks.cand, B * HW * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&ks.skey, B * HW * sizeof(unsigned long long)));
-  OSB_CUDA(cudaMalloc(&ks.cmask, B * 2 * HW * sizeof(unsigned long long)));
-  OSB_CUDA(cudaMalloc(&ks.counts, B * 8 * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&ks.cnorm, B * 256 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_nk, B * sizeof(int32_t)));
-  OSB_CUDA(cudaMalloc(&d_kpts, B * max_num * 2 * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_conf, B * max_num * sizeof(float)));
-  OSB_CUDA(cudaMalloc(&d_out, B * max_num * 64 * sizeof(float)));
+  OSB_TRY(res.alloc(&d_semi, B * HW));
+  OSB_TRY(res.alloc(&d_desc, B * Hc * Wc * 256));
+  OSB_TRY(res.alloc(&ks.state, B * HW));
+  OSB_TRY(res.alloc(&ks.surv, B * HW));
+  OSB_TRY(res.alloc(&ks.cand, B * HW));
+  OSB_TRY(res.alloc(&ks.skey, B * HW));
+  OSB_TRY(res.alloc(&ks.cmask, B * 2 * HW));
+  OSB_TRY(res.alloc(&ks.counts, B * 8));
+  OSB_TRY(res.alloc(&ks.cnorm, B * 256));
+  OSB_TRY(res.alloc(&d_nk, B));
+  OSB_TRY(res.alloc(&d_kpts, B * max_num * 2));
+  OSB_TRY(res.alloc(&d_conf, B * max_num));
+  OSB_TRY(res.alloc(&d_out, B * max_num * 64));
   OSB_CUDA(cudaMemset(d_nk, 0, B * sizeof(int32_t)));
   OSB_CUDA(cudaMemset(ks.surv, 0, B * HW));
   return OSB_OK;
 }
 
-void SuperPoint::release() {
-  cudaFree(w1a); cudaFree(b1a); cudaFree(lut); cudaFree(pca_compT); cudaFree(pca_mean_d);
-  for (int i = 1; i < 12; ++i) { conv_layer_free(&L[i]); umma_layer_free(&UL[i]); }
-  for (int i = 0; i < 20; ++i) if (lev[i]) cudaEventDestroy(lev[i]);
-  cudaFree(d_img); cudaFree(actA); cudaFree(actB); cudaFree(d_logits); cudaFree(d_semi); cudaFree(d_desc);
-  cudaFree(ks.state); cudaFree(ks.surv); cudaFree(ks.cand); cudaFree(ks.skey); cudaFree(ks.cmask); cudaFree(ks.counts); cudaFree(ks.cnorm);
-  cudaFree(d_nk); cudaFree(d_kpts); cudaFree(d_conf); cudaFree(d_out);
-  if (stream) cudaStreamDestroy(stream);
-  if (kp_stream) cudaStreamDestroy(kp_stream);
-  if (ev_semi) cudaEventDestroy(ev_semi);
-  if (ev_kp) cudaEventDestroy(ev_kp);
-}
-
 // tensor-core network: every activation is a pair of fp16 planes (hi, lo) scaled by SP_ACT_SCALE; the planes of a
 // layer's output live in the ping-pong buffer the next layer's TMA descriptors point at.
 osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp) {
-  osb_status s;
-#define RUN(x) do { s = (x); if (s != OSB_OK) return s; } while (0)
   const float SA = SP_ACT_SCALE;
   n_lev = 0;
   mark(st);
@@ -152,31 +127,31 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
     return umma_conv_forward(UL[i], tmA[i], tmB[i], B, h, w, SA, in_hi[out_layer], in_lo[out_layer], nullptr,
                              SP_COUT[i], SP_COUT[i], SA, 1, pool, st);
   };
-  RUN(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st));   // conv1a            -> A
+  OSB_TRY(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st));   // conv1a            -> A
   mark(st);
-  RUN(conv(1, H, W, 2, 1));                                                               // conv1b + pool     -> B
+  OSB_TRY(conv(1, H, W, 2, 1));                                                               // conv1b + pool     -> B
   mark(st);
-  RUN(conv(2, H / 2, W / 2, 3, 0));                                                       // conv2a            -> A
+  OSB_TRY(conv(2, H / 2, W / 2, 3, 0));                                                       // conv2a            -> A
   mark(st);
-  RUN(conv(3, H / 2, W / 2, 4, 1));                                                       // conv2b + pool     -> B
+  OSB_TRY(conv(3, H / 2, W / 2, 4, 1));                                                       // conv2b + pool     -> B
   mark(st);
-  RUN(conv(4, H / 4, W / 4, 5, 0));                                                       // conv3a            -> A
+  OSB_TRY(conv(4, H / 4, W / 4, 5, 0));                                                       // conv3a            -> A
   mark(st);
-  RUN(conv(5, H / 4, W / 4, 6, 1));                                                       // conv3b + pool     -> B
+  OSB_TRY(conv(5, H / 4, W / 4, 6, 1));                                                       // conv3b + pool     -> B
   mark(st);
-  RUN(conv(6, Hc, Wc, 7, 0));                                                             // conv4a            -> A
+  OSB_TRY(conv(6, Hc, Wc, 7, 0));                                                             // conv4a            -> A
   mark(st);
-  RUN(conv(7, Hc, Wc, 8, 0));                                                             // conv4b            -> B (x)
+  OSB_TRY(conv(7, Hc, Wc, 8, 0));                                                             // conv4b            -> B (x)
   mark(st);
-  RUN(conv(8, Hc, Wc, 9, 0));                                                             // convPa            -> A
+  OSB_TRY(conv(8, Hc, Wc, 9, 0));                                                             // convPa            -> A
   mark(st);
   if (fused_softmax) {
-    RUN(umma_conv_softmax_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, d_semi, st));      // convPb + softmax + pixel shuffle
+    OSB_TRY(umma_conv_softmax_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, d_semi, st));      // convPb + softmax + pixel shuffle
     mark(st);
   } else {
-    RUN(umma_conv_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, nullptr, nullptr, d_logits, 80, 80, 1.f, 0, 0, st));   // convPb
+    OSB_TRY(umma_conv_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, nullptr, nullptr, d_logits, 80, 80, 1.f, 0, 0, st));   // convPb
     mark(st);
-    RUN(sp_softmax_shuffle(d_logits, 80, d_semi, B, Hc, Wc, st));
+    OSB_TRY(sp_softmax_shuffle(d_logits, 80, d_semi, B, Hc, Wc, st));
   }
   // the keypoint kernel (one CTA per image, latency-bound) runs beside the descriptor head, which leaves it B SMs
   const bool fork = kp && overlap_kp && !layer_prof && kp_stream;
@@ -184,47 +159,43 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
   if (fork) {
     OSB_CUDA(cudaEventRecord(ev_semi, st));
     OSB_CUDA(cudaStreamWaitEvent(kp_stream, ev_semi, 0));
-    RUN(keypoints(B, *kp, kp_stream));
+    OSB_TRY(keypoints(B, *kp, kp_stream));
     OSB_CUDA(cudaEventRecord(ev_kp, kp_stream));
     head_ctas = std::max(1, persistent_ctas() - B);
   }
-  RUN(umma_conv_forward(UL[10], tmA[10], tmB[10], B, Hc, Wc, SA, in_hi[11], in_lo[11], nullptr, SP_COUT[10], SP_COUT[10],
-                        SA, 1, 0, st, head_ctas));                                        // convDa (reads B)  -> A
+  OSB_TRY(umma_conv_forward(UL[10], tmA[10], tmB[10], B, Hc, Wc, SA, in_hi[11], in_lo[11], nullptr, SP_COUT[10], SP_COUT[10],
+                            SA, 1, 0, st, head_ctas));                                        // convDa (reads B)  -> A
   mark(st);
-  RUN(umma_conv_forward(UL[11], tmA[11], tmB[11], B, Hc, Wc, SA, nullptr, nullptr, d_desc, 256, 256, 1.f, 0, 0, st,
-                        head_ctas));                                                      // convDb
+  OSB_TRY(umma_conv_forward(UL[11], tmA[11], tmB[11], B, Hc, Wc, SA, nullptr, nullptr, d_desc, 256, 256, 1.f, 0, 0, st,
+                            head_ctas));                                                      // convDb
   mark(st);
-  RUN(l2norm_cells(d_desc, (int64_t)B * Hc * Wc, 256, st));
+  OSB_TRY(l2norm_cells(d_desc, (int64_t)B * Hc * Wc, 256, st));
   if (fork) OSB_CUDA(cudaStreamWaitEvent(st, ev_kp, 0));
-  else if (kp) RUN(keypoints(B, *kp, st));
-#undef RUN
+  else if (kp) OSB_TRY(keypoints(B, *kp, st));
   return OSB_OK;
 }
 
 // the network: u8 images (device) -> d_semi, d_desc
 osb_status SuperPoint::network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp) {
   if (use_umma) return network_umma(img_dev, B, st, kp);
-  osb_status s;
-#define RUN(x) do { s = (x); if (s != OSB_OK) return s; } while (0)
-  RUN(conv_first_forward(w1a, b1a, lut, img_dev, actA, B, H, W, 64, 1, ACT_RELU, st));      // conv1a
-  RUN(conv_forward(L[1], actA, actB, B, H, W, 64, ACT_RELU, st));                            // conv1b
-  RUN(maxpool2x2_forward(actB, actA, B, H, W, 64, st));
-  RUN(conv_forward(L[2], actA, actB, B, H / 2, W / 2, 64, ACT_RELU, st));                    // conv2a
-  RUN(conv_forward(L[3], actB, actA, B, H / 2, W / 2, 64, ACT_RELU, st));                    // conv2b
-  RUN(maxpool2x2_forward(actA, actB, B, H / 2, W / 2, 64, st));
-  RUN(conv_forward(L[4], actB, actA, B, H / 4, W / 4, 128, ACT_RELU, st));                   // conv3a
-  RUN(conv_forward(L[5], actA, actB, B, H / 4, W / 4, 128, ACT_RELU, st));                   // conv3b
-  RUN(maxpool2x2_forward(actB, actA, B, H / 4, W / 4, 128, st));
-  RUN(conv_forward(L[6], actA, actB, B, Hc, Wc, 128, ACT_RELU, st));                         // conv4a
-  RUN(conv_forward(L[7], actB, actA, B, Hc, Wc, 128, ACT_RELU, st));                         // conv4b
-  RUN(conv_forward(L[8], actA, actB, B, Hc, Wc, 256, ACT_RELU, st));                         // convPa
-  RUN(conv_forward(L[9], actB, d_logits, B, Hc, Wc, 72, ACT_NONE, st));                      // convPb (65 -> stride 72)
-  RUN(conv_forward(L[10], actA, actB, B, Hc, Wc, 256, ACT_RELU, st));                        // convDa
-  RUN(conv_forward(L[11], actB, d_desc, B, Hc, Wc, 256, ACT_NONE, st));                      // convDb
-  RUN(l2norm_cells(d_desc, (int64_t)B * Hc * Wc, 256, st));
-  RUN(sp_softmax_shuffle(d_logits, 72, d_semi, B, Hc, Wc, st));
-  if (kp) RUN(keypoints(B, *kp, st));
-#undef RUN
+  OSB_TRY(conv_first_forward(w1a, b1a, lut, img_dev, actA, B, H, W, 64, 1, ACT_RELU, st));  // conv1a
+  OSB_TRY(conv_forward(L[1], actA, actB, B, H, W, 64, ACT_RELU, st));                        // conv1b
+  OSB_TRY(maxpool2x2_forward(actB, actA, B, H, W, 64, st));
+  OSB_TRY(conv_forward(L[2], actA, actB, B, H / 2, W / 2, 64, ACT_RELU, st));                // conv2a
+  OSB_TRY(conv_forward(L[3], actB, actA, B, H / 2, W / 2, 64, ACT_RELU, st));                // conv2b
+  OSB_TRY(maxpool2x2_forward(actA, actB, B, H / 2, W / 2, 64, st));
+  OSB_TRY(conv_forward(L[4], actB, actA, B, H / 4, W / 4, 128, ACT_RELU, st));               // conv3a
+  OSB_TRY(conv_forward(L[5], actA, actB, B, H / 4, W / 4, 128, ACT_RELU, st));               // conv3b
+  OSB_TRY(maxpool2x2_forward(actB, actA, B, H / 4, W / 4, 128, st));
+  OSB_TRY(conv_forward(L[6], actA, actB, B, Hc, Wc, 128, ACT_RELU, st));                     // conv4a
+  OSB_TRY(conv_forward(L[7], actB, actA, B, Hc, Wc, 128, ACT_RELU, st));                     // conv4b
+  OSB_TRY(conv_forward(L[8], actA, actB, B, Hc, Wc, 256, ACT_RELU, st));                     // convPa
+  OSB_TRY(conv_forward(L[9], actB, d_logits, B, Hc, Wc, 72, ACT_NONE, st));                  // convPb (65 -> stride 72)
+  OSB_TRY(conv_forward(L[10], actA, actB, B, Hc, Wc, 256, ACT_RELU, st));                    // convDa
+  OSB_TRY(conv_forward(L[11], actB, d_desc, B, Hc, Wc, 256, ACT_NONE, st));                  // convDb
+  OSB_TRY(l2norm_cells(d_desc, (int64_t)B * Hc * Wc, 256, st));
+  OSB_TRY(sp_softmax_shuffle(d_logits, 72, d_semi, B, Hc, Wc, st));
+  if (kp) OSB_TRY(keypoints(B, *kp, st));
   return OSB_OK;
 }
 
@@ -271,19 +242,15 @@ extern "C" osb_status osb_superpoint_create(osb_superpoint** out, const float* w
                                             int height, float thres, int max_num, const float* pca_comp,
                                             const float* pca_mean, int max_batch) {
   OSB_REQUIRE(out != nullptr, "null out");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_superpoint* h = new osb_superpoint();
+  OSB_TRY(require_device());
+  std::unique_ptr<osb_superpoint> h(new osb_superpoint());
   h->device = current_device();
-  s = h->sp.init(weights, n_weights, width, height, thres, max_num, pca_comp, pca_mean, max_batch);
-  if (s != OSB_OK) { h->sp.release(); delete h; return s; }
-  *out = h;
+  OSB_TRY(h->sp.init(weights, n_weights, width, height, thres, max_num, pca_comp, pca_mean, max_batch));
+  *out = h.release();
   return OSB_OK;
 }
 
 extern "C" osb_status osb_superpoint_destroy(osb_superpoint* h) {
-  if (!h) return OSB_OK;
-  h->sp.release();
   delete h;
   return OSB_OK;
 }

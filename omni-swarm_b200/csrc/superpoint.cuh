@@ -10,6 +10,7 @@ size_t sp_expected_weights();
 size_t nv_expected_weights();
 
 struct SuperPoint {
+  Resources res;                   // every buffer, stream and event below
   int W = 0, H = 0, Wc = 0, Hc = 0, max_num = 0, max_batch = 0, last_batch = 0;
   float thres = 0.f;
   cudaStream_t stream = nullptr;
@@ -32,11 +33,10 @@ struct SuperPoint {
   bool layer_prof = false;
   cudaEvent_t lev[20] = {};
   int n_lev = 0;
-  void mark(cudaStream_t st) { if (layer_prof && n_lev < 20) { if (!lev[n_lev]) cudaEventCreate(&lev[n_lev]); cudaEventRecord(lev[n_lev++], st); } }
+  void mark(cudaStream_t st) { if (layer_prof && n_lev < 20) { if (!lev[n_lev]) res.event(&lev[n_lev]); cudaEventRecord(lev[n_lev++], st); } }
 
   osb_status init(const float* weights, size_t n_weights, int width, int height, float thres, int max_num,
                   const float* pca_comp, const float* pca_mean, int max_batch);
-  void release();
   // keypoint extraction needs only the detector head: when a KpJob is passed, the network launches it on `kp_stream`
   // as soon as the heat map exists and runs the descriptor head beside it (on B fewer SMs); `st` re-joins before return
   struct KpJob { int32_t* nk; float* kpts; float* conf; };
@@ -55,6 +55,7 @@ struct SuperPoint {
 };
 
 struct NetVLAD {
+  Resources res;                   // every buffer and the stream below
   int W = 0, H = 0, max_batch = 0;
   cudaStream_t stream = nullptr;
   float *w0 = nullptr, *b0 = nullptr, *lut = nullptr, *pw0_kc = nullptr, *pw0_b = nullptr;
@@ -72,7 +73,6 @@ struct NetVLAD {
   __half* planes = nullptr;
 
   osb_status init(const float* weights, size_t n_weights, int width, int height, int max_batch);
-  void release();
   osb_status infer_dev(const uint8_t* img_dev, int B, float* out_dev, cudaStream_t st);
 };
 

@@ -81,6 +81,7 @@ typedef CUresult (*PFN_memsetD32Async)(CUdeviceptr, unsigned int, size_t, CUstre
 constexpr int SWARM_MAX_WORLD = 64;
 
 struct osb_swarm {
+  Resources res;                               // the side stream and the two events
   int device = 0;
   int rank = 0, world = 1;
   ncclComm_t comm = nullptr;
@@ -175,30 +176,24 @@ extern "C" osb_status osb_swarm_destroy(osb_swarm* h) {
     if (r != h->rank && h->peer[r]) cudaIpcCloseMemHandle(h->peer[r]);
   if (h->inbox) cudaFree(h->inbox);
   if (h->comm) { NcclApi* api = nccl_api(); if (api) api->CommDestroy(h->comm); }
-  if (h->ev_ready) cudaEventDestroy(h->ev_ready);
-  if (h->ev_done) cudaEventDestroy(h->ev_done);
-  if (h->side) cudaStreamDestroy(h->side);
   delete h;
   return OSB_OK;
 }
 
 extern "C" osb_status osb_swarm_init(osb_swarm** out, const uint8_t* id, int rank, int world) {
   OSB_REQUIRE(out != nullptr && world >= 1 && rank >= 0 && rank < world, "bad rank / world");
-  osb_status s = require_device();
-  if (s != OSB_OK) return s;
-  osb_swarm* h = new osb_swarm();
+  OSB_TRY(require_device());
+  // nothing but the owner's stream and events exists until the communicator does, so an early return needs no destroy
+  std::unique_ptr<osb_swarm> h(new osb_swarm());
   h->rank = rank; h->world = world;
   h->device = current_device();
-#define SW_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { set_error("osb_swarm_init", cudaGetErrorString(e_)); osb_swarm_destroy(h); return OSB_ERR_CUDA; } } while (0)
-  SW_CUDA(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-  SW_CUDA(cudaEventCreateWithFlags(&h->ev_ready, cudaEventDisableTiming));
-  SW_CUDA(cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming));
-#undef SW_CUDA
+  OSB_TRY(h->res.stream(&h->side));
+  OSB_TRY(h->res.event(&h->ev_ready, cudaEventDisableTiming));
+  OSB_TRY(h->res.event(&h->ev_done, cudaEventDisableTiming));
   if (world > 1) {
     NcclApi* api = nccl_api();
     if (!api || !id) {
       set_error("osb_swarm_init", api ? "null unique id" : "libnccl.so.2 could not be opened");
-      osb_swarm_destroy(h);
       return OSB_ERR_INVALID;
     }
     ncclUniqueId uid;
@@ -206,13 +201,11 @@ extern "C" osb_status osb_swarm_init(osb_swarm** out, const uint8_t* id, int ran
     ncclResult_t r = api->CommInitRank(&h->comm, world, uid, rank);
     if (r != ncclSuccess) {
       set_error("osb_swarm_init: ncclCommInitRank", api->GetErrorString(r));
-      h->comm = nullptr;
-      osb_swarm_destroy(h);
       return OSB_ERR_CUDA;
     }
-    h->p2p = swarm_setup_p2p(h, api);
+    h->p2p = swarm_setup_p2p(h.get(), api);
   }
-  *out = h;
+  *out = h.release();
   return OSB_OK;
 }
 

@@ -21,8 +21,23 @@ def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
-class SuperPoint:
+class _Handle:
+    """One library handle in `self._h`: `close()`, also run when the object is collected, destroys it once."""
+
+    _destroy = ""        # name of the handle's osb_*_destroy
+
+    def close(self):
+        if getattr(self, "_h", None):
+            getattr(self._lib, self._destroy)(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+class SuperPoint(_Handle):
     """`inference(image) -> (keypoints [N,2] f32 (x,y) by descending confidence, descriptors [N,64])`."""
+
+    _destroy = "osb_superpoint_destroy"
 
     def __init__(self, weights: np.ndarray, pca_comp: np.ndarray, pca_mean: np.ndarray, width: int, height: int,
                  thres: float = 0.015, max_num: int = 200, max_batch: int = 8):
@@ -33,13 +48,6 @@ class SuperPoint:
         self._h = C.c_void_p()
         _l.check(self._lib.osb_superpoint_create(C.byref(self._h), _l.ptr(w), w.size, width, height, thres, max_num,
                                                  _l.ptr(pc), _l.ptr(pm), max_batch))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_superpoint_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def _outputs(self, B):
         return (np.zeros(B, np.int32), np.zeros((B, self.max_num, 2), np.float32),
@@ -92,8 +100,10 @@ class SuperPoint:
         return out
 
 
-class NetVLAD:
+class NetVLAD(_Handle):
     """`inference(image) -> [4096] f32` (mobilenetvlad_tensorrt.cpp:4-15)."""
+
+    _destroy = "osb_netvlad_destroy"
 
     def __init__(self, weights: np.ndarray, width: int, height: int, max_batch: int = 4):
         self._lib = _l.load()
@@ -101,13 +111,6 @@ class NetVLAD:
         w = _f32(weights).reshape(-1)
         self._h = C.c_void_p()
         _l.check(self._lib.osb_netvlad_create(C.byref(self._h), _l.ptr(w), w.size, width, height, max_batch))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_netvlad_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def inference_batch(self, images: np.ndarray) -> np.ndarray:
         images = np.ascontiguousarray(images, dtype=np.uint8)
@@ -120,21 +123,16 @@ class NetVLAD:
         return self.inference_batch(image[None])[0]
 
 
-class IndexFlatIP:
+class IndexFlatIP(_Handle):
     """faiss::IndexFlatIP look-alike: `add(x)`, `search(q, k) -> (D, I)`, `ntotal`."""
+
+    _destroy = "osb_db_destroy"
 
     def __init__(self, d: int, capacity: int = 16384):
         self._lib = _l.load()
         self.d = d
         self._h = C.c_void_p()
         _l.check(self._lib.osb_db_create(C.byref(self._h), d, capacity))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_db_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     @property
     def ntotal(self) -> int:
@@ -167,21 +165,16 @@ class IndexFlatIP:
         _l.check(self._lib.osb_db_reset(self._h))
 
 
-class BFMatcher:
+class BFMatcher(_Handle):
     """cv::BFMatcher(cv::NORM_L2, crossCheck=True): `match(query, train) -> (queryIdx, trainIdx, distance)`."""
+
+    _destroy = "osb_matcher_destroy"
 
     def __init__(self, max_pairs: int = 8, max_n: int = 200, dim: int = 64):
         self._lib = _l.load()
         self.max_pairs, self.max_n, self.dim = max_pairs, max_n, dim
         self._h = C.c_void_p()
         _l.check(self._lib.osb_matcher_create(C.byref(self._h), max_pairs, max_n, dim))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_matcher_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def match_batch(self, queries, trains):
         P = len(queries)
@@ -221,20 +214,15 @@ def homography_ransac(src_list, dst_list, thresh: float = 3.0, seed: int = 0):
     return [(mask[i, :n[i]].copy(), int(ninl[i]), int(win[i])) for i in range(n_pairs)]
 
 
-class PoseGraphSolver:
+class PoseGraphSolver(_Handle):
     """Flat-array form of SwarmLocalizationSolver::solve_once: `solve(graph) -> (poses, summary)`."""
+
+    _destroy = "osb_solver_destroy"
 
     def __init__(self, max_nodes: int = 4096, max_factors: int = 32768):
         self._lib = _l.load()
         self._h = C.c_void_p()
         _l.check(self._lib.osb_solver_create(C.byref(self._h), max_nodes, max_factors))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_solver_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def default_options(self) -> _l.SolveOptions:
         o = _l.SolveOptions()
@@ -368,8 +356,10 @@ class PoseGraphSolver:
         return r, Ja, Jb
 
 
-class KeyframeFrontend:
+class KeyframeFrontend(_Handle):
     """The per-keyframe pipeline (extract -> ingest -> query) on one GPU."""
+
+    _destroy = "osb_frontend_destroy"
 
     def __init__(self, sp_weights, pca_comp, pca_mean, nv_weights, width=640, height=480, n_dirs=4, max_num=200,
                  sp_thres=0.015, self_id=0, db_capacity=16384, inner_product_thres=0.3, init_mode_product_thres=0.2,
@@ -391,13 +381,6 @@ class KeyframeFrontend:
         self._h = C.c_void_p()
         _l.check(self._lib.osb_frontend_create(C.byref(self._h), C.byref(cfg), _l.ptr(spw), spw.size, _l.ptr(pc),
                                                _l.ptr(pm), _l.ptr(nvw), nvw.size))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_frontend_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def process(self, images_up: np.ndarray, images_down: np.ndarray, msg_id: int):
         """HOST images [n_dirs,H,W] u8 -> (KeyframeRecord, LoopResult); one synchronisation."""
@@ -594,10 +577,12 @@ def pcm_outlier_rejection(edges, pcm_thres: float, odom_pos_cov_per_m: float, od
     return (out, adj, smd) if want_matrices else out
 
 
-class Swarm:
+class Swarm(_Handle):
     """The swarm-wide keyframe exchange behind the C ABI (osb_swarm_*): one ncclAllGather of the fixed-size keyframe
     record per round; replaces LoopNet::broadcast_fisheye_desc / image_desc_callback (loop_net.cpp:20-120,142-172).
     `unique_id()` on rank 0, hand the 128 bytes to the other ranks, then `Swarm(id, rank, world)` everywhere."""
+
+    _destroy = "osb_swarm_destroy"
 
     @staticmethod
     def unique_id() -> bytes:
@@ -615,13 +600,6 @@ class Swarm:
         _l.check(self._lib.osb_swarm_init(C.byref(self._h), idbuf, rank, world))
         self.rank, self.world = rank, world
         self.transport = "p2p copy engines" if self._lib.osb_swarm_transport(self._h) == 1 else "nccl"
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.osb_swarm_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def exchange(self, record_dev: int, gathered_dev: int, stream: int):
         """this rank's record -> gathered[world] in rank order, enqueued on `stream` (osb_swarm_exchange)"""
@@ -790,3 +768,8 @@ def nv_head_parity(assign_w, assign_b, centroids, x):
 
 def launch_count() -> int:
     return int(_l.load().osb_launch_count())
+
+
+def live_resources() -> int:
+    """device buffers, pinned buffers, streams and events the library holds right now (osb_live_resources)"""
+    return int(_l.load().osb_live_resources())

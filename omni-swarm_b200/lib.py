@@ -101,6 +101,7 @@ _SIG = {
     "osb_version": (C.c_char_p, []),
     "osb_device_count": (C.c_int, []),
     "osb_launch_count": (C.c_int64, []),
+    "osb_live_resources": (C.c_int64, []),
     "osb_set_sm_budget": (None, [C.c_int]),
     "osb_superpoint_create": (C.c_int, [C.POINTER(_P), _P, C.c_size_t, C.c_int, C.c_int, C.c_float, C.c_int, _P, _P, C.c_int]),
     "osb_superpoint_destroy": (C.c_int, [_P]),

@@ -55,3 +55,25 @@ def test_product_never_imports_oracle():
             if f.endswith((".py", ".cu", ".cuh", ".h")):
                 src = open(os.path.join(dirpath, f)).read()
                 assert "import oracle" not in src and "from oracle" not in src, f
+
+
+RAW_ACQUIRE_RELEASE = re.compile(
+    r"\bcuda(Malloc|Free|HostAlloc|FreeHost|StreamCreate\w*|StreamDestroy|EventCreate\w*|EventDestroy)\s*\(")
+
+
+def test_cuda_resources_are_acquired_only_through_the_owner():
+    """Every device buffer, pinned buffer, stream and event is acquired and released by osb::Resources (common.cuh),
+    so that destroy and every error path free all of it.  The one exception is swarm.cu's copy-engine transport: the
+    IPC-exported inbox and the two buffers its handles are gathered through."""
+    csrc = os.path.join(ROOT, "omni-swarm_b200", "csrc")
+    raw = []
+    for f in sorted(os.listdir(csrc)):
+        if not f.endswith((".cu", ".cuh")) or f == "common.cuh":
+            continue
+        for i, line in enumerate(open(os.path.join(csrc, f)), 1):
+            if not RAW_ACQUIRE_RELEASE.search(line):
+                continue
+            if f == "swarm.cu" and re.search(r"\b(inbox|d_all|d_flag)\b", line):
+                continue
+            raw.append(f"{f}:{i}: {line.strip()}")
+    assert not raw, "raw CUDA acquire / release outside common.cuh:\n" + "\n".join(raw)
