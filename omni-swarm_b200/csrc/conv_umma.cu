@@ -24,6 +24,12 @@
 // HBM/L2 footprint as fp32 activations.  Measured against the oracle: see tests/test_gpu_superpoint.py.
 // Warp roles (384 threads): warpgroups 0-1 = MMA + epilogue, warpgroup 2 = producer (one elected thread issues the TMA
 // copies).  Persistent over tiles; the producer runs up to two A boxes and the weight ring ahead of the MMAs.
+//
+// The 64 -> 64 channel 3x3 layers (conv1b, conv2a, conv2b: 65 % of the network's MACs) run in conv_res64_kernel instead:
+// the 9 taps' weights stay resident in shared memory, and the GEMM is transposed, D[64 oc][128 px] = W * X^T, so that each
+// MMA is m64n128k16 with the weight slab as the 64-row operand and the whole tile's A box as the 128-column one (three
+// such MMAs read 18 KB of shared memory per 192 tensor clocks, where six m64n64k16 of the form above read 24 KB).  Each
+// consumer warpgroup computes whole tiles, alternating with the other, so that one's epilogue runs under the other's MMAs.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cmath>
@@ -50,17 +56,20 @@ constexpr int UM_CONSUMERS = 256;
 constexpr int UM_THREADS = UM_CONSUMERS + 128;
 constexpr int UM_PRODUCER_REGS = 40, UM_CONSUMER_REGS = 232;
 static_assert(128 * UM_PRODUCER_REGS + UM_CONSUMERS * UM_CONSUMER_REGS <= 65536, "register file");
-// RES = true (64 -> 64 channel 3x3 layers: conv1b, conv2a, conv2b = 65 % of the network's FLOPs): the 9 taps' weight
-// planes (144 KB) stay resident in shared memory for the CTA's whole life instead of streaming through a ring.
-template <int N, bool RES>
+constexpr int UM_A_RING = UM_A_SLOTS * 2 * UM_A_SLOT;            // 80 KB
+template <int N>
 struct UmmaCfg {
   static constexpr int B_BYTES = N * 128;                        // one weight plane of one tap / slab
   static constexpr int B_SLOT = 2 * B_BYTES;                     // hi + lo
-  static constexpr int B_SLOTS = RES ? 9 : (N <= 64) ? 6 : (N <= 80) ? 5 : 4;
-  static constexpr int A_RING = UM_A_SLOTS * 2 * UM_A_SLOT;      // 80 KB
-  static constexpr int SMEM_BYTES = A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static constexpr int B_SLOTS = (N <= 64) ? 6 : (N <= 80) ? 5 : 4;
+  static constexpr int SMEM_BYTES = UM_A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
 };
+// conv_res64_kernel: the 9 taps' weight planes (9 x 16 KB) stay resident in shared memory for the CTA's whole life
+constexpr int R64_W_PLANE = 64 * 128;                            // [64 oc][64 ch] fp16
+constexpr int R64_W_SLOT = 2 * R64_W_PLANE;                      // W_hi | W_lo of one tap
+constexpr int R64_SMEM_BYTES = UM_A_RING + 9 * R64_W_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
+static_assert(R64_SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
 
 struct UmmaArgs {
   const float* bias;       // [N]
@@ -82,15 +91,15 @@ struct UmmaArgs {
                            //    8x8 pixel shuffle straight into the heat map `out_f32` ([B][8H][8W])
 };
 
-template <int N, bool RES, bool SPLIT>
+template <int N, bool SPLIT>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
-  using Cfg = UmmaCfg<N, RES>;
+  using Cfg = UmmaCfg<N>;
   constexpr int AS = UM_A_SLOTS, BS = Cfg::B_SLOTS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t b_base = smem_base + Cfg::A_RING;
+  const uint32_t b_base = smem_base + UM_A_RING;
   const uint32_t bar_base = b_base + BS * Cfg::B_SLOT;                   // 8-byte barriers
   auto a_full = [&](int s) { return bar_base + 8u * s; };
   auto a_empty = [&](int s) { return bar_base + 8u * (AS + s); };
@@ -107,7 +116,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
   const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_ROW;   // bytes of one A plane box
 
   if (threadIdx.x == 0) {
-    // the empty barriers count one arrival per consumer warpgroup; with RES the b_full barriers are filled once
+    // the empty barriers count one arrival per consumer warpgroup
     for (int s = 0; s < AS; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 2); }
     for (int s = 0; s < BS; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -120,16 +129,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
   if (threadIdx.x >= UM_CONSUMERS) {
     const int pt = threadIdx.x - UM_CONSUMERS;             // producer thread
     setmaxnreg_dec<UM_PRODUCER_REGS>();
-    if (RES && pt < 32 && elect_one()) {
-      // all 9 taps (one 64-channel slab) once: slot t holds tap t.  Issued BEFORE the dependency wait: weights are
-      // constants, so under programmatic dependent launch they stream in while the previous layer is still draining.
-      for (int t = 0; t < 9; ++t) {
-        const uint32_t sb = b_base + t * Cfg::B_SLOT;
-        mbar_expect_tx(b_full(t), Cfg::B_SLOT);
-        tma_load_3d(sb, &tm_w_hi, b_full(t), 0, P.n_off, t);
-        tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(t), 0, P.n_off, t);
-      }
-    }
     // the activations are the previous kernel's output: wait for the whole grid we depend on (no-op without PDL)
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (pt < 32 && elect_one()) {
@@ -149,7 +148,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             tma_load_4d(sa, &tm_a_hi, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
             tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
             if (++as == AS) { as = 0; aph ^= 1; }
-            for (int ky = 0; ky < P.ks && !RES; ++ky) {
+            for (int ky = 0; ky < P.ks; ++ky) {
               mbar_wait(b_empty(bs), bph ^ 1);
               const uint32_t sb = b_base + bs * Cfg::B_SLOT;
               mbar_expect_tx(b_full(bs), Cfg::B_SLOT);
@@ -170,8 +169,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
     const bool signaller = (threadIdx.x & 127) == 0;
     int as = 0; uint32_t aph = 0;
     int bs = 0; uint32_t bph = 0;
-    if (RES)
-      for (int t = 0; t < 9; ++t) mbar_wait(b_full(t), 0);
     // buffers are released once the MMAs that read them have retired: one warpgroup arrival on each empty barrier.  The MMAs
     // of one vertical tap form one commit group, and a group's buffers (its weight slot; the A box after its last tap) are
     // released when the NEXT group has been issued and this one has completed -- so a warpgroup holds at most two weight
@@ -195,16 +192,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
           mbar_wait(a_full(as), aph);
           const uint32_t sa = smem_base + as * (2 * UM_A_SLOT) + cw * 1024;
           for (int ky = 0; ky < P.ks; ++ky) {
-            uint32_t sb;
-            int b_slot = -1;
-            if (RES) {
-              sb = b_base + (ky * 3 + kx) * Cfg::B_SLOT;
-            } else {
-              mbar_wait(b_full(bs), bph);
-              sb = b_base + bs * Cfg::B_SLOT;
-              b_slot = bs;
-              if (++bs == BS) { bs = 0; bph ^= 1; }
-            }
+            mbar_wait(b_full(bs), bph);
+            const uint32_t sb = b_base + bs * Cfg::B_SLOT;
+            const int b_slot = bs;
+            if (++bs == BS) { bs = 0; bph ^= 1; }
             // vertical tap ky reads the box from pixel row ky on; core matrices one pixel row (2048 B) apart
             const uint64_t a_hi = wgmma_desc_sw128(sa + ky * UM_ROW, UM_ROW);
             const uint64_t a_lo = wgmma_desc_sw128(sa + UM_A_SLOT + ky * UM_ROW, UM_ROW);
@@ -316,6 +307,208 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
           } else {
             if (in0) store(pix0, c, f[0], f[1]);
             if (in1) store(pix1, c, f[2], f[3]);
+          }
+        }
+      }
+    }
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------
+// 64 -> 64 channel 3x3 layers: weights resident, D[64 oc][128 px] = W * X^T, one warpgroup per tile
+// --------------------------------------------------------------------------------------------------------------
+// Per K step three wgmma m64n128k16: W_hi*X_hi -> main, W_lo*X_hi -> cross, W_hi*X_lo -> cross (the products and the
+// accumulators they go to of conv_umma_kernel, with M and N swapped).
+//   * M operand: the tap's weight slab [64 oc][64 ch] of a resident slot (K-major SWIZZLE_128B, 8-row groups 1024 B apart).
+//   * N operand: the whole 8 x 16 tile from the A box, one 128-byte row per pixel in row-major order, so the 16 8-pixel
+//     core-matrix groups are 1024 B apart; vertical tap ky starts at + ky * 2048 B as before.
+//   * D: warp w of a warpgroup holds output channels 16w + lane/4 and + 8; fragment register 4j + 2h + e is channel
+//     16w + 8h + lane/4 of pixel (j / 2, 8 (j & 1) + 2 (lane & 3) + e) of the tile: row y + 1 is n-group j + 2, so the
+//     fused 2x2 max-pool is all in the thread.
+// Tiles: the CTA's i-th tile belongs to warpgroup i & 1.  The producer fills one ring of two A boxes (hi + lo) in tile
+// order, three boxes per tile.  Each slot has one full barrier per warpgroup, so that a warpgroup's parity sequence counts
+// only its own boxes, and one empty barrier on which the single reader of a box arrives.
+__global__ void __launch_bounds__(UM_THREADS, 1)
+conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+                  const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
+  constexpr int AS = UM_A_SLOTS;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t w_base = smem_base + UM_A_RING;
+  const uint32_t bar_base = w_base + 9 * R64_W_SLOT;                     // 8-byte barriers
+  auto a_full = [&](int g, int s) { return bar_base + 8u * (g * AS + s); };
+  auto a_empty = [&](int s) { return bar_base + 8u * (2 * AS + s); };
+  auto w_full = [&](int t) { return bar_base + 8u * (3 * AS + t); };
+
+  const int lane = threadIdx.x & 31;
+  const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
+  const int n_tiles = P.B * tiles_x * tiles_y;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AS; ++s) { mbar_init(a_full(0, s), 1); mbar_init(a_full(1, s), 1); mbar_init(a_empty(s), 1); }
+    for (int t = 0; t < 9; ++t) mbar_init(w_full(t), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (threadIdx.x >= UM_CONSUMERS) {
+    const int pt = threadIdx.x - UM_CONSUMERS;
+    setmaxnreg_dec<UM_PRODUCER_REGS>();
+    if (pt < 32 && elect_one()) {
+      // all 9 taps once: slot t holds tap t.  Issued BEFORE the dependency wait: weights are constants, so under
+      // programmatic dependent launch they stream in while the previous layer is still draining.
+      for (int t = 0; t < 9; ++t) {
+        const uint32_t sw = w_base + t * R64_W_SLOT;
+        mbar_expect_tx(w_full(t), R64_W_SLOT);
+        tma_load_3d(sw, &tm_w_hi, w_full(t), 0, P.n_off, t);
+        tma_load_3d(sw + R64_W_PLANE, &tm_w_lo, w_full(t), 0, P.n_off, t);
+      }
+    }
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (pt < 32 && elect_one()) {
+      int as = 0; uint32_t aph = 0;
+      for (int i = 0, tile = blockIdx.x; tile < n_tiles; ++i, tile += gridDim.x) {
+        const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+        const int x0 = tx * UM_TW, y0 = ty * UM_TH;
+        for (int kx = 0; kx < 3; ++kx) {
+          mbar_wait(a_empty(as), aph ^ 1);
+          const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+          const uint32_t full = a_full(i & 1, as);
+          mbar_expect_tx(full, 2 * UM_A_SLOT);
+          tma_load_4d(sa, &tm_a_hi, full, 0, x0 + kx - 1, y0 - 1, b);
+          tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, full, 0, x0 + kx - 1, y0 - 1, b);
+          if (++as == AS) { as = 0; aph ^= 1; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<UM_CONSUMER_REGS>();
+    const int g = threadIdx.x >> 7;                          // warpgroup: the CTA's tiles of parity g
+    const int w = (threadIdx.x >> 5) & 3;                    // warp: output channels 16w .. 16w + 15
+    const int r = lane >> 2, t4 = lane & 3;
+    const bool signaller = (threadIdx.x & 127) == 0;
+    for (int t = 0; t < 9; ++t) mbar_wait(w_full(t), 0);
+    const float bias[2] = {__ldg(P.bias + P.n_off + 16 * w + r), __ldg(P.bias + P.n_off + 16 * w + 8 + r)};
+    uint32_t fph = 0;                                        // bit s: parity of this warpgroup's next box in slot s
+    for (int i = g, tile = blockIdx.x + g * gridDim.x; tile < n_tiles; i += 2, tile += 2 * gridDim.x) {
+      // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo
+      float acc[64], cross[64];
+#pragma unroll
+      for (int k = 0; k < 64; ++k) { acc[k] = 0.f; cross[k] = 0.f; }
+      uint32_t scale_d = 0;
+      int pend = -1;                                         // box to release once the last group that reads it retires
+      for (int kx = 0; kx < 3; ++kx) {
+        const int as = (3 * i + kx) % AS;                    // box kx of the CTA's i-th tile is the ring's (3i + kx)-th
+        mbar_wait(a_full(g, as), (fph >> as) & 1u);
+        fph ^= 1u << as;
+        const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+        for (int ky = 0; ky < 3; ++ky) {
+          const uint32_t sw = w_base + (ky * 3 + kx) * R64_W_SLOT;
+          const uint64_t w_hi = wgmma_desc_sw128(sw, 1024), w_lo = wgmma_desc_sw128(sw + R64_W_PLANE, 1024);
+          const uint64_t x_hi = wgmma_desc_sw128(sa + ky * UM_ROW, 1024);
+          const uint64_t x_lo = wgmma_desc_sw128(sa + UM_A_SLOT + ky * UM_ROW, 1024);
+#pragma unroll
+          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < UM_KC / 16; ++k) {
+            const uint64_t adv = (uint64_t)(k * 32 >> 4);
+            Wgmma<128>::mma(acc, w_hi + adv, x_hi + adv, scale_d);       // hi*hi -> main
+            Wgmma<128>::mma(cross, w_lo + adv, x_hi + adv, scale_d);     // lo*hi -> cross
+            Wgmma<128>::mma(cross, w_hi + adv, x_lo + adv, 1u);          // hi*lo -> cross
+            scale_d = 1;
+          }
+          wgmma_commit();
+#pragma unroll
+          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+          wgmma_wait<1>();
+          if (signaller && pend >= 0) mbar_arrive(a_empty(pend));
+          pend = (ky == 2) ? as : -1;
+        }
+      }
+      wgmma_wait<0>();
+      if (signaller) mbar_arrive(a_empty(pend));
+#pragma unroll
+      for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+
+      // ---- epilogue ----
+      const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+      const int x0 = tx * UM_TW, y0 = ty * UM_TH;
+      auto value = [&](int k, int h) {                       // fragment register k, channel half h
+        float a = fmaf(acc[k] + cross[k], P.inv_scale, bias[h]);
+        if (P.relu) a = fmaxf(a, 0.f);
+        if (P.relu == 2) a = fminf(a, 6.f);
+        return a;
+      };
+      // split a channel's values of two pixels into the planes and transpose the 8 x 8 (channel x pixel) blocks of the
+      // warp: afterwards lane l holds channels 2 (l % 4), + 1 of pixel l / 4, so a quad writes 16 contiguous bytes
+      auto split_t = [&](float v0, float v1, uint32_t& th, uint32_t& tl) {
+        const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
+        const __half2 hp = __floats2half2_rn(s0, s1);          // packed conversions: the roundings of two scalar ones
+        const float2 hf = __half22float2(hp);
+        const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+        th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
+        tl = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&lp));
+      };
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int cb = 16 * w + 8 * h;                       // first channel of the warp's 8-channel block
+        if (cb >= P.out_c) continue;                         // warp-uniform
+        const int c_own = P.n_off + cb + r, c_st = P.n_off + cb + 2 * t4;
+        if (P.pool) {
+          // pooled row py of the tile, pooled column 4k + t4 from n-groups j = 4py + k and j + 2
+          const int Hp = P.H >> 1, Wp = P.W >> 1;
+#pragma unroll
+          for (int py = 0; py < UM_TH / 2; ++py) {
+            float m[2];
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const int j = 4 * py + k;
+              m[k] = fmaxf(fmaxf(value(4 * j + 2 * h, h), value(4 * (j + 2) + 2 * h, h)),
+                           fmaxf(value(4 * j + 2 * h + 1, h), value(4 * (j + 2) + 2 * h + 1, h)));
+            }
+            const int gpy = ty * (UM_TH / 2) + py;
+            if (P.out_f32) {
+#pragma unroll
+              for (int k = 0; k < 2; ++k) {
+                const int gpx = tx * (UM_TW / 2) + 4 * k + t4;
+                if (gpy < Hp && gpx < Wp)
+                  P.out_f32[(((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_own] = m[k];
+              }
+            } else {
+              // column 2 t4 + k of the block is pooled pixel 4k + t4: after the transpose lane l holds pixel
+              // 4 ((l / 4) & 1) + (l / 4) / 2
+              uint32_t th, tl;
+              split_t(m[0], m[1], th, tl);
+              const int gpx = tx * (UM_TW / 2) + 4 * (r & 1) + (r >> 1);
+              if (gpy < Hp && gpx < Wp) {
+                const size_t o = (((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_st;
+                *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
+                *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
+              }
+            }
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int gy = y0 + (j >> 1), xb = x0 + 8 * (j & 1);
+            const float v0 = value(4 * j + 2 * h, h), v1 = value(4 * j + 2 * h + 1, h);
+            if (P.out_f32) {
+              const int gx = xb + 2 * t4;
+              const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_own;
+              if (gy < P.H && gx < P.W) P.out_f32[o] = v0;
+              if (gy < P.H && gx + 1 < P.W) P.out_f32[o + P.out_cstride] = v1;
+            } else {
+              uint32_t th, tl;
+              split_t(v0, v1, th, tl);
+              const int gx = xb + r;
+              if (gy < P.H && gx < P.W) {
+                const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_st;
+                *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
+                *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
+              }
+            }
           }
         }
       }
@@ -507,24 +700,31 @@ osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half*
 // take the SMs the concurrent NetVLAD stream of the front-end would otherwise fill.
 static const bool g_conv_pdl = [] { const char* e = getenv("OSB_CONV_PDL"); return e && atoi(e) != 0; }();
 
-template <int N, bool RES, bool SPLIT = false>
-static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
-                              cudaStream_t st, int max_ctas, bool box128 = false) {
-  using Cfg = UmmaCfg<N, RES>;
-  OSB_SMEM_OPT_IN((conv_umma_kernel<N, RES, SPLIT>), Cfg::SMEM_BYTES);
+// one instantiation per kernel: the shared-memory opt-in is remembered per instantiation
+template <auto kernel>
+static osb_status launch_persistent(int smem_bytes, const CUtensorMap& a_hi, const CUtensorMap& a_lo,
+                                    const CUtensorMap& w_hi, const CUtensorMap& w_lo, const UmmaArgs& P, cudaStream_t st,
+                                    int max_ctas) {
+  OSB_SMEM_OPT_IN(kernel, smem_bytes);
   const int tiles = P.B * cdiv(P.W, UM_TW) * cdiv(P.H, UM_TH) * P.n_split;
   // persistent CTAs, one per SM; `max_ctas` leaves SMs free for a kernel running beside this one on another stream
   const int grid = std::min(tiles, persistent_ctas(max_ctas));
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(UM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = st;
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(UM_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = g_conv_pdl ? 1 : 0;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  OSB_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<N, RES, SPLIT>, a_hi, a_lo, box128 ? L.tm_hi128 : L.tm_hi,
-                              box128 ? L.tm_lo128 : L.tm_lo, P));
+  OSB_CUDA(cudaLaunchKernelEx(&cfg, kernel, a_hi, a_lo, w_hi, w_lo, P));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return OSB_OK;
+}
+
+template <int N, bool SPLIT = false>
+static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
+                              cudaStream_t st, int max_ctas, bool box128 = false) {
+  return launch_persistent<conv_umma_kernel<N, SPLIT>>(UmmaCfg<N>::SMEM_BYTES, a_hi, a_lo,
+                           box128 ? L.tm_hi128 : L.tm_hi, box128 ? L.tm_lo128 : L.tm_lo, P, st, max_ctas);
 }
 
 // the arguments that follow from the layer and its input; the caller adds the output and the epilogue
@@ -545,14 +745,15 @@ osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const 
   P.out_scale = out_scale; P.relu = relu; P.pool = pool;
   switch (L.n_pad) {
     case 64:
-      if (L.ks == 3 && L.cin == UM_KC) return launch_umma<64, true>(a_hi, a_lo, L, P, st, max_ctas);   // weights resident
-      return launch_umma<64, false>(a_hi, a_lo, L, P, st, max_ctas);
-    case 80: return launch_umma<80, false>(a_hi, a_lo, L, P, st, max_ctas);
-    case 128: return launch_umma<128, false>(a_hi, a_lo, L, P, st, max_ctas);
+      if (L.ks == 3 && L.cin == UM_KC)            // weights resident, transposed GEMM
+        return launch_persistent<conv_res64_kernel>(R64_SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st, max_ctas);
+      return launch_umma<64>(a_hi, a_lo, L, P, st, max_ctas);
+    case 80: return launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
+    case 128: return launch_umma<128>(a_hi, a_lo, L, P, st, max_ctas);
     case 256:                                     // 2 / 4 items of 128 channels per tile (a 256-wide accumulator pair
     case 512:                                     // would not fit a warpgroup's registers)
       P.n_split = L.n_pad / 128;
-      return launch_umma<128, false, true>(a_hi, a_lo, L, P, st, max_ctas, true);
+      return launch_umma<128, true>(a_hi, a_lo, L, P, st, max_ctas, true);
   }
   set_error("umma_conv_forward", "unsupported N");
   return OSB_ERR_INVALID;
@@ -565,7 +766,7 @@ osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi
   OSB_REQUIRE(L.n_pad == 80 && L.cout == 65 && L.ks == 1, "fused detector head expects the 65-logit 1x1 layer");
   UmmaArgs P = umma_args(L, B, H, W, act_scale);
   P.out_f32 = semi; P.out_c = 80; P.out_cstride = 80; P.out_scale = 1.f; P.epi = 1;
-  return launch_umma<80, false>(a_hi, a_lo, L, P, st, max_ctas);
+  return launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
 }
 
 // depthwise 3x3 (pad 1, stride s) + bias + ReLU6 on fp32 NHWC input, output as split fp16 planes for the pointwise

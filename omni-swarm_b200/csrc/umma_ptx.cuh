@@ -66,6 +66,13 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accesses of an accumulator register across the asynchronous MMAs that own it
 __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// 8 x 8 matrix of b16 transposed across a CONVERGED warp: lane l holds row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1 (the
+// lower 16 bits), before and after
+__device__ __forceinline__ uint32_t movmatrix_trans(uint32_t a) {
+  uint32_t d;
+  asm volatile("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;" : "=r"(d) : "r"(a));
+  return d;
+}
 
 // D[64 x W] (+)= A[64 x 16] * B[W x 16]^T, f16 operands from shared memory (K-major descriptors), f32 accumulators in
 // registers (W / 2 per thread).  scale_d = 0 overwrites D.
