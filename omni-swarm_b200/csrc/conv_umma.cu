@@ -91,6 +91,26 @@ struct UmmaArgs {
                            //    8x8 pixel shuffle straight into the heat map `out_f32` ([B][8H][8W])
 };
 
+// 4 x 4 transpose of 32-bit words across the four lanes of a quad (t4 = lane % 4): on return v[k] is the word v[t4] of
+// quad lane k.  Round r takes word (t4 - r) % 4 from lane (t4 + r) % 4; all indices stay compile-time after unrolling.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t4) {
+  uint32_t o[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) o[k] = (k == t4) ? v[k] : 0u;
+#pragma unroll
+  for (int r = 1; r < 4; ++r) {
+    const int send = (t4 - r) & 3, from = (t4 + r) & 3;
+    uint32_t s = v[0];
+#pragma unroll
+    for (int k = 1; k < 4; ++k) s = (send == k) ? v[k] : s;
+    const uint32_t got = __shfl_sync(0xffffffffu, s, (threadIdx.x & 28) | from);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) o[k] = (from == k) ? got : o[k];
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) v[k] = o[k];
+}
+
 template <int N, bool SPLIT>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -287,6 +307,45 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             *reinterpret_cast<__half2*>(P.out_lo + pix * P.out_cstride + n_off + c) = lp;
           }
         };
+        if (N % 32 == 0 && !P.pool && !P.out_f32) {
+          // planes without pooling: the quad holds 8 channels (16 bytes) of its pixel for every block j.  Four blocks are
+          // transposed across the quad at a time so that each lane stores one block whole: one 16-byte store where the
+          // loop below issues four 4-byte ones
+#pragma unroll
+          for (int q = 0; q < N / 32; ++q) {
+            if (n_off - P.n_off + 32 * q >= P.out_c) continue;           // warp-uniform
+            uint32_t h[2][4], l[2][4];                                   // [pixel row][block 4q + k]
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const int j = 4 * q + k, c = 8 * j + 2 * t4;
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                float a0 = value(4 * j + 2 * r, c), a1 = value(4 * j + 2 * r + 1, c + 1);
+                if (P.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                if (P.relu == 2) { a0 = fminf(a0, 6.f); a1 = fminf(a1, 6.f); }
+                const float s0 = a0 * P.out_scale, s1 = a1 * P.out_scale;
+                const __half2 hp = __floats2half2_rn(s0, s1);        // the roundings of `store` below
+                const float2 hf = __half22float2(hp);
+                const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+                h[r][k] = *reinterpret_cast<const uint32_t*>(&hp);
+                l[r][k] = *reinterpret_cast<const uint32_t*>(&lp);
+              }
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) { quad_transpose(h[r], t4); quad_transpose(l[r], t4); }
+            const int cb = n_off + 8 * (4 * q + t4);                     // the block this lane stores
+            if (cb - P.n_off >= P.out_c) continue;
+            if (in0) {
+              *reinterpret_cast<uint4*>(P.out_hi + pix0 * P.out_cstride + cb) = make_uint4(h[0][0], h[0][1], h[0][2], h[0][3]);
+              *reinterpret_cast<uint4*>(P.out_lo + pix0 * P.out_cstride + cb) = make_uint4(l[0][0], l[0][1], l[0][2], l[0][3]);
+            }
+            if (in1) {
+              *reinterpret_cast<uint4*>(P.out_hi + pix1 * P.out_cstride + cb) = make_uint4(h[1][0], h[1][1], h[1][2], h[1][3]);
+              *reinterpret_cast<uint4*>(P.out_lo + pix1 * P.out_cstride + cb) = make_uint4(l[1][0], l[1][1], l[1][2], l[1][3]);
+            }
+          }
+          continue;
+        }
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
           if (n_off - P.n_off + 8 * j >= P.out_c) continue;            // warp-uniform
