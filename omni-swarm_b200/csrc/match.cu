@@ -23,6 +23,7 @@ constexpr int DB_CHUNK_MAX = 512;  // rows per CTA
 //     otherwise the host launches db_merge_kernel.
 constexpr int DB_MERGE_MAX = 3584;       // heads + k*k candidate keys must fit the 32 KB key buffer
 constexpr int DB_FUSE_KMAX = 16;
+constexpr size_t DB_SCAN_SMEM = 200 * 1024;   // db_scan_kernel's dynamic shared-memory opt-in: Q x (dim + DB_CHUNK_MAX) floats
 
 __device__ __forceinline__ unsigned long long db_key(float s, int64_t id) {
   if (id < 0) return ~0ull;
@@ -308,7 +309,7 @@ static osb_status launch_scan(const float* db, int64_t n, const int64_t* n_dev, 
     return OSB_OK;
   }
   const size_t smem = std::max(merge_bytes, ((size_t)Q * dim + (size_t)Q * DB_CHUNK_MAX) * sizeof(float));
-  OSB_SMEM_OPT_IN((db_scan_kernel<Q, R>), 200 * 1024);
+  OSB_SMEM_OPT_IN((db_scan_kernel<Q, R>), DB_SCAN_SMEM);
   OSB_LAUNCH((db_scan_kernel<Q, R>), grid, DB_THREADS, smem, st, db, n, n_dev, dim, q, nq, k, ps, pi, os, oi, done, fuse);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
@@ -338,8 +339,11 @@ osb_status db_search_device(const float* rows, int64_t n, const int64_t* n_dev, 
   const bool coop = (dim == DB_COOP_DIM) && chunk <= DB_COOP_CHUNK;
   if (coop) grid = (int)std::max<int64_t>(1, std::min<int64_t>(grid, n));
   const int fuse = (done != nullptr && k <= DB_FUSE_KMAX && grid <= DB_MERGE_MAX) ? 1 : 0;
-  for (int q0 = 0; q0 < nq; q0 += 8) {
-    const int nb = min(8, nq - q0);
+  // queries per pass: 8 while db_scan_kernel<8,4>'s query slab and score rows fit its shared memory (dim <= 5888),
+  // else 4, which fits up to dim 12288
+  const int pass = (8 * ((size_t)dim + DB_CHUNK_MAX) * sizeof(float) <= DB_SCAN_SMEM) ? 8 : 4;
+  for (int q0 = 0; q0 < nq; q0 += pass) {
+    const int nb = min(pass, nq - q0);
     const float* qp = q_dev + (size_t)q0 * dim;
     float* os = scores_dev + (size_t)q0 * k;
     int64_t* oi = ids_dev + (size_t)q0 * k;

@@ -1,7 +1,8 @@
 """Forward-error bounds of the fp32 CUDA-core kernels, and the float64 values they bound.
 
-The fp32 convolutions (csrc/conv_ffma.cu), NetVLAD's fused block 0 and its head (csrc/netvlad.cu) are compared element by
-element with a float64 reference of the same operation on the same fp32 inputs.  The bounds are the standard ones of
+The fp32 convolutions (csrc/conv_ffma.cu), NetVLAD's fused block 0 and its head (csrc/netvlad.cu), the keypoint
+descriptors (csrc/postproc.cu) and the database's inner products (csrc/match.cu) are compared element by element with a
+float64 reference of the same operation on the same fp32 inputs.  The bounds are the standard ones of
 fp32 arithmetic (Higham, Accuracy and Stability of Numerical Algorithms, ch. 3) with u = 2^-24 and
 gamma_n = n u / (1 - n u); they hold for ANY summation order and assume only what the build guarantees (no fast math:
 expf within 2 ulp, sqrtf and division correctly rounded):
@@ -13,7 +14,7 @@ expf within 2 ulp, sqrtf and division correctly rounded):
     per location) are checked normwise, not element by element.
 
 tests/test_fp32_bounds.py shows on the CPU that fp32 arithmetic stays within them and that defects exceed them;
-tests/test_gpu_fp32_stages.py applies them to the kernels.  Every function takes NHWC numpy arrays and computes in
+tests/test_gpu_fp32_stages.py, test_gpu_keypoints_descriptors.py and test_gpu_db_scan.py apply them to the kernels.  Every function takes NHWC numpy arrays and computes in
 torch float64 on `device` ("cpu" or "cuda"); results come back as float64 numpy arrays.
 """
 import numpy as np
@@ -217,6 +218,101 @@ def head_fp32(x, aw, ab, cent):
     return {"mu": mu.numpy(), "xn": xn.numpy(), "logits": z.numpy(), "assign": a.numpy(), "out": v.numpy()}
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# keypoint descriptors (sp_desc_norm_kernel, sp_desc_pca_kernel) and database inner products (db_scan kernels)
+# ---------------------------------------------------------------------------------------------------------------------
+def desc_taps(kpts, W, H, *, align_corners=False):
+    """grid_sample's bilinear taps of keypoints kpts [N,2] (x, y pixels) on the Wc x Hc cell map, in fp32 with ATen's
+    operation order, every step rounded to nearest as csrc/postproc.cu::bilinear_taps does: gx = 2 kx / W - 1,
+    ix = ((gx + 1) Wc - 1) / 2.  These are INPUTS of the float64 reference; their rounding is not charged to the kernel.
+    Returns (x0 [N], y0 [N], weights [N,4] for the taps (x0,y0), (x0+1,y0), (x0,y0+1), (x0+1,y0+1))."""
+    f = np.float32
+    one, two = f(1), f(2)
+    kx, ky = np.asarray(kpts, f)[:, 0], np.asarray(kpts, f)[:, 1]
+    Wc, Hc = W // 8, H // 8
+    gx = two * kx / f(W) - one
+    gy = two * ky / f(H) - one
+    if align_corners:
+        ix, iy = (gx + one) / two * f(Wc - 1), (gy + one) / two * f(Hc - 1)
+    else:
+        ix, iy = ((gx + one) * f(Wc) - one) / two, ((gy + one) * f(Hc) - one) / two
+    fx, fy = np.floor(ix), np.floor(iy)
+    ex, ey = fx + one, fy + one
+    w = np.stack([(ex - ix) * (ey - iy), (ix - fx) * (ey - iy), (ex - ix) * (iy - fy), (ix - fx) * (iy - fy)], 1)
+    return fx.astype(np.int64), fy.astype(np.int64), w.astype(f)
+
+
+def desc_tap_values(desc, x0, y0, *, clamp=False):
+    """the four tap values [N,4,256] of desc [256,Hc,Wc]: taps outside the map are 0 (zeros padding), or the nearest
+    cell's with clamp=True"""
+    C, Hc, Wc = desc.shape
+    d = np.asarray(desc, np.float64)
+    out = []
+    for dx, dy in ((0, 0), (1, 0), (0, 1), (1, 1)):
+        x, y = x0 + dx, y0 + dy
+        inside = (x >= 0) & (x < Wc) & (y >= 0) & (y < Hc)
+        v = d[:, np.clip(y, 0, Hc - 1), np.clip(x, 0, Wc - 1)].T          # [N,256]
+        out.append(v if clamp else v * inside[:, None])
+    return np.stack(out, 1)
+
+
+def desc_ref(desc, kpts, W, H, pca_comp, pca_mean, *, taps=None, n_norm=None):
+    """float64 descriptors of keypoints kpts [N,2] (computeDescriptors: bilinear sample, per-channel L2 norm over the N
+    keypoints, centre by the PCA mean, project) from the fp32 map desc [256,Hc,Wc] and fp32 tap weights (desc_taps), with
+    the element-wise bound of an fp32 computation in any summation order:
+      sample     v = sum_t w_t d_t                      e_v  = gamma_4 sum_t |w_t||d_t|
+      norm^2     q_c = sum_n v^2                        |dq| <= gamma_{N+1} sum (|v| + e_v)^2 + sum (2|v| e_v + e_v^2)
+      norm       cn = sqrt(q)                           rel(cn) <= |dq| / (2 q) + u
+      centred    z = v / cn - mu                        |dz| <= |v / cn| (rel(cn) + u) + e_v / cn + u |z|   (first order, x(1+2^-20))
+      output     y_o = sum_c z_c W_oc                   |dy| <= gamma_257 sum_c (|z| + |dz|) |W_oc| + sum_c |W_oc| |dz_c|
+    A channel whose norm is 0 makes every output NaN (0 / 0), as in the reference; its bound is then NaN too.
+    `taps` = (x0, y0, weights) overrides desc_taps (defect models); `n_norm` = the number of leading keypoints in the norm.
+    Returns (y64 [N,64], bound [N,64])."""
+    kpts = np.asarray(kpts, np.float32)
+    N = kpts.shape[0]
+    x0, y0, w = desc_taps(kpts, W, H) if taps is None else taps
+    dv = desc_tap_values(desc, x0, y0)                                      # [N,4,256]
+    w64 = np.asarray(w, np.float64)[..., None]
+    v = (w64 * dv).sum(1)                                                   # [N,256]
+    ev = gamma(4) * (np.abs(w64) * np.abs(dv)).sum(1)
+    nn = N if n_norm is None else n_norm
+    av = np.abs(v[:nn])
+    q = (v[:nn] ** 2).sum(0)
+    dq = gamma(nn + 1) * ((av + ev[:nn]) ** 2).sum(0) + (2 * av * ev[:nn] + ev[:nn] ** 2).sum(0)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        cn = np.sqrt(q)
+        rel_cn = dq / (2 * q) + U
+        vc = v / cn
+        z = vc - np.asarray(pca_mean, np.float64)[None]
+        dz = (np.abs(vc) * (rel_cn + U) + ev / cn + U * np.abs(z)) * (1 + 2.0 ** -20)
+    Wo = np.asarray(pca_comp, np.float64)                                   # [64,256]
+    y = z @ Wo.T
+    bound = gamma(257) * ((np.abs(z) + dz) @ np.abs(Wo).T) + dz @ np.abs(Wo).T
+    return y, bound
+
+
+def desc_fp32(desc, kpts, W, H, pca_comp, pca_mean):
+    """the descriptor chain in numpy fp32 in the kernels' order of operations (a second fp32 model beside the oracle's
+    torch grid_sample): taps summed nw, ne, sw, se; squares summed over keypoints; sum over channels by matmul"""
+    f = np.float32
+    x0, y0, w = desc_taps(kpts, W, H)
+    dv = desc_tap_values(desc, x0, y0).astype(f)
+    v = np.zeros((dv.shape[0], dv.shape[2]), f)
+    for t in range(4):
+        v = v + dv[:, t] * w[:, t:t + 1]
+    cn = np.sqrt((v * v).sum(0, dtype=f))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        z = v / cn - np.asarray(pca_mean, f)[None]
+    return z @ np.asarray(pca_comp, f).T
+
+
+def ip_ref(rows, q):
+    """float64 inner products s [nq, n] of fp32 rows [n, dim] and queries [nq, dim], and the bound of an fp32 dot
+    product in any order: |s' - s| <= gamma_dim sum_i |q_i x_i|"""
+    r, qq = np.asarray(rows, np.float64), np.asarray(q, np.float64)
+    return qq @ r.T, gamma(r.shape[1]) * (np.abs(qq) @ np.abs(r).T)
+
+
 def ratio(y, ref, bound):
     """max |y - ref| / bound; inf if y has a non-finite value, or the error is non-zero where the bound is 0"""
     y = np.asarray(y, np.float64)
@@ -269,3 +365,64 @@ def head_case(regime, B, h, w, seed=0):
         ab -= 120.0
         ab[DEAD] -= 300.0
     return x.astype(np.float32), ab, aw, cent
+
+
+DESC_MAPS = [(12, 8), (50, 26), (80, 60)]   # cell maps of 96x64, 400x208 and 640x480 images
+DESC_N = [1, 15, 16, 17, 31, 32, 33, 200, 8192]
+DESC_THRES = 0.015
+
+
+def window_coupled(L, others, W):
+    """whether flat address L lies in the 9x9 flat-address NMS window (column wrap included) of each of `others`"""
+    d = np.asarray(others, np.int64) - int(L)
+    return np.any([np.abs(d - k * W) <= 4 for k in range(-4, 5)], axis=0)
+
+
+def desc_case(Wc, Hc, N, cells="unit", seed=0):
+    """a heat-map [H,W] with exactly N NMS survivors and a descriptor map [256,Hc,Wc] (fp32).  The first survivors are
+    the corners and points on every edge, in the order (0,0), (W-1,H-1), the other corners, then edges, all at one
+    confidence (ties never suppress each other); the rest are interior points of a 5-pixel lattice with distinct lower
+    confidences, away from the edge points' windows.  cells: "unit" (unit-norm cells like the network's), "raw" (cell
+    norms spread over three decades) or "dead" (unit cells, channel 7 zero everywhere: a zero channel norm)."""
+    W, H = 8 * Wc, 8 * Hc
+    rng = np.random.default_rng(seed * 1000 + N)
+    xs = [W // 3, W // 2, 2 * W // 3]
+    ys = [H // 3, H // 2, 2 * H // 3]
+    edge = [(0, 0), (W - 1, H - 1), (W - 1, 0), (0, H - 1)] + [(x, 0) for x in xs] + [(x, H - 1) for x in xs] + \
+           [(0, y) for y in ys] + [(W - 1, y) for y in ys[1:]]
+    edge = edge[:N]
+    semi = np.zeros((H, W), np.float32)
+    flat = [y * W + x for x, y in edge]
+    for x, y in edge:
+        semi[y, x] = 0.9
+    n_in = N - len(edge)
+    if n_in:
+        gx, gy = np.meshgrid(np.arange(5, W - 8, 5), np.arange(5, H - 4, 5))
+        lat = (gy * W + gx).reshape(-1)
+        far = np.ones(lat.size, bool)
+        for L in flat:
+            far &= ~window_coupled(L, lat, W)
+        lat = lat[far]
+        assert lat.size >= n_in, "map too small for N"
+        lat = rng.choice(lat, n_in, replace=False)
+        conf = 0.02 + 0.85 * (rng.permutation(n_in) + 1) / (n_in + 1)
+        semi.reshape(-1)[lat] = conf.astype(np.float32)
+    desc = rng.standard_normal((256, Hc, Wc))
+    desc /= np.linalg.norm(desc, axis=0, keepdims=True)
+    # the cells under the LAST keypoint (lowest confidence; among the tied edge points the last in raster order) point
+    # almost along channel 5, so that keypoint carries a visible share of that channel's norm even at N = 8192
+    # (and, in "raw", have the largest norm)
+    scale = 10.0 ** rng.uniform(-1.5, 1.5, (1, Hc, Wc))
+    last = max(flat) if not n_in else int(lat[np.argmin(conf)])
+    x0, y0, _ = desc_taps(np.array([[last % W, last // W]]), W, H)
+    for dx in (0, 1):
+        for dy in (0, 1):
+            if 0 <= x0[0] + dx < Wc and 0 <= y0[0] + dy < Hc:
+                cell = desc[:, y0[0] + dy, x0[0] + dx] + 30.0 * np.eye(256)[5]
+                desc[:, y0[0] + dy, x0[0] + dx] = cell / np.linalg.norm(cell)
+                scale[0, y0[0] + dy, x0[0] + dx] = 10.0 ** 1.5
+    if cells == "raw":
+        desc *= scale
+    elif cells == "dead":
+        desc[7] = 0.0
+    return semi, desc.astype(np.float32)

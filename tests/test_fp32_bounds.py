@@ -190,3 +190,108 @@ def test_head_model_is_the_oracle():
     feats = x[0].permute(1, 2, 0).reshape(1, -1, 128).numpy()
     out = fb.head_fp32(feats, nvw["assign.weight"], nvw["assign.bias"], nvw["centroids"])["out"][0]
     assert np.abs(out - ref).max() < 1e-6
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# keypoint descriptors and database inner products (tests/test_gpu_keypoints_descriptors.py, tests/test_gpu_db_scan.py)
+# ---------------------------------------------------------------------------------------------------------------------
+def desc_defects(desc, kpts, W, H, comp, mean, max_num):
+    """float64 models of wrong descriptor kernels; each must leave the bound of fb.desc_ref at these shapes"""
+    N = len(kpts)
+    x0, y0, w = fb.desc_taps(kpts, W, H)
+    out = {}
+
+    def chain(v, n_norm=N, extra=None, centre=True, channels=256):
+        q = (v[:n_norm] ** 2).sum(0) + (0.0 if extra is None else extra)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            z = v / np.sqrt(q) - (mean.astype(np.float64) if centre else 0.0)
+        return z[:, :channels] @ comp.astype(np.float64)[:, :channels].T
+
+    def sample(taps, clamp=False):
+        return (np.asarray(taps[2], np.float64)[..., None] * fb.desc_tap_values(desc, taps[0], taps[1], clamp=clamp)).sum(1)
+
+    v = sample((x0, y0, w))
+    out["out-of-range taps clamped"] = chain(sample((x0, y0, w), clamp=True))
+    out["last keypoint dropped from the norm"] = chain(v, n_norm=N - 1)
+    if max_num > N:   # the unused slots of a zero-filled keypoint buffer sample at (0, 0)
+        out["norm over max_num slots"] = chain(v, extra=(max_num - N) * sample(fb.desc_taps(np.zeros((1, 2)), W, H))[0] ** 2)
+    out["last 8 PCA channels skipped"] = chain(v, channels=248)
+    out["mean not subtracted"] = chain(v, centre=False)
+    if W != H:
+        out["x and y swapped"] = chain(sample(fb.desc_taps(np.asarray(kpts)[:, ::-1], H, W)))
+    out["align_corners=True"] = chain(sample(fb.desc_taps(kpts, W, H, align_corners=True)))
+    return out
+
+
+DESC_CPU_CASES = [(m, n) for m in fb.DESC_MAPS for n in fb.DESC_N if n <= 200 or m == (80, 60)]
+
+
+@pytest.mark.parametrize("cells", ["unit", "raw"])
+@pytest.mark.parametrize("case", DESC_CPU_CASES, ids=lambda c: "{}x{}_N{}".format(*c[0], c[1]))
+def test_descriptor_bound(case, cells):
+    """the oracle's torch chain (grid_sample) and a numpy fp32 chain stay within fb.desc_ref's bound, element by element;
+    the fp32 tap weights reproduce grid_sample; every defect leaves the bound"""
+    from oracle import frontend_ref as fr
+    (Wc, Hc), N = case
+    W, H = 8 * Wc, 8 * Hc
+    comp, mean = synth.pca_matrices(0)
+    semi, desc = fb.desc_case(Wc, Hc, N, cells)
+    kpts, _ = fr.get_keypoints(semi, fb.DESC_THRES, 8192)
+    assert len(kpts) == N and tuple(kpts[0]) == (0, 0)
+    y64, bound = fb.desc_ref(desc, kpts, W, H, comp, mean)
+    assert np.isfinite(y64).all()
+    for name, y in (("torch", fr.compute_descriptors(desc, kpts, W, H, comp, mean)),
+                    ("numpy", fb.desc_fp32(desc, kpts, W, H, comp, mean))):
+        r = fb.ratio(y, y64, bound)
+        print(f"{case} {cells}: {name} fp32 {r:.2e} of the bound")
+        assert r <= 1.0, name
+    # fb.desc_taps is grid_sample's sampling: its samples agree with grid_sample's up to the sum's rounding and a few
+    # ulp of the tap coordinates (ATen's vectorised CPU path rounds the unnormalisation differently); align_corners=True
+    # does not
+    g = torch.zeros((1, 1, N, 2))
+    fk = torch.from_numpy(kpts)
+    g[0, 0, :, 0] = 2.0 * fk[:, 0] / W - 1
+    g[0, 0, :, 1] = 2.0 * fk[:, 1] / H - 1
+    gs = F.grid_sample(t32(desc)[None], g, mode="bilinear", padding_mode="zeros", align_corners=False)[0, :, 0].T.numpy()
+    for ac in (False, True):
+        x0, y0, w = fb.desc_taps(kpts, W, H, align_corners=ac)
+        dv = fb.desc_tap_values(desc, x0, y0)
+        v64 = (w.astype(np.float64)[..., None] * dv).sum(1)
+        tol = fb.gamma(4) * (np.abs(w.astype(np.float64))[..., None] * np.abs(dv)).sum(1) + \
+            8 * fb.U * max(Wc, Hc) * np.abs(desc).max(axis=(1, 2))
+        assert (fb.ratio(gs, v64, tol) <= 1.0) != ac
+    for name, y in desc_defects(desc, kpts, W, H, comp, mean, 8192).items():
+        r = fb.ratio(y, y64, bound)
+        print(f"{case} {cells}: {name} {r:.3g}x")
+        # one keypoint's channel norm is |v|, so v / cn = sign(v): a defect that only rescales its sample cannot show
+        if N > 1 or name not in SCALE_ONLY:
+            assert r > 1.0, name
+
+
+SCALE_ONLY = {"out-of-range taps clamped", "x and y swapped", "align_corners=True"}
+
+
+def test_descriptor_zero_channel_is_nan():
+    """a channel whose norm over the keypoints is 0 makes every output NaN, in the oracle and in the reference model"""
+    from oracle import frontend_ref as fr
+    comp, mean = synth.pca_matrices(0)
+    semi, desc = fb.desc_case(12, 8, 33, "dead")
+    kpts, _ = fr.get_keypoints(semi, fb.DESC_THRES, 8192)
+    y64, _ = fb.desc_ref(desc, kpts, 96, 64, comp, mean)
+    assert np.isnan(y64).all() and np.isnan(fr.compute_descriptors(desc, kpts, 96, 64, comp, mean)).all()
+
+
+@pytest.mark.parametrize("dim", [4, 256, 4096, 8192])
+def test_inner_product_bound(dim):
+    """fp32 dot products (torch and numpy, any order) within fb.ip_ref's bound; one term dropped or a row off by one ulp
+    in its largest element leaves it"""
+    rng = np.random.default_rng(dim)
+    rows = rng.standard_normal((300, dim)).astype(np.float32)
+    rows[100:200] = rows[0] + (1e-7 * rng.standard_normal((100, dim))).astype(np.float32)   # near ties
+    q = rng.standard_normal((5, dim)).astype(np.float32)
+    s64, bound = fb.ip_ref(rows, q)
+    assert fb.ratio((t32(q) @ t32(rows).T).numpy(), s64, bound) <= 1.0
+    assert fb.ratio(q @ rows.T, s64, bound) <= 1.0
+    assert fb.ratio(np.cumsum(q[:, None, :] * rows[None], axis=-1, dtype=np.float32)[..., -1], s64, bound) <= 1.0
+    dropped = q[:, :-1].astype(np.float64) @ rows[:, :-1].astype(np.float64).T
+    assert fb.ratio(dropped, s64, bound) > 1.0

@@ -156,3 +156,16 @@ def test_matcher_golden_and_ties(gpu):
     b = np.concatenate([a[:10], a[:10]], 0)
     qi, ti, dist = m.match(a, b)
     assert qi.tolist() == list(range(10)) and ti.tolist() == list(range(10)) and (dist == 0).all()
+
+
+def test_matcher_at_its_cap(gpu):
+    """max_n = 256, the largest the matcher accepts: 256 x 256 and 256 x 1 pairs, bit-exact"""
+    m = host.BFMatcher(max_pairs=2, max_n=256)
+    a = synth.local_descriptors(256, 50)
+    qs = [a, synth.local_descriptors(256, 51)]
+    ts = [synth.local_descriptors(256, 52, base=a), synth.local_descriptors(1, 53)]
+    for (qi, ti, dist), q, t in zip(m.match_batch(qs, ts), qs, ts):
+        rq, rt, rd = fr.bf_crosscheck(q, t)
+        assert np.array_equal(qi, rq) and np.array_equal(ti, rt) and np.array_equal(dist, rd)
+    assert len(rq) == 1
+    m.close()
