@@ -87,6 +87,18 @@ osb_status osb_superpoint_read(osb_superpoint* h, int what, int image, float* ou
  * convPb, convDa, convDb in milliseconds (CUDA events on the handle's stream). */
 osb_status osb_superpoint_set_profiling(osb_superpoint* h, int enable);
 osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int n);
+/* Network precision of the tensor-core path (SuperPoint, NetVLAD, and both networks of the front-end):
+ *  OSB_PRECISION_SPLIT_FP16 (the default): every operand is carried as two fp16 planes and each K step computes three
+ *    products, which matches an fp32 network to ~1e-6 relative;
+ *  OSB_PRECISION_FP16: plain fp16 operands (the precision of the reference's fp16 TensorRT engines): the hi planes only,
+ *    one product per K step, fp32 accumulation.  Heat-map and descriptors move by ~1e-3 (DESIGN.md section 3).
+ * The weights are uploaded once and both precisions read them; switching acquires nothing and is serialised with the
+ * handle's other calls, and switching back gives the outputs of a handle that never switched.  A handle created under
+ * OSB_SP_CONV=ffma (fp32 CUDA cores) accepts only OSB_PRECISION_SPLIT_FP16 (OSB_ERR_INVALID otherwise).  Everything
+ * outside the convolutions (conv1a's arithmetic, softmax, L2 norms, keypoints, NetVLAD's head) stays fp32. */
+#define OSB_PRECISION_SPLIT_FP16 0
+#define OSB_PRECISION_FP16 1
+osb_status osb_superpoint_set_precision(osb_superpoint* h, int precision);
 
 /* Convolution parity hooks (tests only): ONE layer of the tensor-core path, run by the same host functions and kernels
  * as the SuperPoint / NetVLAD networks, on caller-supplied operands.  Weights and biases are HOST fp32, OIHW; activation
@@ -112,6 +124,16 @@ osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8
 osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
                              int channels, int stride, int generic, float out_scale, void* out_hi, void* out_lo,
                              void* stream);
+/* The same three in OSB_PRECISION_FP16: one fp16 plane in_hi = fp16(s * x) in, one plane out_hi out (no lo planes). */
+osb_status osb_conv_layer_fp16_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
+                                      const void* in_hi, int batch, int height, int width, float act_scale, int relu,
+                                      int pool, int out_c, int out_cstride, int max_ctas, int mode, float* out_f32,
+                                      void* out_hi, float out_scale, void* stream);
+osb_status osb_conv_first_fp16_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch,
+                                      int height, int width, float act_scale, void* out_hi, void* stream);
+osb_status osb_dwconv_fp16_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
+                                  int width, int channels, int stride, int generic, float out_scale, void* out_hi,
+                                  void* stream);
 /* The same for the fp32 CUDA-core path (OSB_SP_CONV=ffma, and the layers both paths run in fp32); fp32 NHWC device
  * operands, act 0 none / 1 ReLU / 2 ReLU6:
  *  conv_ffma:       w [cout][cin][ks][ks] (cin a multiple of 8, ks 1 or 3), x [batch][H][W][cin] ->
@@ -144,6 +166,8 @@ osb_status osb_netvlad_create(osb_netvlad** out, const float* weights, size_t n_
 osb_status osb_netvlad_destroy(osb_netvlad* h);
 osb_status osb_netvlad_infer(osb_netvlad* h, const uint8_t* images, int batch, float* out);
 osb_status osb_netvlad_infer_dev(osb_netvlad* h, const uint8_t* images_dev, int batch, float* out_dev, void* stream);
+/* OSB_PRECISION_SPLIT_FP16 / OSB_PRECISION_FP16 of the pointwise convolutions (see osb_superpoint_set_precision) */
+osb_status osb_netvlad_set_precision(osb_netvlad* h, int precision);
 /* NetVLAD parity hooks (tests only): two parts of the network run by the host functions osb_netvlad_infer_dev calls,
  * conventions as the convolution hooks above (host OIHW weights, device fp32 NHWC activations, one synchronise):
  *  nv_block0: block 0 of the default path, depthwise 3x3 (dw_w [32][1][3][3]) + ReLU6 -> pointwise pw_w [64][32][1][1] +
@@ -595,6 +619,8 @@ osb_status osb_frontend_db_set_geometry(osb_frontend* h, int remote, int64_t fir
  * [4] add_to_database  [5] database scans (remote + local)  [6] acceptance rule + per-direction match  [7] unused */
 osb_status osb_frontend_set_profiling(osb_frontend* h, int enable);
 osb_status osb_frontend_stage_ms(osb_frontend* h, float* ms8);
+/* precision of both networks of the front-end (SuperPoint and NetVLAD; see osb_superpoint_set_precision) */
+osb_status osb_frontend_set_precision(osb_frontend* h, int precision);
 /* ------------------------------------------------------------------------------------------------------------
  * Swarm-wide keyframe exchange -- replaces LoopNet::broadcast_fisheye_desc / image_desc_callback
  *   (swarm_loop/src/loop_net.cpp:20-120,142-172; called from swarm_loop/src/swarm_loop.cpp:167): the LCM UDP multicast of

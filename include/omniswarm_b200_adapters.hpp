@@ -47,6 +47,8 @@ class SuperPointB200 {
   ~SuperPointB200() { osb_superpoint_destroy(h_); }
   SuperPointB200(const SuperPointB200&) = delete;
   SuperPointB200& operator=(const SuperPointB200&) = delete;
+  // OSB_PRECISION_SPLIT_FP16 (default) or OSB_PRECISION_FP16, the precision of the reference's fp16 engines
+  void set_precision(int precision) { check(osb_superpoint_set_precision(h_, precision), "osb_superpoint_set_precision"); }
 
   // raw form: one 8-bit grey image [height][width]; keypoints as (x,y) pairs ordered by descending confidence
   void inference(const uint8_t* image, std::vector<std::pair<float, float>>& keypoints, std::vector<float>& local_descriptors) {
@@ -82,6 +84,7 @@ class MobileNetVLADB200 {
     check(osb_netvlad_create(&h_, weights.data(), weights.size(), width, height, 4), "osb_netvlad_create");
   }
   ~MobileNetVLADB200() { osb_netvlad_destroy(h_); }
+  void set_precision(int precision) { check(osb_netvlad_set_precision(h_, precision), "osb_netvlad_set_precision"); }
   std::vector<float> inference(const uint8_t* image) {
     std::vector<float> out(OSB_DEEP_DESC_SIZE);
     check(osb_netvlad_infer(h_, image, 1, out.data()), "osb_netvlad_infer");

@@ -56,20 +56,36 @@ constexpr int UM_CONSUMERS = 256;
 constexpr int UM_THREADS = UM_CONSUMERS + 128;
 constexpr int UM_PRODUCER_REGS = 40, UM_CONSUMER_REGS = 232;
 static_assert(128 * UM_PRODUCER_REGS + UM_CONSUMERS * UM_CONSUMER_REGS <= 65536, "register file");
-constexpr int UM_A_RING = UM_A_SLOTS * 2 * UM_A_SLOT;            // 80 KB
-template <int N>
+// FP16 = true is the plain-fp16 form of every kernel below (OSB_PRECISION_FP16): only the hi planes are read and written,
+// one MMA per K step.  Its slots hold one plane, so the same 80 KB ring carries four A boxes and the weight ring twice
+// the slots of the split form (B_SLOT = B_BYTES).
+template <int N, bool FP16 = false>
 struct UmmaCfg {
+  static constexpr int PLANES = FP16 ? 1 : 2;
+  static constexpr int A_SLOTS = FP16 ? 4 : UM_A_SLOTS;
+  static constexpr int A_RING = A_SLOTS * PLANES * UM_A_SLOT;    // 80 KB either way
   static constexpr int B_BYTES = N * 128;                        // one weight plane of one tap / slab
-  static constexpr int B_SLOT = 2 * B_BYTES;                     // hi + lo
-  static constexpr int B_SLOTS = (N <= 64) ? 6 : (N <= 80) ? 5 : 4;
-  static constexpr int SMEM_BYTES = UM_A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static constexpr int B_SLOT = PLANES * B_BYTES;                // hi (+ lo)
+  static constexpr int B_SLOTS = FP16 ? ((N <= 64) ? 12 : (N <= 80) ? 10 : 8) : ((N <= 64) ? 6 : (N <= 80) ? 5 : 4);
+  static constexpr int SMEM_BYTES = A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
+  static_assert(2 * (A_SLOTS + B_SLOTS) * 8 <= 256, "barriers exceed their 256 bytes");
 };
-// conv_res64_kernel: the 9 taps' weight planes (9 x 16 KB) stay resident in shared memory for the CTA's whole life
-constexpr int R64_W_PLANE = 64 * 128;                            // [64 oc][64 ch] fp16
-constexpr int R64_W_SLOT = 2 * R64_W_PLANE;                      // W_hi | W_lo of one tap
-constexpr int R64_SMEM_BYTES = UM_A_RING + 9 * R64_W_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
-static_assert(R64_SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
+// conv_res64_kernel: the 9 taps' weight planes (9 x 16 KB, or 9 x 8 KB of W_hi in fp16) stay resident in shared memory
+// for the CTA's whole life.  The fp16 form spends the freed 72 KB on a ring of six hi boxes (120 KB): with three boxes per
+// tile, warpgroup 0's tiles always land in slots 0-2 and warpgroup 1's in slots 3-5, so the producer fills a warpgroup's
+// next tile while the other warpgroup still holds its own.
+template <bool FP16 = false>
+struct R64Cfg {
+  static constexpr int PLANES = FP16 ? 1 : 2;
+  static constexpr int A_SLOTS = FP16 ? 6 : UM_A_SLOTS;
+  static constexpr int A_RING = A_SLOTS * PLANES * UM_A_SLOT;
+  static constexpr int W_PLANE = 64 * 128;                       // [64 oc][64 ch] fp16
+  static constexpr int W_SLOT = PLANES * W_PLANE;                // W_hi (| W_lo) of one tap
+  static constexpr int SMEM_BYTES = A_RING + 9 * W_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
+  static_assert((3 * A_SLOTS + 9) * 8 <= 256, "barriers exceed their 256 bytes");
+};
 
 struct UmmaArgs {
   const float* bias;       // [N]
@@ -111,15 +127,16 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t4) {
   for (int k = 0; k < 4; ++k) v[k] = o[k];
 }
 
-template <int N, bool SPLIT>
+// FP16: the plain-fp16 form (UmmaCfg): tm_a_lo / tm_w_lo and P.out_lo are not used
+template <int N, bool SPLIT, bool FP16 = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
-  using Cfg = UmmaCfg<N>;
-  constexpr int AS = UM_A_SLOTS, BS = Cfg::B_SLOTS;
+  using Cfg = UmmaCfg<N, FP16>;
+  constexpr int AS = Cfg::A_SLOTS, BS = Cfg::B_SLOTS, A_STRIDE = Cfg::PLANES * UM_A_SLOT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t b_base = smem_base + UM_A_RING;
+  const uint32_t b_base = smem_base + Cfg::A_RING;
   const uint32_t bar_base = b_base + BS * Cfg::B_SLOT;                   // 8-byte barriers
   auto a_full = [&](int s) { return bar_base + 8u * s; };
   auto a_empty = [&](int s) { return bar_base + 8u * (AS + s); };
@@ -163,17 +180,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
           for (int cs = 0; cs < P.cin_slabs; ++cs) {
             // activation box: tile rows + vertical halo at the kx-shifted column, shared by the ks vertical taps
             mbar_wait(a_empty(as), aph ^ 1);
-            const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
-            mbar_expect_tx(a_full(as), 2 * a_box_bytes);
+            const uint32_t sa = smem_base + as * A_STRIDE;
+            mbar_expect_tx(a_full(as), Cfg::PLANES * a_box_bytes);
             tma_load_4d(sa, &tm_a_hi, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
-            tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
+            if constexpr (!FP16) tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(as), cs * UM_KC, x0 + kx - halo, y0 - halo, b);
             if (++as == AS) { as = 0; aph ^= 1; }
             for (int ky = 0; ky < P.ks; ++ky) {
               mbar_wait(b_empty(bs), bph ^ 1);
               const uint32_t sb = b_base + bs * Cfg::B_SLOT;
               mbar_expect_tx(b_full(bs), Cfg::B_SLOT);
               tma_load_3d(sb, &tm_w_hi, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
-              tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
+              if constexpr (!FP16) tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
               if (++bs == BS) { bs = 0; bph ^= 1; }
             }
           }
@@ -201,16 +218,16 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
       // two fragments of the same shape (N/2 registers each): main = hi*hi, cross = hi*lo + lo*hi.  Disjoint register sets --
-      // an MMA into part of another MMA's fragment would make the compiler serialize the wgmma pipeline
-      float acc[N / 2], cross[N / 2];
+      // an MMA into part of another MMA's fragment would make the compiler serialize the wgmma pipeline.  fp16: main only
+      float acc[N / 2], cross[FP16 ? 1 : N / 2];
 #pragma unroll
-      for (int i = 0; i < N / 2; ++i) { acc[i] = 0.f; cross[i] = 0.f; }
+      for (int i = 0; i < N / 2; ++i) { acc[i] = 0.f; if constexpr (!FP16) cross[i] = 0.f; }
       uint32_t scale_d = 0;
       int pend_a = -1, pend_b = -1;                          // buffers of the last committed group
       for (int kx = 0; kx < P.ks; ++kx) {
         for (int cs = 0; cs < P.cin_slabs; ++cs) {
           mbar_wait(a_full(as), aph);
-          const uint32_t sa = smem_base + as * (2 * UM_A_SLOT) + cw * 1024;
+          const uint32_t sa = smem_base + as * A_STRIDE + cw * 1024;
           for (int ky = 0; ky < P.ks; ++ky) {
             mbar_wait(b_full(bs), bph);
             const uint32_t sb = b_base + bs * Cfg::B_SLOT;
@@ -223,19 +240,21 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             // the warpgroup is converged again after the barrier waits: fence the accumulators here, right before the
             // tap's MMAs, so that no compiler-inserted fence lands on a divergent path and serializes the MMA pipeline
 #pragma unroll
-            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); if constexpr (!FP16) fence_operand(cross[i]); }
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < UM_KC / 16; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);     // advance 16 fp16 = 32 bytes inside the swizzle row
               Wgmma<N>::mma(acc, a_hi + adv, b_hi + adv, scale_d);        // hi*hi -> main
-              Wgmma<N>::mma(cross, a_hi + adv, b_lo + adv, scale_d);      // hi*lo -> cross
-              Wgmma<N>::mma(cross, a_lo + adv, b_hi + adv, 1u);           // lo*hi -> cross
+              if constexpr (!FP16) {
+                Wgmma<N>::mma(cross, a_hi + adv, b_lo + adv, scale_d);    // hi*lo -> cross
+                Wgmma<N>::mma(cross, a_lo + adv, b_hi + adv, 1u);         // lo*hi -> cross
+              }
               scale_d = 1;
             }
             wgmma_commit();
 #pragma unroll
-            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+            for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); if constexpr (!FP16) fence_operand(cross[i]); }
             wgmma_wait<1>();                                 // the previous group has retired
             release(pend_a, pend_b);
             pend_a = (ky == P.ks - 1) ? as : -1;
@@ -247,7 +266,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
       wgmma_wait<0>();
       release(pend_a, pend_b);
 #pragma unroll
-      for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); fence_operand(cross[i]); }
+      for (int i = 0; i < N / 2; ++i) { fence_operand(acc[i]); if constexpr (!FP16) fence_operand(cross[i]); }
 
       // ---- epilogue: registers [4j, 4j+1] hold channels 8j + 2*t4 + {0,1} of pixel (y, x), [4j+2, 4j+3] of (y+1, x) ----
       const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
@@ -255,7 +274,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
       const bool in0 = y < P.H && x < P.W, in1 = y + 1 < P.H && x < P.W;
       const size_t pix0 = ((size_t)b * P.H + y) * P.W + x, pix1 = pix0 + P.W;
       auto value = [&](int r, int c) {                       // r = register index of the main accumulator
-        return fmaf(acc[r] + cross[r], P.inv_scale, __ldg(P.bias + n_off + c));
+        if constexpr (FP16) return fmaf(acc[r], P.inv_scale, __ldg(P.bias + n_off + c));
+        else return fmaf(acc[r] + cross[r], P.inv_scale, __ldg(P.bias + n_off + c));
       };
       if (P.epi == 1) {
         // fused detector head (superpoint.ipynb:190-198): softmax over the 65 logits of a cell, which four lanes of a quad
@@ -301,10 +321,14 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
             const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
             // packed conversions (cvt.rn.f16x2.f32: the roundings of two scalar conversions)
             const __half2 hp = __floats2half2_rn(s0, s1);
-            const float2 hf = __half22float2(hp);
-            const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
-            *reinterpret_cast<__half2*>(P.out_hi + pix * P.out_cstride + n_off + c) = hp;
-            *reinterpret_cast<__half2*>(P.out_lo + pix * P.out_cstride + n_off + c) = lp;
+            if constexpr (FP16) {
+              *reinterpret_cast<__half2*>(P.out_hi + pix * P.out_cstride + n_off + c) = hp;
+            } else {
+              const float2 hf = __half22float2(hp);
+              const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+              *reinterpret_cast<__half2*>(P.out_hi + pix * P.out_cstride + n_off + c) = hp;
+              *reinterpret_cast<__half2*>(P.out_lo + pix * P.out_cstride + n_off + c) = lp;
+            }
           }
         };
         if (N % 32 == 0 && !P.pool && !P.out_f32) {
@@ -325,23 +349,29 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                 if (P.relu == 2) { a0 = fminf(a0, 6.f); a1 = fminf(a1, 6.f); }
                 const float s0 = a0 * P.out_scale, s1 = a1 * P.out_scale;
                 const __half2 hp = __floats2half2_rn(s0, s1);        // the roundings of `store` below
-                const float2 hf = __half22float2(hp);
-                const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
-                h[r][k] = *reinterpret_cast<const uint32_t*>(&hp);
-                l[r][k] = *reinterpret_cast<const uint32_t*>(&lp);
+                if constexpr (FP16) {
+                  h[r][k] = *reinterpret_cast<const uint32_t*>(&hp);
+                } else {
+                  const float2 hf = __half22float2(hp);
+                  const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+                  h[r][k] = *reinterpret_cast<const uint32_t*>(&hp);
+                  l[r][k] = *reinterpret_cast<const uint32_t*>(&lp);
+                }
               }
             }
 #pragma unroll
-            for (int r = 0; r < 2; ++r) { quad_transpose(h[r], t4); quad_transpose(l[r], t4); }
+            for (int r = 0; r < 2; ++r) { quad_transpose(h[r], t4); if constexpr (!FP16) quad_transpose(l[r], t4); }
             const int cb = n_off + 8 * (4 * q + t4);                     // the block this lane stores
             if (cb - P.n_off >= P.out_c) continue;
             if (in0) {
               *reinterpret_cast<uint4*>(P.out_hi + pix0 * P.out_cstride + cb) = make_uint4(h[0][0], h[0][1], h[0][2], h[0][3]);
-              *reinterpret_cast<uint4*>(P.out_lo + pix0 * P.out_cstride + cb) = make_uint4(l[0][0], l[0][1], l[0][2], l[0][3]);
+              if constexpr (!FP16)
+                *reinterpret_cast<uint4*>(P.out_lo + pix0 * P.out_cstride + cb) = make_uint4(l[0][0], l[0][1], l[0][2], l[0][3]);
             }
             if (in1) {
               *reinterpret_cast<uint4*>(P.out_hi + pix1 * P.out_cstride + cb) = make_uint4(h[1][0], h[1][1], h[1][2], h[1][3]);
-              *reinterpret_cast<uint4*>(P.out_lo + pix1 * P.out_cstride + cb) = make_uint4(l[1][0], l[1][1], l[1][2], l[1][3]);
+              if constexpr (!FP16)
+                *reinterpret_cast<uint4*>(P.out_lo + pix1 * P.out_cstride + cb) = make_uint4(l[1][0], l[1][1], l[1][2], l[1][3]);
             }
           }
           continue;
@@ -387,13 +417,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
 // Tiles: the CTA's i-th tile belongs to warpgroup i & 1.  The producer fills one ring of two A boxes (hi + lo) in tile
 // order, three boxes per tile.  Each slot has one full barrier per warpgroup, so that a warpgroup's parity sequence counts
 // only its own boxes, and one empty barrier on which the single reader of a box arrives.
+// FP16: one wgmma W_hi*X_hi per K step on hi-only boxes and resident W_hi (R64Cfg); tm_a_lo / tm_w_lo are not used.
+template <bool FP16 = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
-  constexpr int AS = UM_A_SLOTS;
+  using Cfg = R64Cfg<FP16>;
+  constexpr int AS = Cfg::A_SLOTS, A_STRIDE = Cfg::PLANES * UM_A_SLOT;
+  constexpr int R64_W_PLANE = Cfg::W_PLANE, R64_W_SLOT = Cfg::W_SLOT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w_base = smem_base + UM_A_RING;
+  const uint32_t w_base = smem_base + Cfg::A_RING;
   const uint32_t bar_base = w_base + 9 * R64_W_SLOT;                     // 8-byte barriers
   auto a_full = [&](int g, int s) { return bar_base + 8u * (g * AS + s); };
   auto a_empty = [&](int s) { return bar_base + 8u * (2 * AS + s); };
@@ -421,7 +455,7 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         const uint32_t sw = w_base + t * R64_W_SLOT;
         mbar_expect_tx(w_full(t), R64_W_SLOT);
         tma_load_3d(sw, &tm_w_hi, w_full(t), 0, P.n_off, t);
-        tma_load_3d(sw + R64_W_PLANE, &tm_w_lo, w_full(t), 0, P.n_off, t);
+        if constexpr (!FP16) tma_load_3d(sw + R64_W_PLANE, &tm_w_lo, w_full(t), 0, P.n_off, t);
       }
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -432,11 +466,11 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         const int x0 = tx * UM_TW, y0 = ty * UM_TH;
         for (int kx = 0; kx < 3; ++kx) {
           mbar_wait(a_empty(as), aph ^ 1);
-          const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+          const uint32_t sa = smem_base + as * A_STRIDE;
           const uint32_t full = a_full(i & 1, as);
-          mbar_expect_tx(full, 2 * UM_A_SLOT);
+          mbar_expect_tx(full, A_STRIDE);
           tma_load_4d(sa, &tm_a_hi, full, 0, x0 + kx - 1, y0 - 1, b);
-          tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, full, 0, x0 + kx - 1, y0 - 1, b);
+          if constexpr (!FP16) tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, full, 0, x0 + kx - 1, y0 - 1, b);
           if (++as == AS) { as = 0; aph ^= 1; }
         }
       }
@@ -451,36 +485,38 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     const float bias[2] = {__ldg(P.bias + P.n_off + 16 * w + r), __ldg(P.bias + P.n_off + 16 * w + 8 + r)};
     uint32_t fph = 0;                                        // bit s: parity of this warpgroup's next box in slot s
     for (int i = g, tile = blockIdx.x + g * gridDim.x; tile < n_tiles; i += 2, tile += 2 * gridDim.x) {
-      // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo
-      float acc[64], cross[64];
+      // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo.  fp16: main only
+      float acc[64], cross[FP16 ? 1 : 64];
 #pragma unroll
-      for (int k = 0; k < 64; ++k) { acc[k] = 0.f; cross[k] = 0.f; }
+      for (int k = 0; k < 64; ++k) { acc[k] = 0.f; if constexpr (!FP16) cross[k] = 0.f; }
       uint32_t scale_d = 0;
       int pend = -1;                                         // box to release once the last group that reads it retires
       for (int kx = 0; kx < 3; ++kx) {
         const int as = (3 * i + kx) % AS;                    // box kx of the CTA's i-th tile is the ring's (3i + kx)-th
         mbar_wait(a_full(g, as), (fph >> as) & 1u);
         fph ^= 1u << as;
-        const uint32_t sa = smem_base + as * (2 * UM_A_SLOT);
+        const uint32_t sa = smem_base + as * A_STRIDE;
         for (int ky = 0; ky < 3; ++ky) {
           const uint32_t sw = w_base + (ky * 3 + kx) * R64_W_SLOT;
           const uint64_t w_hi = wgmma_desc_sw128(sw, 1024), w_lo = wgmma_desc_sw128(sw + R64_W_PLANE, 1024);
           const uint64_t x_hi = wgmma_desc_sw128(sa + ky * UM_ROW, 1024);
           const uint64_t x_lo = wgmma_desc_sw128(sa + UM_A_SLOT + ky * UM_ROW, 1024);
 #pragma unroll
-          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
           wgmma_fence();
 #pragma unroll
           for (int k = 0; k < UM_KC / 16; ++k) {
             const uint64_t adv = (uint64_t)(k * 32 >> 4);
             Wgmma<128>::mma(acc, w_hi + adv, x_hi + adv, scale_d);       // hi*hi -> main
-            Wgmma<128>::mma(cross, w_lo + adv, x_hi + adv, scale_d);     // lo*hi -> cross
-            Wgmma<128>::mma(cross, w_hi + adv, x_lo + adv, 1u);          // hi*lo -> cross
+            if constexpr (!FP16) {
+              Wgmma<128>::mma(cross, w_lo + adv, x_hi + adv, scale_d);   // lo*hi -> cross
+              Wgmma<128>::mma(cross, w_hi + adv, x_lo + adv, 1u);        // hi*lo -> cross
+            }
             scale_d = 1;
           }
           wgmma_commit();
 #pragma unroll
-          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+          for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
           wgmma_wait<1>();
           if (signaller && pend >= 0) mbar_arrive(a_empty(pend));
           pend = (ky == 2) ? as : -1;
@@ -489,26 +525,33 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       wgmma_wait<0>();
       if (signaller) mbar_arrive(a_empty(pend));
 #pragma unroll
-      for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); fence_operand(cross[k]); }
+      for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
 
       // ---- epilogue ----
       const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
       const int x0 = tx * UM_TW, y0 = ty * UM_TH;
       auto value = [&](int k, int h) {                       // fragment register k, channel half h
-        float a = fmaf(acc[k] + cross[k], P.inv_scale, bias[h]);
+        float a;
+        if constexpr (FP16) a = fmaf(acc[k], P.inv_scale, bias[h]);
+        else a = fmaf(acc[k] + cross[k], P.inv_scale, bias[h]);
         if (P.relu) a = fmaxf(a, 0.f);
         if (P.relu == 2) a = fminf(a, 6.f);
         return a;
       };
       // split a channel's values of two pixels into the planes and transpose the 8 x 8 (channel x pixel) blocks of the
-      // warp: afterwards lane l holds channels 2 (l % 4), + 1 of pixel l / 4, so a quad writes 16 contiguous bytes
+      // warp: afterwards lane l holds channels 2 (l % 4), + 1 of pixel l / 4, so a quad writes 16 contiguous bytes.
+      // fp16: the hi plane only (tl is not written)
       auto split_t = [&](float v0, float v1, uint32_t& th, uint32_t& tl) {
         const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
         const __half2 hp = __floats2half2_rn(s0, s1);          // packed conversions: the roundings of two scalar ones
-        const float2 hf = __half22float2(hp);
-        const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
-        th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
-        tl = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&lp));
+        if constexpr (FP16) {
+          th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
+        } else {
+          const float2 hf = __half22float2(hp);
+          const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+          th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
+          tl = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&lp));
+        }
       };
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -544,7 +587,7 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               if (gpy < Hp && gpx < Wp) {
                 const size_t o = (((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_st;
                 *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
-                *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
+                if constexpr (!FP16) *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
               }
             }
           }
@@ -565,7 +608,7 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               if (gy < P.H && gx < P.W) {
                 const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_st;
                 *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
-                *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
+                if constexpr (!FP16) *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
               }
             }
           }
@@ -578,18 +621,22 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 // --------------------------------------------------------------------------------------------------------------
 // first layer (Cin = 1) and 2x2 max-pool on split planes, re-split after the fp32 op
 // --------------------------------------------------------------------------------------------------------------
+// FP16 (here and in the three kernels below): the fp32 arithmetic is the same, only the hi plane is written
+template <bool FP16>
 __device__ __forceinline__ void split_store8(__half* hi, __half* lo, const float* f, float scale) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const float s0 = f[2 * i] * scale, s1 = f[2 * i + 1] * scale;
     const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
-    const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
     h[i] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-    l[i] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+    if constexpr (!FP16) {
+      const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
+      l[i] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+    }
   }
   *reinterpret_cast<uint4*>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(lo) = make_uint4(l[0], l[1], l[2], l[3]);
+  if constexpr (!FP16) *reinterpret_cast<uint4*>(lo) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
 // conv1a (Cin = 1) + bias + ReLU -> split fp16 planes.  Thread = (8 output channels, one pixel column of a 32 x 8 tile):
@@ -599,6 +646,7 @@ __device__ __forceinline__ void split_store8(__half* hi, __half* lo, const float
 // a warp stores 4 pixels x 128 B contiguously per plane, no staging of the output.  The plane scale (a power of two) is
 // folded into weights and bias, and the 9 taps (ky-major) accumulate onto the bias.
 constexpr int CF_TW = 32, CF_TH = 8;
+template <bool FP16 = false>
 __global__ void __launch_bounds__(256)
 conv_first_split_kernel(const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ lut,
                         const uint8_t* __restrict__ img, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
@@ -651,13 +699,15 @@ conv_first_split_kernel(const float* __restrict__ w, const float* __restrict__ b
         }
         const float s0 = fmaxf(a0, 0.f), s1 = fmaxf(a1, 0.f);
         const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
-        const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
         h[j2] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-        l[j2] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+        if constexpr (!FP16) {
+          const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
+          l[j2] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+        }
       }
       const size_t chunk = (((size_t)b * H + y) * W + x) * 8 + cg;          // 16-byte chunk index inside the plane
       reinterpret_cast<uint4*>(out_hi)[chunk] = make_uint4(h[0], h[1], h[2], h[3]);
-      reinterpret_cast<uint4*>(out_lo)[chunk] = make_uint4(l[0], l[1], l[2], l[3]);
+      if constexpr (!FP16) reinterpret_cast<uint4*>(out_lo)[chunk] = make_uint4(l[0], l[1], l[2], l[3]);
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { in[0][k] = in[1][k]; in[1][k] = in[2][k]; }
@@ -779,12 +829,14 @@ static osb_status launch_persistent(int smem_bytes, const CUtensorMap& a_hi, con
   return OSB_OK;
 }
 
-template <int N, bool SPLIT = false>
+template <int N, bool SPLIT = false, bool FP16 = false>
 static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
                               cudaStream_t st, int max_ctas, bool box128 = false) {
-  return launch_persistent<conv_umma_kernel<N, SPLIT>>(UmmaCfg<N>::SMEM_BYTES, a_hi, a_lo,
+  return launch_persistent<conv_umma_kernel<N, SPLIT, FP16>>(UmmaCfg<N, FP16>::SMEM_BYTES, a_hi, a_lo,
                            box128 ? L.tm_hi128 : L.tm_hi, box128 ? L.tm_lo128 : L.tm_lo, P, st, max_ctas);
 }
+
+static bool precision_fp16(int precision) { return precision == OSB_PRECISION_FP16; }
 
 // the arguments that follow from the layer and its input; the caller adds the output and the epilogue
 static UmmaArgs umma_args(const UmmaLayer& L, int B, int H, int W, float act_scale) {
@@ -794,42 +846,52 @@ static UmmaArgs umma_args(const UmmaLayer& L, int B, int H, int W, float act_sca
   return P;
 }
 
-osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
-                             float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
-                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas) {
-  OSB_REQUIRE(!pool || (H % 2 == 0 && W % 2 == 0), "fused max-pool needs even H and W");
-  OSB_REQUIRE(out_c % 16 == 0 && out_c <= L.n_pad && out_cstride % 8 == 0, "tensor-core conv: bad output channel layout");
-  UmmaArgs P = umma_args(L, B, H, W, act_scale);
-  P.out_hi = out_hi; P.out_lo = out_lo; P.out_f32 = out_f32; P.out_c = out_c; P.out_cstride = out_cstride;
-  P.out_scale = out_scale; P.relu = relu; P.pool = pool;
+template <bool FP16>
+static osb_status umma_conv_launch(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, UmmaArgs& P,
+                                   cudaStream_t st, int max_ctas) {
   switch (L.n_pad) {
     case 64:
       if (L.ks == 3 && L.cin == UM_KC)            // weights resident, transposed GEMM
-        return launch_persistent<conv_res64_kernel>(R64_SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st, max_ctas);
-      return launch_umma<64>(a_hi, a_lo, L, P, st, max_ctas);
-    case 80: return launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
-    case 128: return launch_umma<128>(a_hi, a_lo, L, P, st, max_ctas);
+        return launch_persistent<conv_res64_kernel<FP16>>(R64Cfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st,
+                                                          max_ctas);
+      return launch_umma<64, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+    case 80: return launch_umma<80, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+    case 128: return launch_umma<128, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
     case 256:                                     // 2 / 4 items of 128 channels per tile (a 256-wide accumulator pair
     case 512:                                     // would not fit a warpgroup's registers)
       P.n_split = L.n_pad / 128;
-      return launch_umma<128, true>(a_hi, a_lo, L, P, st, max_ctas, true);
+      return launch_umma<128, true, FP16>(a_hi, a_lo, L, P, st, max_ctas, true);
   }
   set_error("umma_conv_forward", "unsupported N");
   return OSB_ERR_INVALID;
 }
 
+osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
+                             float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
+                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas, int precision) {
+  OSB_REQUIRE(!pool || (H % 2 == 0 && W % 2 == 0), "fused max-pool needs even H and W");
+  OSB_REQUIRE(out_c % 16 == 0 && out_c <= L.n_pad && out_cstride % 8 == 0, "tensor-core conv: bad output channel layout");
+  UmmaArgs P = umma_args(L, B, H, W, act_scale);
+  P.out_hi = out_hi; P.out_lo = out_lo; P.out_f32 = out_f32; P.out_c = out_c; P.out_cstride = out_cstride;
+  P.out_scale = out_scale; P.relu = relu; P.pool = pool;
+  return precision_fp16(precision) ? umma_conv_launch<true>(L, a_hi, a_lo, P, st, max_ctas)
+                                   : umma_conv_launch<false>(L, a_hi, a_lo, P, st, max_ctas);
+}
+
 // detector head: convPb (256 -> 65, 1x1) with the softmax + 8x8 pixel shuffle fused into the epilogue; `semi` is the heat
 // map [B][8H][8W]
 osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
-                                     float act_scale, float* semi, cudaStream_t st, int max_ctas) {
+                                     float act_scale, float* semi, cudaStream_t st, int max_ctas, int precision) {
   OSB_REQUIRE(L.n_pad == 80 && L.cout == 65 && L.ks == 1, "fused detector head expects the 65-logit 1x1 layer");
   UmmaArgs P = umma_args(L, B, H, W, act_scale);
   P.out_f32 = semi; P.out_c = 80; P.out_cstride = 80; P.out_scale = 1.f; P.epi = 1;
-  return launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
+  return precision_fp16(precision) ? launch_umma<80, false, true>(a_hi, a_lo, L, P, st, max_ctas)
+                                   : launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
 }
 
 // depthwise 3x3 (pad 1, stride s) + bias + ReLU6 on fp32 NHWC input, output as split fp16 planes for the pointwise
 // tensor-core conv that follows; one thread per (output pixel, 8 channels)
+template <bool FP16 = false>
 __global__ void dwconv3x3_split_kernel(const float* __restrict__ w, const float* __restrict__ bias,
                                        const float* __restrict__ x, __half* __restrict__ out_hi,
                                        __half* __restrict__ out_lo, int H, int W, int Ho, int Wo, int C, int stride,
@@ -859,12 +921,13 @@ __global__ void dwconv3x3_split_kernel(const float* __restrict__ w, const float*
     }
 #pragma unroll
   for (int j = 0; j < 8; ++j) a[j] = fminf(fmaxf(a[j] + bias[c + j], 0.f), 6.f);
-  split_store8(out_hi + (size_t)i * 8, out_lo + (size_t)i * 8, a, out_scale);
+  split_store8<FP16>(out_hi + (size_t)i * 8, out_lo + (size_t)i * 8, a, out_scale);
 }
 
 // stride-1 variant: one thread per (4 consecutive output pixels of a row, 8 channels).  The 3 x 6 input window is read
 // once (36 float4 instead of 72 for four single-pixel threads) and the 9 x 8 weights once per thread; same tap order per
 // output as the kernel above, so the planes are bit-identical.
+template <bool FP16 = false>
 __global__ void dwconv3x3_split_s1x4_kernel(const float* __restrict__ w, const float* __restrict__ bias,
                                             const float* __restrict__ x, __half* __restrict__ out_hi,
                                             __half* __restrict__ out_lo, int H, int W, int C, float out_scale,
@@ -926,31 +989,37 @@ __global__ void dwconv3x3_split_s1x4_kernel(const float* __restrict__ w, const f
 #pragma unroll
     for (int j = 0; j < 8; ++j) a[q][j] = fminf(fmaxf(a[q][j] + bb[j], 0.f), 6.f);
     const size_t o = ((((size_t)b * H + oy) * W + ox) * C8 + (c >> 3)) * 8;
-    split_store8(out_hi + o, out_lo + o, a[q], out_scale);
+    split_store8<FP16>(out_hi + o, out_lo + o, a[q], out_scale);
   }
 }
 
 osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const float* x, __half* out_hi, __half* out_lo,
-                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4) {
+                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4,
+                               int precision) {
   const int Ho = H / stride, Wo = W / stride;
+  const bool fp16 = precision_fp16(precision);
   if (stride == 1 && s1x4) {
     const int64_t total4 = (int64_t)B * H * ((W + 3) / 4) * (C / 8);
-    OSB_LAUNCH(dwconv3x3_split_s1x4_kernel, (unsigned)cdiv64(total4, 128), 128, 0, st, w_tap_c, bias, x, out_hi, out_lo,
-               H, W, C, out_scale, total4);
+    const auto kernel = fp16 ? dwconv3x3_split_s1x4_kernel<true> : dwconv3x3_split_s1x4_kernel<false>;
+    OSB_LAUNCH(kernel, (unsigned)cdiv64(total4, 128), 128, 0, st, w_tap_c, bias, x, out_hi, out_lo, H, W, C, out_scale,
+               total4);
     OSB_CHECK_LAUNCH();
     return OSB_OK;
   }
   const int64_t total = (int64_t)B * Ho * Wo * (C / 8);
-  OSB_LAUNCH(dwconv3x3_split_kernel, (unsigned)cdiv64(total, 256), 256, 0, st, w_tap_c, bias, x, out_hi, out_lo, H, W,
-             Ho, Wo, C, stride, out_scale, total);
+  const auto kernel = fp16 ? dwconv3x3_split_kernel<true> : dwconv3x3_split_kernel<false>;
+  OSB_LAUNCH(kernel, (unsigned)cdiv64(total, 256), 256, 0, st, w_tap_c, bias, x, out_hi, out_lo, H, W, Ho, Wo, C, stride,
+             out_scale, total);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }
 
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
-                              __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st) {
+                              __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st,
+                              int precision) {
   dim3 grid(cdiv(W, CF_TW), cdiv(H, CF_TH), B);
-  OSB_LAUNCH(conv_first_split_kernel, grid, 256, 0, st, w_tap_cout, bias, lut, img, out_hi, out_lo, H, W, out_scale);
+  const auto kernel = precision_fp16(precision) ? conv_first_split_kernel<true> : conv_first_split_kernel<false>;
+  OSB_LAUNCH(kernel, grid, 256, 0, st, w_tap_cout, bias, lut, img, out_hi, out_lo, H, W, out_scale);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }
@@ -962,15 +1031,12 @@ osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const 
 // --------------------------------------------------------------------------------------------------------------
 using namespace osb;
 
-extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
-                                            const void* in_hi, const void* in_lo, int batch, int height, int width,
-                                            float act_scale, int relu, int pool, int out_c, int out_cstride, int max_ctas,
-                                            int mode, float* out_f32, void* out_hi, void* out_lo, float out_scale,
-                                            void* stream) {
-  OSB_REQUIRE(w && bias && in_hi && in_lo, "null argument");
-  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (ks == 1 || ks == 3), "bad geometry");
-  OSB_REQUIRE(relu >= 0 && relu <= 2 && mode >= 0 && mode <= 2, "relu must be 0..2, mode 0 (fp32), 1 (planes) or 2 (softmax)");
-  OSB_REQUIRE(mode == 1 ? (out_hi && out_lo) : (out_f32 != nullptr), "null output");
+// the hooks below share these bodies; in plain fp16 (OSB_PRECISION_FP16) in_lo / out_lo are never read or written, and
+// the lo activation map is made over the hi plane
+static osb_status conv_layer_hook(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
+                                  const void* in_hi, const void* in_lo, int batch, int height, int width, float act_scale,
+                                  int relu, int pool, int out_c, int out_cstride, int max_ctas, int mode, float* out_f32,
+                                  void* out_hi, void* out_lo, float out_scale, void* stream, int precision) {
   OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
   Resources res;
@@ -980,20 +1046,17 @@ extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, i
   OSB_TRY(umma_layer_upload(res, &L, w, bias, cin, cout, ks, w_scale));
   OSB_TRY(umma_act_maps(&a_hi, &a_lo, (__half*)in_hi, (__half*)in_lo, batch, height, width, cin, ks));
   if (mode == 2)
-    OSB_TRY(umma_conv_softmax_forward(L, a_hi, a_lo, batch, height, width, act_scale, out_f32, st, max_ctas));
+    OSB_TRY(umma_conv_softmax_forward(L, a_hi, a_lo, batch, height, width, act_scale, out_f32, st, max_ctas, precision));
   else
     OSB_TRY(umma_conv_forward(L, a_hi, a_lo, batch, height, width, act_scale, mode == 1 ? (__half*)out_hi : nullptr,
                               mode == 1 ? (__half*)out_lo : nullptr, mode == 0 ? out_f32 : nullptr, out_c, out_cstride,
-                              out_scale, relu, pool, st, max_ctas));
+                              out_scale, relu, pool, st, max_ctas, precision));
   OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
 }
 
-extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch,
-                                            int height, int width, float act_scale, void* out_hi, void* out_lo,
-                                            void* stream) {
-  OSB_REQUIRE(w1a && b1a && images_dev && out_hi && out_lo, "null argument");
-  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+static osb_status conv_first_hook(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch, int height,
+                                  int width, float act_scale, void* out_hi, void* out_lo, void* stream, int precision) {
   OSB_TRY(require_device());
   const cudaStream_t st = (cudaStream_t)stream;
   Resources res;
@@ -1004,15 +1067,15 @@ extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, 
   OSB_TRY(upload_tap_major(res, &wd, w1a, 64));
   OSB_TRY(res.upload(&bd, b1a, 64));
   OSB_TRY(res.upload(&lut, l.data(), 256));
-  OSB_TRY(umma_first_forward(wd, bd, lut, images_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, act_scale, st));
+  OSB_TRY(umma_first_forward(wd, bd, lut, images_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, act_scale, st,
+                             precision));
   OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
 }
 
-extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
-                                        int width, int channels, int stride, int generic, float out_scale, void* out_hi,
-                                        void* out_lo, void* stream) {
-  OSB_REQUIRE(w && bias && x_dev && out_hi && out_lo, "null argument");
+static osb_status dwconv_hook(const float* w, const float* bias, const float* x_dev, int batch, int height, int width,
+                              int channels, int stride, int generic, float out_scale, void* out_hi, void* out_lo,
+                              void* stream, int precision) {
   OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0 && (stride == 1 || stride == 2),
               "bad geometry (channels must be a multiple of 8, stride 1 or 2)");
   OSB_TRY(require_device());
@@ -1023,7 +1086,65 @@ extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const
   OSB_TRY(upload_tap_major(res, &wd, w, channels));
   OSB_TRY(res.upload(&bd, bias, channels));
   OSB_TRY(umma_dwconv_forward(wd, bd, x_dev, (__half*)out_hi, (__half*)out_lo, batch, height, width, channels, stride,
-                              out_scale, st, !generic));
+                              out_scale, st, !generic, precision));
   OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
+}
+
+extern "C" osb_status osb_conv_layer_parity(const float* w, const float* bias, int cin, int cout, int ks, float w_scale,
+                                            const void* in_hi, const void* in_lo, int batch, int height, int width,
+                                            float act_scale, int relu, int pool, int out_c, int out_cstride, int max_ctas,
+                                            int mode, float* out_f32, void* out_hi, void* out_lo, float out_scale,
+                                            void* stream) {
+  OSB_REQUIRE(w && bias && in_hi && in_lo, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (ks == 1 || ks == 3), "bad geometry");
+  OSB_REQUIRE(relu >= 0 && relu <= 2 && mode >= 0 && mode <= 2, "relu must be 0..2, mode 0 (fp32), 1 (planes) or 2 (softmax)");
+  OSB_REQUIRE(mode == 1 ? (out_hi && out_lo) : (out_f32 != nullptr), "null output");
+  return conv_layer_hook(w, bias, cin, cout, ks, w_scale, in_hi, in_lo, batch, height, width, act_scale, relu, pool, out_c,
+                         out_cstride, max_ctas, mode, out_f32, out_hi, out_lo, out_scale, stream, OSB_PRECISION_SPLIT_FP16);
+}
+
+extern "C" osb_status osb_conv_layer_fp16_parity(const float* w, const float* bias, int cin, int cout, int ks,
+                                                 float w_scale, const void* in_hi, int batch, int height, int width,
+                                                 float act_scale, int relu, int pool, int out_c, int out_cstride,
+                                                 int max_ctas, int mode, float* out_f32, void* out_hi, float out_scale,
+                                                 void* stream) {
+  OSB_REQUIRE(w && bias && in_hi, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0 && (ks == 1 || ks == 3), "bad geometry");
+  OSB_REQUIRE(relu >= 0 && relu <= 2 && mode >= 0 && mode <= 2, "relu must be 0..2, mode 0 (fp32), 1 (planes) or 2 (softmax)");
+  OSB_REQUIRE(mode == 1 ? (out_hi != nullptr) : (out_f32 != nullptr), "null output");
+  return conv_layer_hook(w, bias, cin, cout, ks, w_scale, in_hi, in_hi, batch, height, width, act_scale, relu, pool, out_c,
+                         out_cstride, max_ctas, mode, out_f32, out_hi, nullptr, out_scale, stream, OSB_PRECISION_FP16);
+}
+
+extern "C" osb_status osb_conv_first_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch,
+                                            int height, int width, float act_scale, void* out_hi, void* out_lo,
+                                            void* stream) {
+  OSB_REQUIRE(w1a && b1a && images_dev && out_hi && out_lo, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+  return conv_first_hook(w1a, b1a, images_dev, batch, height, width, act_scale, out_hi, out_lo, stream,
+                         OSB_PRECISION_SPLIT_FP16);
+}
+
+extern "C" osb_status osb_conv_first_fp16_parity(const float* w1a, const float* b1a, const uint8_t* images_dev, int batch,
+                                                 int height, int width, float act_scale, void* out_hi, void* stream) {
+  OSB_REQUIRE(w1a && b1a && images_dev && out_hi, "null argument");
+  OSB_REQUIRE(batch > 0 && height > 0 && width > 0, "bad geometry");
+  return conv_first_hook(w1a, b1a, images_dev, batch, height, width, act_scale, out_hi, nullptr, stream, OSB_PRECISION_FP16);
+}
+
+extern "C" osb_status osb_dwconv_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
+                                        int width, int channels, int stride, int generic, float out_scale, void* out_hi,
+                                        void* out_lo, void* stream) {
+  OSB_REQUIRE(w && bias && x_dev && out_hi && out_lo, "null argument");
+  return dwconv_hook(w, bias, x_dev, batch, height, width, channels, stride, generic, out_scale, out_hi, out_lo, stream,
+                     OSB_PRECISION_SPLIT_FP16);
+}
+
+extern "C" osb_status osb_dwconv_fp16_parity(const float* w, const float* bias, const float* x_dev, int batch, int height,
+                                             int width, int channels, int stride, int generic, float out_scale,
+                                             void* out_hi, void* stream) {
+  OSB_REQUIRE(w && bias && x_dev && out_hi, "null argument");
+  return dwconv_hook(w, bias, x_dev, batch, height, width, channels, stride, generic, out_scale, out_hi, nullptr, stream,
+                     OSB_PRECISION_FP16);
 }

@@ -28,18 +28,24 @@ osb_status umma_layer_upload(Resources& res, UmmaLayer* L, const float* w_oihw, 
 osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half* p_lo, int B, int H, int W, int C,
                          int ks);
 // relu: 0 none, 1 ReLU, 2 ReLU6.  y = act(conv(x) + b), optionally followed by a fused 2x2 max-pool (pool = 1: output is [B][H/2][W/2][C]);
-// output either as split fp16 planes (out_hi/out_lo, scaled by out_scale) or as fp32
+// output either as split fp16 planes (out_hi/out_lo, scaled by out_scale) or as fp32.
+// precision (these four functions): OSB_PRECISION_SPLIT_FP16 (default) reads and writes both planes, OSB_PRECISION_FP16
+// only the hi planes (one MMA per K step; out_lo and the lo input planes are not touched).  The weights are the same.
 osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                              float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
-                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas = 0);
+                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas = 0,
+                             int precision = OSB_PRECISION_SPLIT_FP16);
 osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
-                                     float act_scale, float* semi, cudaStream_t st, int max_ctas = 0);
+                                     float act_scale, float* semi, cudaStream_t st, int max_ctas = 0,
+                                     int precision = OSB_PRECISION_SPLIT_FP16);
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
-                              __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st);
+                              __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st,
+                              int precision = OSB_PRECISION_SPLIT_FP16);
 osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
 // depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv).  Stride 1 runs
 // the four-pixel kernel unless s1x4 = false (the generic kernel; the planes are bit-identical)
 osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const float* x, __half* out_hi, __half* out_lo,
-                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4 = true);
+                               int B, int H, int W, int C, int stride, float out_scale, cudaStream_t st, bool s1x4 = true,
+                               int precision = OSB_PRECISION_SPLIT_FP16);
 }  // namespace osb

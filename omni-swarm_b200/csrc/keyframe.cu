@@ -511,6 +511,13 @@ extern "C" osb_status osb_frontend_create(osb_frontend** out, const osb_frontend
   return OSB_OK;
 }
 
+extern "C" osb_status osb_frontend_set_precision(osb_frontend* h, int precision) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(h->sp.set_precision(precision));            // the same check for both networks: nv accepts what sp accepted
+  return h->nv.set_precision(precision);
+}
+
 extern "C" osb_status osb_frontend_destroy(osb_frontend* h) {
   delete h;
   return OSB_OK;

@@ -354,15 +354,15 @@ osb_status NetVLAD::infer_dev(const uint8_t* img_dev, int B, float* out_dev, cud
     } else if (use_umma) {
       // depthwise (fp32 -> split planes) then pointwise on the tensor cores (planes -> fp32, or planes for the projection)
       OSB_TRY(umma_dwconv_forward(blk[i].dw, blk[i].dwb, cur, pl_hi[i], pl_lo[i], B, h, w, blk[i].cin, blk[i].stride,
-                                  NV_ACT_SCALE, st));
+                                  NV_ACT_SCALE, st, true, precision));
       h /= blk[i].stride; w /= blk[i].stride;
       if (i < 6) {
         OSB_TRY(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actA, blk[i].cout,
-                                  blk[i].cout, 1.f, 2, 0, st));
+                                  blk[i].cout, 1.f, 2, 0, st, 0, precision));
         cur = actA;
       } else {
         OSB_TRY(umma_conv_forward(upw[i], tmA[i], tmB[i], B, h, w, NV_ACT_SCALE, pl_hi[7], pl_lo[7], nullptr, blk[i].cout,
-                                  blk[i].cout, NV_ACT_SCALE, 2, 0, st));
+                                  blk[i].cout, NV_ACT_SCALE, 2, 0, st, 0, precision));
       }
     } else {
       OSB_TRY(dwconv3x3_forward(blk[i].dw, blk[i].dwb, actA, actB, B, h, w, blk[i].cin, blk[i].stride, ACT_RELU6, st));
@@ -371,7 +371,8 @@ osb_status NetVLAD::infer_dev(const uint8_t* img_dev, int B, float* out_dev, cud
     }
   }
   if (use_umma)
-    OSB_TRY(umma_conv_forward(uproj, tmA[7], tmB[7], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actB, NV_D, NV_D, 1.f, 0, 0, st));
+    OSB_TRY(umma_conv_forward(uproj, tmA[7], tmB[7], B, h, w, NV_ACT_SCALE, nullptr, nullptr, actB, NV_D, NV_D, 1.f, 0, 0, st,
+                              0, precision));
   else
     OSB_TRY(conv_forward(proj, actA, actB, B, h, w, NV_D, ACT_NONE, st));
   OSB_TRY(nv_head_forward(assign, centroids, actB, B, h, w, d_mu, d_assign, d_part, d_psum, out_dev, st));
@@ -410,6 +411,12 @@ extern "C" osb_status osb_netvlad_infer_dev(osb_netvlad* h, const uint8_t* image
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   return h->nv.infer_dev(images_dev, batch, out_dev, (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_netvlad_set_precision(osb_netvlad* h, int precision) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  std::lock_guard<std::mutex> lk(h->mu);
+  return h->nv.set_precision(precision);
 }
 
 extern "C" osb_status osb_netvlad_infer(osb_netvlad* h, const uint8_t* images, int batch, float* out) {

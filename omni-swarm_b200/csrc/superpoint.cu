@@ -125,9 +125,9 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
   // of layer `out_layer`
   auto conv = [&](int i, int h, int w, int out_layer, int pool) {
     return umma_conv_forward(UL[i], tmA[i], tmB[i], B, h, w, SA, in_hi[out_layer], in_lo[out_layer], nullptr,
-                             SP_COUT[i], SP_COUT[i], SA, 1, pool, st);
+                             SP_COUT[i], SP_COUT[i], SA, 1, pool, st, 0, precision);
   };
-  OSB_TRY(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st));   // conv1a            -> A
+  OSB_TRY(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st, precision));   // conv1a -> A
   mark(st);
   OSB_TRY(conv(1, H, W, 2, 1));                                                               // conv1b + pool     -> B
   mark(st);
@@ -146,10 +146,11 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
   OSB_TRY(conv(8, Hc, Wc, 9, 0));                                                             // convPa            -> A
   mark(st);
   if (fused_softmax) {
-    OSB_TRY(umma_conv_softmax_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, d_semi, st));      // convPb + softmax + pixel shuffle
+    OSB_TRY(umma_conv_softmax_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, d_semi, st, 0, precision));   // convPb + softmax + pixel shuffle
     mark(st);
   } else {
-    OSB_TRY(umma_conv_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, nullptr, nullptr, d_logits, 80, 80, 1.f, 0, 0, st));   // convPb
+    OSB_TRY(umma_conv_forward(UL[9], tmA[9], tmB[9], B, Hc, Wc, SA, nullptr, nullptr, d_logits, 80, 80, 1.f, 0, 0, st, 0,
+                              precision));   // convPb
     mark(st);
     OSB_TRY(sp_softmax_shuffle(d_logits, 80, d_semi, B, Hc, Wc, st));
   }
@@ -164,10 +165,10 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
     head_ctas = std::max(1, persistent_ctas() - B);
   }
   OSB_TRY(umma_conv_forward(UL[10], tmA[10], tmB[10], B, Hc, Wc, SA, in_hi[11], in_lo[11], nullptr, SP_COUT[10], SP_COUT[10],
-                            SA, 1, 0, st, head_ctas));                                        // convDa (reads B)  -> A
+                            SA, 1, 0, st, head_ctas, precision));                             // convDa (reads B)  -> A
   mark(st);
   OSB_TRY(umma_conv_forward(UL[11], tmA[11], tmB[11], B, Hc, Wc, SA, nullptr, nullptr, d_desc, 256, 256, 1.f, 0, 0, st,
-                            head_ctas));                                                      // convDb
+                            head_ctas, precision));                                           // convDb
   mark(st);
   OSB_TRY(l2norm_cells(d_desc, (int64_t)B * Hc * Wc, 256, st));
   if (fork) OSB_CUDA(cudaStreamWaitEvent(st, ev_kp, 0));
@@ -311,6 +312,12 @@ extern "C" osb_status osb_superpoint_set_profiling(osb_superpoint* h, int enable
   h->sp.layer_prof = enable != 0;
   h->sp.n_lev = 0;
   return OSB_OK;
+}
+
+extern "C" osb_status osb_superpoint_set_precision(osb_superpoint* h, int precision) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  std::lock_guard<std::mutex> lk(h->mu);
+  return h->sp.set_precision(precision);
 }
 
 extern "C" osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int n) {

@@ -9,6 +9,16 @@ namespace osb {
 size_t sp_expected_weights();
 size_t nv_expected_weights();
 
+// a network's precision switch: OSB_PRECISION_FP16 needs the tensor-core path (not OSB_SP_CONV=ffma)
+inline osb_status umma_set_precision(bool use_umma, int* precision, int p) {
+  OSB_REQUIRE(p == OSB_PRECISION_SPLIT_FP16 || p == OSB_PRECISION_FP16,
+              "precision must be OSB_PRECISION_SPLIT_FP16 or OSB_PRECISION_FP16");
+  OSB_REQUIRE(use_umma || p == OSB_PRECISION_SPLIT_FP16,
+              "plain fp16 needs the tensor-core convolutions (the handle was created under OSB_SP_CONV=ffma)");
+  *precision = p;
+  return OSB_OK;
+}
+
 struct SuperPoint {
   Resources res;                   // every buffer, stream and event below
   int W = 0, H = 0, Wc = 0, Hc = 0, max_num = 0, max_batch = 0, last_batch = 0;
@@ -26,6 +36,7 @@ struct SuperPoint {
 
   // tensor-core path (conv_umma.cu): weights as split fp16 planes, one pair of TMA descriptors per conv input
   bool use_umma = true;
+  int precision = OSB_PRECISION_SPLIT_FP16;   // of the tensor-core path; fp16 reads and writes the hi planes only
   UmmaLayer UL[12];
   CUtensorMap tmA[12], tmB[12];     // [layer] -> (hi, lo) descriptors of that layer's INPUT planes
   __half *in_hi[12] = {}, *in_lo[12] = {};
@@ -37,6 +48,7 @@ struct SuperPoint {
 
   osb_status init(const float* weights, size_t n_weights, int width, int height, float thres, int max_num,
                   const float* pca_comp, const float* pca_mean, int max_batch);
+  osb_status set_precision(int p) { return umma_set_precision(use_umma, &precision, p); }
   // keypoint extraction needs only the detector head: when a KpJob is passed, the network launches it on `kp_stream`
   // as soon as the heat map exists and runs the descriptor head beside it (on B fewer SMs); `st` re-joins before return
   struct KpJob { int32_t* nk; float* kpts; float* conf; };
@@ -67,12 +79,14 @@ struct NetVLAD {
   float *d_mu = nullptr, *d_part = nullptr, *d_psum = nullptr;
   // tensor-core pointwise path: blocks 1..6 and the projection read split fp16 planes written by the depthwise kernel
   bool use_umma = true;
+  int precision = OSB_PRECISION_SPLIT_FP16;
   UmmaLayer upw[7], uproj;
   CUtensorMap tmA[8], tmB[8];           // [block] (7 = projection) descriptors of the pointwise conv's input planes
   __half *pl_hi[8] = {}, *pl_lo[8] = {};
   __half* planes = nullptr;
 
   osb_status init(const float* weights, size_t n_weights, int width, int height, int max_batch);
+  osb_status set_precision(int p) { return umma_set_precision(use_umma, &precision, p); }
   osb_status infer_dev(const uint8_t* img_dev, int B, float* out_dev, cudaStream_t st);
 };
 

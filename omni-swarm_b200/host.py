@@ -21,6 +21,17 @@ def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
+PRECISIONS = {"split_fp16": _l.PRECISION_SPLIT_FP16, "fp16": _l.PRECISION_FP16}
+
+
+def _precision(name: str) -> int:
+    """'split_fp16' (the default: two fp16 planes per operand, fp32-level accuracy) or 'fp16' (plain fp16 operands, the
+    precision of the reference's fp16 TensorRT engines) -> OSB_PRECISION_*"""
+    if name not in PRECISIONS:
+        raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, not {name!r}")
+    return PRECISIONS[name]
+
+
 class _Handle:
     """One library handle in `self._h`: `close()`, also run when the object is collected, destroys it once."""
 
@@ -90,6 +101,10 @@ class SuperPoint(_Handle):
         _l.check(self._lib.osb_superpoint_set_profiling(self._h, 0))
         return {k: float(v) for k, v in zip(self.LAYERS, ms)}
 
+    def set_precision(self, precision: str):
+        """'split_fp16' (default) or 'fp16' for the network's tensor-core convolutions (osb_superpoint_set_precision)"""
+        _l.check(self._lib.osb_superpoint_set_precision(self._h, _precision(precision)))
+
     def read(self, what: str, image: int = 0) -> np.ndarray:
         H, W = self.height, self.width
         shapes = {"semi": (0, (H, W)), "desc": (1, (256, H // 8, W // 8)), "conf": (2, (self.max_num,)),
@@ -121,6 +136,10 @@ class NetVLAD(_Handle):
 
     def inference(self, image: np.ndarray) -> np.ndarray:
         return self.inference_batch(image[None])[0]
+
+    def set_precision(self, precision: str):
+        """'split_fp16' (default) or 'fp16' for the pointwise convolutions (osb_netvlad_set_precision)"""
+        _l.check(self._lib.osb_netvlad_set_precision(self._h, _precision(precision)))
 
 
 class IndexFlatIP(_Handle):
@@ -418,6 +437,10 @@ class KeyframeFrontend(_Handle):
     def set_profiling(self, enable: bool):
         _l.check(self._lib.osb_frontend_set_profiling(self._h, int(enable)))
 
+    def set_precision(self, precision: str):
+        """'split_fp16' (default) or 'fp16' for both networks of the front-end (osb_frontend_set_precision)"""
+        _l.check(self._lib.osb_frontend_set_precision(self._h, _precision(precision)))
+
     def stage_ms(self) -> dict:
         ms = np.zeros(8, np.float32)
         _l.check(self._lib.osb_frontend_stage_ms(self._h, _l.ptr(ms)))
@@ -675,6 +698,57 @@ def dwconv_parity(w, bias, x, out_scale: float, *, stride: int = 1, generic: boo
         _l.ptr(w), _l.ptr(b), C.c_void_p(x.data_ptr()), B, H, W, Cn, int(stride), int(generic), float(out_scale),
         C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()), C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
     return hi, lo
+
+
+def conv_layer_fp16_parity(w, bias, in_hi, act_scale: float, *, w_scale: float = 1024.0, relu: int = 0, pool: int = 0,
+                           out_c: int | None = None, out_cstride: int | None = None, max_ctas: int = 0, mode: str = "f32",
+                           out_scale: float = 1.0):
+    """conv_layer_parity in plain fp16 (osb_conv_layer_fp16_parity): one input plane in_hi = fp16(act_scale * x); mode
+    "planes" returns the one output plane [B,Ho,Wo,out_cstride] float16, "f32" / "softmax" as conv_layer_parity."""
+    import torch
+    w, b = _f32(w), _f32(bias)
+    cout, cin, ks = w.shape[0], w.shape[1], w.shape[2]
+    B, H, W, c = in_hi.shape
+    assert c == cin and in_hi.dtype == torch.float16 and in_hi.is_contiguous()
+    n_pad = 64 if cout <= 64 else 80 if cout <= 80 else 128 if cout <= 128 else 256 if cout <= 256 else 512
+    out_c = n_pad if out_c is None else out_c
+    out_cstride = out_c if out_cstride is None else out_cstride
+    Ho, Wo = (H // 2, W // 2) if pool else (H, W)
+    dev = in_hi.device
+    f32 = hi = None
+    if mode == "softmax":
+        f32 = torch.full((B, 8 * H, 8 * W), float("nan"), dtype=torch.float32, device=dev)
+    elif mode == "f32":
+        f32 = torch.full((B, Ho, Wo, out_cstride), float("nan"), dtype=torch.float32, device=dev)
+    else:
+        hi = torch.full((B, Ho, Wo, out_cstride), float("nan"), dtype=torch.float16, device=dev)
+    code = {"f32": 0, "planes": 1, "softmax": 2}[mode]
+    dp = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    _l.check(_l.load().osb_conv_layer_fp16_parity(
+        _l.ptr(w), _l.ptr(b), cin, cout, ks, float(w_scale), dp(in_hi), B, H, W, float(act_scale), int(relu), int(pool),
+        out_c, out_cstride, int(max_ctas), code, dp(f32), dp(hi), float(out_scale), _stream(dev)))
+    return hi if mode == "planes" else f32
+
+
+def conv_first_fp16_parity(w1a, b1a, images, act_scale: float):
+    """conv_first_parity in plain fp16 (osb_conv_first_fp16_parity): -> the hi plane [B,H,W,64] float16 only."""
+    import torch
+    B, H, W = images.shape
+    hi = torch.full((B, H, W, 64), float("nan"), dtype=torch.float16, device=images.device)
+    _l.check(_l.load().osb_conv_first_fp16_parity(_l.ptr(_f32(w1a)), _l.ptr(_f32(b1a)), C.c_void_p(images.data_ptr()), B,
+                                                  H, W, float(act_scale), C.c_void_p(hi.data_ptr()), _stream(images.device)))
+    return hi
+
+
+def dwconv_fp16_parity(w, bias, x, out_scale: float, *, stride: int = 1, generic: bool = False):
+    """dwconv_parity in plain fp16 (osb_dwconv_fp16_parity): -> the hi plane [B,H/stride,W/stride,C] float16 only."""
+    import torch
+    B, H, W, Cn = x.shape
+    hi = torch.full((B, H // stride, W // stride, Cn), float("nan"), dtype=torch.float16, device=x.device)
+    _l.check(_l.load().osb_dwconv_fp16_parity(_l.ptr(_f32(w)), _l.ptr(_f32(bias)), C.c_void_p(x.data_ptr()), B, H, W, Cn,
+                                              int(stride), int(generic), float(out_scale), C.c_void_p(hi.data_ptr()),
+                                              _stream(x.device)))
+    return hi
 
 
 _GUARD = 64          # floats after an fp32 hook output, pre-filled with NaN like the output: a store past the end shows

@@ -14,6 +14,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libomniswarm_b200.so")
 
 OK, ERR_INVALID, ERR_CUDA, ERR_CAPACITY, ERR_NO_DEVICE = 0, 1, 2, 3, 4
+PRECISION_SPLIT_FP16, PRECISION_FP16 = 0, 1
 MAX_DIRS, MAX_KPTS, FEATURE_DESC_SIZE, DEEP_DESC_SIZE = 4, 200, 64, 4096
 REMOTE_MAGIN_NUMBER = 1000000
 SWARM_ID_BYTES = 128
@@ -111,16 +112,24 @@ _SIG = {
     "osb_superpoint_read": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t]),
     "osb_superpoint_set_profiling": (C.c_int, [_P, C.c_int]),
     "osb_superpoint_layer_ms": (C.c_int, [_P, _P, C.c_int]),
+    "osb_superpoint_set_precision": (C.c_int, [_P, C.c_int]),
     "osb_conv_layer_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int,
                                         C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                         C.c_float, _P]),
     "osb_conv_first_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
     "osb_dwconv_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P,
                                     _P]),
+    "osb_conv_layer_fp16_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, C.c_int, C.c_int, C.c_int,
+                                             C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
+                                             C.c_float, _P]),
+    "osb_conv_first_fp16_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P]),
+    "osb_dwconv_fp16_parity": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P,
+                                         _P]),
     "osb_netvlad_create": (C.c_int, [C.POINTER(_P), _P, C.c_size_t, C.c_int, C.c_int, C.c_int]),
     "osb_netvlad_destroy": (C.c_int, [_P]),
     "osb_netvlad_infer": (C.c_int, [_P, _P, C.c_int, _P]),
     "osb_netvlad_infer_dev": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "osb_netvlad_set_precision": (C.c_int, [_P, C.c_int]),
     "osb_conv_ffma_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                        _P, _P]),
     "osb_conv_first_ffma_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
@@ -174,6 +183,7 @@ _SIG = {
     "osb_frontend_finish": (C.c_int, [_P, _P]),
     "osb_frontend_set_profiling": (C.c_int, [_P, C.c_int]),
     "osb_frontend_stage_ms": (C.c_int, [_P, _P]),
+    "osb_frontend_set_precision": (C.c_int, [_P, C.c_int]),
     "osb_frontend_db_size": (C.c_int64, [_P, C.c_int]),
     "osb_frontend_db_reset": (C.c_int, [_P]),
     "osb_frontend_db_load": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P]),
