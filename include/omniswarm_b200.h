@@ -569,6 +569,17 @@ osb_status osb_frontend_ingest_own(osb_frontend* h, const osb_keyframe_record* r
  * is written to `result_dev` (DEVICE).  init_mode / nonkeyframe as loop_detector.cpp:176. */
 osb_status osb_frontend_query(osb_frontend* h, const osb_keyframe_record* record_dev, int init_mode,
                               int nonkeyframe, osb_loop_result* result_dev, void* stream);
+/* query_from_database for keyframes received from other drones (loop_detector.cpp:98-119,191-195), a batch at once,
+ * e.g. the all-gather output of a round.  For every r != skip whose drone_id != self_id, results_dev[r] is what
+ * osb_frontend_query(h, records_dev + r, init_mode[r], 0, ...) would write at this point of `stream`.  Reads the local
+ * store only: the remote store, and whether the records have been ingested yet, do not affect the results.
+ * Records r == skip or with drone_id == self_id get the gate-closed result (hit_id -1, hit_score -1, accepted 0, every
+ * direction slot -1, n_matches 0; with the geometric filter n_geo 0 and geo_valid 0).  init_mode: HOST array [n_records]
+ * of 0/1 or NULL (all 0).  0 <= n_records <= 64 (the ingest limit); n_records == 0 does nothing.  The first call acquires
+ * the handle's scratch for 64 records (about 4 * 64 * max_num^2 floats); no later call allocates.  No host
+ * synchronisation.  nonkeyframe is not an argument: the reference ignores it for foreign keyframes (:191-195). */
+osb_status osb_frontend_query_received(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records, int skip,
+                                       const uint8_t* init_mode, osb_loop_result* results_dev, void* stream);
 /* the whole single-drone step with HOST buffers: extract + ingest(own) + query, one synchronisation at the end. */
 osb_status osb_frontend_process(osb_frontend* h, const uint8_t* images_up, const uint8_t* images_down,
                                 int32_t msg_id, osb_keyframe_record* record_host, osb_loop_result* result_host);

@@ -11,11 +11,13 @@ osb_status db_search_device(const float* rows, int64_t n, const int64_t* n_dev, 
                             int k, float* part_scores, int64_t* part_ids, unsigned int* done, float* scores_dev, int64_t* ids_dev,
                             cudaStream_t st);
 // q/t: device tables of n_pairs pointers to [<=max_n][64] descriptor blocks
-// outputs (qi/ti/dout/map_out) are [n_pairs][out_stride]
+// outputs (qi/ti/dout/map_out) are [n_pairs][out_stride] and n_out [n_pairs] -- or, with group > 0, pair p = group * g + s
+// writes them at g * group_stride + s * out_stride and g * group_stride + s (elements): the pairs of record g land in the
+// g-th of an array of structs
 osb_status bf_match_device(int n_pairs, int max_n, int out_stride, const float* const* q, const int32_t* nq,
                            const float* const* t,
                            const int32_t* nt, float* dist_scratch, int32_t* qi, int32_t* ti, float* dout,
-                           int32_t* n_out, int32_t* map_out, cudaStream_t st);
+                           int32_t* n_out, int32_t* map_out, cudaStream_t st, int group = 0, size_t group_stride = 0);
 
 // ---- conv_ffma.cu --------------------------------------------------------------------------------------------
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_RELU6 = 2 };

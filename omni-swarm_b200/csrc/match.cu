@@ -426,8 +426,9 @@ constexpr int BF_MAXN = 256;                       // max_n <= 256 (one thread p
 constexpr int BF_CC_THREADS = 1024;
 __global__ void __launch_bounds__(BF_CC_THREADS)
 bf_crosscheck_kernel(const float* __restrict__ dist, const int32_t* __restrict__ nq, const int32_t* __restrict__ nt,
-                     int max_n, int out_stride, int32_t* __restrict__ qi, int32_t* __restrict__ ti,
-                     float* __restrict__ dout, int32_t* __restrict__ n_out, int32_t* __restrict__ map_out) {
+                     int max_n, int out_stride, int group, size_t group_stride, int32_t* __restrict__ qi,
+                     int32_t* __restrict__ ti, float* __restrict__ dout, int32_t* __restrict__ n_out,
+                     int32_t* __restrict__ map_out) {
   __shared__ int fwd[BF_MAXN];
   __shared__ float fdist[BF_MAXN];
   __shared__ unsigned long long ckey[BF_MAXN];
@@ -436,6 +437,8 @@ bf_crosscheck_kernel(const float* __restrict__ dist, const int32_t* __restrict__
   constexpr int NW = BF_CC_THREADS / 32, CPL = BF_MAXN / 32;
   const int n_q = nq[pair], n_t = nt[pair];
   const float* dp = dist + (size_t)pair * max_n * max_n;
+  // pair = group * g + s writes its lists at g * group_stride + s * out_stride and its count at g * group_stride + s
+  const size_t gbase = (size_t)(pair / group) * group_stride, obase = gbase + (size_t)(pair % group) * out_stride;
   if (tid < BF_MAXN) ckey[tid] = ~0ull;
   __syncthreads();
   unsigned long long cbest[CPL];
@@ -480,24 +483,25 @@ bf_crosscheck_kernel(const float* __restrict__ dist, const int32_t* __restrict__
   for (int w = 0; w < 8; ++w) { if (w < warp) base += warp_cnt[w]; total += warp_cnt[w]; }
   if (keep) {
     const int pos = base + __popc(bal & ((1u << lane) - 1u));
-    qi[(size_t)pair * out_stride + pos] = tid;
-    ti[(size_t)pair * out_stride + pos] = fwd[tid];
-    dout[(size_t)pair * out_stride + pos] = fdist[tid];
+    qi[obase + pos] = tid;
+    ti[obase + pos] = fwd[tid];
+    dout[obase + pos] = fdist[tid];
   }
-  if (map_out != nullptr && tid < max_n) map_out[(size_t)pair * out_stride + tid] = keep ? fwd[tid] : -1;
-  if (tid == 0) n_out[pair] = total;
+  if (map_out != nullptr && tid < max_n) map_out[obase + tid] = keep ? fwd[tid] : -1;
+  if (tid == 0) n_out[gbase + pair % group] = total;
 }
 
 osb_status bf_match_device(int n_pairs, int max_n, int out_stride, const float* const* q, const int32_t* nq,
                            const float* const* t,
                            const int32_t* nt, float* dist_scratch, int32_t* qi, int32_t* ti, float* dout,
-                           int32_t* n_out, int32_t* map_out, cudaStream_t st) {
+                           int32_t* n_out, int32_t* map_out, cudaStream_t st, int group, size_t group_stride) {
   if (n_pairs <= 0) return OSB_OK;
+  if (group <= 0) { group = n_pairs; group_stride = 0; }     // one group: pair p at p * out_stride, count at p
   dim3 g1(cdiv(max_n, BF_ROWS), n_pairs);
   OSB_LAUNCH(bf_dist_kernel, g1, 256, 0, st, q, nq, t, nt, max_n, dist_scratch);
   OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(bf_crosscheck_kernel, n_pairs, BF_CC_THREADS, 0, st, dist_scratch, nq, nt, max_n, out_stride, qi, ti, dout, n_out,
-             map_out);
+  OSB_LAUNCH(bf_crosscheck_kernel, n_pairs, BF_CC_THREADS, 0, st, dist_scratch, nq, nt, max_n, out_stride, group,
+             group_stride, qi, ti, dout, n_out, map_out);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

@@ -428,6 +428,18 @@ class KeyframeFrontend(_Handle):
         _l.check(self._lib.osb_frontend_query(self._h, C.c_void_p(record_dev), int(init_mode), int(nonkeyframe),
                                               C.c_void_p(result_dev), C.c_void_p(stream)))
 
+    def query_received(self, records_dev: int, n_records: int, skip: int, results_dev: int, stream: int, init_mode=None):
+        """query_from_database for a batch of keyframes received from other drones (osb_frontend_query_received): record r
+        != skip with a foreign drone_id -> results_dev[r], one scan of the local store for the batch.  init_mode: None (all
+        off) or n_records flags."""
+        flags = None
+        if init_mode is not None:
+            flags = np.ascontiguousarray(np.asarray(init_mode, dtype=bool), np.uint8)
+            assert flags.shape == (n_records,), "init_mode needs one flag per record"
+        _l.check(self._lib.osb_frontend_query_received(self._h, C.c_void_p(records_dev), n_records, skip,
+                                                       None if flags is None else _l.ptr(flags), C.c_void_p(results_dev),
+                                                       C.c_void_p(stream)))
+
     def finish(self, stream: int):
         _l.check(self._lib.osb_frontend_finish(self._h, C.c_void_p(stream)))
 

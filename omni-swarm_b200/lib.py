@@ -179,6 +179,7 @@ _SIG = {
     "osb_frontend_ingest": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     "osb_frontend_ingest_own": (C.c_int, [_P, _P, _P]),
     "osb_frontend_query": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
+    "osb_frontend_query_received": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "osb_frontend_process": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
     "osb_frontend_finish": (C.c_int, [_P, _P]),
     "osb_frontend_set_profiling": (C.c_int, [_P, C.c_int]),
