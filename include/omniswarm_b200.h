@@ -473,8 +473,9 @@ osb_status osb_pnp_ransac_dev(const float* pts3d_dev, const float* pts2d_dev, co
  * Keyframe front-end -- the per-keyframe pipeline of LoopCam::on_flattened_images (loop_cam.cpp:178-229 ->
  *   generate_stereo_image_descriptor :341-523) followed by LoopDetector::on_image_recv's database work
  *   (loop_detector.cpp:89-104,150-287) and compute_correspond_features' matcher (loop_detector.cpp:539-587),
- *   kept resident on the GPU.  Triangulation / PnP / homography RANSAC stay host code in the reference and
- *   are out of scope (SURVEY.md section 8f).
+ *   kept resident on the GPU.  With the cameras set, the triangulation (or depth look-up) runs inside extract; with the
+ *   geometric filter, the homography RANSAC runs inside query; and osb_frontend_compute_loop turns a round's hits into
+ *   loop edges (correspondences, PnP-RANSAC and the reference's checks) on the device as well.
  *
  * One keyframe = n_dirs directions x (up image, down image) (STEREO_FISHEYE: n_dirs=4, 8 images).
  * osb_keyframe_record is the fixed-size record every drone contributes to the swarm-wide exchange
@@ -632,6 +633,86 @@ osb_status osb_frontend_set_profiling(osb_frontend* h, int enable);
 osb_status osb_frontend_stage_ms(osb_frontend* h, float* ms8);
 /* precision of both networks of the front-end (SuperPoint and NetVLAD; see osb_superpoint_set_precision) */
 osb_status osb_frontend_set_precision(osb_frontend* h, int precision);
+
+/* Loop edges on the device -- LoopDetector::compute_loop + the frame-level compute_correspond_features
+ *   (loop_detector.cpp:431-537, 627-836): for every hit of a query, the correspondences of its direction pairs, PnP-RANSAC
+ *   (osb_pnp_ransac's kernel), pnp_result_verify and the odometry-consistency check.
+ * osb_loop_params: the constants of swarm_loop.cpp:221-256.  osb_loop_candidate: what only the host knows about candidate i
+ *   (the poses of the two keyframes, init_mode, and for same-drone loops the ego-motion between the two stamps).
+ * Roles (:113-118, :637).  results[i].swapped == 0: new = records[i], old = the local row of the hit, main_dir_new =
+ *   query_dir, main_dir_old = hit_dir.  swapped == 1: new = the remote keyframe of the hit (its 3-D landmarks come from the
+ *   remote store), old = records[i], and the two main directions are exchanged.  The old frame is always this drone's own, so
+ *   its 2-D landmarks are lifted through the handle's camera: the depth camera (set_depth_camera) or the left cameras
+ *   (set_cameras); a handle with neither or both gets OSB_ERR_INVALID, as does one without geometric_filter (the reference
+ *   builds with USE_FUNDMENTAL) or without set_loop_params.
+ * Correspondences, in the slot order of osb_loop_result (the reference's dirs_new): slot j contributes geo_new / geo_old when
+ *   geo_valid[j] == 1; when geo_valid[j] == 0 it contributes the 0-3 matches whose new landmark is flagged (the per-image
+ *   function pushes them before it returns false, and the frame-level caller ignores the return value, :488).  The 3-D point
+ *   is the new landmark's landmarks_3d; the 2-D point is the old landmark's liftProjective (fp64, rounded to float) rotated
+ *   into the old main direction by rotate_pt_norm2d(pt, q_ext_old[main_dir_old]^-1 q_ext_old[dir_old]) (fp64, z clamped to
+ *   +-1e-3 as :419-425, rounded to float).  A slot counts towards matched_dir_count when it contributes >= min_match_per_dir.
+ * PnP: iterations 100 (1000 in init_mode), min_loop_num (init_mode_min_loop_num in init_mode), extrinsic = the old camera
+ *   of main_dir_old, prior = (pose_now^-1 pose_old extrinsic)^-1 evaluated left to right without fused multiply-adds (the
+ *   value oracle/loop_ref.py computes), same_drone = drone_id_a == drone_id_b.  These are exactly the osb_pnp_params a host
+ *   caller of osb_pnp_ransac would pass.
+ * set_loop_params: allocates the remote store's landmarks_3d plane (db_capacity x max_num x 3 floats) on its first call, and
+ *   from then on ingest keeps the 3-D landmarks of remote keyframes; OSB_ERR_INVALID once the remote store holds rows.
+ *   Without it nothing is allocated and ingest is unchanged.
+ * compute_loop: 1 <= n <= 64 candidates; records_dev / results_dev are what osb_frontend_query (n = 1) or
+ *   osb_frontend_query_received wrote, with the stores as they are now; cand is a HOST array [n]; out_dev [n] (DEVICE).  The
+ *   candidates travel as kernel parameters, so there is no host synchronisation; the first call acquires the scratch for 64
+ *   candidates and no later call allocates. */
+#define OSB_LOOP_ACCEPTED 0
+#define OSB_LOOP_NO_HIT 1                 /* accepted == 0 */
+#define OSB_LOOP_NO_FRAME 2               /* the hit is a row put in with db_load (hit_msg_id == -1), or has no 3-D landmarks */
+#define OSB_LOOP_FEW_LANDMARKS 3          /* new.landmark_num (sum of n_kpts) < min_loop_num (:632) */
+#define OSB_LOOP_CORRESPONDENCE_FAILED 4  /* no correspondence, or matched_dir_count < min_direction_loop (:532) */
+#define OSB_LOOP_TOO_FEW_COMMON 5         /* n_corr <= min_loop_num, and not (init_mode and n_corr > init_mode_min_loop_num) (:671) */
+#define OSB_LOOP_PNP_FAILED 6             /* no PnP model with >= 4 inliers */
+#define OSB_LOOP_NOT_VERIFIED 7           /* pnp_result_verify (:317-336) */
+#define OSB_LOOP_ODOMETRY_INCONSISTENT 8  /* check_loop_odometry_consistency (:294-315) */
+typedef struct {
+  int32_t min_loop_num;            /* MIN_LOOP_NUM (15) */
+  int32_t init_mode_min_loop_num;  /* INIT_MODE_MIN_LOOP_NUM (10) */
+  int32_t min_match_per_dir;       /* MIN_MATCH_PRE_DIR (15) */
+  int32_t min_direction_loop;      /* MIN_DIRECTION_LOOP (3) */
+  int32_t is_4dof;
+  float reproj_thresh;             /* 3, as the reference passes it (normalised units, :390-391) */
+  uint32_t seed;                   /* seed of the deterministic PnP-RANSAC */
+  int32_t reserved;
+  double rperr_thres;              /* RPERR_THRES */
+  double accept_loop_yaw_rad;      /* ACCEPT_LOOP_YAW_RAD */
+  double max_loop_dis;             /* MAX_LOOP_DIS */
+  double odometry_consistency_threshold;
+} osb_loop_params;
+typedef struct {
+  int32_t init_mode;
+  int32_t reserved;
+  double pose_query[7];            /* pose_drone of records[i] (x y z, qw qx qy qz) */
+  double pose_hit[7];              /* pose_drone of the hit keyframe (results[i].hit_msg_id) */
+  double odom_rel[7];              /* same drone only: ego_motion_traj.get_relative_pose_by_ts(ts_a, ts_b) (:302) */
+  double odom_edge_cov[36];        /* same drone only: odometry + edge covariance, 6x6 row-major (:303) */
+} osb_loop_candidate;
+typedef struct {
+  int32_t status;                  /* OSB_LOOP_* */
+  int32_t drone_id_a, drone_id_b;  /* a = old, b = new (:790-800) */
+  int32_t msg_id_a, msg_id_b;
+  int32_t main_dir_new, main_dir_old;
+  int32_t matched_dir_count;
+  int32_t n_corr;                  /* correspondences (new_norm_2d.size()) */
+  int32_t reserved;
+  osb_pnp_result pnp;              /* the PnP stage as osb_pnp_ransac writes it; zero when no PnP ran */
+  double relative_pose[7];         /* DP_old_to_new as to_ros_pose(): x y z, qw qx qy qz; zero when PnP found no model */
+  int32_t corr_dir_new[OSB_MAX_DIRS * OSB_MAX_KPTS];   /* index2dirindex_new (:527): direction and landmark index of */
+  int32_t corr_idx_new[OSB_MAX_DIRS * OSB_MAX_KPTS];   /* correspondence k, k < n_corr */
+  int32_t corr_dir_old[OSB_MAX_DIRS * OSB_MAX_KPTS];   /* index2dirindex_old (:521) */
+  int32_t corr_idx_old[OSB_MAX_DIRS * OSB_MAX_KPTS];
+  uint8_t inlier[OSB_MAX_DIRS * OSB_MAX_KPTS];          /* PnP inlier mask over the correspondences (0 beyond n_corr) */
+} osb_loop_edge_result;
+osb_status osb_frontend_set_loop_params(osb_frontend* h, const osb_loop_params* p);
+osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev, const osb_loop_result* results_dev,
+                                     int n, const osb_loop_candidate* cand /*HOST [n]*/, osb_loop_edge_result* out_dev,
+                                     void* stream);
 /* ------------------------------------------------------------------------------------------------------------
  * Swarm-wide keyframe exchange -- replaces LoopNet::broadcast_fisheye_desc / image_desc_callback
  *   (swarm_loop/src/loop_net.cpp:20-120,142-172; called from swarm_loop/src/swarm_loop.cpp:167): the LCM UDP multicast of

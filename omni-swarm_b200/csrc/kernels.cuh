@@ -86,4 +86,13 @@ osb_status homography_ransac_device(const float* src_dev, const float* dst_dev, 
                                     float thresh, uint32_t seed, uint8_t* mask_dev, int32_t* n_inl_dev, int32_t* winner_dev,
                                     cudaStream_t st, unsigned int* scratch /* 2 * n_pairs words, zero between launches */);
 
+// ---- pnp.cu ----------------------------------------------------------------------------------------------------
+// deterministic PnP-RANSAC + the reference's checks, one CTA of PNP_THREADS per candidate (osb_pnp_ransac_dev; also launched
+// by osb_frontend_compute_loop on the correspondences it assembles).  max_n <= PNP_MAXN.
+constexpr int PNP_THREADS = 256;
+constexpr int PNP_MAXN = 1024;
+__global__ void __launch_bounds__(PNP_THREADS)
+pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts2d, const int32_t* __restrict__ n_pts, int max_n,
+                  const osb_pnp_params* __restrict__ params, uint8_t* __restrict__ mask_out, osb_pnp_result* __restrict__ results);
+
 }  // namespace osb

@@ -12,6 +12,7 @@
 // a single host synchronisation at the very end (the reference synchronised after every engine call,
 // swarm_loop/src/tensorrt_generic.cpp:73).
 #include "superpoint.cuh"
+#include "pose_algebra.cuh"
 #include <atomic>
 
 namespace osb {
@@ -46,6 +47,8 @@ struct DbView {
   int32_t* frame_drone;        // [cap]   drone_id of the keyframe
   float* top_scores;           // [KMAX]
   int64_t* top_ids;            // [KMAX]
+  float* l3d;                  // [cap][max_num][3] landmarks_3d of the row: the remote store after osb_frontend_set_loop_params
+                               // (the new side of a swapped loop edge); null otherwise
 };
 
 // both databases, passed to the kernels by value: db[0] local, db[1] remote (so db[is_remote])
@@ -196,6 +199,11 @@ __global__ void fe_copy_rows_kernel(const osb_keyframe_record* __restrict__ recs
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     kp[2 * i] = rec->kpts[d][i][0]; kp[2 * i + 1] = rec->kpts[d][i][1];
     fl[i] = rec->landmarks_flag[d][i];
+  }
+  if (db.l3d) {
+    const float* p = &rec->landmarks_3d[d][0][0];
+    float* __restrict__ l3 = db.l3d + (size_t)row * max_num * 3;
+    for (int i = threadIdx.x; i < n * 3; i += blockDim.x) l3[i] = p[i];
   }
   if (threadIdx.x == 0) db.nk[row] = n;
 }
@@ -399,6 +407,224 @@ struct FeMatchScratch {
   unsigned int* g_keys = nullptr;             // 2 * slots, zero between launches
 };
 
+// ---- loop edges: LoopDetector::compute_loop + the frame-level compute_correspond_features (loop_detector.cpp:431-537,
+// 627-836), one CTA per candidate: assemble (gates, correspondences, PnP inputs) -> pnp_ransac_kernel -> finalise --------
+constexpr int LC_MAX = FE_MAX_RECORDS;                    // candidates per call
+constexpr int LC_MAXN = OSB_MAX_DIRS * OSB_MAX_KPTS;      // correspondences per candidate (:455-530: four pairs of <= 200)
+constexpr int LC_PENDING = -1;                            // status between assemble and finalise: the PnP stage decides
+static_assert(LC_MAXN <= PNP_MAXN, "a frame's correspondences must fit the PnP kernel");
+
+struct LoopCams {              // the old (own) frame's camera: pinhole fx fy cx cy and the extrinsics of every direction
+  double K[4];
+  double ext[OSB_MAX_DIRS][7];
+};
+struct LoopCandBatch {         // the host's candidates, passed as kernel parameters (sm_90 takes up to 32 KB of them)
+  osb_loop_candidate c[LC_MAX];
+};
+
+// Swarm::Pose algebra in the evaluation order of oracle/pcm_ref.py with every product rounded on its own (__dmul_rn is never
+// contracted into an FMA): the PnP prior and the rotated points are then the bits a numpy host caller computes
+__device__ __forceinline__ double lc_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ void lc_cross(const double* a, const double* b, double* o) {
+  o[0] = lc_mul(a[1], b[2]) - lc_mul(a[2], b[1]);
+  o[1] = lc_mul(a[2], b[0]) - lc_mul(a[0], b[2]);
+  o[2] = lc_mul(a[0], b[1]) - lc_mul(a[1], b[0]);
+}
+__device__ __forceinline__ void lc_q_rot(const double* q, const double* v, double* o) {    // v + 2 (w (u x v) + u x (u x v))
+  double c[3], d[3];
+  lc_cross(q + 1, v, c);
+  lc_cross(q + 1, c, d);
+  for (int k = 0; k < 3; ++k) o[k] = v[k] + lc_mul(2.0, lc_mul(q[0], c[k]) + d[k]);
+}
+__device__ __forceinline__ void lc_q_mul(const double* a, const double* b, double* o) {
+  o[0] = lc_mul(a[0], b[0]) - lc_mul(a[1], b[1]) - lc_mul(a[2], b[2]) - lc_mul(a[3], b[3]);
+  o[1] = lc_mul(a[0], b[1]) + lc_mul(a[1], b[0]) + lc_mul(a[2], b[3]) - lc_mul(a[3], b[2]);
+  o[2] = lc_mul(a[0], b[2]) - lc_mul(a[1], b[3]) + lc_mul(a[2], b[0]) + lc_mul(a[3], b[1]);
+  o[3] = lc_mul(a[0], b[3]) + lc_mul(a[1], b[2]) - lc_mul(a[2], b[1]) + lc_mul(a[3], b[0]);
+}
+__device__ __forceinline__ void lc_pose_mul(const double* a, const double* b, double* o) {     // poses x y z, qw qx qy qz
+  double r[3];
+  lc_q_rot(a + 3, b, r);
+  for (int k = 0; k < 3; ++k) o[k] = a[k] + r[k];
+  lc_q_mul(a + 3, b + 3, o + 3);
+}
+__device__ __forceinline__ void lc_pose_inv(const double* a, double* o) {
+  const double qc[4] = {a[3], -a[4], -a[5], -a[6]};
+  double r[3];
+  lc_q_rot(qc, a, r);
+  for (int k = 0; k < 3; ++k) o[k] = -r[k];
+  for (int k = 0; k < 4; ++k) o[3 + k] = qc[k];
+}
+// liftProjective of the distortion-free pinhole in fp64, rounded to float (toCV), then rotate_pt_norm2d (:415-428) in fp64
+// from that float, z clamped to +-1e-3, rounded to float
+__device__ __forceinline__ float2 lc_lift_rotate(float kx, float ky, const double (&K)[4], const double (&dq)[4]) {
+  const float u = (float)(((double)kx - K[2]) / K[0]), v = (float)(((double)ky - K[3]) / K[1]);
+  const double p[3] = {(double)u, (double)v, 1.0};
+  double r[3];
+  lc_q_rot(dq, p, r);
+  double z = r[2];
+  if (z < 1e-3 && z > 0) z = 1e-3;
+  if (z > -1e-3 && z < 0) z = -1e-3;
+  return make_float2((float)(r[0] / z), (float)(r[1] / z));
+}
+
+__global__ void __launch_bounds__(256)
+lc_assemble_kernel(const osb_keyframe_record* __restrict__ recs, const osb_loop_result* __restrict__ results,
+                   const __grid_constant__ FeStores dbs, const __grid_constant__ LoopCandBatch cands,
+                   const __grid_constant__ LoopCams cam, const osb_loop_params lp, int query_dir, int max_num,
+                   osb_loop_edge_result* __restrict__ out, float* __restrict__ pts3d, float* __restrict__ pts2d,
+                   int32_t* __restrict__ n_pts, osb_pnp_params* __restrict__ params) {
+  const int c = blockIdx.x, tid = threadIdx.x;
+  const osb_keyframe_record* rec = recs + c;
+  const osb_loop_result* res = results + c;
+  const osb_loop_candidate& cd = cands.c[c];
+  osb_loop_edge_result* o = out + c;
+  const DbView &L = dbs.db[0], &R = dbs.db[1];
+  // roles (:113-118): swapped -> the remote hit is "new", this drone's record "old"; the old frame is always our own (:637)
+  const bool swapped = res->swapped != 0, init_mode = cd.init_mode != 0;
+  const int main_new = swapped ? res->hit_dir : query_dir, main_old = swapped ? query_dir : res->hit_dir;
+  int status = LC_PENDING, fs = -1;
+  if (!res->accepted) {
+    status = OSB_LOOP_NO_HIT;
+  } else {
+    const bool hit_remote = res->hit_id >= OSB_REMOTE_MAGIN_NUMBER;
+    const DbView& hdb = dbs.db[hit_remote];
+    fs = hdb.row_frame[hit_remote ? res->hit_id - OSB_REMOTE_MAGIN_NUMBER : res->hit_id];
+    // a row put in with db_load has no keyframe behind it; the new side of a swapped edge needs the remote 3-D plane
+    if (res->hit_msg_id == -1 || (swapped && R.l3d == nullptr) || hit_remote != swapped) status = OSB_LOOP_NO_FRAME;
+  }
+  if (status == LC_PENDING) {                               // new_frame_desc.landmark_num < MIN_LOOP_NUM (:632)
+    int lm = 0;
+    for (int d = 0; d < OSB_MAX_DIRS; ++d) {
+      if (swapped) { const int row = R.frame_rows[fs * OSB_MAX_DIRS + d]; lm += row >= 0 ? R.nk[row] : 0; }
+      else lm += d < rec->n_dirs ? rec->n_kpts[d] : 0;
+    }
+    if (lm < lp.min_loop_num) status = OSB_LOOP_FEW_LANDMARKS;
+  }
+  // correspondences, direction pair by direction pair in slot order (:477-530); the status is uniform over the block
+  int total = 0, matched_dirs = 0;
+  if (status == LC_PENDING) {
+    for (int j = 0; j < OSB_MAX_DIRS; ++j) {
+      const int dn = res->dir_new[j], dold = res->dir_old[j];
+      if (dn < 0) continue;
+      const int32_t* fl_new;                                // new side: landmarks_flag and landmarks_3d
+      const float* p3_new;
+      const float* k_old;                                   // old side: landmarks_2d
+      if (swapped) {
+        const int rn = R.frame_rows[fs * OSB_MAX_DIRS + dn];
+        fl_new = R.lflag + (size_t)rn * max_num;
+        p3_new = R.l3d + (size_t)rn * max_num * 3;
+        k_old = &rec->kpts[dold][0][0];
+      } else {
+        fl_new = &rec->landmarks_flag[dn][0];
+        p3_new = &rec->landmarks_3d[dn][0][0];
+        k_old = L.kpts + (size_t)L.frame_rows[fs * OSB_MAX_DIRS + dold] * max_num * 2;
+      }
+      // geo_valid: the filtered lists.  Otherwise the 0-3 flagged matches the per-image function pushed before its
+      // `return false` (:574-587, :598-600), which the frame-level caller appends all the same (:488)
+      const bool geo = res->geo_valid[j] != 0;
+      const int n = geo ? res->n_geo[j] : res->n_matches[j];
+      bool keep = false;
+      int qi = 0, ti = 0;
+      if (tid < n) {
+        qi = geo ? res->geo_new[j][tid] : res->match_new[j][tid];
+        ti = geo ? res->geo_old[j][tid] : res->match_old[j][tid];
+        keep = geo || fl_new[qi] != 0;
+      }
+      int cnt;
+      const int pos = total + fe_block_compact(keep, &cnt);
+      if (keep) {
+        o->corr_dir_new[pos] = dn; o->corr_idx_new[pos] = qi;        // index2dirindex_new / _old (:521, :527)
+        o->corr_dir_old[pos] = dold; o->corr_idx_old[pos] = ti;
+        float* X = pts3d + ((size_t)c * LC_MAXN + pos) * 3;
+        X[0] = p3_new[qi * 3]; X[1] = p3_new[qi * 3 + 1]; X[2] = p3_new[qi * 3 + 2];
+        const double* qm = cam.ext[main_old] + 3;           // dq_old = main_quat_old^-1 * extrinsic_old[dir_old].att (:516)
+        const double qmi[4] = {qm[0], -qm[1], -qm[2], -qm[3]};
+        double dq[4];
+        lc_q_mul(qmi, cam.ext[dold] + 3, dq);
+        reinterpret_cast<float2*>(pts2d)[(size_t)c * LC_MAXN + pos] = lc_lift_rotate(k_old[2 * ti], k_old[2 * ti + 1], cam.K, dq);
+      }
+      total += cnt;
+      matched_dirs += cnt >= lp.min_match_per_dir ? 1 : 0;  // _new_3d.size() >= MIN_MATCH_PRE_DIR (:503)
+      __syncthreads();                                      // fe_block_compact's warp counts are reused by the next slot
+    }
+    if (!(total > 0 && matched_dirs >= lp.min_direction_loop)) status = OSB_LOOP_CORRESPONDENCE_FAILED;       // :532
+    else if (!(total > lp.min_loop_num || (init_mode && total > lp.init_mode_min_loop_num))) status = OSB_LOOP_TOO_FEW_COMMON;
+  }
+  if (tid != 0) return;
+  o->status = status;
+  o->drone_id_a = swapped ? rec->drone_id : res->hit_drone_id;  o->drone_id_b = swapped ? res->hit_drone_id : rec->drone_id;
+  o->msg_id_a = swapped ? rec->msg_id : res->hit_msg_id;        o->msg_id_b = swapped ? res->hit_msg_id : rec->msg_id;
+  o->main_dir_new = main_new; o->main_dir_old = main_old;
+  o->matched_dir_count = matched_dirs; o->n_corr = total; o->reserved = 0;
+  // compute_relative_pose's inputs (:672-684, :376-391), exactly the osb_pnp_params of a host caller of osb_pnp_ransac
+  const bool run = status == LC_PENDING;
+  n_pts[c] = run ? total : 0;
+  osb_pnp_params p;
+  memset(&p, 0, sizeof(p));
+  p.iterations = init_mode ? 1000 : 100;
+  p.reproj_thresh = lp.reproj_thresh; p.seed = lp.seed; p.is_4dof = lp.is_4dof;
+  p.min_loop_num = init_mode ? lp.init_mode_min_loop_num : lp.min_loop_num;
+  p.same_drone = o->drone_id_a == o->drone_id_b ? 1 : 0;
+  p.rperr_thres = lp.rperr_thres; p.accept_loop_yaw_rad = lp.accept_loop_yaw_rad; p.max_loop_dis = lp.max_loop_dis;
+  p.odometry_consistency_threshold = lp.odometry_consistency_threshold;
+  p.prior[3] = p.extrinsic[3] = p.drone_pose_now[3] = p.drone_pose_old[3] = 1.0;
+  if (run) {
+    const double* now = swapped ? cd.pose_hit : cd.pose_query;
+    const double* old = swapped ? cd.pose_query : cd.pose_hit;
+    for (int k = 0; k < 7; ++k) { p.extrinsic[k] = cam.ext[main_old][k]; p.drone_pose_now[k] = now[k]; p.drone_pose_old[k] = old[k]; }
+    double a[7], b[7], e[7];                                // prior = (now^-1 old extrinsic)^-1, left to right
+    lc_pose_inv(now, a);
+    lc_pose_mul(a, old, b);
+    lc_pose_mul(b, p.extrinsic, e);
+    lc_pose_inv(e, p.prior);
+    for (int k = 0; k < 7; ++k) p.odom_rel[k] = cd.odom_rel[k];
+    for (int k = 0; k < 36; ++k) p.odom_edge_cov[k] = cd.odom_edge_cov[k];
+  }
+  params[c] = p;
+}
+
+// after the PnP stage: the status of the candidates that reached it, the PnP result, DP_old_to_new as a 7-pose, and the
+// inlier mask in correspondence order
+__global__ void __launch_bounds__(256)
+lc_finalise_kernel(const uint8_t* __restrict__ mask, const osb_pnp_result* __restrict__ pnp,
+                   const osb_pnp_params* __restrict__ params, osb_loop_edge_result* __restrict__ out) {
+  const int c = blockIdx.x, tid = threadIdx.x;
+  osb_loop_edge_result* o = out + c;
+  const bool ran = o->status == LC_PENDING;
+  for (int i = tid; i < LC_MAXN; i += blockDim.x) o->inlier[i] = ran ? mask[(size_t)c * LC_MAXN + i] : 0;
+  __syncthreads();                                          // every thread has read the status before thread 0 rewrites it
+  if (tid != 0) return;
+  const osb_pnp_result r = pnp[c];
+  for (int k = 0; k < 7; ++k) o->relative_pose[k] = 0.0;
+  if (!ran) { memset(&o->pnp, 0, sizeof(o->pnp)); return; }
+  o->pnp = r;
+  o->status = !r.pnp_success ? OSB_LOOP_PNP_FAILED : !r.verified ? OSB_LOOP_NOT_VERIFIED
+              : !r.odometry_consistent ? OSB_LOOP_ODOMETRY_INCONSISTENT : OSB_LOOP_ACCEPTED;
+  if (!r.pnp_success) return;
+  // DeltaPose(p_drone_old_in_new, drone_pose_now, is_4dof) (:393-400) as a pose; its x y z and yaw are r.dp_old_to_new
+  const osb_pnp_params& prm = params[c];
+  const PoseD P = load_pose(r.pose_cam);
+  const PoseD old_in_new = pose_mul(pose_inv(P), pose_inv(load_pose(prm.extrinsic)));
+  const PoseD now = load_pose(prm.drone_pose_now);
+  PoseD dp;
+  if (prm.is_4dof) {
+    double ea[3], eb[3];
+    quat2eulers(old_in_new.q, ea); quat2eulers(now.q, eb);
+    const double cs = cos(ea[2]), sn = sin(ea[2]);
+    const double dx = now.t[0] - old_in_new.t[0], dy = now.t[1] - old_in_new.t[1];
+    dp.t[0] = cs * dx + sn * dy; dp.t[1] = -sn * dx + cs * dy; dp.t[2] = now.t[2] - old_in_new.t[2];
+    double a = eb[2] - ea[2];
+    a = a - 2.0 * M_PI * floor((a + M_PI) / (2.0 * M_PI));
+    const double rv[3] = {0.0, 0.0, a};
+    quat_from_rotvec(rv, dp.q);
+  } else {
+    dp = pose_mul(pose_inv(old_in_new), now);
+  }
+  for (int k = 0; k < 3; ++k) o->relative_pose[k] = dp.t[k];
+  for (int k = 0; k < 4; ++k) o->relative_pose[3 + k] = dp.q[k];
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -439,6 +665,16 @@ struct osb_frontend {
   bool have_depth_camera = false;
   double depth_K[4] = {0, 0, 0, 0}, depth_ext[OSB_MAX_DIRS][7], near_thres = 0.3, far_thres = 10.0;
   uint16_t* d_depth = nullptr;   // [n_dirs][H][W] mm, staging of the host-buffer depth extracts
+  // loop edges (osb_frontend_set_loop_params / osb_frontend_compute_loop): the PnP stage's inputs and outputs for LC_MAX
+  // candidates, acquired by the first compute_loop (lc_ready)
+  bool have_loop_params = false;
+  osb_loop_params loop_params{};
+  bool lc_ready = false;
+  float *d_lc_pts3d = nullptr, *d_lc_pts2d = nullptr;   // [LC_MAX][LC_MAXN][3] / [2]
+  int32_t* d_lc_n = nullptr;
+  osb_pnp_params* d_lc_params = nullptr;
+  uint8_t* d_lc_mask = nullptr;                           // [LC_MAX][LC_MAXN]
+  osb_pnp_result* d_lc_pnp = nullptr;
   int32_t* d_assign = nullptr;   // [max_records][4]
   int max_records = FE_MAX_RECORDS;
   osb_keyframe_record* d_record = nullptr;   // used by process()
@@ -931,6 +1167,71 @@ extern "C" osb_status osb_frontend_query_received(osb_frontend* h, const osb_key
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   return fe_query_received(h, records_dev, n_records, skip, mask, results_dev, (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_frontend_set_loop_params(osb_frontend* h, const osb_loop_params* p) {
+  OSB_REQUIRE(h && p, "null argument");
+  OSB_REQUIRE(p->min_loop_num >= 0 && p->init_mode_min_loop_num >= 0 && p->min_match_per_dir >= 0 &&
+              p->min_direction_loop >= 0, "negative count threshold");
+  OSB_REQUIRE(p->reproj_thresh > 0.f, "reproj_thresh must be positive");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(fe_refresh_counts(h, h->stream));
+  // rows ingested so far carry no 3-D landmarks: the plane would hand stale points to a swapped edge
+  OSB_REQUIRE(h->db[1].upper == 0, "the remote store already holds rows: set the loop parameters before the first ingest");
+  DbStore& R = h->db[1];
+  if (!R.v.l3d) OSB_TRY(h->res.alloc(&R.v.l3d, (size_t)R.cap * h->cfg.max_num * 3));
+  h->loop_params = *p;
+  h->have_loop_params = true;
+  return OSB_OK;
+}
+
+// compute_loop's scratch for LC_MAX candidates (about 1 MB), acquired once by its first call
+static osb_status fe_lc_alloc(osb_frontend* h) {
+  if (h->lc_ready) return OSB_OK;
+  Resources& m = h->res;
+  OSB_TRY(m.alloc(&h->d_lc_pts3d, (size_t)LC_MAX * LC_MAXN * 3));
+  OSB_TRY(m.alloc(&h->d_lc_pts2d, (size_t)LC_MAX * LC_MAXN * 2));
+  OSB_TRY(m.alloc(&h->d_lc_n, LC_MAX));
+  OSB_TRY(m.alloc(&h->d_lc_params, LC_MAX));
+  OSB_TRY(m.alloc(&h->d_lc_mask, (size_t)LC_MAX * LC_MAXN));
+  OSB_TRY(m.alloc(&h->d_lc_pnp, LC_MAX));
+  h->lc_ready = true;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                                const osb_loop_result* results_dev, int n, const osb_loop_candidate* cand,
+                                                osb_loop_edge_result* out_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 1 && n <= LC_MAX, "n must be 1..64");
+  OSB_REQUIRE(records_dev && results_dev && cand && out_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->have_loop_params, "no loop parameters: call osb_frontend_set_loop_params first");
+  OSB_REQUIRE(h->cfg.geometric_filter != 0, "compute_loop needs geometric_filter = 1 (the reference's USE_FUNDMENTAL path)");
+  OSB_REQUIRE(h->have_cameras != h->have_depth_camera,
+              "compute_loop needs the old frame's camera: exactly one of set_cameras / set_depth_camera");
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_TRY(fe_lc_alloc(h));
+  LoopCams cam{};
+  const bool depth = h->have_depth_camera;
+  for (int i = 0; i < 4; ++i) cam.K[i] = depth ? h->depth_K[i] : h->K[i];
+  for (int d = 0; d < OSB_MAX_DIRS; ++d)
+    for (int i = 0; i < 7; ++i)
+      cam.ext[d][i] = d < h->cfg.n_dirs ? (depth ? h->depth_ext[d][i] : h->left_ext[d][i]) : (i == 3 ? 1.0 : 0.0);
+  LoopCandBatch cb;
+  memset(&cb, 0, sizeof(cb));
+  memcpy(cb.c, cand, (size_t)n * sizeof(osb_loop_candidate));
+  OSB_LAUNCH(lc_assemble_kernel, n, 256, 0, st, records_dev, results_dev, fe_stores(h), cb, cam, h->loop_params,
+             h->cfg.query_dir, h->cfg.max_num, out_dev, h->d_lc_pts3d, h->d_lc_pts2d, h->d_lc_n, h->d_lc_params);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(pnp_ransac_kernel, n, PNP_THREADS, 0, st, h->d_lc_pts3d, h->d_lc_pts2d, h->d_lc_n, LC_MAXN, h->d_lc_params,
+             h->d_lc_mask, h->d_lc_pnp);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(lc_finalise_kernel, n, 256, 0, st, h->d_lc_mask, h->d_lc_pnp, h->d_lc_params, out_dev);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
 }
 
 // exact host-side row counts.  The counts are read on `st`, which need not be the stream that carried the last ingest

@@ -19,8 +19,7 @@
 
 namespace osb {
 
-constexpr int PNP_THREADS = 256;
-constexpr int PNP_MAXN = 1024;
+// PNP_THREADS and PNP_MAXN: kernels.cuh
 constexpr int PNP_HYP_ITERS = 8;        // oracle/pnp_ref.py HYP_ITERS
 constexpr int PNP_REFINE_ITERS = 12;    // REFINE_ITERS
 

@@ -440,6 +440,37 @@ class KeyframeFrontend(_Handle):
                                                        None if flags is None else _l.ptr(flags), C.c_void_p(results_dev),
                                                        C.c_void_p(stream)))
 
+    def set_loop_params(self, min_loop_num=15, init_mode_min_loop_num=10, min_match_per_dir=15, min_direction_loop=3,
+                        is_4dof=True, reproj_thresh=3.0, seed=0, rperr_thres=10 * np.pi / 180,
+                        accept_loop_yaw_rad=30 * np.pi / 180, max_loop_dis=5.0, odometry_consistency_threshold=2.0):
+        """the constants of compute_loop (swarm_loop.cpp:221-256, loop_defines.h defaults); before the first remote ingest"""
+        p = _l.LoopParams(min_loop_num=min_loop_num, init_mode_min_loop_num=init_mode_min_loop_num,
+                          min_match_per_dir=min_match_per_dir, min_direction_loop=min_direction_loop, is_4dof=int(is_4dof),
+                          reproj_thresh=reproj_thresh, seed=seed, rperr_thres=rperr_thres,
+                          accept_loop_yaw_rad=accept_loop_yaw_rad, max_loop_dis=max_loop_dis,
+                          odometry_consistency_threshold=odometry_consistency_threshold)
+        _l.check(self._lib.osb_frontend_set_loop_params(self._h, C.byref(p)))
+
+    @staticmethod
+    def loop_candidates(cands):
+        """list of dicts (pose_query [7], pose_hit [7]; optional init_mode, odom_rel [7], cov [6,6]) -> LoopCandidate array"""
+        arr = (_l.LoopCandidate * len(cands))()
+        for a, c in zip(arr, cands):
+            a.init_mode = int(bool(c.get("init_mode", False)))
+            a.pose_query[:] = [float(x) for x in c["pose_query"]]
+            a.pose_hit[:] = [float(x) for x in c["pose_hit"]]
+            a.odom_rel[:] = [float(x) for x in c.get("odom_rel", [0, 0, 0, 1, 0, 0, 0])]
+            a.odom_edge_cov[:] = [float(x) for x in np.asarray(c.get("cov", np.eye(6)), np.float64).reshape(-1)]
+        return arr
+
+    def compute_loop(self, records_dev: int, results_dev: int, cands, out_dev: int, stream: int):
+        """loop edges of n = len(cands) query results (osb_frontend_compute_loop): records_dev / results_dev [n] as query or
+        query_received wrote them, cands a list of dicts (see loop_candidates) -> LoopEdgeResult [n] at out_dev, no
+        synchronisation"""
+        arr = self.loop_candidates(cands)
+        _l.check(self._lib.osb_frontend_compute_loop(self._h, C.c_void_p(records_dev), C.c_void_p(results_dev), len(cands),
+                                                     arr, C.c_void_p(out_dev), C.c_void_p(stream)))
+
     def finish(self, stream: int):
         _l.check(self._lib.osb_frontend_finish(self._h, C.c_void_p(stream)))
 

@@ -85,6 +85,33 @@ class PnpResult(C.Structure):
                 ("pose_cam", C.c_double * 7), ("dp_old_to_new", C.c_double * 4)]
 
 
+(LOOP_ACCEPTED, LOOP_NO_HIT, LOOP_NO_FRAME, LOOP_FEW_LANDMARKS, LOOP_CORRESPONDENCE_FAILED, LOOP_TOO_FEW_COMMON,
+ LOOP_PNP_FAILED, LOOP_NOT_VERIFIED, LOOP_ODOMETRY_INCONSISTENT) = range(9)
+LOOP_MAXN = MAX_DIRS * MAX_KPTS
+
+
+class LoopParams(C.Structure):
+    _fields_ = [("min_loop_num", C.c_int32), ("init_mode_min_loop_num", C.c_int32), ("min_match_per_dir", C.c_int32),
+                ("min_direction_loop", C.c_int32), ("is_4dof", C.c_int32), ("reproj_thresh", C.c_float),
+                ("seed", C.c_uint32), ("reserved", C.c_int32), ("rperr_thres", C.c_double),
+                ("accept_loop_yaw_rad", C.c_double), ("max_loop_dis", C.c_double),
+                ("odometry_consistency_threshold", C.c_double)]
+
+
+class LoopCandidate(C.Structure):
+    _fields_ = [("init_mode", C.c_int32), ("reserved", C.c_int32), ("pose_query", C.c_double * 7),
+                ("pose_hit", C.c_double * 7), ("odom_rel", C.c_double * 7), ("odom_edge_cov", C.c_double * 36)]
+
+
+class LoopEdgeResult(C.Structure):
+    _fields_ = [("status", C.c_int32), ("drone_id_a", C.c_int32), ("drone_id_b", C.c_int32), ("msg_id_a", C.c_int32),
+                ("msg_id_b", C.c_int32), ("main_dir_new", C.c_int32), ("main_dir_old", C.c_int32),
+                ("matched_dir_count", C.c_int32), ("n_corr", C.c_int32), ("reserved", C.c_int32), ("pnp", PnpResult),
+                ("relative_pose", C.c_double * 7), ("corr_dir_new", C.c_int32 * LOOP_MAXN),
+                ("corr_idx_new", C.c_int32 * LOOP_MAXN), ("corr_dir_old", C.c_int32 * LOOP_MAXN),
+                ("corr_idx_old", C.c_int32 * LOOP_MAXN), ("inlier", C.c_uint8 * LOOP_MAXN)]
+
+
 class FrontendConfig(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_dirs", C.c_int32), ("max_num", C.c_int32),
                 ("sp_thres", C.c_float), ("self_id", C.c_int32), ("db_capacity", C.c_int32),
@@ -95,6 +122,7 @@ class FrontendConfig(C.Structure):
 
 RECORD_BYTES = C.sizeof(KeyframeRecord)
 RESULT_BYTES = C.sizeof(LoopResult)
+EDGE_BYTES = C.sizeof(LoopEdgeResult)
 
 _P = C.c_void_p
 _SIG = {
@@ -180,6 +208,8 @@ _SIG = {
     "osb_frontend_ingest_own": (C.c_int, [_P, _P, _P]),
     "osb_frontend_query": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "osb_frontend_query_received": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "osb_frontend_set_loop_params": (C.c_int, [_P, C.POINTER(LoopParams)]),
+    "osb_frontend_compute_loop": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
     "osb_frontend_process": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
     "osb_frontend_finish": (C.c_int, [_P, _P]),
     "osb_frontend_set_profiling": (C.c_int, [_P, C.c_int]),

@@ -547,3 +547,44 @@ def pnp_case(n: int = 200, outlier_frac: float = 0.25, seed: int = 0, noise: flo
                         pose_true)
     return dict(X=X.astype(np.float32), uv=uv.astype(np.float32), inlier=inlier, pose_true=pose_true, prior=prior,
                 extrinsic=extrinsic, drone_pose_now=drone_pose_now, drone_pose_old=drone_pose_old)
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# A four-direction loop candidate with exactly representable geometry (osb_frontend_compute_loop)
+# ----------------------------------------------------------------------------------------------------------------
+def loop_scene(yaw: float = 0.15, t_new=(0.25, -0.125, 0.0625), depths=(2.0, 4.0, 2.0, 4.0), fx: float = 64.0,
+               cx: float = 48.0, cy: float = 32.0):
+    """The old drone at the origin of the shared odometry frame, four cameras at its centre looking along body +x rotated
+    by 0, 90, 180 and 270 degrees of yaw; direction d sees a fronto-parallel plane at depth depths[d].  The points of a
+    direction sit at unit-depth ray (a, b, 1) with a in {+-1/4, +-1/2, +-1} and b a multiple of 1/8, so the old pixels, their
+    lift, the rotation into any other direction and the 3-D points are all exact in float32.  The new drone is at
+    (t_new, yaw).  Returns dict(K (fx fy cx cy), ext [4,7], pose_old, pose_new, delta_true (x y z, qw qx qy qz: the 4-DoF
+    DP_old_to_new), and per direction kp_old [n,2], kp_new [n,2] (pixels, the new camera), X [n,3] (float32))."""
+    Rcb = np.array([[0.0, 0.0, 1.0], [-1.0, 0.0, 0.0], [0.0, -1.0, 0.0]])     # camera z = body x, x = -body y, y = -body z
+    q_base = np.array([0.5, -0.5, 0.5, -0.5])                                  # the quaternion of Rcb
+    pa = _PoseAlgebra
+    K = np.array([fx, fx, cx, cy])
+    ext, kp_old, kp_new, X = [], [], [], []
+    pose_old = np.array([0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0])
+    pose_new = np.concatenate([np.asarray(t_new, np.float64), _quat_from_rotvec(np.array([0.0, 0.0, yaw]))])
+    a_vals = np.array([-1.0, -0.5, -0.25, 0.25, 0.5, 1.0])
+    b_vals = np.arange(-6, 7) / 8.0
+    for d in range(4):
+        qd = pa.q_mul(_quat_from_rotvec(np.array([0.0, 0.0, d * np.pi / 2])), q_base)
+        ext.append(np.concatenate([[0.0, 0.0, 0.0], qd]))
+        Rz = np.rint(np.array([[np.cos(d * np.pi / 2), -np.sin(d * np.pi / 2), 0], [np.sin(d * np.pi / 2), np.cos(d * np.pi / 2), 0],
+                               [0, 0, 1]]))
+        R = Rz @ Rcb                                                           # exact: entries 0, +-1
+        a, b = np.meshgrid(a_vals, b_vals, indexing="ij")
+        ray = np.stack([a.ravel(), b.ravel(), np.ones(a.size)], 1)
+        pc = ray * depths[d]
+        Xw = pc @ R.T
+        X.append(Xw.astype(np.float32))
+        kp_old.append(np.stack([fx * ray[:, 0] + cx, fx * ray[:, 1] + cy], 1).astype(np.float32))
+        cam_new = pa.pose_mul(pose_new, ext[-1])
+        qc = cam_new[3:] * np.array([1.0, -1.0, -1.0, -1.0])
+        pn = np.stack([pa.q_rot(qc, x - cam_new[:3]) for x in Xw])
+        kp_new.append(np.stack([fx * pn[:, 0] / pn[:, 2] + cx, fx * pn[:, 1] / pn[:, 2] + cy], 1).astype(np.float32))
+    delta = pose_new.copy()                                                   # the old drone is the origin
+    return dict(K=K, ext=np.array(ext), pose_old=pose_old, pose_new=pose_new, delta_true=delta, kp_old=kp_old, kp_new=kp_new,
+                X=X)
