@@ -379,6 +379,47 @@ osb_status osb_pcm(const osb_loop_edge* edges, int n, double pcm_thres, double o
 osb_status osb_pcm_dev(const osb_loop_edge* edges_dev, int n, double pcm_thres, double odom_pos_cov_per_m,
                        double odom_ang_cov_per_m, int32_t* clique_dev, int32_t* clique_size_dev, uint8_t* adj_dev,
                        double* smd_dev, void* stream);
+/* Persistent PCM state -- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges (swarm_outlier_rejection.cpp:98-167, 173-297)
+ *   with the state it keeps between solves: the consistency graph and the loops of every drone pair stay on the device, a
+ *   call checks only its new loops (O(new x L) pair checks, not O(L^2)) and reruns maxCliqueHeu on the pairs that gained any.
+ * reject(): loop edges[i] carries the LoopEdge::id ids[i].  As :106-139:
+ *   - a loop whose id an earlier call stored is skipped: the FIRST-seen values of an id are the ones used (the reference
+ *     ignores the values re-anchoring gives the same id later);
+ *   - routing: a loop belongs to the unordered pair {id_a, id_b}; with `redundant` every pair is processed, else only the
+ *     pairs that contain self_id, (self, self) included.  Loops of other pairs are neither stored nor marked as seen, so
+ *     they count as new again on the next call;
+ *   - a pair's new loops are appended in call order (the same id twice in one call is appended twice), each checked against
+ *     every earlier loop of its pair with edge1 = the later loop, so its graph is bit-identical to osb_pcm's on the pair's
+ *     whole insertion-ordered list; every pair that gained a loop reruns maxCliqueHeu on its whole graph and its inlier set
+ *     becomes the clique's ids, replacing whatever set_inliers wrote;
+ *   - keep[i] = 1 iff edge i is in the returned good_loops (:141-157): its pair has no inlier set, or its id is in the set.
+ *   A call that would push a pair past pair_capacity or the state past max_pairs returns OSB_ERR_CAPACITY and changes
+ *   nothing.  A call that routes nothing new launches no kernel; otherwise it makes one copy up (pinned staging), two
+ *   launches, one copy down and one synchronisation on the handle's stream.
+ * inliers(): good_loops_set[a][b] in ascending id order (what broadcast_good_loops sends); *n = its size, -1 if the pair has
+ *   none; ids may be NULL to query the size, else OSB_ERR_CAPACITY when the set exceeds cap.
+ * set_inliers(): good_ids_handle (:37-56): replaces the pair's set with ids[0..n); ignored when the pair contains self_id.
+ *   (The reference's handler inserts the indices 0..inlier_id_size-1, not msg->inlier_ids: the adapter decides what to pass.)
+ * pair(): read-out for tests: the pair's loop count *n (0 for an unknown pair), its ids in insertion order [n], adjacency
+ *   [n][n] (1 = consistent), its last clique in maxCliqueHeu order and its size; every output but n may be NULL.
+ * Memory: create holds a stream, max_pairs x (48 + 480 pair_capacity) bytes of pinned and of device staging and
+ *   max_pairs x (1 + pair_capacity) x 4 bytes of clique output on each side.  A pair's first loop acquires its slot,
+ *   pair_capacity x (488 + 4 ceil(pair_capacity / 32)) bytes (4.1 MB at 4096), kept until destroy; nothing else is acquired. */
+typedef struct {
+  int32_t self_id;
+  int32_t redundant;             /* SwarmLocalOutlierRejectionParams::redundant */
+  int32_t max_pairs;             /* unordered drone pairs {a,b}, a == b allowed (intra-drone loops) */
+  int32_t pair_capacity;         /* edges per pair, 1..4096 (the clique kernel's bitset bound) */
+  double pcm_thres, odom_pos_cov_per_m, odom_ang_cov_per_m;
+} osb_pcm_state_params;
+typedef struct osb_pcm_state osb_pcm_state;
+osb_status osb_pcm_state_create(osb_pcm_state** out, const osb_pcm_state_params* p);
+osb_status osb_pcm_state_destroy(osb_pcm_state* s);
+osb_status osb_pcm_state_reject(osb_pcm_state* s, const osb_loop_edge* edges, const int64_t* ids, int n, uint8_t* keep);
+osb_status osb_pcm_state_inliers(osb_pcm_state* s, int32_t id_a, int32_t id_b, int64_t* ids, int cap, int32_t* n);
+osb_status osb_pcm_state_set_inliers(osb_pcm_state* s, int32_t id_a, int32_t id_b, const int64_t* ids, int n);
+osb_status osb_pcm_state_pair(osb_pcm_state* s, int32_t id_a, int32_t id_b, int32_t* n, int64_t* ids, uint8_t* adj,
+                              int32_t* clique, int32_t* clique_size);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Geometric filter of the loop matcher (SURVEY.md 8f-1, first half) -- the inlier mask of

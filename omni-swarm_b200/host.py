@@ -618,6 +618,24 @@ def pnp_ransac(cases, max_n: int | None = None):
     return [(mask[i, :n[i]].copy(), res[i]) for i in range(nc)]
 
 
+def loop_edges(edges):
+    """edge dicts (id_a, id_b, rel [7], cov [6,6], odom_a [7], odom_b [7], len_a, len_b) -> osb_loop_edge [n] as a
+    float64 array [n, 60] (word 0 holds id_a, id_b as two int32), the bytes the C ABI reads"""
+    n = len(edges)
+    arr = np.zeros((n, 60), np.float64)
+    if n:
+        ids = arr.view(np.int32)
+        ids[:, 0] = [int(e["id_a"]) for e in edges]
+        ids[:, 1] = [int(e["id_b"]) for e in edges]
+        arr[:, 1:8] = [e["rel"] for e in edges]
+        arr[:, 8:44] = np.asarray([np.asarray(e["cov"], np.float64).reshape(-1) for e in edges])
+        arr[:, 44:51] = [e["odom_a"] for e in edges]
+        arr[:, 51:58] = [e["odom_b"] for e in edges]
+        arr[:, 58] = [float(e["len_a"]) for e in edges]
+        arr[:, 59] = [float(e["len_b"]) for e in edges]
+    return arr
+
+
 def pcm_outlier_rejection(edges, pcm_thres: float, odom_pos_cov_per_m: float, odom_ang_cov_per_m: float,
                           want_matrices: bool = False):
     """SwarmLocalOutlierRejection::OutlierRejectionLoopEdgesPCM (swarm_outlier_rejection.cpp:173-297) for the loop edges of
@@ -625,22 +643,67 @@ def pcm_outlier_rejection(edges, pcm_thres: float, odom_pos_cov_per_m: float, od
     insertion order -> indices of the kept loops in maxCliqueHeu's order (+ adjacency and smd matrices on request)."""
     lib = _l.load()
     n = len(edges)
-    arr = (_l.LoopEdge * n)()
-    for i, e in enumerate(edges):
-        a = arr[i]
-        a.id_a, a.id_b, a.len_a, a.len_b = int(e["id_a"]), int(e["id_b"]), float(e["len_a"]), float(e["len_b"])
-        a.rel_pose[:] = [float(x) for x in e["rel"]]
-        a.cov[:] = [float(x) for x in np.asarray(e["cov"], np.float64).reshape(-1)]
-        a.odom_a[:] = [float(x) for x in e["odom_a"]]
-        a.odom_b[:] = [float(x) for x in e["odom_b"]]
+    arr = loop_edges(edges)
     clique = np.zeros(n, np.int32)
     size = C.c_int32(0)
     adj = np.zeros((n, n), np.uint8) if want_matrices else None
     smd = np.zeros((n, n), np.float64) if want_matrices else None
-    _l.check(lib.osb_pcm(arr, n, float(pcm_thres), float(odom_pos_cov_per_m), float(odom_ang_cov_per_m), _l.ptr(clique),
+    _l.check(lib.osb_pcm(_l.ptr(arr), n, float(pcm_thres), float(odom_pos_cov_per_m), float(odom_ang_cov_per_m), _l.ptr(clique),
                          C.byref(size), _l.ptr(adj), _l.ptr(smd)))
     out = clique[:size.value].copy()
     return (out, adj, smd) if want_matrices else out
+
+
+class PcmState(_Handle):
+    """SwarmLocalOutlierRejection (swarm_outlier_rejection.cpp:37-56, 98-297) with its per-drone-pair PCM state resident on
+    the device (osb_pcm_state_*): `reject(edges, ids)` is OutlierRejectionLoopEdges -> keep mask of good_loops,
+    `inliers(a, b)` what broadcast_good_loops sends, `set_inliers(a, b, ids)` good_ids_handle, `pair(a, b)` the read-out."""
+
+    _destroy = "osb_pcm_state_destroy"
+
+    def __init__(self, self_id: int, redundant: bool, pcm_thres: float, odom_pos_cov_per_m: float,
+                 odom_ang_cov_per_m: float, max_pairs: int = 16, pair_capacity: int = 4096):
+        self._lib = _l.load()
+        self._h = C.c_void_p()
+        p = _l.PcmStateParams(int(self_id), int(bool(redundant)), int(max_pairs), int(pair_capacity), float(pcm_thres),
+                              float(odom_pos_cov_per_m), float(odom_ang_cov_per_m))
+        _l.check(self._lib.osb_pcm_state_create(C.byref(self._h), C.byref(p)))
+
+    def reject(self, edges, ids) -> np.ndarray:
+        """edges: edge dicts (as pcm_outlier_rejection) or an already packed loop_edges() array; ids: LoopEdge::id each
+        -> keep [n] bool"""
+        arr = edges if isinstance(edges, np.ndarray) else loop_edges(edges)
+        ids = np.ascontiguousarray(ids, np.int64)
+        assert arr.shape == (len(ids), 60)
+        keep = np.zeros(len(ids), np.uint8)
+        _l.check(self._lib.osb_pcm_state_reject(self._h, _l.ptr(arr), _l.ptr(ids), len(ids), _l.ptr(keep)))
+        return keep.astype(bool)
+
+    def inliers(self, a: int, b: int):
+        """the pair's inlier ids ascending, or None when it has no set"""
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_pcm_state_inliers(self._h, a, b, None, 0, C.byref(n)))
+        if n.value < 0:
+            return None
+        out = np.zeros(n.value, np.int64)
+        _l.check(self._lib.osb_pcm_state_inliers(self._h, a, b, _l.ptr(out), n.value, C.byref(n)))
+        return out
+
+    def set_inliers(self, a: int, b: int, ids):
+        ids = np.ascontiguousarray(ids, np.int64)
+        _l.check(self._lib.osb_pcm_state_set_inliers(self._h, a, b, _l.ptr(ids), len(ids)))
+
+    def pair(self, a: int, b: int):
+        """-> (ids [n] in insertion order, adjacency [n,n] uint8, last clique in maxCliqueHeu order)"""
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_pcm_state_pair(self._h, a, b, C.byref(n), None, None, None, None))
+        ids = np.zeros(n.value, np.int64)
+        adj = np.zeros((n.value, n.value), np.uint8)
+        clique = np.zeros(n.value, np.int32)
+        size = C.c_int32(0)
+        _l.check(self._lib.osb_pcm_state_pair(self._h, a, b, C.byref(n), _l.ptr(ids), _l.ptr(adj), _l.ptr(clique),
+                                              C.byref(size)))
+        return ids, adj, clique[:size.value].copy()
 
 
 class Swarm(_Handle):

@@ -70,6 +70,11 @@ class LoopEdge(C.Structure):
                 ("odom_a", C.c_double * 7), ("odom_b", C.c_double * 7), ("len_a", C.c_double), ("len_b", C.c_double)]
 
 
+class PcmStateParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("redundant", C.c_int32), ("max_pairs", C.c_int32), ("pair_capacity", C.c_int32),
+                ("pcm_thres", C.c_double), ("odom_pos_cov_per_m", C.c_double), ("odom_ang_cov_per_m", C.c_double)]
+
+
 class PnpParams(C.Structure):
     _fields_ = [("iterations", C.c_int32), ("reproj_thresh", C.c_float), ("seed", C.c_uint32), ("is_4dof", C.c_int32),
                 ("min_loop_num", C.c_int32), ("same_drone", C.c_int32), ("rperr_thres", C.c_double),
@@ -233,6 +238,12 @@ _SIG = {
     "osb_pnp_ransac_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "osb_pcm": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P]),
     "osb_pcm_dev": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
+    "osb_pcm_state_create": (C.c_int, [C.POINTER(_P), C.POINTER(PcmStateParams)]),
+    "osb_pcm_state_destroy": (C.c_int, [_P]),
+    "osb_pcm_state_reject": (C.c_int, [_P, _P, _P, C.c_int, _P]),
+    "osb_pcm_state_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int, C.POINTER(C.c_int32)]),
+    "osb_pcm_state_set_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int]),
+    "osb_pcm_state_pair": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, C.POINTER(C.c_int32)]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),

@@ -505,6 +505,42 @@ def pcm_edges(n: int = 60, outlier_frac: float = 0.3, seed: int = 0, flip_frac: 
     return [edges[i] for i in order]
 
 
+def pcm_swarm_rounds(n_drones: int = 5, rounds: int = 6, per_round: int = 8, outlier_frac: float = 0.3, seed: int = 0,
+                     n_duplicates: int = 2, n_perturbed: int = 2):
+    """The loop edges OutlierRejectionLoopEdges receives before successive solves of a swarm of drones 1..n_drones: every
+    unordered pair {a, b} (a == b: intra-drone loops) gains 1..per_round new loops per round (pcm_edges of that pair).  As
+    find_available_loops_detections does, every round re-submits every earlier loop before its new ones; `n_perturbed` of
+    the re-submitted loops carry perturbed values (re-anchoring gives the same id other values), and `n_duplicates` of the
+    round's new loops are submitted twice with the same id.  Ids are above 2^32.
+    -> [(edges, ids int64 [n])] per round."""
+    rng = np.random.default_rng(seed + 9100)
+    drones = range(1, n_drones + 1)
+    pairs = [(a, b) for a in drones for b in drones if a <= b]
+    counts = rng.integers(1, per_round + 1, size=(len(pairs), rounds))
+    per_pair = []
+    for pi, (a, b) in enumerate(pairs):
+        es = pcm_edges(int(counts[pi].sum()), outlier_frac, seed * 1000 + pi, id_a=a, id_b=b)
+        per_pair.append([(e, (1 << 32) + (pi << 20) + 7 * k + 3) for k, e in enumerate(es)])
+    out, earlier, taken = [], [], np.zeros(len(pairs), int)
+    for r in range(rounds):
+        new = []
+        for pi in range(len(pairs)):
+            c = int(counts[pi, r])
+            new += per_pair[pi][taken[pi]:taken[pi] + c]
+            taken[pi] += c
+        new = [new[i] for i in rng.permutation(len(new))]
+        old = list(earlier)
+        for i in (rng.choice(len(old), min(n_perturbed, len(old)), replace=False) if old else []):
+            e, lid = old[i]
+            moved = dict(e, rel=e["rel"] + np.array([0.4, -0.3, 0.2, 0, 0, 0, 0]))
+            old[i] = (moved, lid)
+        dup = [new[i] for i in rng.choice(len(new), min(n_duplicates, len(new)), replace=False)]
+        sub = old + new + dup
+        out.append(([e for e, _ in sub], np.array([i for _, i in sub], np.int64)))
+        earlier += new
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # 3-D / 2-D correspondences of one loop candidate for the PnP stage (SURVEY.md 8f-1, second half)
 # ----------------------------------------------------------------------------------------------------------------
