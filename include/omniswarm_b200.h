@@ -528,6 +528,8 @@ typedef struct {
   int32_t msg_id;
   int32_t n_dirs;
   int32_t reserved;
+  /* the image fields below are the up image's; with osb_frontend_set_main_camera(OSB_MAIN_CAMERA_DOWN) the down image's and
+     stereo_match the other way round (see there) */
   int32_t n_kpts[OSB_MAX_DIRS];                                        /* landmark_num per direction (up image) */
   int32_t n_kpts_down[OSB_MAX_DIRS];
   float global_desc[OSB_MAX_DIRS][OSB_DEEP_DESC_SIZE];                 /* image_desc */
@@ -674,6 +676,22 @@ osb_status osb_frontend_set_profiling(osb_frontend* h, int enable);
 osb_status osb_frontend_stage_ms(osb_frontend* h, float* ms8);
 /* precision of both networks of the front-end (SuperPoint and NetVLAD; see osb_superpoint_set_precision) */
 osb_status osb_frontend_set_precision(osb_frontend* h, int precision);
+/* Which camera of each stereo pair is the main one (the reference's LOWER_CAM_AS_MAIN, swarm_loop.cpp:243).
+ * OSB_MAIN_CAMERA_UP (the default): the record as described above.  OSB_MAIN_CAMERA_DOWN (loop_cam.cpp:341-523): SuperPoint
+ * runs on both images as before, NetVLAD on the DOWN images, and direction d of the record is the down image's:
+ *   kpts, local_desc, n_kpts, landmarks_3d and landmarks_flag are the down image's; n_kpts_down is the UP count;
+ *   stereo_match[d][j] is the up index mutually matched to down keypoint j, or -1;
+ *   with set_cameras the pair is triangulated as in UP mode (in-front test on the up camera) and the point and flag land
+ *   on the down keypoint; without cameras landmarks_flag = stereo_match >= 0;
+ *   when the up count is <= accept_min_3d_pts (the reference returns the up descriptor, which has no global descriptor):
+ *   kpts / local_desc / n_kpts are the up image's, n_kpts_down the up count too, stereo_match -1, no flags and a ZERO
+ *   global_desc, so the direction still adds its database row and no query can accept it.
+ * compute_loop lifts the old frame through the right extrinsics of set_cameras.  Ingest, query and query_received read only
+ * the record and are unchanged.  The call allocates nothing and applies from the next extract on.  OSB_ERR_INVALID after
+ * set_depth_camera; set_depth_camera and the depth extracts return OSB_ERR_INVALID on a DOWN handle. */
+#define OSB_MAIN_CAMERA_UP 0
+#define OSB_MAIN_CAMERA_DOWN 1
+osb_status osb_frontend_set_main_camera(osb_frontend* h, int which);
 
 /* Loop edges on the device -- LoopDetector::compute_loop + the frame-level compute_correspond_features
  *   (loop_detector.cpp:431-537, 627-836): for every hit of a query, the correspondences of its direction pairs, PnP-RANSAC
@@ -684,7 +702,7 @@ osb_status osb_frontend_set_precision(osb_frontend* h, int precision);
  *   query_dir, main_dir_old = hit_dir.  swapped == 1: new = the remote keyframe of the hit (its 3-D landmarks come from the
  *   remote store), old = records[i], and the two main directions are exchanged.  The old frame is always this drone's own, so
  *   its 2-D landmarks are lifted through the handle's camera: the depth camera (set_depth_camera) or the left cameras
- *   (set_cameras); a handle with neither or both gets OSB_ERR_INVALID, as does one without geometric_filter (the reference
+ *   (set_cameras; the right ones after osb_frontend_set_main_camera(OSB_MAIN_CAMERA_DOWN)); a handle with neither or both gets OSB_ERR_INVALID, as does one without geometric_filter (the reference
  *   builds with USE_FUNDMENTAL) or without set_loop_params.
  * Correspondences, in the slot order of osb_loop_result (the reference's dirs_new): slot j contributes geo_new / geo_old when
  *   geo_valid[j] == 1; when geo_valid[j] == 0 it contributes the 0-3 matches whose new landmark is flagged (the per-image

@@ -55,7 +55,11 @@ __device__ __forceinline__ void rot_rows(const double* q, double (&R)[3][3]) {  
 
 struct LiftCam { double fx, fy, cx, cy; };
 
-// one thread per up keypoint of one direction
+// one thread per up keypoint of one direction.  DOWN (LOWER_CAM_AS_MAIN): the 3-D point goes to the down keypoint's slot,
+// as ides_down.landmarks_3d[idx_down] (loop_cam.cpp:443-444); the in-front test stays on the up camera (:418-425).  The
+// slots of unflagged down keypoints are left as they are (each slot has at most one writer, the thread of its up partner,
+// so there is nothing to clear them without a race): read pts3d only where flag_down is set.
+template <bool DOWN>
 __global__ void stereo_lift_kernel(const float* __restrict__ kp_up, const float* __restrict__ kp_down,
                                    const int32_t* __restrict__ match, const int32_t* __restrict__ n_up,
                                    const int32_t* __restrict__ n_down, int max_n, LiftCam cam,
@@ -65,7 +69,7 @@ __global__ void stereo_lift_kernel(const float* __restrict__ kp_up, const float*
   const int d = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= max_n) return;
   const size_t o = (size_t)d * max_n + i;
-  pts3d[o * 3] = 0.f; pts3d[o * 3 + 1] = 0.f; pts3d[o * 3 + 2] = 0.f;
+  if (!DOWN) { pts3d[o * 3] = 0.f; pts3d[o * 3 + 1] = 0.f; pts3d[o * 3 + 2] = 0.f; }
   flag_up[o] = 0;
   // (flag_down is cleared by the caller: several up keypoints never share a down keypoint -- the match is one-to-one)
   const int nu = n_up[d];
@@ -112,7 +116,8 @@ __global__ void stereo_lift_kernel(const float* __restrict__ kp_up, const float*
   // in front of the up camera: (R0^T (p - t0)).z
   const double zc = R0[0][2] * (p[0] - pu[0]) + R0[1][2] * (p[1] - pu[1]) + R0[2][2] * (p[2] - pu[2]);
   if (err > triangle_thres || zc < 0.0 || !(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]))) return;
-  pts3d[o * 3] = (float)p[0]; pts3d[o * 3 + 1] = (float)p[1]; pts3d[o * 3 + 2] = (float)p[2];
+  const size_t op = DOWN ? oj : o;
+  pts3d[op * 3] = (float)p[0]; pts3d[op * 3 + 1] = (float)p[1]; pts3d[op * 3 + 2] = (float)p[2];
   flag_up[o] = 1;
   flag_down[oj] = 1;
 }
@@ -145,11 +150,15 @@ __global__ void depth_lift_kernel(const float* __restrict__ kp, const int32_t* _
 osb_status stereo_lift_device(const float* kp_up, const float* kp_down, const int32_t* match, const int32_t* n_up,
                               const int32_t* n_down, int n_dirs, int max_n, const double* K, const double* pose_up,
                               const double* pose_down, double triangle_thres, int min_pts, float* pts3d, uint8_t* flag_up,
-                              uint8_t* flag_down, cudaStream_t st) {
+                              uint8_t* flag_down, cudaStream_t st, bool down_main) {
   OSB_CUDA(cudaMemsetAsync(flag_down, 0, (size_t)n_dirs * max_n, st));
   const LiftCam cam{K[0], K[1], K[2], K[3]};
-  OSB_LAUNCH(stereo_lift_kernel, dim3(cdiv(max_n, 64), n_dirs), 64, 0, st, kp_up, kp_down, match, n_up, n_down, max_n, cam,
-             pose_up, pose_down, triangle_thres, min_pts, pts3d, flag_up, flag_down);
+  if (down_main)
+    OSB_LAUNCH(stereo_lift_kernel<true>, dim3(cdiv(max_n, 64), n_dirs), 64, 0, st, kp_up, kp_down, match, n_up, n_down, max_n,
+               cam, pose_up, pose_down, triangle_thres, min_pts, pts3d, flag_up, flag_down);
+  else
+    OSB_LAUNCH(stereo_lift_kernel<false>, dim3(cdiv(max_n, 64), n_dirs), 64, 0, st, kp_up, kp_down, match, n_up, n_down, max_n,
+               cam, pose_up, pose_down, triangle_thres, min_pts, pts3d, flag_up, flag_down);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

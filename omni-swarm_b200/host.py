@@ -484,6 +484,14 @@ class KeyframeFrontend(_Handle):
         """'split_fp16' (default) or 'fp16' for both networks of the front-end (osb_frontend_set_precision)"""
         _l.check(self._lib.osb_frontend_set_precision(self._h, _precision(precision)))
 
+    def set_main_camera(self, which: str):
+        """'up' (default) or 'down': the reference's LOWER_CAM_AS_MAIN (osb_frontend_set_main_camera).  With 'down' the
+        record is the down image's, NetVLAD runs on the down images and compute_loop uses the right extrinsics."""
+        cams = {"up": _l.MAIN_CAMERA_UP, "down": _l.MAIN_CAMERA_DOWN}
+        if which not in cams:
+            raise ValueError(f"main camera must be 'up' or 'down', not {which!r}")
+        _l.check(self._lib.osb_frontend_set_main_camera(self._h, cams[which]))
+
     def stage_ms(self) -> dict:
         ms = np.zeros(8, np.float32)
         _l.check(self._lib.osb_frontend_stage_ms(self._h, _l.ptr(ms)))
