@@ -186,9 +186,23 @@ osb_status osb_nv_head_parity(const float* assign_w, const float* assign_b, cons
  *   add: loop_detector.cpp:166,169; search: loop_detector.cpp:213; ntotal: loop_detector.cpp:291).
  * Exact float32 inner product, top-k by descending score, ties by ascending row id, ids = -1 and
  * scores = -inf where fewer than k rows exist.  Rows live in HBM, row-major [capacity][dim].
+ *
+ * Row storage (osb_db_create_storage, osb_frontend_set_db_storage):
+ *  OSB_DB_STORAGE_FP32 (the default, osb_db_create): rows as given -- faiss::IndexFlatIP's semantics.
+ *  OSB_DB_STORAGE_FP16: every row element is stored as __float2half_rn(x) (round to nearest even, overflow to +-inf;
+ *   numpy's astype(float16)), on the device, whichever call adds it.  Half the HBM per row and half the bytes per scan.
+ *   Queries stay fp32: a score is the fp32 inner product of the query with the row converted exactly to fp32, so a search
+ *   returns byte-identical ids and scores to a search of an fp32 database holding the rows already rounded to fp16.  For
+ *   unit-norm rows of dim 4096 a score moves by at most 2^-11 sum|q_i x_i| + 2^-25 sum|q_i| (<= 4.9e-4 + 1.9e-6 for a
+ *   unit query); results near a threshold or a tie can change.
  * -----------------------------------------------------------------------------------------------------------*/
 typedef struct osb_db osb_db;
-osb_status osb_db_create(osb_db** out, int dim, int64_t capacity);
+#define OSB_DB_STORAGE_FP32 0
+#define OSB_DB_STORAGE_FP16 1
+osb_status osb_db_create(osb_db** out, int dim, int64_t capacity);       /* = osb_db_create_storage(..., OSB_DB_STORAGE_FP32) */
+/* capacity x dim elements of the storage's type; OSB_ERR_INVALID for any other storage value.  add / add_dev convert on the
+ * device (the host form stages through the handle's own 64-row buffer); capacity errors, reset and size as for fp32. */
+osb_status osb_db_create_storage(osb_db** out, int dim, int64_t capacity, int storage);
 osb_status osb_db_destroy(osb_db* h);
 osb_status osb_db_add(osb_db* h, int64_t n, const float* x, int64_t* first_id);
 osb_status osb_db_add_dev(osb_db* h, int64_t n, const float* x_dev, int64_t* first_id, void* stream);
@@ -633,7 +647,8 @@ osb_status osb_frontend_finish(osb_frontend* h, void* stream);
 int64_t osb_frontend_db_size(osb_frontend* h, int remote);
 osb_status osb_frontend_db_reset(osb_frontend* h);
 /* bulk-load rows into a database without running the networks (benchmark / replay set-up): global descriptors
- * [n][4096] and optional local descriptors [n][max_num][64] + counts [n] (HOST). */
+ * [n][4096] and optional local descriptors [n][max_num][64] + counts [n] (HOST).  In OSB_DB_STORAGE_FP16 the global
+ * descriptors are converted on the device through a 4 MB staging buffer acquired by the first such load. */
 osb_status osb_frontend_db_load(osb_frontend* h, int remote, int64_t n, const float* global_desc,
                                 const float* local_desc, const int32_t* n_kpts);
 /* Stereo triangulation inside extract (SURVEY.md 8f-3): with the cameras set, every keyframe's record carries the
@@ -676,6 +691,13 @@ osb_status osb_frontend_set_profiling(osb_frontend* h, int enable);
 osb_status osb_frontend_stage_ms(osb_frontend* h, float* ms8);
 /* precision of both networks of the front-end (SuperPoint and NetVLAD; see osb_superpoint_set_precision) */
 osb_status osb_frontend_set_precision(osb_frontend* h, int precision);
+/* Row storage of both keyframe databases' global descriptors (OSB_DB_STORAGE_FP32, the default, or OSB_DB_STORAGE_FP16;
+ * see osb_db).  Ingest and osb_frontend_db_load round every global-descriptor element with __float2half_rn in fp16; local
+ * descriptors, keypoints, flags and landmarks_3d stay fp32, and queries read the records' fp32 descriptors.  Valid only while
+ * both databases are empty (no ingest or db_load since create or osb_frontend_db_reset, even one not yet synchronised);
+ * otherwise OSB_ERR_INVALID and the handle is unchanged.  The two [db_capacity][4096] row planes are freed and acquired
+ * anew (fp16 holds db_capacity x 8 KB less per database).  osb_frontend_db_reset keeps the storage. */
+osb_status osb_frontend_set_db_storage(osb_frontend* h, int storage);
 /* Which camera of each stereo pair is the main one (the reference's LOWER_CAM_AS_MAIN, swarm_loop.cpp:243).
  * OSB_MAIN_CAMERA_UP (the default): the record as described above.  OSB_MAIN_CAMERA_DOWN (loop_cam.cpp:341-523): SuperPoint
  * runs on both images as before, NetVLAD on the DOWN images, and direction d of the record is the down image's:

@@ -106,7 +106,11 @@ class MobileNetVLADB200 {
 class IndexFlatIPB200 {
  public:
   typedef int64_t idx_t;
-  explicit IndexFlatIPB200(int d, int64_t capacity = 65536) : d(d) { check(osb_db_create(&h_, d, capacity), "osb_db_create"); }
+  // use_float16: rows stored as fp16 (faiss GpuIndexFlatConfig::useFloat16; see OSB_DB_STORAGE_FP16)
+  explicit IndexFlatIPB200(int d, int64_t capacity = 65536, bool use_float16 = false) : d(d) {
+    check(osb_db_create_storage(&h_, d, capacity, use_float16 ? OSB_DB_STORAGE_FP16 : OSB_DB_STORAGE_FP32),
+          "osb_db_create_storage");
+  }
   ~IndexFlatIPB200() { osb_db_destroy(h_); }
   void add(idx_t n, const float* x) { check(osb_db_add(h_, n, x, nullptr), "osb_db_add"); ntotal = osb_db_size(h_); }
   void search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const {

@@ -6,10 +6,15 @@ namespace osb {
 
 // ---- match.cu ------------------------------------------------------------------------------------------------
 int db_scan_grid(int64_t n, int64_t* chunk_out);
+// rows: [n][dim] float, or __half with storage == OSB_DB_STORAGE_FP16 (the queries stay fp32)
 // n_dev (optional): true row count in device memory, n is then an upper bound used to size the grid
-osb_status db_search_device(const float* rows, int64_t n, const int64_t* n_dev, int dim, const float* q_dev, int nq,
-                            int k, float* part_scores, int64_t* part_ids, unsigned int* done, float* scores_dev, int64_t* ids_dev,
-                            cudaStream_t st);
+osb_status db_search_device(const void* rows, int storage, int64_t n, const int64_t* n_dev, int dim, const float* q_dev,
+                            int nq, int k, float* part_scores, int64_t* part_ids, unsigned int* done, float* scores_dev,
+                            int64_t* ids_dev, cudaStream_t st);
+// the row plane of a database: n elements of float, or of __half for OSB_DB_STORAGE_FP16, owned by `m`
+osb_status db_rows_alloc(Resources& m, void** rows, size_t n, int storage);
+// dst[i] = __float2half_rn(src[i]) for n elements (n a multiple of 4) of device memory, on `st`
+osb_status db_rows_to_half(__half* dst, const float* src, size_t n, cudaStream_t st);
 // q/t: device tables of n_pairs pointers to [<=max_n][64] descriptor blocks
 // outputs (qi/ti/dout/map_out) are [n_pairs][out_stride] and n_out [n_pairs] -- or, with group > 0, pair p = group * g + s
 // writes them at g * group_stride + s * out_stride and g * group_stride + s (elements): the pairs of record g land in the

@@ -37,7 +37,8 @@ struct FeFeedback {
 // what the kernels see of one database
 struct DbView {
   DbDev* dev;
-  float* rows;                 // [cap][4096]
+  int storage;                 // OSB_DB_STORAGE_FP32 / _FP16: the element type of `rows`
+  void* rows;                  // [cap][4096] float or __half
   float* ldesc;                // [cap][max_num][64]
   float* kpts;                 // [cap][max_num][2]   landmarks_2d of the row (geometric filter)
   int32_t* lflag;              // [cap][max_num]      landmarks_flag of the row (non-zero = the landmark has a 3-D point)
@@ -83,6 +84,7 @@ using FePairs = FePairsT<OSB_MAX_DIRS>;
 
 constexpr int FE_KMAX = 32;
 constexpr int FE_MAX_RECORDS = 64;     // records per ingest / received-keyframe query (one bit each in a 64-bit mask)
+constexpr int FE_LOAD_ROWS = 256;      // rows per staging step of osb_frontend_db_load into an fp16 store (4 MB)
 constexpr int FE_RQ_K = 5 + 1;         // SEARCH_NEAREST_NUM + max_index of a received keyframe's query (loop_detector.cpp:191-195)
 using FeBatchPairs = FePairsT<OSB_MAX_DIRS * FE_MAX_RECORDS>;
 
@@ -215,8 +217,17 @@ __global__ void fe_copy_rows_kernel(const osb_keyframe_record* __restrict__ recs
   const int row = a & ((1 << 30) - 1);
   const osb_keyframe_record* rec = recs + r;
   const float4* g = reinterpret_cast<const float4*>(&rec->global_desc[d][0]);
-  float4* __restrict__ gd = reinterpret_cast<float4*>(db.rows + (size_t)row * OSB_DEEP_DESC_SIZE);
-  for (int i = threadIdx.x; i < OSB_DEEP_DESC_SIZE / 4; i += blockDim.x) gd[i] = g[i];
+  if (db.storage == OSB_DB_STORAGE_FP16) {
+    __half2* __restrict__ gd = reinterpret_cast<__half2*>(static_cast<__half*>(db.rows) + (size_t)row * OSB_DEEP_DESC_SIZE);
+    for (int i = threadIdx.x; i < OSB_DEEP_DESC_SIZE / 4; i += blockDim.x) {
+      const float4 v = g[i];
+      gd[2 * i] = __floats2half2_rn(v.x, v.y);
+      gd[2 * i + 1] = __floats2half2_rn(v.z, v.w);
+    }
+  } else {
+    float4* __restrict__ gd = reinterpret_cast<float4*>(static_cast<float*>(db.rows) + (size_t)row * OSB_DEEP_DESC_SIZE);
+    for (int i = threadIdx.x; i < OSB_DEEP_DESC_SIZE / 4; i += blockDim.x) gd[i] = g[i];
+  }
   const int n = min(rec->n_kpts[d], max_num);
   const float4* l = reinterpret_cast<const float4*>(&rec->local_desc[d][0][0]);
   float4* __restrict__ ld = reinterpret_cast<float4*>(db.ldesc + (size_t)row * max_num * OSB_FEATURE_DESC_SIZE);
@@ -706,6 +717,8 @@ struct osb_frontend {
   uint8_t* d_lc_mask = nullptr;                           // [LC_MAX][LC_MAXN]
   osb_pnp_result* d_lc_pnp = nullptr;
   int32_t* d_assign = nullptr;   // [max_records][4]
+  float* d_load_stage = nullptr;   // [FE_LOAD_ROWS][4096]: osb_frontend_db_load's fp32 -> fp16 staging, acquired by the first
+                                   // load into an fp16 store
   int max_records = FE_MAX_RECORDS;
   osb_keyframe_record* d_record = nullptr;   // used by process()
   osb_loop_result* d_result = nullptr;
@@ -738,7 +751,8 @@ static osb_status dbstore_alloc(Resources& m, DbStore& s, int64_t cap, int max_n
   const size_t c = (size_t)cap, cn = c * max_num;
   OSB_TRY(m.alloc(&v.dev, 1));
   OSB_CUDA(cudaMemset(v.dev, 0, sizeof(DbDev)));
-  OSB_TRY(m.alloc(&v.rows, c * OSB_DEEP_DESC_SIZE));
+  v.storage = OSB_DB_STORAGE_FP32;
+  OSB_TRY(db_rows_alloc(m, &v.rows, c * OSB_DEEP_DESC_SIZE, v.storage));
   OSB_TRY(m.alloc(&v.ldesc, cn * OSB_FEATURE_DESC_SIZE));
   OSB_TRY(m.alloc(&v.kpts, cn * 2));
   OSB_TRY(m.alloc(&v.lflag, cn));
@@ -846,6 +860,33 @@ extern "C" osb_status osb_frontend_set_precision(osb_frontend* h, int precision)
   std::lock_guard<std::mutex> lk(h->mu);
   OSB_TRY(h->sp.set_precision(precision));            // the same check for both networks: nv accepts what sp accepted
   return h->nv.set_precision(precision);
+}
+
+extern "C" osb_status osb_frontend_set_db_storage(osb_frontend* h, int storage) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(storage == OSB_DB_STORAGE_FP32 || storage == OSB_DB_STORAGE_FP16,
+              "storage must be OSB_DB_STORAGE_FP32 or OSB_DB_STORAGE_FP16");
+  std::lock_guard<std::mutex> lk(h->mu);
+  // the host bounds are charged when an ingest is enqueued, so 0 also rules out an ingest that has not run yet
+  OSB_REQUIRE(h->db[0].upper == 0 && h->db[1].upper == 0,
+              "the databases already hold rows: set the storage right after create or osb_frontend_db_reset");
+  DeviceGuard dg(h->device);
+  if (storage == h->db[0].v.storage) return OSB_OK;
+  // both new planes first, so that a failed allocation leaves the handle as it was
+  void* rows[2] = {nullptr, nullptr};
+  for (int i = 0; i < 2; ++i) {
+    const osb_status s = db_rows_alloc(h->res, &rows[i], (size_t)h->db[i].cap * OSB_DEEP_DESC_SIZE, storage);
+    if (s != OSB_OK) {
+      if (i == 1) h->res.release(rows[0]);
+      return s;
+    }
+  }
+  for (int i = 0; i < 2; ++i) {
+    h->res.release(h->db[i].v.rows);
+    h->db[i].v.rows = rows[i];
+    h->db[i].v.storage = storage;
+  }
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_frontend_destroy(osb_frontend* h) {
@@ -1131,9 +1172,9 @@ static osb_status fe_query(osb_frontend* h, const osb_keyframe_record* rec, int 
   // a store that has never received a row needs no scan: its top-k list still holds the -1 labels it was created with
   // (upper is an upper bound of ntotal, so 0 is exact)
   if (R.upper > 0 &&
-      (s = db_search_device(R.v.rows, std::min(R.upper, R.cap), &R.v.dev->ntotal, OSB_DEEP_DESC_SIZE, q, 1, qp.k_remote,
+      (s = db_search_device(R.v.rows, R.v.storage, std::min(R.upper, R.cap), &R.v.dev->ntotal, OSB_DEEP_DESC_SIZE, q, 1, qp.k_remote,
                             R.part_scores, R.part_ids, R.done, R.v.top_scores, R.v.top_ids, st)) != OSB_OK) return s;
-  if ((s = db_search_device(L.v.rows, std::min(L.upper, L.cap), &L.v.dev->ntotal, OSB_DEEP_DESC_SIZE, q, 1, qp.k_local,
+  if ((s = db_search_device(L.v.rows, L.v.storage, std::min(L.upper, L.cap), &L.v.dev->ntotal, OSB_DEEP_DESC_SIZE, q, 1, qp.k_local,
                             L.part_scores, L.part_ids, L.done, L.v.top_scores, L.v.top_ids, st)) != OSB_OK) return s;
   fe_mark(h, 6, st);
   qp.n = 1;
@@ -1186,7 +1227,7 @@ static osb_status fe_query_received(osb_frontend* h, const osb_keyframe_record* 
   OSB_CUDA(cudaMemcpy2DAsync(h->d_rq_desc, OSB_DEEP_DESC_SIZE * sizeof(float), &recs->global_desc[c.query_dir][0],
                              sizeof(osb_keyframe_record), OSB_DEEP_DESC_SIZE * sizeof(float), n, cudaMemcpyDeviceToDevice, st));
   // one scan of the local store for all n (8 queries per pass), top-k per record into the batch's own lists
-  if ((s = db_search_device(L.v.rows, std::min(L.upper, L.cap), &L.v.dev->ntotal, OSB_DEEP_DESC_SIZE, h->d_rq_desc, n,
+  if ((s = db_search_device(L.v.rows, L.v.storage, std::min(L.upper, L.cap), &L.v.dev->ntotal, OSB_DEEP_DESC_SIZE, h->d_rq_desc, n,
                             FE_RQ_K, L.part_scores, L.part_ids, L.done, h->d_rq_scores, h->d_rq_ids, st)) != OSB_OK) return s;
   QueryParams qp = fe_query_params(h);
   qp.n = n;
@@ -1469,8 +1510,19 @@ extern "C" osb_status osb_frontend_db_load(osb_frontend* h, int remote, int64_t 
   OSB_CUDA(cudaMemcpy(&hd, v.dev, sizeof(DbDev), cudaMemcpyDeviceToHost));
   // the frame tables are [cap] too, and a keyframe without keypoints adds a frame but no row (nframes may exceed ntotal)
   if ((int64_t)hd.nframes + n > S.cap) { set_error("osb_frontend_db_load", "frame table capacity exceeded"); return OSB_ERR_CAPACITY; }
-  OSB_CUDA(cudaMemcpyAsync(v.rows + (size_t)base * OSB_DEEP_DESC_SIZE, global_desc,
-                           (size_t)n * OSB_DEEP_DESC_SIZE * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (v.storage == OSB_DB_STORAGE_FP16) {
+    if (!h->d_load_stage) OSB_TRY(h->res.alloc(&h->d_load_stage, (size_t)FE_LOAD_ROWS * OSB_DEEP_DESC_SIZE));
+    for (int64_t r0 = 0; r0 < n; r0 += FE_LOAD_ROWS) {    // stream order protects the staging buffer's reuse
+      const size_t e = (size_t)std::min<int64_t>(FE_LOAD_ROWS, n - r0) * OSB_DEEP_DESC_SIZE;
+      OSB_CUDA(cudaMemcpyAsync(h->d_load_stage, global_desc + (size_t)r0 * OSB_DEEP_DESC_SIZE, e * sizeof(float),
+                               cudaMemcpyHostToDevice, st));
+      OSB_TRY(db_rows_to_half(static_cast<__half*>(v.rows) + (size_t)(base + r0) * OSB_DEEP_DESC_SIZE, h->d_load_stage, e,
+                              st));
+    }
+  } else {
+    OSB_CUDA(cudaMemcpyAsync(static_cast<float*>(v.rows) + (size_t)base * OSB_DEEP_DESC_SIZE, global_desc,
+                             (size_t)n * OSB_DEEP_DESC_SIZE * sizeof(float), cudaMemcpyHostToDevice, st));
+  }
   std::vector<int32_t> nk(n), rf(n), rd(n), fr((size_t)n * OSB_MAX_DIRS, -1), fm(n, -1);
   for (int64_t i = 0; i < n; ++i) {
     nk[i] = (local_desc && n_kpts) ? std::min(n_kpts[i], mn) : 0;

@@ -37,6 +37,19 @@ __device__ __forceinline__ float db_key_score(unsigned long long key) {
   return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
 }
 
+// the one row loader of both scan kernels: V is a group of 4 consecutive row elements, ld() returns them as fp32.  An fp16
+// row is read at the same group (float4 column) index as an fp32 one, 8 bytes instead of 16, so every lane's fmaf chain is
+// the fp32 kernel's own and an fp16 store scores exactly like an fp32 store holding the same rows already rounded to fp16.
+template <typename T> struct DbRow4;
+template <> struct DbRow4<float> {
+  using V = float4;
+  static __device__ __forceinline__ float4 ld(const V* p) { return ld_stream_f4(p); }
+};
+template <> struct DbRow4<__half> {
+  using V = uint2;
+  static __device__ __forceinline__ float4 ld(const V* p) { return ld_stream_h4(reinterpret_cast<const __half*>(p)); }
+};
+
 __device__ void db_emit_and_merge(const float* ss, int ss_stride, int nrows, int64_t row0, int nq, int k,
                                   float* __restrict__ part_scores, int64_t* __restrict__ part_ids,
                                   float* __restrict__ out_scores, int64_t* __restrict__ out_ids, unsigned int* done,
@@ -111,7 +124,7 @@ __device__ void db_emit_and_merge(const float* ss, int ss_stride, int nrows, int
 }
 
 // -------------------------------------------------------------------------------------------------------------
-// db_scan_coop_kernel<Q>: small databases (<= DB_COOP_CHUNK rows per CTA, i.e. <= ~19 k rows; dim = 4096).  With few
+// db_scan_coop_kernel<T,Q>: small databases (<= DB_COOP_CHUNK rows per CTA, i.e. <= ~19 k rows; dim = 4096).  With few
 // rows per CTA the warp-per-row scheme leaves half the warps idle (10 k rows / 296 CTAs = 34 rows = 9 groups of 4 for
 // 16 warps) and too few bytes in flight.  Here ALL 16 warps share every row: warp w owns float4 columns
 // [64w, 64w+64) -- its slice of the queries lives in registers (no shared-memory query copy at all), each lane has
@@ -121,9 +134,9 @@ __device__ void db_emit_and_merge(const float* ss, int ss_stride, int nrows, int
 constexpr int DB_COOP_CHUNK = 64;
 constexpr int DB_COOP_DIM = 4096;
 
-template <int Q>
+template <typename T, int Q>
 __global__ void __launch_bounds__(DB_THREADS, (Q <= 2) ? 2 : 1)
-db_scan_coop_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* __restrict__ n_dev,
+db_scan_coop_kernel(const T* __restrict__ db, int64_t n_val, const int64_t* __restrict__ n_dev,
                     const float* __restrict__ q, int nq, int k, float* __restrict__ part_scores,
                     int64_t* __restrict__ part_ids, float* __restrict__ out_scores, int64_t* __restrict__ out_ids,
                     unsigned int* done, int fuse) {
@@ -150,7 +163,8 @@ db_scan_coop_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* 
     for (int c = 0; c < C; ++c)
       wq[qq][c] = (qq < nq) ? __ldg(reinterpret_cast<const float4*>(q) + (size_t)qq * DIM4 + col + c * 32)
                             : make_float4(0.f, 0.f, 0.f, 0.f);
-  const float4* base = reinterpret_cast<const float4*>(db) + row0 * DIM4 + col;
+  using V = typename DbRow4<T>::V;
+  const V* base = reinterpret_cast<const V*>(db) + row0 * DIM4 + col;
 #pragma unroll 2
   for (int r0 = 0; r0 < nrows; r0 += R) {
     float4 v[R][C];
@@ -158,7 +172,7 @@ db_scan_coop_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* 
     for (int r = 0; r < R; ++r) {
       const int row = min(r0 + r, nrows - 1);                      // clamped: the surplus loads hit a valid row
 #pragma unroll
-      for (int c = 0; c < C; ++c) v[r][c] = ld_stream_f4(base + (size_t)row * DIM4 + c * 32);
+      for (int c = 0; c < C; ++c) v[r][c] = DbRow4<T>::ld(base + (size_t)row * DIM4 + c * 32);
     }
 #pragma unroll
     for (int r = 0; r < R; ++r)
@@ -190,15 +204,15 @@ db_scan_coop_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* 
 }
 
 // -------------------------------------------------------------------------------------------------------------
-// db_scan_kernel<Q,R>: each warp owns R consecutive rows at a time and dots them with Q queries held in shared
+// db_scan_kernel<T,Q,R>: each warp owns R consecutive rows at a time and dots them with Q queries held in shared
 // memory; a lane streams float4 columns lane, lane+32, ... of all R rows (R independent 16-byte loads in flight,
 // 512 contiguous bytes per row per warp instruction).  Scores of the CTA's row chunk are parked in shared memory
 // and the CTA emits its own top-k by rank counting (score desc, row id asc: the library's documented tie rule).
 // -------------------------------------------------------------------------------------------------------------
 
-template <int Q, int R>
+template <typename T, int Q, int R>
 __global__ void __launch_bounds__(DB_THREADS)
-db_scan_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* __restrict__ n_dev, int dim,
+db_scan_kernel(const T* __restrict__ db, int64_t n_val, const int64_t* __restrict__ n_dev, int dim,
                const float* __restrict__ q, int nq, int k, float* __restrict__ part_scores,
                int64_t* __restrict__ part_ids, float* __restrict__ out_scores, int64_t* __restrict__ out_ids,
                unsigned int* done, int fuse) {
@@ -226,12 +240,13 @@ db_scan_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* __res
   const int ngroups = (nrows + R - 1) / R;
   for (int g = warp; g < ngroups; g += nwarps) {
     const int64_t r0 = row0 + (int64_t)g * R;
-    const float4* rp[R];
+    using V = typename DbRow4<T>::V;
+    const V* rp[R];
     bool valid[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       valid[r] = (r0 + r) < row0 + nrows;
-      rp[r] = reinterpret_cast<const float4*>(db + (valid[r] ? (r0 + r) : r0) * (int64_t)dim);
+      rp[r] = reinterpret_cast<const V*>(db + (valid[r] ? (r0 + r) : r0) * (int64_t)dim);
     }
     float acc[R][Q];
 #pragma unroll
@@ -242,7 +257,7 @@ db_scan_kernel(const float* __restrict__ db, int64_t n_val, const int64_t* __res
     for (int j = lane; j < dim4; j += 32) {
       float4 v[R];
 #pragma unroll
-      for (int r = 0; r < R; ++r) v[r] = ld_stream_f4(rp[r] + j);
+      for (int r = 0; r < R; ++r) v[r] = DbRow4<T>::ld(rp[r] + j);
 #pragma unroll
       for (int qq = 0; qq < Q; ++qq) {
         const float4 w = reinterpret_cast<const float4*>(sq + (size_t)qq * dim)[j];
@@ -295,22 +310,22 @@ db_merge_kernel(const float* __restrict__ part_scores, const int64_t* __restrict
   if (lane == 0 && rank < k) { out_scores[qq * k + rank] = si; out_ids[qq * k + rank] = idi; }
 }
 
-template <int Q>
-static osb_status launch_scan(const float* db, int64_t n, const int64_t* n_dev, int dim, const float* q, int nq,
+template <int Q, typename T>
+static osb_status launch_scan(const T* db, int64_t n, const int64_t* n_dev, int dim, const float* q, int nq,
                               int k, int grid, bool coop, float* ps, int64_t* pi, float* os, int64_t* oi,
                               unsigned int* done, int fuse, cudaStream_t st) {
   constexpr int R = 4;
   const size_t merge_bytes = fuse ? (size_t)(DB_MERGE_MAX + DB_FUSE_KMAX * DB_FUSE_KMAX) * sizeof(unsigned long long) : 0;
   if (coop) {
     const size_t smem = std::max(merge_bytes, (size_t)(DB_THREADS / 32 + 1) * DB_COOP_CHUNK * Q * sizeof(float));
-    OSB_SMEM_OPT_IN(db_scan_coop_kernel<Q>, 64 * 1024);
-    OSB_LAUNCH((db_scan_coop_kernel<Q>), grid, DB_THREADS, smem, st, db, n, n_dev, q, nq, k, ps, pi, os, oi, done, fuse);
+    OSB_SMEM_OPT_IN((db_scan_coop_kernel<T, Q>), 64 * 1024);
+    OSB_LAUNCH((db_scan_coop_kernel<T, Q>), grid, DB_THREADS, smem, st, db, n, n_dev, q, nq, k, ps, pi, os, oi, done, fuse);
     OSB_CHECK_LAUNCH();
     return OSB_OK;
   }
   const size_t smem = std::max(merge_bytes, ((size_t)Q * dim + (size_t)Q * DB_CHUNK_MAX) * sizeof(float));
-  OSB_SMEM_OPT_IN((db_scan_kernel<Q, R>), DB_SCAN_SMEM);
-  OSB_LAUNCH((db_scan_kernel<Q, R>), grid, DB_THREADS, smem, st, db, n, n_dev, dim, q, nq, k, ps, pi, os, oi, done, fuse);
+  OSB_SMEM_OPT_IN((db_scan_kernel<T, Q, R>), DB_SCAN_SMEM);
+  OSB_LAUNCH((db_scan_kernel<T, Q, R>), grid, DB_THREADS, smem, st, db, n, n_dev, dim, q, nq, k, ps, pi, os, oi, done, fuse);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }
@@ -329,8 +344,9 @@ int db_scan_grid(int64_t n, int64_t* chunk_out) {
 }
 
 // device-side search of up to 8 queries per pass; the scratch holds 8*grid_max*k floats / int64 and one ticket counter
-// (zero between searches).  n is an upper bound of *n_dev when n_dev is given.
-osb_status db_search_device(const float* rows, int64_t n, const int64_t* n_dev, int dim, const float* q_dev, int nq,
+// (zero between searches).  n is an upper bound of *n_dev when n_dev is given.  rows are float or, with
+// storage == OSB_DB_STORAGE_FP16, __half; the grid, kernel choice, passes and merge do not depend on the storage.
+osb_status db_search_device(const void* rows, int storage, int64_t n, const int64_t* n_dev, int dim, const float* q_dev, int nq,
                             int k, float* part_scores, int64_t* part_ids, unsigned int* done, float* scores_dev,
                             int64_t* ids_dev, cudaStream_t st) {
   int64_t chunk;
@@ -347,11 +363,14 @@ osb_status db_search_device(const float* rows, int64_t n, const int64_t* n_dev, 
     const float* qp = q_dev + (size_t)q0 * dim;
     float* os = scores_dev + (size_t)q0 * k;
     int64_t* oi = ids_dev + (size_t)q0 * k;
-    osb_status s;
-    if (nb == 1) s = launch_scan<1>(rows, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
-    else if (nb == 2) s = launch_scan<2>(rows, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
-    else if (nb <= 4) s = launch_scan<4>(rows, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
-    else s = launch_scan<8>(rows, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
+    auto scan = [&](auto* r) {
+      if (nb == 1) return launch_scan<1>(r, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
+      if (nb == 2) return launch_scan<2>(r, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
+      if (nb <= 4) return launch_scan<4>(r, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
+      return launch_scan<8>(r, n, n_dev, dim, qp, nb, k, grid, coop, part_scores, part_ids, os, oi, done, fuse, st);
+    };
+    const osb_status s = storage == OSB_DB_STORAGE_FP16 ? scan(static_cast<const __half*>(rows))
+                                                        : scan(static_cast<const float*>(rows));
     if (s != OSB_OK) return s;
     if (!fuse) {
       OSB_LAUNCH(db_merge_kernel, dim3(cdiv(grid * k, 32), nb), 1024, 0, st, part_scores, part_ids, grid * k, k, os, oi);
@@ -491,6 +510,37 @@ bf_crosscheck_kernel(const float* __restrict__ dist, const int32_t* __restrict__
   if (tid == 0) n_out[gbase + pair % group] = total;
 }
 
+osb_status db_rows_alloc(Resources& m, void** rows, size_t n, int storage) {
+  if (storage == OSB_DB_STORAGE_FP16) {
+    __half* p = nullptr;
+    OSB_TRY(m.alloc(&p, n));
+    *rows = p;
+  } else {
+    float* p = nullptr;
+    OSB_TRY(m.alloc(&p, n));
+    *rows = p;
+  }
+  return OSB_OK;
+}
+
+__global__ void db_rows_to_half_kernel(__half2* __restrict__ dst, const float4* __restrict__ src, size_t n4) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+    const float4 v = src[i];
+    dst[2 * i] = __floats2half2_rn(v.x, v.y);
+    dst[2 * i + 1] = __floats2half2_rn(v.z, v.w);
+  }
+}
+
+osb_status db_rows_to_half(__half* dst, const float* src, size_t n, cudaStream_t st) {
+  const size_t n4 = n / 4;
+  if (n4 == 0) return OSB_OK;
+  const int grid = (int)std::min<size_t>(cdiv64((int64_t)n4, 256), (size_t)8 * num_sms());
+  OSB_LAUNCH(db_rows_to_half_kernel, grid, 256, 0, st, reinterpret_cast<__half2*>(dst),
+             reinterpret_cast<const float4*>(src), n4);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
 osb_status bf_match_device(int n_pairs, int max_n, int out_stride, const float* const* q, const int32_t* nq,
                            const float* const* t,
                            const int32_t* nt, float* dist_scratch, int32_t* qi, int32_t* ti, float* dout,
@@ -518,7 +568,8 @@ struct osb_db {
   int device = 0;
   int dim = 0;
   int64_t cap = 0, ntotal = 0;
-  float* rows = nullptr;
+  int storage = OSB_DB_STORAGE_FP32;
+  void* rows = nullptr;             // [cap][dim] float, or __half in OSB_DB_STORAGE_FP16
   float* part_scores = nullptr;
   int64_t* part_ids = nullptr;
   unsigned int* done = nullptr;     // ticket counter of the fused merge
@@ -530,16 +581,18 @@ struct osb_db {
   std::mutex mu;
 };
 
-extern "C" osb_status osb_db_create(osb_db** out, int dim, int64_t capacity) {
+extern "C" osb_status osb_db_create_storage(osb_db** out, int dim, int64_t capacity, int storage) {
   OSB_REQUIRE(out != nullptr && dim > 0 && dim % 4 == 0 && dim <= 8192 && capacity > 0, "bad dim/capacity");
+  OSB_REQUIRE(storage == OSB_DB_STORAGE_FP32 || storage == OSB_DB_STORAGE_FP16,
+              "storage must be OSB_DB_STORAGE_FP32 or OSB_DB_STORAGE_FP16");
   OSB_TRY(require_device());
   std::unique_ptr<osb_db> h(new osb_db());
   h->device = current_device();
-  h->dim = dim; h->cap = capacity;
+  h->dim = dim; h->cap = capacity; h->storage = storage;
   int64_t chunk;
   h->grid_max = db_scan_grid(capacity, &chunk);
   OSB_TRY(h->res.stream(&h->stream));
-  OSB_TRY(h->res.alloc(&h->rows, (size_t)capacity * dim));
+  OSB_TRY(db_rows_alloc(h->res, &h->rows, (size_t)capacity * dim, storage));
   OSB_TRY(h->res.alloc(&h->part_scores, (size_t)8 * h->grid_max * h->kmax));
   OSB_TRY(h->res.alloc(&h->part_ids, (size_t)8 * h->grid_max * h->kmax));
   OSB_TRY(h->res.alloc(&h->done, 1));
@@ -549,6 +602,10 @@ extern "C" osb_status osb_db_create(osb_db** out, int dim, int64_t capacity) {
   OSB_TRY(h->res.alloc(&h->d_ids, (size_t)h->qmax * h->kmax));
   *out = h.release();
   return OSB_OK;
+}
+
+extern "C" osb_status osb_db_create(osb_db** out, int dim, int64_t capacity) {
+  return osb_db_create_storage(out, dim, capacity, OSB_DB_STORAGE_FP32);
 }
 
 extern "C" osb_status osb_db_destroy(osb_db* h) {
@@ -572,8 +629,19 @@ static osb_status db_add_impl(osb_db* h, int64_t n, const float* x, int64_t* fir
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   if (h->ntotal + n > h->cap) { set_error("osb_db_add", "capacity exceeded"); return OSB_ERR_CAPACITY; }
-  if (n > 0)
-    OSB_CUDA(cudaMemcpyAsync(h->rows + (size_t)h->ntotal * h->dim, x, (size_t)n * h->dim * sizeof(float), kind, st));
+  const size_t off = (size_t)h->ntotal * h->dim;
+  if (n > 0 && h->storage == OSB_DB_STORAGE_FP32) {
+    OSB_CUDA(cudaMemcpyAsync(static_cast<float*>(h->rows) + off, x, (size_t)n * h->dim * sizeof(float), kind, st));
+  } else if (n > 0 && kind == cudaMemcpyDeviceToDevice) {
+    OSB_TRY(db_rows_to_half(static_cast<__half*>(h->rows) + off, x, (size_t)n * h->dim, st));
+  } else if (n > 0) {
+    // host rows: staged through the query buffer d_q, qmax rows at a time (stream order protects its reuse)
+    for (int64_t r0 = 0; r0 < n; r0 += h->qmax) {
+      const size_t e = (size_t)std::min<int64_t>(h->qmax, n - r0) * h->dim;
+      OSB_CUDA(cudaMemcpyAsync(h->d_q, x + (size_t)r0 * h->dim, e * sizeof(float), kind, st));
+      OSB_TRY(db_rows_to_half(static_cast<__half*>(h->rows) + off + (size_t)r0 * h->dim, h->d_q, e, st));
+    }
+  }
   if (first_id) *first_id = h->ntotal;
   h->ntotal += n;
   if (sync) OSB_CUDA(cudaStreamSynchronize(st));
@@ -596,7 +664,7 @@ extern "C" osb_status osb_db_search_dev(osb_db* h, int64_t nq, const float* q_de
   OSB_REQUIRE(k > 0 && k <= h->kmax && nq > 0, "k must be in 1..64 and nq > 0");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  return db_search_device(h->rows, h->ntotal, nullptr, h->dim, q_dev, (int)nq, k, h->part_scores, h->part_ids, h->done, scores_dev,
+  return db_search_device(h->rows, h->storage, h->ntotal, nullptr, h->dim, q_dev, (int)nq, k, h->part_scores, h->part_ids, h->done, scores_dev,
                           ids_dev, (cudaStream_t)stream);
 }
 
@@ -643,7 +711,7 @@ extern "C" osb_status osb_db_search(osb_db* h, int64_t nq, const float* q, int k
     const int nb = (int)std::min<int64_t>(h->qmax, nq - q0);
     OSB_CUDA(cudaMemcpyAsync(h->d_q, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float),
                              cudaMemcpyHostToDevice, h->stream));
-    osb_status s = db_search_device(h->rows, h->ntotal, nullptr, h->dim, h->d_q, nb, k, h->part_scores, h->part_ids, h->done,
+    osb_status s = db_search_device(h->rows, h->storage, h->ntotal, nullptr, h->dim, h->d_q, nb, k, h->part_scores, h->part_ids, h->done,
                                     h->d_scores, h->d_ids, h->stream);
     if (s != OSB_OK) return s;
     OSB_CUDA(cudaMemcpyAsync(scores + (size_t)q0 * k, h->d_scores, (size_t)nb * k * sizeof(float),

@@ -24,6 +24,17 @@ def _f32(a):
 PRECISIONS = {"split_fp16": _l.PRECISION_SPLIT_FP16, "fp16": _l.PRECISION_FP16}
 
 
+DB_STORAGES = {"fp32": _l.DB_STORAGE_FP32, "fp16": _l.DB_STORAGE_FP16}
+
+
+def _db_storage(name: str) -> int:
+    """'fp32' (the default: rows as given, faiss::IndexFlatIP) or 'fp16' (rows rounded to nearest-even fp16, half the bytes
+    per scan; queries stay fp32) -> OSB_DB_STORAGE_*"""
+    if name not in DB_STORAGES:
+        raise ValueError(f"storage must be one of {sorted(DB_STORAGES)}, not {name!r}")
+    return DB_STORAGES[name]
+
+
 def _precision(name: str) -> int:
     """'split_fp16' (the default: two fp16 planes per operand, fp32-level accuracy) or 'fp16' (plain fp16 operands, the
     precision of the reference's fp16 TensorRT engines) -> OSB_PRECISION_*"""
@@ -147,11 +158,12 @@ class IndexFlatIP(_Handle):
 
     _destroy = "osb_db_destroy"
 
-    def __init__(self, d: int, capacity: int = 16384):
+    def __init__(self, d: int, capacity: int = 16384, storage: str = "fp32"):
+        """storage 'fp16' keeps every row as float16 (round to nearest even; osb_db_create_storage)"""
         self._lib = _l.load()
         self.d = d
         self._h = C.c_void_p()
-        _l.check(self._lib.osb_db_create(C.byref(self._h), d, capacity))
+        _l.check(self._lib.osb_db_create_storage(C.byref(self._h), d, capacity, _db_storage(storage)))
 
     @property
     def ntotal(self) -> int:
@@ -483,6 +495,11 @@ class KeyframeFrontend(_Handle):
     def set_precision(self, precision: str):
         """'split_fp16' (default) or 'fp16' for both networks of the front-end (osb_frontend_set_precision)"""
         _l.check(self._lib.osb_frontend_set_precision(self._h, _precision(precision)))
+
+    def set_db_storage(self, storage: str):
+        """'fp32' (default) or 'fp16' for the global-descriptor rows of both databases (osb_frontend_set_db_storage); only
+        while both are empty"""
+        _l.check(self._lib.osb_frontend_set_db_storage(self._h, _db_storage(storage)))
 
     def set_main_camera(self, which: str):
         """'up' (default) or 'down': the reference's LOWER_CAM_AS_MAIN (osb_frontend_set_main_camera).  With 'down' the

@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(CSRC, "libomniswarm_b200.so")
 OK, ERR_INVALID, ERR_CUDA, ERR_CAPACITY, ERR_NO_DEVICE = 0, 1, 2, 3, 4
 PRECISION_SPLIT_FP16, PRECISION_FP16 = 0, 1
 MAIN_CAMERA_UP, MAIN_CAMERA_DOWN = 0, 1
+DB_STORAGE_FP32, DB_STORAGE_FP16 = 0, 1
 MAX_DIRS, MAX_KPTS, FEATURE_DESC_SIZE, DEEP_DESC_SIZE = 4, 200, 64, 4096
 REMOTE_MAGIN_NUMBER = 1000000
 SWARM_ID_BYTES = 128
@@ -172,6 +173,7 @@ _SIG = {
     "osb_nv_block0_parity": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "osb_nv_head_parity": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "osb_db_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int64]),
+    "osb_db_create_storage": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int64, C.c_int]),
     "osb_db_destroy": (C.c_int, [_P]),
     "osb_db_add": (C.c_int, [_P, C.c_int64, _P, C.POINTER(C.c_int64)]),
     "osb_db_add_dev": (C.c_int, [_P, C.c_int64, _P, C.POINTER(C.c_int64), _P]),
@@ -222,6 +224,7 @@ _SIG = {
     "osb_frontend_stage_ms": (C.c_int, [_P, _P]),
     "osb_frontend_set_precision": (C.c_int, [_P, C.c_int]),
     "osb_frontend_set_main_camera": (C.c_int, [_P, C.c_int]),
+    "osb_frontend_set_db_storage": (C.c_int, [_P, C.c_int]),
     "osb_frontend_db_size": (C.c_int64, [_P, C.c_int]),
     "osb_frontend_db_reset": (C.c_int, [_P]),
     "osb_frontend_db_load": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P]),
