@@ -2,8 +2,9 @@
 //
 // Layers: swarm_loop/superpoint.ipynb:143-158 of the reference (3x3 pad 1 and 1x1 convolutions, NHWC here).
 //
-// Implicit GEMM, one CTA tile = 8 x 16 output pixels (M = 128) x N output channels (N = 64, 80 or 128; layers of 256 / 512
-// channels run as 2 / 4 work items of 128 channels per tile):
+// Implicit GEMM, one CTA tile = 8 x 16 output pixels (M = 128) x N output channels (conv_umma_kernel: N = 64 or 80; the
+// 128-channel layers, and those of 256 / 512 channels as 2 / 4 work items of 128 channels per tile, run transposed in
+// conv_stream_t_kernel, below):
 //   * A operand: for every horizontal filter tap kx and every 64-channel slab, ONE TMA box {64 ch, 16 x, 8 + 2 y, 1 image}
 //     fetched at the kx-shifted coordinate; out-of-image elements are zero-filled by the TMA unit, which is the
 //     convolution's zero padding.  The box lands in shared memory as one 128-byte row per pixel with the 128-byte swizzle,
@@ -61,12 +62,13 @@ static_assert(128 * UM_PRODUCER_REGS + UM_CONSUMERS * UM_CONSUMER_REGS <= 65536,
 // the slots of the split form (B_SLOT = B_BYTES).
 template <int N, bool FP16 = false>
 struct UmmaCfg {
+  static_assert(N == 64 || N == 80, "128-channel layers run in conv_stream_t_kernel");
   static constexpr int PLANES = FP16 ? 1 : 2;
   static constexpr int A_SLOTS = FP16 ? 4 : UM_A_SLOTS;
   static constexpr int A_RING = A_SLOTS * PLANES * UM_A_SLOT;    // 80 KB either way
   static constexpr int B_BYTES = N * 128;                        // one weight plane of one tap / slab
   static constexpr int B_SLOT = PLANES * B_BYTES;                // hi (+ lo)
-  static constexpr int B_SLOTS = FP16 ? ((N <= 64) ? 12 : (N <= 80) ? 10 : 8) : ((N <= 64) ? 6 : (N <= 80) ? 5 : 4);
+  static constexpr int B_SLOTS = FP16 ? ((N <= 64) ? 12 : 10) : ((N <= 64) ? 6 : 5);
   static constexpr int SMEM_BYTES = A_RING + B_SLOTS * B_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
   static_assert(2 * (A_SLOTS + B_SLOTS) * 8 <= 256, "barriers exceed their 256 bytes");
@@ -85,6 +87,24 @@ struct R64Cfg {
   static constexpr int SMEM_BYTES = A_RING + 9 * W_SLOT + 1024 /*alignment slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
   static_assert((3 * A_SLOTS + 9) * 8 <= 256, "barriers exceed their 256 bytes");
+};
+// conv_stream_t_kernel: a ring of A boxes read by both consumer warpgroups, and per warpgroup a ring of weight HALF slots
+// (the 64 rows [64g, 64g + 64) of the item's 128-row slab; hi (+ lo)).  Split: 3 boxes of 40 KB + 2 x 3 half slots of
+// 16 KB = 216 KB; fp16: 6 boxes of 20 KB + 2 x 6 half slots of 8 KB = 216 KB.  With the commit-group release rule a
+// warpgroup holds at most two boxes and two of its half slots, so any ring of at least 3 boxes and 3 half slots runs,
+// with room for one warpgroup to run ahead of the other.
+template <bool FP16 = false>
+struct StreamTCfg {
+  static constexpr int PLANES = FP16 ? 1 : 2;
+  static constexpr int A_SLOTS = FP16 ? 6 : 3;
+  static constexpr int A_RING = A_SLOTS * PLANES * UM_A_SLOT;    // 120 KB either way
+  static constexpr int W_PLANE = 64 * 128;                       // [64 oc][64 ch] fp16
+  static constexpr int W_SLOT = PLANES * W_PLANE;                // W_hi (| W_lo) of one half
+  static constexpr int W_SLOTS = FP16 ? 6 : 3;                   // per warpgroup
+  static constexpr int SMEM_BYTES = A_RING + 2 * W_SLOTS * W_SLOT + 1024 /*alignment slack*/ + 512 /*barriers*/;
+  static_assert(A_SLOTS >= 3 && W_SLOTS >= 3, "the rings need three slots each for the two warpgroups to run apart");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared-memory plan exceeds the 227 KB of an H100 block");
+  static_assert(2 * (A_SLOTS + 2 * W_SLOTS) * 8 <= 512, "barriers exceed their 512 bytes");
 };
 
 struct UmmaArgs {
@@ -128,7 +148,7 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t4) {
 }
 
 // FP16: the plain-fp16 form (UmmaCfg): tm_a_lo / tm_w_lo and P.out_lo are not used
-template <int N, bool SPLIT, bool FP16 = false>
+template <int N, bool FP16 = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
@@ -146,9 +166,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
   const int lane = threadIdx.x & 31;
   const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
   const int n_tiles = P.B * tiles_x * tiles_y;
-  // work item = (tile, channel block): items of one tile are adjacent, so concurrent CTAs share its activations in L2
-  const int n_split = SPLIT ? P.n_split : 1;          // compile-time 1 for ordinary layers: no div / mod per item
-  const int n_items = n_tiles * n_split;
   const int halo = P.ks / 2;
   const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_ROW;   // bytes of one A plane box
 
@@ -172,8 +189,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
       // ===================== TMA producer =====================
       int as = 0; uint32_t aph = 0;
       int bs = 0; uint32_t bph = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
         const int x0 = tx * UM_TW, y0 = ty * UM_TH;
         for (int kx = 0; kx < P.ks; ++kx) {
@@ -189,8 +205,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
               mbar_wait(b_empty(bs), bph ^ 1);
               const uint32_t sb = b_base + bs * Cfg::B_SLOT;
               mbar_expect_tx(b_full(bs), Cfg::B_SLOT);
-              tma_load_3d(sb, &tm_w_hi, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
-              if constexpr (!FP16) tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, n_off, ky * P.ks + kx);
+              tma_load_3d(sb, &tm_w_hi, b_full(bs), cs * UM_KC, P.n_off, ky * P.ks + kx);
+              if constexpr (!FP16) tma_load_3d(sb + Cfg::B_BYTES, &tm_w_lo, b_full(bs), cs * UM_KC, P.n_off, ky * P.ks + kx);
               if (++bs == BS) { bs = 0; bph ^= 1; }
             }
           }
@@ -215,8 +231,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
       if (a_slot >= 0) mbar_arrive(a_empty(a_slot));
       if (b_slot >= 0) mbar_arrive(b_empty(b_slot));
     };
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * N : P.n_off;
+    const int n_off = P.n_off;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // two fragments of the same shape (N/2 registers each): main = hi*hi, cross = hi*lo + lo*hi.  Disjoint register sets --
       // an MMA into part of another MMA's fragment would make the compiler serialize the wgmma pipeline.  fp16: main only
       float acc[N / 2], cross[FP16 ? 1 : N / 2];
@@ -418,6 +434,117 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
 // order, three boxes per tile.  Each slot has one full barrier per warpgroup, so that a warpgroup's parity sequence counts
 // only its own boxes, and one empty barrier on which the single reader of a box arrives.
 // FP16: one wgmma W_hi*X_hi per K step on hi-only boxes and resident W_hi (R64Cfg); tm_a_lo / tm_w_lo are not used.
+//
+// tr_epilogue: bias, ReLU / ReLU6, optional 2x2 max-pool and the stores of one warpgroup's D[64 oc][128 px] fragment of
+// this layout (conv_res64_kernel and conv_stream_t_kernel).  c_abs is the output channel of fragment row 0, c_rel the
+// same channel counted from the launch's first one (P.n_off; compared with P.out_c); bias[h] is channel
+// c_abs + 16w + 8h + lane/4.  NHWC outputs want channel-contiguous stores, so the split planes and the fp32 values are
+// transposed across the warp in registers (movmatrix): afterwards a quad holds one pixel's 8-channel block.
+template <bool FP16>
+__device__ __forceinline__ void tr_epilogue(const float (&acc)[64], const float (&cross)[FP16 ? 1 : 64],
+                                            const float (&bias)[2], int c_abs, int c_rel, int tile, int tiles_x,
+                                            int tiles_y, const UmmaArgs& P, int w, int r, int t4) {
+  if (c_rel + 16 * w >= P.out_c) return;                     // warp-uniform; out_c is a multiple of 16
+  const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+  const int x0 = tx * UM_TW, y0 = ty * UM_TH;
+  auto value = [&](int k, int h) {                           // fragment register k, channel half h
+    float a;
+    if constexpr (FP16) a = fmaf(acc[k], P.inv_scale, bias[h]);
+    else a = fmaf(acc[k] + cross[k], P.inv_scale, bias[h]);
+    if (P.relu) a = fmaxf(a, 0.f);
+    if (P.relu == 2) a = fminf(a, 6.f);
+    return a;
+  };
+  // split a channel's values of two pixels into the planes and transpose the 8 x 8 (channel x pixel) blocks of the
+  // warp: afterwards lane l holds channels 2 (l % 4), + 1 of pixel l / 4, so a quad holds 16 contiguous bytes.
+  // fp16: the hi plane only (tl is not written)
+  auto split_t = [&](float v0, float v1, uint32_t& th, uint32_t& tl) {
+    const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
+    const __half2 hp = __floats2half2_rn(s0, s1);            // packed conversions: the roundings of two scalar ones
+    if constexpr (FP16) {
+      th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
+    } else {
+      const float2 hf = __half22float2(hp);
+      const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
+      th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
+      tl = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&lp));
+    }
+  };
+  if (!P.pool && !P.out_f32) {
+    // unpooled planes: the four blocks (n-group 2y + k / 2, channel half k % 2) of tile row y are transposed across the
+    // quad as well, so that lane t4 holds block t4 whole and writes it with one 16-byte store: column 8 (t4 / 2) + r,
+    // channels c_abs + 16w + 8 (t4 % 2) .. + 7
+#pragma unroll
+    for (int y = 0; y < UM_TH; ++y) {
+      uint32_t th[4], tl[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int j = 2 * y + (k >> 1), h = k & 1;
+        split_t(value(4 * j + 2 * h, h), value(4 * j + 2 * h + 1, h), th[k], tl[k]);
+      }
+      quad_transpose(th, t4);
+      if constexpr (!FP16) quad_transpose(tl, t4);
+      const int gy = y0 + y, gx = x0 + 8 * (t4 >> 1) + r;
+      if (gy < P.H && gx < P.W) {
+        const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_abs + 16 * w + 8 * (t4 & 1);
+        *reinterpret_cast<uint4*>(P.out_hi + o) = make_uint4(th[0], th[1], th[2], th[3]);
+        if constexpr (!FP16) *reinterpret_cast<uint4*>(P.out_lo + o) = make_uint4(tl[0], tl[1], tl[2], tl[3]);
+      }
+    }
+    return;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int cb = 16 * w + 8 * h;                           // first channel of the warp's 8-channel block
+    const int c_own = c_abs + cb + r, c_st = c_abs + cb + 2 * t4;
+    if (P.pool) {
+      // pooled row py of the tile, pooled column 4k + t4 from n-groups j = 4py + k and j + 2
+      const int Hp = P.H >> 1, Wp = P.W >> 1;
+#pragma unroll
+      for (int py = 0; py < UM_TH / 2; ++py) {
+        float m[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int j = 4 * py + k;
+          m[k] = fmaxf(fmaxf(value(4 * j + 2 * h, h), value(4 * (j + 2) + 2 * h, h)),
+                       fmaxf(value(4 * j + 2 * h + 1, h), value(4 * (j + 2) + 2 * h + 1, h)));
+        }
+        const int gpy = ty * (UM_TH / 2) + py;
+        if (P.out_f32) {
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            const int gpx = tx * (UM_TW / 2) + 4 * k + t4;
+            if (gpy < Hp && gpx < Wp) P.out_f32[(((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_own] = m[k];
+          }
+        } else {
+          // column 2 t4 + k of the block is pooled pixel 4k + t4: after the transpose lane l holds pixel
+          // 4 ((l / 4) & 1) + (l / 4) / 2
+          uint32_t th, tl;
+          split_t(m[0], m[1], th, tl);
+          const int gpx = tx * (UM_TW / 2) + 4 * (r & 1) + (r >> 1);
+          if (gpy < Hp && gpx < Wp) {
+            const size_t o = (((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_st;
+            *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
+            if constexpr (!FP16) *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
+          }
+        }
+      }
+    } else {
+      // fp32: the low and the high 16 bits of each value are transposed as two b16 blocks and put back together, so
+      // that lane l holds channels c_st, c_st + 1 of pixel column 8 (j & 1) + l / 4 for one 8-byte store
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const uint32_t u0 = __float_as_uint(value(4 * j + 2 * h, h)), u1 = __float_as_uint(value(4 * j + 2 * h + 1, h));
+        const uint32_t tlo = movmatrix_trans(__byte_perm(u0, u1, 0x5410)), thi = movmatrix_trans(__byte_perm(u0, u1, 0x7632));
+        const int gy = y0 + (j >> 1), gx = x0 + 8 * (j & 1) + r;
+        if (gy < P.H && gx < P.W)
+          *reinterpret_cast<float2*>(P.out_f32 + (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_st) =
+              make_float2(__uint_as_float(__byte_perm(tlo, thi, 0x5410)), __uint_as_float(__byte_perm(tlo, thi, 0x7632)));
+      }
+    }
+  }
+}
+
 template <bool FP16 = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -527,93 +654,160 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 #pragma unroll
       for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
 
-      // ---- epilogue ----
-      const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
-      const int x0 = tx * UM_TW, y0 = ty * UM_TH;
-      auto value = [&](int k, int h) {                       // fragment register k, channel half h
-        float a;
-        if constexpr (FP16) a = fmaf(acc[k], P.inv_scale, bias[h]);
-        else a = fmaf(acc[k] + cross[k], P.inv_scale, bias[h]);
-        if (P.relu) a = fmaxf(a, 0.f);
-        if (P.relu == 2) a = fminf(a, 6.f);
-        return a;
-      };
-      // split a channel's values of two pixels into the planes and transpose the 8 x 8 (channel x pixel) blocks of the
-      // warp: afterwards lane l holds channels 2 (l % 4), + 1 of pixel l / 4, so a quad writes 16 contiguous bytes.
-      // fp16: the hi plane only (tl is not written)
-      auto split_t = [&](float v0, float v1, uint32_t& th, uint32_t& tl) {
-        const float s0 = v0 * P.out_scale, s1 = v1 * P.out_scale;
-        const __half2 hp = __floats2half2_rn(s0, s1);          // packed conversions: the roundings of two scalar ones
-        if constexpr (FP16) {
-          th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
-        } else {
-          const float2 hf = __half22float2(hp);
-          const __half2 lp = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
-          th = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&hp));
-          tl = movmatrix_trans(*reinterpret_cast<const uint32_t*>(&lp));
-        }
-      };
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int cb = 16 * w + 8 * h;                       // first channel of the warp's 8-channel block
-        if (cb >= P.out_c) continue;                         // warp-uniform
-        const int c_own = P.n_off + cb + r, c_st = P.n_off + cb + 2 * t4;
-        if (P.pool) {
-          // pooled row py of the tile, pooled column 4k + t4 from n-groups j = 4py + k and j + 2
-          const int Hp = P.H >> 1, Wp = P.W >> 1;
-#pragma unroll
-          for (int py = 0; py < UM_TH / 2; ++py) {
-            float m[2];
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const int j = 4 * py + k;
-              m[k] = fmaxf(fmaxf(value(4 * j + 2 * h, h), value(4 * (j + 2) + 2 * h, h)),
-                           fmaxf(value(4 * j + 2 * h + 1, h), value(4 * (j + 2) + 2 * h + 1, h)));
+      tr_epilogue<FP16>(acc, cross, bias, P.n_off, 0, tile, tiles_x, tiles_y, P, w, r, t4);
+    }
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------
+// 128-channel layers (and 256 / 512 as 2 / 4 work items of 128 channels): streamed weights, D[64 oc][128 px] = W * X^T
+// --------------------------------------------------------------------------------------------------------------
+// The MMAs of conv_res64_kernel on conv_umma_kernel's pipeline.  Both consumer warpgroups work on the same item: warpgroup
+// g owns output channels [64g, 64g + 64) of it across all 128 pixels of the tile, reads every A box (the empty barrier
+// counts both readers) and only its own 64 weight rows, which producer warp 1 + g streams through the warpgroup's own
+// ring of half slots (StreamTCfg), so that every weight row still crosses L2 once per item and a warpgroup that runs
+// ahead never waits on the other's weights.  Producer warp 0 loads the A boxes.  Per K step (kx, then slab, then ky,
+// then the four k16 steps, as conv_umma_kernel) three wgmma m64n128k16: W_hi*X_hi -> main, W_lo*X_hi -> cross,
+// W_hi*X_lo -> cross.
+// Skew: warpgroup 1 starts once warpgroup 0 has issued the MMAs of its first box.  From then on the two run a box apart,
+// so that each one's epilogue overlaps the other's MMAs instead of leaving the tensor pipe idle.
+// FP16: one wgmma W_hi*X_hi per K step on hi-only boxes and W_hi-only half slots; tm_a_lo / tm_w_lo are not used.
+template <bool SPLIT, bool FP16 = false>
+__global__ void __launch_bounds__(UM_THREADS, 1)
+conv_stream_t_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+                     const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
+  using Cfg = StreamTCfg<FP16>;
+  constexpr int AS = Cfg::A_SLOTS, WS = Cfg::W_SLOTS, A_STRIDE = Cfg::PLANES * UM_A_SLOT;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t w_base = smem_base + Cfg::A_RING;                       // warpgroup g's half slots at + g * WS * W_SLOT
+  const uint32_t bar_base = w_base + 2 * WS * Cfg::W_SLOT;               // 8-byte barriers
+  auto a_full = [&](int s) { return bar_base + 8u * s; };
+  auto a_empty = [&](int s) { return bar_base + 8u * (AS + s); };
+  auto w_full = [&](int g, int s) { return bar_base + 8u * (2 * AS + g * WS + s); };
+  auto w_empty = [&](int g, int s) { return bar_base + 8u * (2 * AS + 2 * WS + g * WS + s); };
+
+  const int lane = threadIdx.x & 31;
+  const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
+  // work item = (tile, 128-channel block): items of one tile are adjacent, so concurrent CTAs share its activations in L2
+  const int n_split = SPLIT ? P.n_split : 1;          // compile-time 1 for ordinary layers: no div / mod per item
+  const int n_items = P.B * tiles_x * tiles_y * n_split;
+  const int halo = P.ks / 2;
+  const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_ROW;   // bytes of one A plane box
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AS; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 2); }
+    for (int s = 0; s < 2 * WS; ++s) { mbar_init(w_full(0, s), 1); mbar_init(w_empty(0, s), 1); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (threadIdx.x >= UM_CONSUMERS) {
+    const int pw = (threadIdx.x - UM_CONSUMERS) >> 5;      // producer warp: 0 A boxes, 1 + g weight rows of warpgroup g
+    setmaxnreg_dec<UM_PRODUCER_REGS>();
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (pw < 3 && elect_one()) {
+      const int g = pw - 1;
+      int s = 0; uint32_t ph = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
+        const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
+        for (int kx = 0; kx < P.ks; ++kx) {
+          for (int cs = 0; cs < P.cin_slabs; ++cs) {
+            if (pw == 0) {
+              mbar_wait(a_empty(s), ph ^ 1);
+              const uint32_t sa = smem_base + s * A_STRIDE;
+              const int xa = tx * UM_TW + kx - halo, ya = ty * UM_TH - halo;
+              mbar_expect_tx(a_full(s), Cfg::PLANES * a_box_bytes);
+              tma_load_4d(sa, &tm_a_hi, a_full(s), cs * UM_KC, xa, ya, b);
+              if constexpr (!FP16) tma_load_4d(sa + UM_A_SLOT, &tm_a_lo, a_full(s), cs * UM_KC, xa, ya, b);
+              if (++s == AS) { s = 0; ph ^= 1; }
+              continue;
             }
-            const int gpy = ty * (UM_TH / 2) + py;
-            if (P.out_f32) {
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                const int gpx = tx * (UM_TW / 2) + 4 * k + t4;
-                if (gpy < Hp && gpx < Wp)
-                  P.out_f32[(((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_own] = m[k];
-              }
-            } else {
-              // column 2 t4 + k of the block is pooled pixel 4k + t4: after the transpose lane l holds pixel
-              // 4 ((l / 4) & 1) + (l / 4) / 2
-              uint32_t th, tl;
-              split_t(m[0], m[1], th, tl);
-              const int gpx = tx * (UM_TW / 2) + 4 * (r & 1) + (r >> 1);
-              if (gpy < Hp && gpx < Wp) {
-                const size_t o = (((size_t)b * Hp + gpy) * Wp + gpx) * P.out_cstride + c_st;
-                *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
-                if constexpr (!FP16) *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
-              }
-            }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int gy = y0 + (j >> 1), xb = x0 + 8 * (j & 1);
-            const float v0 = value(4 * j + 2 * h, h), v1 = value(4 * j + 2 * h + 1, h);
-            if (P.out_f32) {
-              const int gx = xb + 2 * t4;
-              const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_own;
-              if (gy < P.H && gx < P.W) P.out_f32[o] = v0;
-              if (gy < P.H && gx + 1 < P.W) P.out_f32[o + P.out_cstride] = v1;
-            } else {
-              uint32_t th, tl;
-              split_t(v0, v1, th, tl);
-              const int gx = xb + r;
-              if (gy < P.H && gx < P.W) {
-                const size_t o = (((size_t)b * P.H + gy) * P.W + gx) * P.out_cstride + c_st;
-                *reinterpret_cast<uint32_t*>(P.out_hi + o) = th;
-                if constexpr (!FP16) *reinterpret_cast<uint32_t*>(P.out_lo + o) = tl;
-              }
+            for (int ky = 0; ky < P.ks; ++ky) {
+              mbar_wait(w_empty(g, s), ph ^ 1);
+              const uint32_t sw = w_base + (g * WS + s) * Cfg::W_SLOT;
+              mbar_expect_tx(w_full(g, s), Cfg::W_SLOT);
+              tma_load_3d(sw, &tm_w_hi, w_full(g, s), cs * UM_KC, n_off + 64 * g, ky * P.ks + kx);
+              if constexpr (!FP16)
+                tma_load_3d(sw + Cfg::W_PLANE, &tm_w_lo, w_full(g, s), cs * UM_KC, n_off + 64 * g, ky * P.ks + kx);
+              if (++s == WS) { s = 0; ph ^= 1; }
             }
           }
         }
       }
+    }
+  } else {
+    setmaxnreg_inc<UM_CONSUMER_REGS>();
+    const int g = threadIdx.x >> 7;                          // warpgroup: output channels [64g, 64g + 64) of every item
+    const int w = (threadIdx.x >> 5) & 3;                    // warp: output channels 64g + 16w .. + 15
+    const int r = lane >> 2, t4 = lane & 3;
+    const bool signaller = (threadIdx.x & 127) == 0;
+    const uint32_t w_ring = w_base + g * WS * Cfg::W_SLOT;
+    bool skew_set = g == 1;                                  // warpgroup 0 releases warpgroup 1 once
+    if (g == 1) named_bar_sync(1, 256);
+    // buffers are released once the MMAs that read them have retired (conv_umma_kernel's commit-group rule): one arrival
+    // per warpgroup on the box's empty barrier, the reader's on its half slot's
+    auto release = [&](int a_slot, int w_slot) {
+      if (!signaller) return;
+      if (a_slot >= 0) mbar_arrive(a_empty(a_slot));
+      if (w_slot >= 0) mbar_arrive(w_empty(g, w_slot));
+    };
+    int as = 0; uint32_t aph = 0;
+    int ws = 0; uint32_t wph = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
+      const int c_abs = n_off + 64 * g;
+      const float bias[2] = {__ldg(P.bias + c_abs + 16 * w + r), __ldg(P.bias + c_abs + 16 * w + 8 + r)};
+      // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo.  fp16: main only
+      float acc[64], cross[FP16 ? 1 : 64];
+#pragma unroll
+      for (int k = 0; k < 64; ++k) { acc[k] = 0.f; if constexpr (!FP16) cross[k] = 0.f; }
+      uint32_t scale_d = 0;
+      int pend_a = -1, pend_w = -1;                          // buffers of the last committed group
+      for (int kx = 0; kx < P.ks; ++kx) {
+        for (int cs = 0; cs < P.cin_slabs; ++cs) {
+          mbar_wait(a_full(as), aph);
+          const uint32_t sa = smem_base + as * A_STRIDE;
+          for (int ky = 0; ky < P.ks; ++ky) {
+            mbar_wait(w_full(g, ws), wph);
+            const uint32_t sw = w_ring + ws * Cfg::W_SLOT;
+            const int w_slot = ws;
+            if (++ws == WS) { ws = 0; wph ^= 1; }
+            const uint64_t w_hi = wgmma_desc_sw128(sw, 1024), w_lo = wgmma_desc_sw128(sw + Cfg::W_PLANE, 1024);
+            const uint64_t x_hi = wgmma_desc_sw128(sa + ky * UM_ROW, 1024);
+            const uint64_t x_lo = wgmma_desc_sw128(sa + UM_A_SLOT + ky * UM_ROW, 1024);
+#pragma unroll
+            for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < UM_KC / 16; ++k) {
+              const uint64_t adv = (uint64_t)(k * 32 >> 4);
+              Wgmma<128>::mma(acc, w_hi + adv, x_hi + adv, scale_d);       // hi*hi -> main
+              if constexpr (!FP16) {
+                Wgmma<128>::mma(cross, w_lo + adv, x_hi + adv, scale_d);   // lo*hi -> cross
+                Wgmma<128>::mma(cross, w_hi + adv, x_lo + adv, 1u);        // hi*lo -> cross
+              }
+              scale_d = 1;
+            }
+            wgmma_commit();
+#pragma unroll
+            for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
+            wgmma_wait<1>();
+            release(pend_a, pend_w);
+            pend_a = (ky == P.ks - 1) ? as : -1;
+            pend_w = w_slot;
+          }
+          if (++as == AS) { as = 0; aph ^= 1; }
+          if (!skew_set) { named_bar_arrive(1, 256); skew_set = true; }
+        }
+      }
+      wgmma_wait<0>();
+      release(pend_a, pend_w);
+#pragma unroll
+      for (int k = 0; k < 64; ++k) { fence_operand(acc[k]); if constexpr (!FP16) fence_operand(cross[k]); }
+      tr_epilogue<FP16>(acc, cross, bias, c_abs, c_abs - P.n_off, tile, tiles_x, tiles_y, P, w, r, t4);
     }
   }
 }
@@ -783,14 +977,11 @@ osb_status umma_layer_upload(Resources& res, UmmaLayer* L, const float* w_oihw, 
   OSB_TRY(res.upload(&L->bias, bp.data(), L->n_pad));
   const uint64_t dims[3] = {(uint64_t)cin, (uint64_t)L->n_pad, (uint64_t)L->taps};
   const uint64_t strides[2] = {(uint64_t)cin * 2, (uint64_t)cin * L->n_pad * 2};
-  const uint32_t box[3] = {UM_KC, (uint32_t)std::min(L->n_pad, 256), 1};
+  // one box = the 80 rows of the detector head, else 64 rows: a whole slab of the N = 64 kernels, one warpgroup's half
+  // of a 128-channel work item in conv_stream_t_kernel
+  const uint32_t box[3] = {UM_KC, (uint32_t)(L->n_pad == 80 ? 80 : 64), 1};
   OSB_TRY(umma_make_tmap(&L->tm_hi, L->w_hi, 3, dims, strides, box));
   OSB_TRY(umma_make_tmap(&L->tm_lo, L->w_lo, 3, dims, strides, box));
-  if (L->n_pad >= 256) {                       // 128-row boxes: the layer as n_pad / 128 work items per tile
-    const uint32_t box128[3] = {UM_KC, 128, 1};
-    OSB_TRY(umma_make_tmap(&L->tm_hi128, L->w_hi, 3, dims, strides, box128));
-    OSB_TRY(umma_make_tmap(&L->tm_lo128, L->w_lo, 3, dims, strides, box128));
-  }
   return OSB_OK;
 }
 
@@ -829,11 +1020,18 @@ static osb_status launch_persistent(int smem_bytes, const CUtensorMap& a_hi, con
   return OSB_OK;
 }
 
-template <int N, bool SPLIT = false, bool FP16 = false>
+template <int N, bool FP16 = false>
 static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
-                              cudaStream_t st, int max_ctas, bool box128 = false) {
-  return launch_persistent<conv_umma_kernel<N, SPLIT, FP16>>(UmmaCfg<N, FP16>::SMEM_BYTES, a_hi, a_lo,
-                           box128 ? L.tm_hi128 : L.tm_hi, box128 ? L.tm_lo128 : L.tm_lo, P, st, max_ctas);
+                              cudaStream_t st, int max_ctas) {
+  return launch_persistent<conv_umma_kernel<N, FP16>>(UmmaCfg<N, FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st,
+                                                      max_ctas);
+}
+
+template <bool SPLIT, bool FP16>
+static osb_status launch_stream_t(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
+                                  cudaStream_t st, int max_ctas) {
+  return launch_persistent<conv_stream_t_kernel<SPLIT, FP16>>(StreamTCfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo,
+                                                              P, st, max_ctas);
 }
 
 static bool precision_fp16(int precision) { return precision == OSB_PRECISION_FP16; }
@@ -854,13 +1052,13 @@ static osb_status umma_conv_launch(const UmmaLayer& L, const CUtensorMap& a_hi, 
       if (L.ks == 3 && L.cin == UM_KC)            // weights resident, transposed GEMM
         return launch_persistent<conv_res64_kernel<FP16>>(R64Cfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st,
                                                           max_ctas);
-      return launch_umma<64, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
-    case 80: return launch_umma<80, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
-    case 128: return launch_umma<128, false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+      return launch_umma<64, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+    case 80: return launch_umma<80, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+    case 128: return launch_stream_t<false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
     case 256:                                     // 2 / 4 items of 128 channels per tile (a 256-wide accumulator pair
     case 512:                                     // would not fit a warpgroup's registers)
       P.n_split = L.n_pad / 128;
-      return launch_umma<128, true, FP16>(a_hi, a_lo, L, P, st, max_ctas, true);
+      return launch_stream_t<true, FP16>(a_hi, a_lo, L, P, st, max_ctas);
   }
   set_error("umma_conv_forward", "unsupported N");
   return OSB_ERR_INVALID;
@@ -885,7 +1083,7 @@ osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi
   OSB_REQUIRE(L.n_pad == 80 && L.cout == 65 && L.ks == 1, "fused detector head expects the 65-logit 1x1 layer");
   UmmaArgs P = umma_args(L, B, H, W, act_scale);
   P.out_f32 = semi; P.out_c = 80; P.out_cstride = 80; P.out_scale = 1.f; P.epi = 1;
-  return precision_fp16(precision) ? launch_umma<80, false, true>(a_hi, a_lo, L, P, st, max_ctas)
+  return precision_fp16(precision) ? launch_umma<80, true>(a_hi, a_lo, L, P, st, max_ctas)
                                    : launch_umma<80>(a_hi, a_lo, L, P, st, max_ctas);
 }
 

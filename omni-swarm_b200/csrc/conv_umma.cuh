@@ -17,8 +17,7 @@ struct UmmaLayer {
   float w_scale = 1.f;
   __half *w_hi = nullptr, *w_lo = nullptr;
   float* bias = nullptr;
-  CUtensorMap tm_hi, tm_lo;
-  CUtensorMap tm_hi128, tm_lo128;     // same planes with 128-row boxes (n_pad >= 256 only)
+  CUtensorMap tm_hi, tm_lo;           // boxes of 64 rows (80 for the 80-row detector head)
 };
 
 // the weight planes and bias belong to `res`

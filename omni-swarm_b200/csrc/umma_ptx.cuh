@@ -52,6 +52,14 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// named barrier `id` (1 .. 15; 0 is __syncthreads) over `count` threads, whole warps: bar_arrive does not wait
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // K-major SWIZZLE_128B shared-memory matrix descriptor of wgmma: start >> 4 | LBO (unused for this layout) = 1 << 16 |
 // SBO (byte distance between consecutive 8-row core-matrix groups) >> 4 << 32 | layout SWIZZLE_128B (1) << 62.
 // The start must sit on a 1024-byte swizzle atom; moving it by 32 bytes selects the next K = 16 slice of a 128-byte row.
