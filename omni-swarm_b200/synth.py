@@ -624,3 +624,70 @@ def loop_scene(yaw: float = 0.15, t_new=(0.25, -0.125, 0.0625), depths=(2.0, 4.0
     delta = pose_new.copy()                                                   # the old drone is the origin
     return dict(K=K, ext=np.array(ext), pose_old=pose_old, pose_new=pose_new, delta_true=delta, kp_old=kp_old, kp_new=kp_new,
                 X=X)
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# Inputs of the keyframe front-end: its networks, and keyframe records of loop_scene() built on the host
+# ----------------------------------------------------------------------------------------------------------------
+def frontend_weights(seed: int = 0):
+    """(sp_weights_flat, pca_comp, pca_mean, nv_weights_flat): the first four arguments of host.KeyframeFrontend"""
+    comp, mean = pca_matrices(seed)
+    return flatten_sp_weights(superpoint_weights(seed)), comp, mean, flatten_nv_weights(netvlad_weights(seed))
+
+
+LOOP_SCENE = loop_scene()
+LOOP_NPT = len(LOOP_SCENE["X"][0])                                  # landmarks per direction
+LOOP_G_OLD = descriptor_db(4, 4096, 5)                              # the old keyframe's global descriptor per direction
+LOOP_DESC = [local_descriptors(LOOP_NPT, 40 + d) for d in range(4)]  # the old keyframe's local descriptors per direction
+
+
+def loop_noisy_g(seed: int, sigma: float = 0.05) -> np.ndarray:
+    """LOOP_G_OLD with Gaussian noise of norm ~sigma per direction, renormalised"""
+    rng = np.random.default_rng(seed)
+    g = LOOP_G_OLD + rng.normal(0, sigma / 64, LOOP_G_OLD.shape).astype(np.float32)
+    return g / np.linalg.norm(g, axis=1, keepdims=True)
+
+
+def loop_record(drone: int, msg: int, side: str, seed: int = 0, g: np.ndarray | None = None, n_outliers: int = 4,
+                unflag_every: int = 11, few_flags_dir: int | None = None, scramble: bool = False, g_noise: float = 0.0):
+    """A four-direction keyframe record (lib.KeyframeRecord) of LOOP_SCENE.  side 'old': the old camera's pixels; 'new':
+    the new camera's, points permuted, descriptors noisy, every `unflag_every`-th landmark unflagged and `n_outliers`
+    points per direction moved to random pixels / 3-D (their descriptors still match the old point: outlier matches).
+    few_flags_dir: only two landmarks of that direction flagged (a failed homography pair); scramble: random 3-D points.
+    Global descriptors: g [4][4096] (LOOP_G_OLD if None); with g_noise, a 'new' record adds Gaussian noise of that
+    sigma per element, and either side is renormalised."""
+    from . import lib
+    rng = np.random.default_rng(seed)
+    sc, n = LOOP_SCENE, LOOP_NPT
+    r = lib.KeyframeRecord()
+    r.drone_id, r.msg_id, r.n_dirs = drone, msg, 4
+    for d in range(4):
+        perm = np.arange(n) if side == "old" else rng.permutation(n)
+        kp = (sc["kp_old"][d] if side == "old" else sc["kp_new"][d])[perm].copy()
+        X = sc["X"][d][perm].copy()
+        desc = LOOP_DESC[d][perm] + (0 if side == "old" else rng.normal(0, 0.02, (n, 64)).astype(np.float32))
+        desc /= np.linalg.norm(desc, axis=1, keepdims=True)
+        flag = np.ones(n, np.int32)
+        if side == "new":
+            flag[::unflag_every] = 0
+            out = rng.choice(n, n_outliers, replace=False)
+            kp[out] = rng.uniform(0, 96, (n_outliers, 2))
+            X[out] = rng.normal(0, 3, (n_outliers, 3))
+        if few_flags_dir == d:
+            flag[:] = 0
+            flag[[3, 17]] = 1
+        if scramble:
+            X = rng.normal(0, 3, X.shape).astype(np.float32)
+        gd = LOOP_G_OLD[d] if g is None else g[d]
+        if g_noise:
+            if side == "new":
+                gd = gd + rng.normal(0, g_noise, 4096).astype(np.float32)
+            gd = gd / np.linalg.norm(gd)
+        r.n_kpts[d] = n
+        np.ctypeslib.as_array(r.global_desc[d])[:] = gd
+        np.ctypeslib.as_array(r.local_desc[d])[:n] = desc
+        np.ctypeslib.as_array(r.kpts[d])[:n] = kp
+        np.ctypeslib.as_array(r.landmarks_3d[d])[:n] = X
+        np.ctypeslib.as_array(r.landmarks_flag[d])[:n] = flag
+        np.ctypeslib.as_array(r.stereo_match[d])[:n] = np.where(flag > 0, 0, -1)
+    return r

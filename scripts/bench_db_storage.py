@@ -22,14 +22,13 @@ The card's name, power limit and SM clock (sampled by nvidia-smi during the time
 import argparse
 import json
 import os
-import subprocess
 import sys
-import threading
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import ClockSampler, smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 DIM, K, QDIR, N_DIRS = 4096, 6, 1, 4
@@ -37,36 +36,6 @@ HBM_TBS = 3.35
 FE_ROWS = 50_016
 RB, RS = lib.RECORD_BYTES, lib.RESULT_BYTES
 STORAGES = ("fp32", "fp16")
-
-
-def smi(query):
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    return r.stdout.strip().splitlines()[0]
-
-
-class ClockSampler:
-    """SM clock (MHz) sampled by nvidia-smi every 0.2 s while active"""
-
-    def __init__(self):
-        self.samples, self._stop = [], threading.Event()
-
-    def __enter__(self):
-        self._stop.clear()
-        self._t = threading.Thread(target=self._run, daemon=True)
-        self._t.start()
-        return self
-
-    def _run(self):
-        while not self._stop.wait(0.2):
-            try:
-                self.samples.append(float(smi("clocks.sm").split()[0]))
-            except Exception:
-                pass
-
-    def __exit__(self, *exc):
-        self._stop.set()
-        self._t.join()
 
 
 def unit_rows(n, seed):
@@ -157,13 +126,11 @@ def record(drone, g_row, seed):
 
 
 def frontend_cases(reps, warmup, stream):
-    comp, mean = synth.pca_matrices(0)
     g = synth.descriptor_db(FE_ROWS, DIM, 11)
     fes = {}
     for s in STORAGES:
-        fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                   synth.flatten_nv_weights(synth.netvlad_weights(0)), width=640, height=480,
-                                   n_dirs=N_DIRS, max_num=200, self_id=1, db_capacity=FE_ROWS, match_index_dist=5)
+        fe = host.KeyframeFrontend(*synth.frontend_weights(), width=640, height=480, n_dirs=N_DIRS, max_num=200, self_id=1,
+                                   db_capacity=FE_ROWS, match_index_dist=5)
         fe.set_db_storage(s)
         fe.db_load(g)
         fe.db_load(g, remote=True)

@@ -15,7 +15,6 @@ every round's value beside them.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -23,6 +22,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import gpu_name_and_power  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 W, H, N_DIRS, MAX_NUM = 640, 480, 1, 200
@@ -34,21 +34,10 @@ EXTRINSIC = np.array([[0.08, 0.0, 0.03, 0.5, -0.5, 0.5, -0.5]])   # camera z = b
 POSE_DRONE = np.array([1.0, -2.0, 0.5, 1.0, 0.0, 0.0, 0.0])
 
 
-def gpu_name_and_power():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return None
-
-
 def make_frontend(capacity, depth):
-    comp, mean = synth.pca_matrices(0)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W, height=H, n_dirs=N_DIRS,
-                               max_num=MAX_NUM, sp_thres=0.015, self_id=0, db_capacity=capacity, inner_product_thres=0.3,
-                               match_index_dist=5, zero_bottom_quarter=False, accept_min_3d_pts=10)
+    fe = host.KeyframeFrontend(*synth.frontend_weights(), width=W, height=H, n_dirs=N_DIRS, max_num=MAX_NUM, sp_thres=0.015,
+                               self_id=0, db_capacity=capacity, inner_product_thres=0.3, match_index_dist=5,
+                               zero_bottom_quarter=False, accept_min_3d_pts=10)
     if depth:
         fe.set_depth_camera(K, EXTRINSIC, 0.3, 10.0)
         fe.set_drone_pose(POSE_DRONE)

@@ -17,7 +17,6 @@ The card's name and power limit are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -25,71 +24,16 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
+from oracle.pcm_ref import pose_inv, pose_mul, q_mul, q_rot  # noqa: E402
 
 ND, MN, QDIR = 4, 200, 1
 RB, RS, EB = lib.RECORD_BYTES, lib.RESULT_BYTES, lib.EDGE_BYTES
-SC = synth.loop_scene()
-NPT = len(SC["X"][0])
-G = synth.descriptor_db(ND, 4096, 5)
-DESC = [synth.local_descriptors(NPT, 40 + d) for d in range(ND)]
-
-
-def smi(query):
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    return r.stdout.strip().splitlines()[0]
-
-
-def record(drone, msg, side, seed):
-    rng = np.random.default_rng(seed)
-    r = lib.KeyframeRecord()
-    r.drone_id, r.msg_id, r.n_dirs = drone, msg, ND
-    for d in range(ND):
-        perm = np.arange(NPT) if side == "old" else rng.permutation(NPT)
-        kp = (SC["kp_old"][d] if side == "old" else SC["kp_new"][d])[perm].copy()
-        X = SC["X"][d][perm].copy()
-        desc = DESC[d][perm] + (0 if side == "old" else rng.normal(0, 0.02, (NPT, 64)).astype(np.float32))
-        desc /= np.linalg.norm(desc, axis=1, keepdims=True)
-        flag = np.ones(NPT, np.int32)
-        if side == "new":
-            flag[::11] = 0
-            out = rng.choice(NPT, 4, replace=False)
-            kp[out] = rng.uniform(0, 96, (4, 2))
-            X[out] = rng.normal(0, 3, (4, 3))
-        g = G[d] + (0 if side == "old" else rng.normal(0, 1e-3, 4096).astype(np.float32))
-        r.n_kpts[d] = NPT
-        np.ctypeslib.as_array(r.global_desc[d])[:] = g / np.linalg.norm(g)
-        np.ctypeslib.as_array(r.local_desc[d])[:NPT] = desc
-        np.ctypeslib.as_array(r.kpts[d])[:NPT] = kp
-        np.ctypeslib.as_array(r.landmarks_3d[d])[:NPT] = X
-        np.ctypeslib.as_array(r.landmarks_flag[d])[:NPT] = flag
-        np.ctypeslib.as_array(r.stereo_match[d])[:NPT] = np.where(flag > 0, 0, -1)
-    return r
+SC = synth.LOOP_SCENE
 
 
 # ---- the host path: numpy assembly of compute_correspond_features + the PnP prior ------------------------------------
-def q_mul(a, b):
-    aw, ax, ay, az = a; bw, bx, by, bz = b
-    return np.array([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
-                     aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw])
-
-
-def q_rot(q, v):
-    u = np.broadcast_to(q[1:], v.shape)
-    c = np.cross(u, v)
-    return v + 2.0 * (q[0] * c + np.cross(u, c))
-
-
-def pose_mul(a, b):
-    return np.concatenate([a[:3] + q_rot(a[3:], b[:3]), q_mul(a[3:], b[3:])])
-
-
-def pose_inv(a):
-    qc = a[3:] * np.array([1.0, -1.0, -1.0, -1.0])
-    return np.concatenate([-q_rot(qc, a[:3]), qc])
-
-
 def host_assemble(res, rec, old, K, ext, pose_new, pose_old):
     Xs, uvs = [], []
     main_old = res.hit_dir
@@ -124,17 +68,15 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--host-reps", type=int, default=10)
     a = ap.parse_args()
-    comp, mean = synth.pca_matrices(0)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), width=96, height=64, n_dirs=ND,
-                               max_num=MN, self_id=1, db_capacity=64, match_index_dist=5, geometric_filter=True)
+    fe = host.KeyframeFrontend(*synth.frontend_weights(), width=96, height=64, n_dirs=ND, max_num=MN, self_id=1, db_capacity=64,
+                               match_index_dist=5, geometric_filter=True)
     fe.set_cameras(SC["K"], SC["ext"], SC["ext"], 0.006)
     fe.set_loop_params(odometry_consistency_threshold=10.0)
     st = torch.cuda.current_stream().cuda_stream
-    old = record(1, 100, "old", 0)
+    old = synth.loop_record(1, 100, "old", 0, g_noise=1e-3)
     ot = torch.frombuffer(bytearray(bytes(old)), dtype=torch.uint8).cuda()
     fe.ingest_own(ot.data_ptr(), st)
-    recs = [record(2 + r % 3, 200 + r, "new", 10 + r) for r in range(64)]
+    recs = [synth.loop_record(2 + r % 3, 200 + r, "new", 10 + r, g_noise=1e-3) for r in range(64)]
     rt = torch.frombuffer(bytearray(b"".join(bytes(r) for r in recs)), dtype=torch.uint8).cuda()
     res_t = torch.zeros(64 * RS, dtype=torch.uint8, device="cuda")
     fe.query_received(rt.data_ptr(), 64, -1, res_t.data_ptr(), st)

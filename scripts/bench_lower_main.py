@@ -13,28 +13,19 @@ reported with every round's value beside them, and the SM clock sampled after th
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import gpu_name_and_power, smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 W, H, N_DIRS, MAX_NUM = 640, 480, 4, 200
 DB_ROWS = 10_000
 POOL = 8                  # distinct keyframes cycled through
 K = np.array([320.0, 320.0, 320.0, 240.0])
-
-
-def nvidia_smi(query):
-    try:
-        r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                           timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return None
 
 
 def rig():
@@ -48,11 +39,9 @@ def rig():
 
 
 def make_frontend():
-    comp, mean = synth.pca_matrices(0)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W, height=H, n_dirs=N_DIRS,
-                               max_num=MAX_NUM, sp_thres=0.015, self_id=0, db_capacity=DB_ROWS + 4096,
-                               inner_product_thres=0.3, match_index_dist=5, zero_bottom_quarter=True, accept_min_3d_pts=10)
+    fe = host.KeyframeFrontend(*synth.frontend_weights(), width=W, height=H, n_dirs=N_DIRS, max_num=MAX_NUM, sp_thres=0.015,
+                               self_id=0, db_capacity=DB_ROWS + 4096, inner_product_thres=0.3, match_index_dist=5,
+                               zero_bottom_quarter=True, accept_min_3d_pts=10)
     left, right = rig()
     fe.set_cameras(K, left, right, 0.006)
     fe.set_drone_pose(np.array([1.0, -2.0, 0.5, 1.0, 0.0, 0.0, 0.0]))
@@ -104,9 +93,9 @@ def main():
                 g = synth.descriptor_db(2000, 4096, 50 + s)
                 ld = np.random.default_rng(s).standard_normal((2000, MAX_NUM, 64)).astype(np.float32)
                 fe.db_load(g, ld, np.full(2000, MAX_NUM, np.int32), remote=False)
-    clock = nvidia_smi("clocks.sm")
+    clock = smi("clocks.sm")
     fe.close()
-    out = {"bench": "lower_main", "gpu": nvidia_smi("name,power.limit"), "sm_clock": clock, "steps": args.steps,
+    out = {"bench": "lower_main", "gpu": gpu_name_and_power(), "sm_clock": clock, "steps": args.steps,
            "rounds": args.rounds, "db_rows": DB_ROWS, "images": f"{N_DIRS}x2 {W}x{H}"}
     for mode in ("up", "down"):
         out[f"kf_per_s_{mode}"] = float(np.median(kfs[mode]))

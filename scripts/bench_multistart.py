@@ -12,7 +12,6 @@ against ground truth; on the init graph at K = 3 also K x the oracle's solve_fas
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -21,18 +20,10 @@ for _v in ("OMP_NUM_THREADS", "OPENBLAS_NUM_THREADS", "MKL_NUM_THREADS"):
     os.environ.setdefault(_v, "1")                   # the CPU stand-in runs on one thread, as the reference's solver
 import numpy as np  # noqa: E402
 
+from gpu_env import gpu_name_and_power  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 from oracle import multistart_ref as mr  # noqa: E402
 from oracle import solver_ref as sr  # noqa: E402
-
-
-def gpu_name_and_power():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return None
 
 
 def main():

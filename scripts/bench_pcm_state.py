@@ -18,7 +18,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,17 +25,12 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 THRES, POS, ANG = 15.0, 1e-4, 1e-5
 NEW_PER_ROUND = 4
 SIZES = (250, 1000, 2000, 4000)
-
-
-def smi(query):
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    return r.stdout.strip().splitlines()[0]
 
 
 def main():

@@ -16,14 +16,13 @@ and the card's name, power limit and SM clock, sampled by nvidia-smi while the k
 import argparse
 import json
 import os
-import subprocess
 import sys
-import threading
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import ClockSampler, smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 W, H, N_DIRS, MAX_NUM, SP_BATCH, NV_BATCH = 640, 480, 4, 200, 8, 4
@@ -36,36 +35,6 @@ SP_CONVS = {"conv1b+pool": (64, 64, 9, 1), "conv2a": (64, 64, 9, 2), "conv2b+poo
             "conv3a": (64, 128, 9, 4), "conv3b+pool": (128, 128, 9, 4), "conv4a": (128, 128, 9, 8),
             "conv4b": (128, 128, 9, 8), "convPa": (128, 256, 9, 8), "convPb": (256, 80, 1, 8), "convDa": (128, 256, 9, 8),
             "convDb": (256, 256, 1, 8)}
-
-
-def smi(query):
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    return r.stdout.strip().splitlines()[0]
-
-
-class ClockSampler:
-    """SM clock (MHz) sampled by nvidia-smi every 0.2 s while active"""
-
-    def __init__(self):
-        self.samples, self._stop = [], threading.Event()
-
-    def __enter__(self):
-        self._stop.clear()
-        self._t = threading.Thread(target=self._run, daemon=True)
-        self._t.start()
-        return self
-
-    def _run(self):
-        while not self._stop.wait(0.2):
-            try:
-                self.samples.append(float(smi("clocks.sm").split()[0]))
-            except (OSError, subprocess.SubprocessError, ValueError, IndexError):
-                pass
-
-    def __exit__(self, *exc):
-        self._stop.set()
-        self._t.join()
 
 
 def mma_tflops(layer, ms, mode):
@@ -84,8 +53,7 @@ def main():
     assert lib.load().osb_device_count() > 0, "needs a CUDA device"
     name, power = smi("name"), smi("power.limit")
     st = torch.cuda.current_stream().cuda_stream
-    comp, mean = synth.pca_matrices(0)
-    spw, nvw = synth.flatten_sp_weights(synth.superpoint_weights(0)), synth.flatten_nv_weights(synth.netvlad_weights(0))
+    spw, comp, mean, nvw = synth.frontend_weights()
 
     sp = host.SuperPoint(spw, comp, mean, W, H, 0.015, MAX_NUM, max_batch=SP_BATCH)
     nv = host.NetVLAD(nvw, W, H, max_batch=NV_BATCH)

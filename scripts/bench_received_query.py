@@ -18,50 +18,19 @@ store's bytes over the scan time, as a fraction of the H100 SXM's 3.35 TB/s.  Th
 import argparse
 import json
 import os
-import subprocess
 import sys
-import threading
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from gpu_env import ClockSampler, smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 W, H, N_DIRS, MAX_NUM, QDIR = 640, 480, 4, 200, 1
 N_OWN = 4
 HBM_TBS = 3.35
 RB, RS = lib.RECORD_BYTES, lib.RESULT_BYTES
-
-
-def smi(query):
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    return r.stdout.strip().splitlines()[0]
-
-
-class ClockSampler:
-    """SM clock (MHz) sampled by nvidia-smi every 0.2 s while active"""
-
-    def __init__(self):
-        self.samples, self._stop = [], threading.Event()
-
-    def __enter__(self):
-        self._stop.clear()
-        self._t = threading.Thread(target=self._run, daemon=True)
-        self._t.start()
-        return self
-
-    def _run(self):
-        while not self._stop.wait(0.2):
-            try:
-                self.samples.append(float(smi("clocks.sm").split()[0]))
-            except Exception:
-                pass
-
-    def __exit__(self, *exc):
-        self._stop.set()
-        self._t.join()
 
 
 def images(seed, noisy=False):
@@ -76,11 +45,9 @@ def images(seed, noisy=False):
 
 
 def make_frontend(rows, geometric_filter):
-    comp, mean = synth.pca_matrices(0)
-    return host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                 synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W, height=H, n_dirs=N_DIRS,
-                                 max_num=MAX_NUM, self_id=1, db_capacity=rows + 64, match_index_dist=5,
-                                 geometric_filter=bool(geometric_filter), ransac_seed=1)
+    return host.KeyframeFrontend(*synth.frontend_weights(), width=W, height=H, n_dirs=N_DIRS, max_num=MAX_NUM, self_id=1,
+                                 db_capacity=rows + 64, match_index_dist=5, geometric_filter=bool(geometric_filter),
+                                 ransac_seed=1)
 
 
 def build_store(fe, rows, g, stream):

@@ -13,6 +13,8 @@ import pytest
 from omniswarm_b200 import host, lib, synth
 from oracle import db_storage_ref as dsr
 from oracle import frontend_ref as fr
+from frontend_harness import EB, RS, filled, upload
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
@@ -182,22 +184,14 @@ def test_add_paths_capacity_and_reset(gpu):
 # ---------------------------------------------------------------------------------------------------------------------
 # front-end
 # ---------------------------------------------------------------------------------------------------------------------
-W0, H0, ND, MN = 96, 64, 4, 200
-RB, RS, EB = lib.RECORD_BYTES, lib.RESULT_BYTES, lib.EDGE_BYTES
+ND, MN = 4, 200
 QDIR = 1
-SC = synth.loop_scene()
-NPT = len(SC["X"][0])
-DESC = [synth.local_descriptors(NPT, 40 + d) for d in range(ND)]
-FILL = 0x5A
+SC, NPT, DESC = synth.LOOP_SCENE, synth.LOOP_NPT, synth.LOOP_DESC
+CONFIG = dict(init_mode_product_thres=0.2, match_index_dist=2, ransac_seed=0)
 
 
 def make_frontend(cap, gf, storage=None):
-    comp, mean = synth.pca_matrices(0)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W0, height=H0, n_dirs=ND,
-                               max_num=MN, sp_thres=0.015, self_id=1, db_capacity=cap, inner_product_thres=0.3,
-                               init_mode_product_thres=0.2, match_index_dist=2, accept_min_3d_pts=3,
-                               geometric_filter=bool(gf), ransac_seed=0)
+    fe = fh.make_frontend(CONFIG, db_capacity=cap, geometric_filter=bool(gf))
     if storage:
         fe.set_db_storage(storage)
     if gf:
@@ -207,27 +201,8 @@ def make_frontend(cap, gf, storage=None):
 
 
 def record(drone, msg, side, g, seed=0):
-    """a keyframe of synth.loop_scene: the old camera's pixels or the new one's (permuted, noisy descriptors, some
-    landmarks unflagged); global descriptor g [ND][4096]"""
-    rng = np.random.default_rng(seed)
-    r = lib.KeyframeRecord()
-    r.drone_id, r.msg_id, r.n_dirs = drone, msg, ND
-    for d in range(ND):
-        perm = np.arange(NPT) if side == "old" else rng.permutation(NPT)
-        kp = (SC["kp_old"][d] if side == "old" else SC["kp_new"][d])[perm]
-        desc = DESC[d][perm] + (0 if side == "old" else rng.normal(0, 0.02, (NPT, 64)).astype(np.float32))
-        desc /= np.linalg.norm(desc, axis=1, keepdims=True)
-        flag = np.ones(NPT, np.int32)
-        if side == "new":
-            flag[::11] = 0
-        r.n_kpts[d] = NPT
-        np.ctypeslib.as_array(r.global_desc[d])[:] = g[d]
-        np.ctypeslib.as_array(r.local_desc[d])[:NPT] = desc
-        np.ctypeslib.as_array(r.kpts[d])[:NPT] = kp
-        np.ctypeslib.as_array(r.landmarks_3d[d])[:NPT] = SC["X"][d][perm]
-        np.ctypeslib.as_array(r.landmarks_flag[d])[:NPT] = flag
-        np.ctypeslib.as_array(r.stereo_match[d])[:NPT] = np.where(flag > 0, 0, -1)
-    return r
+    """a keyframe of synth.loop_scene without outlier matches; global descriptor g [ND][4096]"""
+    return synth.loop_record(drone, msg, side, seed, g, n_outliers=0)
 
 
 def rounded(rec):
@@ -244,9 +219,8 @@ class Pair:
     store"""
 
     def __init__(self, n_loaded, gf, large):
-        import torch
-        self.torch, self.gf = torch, gf
-        self.st = torch.cuda.current_stream().cuda_stream
+        self.gf = gf
+        self.st = fh.stream()
         cap = n_loaded + 64 * ND + 16 * ND
         self.a, self.b = make_frontend(cap, gf), make_frontend(cap, gf, "fp16")
         self.g = synth.descriptor_db(n_loaded, 4096, 11)
@@ -254,7 +228,7 @@ class Pair:
         self.old = record(1, 100, "old", g_old)
         own = [self.old] + [record(1, 101 + i, "old", synth.descriptor_db(ND, 4096, 60 + i)) for i in range(3)]
         for r in own:
-            self.each(lambda fe, rec: fe.ingest_own(self.up([rec]).data_ptr(), self.st), r)
+            self.each(lambda fe, rec: fe.ingest_own(upload([rec]).data_ptr(), self.st), r)
         n_own = len(own) * ND
         for fe, g in ((self.a, dsr.round_rows_fp16(self.g)), (self.b, self.g)):
             if large:
@@ -281,12 +255,9 @@ class Pair:
                 g = synth.descriptor_db(ND, 4096, 300 + r)
             g = g / np.linalg.norm(g, axis=1, keepdims=True)
             self.recs.append(record(2 + r % 3, 300 + r, "new", g.astype(np.float32), seed=20 + r))
-        self.recs_t = self.up(self.recs)
-        self.each(lambda fe, t: fe.ingest(t.data_ptr(), 16, -1, self.st), self.recs[:16], lambda rs: self.up(rs))
+        self.recs_t = upload(self.recs)
+        self.each(lambda fe, t: fe.ingest(t.data_ptr(), 16, -1, self.st), self.recs[:16], upload)
         self.a.finish(self.st); self.b.finish(self.st)
-
-    def up(self, recs):
-        return self.torch.frombuffer(bytearray(b"".join(bytes(r) for r in recs)), dtype=self.torch.uint8).cuda()
 
     def each(self, fn, recs, conv=lambda r: r):
         """fn(fp32 handle, pre-rounded records); fn(fp16 handle, original records)"""
@@ -294,13 +265,10 @@ class Pair:
         fn(self.a, conv(pre))
         fn(self.b, conv(recs))
 
-    def buf(self, nbytes):
-        return self.torch.full((nbytes,), FILL, dtype=self.torch.uint8, device="cuda")
-
     def query(self, rec_t, nonkeyframe):
         out = []
         for fe in (self.a, self.b):
-            res = self.buf(RS)
+            res = filled(RS)
             fe.query(rec_t.data_ptr(), res.data_ptr(), self.st, nonkeyframe=nonkeyframe)
             fe.finish(self.st)
             out.append(res)
@@ -309,7 +277,7 @@ class Pair:
     def received(self, n, init):
         out = []
         for fe in (self.a, self.b):
-            res = self.buf(n * RS)
+            res = filled(n * RS)
             fe.query_received(self.recs_t.data_ptr(), n, -1, res.data_ptr(), self.st, init_mode=init)
             fe.finish(self.st)
             out.append(res)
@@ -318,16 +286,11 @@ class Pair:
     def loop(self, rec_t, res_pair, cands):
         out = []
         for fe, res in zip((self.a, self.b), res_pair):
-            e = self.buf(len(cands) * EB)
+            e = filled(len(cands) * EB)
             fe.compute_loop(rec_t.data_ptr(), res.data_ptr(), cands, e.data_ptr(), self.st)
             fe.finish(self.st)
             out.append(e.cpu().numpy().tobytes())
         return out
-
-
-def results(t, n):
-    raw = t.cpu().numpy().tobytes()
-    return [lib.LoopResult.from_buffer_copy(raw[i * RS:(i + 1) * RS]) for i in range(n)]
 
 
 @pytest.mark.parametrize("large", [False, True], ids=["coop_scan", "row_scan"])
@@ -341,12 +304,12 @@ def test_frontend_identity(gpu, large, gf):
     # are the old keyframe's at inner product ~0.86, so that the received keyframes near the old one hit the old one.
     g_new = synth.descriptor_db(ND, 4096, 5) + np.random.default_rng(1).normal(0, 0.6 / 64, (ND, 4096))
     new = record(1, 200, "new", (g_new / np.linalg.norm(g_new, axis=1, keepdims=True)).astype(np.float32), seed=1)
-    nt = p.up([new])
-    p.each(lambda fe, rec: fe.ingest_own(p.up([rec]).data_ptr(), p.st), new)
+    nt = upload([new])
+    p.each(lambda fe, rec: fe.ingest_own(upload([rec]).data_ptr(), p.st), new)
     for nonkey in (False, True):
         a, b = p.query(nt, nonkey)
         assert a.cpu().numpy().tobytes() == b.cpu().numpy().tobytes(), f"query (nonkeyframe {nonkey}) differs"
-        r = results(a, 1)[0]
+        r = fh.results(a, 1)[0]
         accepted += r.accepted
         if gf and r.accepted:
             cand = dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], odom_rel=SC["delta_true"], cov=np.eye(6) * 0.01)
@@ -357,7 +320,7 @@ def test_frontend_identity(gpu, large, gf):
         init = [r % 3 == 1 for r in range(n)]
         a, b = p.received(n, init)
         assert a.cpu().numpy().tobytes() == b.cpu().numpy().tobytes(), f"query_received n={n} differs"
-        res = results(a, n)
+        res = fh.results(a, n)
         accepted += sum(x.accepted for x in res)
         if gf and n == 64:
             cands = [dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], init_mode=init[r]) for r in range(n)]
@@ -390,18 +353,18 @@ def test_setter_rules_memory_and_resources(gpu):
         assert fe._lib.osb_frontend_set_db_storage(fe._h, lib.DB_STORAGE_FP32) == lib.ERR_INVALID
         fe.db_reset()
     # after an ingest that has not been synchronised
-    rt = torch.frombuffer(bytearray(bytes(record(1, 5, "old", g[:ND]))), dtype=torch.uint8).cuda()
+    rt = upload([record(1, 5, "old", g[:ND])])
     fe.ingest_own(rt.data_ptr(), st)
     assert fe._lib.osb_frontend_set_db_storage(fe._h, lib.DB_STORAGE_FP32) == lib.ERR_INVALID
     fe.finish(st)
     # the refused calls changed nothing: the store still rounds to fp16 -- it answers like a pre-rounded fp32 store
     ref = make_frontend(64, 0)
-    rr = torch.frombuffer(bytearray(bytes(rounded(record(1, 5, "old", g[:ND])))), dtype=torch.uint8).cuda()
+    rr = upload([rounded(record(1, 5, "old", g[:ND]))])
     ref.ingest_own(rr.data_ptr(), st)
-    q = torch.frombuffer(bytearray(bytes(record(2, 9, "new", g[:ND] + np.float32(1e-3), seed=3))), dtype=torch.uint8).cuda()
+    q = upload([record(2, 9, "new", g[:ND] + np.float32(1e-3), seed=3)])
     outs = []
     for h in (fe, ref):
-        o = torch.full((RS,), FILL, dtype=torch.uint8, device="cuda")
+        o = filled(RS)
         h.query_received(q.data_ptr(), 1, -1, o.data_ptr(), st)
         h.finish(st)
         outs.append(o.cpu().numpy().tobytes())
@@ -410,11 +373,11 @@ def test_setter_rules_memory_and_resources(gpu):
     # fp32 -> fp16 -> fp32 while empty: an fp32 handle
     t1, t2 = make_frontend(64, 0), make_frontend(64, 0)
     t1.set_db_storage("fp16"); t1.set_db_storage("fp32")
-    r0 = torch.frombuffer(bytearray(bytes(record(1, 5, "old", g[:ND]))), dtype=torch.uint8).cuda()
+    r0 = upload([record(1, 5, "old", g[:ND])])
     outs = []
     for h in (t1, t2):
         h.ingest_own(r0.data_ptr(), st)
-        o = torch.full((RS,), FILL, dtype=torch.uint8, device="cuda")
+        o = filled(RS)
         h.query_received(q.data_ptr(), 1, -1, o.data_ptr(), st)
         h.finish(st)
         outs.append(o.cpu().numpy().tobytes())

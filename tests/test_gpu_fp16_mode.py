@@ -19,6 +19,8 @@ from oracle import fp16_ref as f16
 from oracle import frontend_ref as fr
 from oracle import split_model as sm
 from test_gpu_conv_layers import LARGE, LAYER_IDS, LAYERS, SMALL, act, check_bound, pool2, ref64
+from frontend_harness import H0, W0, frame_images
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
@@ -199,7 +201,6 @@ def test_fp16_programmatic_dependent_launch_is_bit_identical(tmp_path):
 # ---------------------------------------------------------------------------------------------------------------------
 # whole networks
 # ---------------------------------------------------------------------------------------------------------------------
-W0, H0 = 96, 64
 NET_IMAGES = [synth.image(51, H0, W0), synth.image(52, H0, W0, zero_bottom_quarter=True), synth.image(53, H0, W0)]
 
 
@@ -277,18 +278,7 @@ def test_switching_back_is_bit_identical_and_acquires_nothing(gpu):
 # the front-end
 # ---------------------------------------------------------------------------------------------------------------------
 def make_frontend(**kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, n_dirs=4, max_num=200, sp_thres=0.015, self_id=1, db_capacity=256,
-                inner_product_thres=0.3, match_index_dist=1, zero_bottom_quarter=True, accept_min_3d_pts=3)
-    args.update(kw)
-    return host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                 synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
-
-
-def frame_images(seed):
-    up = np.stack([synth.image(seed * 10 + d, H0, W0) for d in range(4)])
-    down = np.stack([synth.image(seed * 10 + d + 5, H0, W0) for d in range(4)])
-    return up, down
+    return fh.make_frontend(dict(db_capacity=256, match_index_dist=1), **kw)
 
 
 def blanked(a):

@@ -1,31 +1,20 @@
 """GPU: the keyframe pipeline (extract -> add_to_database -> query -> per-direction match) against the oracle
 composed the same way (LoopCam::generate_stereo_image_descriptor + LoopDetector database rule)."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from omniswarm_b200 import synth, host, lib
 from oracle import frontend_ref as fr
+from frontend_harness import H0, RB, RS, W0, frame_images, upload
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0 = 96, 64
+CONFIG = dict(db_capacity=256, match_index_dist=2)
 
 
 def make_frontend(**kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, n_dirs=4, max_num=200, sp_thres=0.015, self_id=1, db_capacity=256,
-                inner_product_thres=0.3, match_index_dist=2, zero_bottom_quarter=True, accept_min_3d_pts=3)
-    args.update(kw)
-    return host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                 synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
-
-
-def frame_images(seed):
-    up = np.stack([synth.image(seed * 10 + d, H0, W0) for d in range(4)])
-    down = np.stack([synth.image(seed * 10 + d + 5, H0, W0) for d in range(4)])
-    return up, down
+    return fh.make_frontend(CONFIG, **kw)
 
 
 def oracle_record(up, down):
@@ -98,9 +87,9 @@ def test_query_rule_device_vs_oracle(gpu):
     for i in range(30, 40):
         det.add_frame(i, 2, [db[i]], [10])
     assert fe.db_size(False) == 30 and fe.db_size(True) == 10
-    stream = torch.cuda.current_stream().cuda_stream
-    rec_t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    stream = fh.stream()
+    rec_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     cases = [(1, 5, False, False), (1, 29, False, False), (1, 35, False, False), (1, 35, False, True),
              (2, 12, False, False), (2, 29, True, False), (1, 27, False, False), (1, 26, False, False)]
     for drone, row, init_mode, nonkf in cases:
@@ -113,7 +102,7 @@ def test_query_rule_device_vs_oracle(gpu):
         rec_t.copy_(torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8))
         fe.query(rec_t.data_ptr(), res_t.data_ptr(), stream, init_mode, nonkf)
         fe.finish(stream)
-        res = lib.LoopResult.from_buffer_copy(res_t.cpu().numpy().tobytes())
+        res = fh.results(res_t, 1)[0]
         rid, rdist = det.query(drone, q, init_mode, nonkf)
         assert res.hit_id == rid, (drone, row, init_mode, nonkf, res.hit_id, rid)
         assert abs(res.hit_score - rdist) < 1e-4
@@ -203,12 +192,12 @@ def test_geometric_filter_on_loaded_rows(gpu):
     smn = np.zeros(mn, np.int32); smn[100:120] = -1                              # 20 new landmarks without a 3-D flag
     np.ctypeslib.as_array(rec.stereo_match[1])[:] = smn
     np.ctypeslib.as_array(rec.landmarks_flag[1])[:] = (smn >= 0)                 # landmarks_flag is what the filter tests (:574)
-    stream = torch.cuda.current_stream().cuda_stream
-    rec_t = torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8).cuda()
-    res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    stream = fh.stream()
+    rec_t = upload([rec])
+    res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     fe.query(rec_t.data_ptr(), res_t.data_ptr(), stream)
     fe.finish(stream)
-    res = lib.LoopResult.from_buffer_copy(res_t.cpu().numpy().tobytes())
+    res = fh.results(res_t, 1)[0]
     assert res.accepted == 1 and res.hit_id == 3 and res.dir_new[0] == 1
     n = res.n_matches[0]
     mnw = list(res.match_new[0][:n]); mo = list(res.match_old[0][:n])
@@ -229,9 +218,7 @@ def test_c3_keyframe_record_vs_oracle(gpu):
     comp, mean = synth.pca_matrices(0)
     w, nvw = synth.superpoint_weights(0), synth.netvlad_weights(0)
     spw = synth.flatten_sp_weights(w)
-    fe = host.KeyframeFrontend(spw, comp, mean, synth.flatten_nv_weights(nvw), width=W, height=H, n_dirs=4, max_num=MN,
-                               sp_thres=0.015, self_id=3, db_capacity=64, match_index_dist=5, zero_bottom_quarter=True,
-                               accept_min_3d_pts=10)
+    fe = make_frontend(width=W, height=H, max_num=MN, self_id=3, db_capacity=64, match_index_dist=5, accept_min_3d_pts=10)
     up = np.stack([synth.image(100 + d, H, W) for d in range(4)])
     down = np.stack([synth.image(200 + d, H, W) for d in range(4)])
     rec, res = fe.process(up, down, msg_id=4242)
@@ -279,19 +266,19 @@ def test_remote_hit_swaps_matcher_roles(gpu):
     the roles exchanged, direction pairing of loop_detector.cpp:455-465 included."""
     import torch
     fe = make_frontend(self_id=1, match_index_dist=5, inner_product_thres=0.3)
-    stream = torch.cuda.current_stream().cuda_stream
-    recs_t = torch.zeros(2 * lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    stream = fh.stream()
+    recs_t = torch.zeros(2 * RB, dtype=torch.uint8, device="cuda")
     frames = [frame_images(31), frame_images(32)]
     for i, (up, down) in enumerate(frames):
         up = np.ascontiguousarray(up); down = np.ascontiguousarray(down)
-        fe.extract(up.ctypes.data, down.ctypes.data, 700 + i, recs_t.data_ptr() + i * lib.RECORD_BYTES, stream)
+        fe.extract(up.ctypes.data, down.ctypes.data, 700 + i, recs_t.data_ptr() + i * RB, stream)
         fe.finish(stream)
     raw = bytearray(recs_t.cpu().numpy().tobytes())
     foreign = []
     for i in range(2):
-        r = lib.KeyframeRecord.from_buffer(raw, i * lib.RECORD_BYTES)
+        r = lib.KeyframeRecord.from_buffer(raw, i * RB)
         r.drone_id = 2                                            # a foreign drone's keyframe
-        foreign.append(lib.KeyframeRecord.from_buffer_copy(bytes(raw[i * lib.RECORD_BYTES:(i + 1) * lib.RECORD_BYTES])))
+        foreign.append(lib.KeyframeRecord.from_buffer_copy(bytes(raw[i * RB:(i + 1) * RB])))
     recs_t.copy_(torch.frombuffer(raw, dtype=torch.uint8))
     fe.ingest(recs_t.data_ptr(), 2, -1, stream)
     fe.finish(stream)
@@ -302,13 +289,13 @@ def test_remote_hit_swaps_matcher_roles(gpu):
     up, down = frames[0]
     shift = lambda a: np.clip(np.roll(a, 2, axis=2).astype(np.int16) + rng.integers(-3, 4, a.shape), 0, 255).astype(np.uint8)
     up2, down2 = np.ascontiguousarray(shift(up)), np.ascontiguousarray(shift(down))
-    own_t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    own_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     fe.extract(up2.ctypes.data, down2.ctypes.data, 900, own_t.data_ptr(), stream)
     fe.query(own_t.data_ptr(), res_t.data_ptr(), stream, init_mode=False, nonkeyframe=True)
     fe.finish(stream)
-    own = lib.KeyframeRecord.from_buffer_copy(own_t.cpu().numpy().tobytes())
-    res = lib.LoopResult.from_buffer_copy(res_t.cpu().numpy().tobytes())
+    own = fh.records(own_t, 1)[0]
+    res = fh.results(res_t, 1)[0]
     assert own.drone_id == 1
     # expected hit: best inner product over the remote rows (max_index = 1: every row is old enough), rows in ingest order
     rows = [(f, d) for f in range(2) for d in range(4) if foreign[f].n_kpts[d] > 0]
@@ -349,10 +336,10 @@ def test_swarm_exchange_single_rank_and_ingest(gpu):
     import torch
     fe = make_frontend(self_id=1, match_index_dist=5)
     sw = host.Swarm(None, 0, 1)
-    stream = torch.cuda.current_stream().cuda_stream
-    rec_t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    g1 = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    g2 = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    stream = fh.stream()
+    rec_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    g1 = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    g2 = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     up, down = (np.ascontiguousarray(a) for a in frame_images(41))
     fe.extract(up.ctypes.data, down.ctypes.data, 5, rec_t.data_ptr(), stream)
     sw.exchange(rec_t.data_ptr(), g1.data_ptr(), stream)
@@ -361,7 +348,7 @@ def test_swarm_exchange_single_rank_and_ingest(gpu):
     fe.ingest(g2.data_ptr(), 1, -1, stream)
     fe.finish(stream)
     assert torch.equal(rec_t, g1) and torch.equal(rec_t, g2)
-    rec = lib.KeyframeRecord.from_buffer_copy(g2.cpu().numpy().tobytes())
+    rec = fh.records(g2, 1)[0]
     assert rec.msg_id == 5 and fe.db_size(False) == sum(1 for d in range(4) if rec.n_kpts[d] > 0) and fe.db_size(True) == 0
     with pytest.raises(host._l.OsbError):
         host.Swarm(None, 0, 2)                     # world > 1 needs the unique id
@@ -373,13 +360,13 @@ def test_ingest_own_equals_ingest_and_remote_store_wakes_up(gpu):
     rows, the same query results -- and the remote store, unscanned while nothing foreign has arrived, takes part in the
     query as soon as a foreign keyframe is ingested afterwards."""
     import torch
-    stream = torch.cuda.current_stream().cuda_stream
+    stream = fh.stream()
     frames = [frame_images(40 + s) for s in range(3)]
     results = []
     for own in (False, True):
         fe = make_frontend(match_index_dist=1)
-        rec_t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-        res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+        rec_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+        res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
         out = []
         for i, (up, down) in enumerate(frames + [frames[0]]):
             up = np.ascontiguousarray(up); down = np.ascontiguousarray(down)
@@ -399,11 +386,11 @@ def test_ingest_own_equals_ingest_and_remote_store_wakes_up(gpu):
             fe.finish(stream)
             raw = bytearray(rec_t.cpu().numpy().tobytes())
             lib.KeyframeRecord.from_buffer(raw).drone_id = 7
-            f_t = torch.frombuffer(raw, dtype=torch.uint8).cuda()
+            f_t = upload([raw])
             fe.ingest(f_t.data_ptr(), 1, -1, stream)
             fe.query(rec_t.data_ptr(), res_t.data_ptr(), stream, nonkeyframe=True)
             fe.finish(stream)
-            res = lib.LoopResult.from_buffer_copy(res_t.cpu().numpy().tobytes())
+            res = fh.results(res_t, 1)[0]
             assert fe.db_size(True) == 4
             assert res.accepted == 1 and res.hit_id >= lib.REMOTE_MAGIN_NUMBER and res.hit_drone_id == 7
         results.append(out)

@@ -10,10 +10,11 @@ from omniswarm_b200 import synth, host, lib
 from oracle import geometry_ref as gr, lift_ref as lr, pcm_ref as pr
 
 import depth_frontend_ref as dfr
+from frontend_harness import H0, RB, RS, W0, depth_frame
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0 = 96, 64
 K0 = np.array([80.0, 80.0, 48.0, 32.0])
 # pose_drone without translation: pose_drone * extrinsic is then the same double on the host and in pcm_ref.pose_mul
 POSE_DRONE = np.concatenate([[0.0, 0.0, 0.0], synth._quat_from_rotvec(np.array([0.05, -0.02, 0.8]))])
@@ -27,13 +28,11 @@ def extrinsics(nd):
                      for d in range(nd)])
 
 
+CONFIG = dict(db_capacity=256, match_index_dist=2, zero_bottom_quarter=False)
+
+
 def make_frontend(nd=2, W=W0, H=H0, K=K0, depth_camera=True, **kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W, height=H, n_dirs=nd, max_num=200, sp_thres=0.015, self_id=1, db_capacity=256,
-                inner_product_thres=0.3, match_index_dist=2, zero_bottom_quarter=False, accept_min_3d_pts=3)
-    args.update(kw)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
+    fe = fh.make_frontend(CONFIG, n_dirs=nd, width=W, height=H, **kw)
     if depth_camera:
         fe.set_depth_camera(K, extrinsics(nd), 0.3, 10.0)
         fe.set_drone_pose(POSE_DRONE)
@@ -41,12 +40,7 @@ def make_frontend(nd=2, W=W0, H=H0, K=K0, depth_camera=True, **kw):
 
 
 def frame(seed, nd=2, W=W0, H=H0):
-    return (np.stack([synth.image(seed * 10 + d, H, W) for d in range(nd)]),
-            np.stack([synth.depth_image(seed * 10 + d, H, W) for d in range(nd)]))
-
-
-def record_of(t):
-    return lib.KeyframeRecord.from_buffer_copy(t.cpu().numpy().tobytes())
+    return depth_frame(seed, nd, W, H)
 
 
 def arr(x):
@@ -57,16 +51,16 @@ def test_network_outputs_equal_the_stereo_up_side(gpu):
     """the same gray images as the up images of a stereo extract: keypoints, descriptors and NetVLAD bit-identical"""
     import torch
     fe = make_frontend()
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     imgs, deps = frame(1)
     down = np.ascontiguousarray(np.stack([synth.image(900 + d, H0, W0) for d in range(2)]))
-    t_st = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    t_dp = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    t_st = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    t_dp = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     up = np.ascontiguousarray(imgs)
     fe.extract(up.ctypes.data, down.ctypes.data, 1, t_st.data_ptr(), st)
     fe.extract_depth(imgs, deps, 2, t_dp.data_ptr(), st)
     fe.finish(st)
-    rs, rd = record_of(t_st), record_of(t_dp)
+    rs, rd = fh.records(t_st, 1)[0], fh.records(t_dp, 1)[0]
     assert (rd.drone_id, rd.msg_id, rd.n_dirs) == (1, 2, 2)
     assert list(rd.n_kpts) == list(rs.n_kpts) and min(rd.n_kpts[:2]) > 3
     for f in ("kpts", "local_desc", "global_desc"):
@@ -81,12 +75,12 @@ def test_landmarks_equal_depth_lift(gpu):
     """landmarks_3d / landmarks_flag bit-identical to osb_depth_lift on the record's own keypoints, and the oracle's lift"""
     import torch
     fe = make_frontend()
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     imgs, deps = frame(2)
-    t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     fe.extract_depth(imgs, deps, 5, t.data_ptr(), st)
     fe.finish(st)
-    rec = record_of(t)
+    rec = fh.records(t, 1)[0]
     ext = extrinsics(2)
     pose_cam = np.array([pr.pose_mul(POSE_DRONE, ext[d]) for d in range(2)])
     n = np.array(rec.n_kpts[:2], np.int32)
@@ -108,12 +102,12 @@ def test_landmarks_equal_depth_lift(gpu):
 def test_accept_min_3d_pts_gate(gpu):
     import torch
     fe = make_frontend(accept_min_3d_pts=200)
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     imgs, deps = frame(2)
-    t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     fe.extract_depth(imgs, deps, 5, t.data_ptr(), st)
     fe.finish(st)
-    rec = record_of(t)
+    rec = fh.records(t, 1)[0]
     assert min(rec.n_kpts[:2]) > 3
     assert not arr(rec.landmarks_flag)[:2].any() and not arr(rec.landmarks_3d)[:2].any()
     fe.close()
@@ -179,9 +173,9 @@ def test_host_and_device_paths_agree(gpu):
     frames = [frame(30 + s) for s in range(3)] + [frame(30)]
     fa = make_frontend(match_index_dist=1, geometric_filter=True)
     fb = make_frontend(match_index_dist=1, geometric_filter=True)
-    st = torch.cuda.current_stream().cuda_stream
-    rec_t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    st = fh.stream()
+    rec_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     accepted = 0
     for i, (imgs, deps) in enumerate(frames):
         ra, sa = fa.process_depth(imgs, deps, msg_id=i)
@@ -201,9 +195,9 @@ def test_host_and_device_paths_agree(gpu):
 def test_errors_and_stereo_unchanged(gpu):
     import torch
     L = lib.load()
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     imgs, deps = frame(3)
-    t = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     fe = make_frontend(depth_camera=False)
     for call in (lambda: fe.extract_depth(imgs, deps, 1, t.data_ptr(), st),
                  lambda: fe.extract_depth(t.data_ptr(), t.data_ptr(), 1, t.data_ptr(), st, device_images=True),

@@ -2,19 +2,23 @@
 LOWER_CAM_AS_MAIN, loop_cam.cpp:341-523) against oracle/lower_main_ref.py, in the STEREO_FISHEYE (4 directions) and the
 STEREO_PINHOLE (1 direction) configurations; the query stages on such records against the oracle pipeline; compute_loop
 through the right extrinsics against the ground truth of synth.loop_scene."""
-import ctypes as C
+import functools
 
 import numpy as np
 import pytest
+import torch
 
 from omniswarm_b200 import synth, host, lib
-from oracle import frontend_ref as fr, loop_ref as lref, lower_main_ref as lm, pcm_ref as pr
+from oracle import frontend_ref as fr, lower_main_ref as lm, pcm_ref as pr
+from frontend_harness import H0, W0, RB, RS, EB
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0, MN = 96, 64, 200
+MN = 200
 K = np.array([80.0, 80.0, 48.0, 32.0])
 POSE_DRONE = np.concatenate([[1.0, 2.0, 0.5], synth._quat_from_rotvec(np.array([0.02, -0.01, 0.4]))])
+CONFIG = dict(db_capacity=64, match_index_dist=2, geometric_filter=True)
 CONFIGS = {"fisheye": dict(n_dirs=4, zero_bottom_quarter=True), "pinhole": dict(n_dirs=1, zero_bottom_quarter=False)}
 arr = np.ctypeslib.as_array
 
@@ -32,12 +36,7 @@ def rig(nd):
 
 
 def make_frontend(cfg, cameras=True, main="down", **kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, max_num=MN, sp_thres=0.015, self_id=1, db_capacity=64, inner_product_thres=0.3,
-                match_index_dist=2, accept_min_3d_pts=3, geometric_filter=True)
-    args.update(CONFIGS[cfg]); args.update(kw)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
+    fe = fh.make_frontend(dict(CONFIG, **CONFIGS[cfg]), **kw)
     if cameras:
         left, right = rig(fe.cfg.n_dirs)
         fe.set_cameras(K, left, right, triangle_thres=10.0)
@@ -141,15 +140,14 @@ def test_down_records_match_oracle(gpu, cfg):
 
 
 def test_switch_back_to_up_is_byte_identical(gpu):
-    import torch
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     up, down = frame(4, 4)
-    out = torch.zeros(3 * lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    out = torch.zeros(3 * RB, dtype=torch.uint8, device="cuda")
     a, b = make_frontend("fisheye", main="down"), make_frontend("fisheye", main="up")
     a.extract(up.ctypes.data, down.ctypes.data, 5, out.data_ptr(), st)
     a.set_main_camera("up")
-    a.extract(up.ctypes.data, down.ctypes.data, 5, out.data_ptr() + lib.RECORD_BYTES, st)
-    b.extract(up.ctypes.data, down.ctypes.data, 5, out.data_ptr() + 2 * lib.RECORD_BYTES, st)
+    a.extract(up.ctypes.data, down.ctypes.data, 5, out.data_ptr() + RB, st)
+    b.extract(up.ctypes.data, down.ctypes.data, 5, out.data_ptr() + 2 * RB, st)
     a.finish(st); b.finish(st)
     raw = out.cpu().numpy().reshape(3, -1)
     assert np.array_equal(raw[1], raw[2]) and not np.array_equal(raw[0], raw[1])
@@ -157,12 +155,11 @@ def test_switch_back_to_up_is_byte_identical(gpu):
 
 
 def test_process_equals_extract_ingest_query(gpu):
-    import torch
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     frames = [frame(5, 4), frame(6, 4), frame(5, 4, shift=2)]
     a, b = make_frontend("fisheye", match_index_dist=5), make_frontend("fisheye", match_index_dist=5)
-    rt = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-    qt = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    rt = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+    qt = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     accepted = 0
     for i, (up, down) in enumerate(frames):
         rec, res = a.process(up, down, msg_id=i)
@@ -179,30 +176,26 @@ def test_process_equals_extract_ingest_query(gpu):
 def test_query_and_query_received_read_the_record(gpu):
     """DOWN records through ingest, query and query_received against LoopDetectorDB + bf_crosscheck on the records' own
     global and local descriptors"""
-    import torch
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     fe = make_frontend("fisheye", match_index_dist=1)
     frames = [frame(7, 4), frame(8, 4), frame(7, 4, shift=2)]
-    recs_t = torch.zeros(3 * lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    recs_t = torch.zeros(3 * RB, dtype=torch.uint8, device="cuda")
     for i, (up, down) in enumerate(frames):
-        fe.extract(up.ctypes.data, down.ctypes.data, 50 + i, recs_t.data_ptr() + i * lib.RECORD_BYTES, st)
+        fe.extract(up.ctypes.data, down.ctypes.data, 50 + i, recs_t.data_ptr() + i * RB, st)
     fe.finish(st)
-    raw = bytearray(recs_t.cpu().numpy().tobytes())
-    recs = [lib.KeyframeRecord.from_buffer_copy(bytes(raw[i * lib.RECORD_BYTES:(i + 1) * lib.RECORD_BYTES])) for i in range(3)]
+    recs = fh.records(recs_t, 3)
     db = fr.LoopDetectorDB(1, inner_product_thres=0.3, match_index_dist=1)
     fe.ingest(recs_t.data_ptr(), 2, -1, st)                         # the two first keyframes, own
     for r in recs[:2]:
         db.add_frame(r.msg_id, 1, [arr(r.global_desc[d]) for d in range(4)], list(r.n_kpts))
-    res_t = torch.zeros(2 * lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
-    fe.query(recs_t.data_ptr() + 2 * lib.RECORD_BYTES, res_t.data_ptr(), st)
+    res_t = torch.zeros(2 * RS, dtype=torch.uint8, device="cuda")
+    fe.query(recs_t.data_ptr() + 2 * RB, res_t.data_ptr(), st)
     r3 = recs[2]
     foreign = lib.KeyframeRecord.from_buffer_copy(bytes(r3)); foreign.drone_id = 2
-    ft = torch.frombuffer(bytearray(bytes(foreign)), dtype=torch.uint8).cuda()
-    fe.query_received(ft.data_ptr(), 1, -1, res_t.data_ptr() + lib.RESULT_BYTES, st)
+    ft = fh.upload([foreign])
+    fe.query_received(ft.data_ptr(), 1, -1, res_t.data_ptr() + RS, st)
     fe.finish(st)
-    out = res_t.cpu().numpy().tobytes()
-    res_own = lib.LoopResult.from_buffer_copy(out[:lib.RESULT_BYTES])
-    res_rcv = lib.LoopResult.from_buffer_copy(out[lib.RESULT_BYTES:])
+    res_own, res_rcv = fh.results(res_t, 2)
     q = arr(r3.global_desc[1])
     for res, drone in ((res_own, 1), (res_rcv, 2)):
         hid, dist = db.query(drone, q, False, False)
@@ -223,99 +216,45 @@ def test_query_and_query_received_read_the_record(gpu):
 
 
 # ---- compute_loop: the old frame is lifted through the RIGHT extrinsics -------------------------------------------------
-SC = synth.loop_scene()                     # its cameras are the right (lower) ones
-NPT = len(SC["X"][0])
+SC = synth.LOOP_SCENE                       # its cameras are the right (lower) ones
 RIGHT = SC["ext"]
 # the upper cameras: 10 cm above, pitched by 0.1 rad about the camera x axis -- a loop edge through them is wrong
 LEFT = np.array([np.concatenate([e[:3] + np.array([0.0, 0.0, 0.1]),
                                  pr.q_mul(e[3:], synth._quat_from_rotvec(np.array([0.1, 0.0, 0.0])))]) for e in RIGHT])
 PARAMS = dict(odometry_consistency_threshold=10.0, seed=3)
-G_OLD = synth.descriptor_db(4, 4096, 5)
-DESC = [synth.local_descriptors(NPT, 40 + d) for d in range(4)]
-
-
-def scene_record(drone, msg, side, seed=0, g=None):
-    rng = np.random.default_rng(seed)
-    r = lib.KeyframeRecord()
-    r.drone_id, r.msg_id, r.n_dirs = drone, msg, 4
-    for d in range(4):
-        perm = np.arange(NPT) if side == "old" else rng.permutation(NPT)
-        kp = (SC["kp_old"][d] if side == "old" else SC["kp_new"][d])[perm]
-        desc = DESC[d][perm] + (0 if side == "old" else rng.normal(0, 0.02, (NPT, 64)).astype(np.float32))
-        desc /= np.linalg.norm(desc, axis=1, keepdims=True)
-        flag = np.ones(NPT, np.int32)
-        if side == "new":
-            flag[::11] = 0
-        r.n_kpts[d] = NPT
-        arr(r.global_desc[d])[:] = G_OLD[d] if g is None else g[d]
-        arr(r.local_desc[d])[:NPT] = desc
-        arr(r.kpts[d])[:NPT] = kp
-        arr(r.landmarks_3d[d])[:NPT] = SC["X"][d][perm]
-        arr(r.landmarks_flag[d])[:NPT] = flag
-        arr(r.stereo_match[d])[:NPT] = np.where(flag > 0, 0, -1)
-    return r
-
-
-def noisy_g(seed):
-    g = G_OLD + np.random.default_rng(seed).normal(0, 0.05 / 64, G_OLD.shape).astype(np.float32)
-    return g / np.linalg.norm(g, axis=1, keepdims=True)
-
-
-def loop_view(rec):
-    n = list(rec.n_kpts)
-    return dict(drone_id=rec.drone_id, msg_id=rec.msg_id, n_kpts=n, kpts=[arr(rec.kpts[d])[:n[d]].copy() for d in range(4)],
-                flags=[arr(rec.landmarks_flag[d])[:n[d]].copy() for d in range(4)],
-                l3d=[arr(rec.landmarks_3d[d])[:n[d]].copy() for d in range(4)])
-
-
-def loop_oracle(res, query_rec, hit_rec, cand):
-    sw = bool(res.swapped)
-    new, old = (loop_view(hit_rec), loop_view(query_rec)) if sw else (loop_view(query_rec), loop_view(hit_rec))
-    main_new, main_old = (res.hit_dir, 1) if sw else (1, res.hit_dir)
-    slots = [dict(dir_new=res.dir_new[j], dir_old=res.dir_old[j], geo_valid=res.geo_valid[j],
-                  geo_new=list(res.geo_new[j][:res.n_geo[j]]), geo_old=list(res.geo_old[j][:res.n_geo[j]]),
-                  match_new=list(res.match_new[j][:res.n_matches[j]]), match_old=list(res.match_old[j][:res.n_matches[j]]))
-             for j in range(4) if res.dir_new[j] >= 0]
-    c = dict(init_mode=False, odom_rel=cand.get("odom_rel", [0, 0, 0, 1, 0, 0, 0]), cov=cand.get("cov", np.eye(6)),
-             pose_now=cand["pose_hit"] if sw else cand["pose_query"], pose_old=cand["pose_query"] if sw else cand["pose_hit"])
-    return lref.compute_loop(dict(accepted=res.accepted, slots=slots), new, old, SC["K"], RIGHT, main_new, main_old, c, PARAMS)
+scene_record = functools.partial(synth.loop_record, n_outliers=0)
 
 
 @pytest.mark.parametrize("hit", ["local", "swapped_remote"])
 def test_loop_edge_uses_the_right_extrinsics(gpu, hit):
-    import torch
-    st = torch.cuda.current_stream().cuda_stream
-    comp, mean = synth.pca_matrices(0)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W0, height=H0, n_dirs=4, max_num=MN,
-                               self_id=1, db_capacity=64, match_index_dist=5, accept_min_3d_pts=3, geometric_filter=True)
+    st = fh.stream()
+    fe = make_frontend("fisheye", cameras=False, main="up", match_index_dist=5)
     fe.set_cameras(SC["K"], LEFT, RIGHT, 0.006)
     fe.set_main_camera("down")
     fe.set_loop_params(**PARAMS)
-    up = lambda recs: torch.frombuffer(bytearray(b"".join(bytes(r) for r in recs)), dtype=torch.uint8).cuda()
     if hit == "local":
-        old, new = scene_record(1, 100, "old"), scene_record(1, 101, "new", seed=1, g=noisy_g(1))
-        ot = up([old]); fe.ingest_own(ot.data_ptr(), st)
+        old, new = scene_record(1, 100, "old"), scene_record(1, 101, "new", seed=1, g=synth.loop_noisy_g(1))
+        ot = fh.upload([old]); fe.ingest_own(ot.data_ptr(), st)
         qrec, hrec = new, old
         cand = dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], odom_rel=SC["delta_true"], cov=np.eye(6) * 0.01)
         nonkf = False
     else:
-        remote = scene_record(2, 200, "new", seed=2, g=noisy_g(2))
-        t = up([remote]); fe.ingest(t.data_ptr(), 1, -1, st)
+        remote = scene_record(2, 200, "new", seed=2, g=synth.loop_noisy_g(2))
+        t = fh.upload([remote]); fe.ingest(t.data_ptr(), 1, -1, st)
         qrec, hrec = scene_record(1, 100, "old"), remote
         cand = dict(pose_query=SC["pose_old"], pose_hit=SC["pose_new"])
         nonkf = True
-    rt = up([qrec]); fe.ingest_own(rt.data_ptr(), st)
-    res_t = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+    rt = fh.upload([qrec]); fe.ingest_own(rt.data_ptr(), st)
+    res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     fe.query(rt.data_ptr(), res_t.data_ptr(), st, nonkeyframe=nonkf)
     fe.finish(st)
-    res = lib.LoopResult.from_buffer_copy(res_t.cpu().numpy().tobytes())
+    res = fh.results(res_t, 1)[0]
     assert res.accepted and bool(res.swapped) == (hit != "local")
-    out = torch.zeros(lib.EDGE_BYTES, dtype=torch.uint8, device="cuda")
+    out = torch.zeros(EB, dtype=torch.uint8, device="cuda")
     fe.compute_loop(rt.data_ptr(), res_t.data_ptr(), [cand], out.data_ptr(), st)
     fe.finish(st)
-    e = lib.LoopEdgeResult.from_buffer_copy(out.cpu().numpy().tobytes())
-    ref = loop_oracle(res, qrec, hrec, cand)
+    e = lib.LoopEdgeResult.from_buffer_copy(fh.edges(out, 1)[0])
+    ref = fh.loop_oracle(res, qrec, hrec, cand, SC["K"], RIGHT, PARAMS)
     assert e.status == ref["status"] == lib.LOOP_ACCEPTED and e.n_corr == ref["n_corr"]
     n = e.n_corr
     assert list(e.corr_idx_new[:n]) == ref["idx_new"].tolist() and list(e.corr_idx_old[:n]) == ref["idx_old"].tolist()
@@ -327,11 +266,10 @@ def test_loop_edge_uses_the_right_extrinsics(gpu, hit):
 
 
 def test_depth_refusals_launches_and_resources(gpu):
-    import torch
-    st = torch.cuda.current_stream().cuda_stream
+    st = fh.stream()
     base = host.live_resources()
     up, down = frame(9, 4)
-    rt = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
+    rt = torch.zeros(RB, dtype=torch.uint8, device="cuda")
     fe = make_frontend("fisheye", main="up")
     fe.extract(up.ctypes.data, down.ctypes.data, 1, rt.data_ptr(), st)        # warm-up
     fe.finish(st)

@@ -4,34 +4,24 @@ osb_frontend_query writes for that record alone, hits and matches must agree wit
 cross-check matcher, and the batch must not read the remote store, whatever it holds."""
 import numpy as np
 import pytest
+import torch
 
 from omniswarm_b200 import synth, host, lib
 from oracle import frontend_ref as fr
+from frontend_harness import FILL, RB, RS, filled, frame_images, upload
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0, ND, MN = 96, 64, 4, 200
-RB, RS = lib.RECORD_BYTES, lib.RESULT_BYTES
+ND, MN = 4, 200
 QDIR = 1
 N_OWN = 4
 SIGMAS = [0.0, 0.5, 2.5, 3.5, 6.0]      # inner product with the source ~ 1, 0.89, 0.37, 0.27, 0.16
-FILL = 0x5A                              # result buffers start with this byte: unwritten fields compare equal too
+CONFIG = dict(db_capacity=256, init_mode_product_thres=0.2, match_index_dist=2)
 
 
 def make_frontend(**kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, n_dirs=ND, max_num=MN, sp_thres=0.015, self_id=1, db_capacity=256,
-                inner_product_thres=0.3, init_mode_product_thres=0.2, match_index_dist=2, zero_bottom_quarter=True,
-                accept_min_3d_pts=3)
-    args.update(kw)
-    return host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                 synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
-
-
-def frame_images(seed):
-    up = np.stack([synth.image(seed * 10 + d, H0, W0) for d in range(ND)])
-    down = np.stack([synth.image(seed * 10 + d + 5, H0, W0) for d in range(ND)])
-    return up, down
+    return fh.make_frontend(CONFIG, **kw)
 
 
 def shifted(seed):
@@ -43,7 +33,6 @@ def shifted(seed):
 
 def coop_rows():
     """rows up to which a search takes the cooperative scan kernel: DB_COOP_CHUNK (64) rows x 2 CTAs per SM"""
-    import torch
     return 64 * 2 * torch.cuda.get_device_properties(0).multi_processor_count
 
 
@@ -61,11 +50,9 @@ class Round:
     records whose query descriptor is a noisy loaded row, at the noise levels of SIGMAS."""
 
     def __init__(self, n_loaded, geometric_filter, local_desc=True, ingest_pool=True):
-        import torch
-        self.torch = torch
         self.gf = geometric_filter
         self.fe = make_frontend(db_capacity=n_loaded + N_OWN * ND + 64 * ND, geometric_filter=geometric_filter)
-        fe, st = self.fe, torch.cuda.current_stream().cuda_stream
+        fe, st = self.fe, fh.stream()
         self.stream = st
         rec_t = torch.zeros(RB, dtype=torch.uint8, device="cuda")
         self.own = []
@@ -74,7 +61,7 @@ class Round:
             fe.extract(up.ctypes.data, down.ctypes.data, 100 + i, rec_t.data_ptr(), st)
             fe.ingest_own(rec_t.data_ptr(), st)
             fe.finish(st)
-            self.own.append(lib.KeyframeRecord.from_buffer_copy(rec_t.cpu().numpy().tobytes()))
+            self.own.append(fh.records(rec_t, 1)[0])
         self.n_own_rows = sum(1 for r in self.own for d in range(ND) if r.n_kpts[d] > 0)
         self.g = synth.descriptor_db(n_loaded, 4096, 11)
         self.ld = synth.local_descriptors(MN, 77)[None].repeat(n_loaded, 0) if local_desc else None
@@ -112,7 +99,7 @@ class Round:
             rec.drone_id, rec.msg_id = 2 + r % 3, 1000 + r
             recs.append(bytes(rec))
         self.recs = [lib.KeyframeRecord.from_buffer_copy(b) for b in recs]
-        self.recs_t = torch.frombuffer(bytearray(b"".join(recs)), dtype=torch.uint8).cuda()
+        self.recs_t = upload(recs)
         if ingest_pool:             # the remote store holds copies of the first 16 records
             fe.ingest(self.recs_t.data_ptr(), 16, -1, st)
             fe.finish(st)
@@ -121,7 +108,7 @@ class Round:
         return self.recs_t.data_ptr() + r * RB
 
     def batch(self, n, skip=-1, init=None, recs_ptr=None):
-        out = self.torch.full((max(n, 1) * RS,), FILL, dtype=self.torch.uint8, device="cuda")
+        out = filled(max(n, 1) * RS)
         self.fe.query_received(self.rec_ptr() if recs_ptr is None else recs_ptr, n, skip, out.data_ptr(), self.stream,
                                init_mode=init)
         self.fe.finish(self.stream)
@@ -129,7 +116,7 @@ class Round:
         return [raw[r * RS:(r + 1) * RS] for r in range(n)]
 
     def single(self, r, init_mode=False):
-        out = self.torch.full((RS,), FILL, dtype=self.torch.uint8, device="cuda")
+        out = filled(RS)
         self.fe.query(self.rec_ptr(r), out.data_ptr(), self.stream, init_mode=init_mode, nonkeyframe=False)
         self.fe.finish(self.stream)
         return out.cpu().numpy().tobytes()
@@ -189,7 +176,6 @@ def test_hits_and_matches_against_oracle(gpu):
     """Hits against LoopDetectorDB.query(drone, q, init_mode, nonkeyframe=False), matches against bf_crosscheck with the
     foreign record as the new side.  Record 3 scores between INIT_MODE_PRODUCT_THRES and INNER_PRODUCT_THRES: it hits
     only with its own init flag set, and its neighbours keep theirs."""
-    import torch
     rd = Round(300, 0)
     det = rd.oracle()
     # record 3 of the batch: a loaded row at inner product ~0.25
@@ -244,14 +230,13 @@ def test_hits_and_matches_against_oracle(gpu):
 
 def test_skip_and_own_records_stay_closed(gpu):
     """`skip` and an own-drone record in the batch get the gate-closed result; the others are unaffected by them."""
-    import torch
     for gf in (0, 1):
         rd = Round(300, gf)
         n = 12
         ref = rd.batch(n)
         raw = bytearray(rd.recs_t.cpu().numpy().tobytes())
         lib.KeyframeRecord.from_buffer(raw, 7 * RB).drone_id = 1               # record 7 is this drone's own
-        recs2 = torch.frombuffer(raw, dtype=torch.uint8).cuda()
+        recs2 = upload([raw])
         assert res_of(ref[7]).accepted == 1 and res_of(ref[11]).accepted == 1  # synthetic records at scores 0.37, 0.89
         got = rd.batch(n, skip=11, recs_ptr=recs2.data_ptr())
         for r in range(n):
@@ -280,10 +265,9 @@ def test_remote_store_and_ingest_order_do_not_matter(gpu):
     qs = np.stack([np.ctypeslib.as_array(rd.recs[r].global_desc[QDIR]) for r in range(n)])
     fe.db_load(qs, remote=True)
     # an own non-keyframe query whose remote top-k is a perfect remote hit
-    import torch
     own = lib.KeyframeRecord.from_buffer_copy(bytes(rd.recs[0]))
     own.drone_id = 1
-    own_t = torch.frombuffer(bytearray(bytes(own)), dtype=torch.uint8).cuda()
+    own_t = upload([own])
     res_t = torch.zeros(RS, dtype=torch.uint8, device="cuda")
     fe.query(own_t.data_ptr(), res_t.data_ptr(), st, nonkeyframe=True)
     fe.finish(st)
@@ -295,12 +279,11 @@ def test_remote_store_and_ingest_order_do_not_matter(gpu):
 
 
 def test_empty_local_store_gives_no_hits(gpu):
-    import torch
     rd = Round(64, 0)
     fe = make_frontend()
     fe.db_load(np.stack([np.ctypeslib.as_array(rd.recs[r].global_desc[QDIR]) for r in range(8)]), remote=True)
-    st = torch.cuda.current_stream().cuda_stream
-    out = torch.full((9 * RS,), FILL, dtype=torch.uint8, device="cuda")
+    st = fh.stream()
+    out = filled(9 * RS)
     fe.query_received(rd.rec_ptr(), 9, -1, out.data_ptr(), st, init_mode=[1] * 9)
     fe.finish(st)
     raw = out.cpu().numpy().tobytes()
@@ -314,11 +297,10 @@ def test_arguments_and_structure(gpu):
     """n = 0 does nothing; n = 65 and null pointers are refused.  One call launches the same kernels for n = 2 and n = 8
     (one scan pass) and one more at n = 9 (the second pass).  The scratch is acquired by the first call only, and destroy
     gives it back."""
-    import torch
     n_start = host.live_resources()
     rd = Round(300, 1)
     fe, st = rd.fe, rd.stream
-    out = torch.full((65 * RS,), FILL, dtype=torch.uint8, device="cuda")
+    out = filled(65 * RS)
     L = fe._lib
     c0, live0 = host.launch_count(), host.live_resources()
     fe.query_received(rd.rec_ptr(), 0, -1, out.data_ptr(), st)

@@ -3,12 +3,14 @@ and the number of kernels one keyframe launches.  Ingest past capacity and db_lo
 refused without touching either store; db_reset must bring a handle back to its freshly created state."""
 import numpy as np
 import pytest
+import torch
 
 from omniswarm_b200 import synth, host, lib
+from frontend_harness import H0, RB, RS, W0, depth_frame, frame_images, upload
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0 = 96, 64
 ND = 4
 K0 = np.array([80.0, 80.0, 48.0, 32.0])
 IDENT = np.array([0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0])
@@ -18,49 +20,34 @@ LAUNCHES_STEREO = 51          # process(): cameras set, geometric filter on
 LAUNCHES_DEPTH = 48           # process_depth()
 
 
+CONFIG = dict(db_capacity=8, match_index_dist=1)
+
+
 def make_frontend(**kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, n_dirs=ND, max_num=200, sp_thres=0.015, self_id=1, db_capacity=8,
-                inner_product_thres=0.3, match_index_dist=1, zero_bottom_quarter=True, accept_min_3d_pts=3)
-    args.update(kw)
-    return host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                                 synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
-
-
-def frame_images(seed):
-    up = np.stack([synth.image(seed * 10 + d, H0, W0) for d in range(ND)])
-    down = np.stack([synth.image(seed * 10 + d + 5, H0, W0) for d in range(ND)])
-    return up, down
-
-
-def depth_frame(seed):
-    return (np.stack([synth.image(seed * 10 + d, H0, W0) for d in range(ND)]),
-            np.stack([synth.depth_image(seed * 10 + d, H0, W0) for d in range(ND)]))
+    return fh.make_frontend(CONFIG, **kw)
 
 
 class Dev:
     """one device record, one device result and the current torch stream"""
 
     def __init__(self, fe):
-        import torch
         self.fe = fe
-        self.stream = torch.cuda.current_stream().cuda_stream
-        self.rec = torch.zeros(lib.RECORD_BYTES, dtype=torch.uint8, device="cuda")
-        self.res = torch.zeros(lib.RESULT_BYTES, dtype=torch.uint8, device="cuda")
+        self.stream = fh.stream()
+        self.rec = torch.zeros(RB, dtype=torch.uint8, device="cuda")
+        self.res = torch.zeros(RS, dtype=torch.uint8, device="cuda")
 
     def extract(self, seed, msg_id, drone_id=None):
-        import torch
         up, down = (np.ascontiguousarray(a) for a in frame_images(seed))
         self.fe.extract(up.ctypes.data, down.ctypes.data, msg_id, self.rec.data_ptr(), self.stream)
         self.fe.finish(self.stream)
         if drone_id is not None:
-            raw = bytearray(self.rec.cpu().numpy().tobytes())
-            lib.KeyframeRecord.from_buffer(raw).drone_id = drone_id
-            self.rec.copy_(torch.frombuffer(raw, dtype=torch.uint8))
+            rec = self.record()
+            rec.drone_id = drone_id
+            self.rec.copy_(upload([rec]))
         return self.record()
 
     def record(self):
-        return lib.KeyframeRecord.from_buffer_copy(self.rec.cpu().numpy().tobytes())
+        return fh.records(self.rec, 1)[0]
 
     def ingest(self):
         self.fe.ingest(self.rec.data_ptr(), 1, -1, self.stream)
@@ -145,12 +132,11 @@ def test_db_load_past_rows_or_frames_is_refused(gpu):
     for d in range(ND):
         rec.n_kpts[d] = 5
     np.ctypeslib.as_array(rec.global_desc[1])[:] = g[2]
-    import torch
-    dev.rec.copy_(torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8))
+    dev.rec.copy_(upload([rec]))
     hit_id, hit_dir, _, accepted, _, hit_msg_id, hit_drone_id = dev.query()[:7]
     assert (accepted, hit_id, hit_dir, hit_msg_id, hit_drone_id) == (1, 2, 1, -1, 1)
     np.ctypeslib.as_array(rec.global_desc[1])[:] = g[12]
-    dev.rec.copy_(torch.frombuffer(bytearray(bytes(rec)), dtype=torch.uint8))
+    dev.rec.copy_(upload([rec]))
     hit_id, _, _, accepted, _, _, hit_drone_id = dev.query(nonkeyframe=True)[:7]
     assert (accepted, hit_id, hit_drone_id) == (1, lib.REMOTE_MAGIN_NUMBER + 4, -1)
     fe.close()

@@ -5,6 +5,8 @@ import pytest
 
 from omniswarm_b200 import synth, host, lib
 from oracle import lift_ref as lr, pcm_ref as pr
+from frontend_harness import H0, W0
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 K = np.array([80.0, 80.0, 48.0, 32.0])            # 96 x 64 flattened pinhole
@@ -83,12 +85,8 @@ def test_depth_lift_matches_oracle(gpu):
 def test_frontend_record_carries_triangulated_landmarks(gpu):
     """osb_frontend_set_cameras: extract triangulates the cross-check stereo pairs on the device and the record's
     landmarks_flag / landmarks_3d are the reference's (loop_cam.cpp:393-432), not the stereo_match >= 0 superset."""
-    W0, H0 = 96, 64
-    comp, mean = synth.pca_matrices(0)
-    spw = synth.flatten_sp_weights(synth.superpoint_weights(0))
-    fe = host.KeyframeFrontend(spw, comp, mean, synth.flatten_nv_weights(synth.netvlad_weights(0)), width=W0, height=H0,
-                               n_dirs=4, max_num=200, sp_thres=0.015, self_id=1, db_capacity=64, match_index_dist=5,
-                               accept_min_3d_pts=3)
+    spw, comp, mean, _ = synth.frontend_weights()
+    fe = fh.make_frontend(db_capacity=64, match_index_dist=5)
     left, right = rig(4)
     pose_drone = np.concatenate([[1.0, 2.0, 0.5], synth._quat_from_rotvec(np.array([0.02, -0.01, 0.4]))])
     up = np.stack([synth.image(300 + d, H0, W0) for d in range(4)])

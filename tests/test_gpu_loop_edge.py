@@ -10,27 +10,22 @@ import numpy as np
 import pytest
 
 from omniswarm_b200 import synth, host, lib
-from oracle import loop_ref as lr
+from frontend_harness import EB, RB, RS, filled, loop_oracle, upload
+import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
-W0, H0, ND, MN = 96, 64, 4, 200
-RB, RS, EB = lib.RECORD_BYTES, lib.RESULT_BYTES, lib.EDGE_BYTES
+ND, MN = 4, 200
 QDIR = 1
-SC = synth.loop_scene()
-NPT = len(SC["X"][0])
+SC, NPT = synth.LOOP_SCENE, synth.LOOP_NPT
 COV = np.eye(6) * 0.01
 PARAMS = dict(odometry_consistency_threshold=10.0, seed=3)
+CONFIG = dict(db_capacity=64, init_mode_product_thres=0.2, match_index_dist=5, geometric_filter=True, ransac_seed=0)
+record, noisy_g = synth.loop_record, synth.loop_noisy_g
 
 
 def make_frontend(cameras="stereo", loop_params=True, **kw):
-    comp, mean = synth.pca_matrices(0)
-    args = dict(width=W0, height=H0, n_dirs=ND, max_num=MN, sp_thres=0.015, self_id=1, db_capacity=64,
-                inner_product_thres=0.3, init_mode_product_thres=0.2, match_index_dist=5, accept_min_3d_pts=3,
-                geometric_filter=True, ransac_seed=0)
-    args.update(kw)
-    fe = host.KeyframeFrontend(synth.flatten_sp_weights(synth.superpoint_weights(0)), comp, mean,
-                               synth.flatten_nv_weights(synth.netvlad_weights(0)), **args)
+    fe = fh.make_frontend(CONFIG, **kw)
     if cameras in ("stereo", "both"):
         fe.set_cameras(SC["K"], SC["ext"], SC["ext"], 0.006)
     if cameras in ("depth", "both"):
@@ -40,123 +35,29 @@ def make_frontend(cameras="stereo", loop_params=True, **kw):
     return fe
 
 
-G_OLD = synth.descriptor_db(ND, 4096, 5)                  # the old keyframe's global descriptor per direction
-DESC = [synth.local_descriptors(NPT, 40 + d) for d in range(ND)]
-
-
-def record(drone, msg, side, seed=0, g=None, n_outliers=4, unflag_every=11, few_flags_dir=None, scramble=False):
-    """side 'old': the old camera's pixels; 'new': the new camera's, points permuted, every `unflag_every`-th landmark
-    unflagged, `n_outliers` points per direction moved to random pixels / 3-D (their descriptors still match the old point:
-    outlier matches).  few_flags_dir: only two landmarks of that direction flagged (a failed homography pair)."""
-    rng = np.random.default_rng(seed)
-    r = lib.KeyframeRecord()
-    r.drone_id, r.msg_id, r.n_dirs = drone, msg, ND
-    for d in range(ND):
-        perm = np.arange(NPT) if side == "old" else rng.permutation(NPT)
-        kp = (SC["kp_old"][d] if side == "old" else SC["kp_new"][d])[perm].copy()
-        X = SC["X"][d][perm].copy()
-        desc = DESC[d][perm] + (0 if side == "old" else rng.normal(0, 0.02, (NPT, 64)).astype(np.float32))
-        desc /= np.linalg.norm(desc, axis=1, keepdims=True)
-        flag = np.ones(NPT, np.int32)
-        if side == "new":
-            flag[::unflag_every] = 0
-            out = rng.choice(NPT, n_outliers, replace=False)
-            kp[out] = rng.uniform(0, 96, (n_outliers, 2))
-            X[out] = rng.normal(0, 3, (n_outliers, 3))
-        if few_flags_dir == d:
-            flag[:] = 0
-            flag[[3, 17]] = 1
-        if scramble:
-            X = rng.normal(0, 3, X.shape).astype(np.float32)
-        r.n_kpts[d] = NPT
-        gd = G_OLD[d] if g is None else g[d]
-        np.ctypeslib.as_array(r.global_desc[d])[:] = gd
-        np.ctypeslib.as_array(r.local_desc[d])[:NPT] = desc
-        np.ctypeslib.as_array(r.kpts[d])[:NPT] = kp
-        np.ctypeslib.as_array(r.landmarks_3d[d])[:NPT] = X
-        np.ctypeslib.as_array(r.landmarks_flag[d])[:NPT] = flag
-        np.ctypeslib.as_array(r.stereo_match[d])[:NPT] = np.where(flag > 0, 0, -1)
-    return r
-
-
-def noisy_g(seed, sigma=0.05):
-    rng = np.random.default_rng(seed)
-    g = G_OLD + rng.normal(0, sigma / 64, G_OLD.shape).astype(np.float32)
-    return g / np.linalg.norm(g, axis=1, keepdims=True)
-
-
-def frame(rec):
-    """what the oracle reads of a record (or of the store row made from it)"""
-    n = list(rec.n_kpts)
-    return dict(drone_id=rec.drone_id, msg_id=rec.msg_id, n_kpts=n,
-                kpts=[np.ctypeslib.as_array(rec.kpts[d])[:n[d]].copy() for d in range(ND)],
-                flags=[np.ctypeslib.as_array(rec.landmarks_flag[d])[:n[d]].copy() for d in range(ND)],
-                l3d=[np.ctypeslib.as_array(rec.landmarks_3d[d])[:n[d]].copy() for d in range(ND)])
-
-
-def hit_of(res):
-    slots = []
-    for j in range(ND):
-        if res.dir_new[j] < 0:
-            continue
-        slots.append(dict(dir_new=res.dir_new[j], dir_old=res.dir_old[j], geo_valid=res.geo_valid[j],
-                          geo_new=list(res.geo_new[j][:res.n_geo[j]]), geo_old=list(res.geo_old[j][:res.n_geo[j]]),
-                          match_new=list(res.match_new[j][:res.n_matches[j]]),
-                          match_old=list(res.match_old[j][:res.n_matches[j]])))
-    return dict(accepted=res.accepted, has_frame=res.hit_msg_id != -1, slots=slots)
-
-
 def oracle(res, query_rec, hit_rec, cand, params=None, K=None):
-    """compute_loop with the roles of the device (:113-118)"""
-    sw = bool(res.swapped)
-    new, old = (frame(hit_rec), frame(query_rec)) if sw else (frame(query_rec), frame(hit_rec) if hit_rec else None)
-    main_new, main_old = (res.hit_dir, QDIR) if sw else (QDIR, res.hit_dir)
-    c = dict(init_mode=cand.get("init_mode", False), odom_rel=cand.get("odom_rel", [0, 0, 0, 1, 0, 0, 0]),
-             cov=cand.get("cov", np.eye(6)),
-             pose_now=cand["pose_hit"] if sw else cand["pose_query"], pose_old=cand["pose_query"] if sw else cand["pose_hit"])
-    return lr.compute_loop(hit_of(res), new, old, SC["K"] if K is None else K, SC["ext"], main_new, main_old, c,
-                           dict(PARAMS, **(params or {})))
+    return loop_oracle(res, query_rec, hit_rec, cand, SC["K"] if K is None else K, SC["ext"],
+                       dict(PARAMS, **(params or {})), QDIR)
 
 
-class Dev:
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.st = torch.cuda.current_stream().cuda_stream
-
-    def up(self, recs):
-        return self.torch.frombuffer(bytearray(b"".join(bytes(r) for r in recs)), dtype=self.torch.uint8).cuda()
-
-    def buf(self, nbytes):
-        return self.torch.full((nbytes,), 0x5A, dtype=self.torch.uint8, device="cuda")
-
-    def results(self, t, n):
-        raw = t.cpu().numpy().tobytes()
-        return [lib.LoopResult.from_buffer_copy(raw[i * RS:(i + 1) * RS]) for i in range(n)]
-
-    def edges(self, t, n):
-        raw = t.cpu().numpy().tobytes()
-        return [raw[i * EB:(i + 1) * EB] for i in range(n)]
-
-
-def own_query(fe, dv, old_rec, new_rec, nonkeyframe=False, ingest_old=True):
+def own_query(fe, st, old_rec, new_rec, nonkeyframe=False, ingest_old=True):
     """ingest the old record, then the new one (own, as on_image_recv does), query the new one -> (rec_t, res_t, result)"""
     if ingest_old:
-        ot = dv.up([old_rec])
-        fe.ingest_own(ot.data_ptr(), dv.st)
-    rt = dv.up([new_rec])
-    fe.ingest_own(rt.data_ptr(), dv.st)
-    res_t = dv.buf(RS)
-    fe.query(rt.data_ptr(), res_t.data_ptr(), dv.st, nonkeyframe=nonkeyframe)
-    fe.finish(dv.st)
-    return rt, res_t, dv.results(res_t, 1)[0]
+        ot = upload([old_rec])
+        fe.ingest_own(ot.data_ptr(), st)
+    rt = upload([new_rec])
+    fe.ingest_own(rt.data_ptr(), st)
+    res_t = filled(RS)
+    fe.query(rt.data_ptr(), res_t.data_ptr(), st, nonkeyframe=nonkeyframe)
+    fe.finish(st)
+    return rt, res_t, fh.results(res_t, 1)[0]
 
 
-def run_loop(fe, dv, rec_ptr, res_ptr, cands):
-    out = dv.buf(len(cands) * EB)
-    fe.compute_loop(rec_ptr, res_ptr, cands, out.data_ptr(), dv.st)
-    fe.finish(dv.st)
-    return dv.edges(out, len(cands))
+def run_loop(fe, st, rec_ptr, res_ptr, cands):
+    out = filled(len(cands) * EB)
+    fe.compute_loop(rec_ptr, res_ptr, cands, out.data_ptr(), st)
+    fe.finish(st)
+    return fh.edges(out, len(cands))
 
 
 def check(raw, ref, truth=True):
@@ -199,13 +100,13 @@ def cand_own(init_mode=False, odom=None):
 
 
 def test_own_query_local_hit_and_pnp_inputs(gpu):
-    dv = Dev()
+    st = fh.stream()
     fe = make_frontend()
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=1, g=noisy_g(1))
-    rt, res_t, res = own_query(fe, dv, old, new)
+    rt, res_t, res = own_query(fe, st, old, new)
     assert res.accepted and not res.swapped and res.hit_dir == QDIR and sum(res.geo_valid) == ND
     cand = cand_own()
-    raw = run_loop(fe, dv, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
+    raw = run_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
     ref = oracle(res, new, old, cand)
     e = check(raw, ref)
     assert e.status == lib.LOOP_ACCEPTED and e.pnp.odometry_consistent == 1 and e.pnp.md < 1e-6
@@ -220,18 +121,18 @@ def test_own_query_local_hit_and_pnp_inputs(gpu):
 
 def test_own_query_remote_hit_is_swapped(gpu):
     """the own keyframe hits a remote one: new = the remote keyframe, its 3-D landmarks read from the remote store"""
-    dv = Dev()
+    st = fh.stream()
     fe = make_frontend()
     remote = record(2, 200, "new", seed=2, g=noisy_g(2))
-    t = dv.up([remote])
-    fe.ingest(t.data_ptr(), 1, -1, dv.st)
+    t = upload([remote])
+    fe.ingest(t.data_ptr(), 1, -1, st)
     own = record(1, 100, "old")
     # the remote record's buffer is overwritten: what compute_loop reads of it must come from the store
-    t.copy_(dv.up([record(2, 200, "new", seed=99, scramble=True)]))
-    rt, res_t, res = own_query(fe, dv, None, own, nonkeyframe=True, ingest_old=False)
+    t.copy_(upload([record(2, 200, "new", seed=99, scramble=True)]))
+    rt, res_t, res = own_query(fe, st, None, own, nonkeyframe=True, ingest_old=False)
     assert res.accepted and res.swapped and res.hit_msg_id == 200 and res.hit_drone_id == 2
     cand = dict(pose_query=SC["pose_old"], pose_hit=SC["pose_new"])
-    raw = run_loop(fe, dv, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
+    raw = run_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
     e = check(raw, oracle(res, own, remote, cand))
     assert e.status == lib.LOOP_ACCEPTED and (e.drone_id_a, e.drone_id_b, e.msg_id_a, e.msg_id_b) == (1, 2, 100, 200)
     assert e.pnp.md == 0.0                                         # inter-drone: no odometry check
@@ -241,11 +142,11 @@ def test_own_query_remote_hit_is_swapped(gpu):
 def test_received_batch_equals_single_calls(gpu):
     """a round of 10 received keyframes: hits with outliers, a failed homography pair (the 1-3-match quirk), init mode,
     misses; one call for all, each equal to its one-candidate call and to the oracle"""
-    dv = Dev()
+    st = fh.stream()
     fe = make_frontend()
     old = record(1, 100, "old")
-    ot = dv.up([old])
-    fe.ingest_own(ot.data_ptr(), dv.st)
+    ot = upload([old])
+    fe.ingest_own(ot.data_ptr(), st)
     recs, cands = [], []
     rng = np.random.default_rng(7)
     for r in range(10):
@@ -254,15 +155,15 @@ def test_received_batch_equals_single_calls(gpu):
                            few_flags_dir=(r % 4) if r in (1, 6) else None))
         cands.append(dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], init_mode=(r == 2),
                           odom_rel=rng.normal(size=7), cov=COV))
-    rt = dv.up(recs)
-    res_t = dv.buf(10 * RS)
-    fe.query_received(rt.data_ptr(), 10, -1, res_t.data_ptr(), dv.st, init_mode=[c["init_mode"] for c in cands])
-    fe.finish(dv.st)
-    results = dv.results(res_t, 10)
-    batch = run_loop(fe, dv, rt.data_ptr(), res_t.data_ptr(), cands)
+    rt = upload(recs)
+    res_t = filled(10 * RS)
+    fe.query_received(rt.data_ptr(), 10, -1, res_t.data_ptr(), st, init_mode=[c["init_mode"] for c in cands])
+    fe.finish(st)
+    results = fh.results(res_t, 10)
+    batch = run_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), cands)
     statuses = []
     for r in range(10):
-        single = run_loop(fe, dv, rt.data_ptr() + r * RB, res_t.data_ptr() + r * RS, [cands[r]])[0]
+        single = run_loop(fe, st, rt.data_ptr() + r * RB, res_t.data_ptr() + r * RS, [cands[r]])[0]
         assert single == batch[r], f"candidate {r}: batch and single call differ"
         e = check(batch[r], oracle(results[r], recs[r], old, cands[r]))
         statuses.append(e.status)
@@ -274,30 +175,30 @@ def test_received_batch_equals_single_calls(gpu):
 
 def test_depth_keyframe_camera(gpu):
     """a depth-camera handle lifts the old frame through set_depth_camera's pinhole and extrinsics"""
-    dv = Dev()
+    st = fh.stream()
     K2 = np.array([80.0, 80.0, 40.0, 30.0])
     fe = make_frontend(cameras=None, loop_params=False)
     fe.set_depth_camera(K2, SC["ext"])
     fe.set_loop_params(**PARAMS)
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=3, g=noisy_g(3))
-    rt, res_t, res = own_query(fe, dv, old, new)
+    rt, res_t, res = own_query(fe, st, old, new)
     cand = cand_own()
-    raw = run_loop(fe, dv, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
+    raw = run_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), [cand])[0]
     check(raw, oracle(res, new, old, cand, K=K2), truth=False)      # the pixels were made for another camera
     fe.close()
 
 
 def test_every_status_code(gpu):
-    dv = Dev()
+    st = fh.stream()
     fe = make_frontend()
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=4, g=noisy_g(4))
-    rt, res_t, res = own_query(fe, dv, old, new)
+    rt, res_t, res = own_query(fe, st, old, new)
     seen = {}
     by_msg = {100: old, 101: new}
 
     def go(params, cand, rec=new, rt_=rt, res_t_=res_t, res_=res):
         fe.set_loop_params(**dict(PARAMS, **params))
-        raw = run_loop(fe, dv, rt_.data_ptr(), res_t_.data_ptr(), [cand])[0]
+        raw = run_loop(fe, st, rt_.data_ptr(), res_t_.data_ptr(), [cand])[0]
         e = check(raw, oracle(res_, rec, by_msg.get(res_.hit_msg_id), cand, params))
         seen[e.status] = seen.get(e.status, 0) + 1
         return e
@@ -313,11 +214,11 @@ def test_every_status_code(gpu):
     far = np.concatenate([SC["delta_true"][:3] + 1.0, SC["delta_true"][3:]])
     assert go(dict(), cand_own(odom=far)).status == lib.LOOP_ODOMETRY_INCONSISTENT
     bad = record(1, 102, "new", seed=5, g=noisy_g(5), scramble=True)
-    bt, bres_t, bres = own_query(fe, dv, None, bad, ingest_old=False)
+    bt, bres_t, bres = own_query(fe, st, None, bad, ingest_old=False)
     assert bres.accepted
     assert go(dict(reproj_thresh=1e-4), cand_own(), bad, bt, bres_t, bres).status == lib.LOOP_PNP_FAILED
     miss = record(1, 103, "new", seed=6, g=synth.descriptor_db(ND, 4096, 77))
-    mt, mres_t, mres = own_query(fe, dv, None, miss, ingest_old=False)
+    mt, mres_t, mres = own_query(fe, st, None, miss, ingest_old=False)
     assert go({}, cand_own(), miss, mt, mres_t, mres).status == lib.LOOP_NO_HIT
     fe.close()
     # a row put in with db_load has no keyframe behind it
@@ -325,9 +226,9 @@ def test_every_status_code(gpu):
     q = record(1, 101, "new", seed=4, g=noisy_g(4))
     fe.db_load(np.stack([np.ctypeslib.as_array(q.global_desc[QDIR])]), synth.local_descriptors(MN, 3)[None],
                np.array([NPT], np.int32))
-    rt2, res_t2, res2 = own_query(fe, dv, old, q)
+    rt2, res_t2, res2 = own_query(fe, st, old, q)
     assert res2.accepted and res2.hit_msg_id == -1
-    raw = run_loop(fe, dv, rt2.data_ptr(), res_t2.data_ptr(), [cand_own()])[0]
+    raw = run_loop(fe, st, rt2.data_ptr(), res_t2.data_ptr(), [cand_own()])[0]
     e = lib.LoopEdgeResult.from_buffer_copy(raw)
     assert e.status == lib.LOOP_NO_FRAME and e.n_corr == 0 and e.pnp.pnp_success == 0
     seen[e.status] = 1
@@ -336,13 +237,13 @@ def test_every_status_code(gpu):
 
 
 def test_arguments_errors_and_resources(gpu):
-    dv = Dev()
+    st = fh.stream()
     base = host.live_resources()
     fe = make_frontend()
     L = fe._lib
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=1, g=noisy_g(1))
-    rt, res_t, res = own_query(fe, dv, old, new)
-    out = dv.buf(65 * EB)
+    rt, res_t, res = own_query(fe, st, old, new)
+    out = filled(65 * EB)
     cands = host.KeyframeFrontend.loop_candidates([cand_own()] * 65)
     c0, live0 = host.launch_count(), host.live_resources()
     for args in ((fe._h, rt.data_ptr(), res_t.data_ptr(), 0, cands, out.data_ptr()),
@@ -354,17 +255,17 @@ def test_arguments_errors_and_resources(gpu):
                  (None, rt.data_ptr(), res_t.data_ptr(), 1, cands, out.data_ptr())):
         h, r, q, n, cd, o = args
         vp = lambda x: None if x is None else C.c_void_p(x)
-        assert L.osb_frontend_compute_loop(h, vp(r), vp(q), n, cd, vp(o), C.c_void_p(dv.st)) == lib.ERR_INVALID
+        assert L.osb_frontend_compute_loop(h, vp(r), vp(q), n, cd, vp(o), C.c_void_p(st)) == lib.ERR_INVALID
     assert L.osb_frontend_set_loop_params(fe._h, None) == lib.ERR_INVALID
     assert host.launch_count() == c0 and host.live_resources() == live0
-    run_loop(fe, dv, rt.data_ptr(), res_t.data_ptr(), [cand_own()])
+    run_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), [cand_own()])
     live1 = host.live_resources()
     assert live1 > live0                                    # the first call acquired the scratch
-    rt64 = dv.up([new] * 64)                                # n candidates read n records and n results
-    res64 = dv.torch.frombuffer(bytearray(bytes(res) * 64), dtype=dv.torch.uint8).cuda()
+    rt64 = upload([new] * 64)                                # n candidates read n records and n results
+    res64 = upload([res] * 64)
     for n in (1, 8, 64):
         c = host.launch_count()
-        fe.compute_loop(rt64.data_ptr(), res64.data_ptr(), [cand_own()] * n, out.data_ptr(), dv.st)
+        fe.compute_loop(rt64.data_ptr(), res64.data_ptr(), [cand_own()] * n, out.data_ptr(), st)
         assert host.launch_count() - c == 3
     assert host.live_resources() == live1
     fe.close()
@@ -375,20 +276,20 @@ def test_arguments_errors_and_resources(gpu):
         assert ei.value.status == lib.ERR_INVALID
         fe.close()
 
-    call = lambda fe: lambda: fe.compute_loop(rt.data_ptr(), res_t.data_ptr(), [cand_own()], out.data_ptr(), dv.st)
+    call = lambda fe: lambda: fe.compute_loop(rt.data_ptr(), res_t.data_ptr(), [cand_own()], out.data_ptr(), st)
     f = make_frontend(loop_params=False); refused(f, call(f))                  # no loop parameters
     f = make_frontend(cameras=None); refused(f, call(f))                       # no camera
     f = make_frontend(cameras="both"); refused(f, call(f))                     # two cameras
     f = make_frontend(geometric_filter=False); refused(f, call(f))             # the reference's USE_FUNDMENTAL path only
     f = make_frontend(loop_params=False)                                       # after a remote ingest: no 3-D plane
-    t = dv.up([record(2, 200, "new")])
-    f.ingest(t.data_ptr(), 1, -1, dv.st)
+    t = upload([record(2, 200, "new")])
+    f.ingest(t.data_ptr(), 1, -1, st)
     refused(f, lambda: f.set_loop_params())
     # without set_loop_params nothing is allocated
     f = make_frontend(loop_params=False)
     live = host.live_resources()
-    f.ingest(t.data_ptr(), 1, -1, dv.st)
-    f.finish(dv.st)
+    f.ingest(t.data_ptr(), 1, -1, st)
+    f.finish(st)
     assert host.live_resources() == live
     f.close()
     assert host.live_resources() == base
