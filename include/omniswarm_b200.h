@@ -436,6 +436,101 @@ osb_status osb_pcm_state_pair(osb_pcm_state* s, int32_t id_a, int32_t id_b, int3
                               int32_t* clique, int32_t* clique_size);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Re-anchoring of loops and detections onto the sliding window (SURVEY.md 8f-4) -- replaces the walk of
+ *   SwarmLocalizationSolver::find_available_loops_detections (swarm_localization_solver.cpp:1594-1666) over every
+ *   measurement ever received: loop_from_src_loop_connection (:1464-1553), find_node_frame_for_measurement_2drones
+ *   (:1429-1462), and the factor choice of setup_problem_with_loops_and_detections (:1064-1100).  One launch per run.
+ * The handle keeps ego_motion_trajs (push_odometry), all_loops / all_detections_6d (add_measurements) and sf_sld_win
+ *   (set_window) on the device.  Stamps are int64 nanoseconds, so every comparison is exact.  DroneTrajectory, NodeFrame and
+ *   LoopEdge come from swarm_msgs, which is not in the reference tree; their arithmetic is defined in oracle/anchor_ref.py:
+ *   a trajectory's length[k] is the sequential fp64 sum of |p_j - p_(j-1)| for j <= k; a look-up at stamp t uses the nearest
+ *   sample (ties to the earlier, clamped at both ends); the odometry covariance between two stamps is
+ *   |length(t2) - length(t1)| * diag(odom_pos_cov_per_m x3, odom_ang_cov_per_m x3).
+ * run(): for measurement i (all loops in order, then all detections in order) out[i] holds, as :1464-1553:
+ *   status: OSB_ANCHOR_EMPTY_WINDOW (no frame), OSB_ANCHOR_BEFORE_WINDOW (frame 0's stamp - stamp_a > begin_min_loop_dt_s,
+ *     strictly; stamp_b is not tested), OSB_ANCHOR_NO_FRAME (drone a or b has no vo_available entry in the window closer than
+ *     10000 s, strictly), OSB_ANCHOR_NO_TRAJECTORY (drone a or b has no odometry), OSB_ANCHOR_DPOS (dpos > det_dpos_thres),
+ *     else OSB_ANCHOR_OK -- tested in this order;
+ *   frame_a/b, node_a/b, stamp_a/b: the anchor of each side (the entry of the drone with the smallest |stamp difference|,
+ *     the earliest frame on ties), its caller pose-block id and stamp; -1 / -1 / 0 when not found;
+ *   dt_err_ns: the two stamp differences summed, 10000 s for a side not found (0 when no search ran: EMPTY_WINDOW,
+ *     BEFORE_WINDOW);
+ *   dpos and edge (for OK and DPOS): dpos = |len(stamp_a) - len(anchor a)| + the same for b; edge.rel_pose =
+ *     DeltaPose(anchor_a.self_pose, self_pose_a, 4-DoF) * relative_pose * DeltaPose(self_pose_b, anchor_b.self_pose, 4-DoF),
+ *     where detections take self_pose_a/b from the trajectories at their stamps (DET4D: yaw only); edge.cov = cov + the
+ *     odometry covariance of both sides; edge.odom_a/b = the anchors' self poses, edge.len_a/b = the lengths at their stamps:
+ *     the edge osb_pcm_state_reject takes;
+ *   skip = 1 unless status is OK, both drones are yaw-observable and node_a != node_b;
+ *   the solver row (factor_type OSB_FACTOR_RELPOSE, ia = node_a, ib = node_b, huber, payload [x y z yaw, S 4x4]) with
+ *     S_ij = sqrt|(cov4^-1)_ij|, cov4 = blkdiag(edge.cov[0:3,0:3], edge.cov[5,5]) (RelativePoseFactor4d::CreateCov6d).
+ *   run_dev writes out_dev[*n_out] on `stream` without synchronising; run copies to the host and synchronises.
+ *   yaw_observable [max_drones] is read during the call.  Every run is one kernel launch (none when there is no measurement).
+ * Errors: a drone id outside 0..max_drones-1, a null pointer, a stamp not after the drone's last one, an unknown type, a
+ *   drone twice in one frame or a malformed frame_first give OSB_ERR_INVALID; exceeding a capacity gives OSB_ERR_CAPACITY.
+ *   Either way the handle is unchanged.  Updates wait for the handle's last run on any stream before they overwrite state.
+ * Memory: create acquires everything (a stream, an event, the trajectories, measurements, window and run output at their
+ *   capacities); nothing is acquired later. */
+#define OSB_MEAS_LOOP 0
+#define OSB_MEAS_DET4D 1
+#define OSB_MEAS_DET6D 2
+#define OSB_ANCHOR_OK 0
+#define OSB_ANCHOR_EMPTY_WINDOW 1
+#define OSB_ANCHOR_BEFORE_WINDOW 2
+#define OSB_ANCHOR_NO_FRAME 3
+#define OSB_ANCHOR_NO_TRAJECTORY 4
+#define OSB_ANCHOR_DPOS 5
+typedef struct {
+  int32_t max_drones;            /* drone ids 0 .. max_drones-1; 1..256 */
+  int32_t max_traj_samples;      /* odometry samples per drone */
+  int32_t max_measurements;      /* loops + detections */
+  int32_t max_window_entries;    /* node frames in the window */
+  double begin_min_loop_dt_s;    /* BEGIN_MIN_LOOP_DT = 1000 (solver.cpp:56) */
+  double det_dpos_thres;
+  double odom_pos_cov_per_m, odom_ang_cov_per_m;
+  int32_t huber;                 /* 1 = HuberLoss(1.0) on every row (0 = debug_no_rejection) */
+  int32_t reserved;
+} osb_anchor_params;
+typedef struct {                 /* a Swarm::LoopEdge (LOOP) or DroneDetection (DET4D / DET6D) */
+  int64_t id;
+  int32_t type, id_a, id_b, reserved;
+  int64_t stamp_a, stamp_b;      /* ns */
+  double relative_pose[7];       /* x y z, qw qx qy qz */
+  double cov[36];                /* 6x6 row-major, translation block first */
+  double self_pose_a[7], self_pose_b[7];
+} osb_measurement;
+typedef struct {                 /* a NodeFrame of the window */
+  int32_t drone_id, vo_available;
+  int32_t block;                 /* the caller's pose-block id (est_poses_idts[id][ts]); shared blocks share an id */
+  int32_t reserved;
+  int64_t stamp;                 /* ns */
+  double self_pose[7];
+} osb_window_entry;
+typedef struct {
+  int64_t id;
+  int32_t type, status;
+  int32_t frame_a, frame_b, node_a, node_b;
+  int64_t stamp_a, stamp_b, dt_err_ns;
+  double dpos;
+  osb_loop_edge edge;
+  int32_t skip, factor_type, ia, ib, huber, reserved;
+  double payload[OSB_PAYLOAD_LEN];
+} osb_anchor_result;
+typedef struct osb_anchor osb_anchor;
+osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_params* p);
+osb_status osb_anchor_destroy(osb_anchor* h);
+/* appends n samples (stamps strictly increasing, also against the drone's last sample); poses [n][7] */
+osb_status osb_anchor_push_odometry(osb_anchor* h, int32_t drone, int n, const int64_t* stamps_ns, const double* poses);
+osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const osb_measurement* m);
+/* n_loops and n_detections held (run() writes n_loops + n_detections results) */
+osb_status osb_anchor_size(osb_anchor* h, int32_t* n_loops, int32_t* n_detections);
+/* replaces the window: frame f holds entries [frame_first[f], frame_first[f+1]) and was taken at frame_stamps_ns[f] */
+osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const int64_t* frame_stamps_ns, const int32_t* frame_first,
+                                 const osb_window_entry* entries);
+osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out, int32_t* n_out);
+osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
+                              void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Geometric filter of the loop matcher (SURVEY.md 8f-1, first half) -- the inlier mask of
  *   cv::findHomography(old_2d, new_2d, CV_RANSAC, 3, mask)            swarm_loop/src/loop_detector.cpp:589-598
  * for n_pairs correspondence sets at once.  src = old_2d, dst = new_2d, [n_pairs][max_n][2] floats, n[pair] points each

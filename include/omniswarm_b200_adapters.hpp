@@ -6,6 +6,7 @@
 //   faiss::IndexFlatIP     (swarm_loop/include/swarm_loop/loop_detector.h:27-29)          -> osb::IndexFlatIPB200
 //   cv::BFMatcher          (swarm_loop/src/loop_cam.cpp:147-150, loop_detector.cpp:564)   -> osb::BFMatcherB200
 //   ceres::Solve in solve_once (swarm_localization/src/swarm_localization_solver.cpp:1695-1712) -> osb::FlatPoseGraph
+//   find_available_loops_detections (swarm_localization_solver.cpp:1594-1666)    -> osb_anchor_* + add_anchored_factors
 //
 // The cv::Mat / cv::Point2f / cv::DMatch overloads are compiled when OSB_WITH_OPENCV is defined (the reference build
 // has OpenCV; this repository's container does not, so tests/cpp/adapter_smoke.cpp exercises the raw-pointer forms).
@@ -253,6 +254,22 @@ class FlatPoseGraph {
   std::vector<int32_t> type_, ia_, ib_;
   std::vector<double> payload_;
 };
+
+// find_available_loops_detections + setup_problem_with_loops_and_detections (swarm_localization_solver.cpp:1594-1666,
+// 1064-1100) on the device: the rows of osb_anchor_run with skip == 0 (and keep[i], e.g. osb_pcm_state_reject's mask over
+// the same rows) become RelativePoseFactor4d blocks of `graph`; blocks[id] is the double[4] of the pose-block id the
+// window entries carry.  Returns the number of factors added.
+inline int add_anchored_factors(FlatPoseGraph& graph, const osb_anchor_result* rows, int n, double* const* blocks,
+                                const uint8_t* keep = nullptr) {
+  int added = 0;
+  for (int i = 0; i < n; ++i) {
+    const osb_anchor_result& r = rows[i];
+    if (r.skip || (keep && !keep[i])) continue;
+    graph.add_relative_pose(blocks[r.ia], blocks[r.ib], r.payload, r.payload + 4, r.huber != 0);
+    ++added;
+  }
+  return added;
+}
 
 // Same interface, but the window lives in the solver between solves (osb_solver_graph_*, SURVEY.md 8f-4): after a solve
 // only the pose blocks and factors added since (add_new_swarm_frame / add_new_loop_connection,

@@ -92,5 +92,32 @@ __device__ __forceinline__ void quat2eulers(const double* q, double (&e)[3]) {
   e[1] = asin(fmin(1.0, fmax(-1.0, 2.0 * (w * y - z * x))));
   e[2] = atan2(2.0 * (w * z + x * y), 1.0 - 2.0 * (y * y + z * z));
 }
+__device__ __forceinline__ double quat_yaw(const double* q) {
+  return atan2(2.0 * (q[0] * q[3] + q[1] * q[2]), 1.0 - 2.0 * (q[2] * q[2] + q[3] * q[3]));
+}
+__device__ __forceinline__ double wrap_angle(double a) {
+  const double pi = 3.141592653589793;
+  return a - 2.0 * pi * floor((a + pi) / (2.0 * pi));
+}
+// Pose::set_yaw_only: position and yaw kept, roll and pitch zero
+__device__ __forceinline__ PoseD pose_yaw_only(const PoseD& p) {
+  PoseD o = p;
+  const double rv[3] = {0.0, 0.0, quat_yaw(p.q)};
+  quat_from_rotvec(rv, o.q);
+  return o;
+}
+// Pose::DeltaPose(a, b, true): the 4-DoF a^-1 b (swarm_localization_factors.hpp:139-149), as oracle/pnp_ref.delta_pose
+__device__ __forceinline__ PoseD delta_pose4(const PoseD& a, const PoseD& b) {
+  const double ya = quat_yaw(a.q), yb = quat_yaw(b.q);
+  const double d0 = b.t[0] - a.t[0], d1 = b.t[1] - a.t[1], d2 = b.t[2] - a.t[2];
+  const double c = cos(ya), s = sin(ya);
+  PoseD o;
+  o.t[0] = c * d0 + s * d1;
+  o.t[1] = -s * d0 + c * d1;
+  o.t[2] = d2;
+  const double rv[3] = {0.0, 0.0, wrap_angle(yb - ya)};
+  quat_from_rotvec(rv, o.q);
+  return o;
+}
 
 }  // namespace osb

@@ -7,6 +7,7 @@ Names, argument meaning and error behaviour follow the reference (paths relative
   BFMatcher         <- cv::BFMatcher(NORM_L2, true)  swarm_loop/src/loop_cam.cpp:147-150
   PoseGraphSolver   <- SwarmLocalizationSolver::solve_once  swarm_localization/src/swarm_localization_solver.cpp:1668
   KeyframeFrontend  <- LoopCam::on_flattened_images + LoopDetector::on_image_recv database work
+  LoopAnchor        <- SwarmLocalizationSolver::find_available_loops_detections  swarm_localization_solver.cpp:1594-1666
 All compute happens in libomniswarm_b200.so; these classes only marshal numpy arrays.
 """
 from __future__ import annotations
@@ -729,6 +730,90 @@ class PcmState(_Handle):
         _l.check(self._lib.osb_pcm_state_pair(self._h, a, b, C.byref(n), _l.ptr(ids), _l.ptr(adj), _l.ptr(clique),
                                               C.byref(size)))
         return ids, adj, clique[:size.value].copy()
+
+
+class LoopAnchor(_Handle):
+    """The re-anchoring walk of SwarmLocalizationSolver::find_available_loops_detections (swarm_localization_solver.cpp:
+    1594-1666, 1429-1553) with ego_motion_trajs, all_loops / all_detections_6d and sf_sld_win resident on the device
+    (osb_anchor_*).  Records are numpy structured arrays of lib.MEASUREMENT_DTYPE / WINDOW_ENTRY_DTYPE; `run` returns one
+    lib.ANCHOR_RESULT_DTYPE row per measurement, loops first, each in arrival order."""
+
+    _destroy = "osb_anchor_destroy"
+
+    def __init__(self, max_drones: int, max_traj_samples: int, max_measurements: int, max_window_entries: int,
+                 det_dpos_thres: float, odom_pos_cov_per_m: float, odom_ang_cov_per_m: float,
+                 begin_min_loop_dt_s: float = 1000.0, huber: bool = True):
+        self._lib = _l.load()
+        self._h = C.c_void_p()
+        self.max_drones = int(max_drones)
+        p = _l.AnchorParams(self.max_drones, int(max_traj_samples), int(max_measurements), int(max_window_entries),
+                            float(begin_min_loop_dt_s), float(det_dpos_thres), float(odom_pos_cov_per_m),
+                            float(odom_ang_cov_per_m), int(bool(huber)), 0)
+        _l.check(self._lib.osb_anchor_create(C.byref(self._h), C.byref(p)))
+
+    def push_odometry(self, drone: int, stamps_ns, poses):
+        """appends samples: stamps int64 ns, strictly increasing; poses [n,7] (x y z, qw qx qy qz)"""
+        stamps = np.ascontiguousarray(stamps_ns, np.int64)
+        poses = np.ascontiguousarray(poses, np.float64).reshape(len(stamps), 7)
+        _l.check(self._lib.osb_anchor_push_odometry(self._h, int(drone), len(stamps), _l.ptr(stamps), _l.ptr(poses)))
+
+    def add_measurements(self, meas):
+        meas = np.ascontiguousarray(meas, _l.MEASUREMENT_DTYPE)
+        _l.check(self._lib.osb_anchor_add_measurements(self._h, len(meas), _l.ptr(meas)))
+
+    def size(self) -> tuple[int, int]:
+        """-> (loops, detections) held"""
+        a, b = C.c_int32(0), C.c_int32(0)
+        _l.check(self._lib.osb_anchor_size(self._h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def set_window(self, frame_stamps_ns, frame_first, entries):
+        """frame f: entries[frame_first[f]:frame_first[f+1]], taken at frame_stamps_ns[f]"""
+        stamps = np.ascontiguousarray(frame_stamps_ns, np.int64)
+        first = np.ascontiguousarray(frame_first, np.int32)
+        entries = np.ascontiguousarray(entries, _l.WINDOW_ENTRY_DTYPE)
+        assert len(first) == len(stamps) + 1
+        _l.check(self._lib.osb_anchor_set_window(self._h, len(stamps), _l.ptr(stamps), _l.ptr(first),
+                                                 _l.ptr(entries) if len(entries) else None))
+
+    def _yaw(self, yaw_observable):
+        y = np.zeros(self.max_drones, np.uint8)
+        if yaw_observable is None:
+            y[:] = 1
+        else:
+            y[:] = np.asarray(yaw_observable, bool)
+        return y
+
+    def run(self, yaw_observable=None) -> np.ndarray:
+        """yaw_observable [max_drones] (None: every drone) -> results [n] of lib.ANCHOR_RESULT_DTYPE"""
+        y = self._yaw(yaw_observable)
+        out = np.zeros(sum(self.size()), _l.ANCHOR_RESULT_DTYPE)
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_anchor_run(self._h, _l.ptr(y), _l.ptr(out) if len(out) else None, C.byref(n)))
+        return out[:n.value]
+
+    def run_dev(self, out_ptr: int, stream: int, yaw_observable=None) -> int:
+        """writes the results to device memory at out_ptr on `stream` without synchronising -> their count"""
+        y = self._yaw(yaw_observable)
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_anchor_run_dev(self._h, _l.ptr(y), C.c_void_p(out_ptr), C.byref(n), C.c_void_p(stream)))
+        return n.value
+
+
+def anchored_factor_rows(res: np.ndarray, keep=None):
+    """the solver rows of the results with skip == 0 (and keep[i], e.g. the PCM keep mask) -> (ftype, ia, ib, payload,
+    huber), the arrays osb_solver_solve takes"""
+    sel = res["skip"] == 0
+    if keep is not None:
+        sel &= np.asarray(keep, bool)
+    r = res[sel]
+    return (r["factor_type"].astype(np.int32), r["ia"].astype(np.int32), r["ib"].astype(np.int32),
+            np.ascontiguousarray(r["payload"]), r["huber"].astype(np.uint8))
+
+
+def anchored_loop_edges(res: np.ndarray) -> np.ndarray:
+    """the re-anchored edges as the packed [n, 60] array PcmState.reject takes"""
+    return np.ascontiguousarray(res["edge"]).view(np.float64).reshape(len(res), 60)
 
 
 class Swarm(_Handle):

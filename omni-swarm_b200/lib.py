@@ -9,6 +9,8 @@ import ctypes as C
 import os
 import subprocess
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libomniswarm_b200.so")
@@ -75,6 +77,30 @@ class LoopEdge(C.Structure):
 class PcmStateParams(C.Structure):
     _fields_ = [("self_id", C.c_int32), ("redundant", C.c_int32), ("max_pairs", C.c_int32), ("pair_capacity", C.c_int32),
                 ("pcm_thres", C.c_double), ("odom_pos_cov_per_m", C.c_double), ("odom_ang_cov_per_m", C.c_double)]
+
+
+class AnchorParams(C.Structure):
+    _fields_ = [("max_drones", C.c_int32), ("max_traj_samples", C.c_int32), ("max_measurements", C.c_int32),
+                ("max_window_entries", C.c_int32), ("begin_min_loop_dt_s", C.c_double), ("det_dpos_thres", C.c_double),
+                ("odom_pos_cov_per_m", C.c_double), ("odom_ang_cov_per_m", C.c_double), ("huber", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+MEAS_LOOP, MEAS_DET4D, MEAS_DET6D = 0, 1, 2
+# numpy views of osb_measurement, osb_window_entry, osb_loop_edge and osb_anchor_result (include/omniswarm_b200.h)
+MEASUREMENT_DTYPE = np.dtype([("id", "<i8"), ("type", "<i4"), ("id_a", "<i4"), ("id_b", "<i4"), ("reserved", "<i4"),
+                              ("stamp_a", "<i8"), ("stamp_b", "<i8"), ("relative_pose", "<f8", 7), ("cov", "<f8", (6, 6)),
+                              ("self_pose_a", "<f8", 7), ("self_pose_b", "<f8", 7)])
+WINDOW_ENTRY_DTYPE = np.dtype([("drone_id", "<i4"), ("vo_available", "<i4"), ("block", "<i4"), ("reserved", "<i4"),
+                               ("stamp", "<i8"), ("self_pose", "<f8", 7)])
+LOOP_EDGE_DTYPE = np.dtype([("id_a", "<i4"), ("id_b", "<i4"), ("rel_pose", "<f8", 7), ("cov", "<f8", (6, 6)),
+                            ("odom_a", "<f8", 7), ("odom_b", "<f8", 7), ("len_a", "<f8"), ("len_b", "<f8")])
+ANCHOR_RESULT_DTYPE = np.dtype([("id", "<i8"), ("type", "<i4"), ("status", "<i4"), ("frame_a", "<i4"), ("frame_b", "<i4"),
+                                ("node_a", "<i4"), ("node_b", "<i4"), ("stamp_a", "<i8"), ("stamp_b", "<i8"),
+                                ("dt_err_ns", "<i8"), ("dpos", "<f8"), ("edge", LOOP_EDGE_DTYPE), ("skip", "<i4"),
+                                ("factor_type", "<i4"), ("ia", "<i4"), ("ib", "<i4"), ("huber", "<i4"), ("reserved", "<i4"),
+                                ("payload", "<f8", PAYLOAD_LEN)])
+ANCHOR_OK, ANCHOR_EMPTY_WINDOW, ANCHOR_BEFORE_WINDOW, ANCHOR_NO_FRAME, ANCHOR_NO_TRAJECTORY, ANCHOR_DPOS = range(6)
 
 
 class PnpParams(C.Structure):
@@ -249,6 +275,14 @@ _SIG = {
     "osb_pcm_state_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int, C.POINTER(C.c_int32)]),
     "osb_pcm_state_set_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int]),
     "osb_pcm_state_pair": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, C.POINTER(C.c_int32)]),
+    "osb_anchor_create": (C.c_int, [C.POINTER(_P), C.POINTER(AnchorParams)]),
+    "osb_anchor_destroy": (C.c_int, [_P]),
+    "osb_anchor_push_odometry": (C.c_int, [_P, C.c_int32, C.c_int, _P, _P]),
+    "osb_anchor_add_measurements": (C.c_int, [_P, C.c_int, _P]),
+    "osb_anchor_size": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "osb_anchor_set_window": (C.c_int, [_P, C.c_int, _P, _P, _P]),
+    "osb_anchor_run": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32)]),
+    "osb_anchor_run_dev": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32), _P]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),

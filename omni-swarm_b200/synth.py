@@ -691,3 +691,84 @@ def loop_record(drone: int, msg: int, side: str, seed: int = 0, g: np.ndarray | 
         np.ctypeslib.as_array(r.landmarks_flag[d])[:n] = flag
         np.ctypeslib.as_array(r.stereo_match[d])[:n] = np.where(flag > 0, 0, -1)
     return r
+
+
+def anchor_swarm(n_drones: int = 5, n_frames: int = 60, n_meas: int = 400, seed: int = 0, kf_dt_s: float = 0.5,
+                 hz: float = 100.0, pre_s: float = 20.0, frac_old: float = 0.05, frac_far: float = 0.1,
+                 with_orphans: bool = True):
+    """A swarm as find_available_loops_detections sees it before a solve (inputs of host.LoopAnchor and of
+    oracle/anchor_ref.anchor).  Drones 0..n_drones-1 fly smooth 3-D curves with yaw and small roll/pitch; each drone's
+    odometry (100 Hz, int64 ns stamps from a realistic epoch) is its ground truth in a per-drone odometry frame.  The window
+    holds n_frames keyframes kf_dt_s apart: each drone appears with its own stamp jitter, 5 % of its entries are missing,
+    5 % have vo_available = 0, and 10 % reuse the previous frame's pose block (a keyframe that did not move).  Measurements
+    (loops, Detection4d, Detection6d; loops may be intra-drone) carry noisy true relative poses and correlated covariances at
+    off-keyframe stamps, mostly inside the window, `frac_far` of them up to 3 s outside it (dpos rejections) and `frac_old`
+    more than 1000 s before it.  With `with_orphans`, drone n_drones has window entries but no odometry and drone
+    n_drones + 1 has odometry but no window entry.
+    -> dict(trajs {drone: (stamps, poses)}, window (frame_stamps, frame_first, entries), meas, max_drones, prm)"""
+    from . import lib as _lib
+    rng = np.random.default_rng(seed + 9100)
+    NS = 1_000_000_000
+    t_epoch = 1_700_000_000 * NS
+    pa = _PoseAlgebra
+    span = n_frames * kf_dt_s
+
+    def gt(d, t):
+        ph = 0.12 * t + 0.9 * d
+        pos = np.array([5.0 * np.sin(ph) + 2.0 * d, 5.0 * (1 - np.cos(ph)) - 1.5 * d, 1.0 + 0.5 * np.sin(0.3 * t + d)])
+        q = _quat_from_rotvec(np.array([0.04 * np.sin(0.7 * t), 0.03 * np.cos(0.5 * t), 0.3 * t + d]))
+        return np.concatenate([pos, q])
+
+    odom_frame = {d: np.concatenate([rng.uniform(-3, 3, 3), _quat_from_rotvec(np.array([0, 0, rng.uniform(-3, 3)]))])
+                  for d in range(n_drones + 2)}
+
+    def odom(d, t):
+        return pa.pose_mul(odom_frame[d], gt(d, t))
+
+    flying = list(range(n_drones)) + ([n_drones + 1] if with_orphans else [])
+    in_window = list(range(n_drones)) + ([n_drones] if with_orphans else [])
+    n_samples = int((pre_s + span + 4.0) * hz)
+    trajs = {}
+    for d in flying:
+        k = np.arange(n_samples)
+        stamps = t_epoch + (k * (NS / hz)).astype(np.int64) + d * 1000
+        trajs[d] = (stamps, np.stack([odom(d, (s - t_epoch) / NS) for s in stamps]))
+    t_win = pre_s
+    frame_stamps = t_epoch + ((t_win + kf_dt_s * np.arange(n_frames)) * NS).astype(np.int64)
+    entries, first, last_block, block = [], [0], {}, 0
+    for f in range(n_frames):
+        for d in in_window:
+            if f > 0 and rng.uniform() < 0.05:
+                continue
+            st = int(frame_stamps[f]) + int(rng.integers(-3_000_000, 3_000_000))
+            if d in last_block and rng.uniform() < 0.1:
+                b = last_block[d]
+            else:
+                b, block = block, block + 1
+            last_block[d] = b
+            entries.append((d, 0 if rng.uniform() < 0.05 else 1, b, 0, st, odom(d, (st - t_epoch) / NS)))
+        first.append(len(entries))
+    entries = np.array(entries, dtype=_lib.WINDOW_ENTRY_DTYPE)
+    meas = np.zeros(n_meas, _lib.MEASUREMENT_DTYPE)
+    ids = list(range(n_drones + (2 if with_orphans else 0)))
+    for i in range(n_meas):
+        typ = int(rng.integers(0, 3))
+        a = int(rng.choice(ids))
+        b = a if (typ == 0 and rng.uniform() < 0.2) else int(rng.choice([x for x in ids if x != a]))
+        u = rng.uniform()
+        if u < frac_old:
+            ta = t_win - 1000.0 - rng.uniform(0.001, 50.0)
+        elif u < frac_old + frac_far:
+            ta = t_win + (span + rng.uniform(0.5, 3.0) if rng.uniform() < 0.5 else -rng.uniform(0.5, 3.0))
+        else:
+            ta = t_win + rng.uniform(-0.2, span)
+        tb = ta if typ != 0 else t_win + rng.uniform(-0.2, span)
+        sa, sb = t_epoch + int(ta * NS), t_epoch + int(tb * NS)
+        rel = pa.pose_mul(pa.pose_inv(gt(a, ta)), gt(b, tb))
+        rel = pa.pose_mul(rel, np.concatenate([rng.normal(0, 0.02, 3), _quat_from_rotvec(rng.normal(0, 0.01, 3))]))
+        rel[3:] /= np.linalg.norm(rel[3:])
+        L = np.tril(rng.normal(0, 0.004, (6, 6)), -1) + np.diag(rng.uniform(0.02, 0.06, 6))
+        meas[i] = (i + (1 << 32), typ, a, b, 0, sa, sb, rel, L @ L.T, odom(a, ta), odom(b, tb))
+    prm = dict(begin_min_loop_dt_s=1000.0, det_dpos_thres=1.0, odom_pos_cov_per_m=1e-3, odom_ang_cov_per_m=2e-4, huber=True)
+    return dict(trajs=trajs, window=(frame_stamps, np.array(first, np.int32), entries), meas=meas,
+                max_drones=n_drones + 2, prm=prm)
