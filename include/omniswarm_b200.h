@@ -416,9 +416,10 @@ osb_status osb_pcm_dev(const osb_loop_edge* edges_dev, int n, double pcm_thres, 
  *   (The reference's handler inserts the indices 0..inlier_id_size-1, not msg->inlier_ids: the adapter decides what to pass.)
  * pair(): read-out for tests: the pair's loop count *n (0 for an unknown pair), its ids in insertion order [n], adjacency
  *   [n][n] (1 = consistent), its last clique in maxCliqueHeu order and its size; every output but n may be NULL.
- * Memory: create holds a stream, max_pairs x (48 + 480 pair_capacity) bytes of pinned and of device staging and
+ * Memory: create holds a stream, max_pairs x (64 + 488 pair_capacity) bytes of pinned and of device staging and
  *   max_pairs x (1 + pair_capacity) x 4 bytes of clique output on each side.  A pair's first loop acquires its slot,
- *   pair_capacity x (488 + 4 ceil(pair_capacity / 32)) bytes (4.1 MB at 4096), kept until destroy; nothing else is acquired. */
+ *   pair_capacity x (508 + 4 ceil(pair_capacity / 32)) bytes + 4 (4.2 MB at 4096), kept until destroy.  The device path
+ *   (osb_pcm_state_reject_anchored, after osb_anchor_run_dev below) acquires more on its first call only. */
 typedef struct {
   int32_t self_id;
   int32_t redundant;             /* SwarmLocalOutlierRejectionParams::redundant */
@@ -529,6 +530,45 @@ osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const int64_t* fra
 osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out, int32_t* n_out);
 osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
                               void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * The solve's chain from re-anchoring to factor rows on the device: run_dev -> reject_anchored -> compact_factors_dev, all
+ *   stream-ordered on one stream, then one copy of the count and of at most that many rows.
+ * osb_pcm_state_reject_anchored(): the PCM rejection of the rows osb_anchor_run_dev wrote, read in place.  Equals
+ *   osb_pcm_state_reject over (rows[i].edge, rows[i].id) for the rows with status == OSB_ANCHOR_OK, in row order, with every
+ *   rule of reject() above; keep_dev[i] = that call's keep for those rows and 0 for every other row.  n is run_dev's n_out.
+ *   Work: seven kernel launches whatever n and however many pairs change (none when n == 0): two passes over the rows find
+ *   the fresh ones (OK, routed, id not in the device's seen set) and compact their indices in row order; one warp plans the
+ *   appends (a pair's new loops keep row order, new pairs take slots in order of first appearance) and checks
+ *   pair_capacity and max_pairs before it writes anything; the consistency-graph growth and maxCliqueHeu run from that
+ *   device-built job list (one clique CTA per possible pair, exiting early when the pair did not change); the inlier sets
+ *   are replaced by the cliques' ids; keep_dev is each OK row's membership in its pair's set.  No host synchronisation and
+ *   no allocation after the first call, so the sequence can be captured into a CUDA graph.  Calls on one handle must be
+ *   ordered: on one stream, or joined by the caller.
+ *   Errors: null pointers or n < 0 return OSB_ERR_INVALID at once.  A call that would exceed pair_capacity or max_pairs is
+ *   refused on the device: the state is unchanged and keep_dev is not written; osb_pcm_state_status() then returns
+ *   OSB_ERR_CAPACITY, and so does (once) the next host-side call on the handle (reject, inliers, set_inliers, pair) instead
+ *   of running.
+ *   One state: the host-side calls and the anchored path may be mixed in any order.  The first anchored call builds the
+ *   device copy from the host record; host-side calls write their changes through to it before they return, and the first
+ *   host-side call after an anchored call synchronises once (on the anchored call's stream; when that call was captured,
+ *   the caller must have run and synchronised the graph) and refreshes the host record from the device.
+ *   Memory of the first call: the slots of all max_pairs pairs not yet acquired (max_pairs x slot size above, 63 MB for
+ *   15 pairs at 4096), a seen table of 8 x 2^ceil(log2(2 max_pairs pair_capacity)) bytes (>= 8 KB; 1 MB for 15 x 4096),
+ *   4 x 4 max_pairs pair_capacity bytes of row indices, an event and small tables.  set_inliers may acquire a buffer for a
+ *   set larger than pair_capacity or of a pair without loops.
+ * osb_pcm_state_status(): synchronises with the last anchored call and writes its status to *last (OSB_OK when none ran);
+ *   returns the same value. */
+osb_status osb_pcm_state_reject_anchored(osb_pcm_state* s, const osb_anchor_result* rows_dev, int n, uint8_t* keep_dev,
+                                         void* stream);
+osb_status osb_pcm_state_status(osb_pcm_state* s, osb_status* last);
+/* osb_anchor_compact_factors_dev(): the rows with skip == 0 && (keep_dev == NULL || keep_dev[i]), in row order, as the
+ *   solver's SoA -- type [k] (OSB_FACTOR_RELPOSE), ia / ib [k] (the rows' pose-block ids), payload [k][OSB_PAYLOAD_LEN],
+ *   huber [k] (0/1) -- exactly what osb::add_anchored_factors appends; *count_dev = k.  All pointers are device memory and
+ *   the outputs must hold n rows.  One launch (also for n == 0, which writes count 0), a block scan: deterministic. */
+osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int n, const uint8_t* keep_dev,
+                                          int32_t* type, int32_t* ia, int32_t* ib, double* payload, uint8_t* huber,
+                                          int32_t* count_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Geometric filter of the loop matcher (SURVEY.md 8f-1, first half) -- the inlier mask of

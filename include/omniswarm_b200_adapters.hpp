@@ -7,6 +7,7 @@
 //   cv::BFMatcher          (swarm_loop/src/loop_cam.cpp:147-150, loop_detector.cpp:564)   -> osb::BFMatcherB200
 //   ceres::Solve in solve_once (swarm_localization/src/swarm_localization_solver.cpp:1695-1712) -> osb::FlatPoseGraph
 //   find_available_loops_detections (swarm_localization_solver.cpp:1594-1666)    -> osb_anchor_* + add_anchored_factors
+//                                                                                   (or add_compacted_factors)
 //
 // The cv::Mat / cv::Point2f / cv::DMatch overloads are compiled when OSB_WITH_OPENCV is defined (the reference build
 // has OpenCV; this repository's container does not, so tests/cpp/adapter_smoke.cpp exercises the raw-pointer forms).
@@ -269,6 +270,17 @@ inline int add_anchored_factors(FlatPoseGraph& graph, const osb_anchor_result* r
     ++added;
   }
   return added;
+}
+
+// The same factors from osb_anchor_compact_factors_dev's SoA after its one copy to the host: count rows of type / ia / ib /
+// payload [count][OSB_PAYLOAD_LEN] / huber.  Returns the number of factors added (count).
+inline int add_compacted_factors(FlatPoseGraph& graph, int count, const int32_t* ia, const int32_t* ib, const double* payload,
+                                 const uint8_t* huber, double* const* blocks) {
+  for (int k = 0; k < count; ++k) {
+    const double* pl = payload + (size_t)k * OSB_PAYLOAD_LEN;
+    graph.add_relative_pose(blocks[ia[k]], blocks[ib[k]], pl, pl + 4, huber[k] != 0);
+  }
+  return count;
 }
 
 // Same interface, but the window lives in the solver between solves (osb_solver_graph_*, SURVEY.md 8f-4): after a solve

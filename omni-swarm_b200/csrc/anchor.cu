@@ -209,6 +209,65 @@ anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
   for (int j = lane; j < RESULT_WORDS; j += 32) dst[j] = s_out[w][j];
 }
 
+// setup_problem_with_loops_and_detections on the device: the rows with skip == 0 (and keep[i]) become the solver's SoA in
+// row order.  One CTA streams the rows in tiles of COMPACT_THREADS x COMPACT_ROWS; thread t owns COMPACT_ROWS consecutive
+// rows of a tile and a block scan of the per-thread counts gives each kept row its output index (no atomics, so the order
+// and the bytes are the same on every run).
+constexpr int COMPACT_THREADS = 1024, COMPACT_ROWS = 4;
+__global__ void __launch_bounds__(COMPACT_THREADS)
+anchor_compact_kernel(const osb_anchor_result* __restrict__ rows, int n, const uint8_t* __restrict__ keep,
+                      int32_t* __restrict__ type, int32_t* __restrict__ ia, int32_t* __restrict__ ib,
+                      double* __restrict__ payload, uint8_t* __restrict__ huber, int32_t* __restrict__ count) {
+  __shared__ int s_warp[COMPACT_THREADS / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int out_base = 0;
+  for (int base = 0; base < n; base += COMPACT_THREADS * COMPACT_ROWS) {
+    const int first = base + threadIdx.x * COMPACT_ROWS;
+    bool sel[COMPACT_ROWS];
+    int mine = 0;
+#pragma unroll
+    for (int r = 0; r < COMPACT_ROWS; ++r) {
+      const int i = first + r;
+      sel[r] = i < n && rows[i].skip == 0 && (keep == nullptr || keep[i] != 0);
+      mine += sel[r];
+    }
+    int inc = mine;                                                // warp-inclusive scan, then across warps
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += u;
+    }
+    if (lane == 31) s_warp[wid] = inc;
+    __syncthreads();
+    if (wid == 0) {
+      int t = s_warp[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, t, o);
+        if (lane >= o) t += u;
+      }
+      s_warp[lane] = t;
+    }
+    __syncthreads();
+    int k = out_base + (wid > 0 ? s_warp[wid - 1] : 0) + inc - mine;
+    const int total = s_warp[COMPACT_THREADS / 32 - 1];
+#pragma unroll
+    for (int r = 0; r < COMPACT_ROWS; ++r) {
+      if (!sel[r]) continue;
+      const osb_anchor_result& row = rows[first + r];
+      type[k] = row.factor_type;
+      ia[k] = row.ia;
+      ib[k] = row.ib;
+      huber[k] = (uint8_t)(row.huber != 0);
+      for (int j = 0; j < OSB_PAYLOAD_LEN; ++j) payload[(size_t)k * OSB_PAYLOAD_LEN + j] = row.payload[j];
+      ++k;
+    }
+    out_base += total;
+    __syncthreads();                                               // s_warp is rewritten by the next tile
+  }
+  if (threadIdx.x == 0) *count = out_base;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -505,6 +564,18 @@ extern "C" osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_obser
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   return anchor_launch(h, yaw_observable, out_dev, n_out, (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int n, const uint8_t* keep_dev,
+                                                     int32_t* type, int32_t* ia, int32_t* ib, double* payload,
+                                                     uint8_t* huber, int32_t* count_dev, void* stream) {
+  OSB_REQUIRE(n >= 0 && count_dev != nullptr, "negative count or null count");
+  OSB_REQUIRE(n == 0 || (rows_dev && type && ia && ib && payload && huber), "null argument");
+  OSB_TRY(require_device());
+  OSB_LAUNCH(anchor_compact_kernel, 1, COMPACT_THREADS, 0, (cudaStream_t)stream, rows_dev, n, keep_dev, type, ia, ib,
+             payload, huber, count_dev);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out, int32_t* n_out) {

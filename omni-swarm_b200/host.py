@@ -731,6 +731,20 @@ class PcmState(_Handle):
                                               C.byref(size)))
         return ids, adj, clique[:size.value].copy()
 
+    def reject_anchored(self, rows_ptr: int, n: int, keep_ptr: int, stream: int):
+        """reject() over the OK rows of osb_anchor_run_dev's output, read in place on the device: writes keep [n] uint8 at
+        keep_ptr on `stream` without synchronising (not written when the call is refused; see status())"""
+        _l.check(self._lib.osb_pcm_state_reject_anchored(self._h, C.c_void_p(rows_ptr), int(n), C.c_void_p(keep_ptr),
+                                                         C.c_void_p(stream)))
+
+    def status(self) -> int:
+        """synchronises with the last reject_anchored call -> its status (lib.OK or lib.ERR_CAPACITY)"""
+        last = C.c_int(0)
+        st = self._lib.osb_pcm_state_status(self._h, C.byref(last))
+        if st not in (_l.OK, last.value):
+            _l.check(st)
+        return last.value
+
 
 class LoopAnchor(_Handle):
     """The re-anchoring walk of SwarmLocalizationSolver::find_available_loops_detections (swarm_localization_solver.cpp:
@@ -809,6 +823,18 @@ def anchored_factor_rows(res: np.ndarray, keep=None):
     r = res[sel]
     return (r["factor_type"].astype(np.int32), r["ia"].astype(np.int32), r["ib"].astype(np.int32),
             np.ascontiguousarray(r["payload"]), r["huber"].astype(np.uint8))
+
+
+def compact_anchored_factors(rows_ptr: int, n: int, keep_ptr, type_ptr: int, ia_ptr: int, ib_ptr: int, payload_ptr: int,
+                             huber_ptr: int, count_ptr: int, stream: int):
+    """anchored_factor_rows on the device (osb_anchor_compact_factors_dev): the rows with skip == 0 and keep[i] (keep_ptr
+    may be None) in row order into device arrays of n rows each -- type / ia / ib int32, payload [n, PAYLOAD_LEN] float64,
+    huber uint8 -- and their number into the int32 at count_ptr, on `stream` without synchronising"""
+    _l.check(_l.load().osb_anchor_compact_factors_dev(C.c_void_p(rows_ptr), int(n),
+                                                      None if keep_ptr is None else C.c_void_p(keep_ptr),
+                                                      C.c_void_p(type_ptr), C.c_void_p(ia_ptr), C.c_void_p(ib_ptr),
+                                                      C.c_void_p(payload_ptr), C.c_void_p(huber_ptr),
+                                                      C.c_void_p(count_ptr), C.c_void_p(stream)))
 
 
 def anchored_loop_edges(res: np.ndarray) -> np.ndarray:

@@ -275,6 +275,8 @@ _SIG = {
     "osb_pcm_state_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int, C.POINTER(C.c_int32)]),
     "osb_pcm_state_set_inliers": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int]),
     "osb_pcm_state_pair": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, C.POINTER(C.c_int32)]),
+    "osb_pcm_state_reject_anchored": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "osb_pcm_state_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "osb_anchor_create": (C.c_int, [C.POINTER(_P), C.POINTER(AnchorParams)]),
     "osb_anchor_destroy": (C.c_int, [_P]),
     "osb_anchor_push_odometry": (C.c_int, [_P, C.c_int32, C.c_int, _P, _P]),
@@ -283,6 +285,7 @@ _SIG = {
     "osb_anchor_set_window": (C.c_int, [_P, C.c_int, _P, _P, _P]),
     "osb_anchor_run": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32)]),
     "osb_anchor_run_dev": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32), _P]),
+    "osb_anchor_compact_factors_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
