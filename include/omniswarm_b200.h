@@ -345,6 +345,43 @@ osb_status osb_solver_graph_get_poses(osb_solver* h, int first, int n, double* p
 osb_status osb_solver_graph_size(osb_solver* h, int32_t* n_nodes, int32_t* n_factors);
 osb_status osb_solver_graph_drop_oldest(osb_solver* h, int n_nodes);
 osb_status osb_solver_solve_resident(osb_solver* h, const osb_solve_options* opt, osb_solve_summary* summary);
+/* The resident graph plus a device-side tail: each solve's loop and detection rows, straight from
+ * osb_anchor_compact_factors_dev's buffers (type / ia / ib / payload / huber in its layout, *count_dev rows), are solved
+ * after the resident factors without reaching the host.  ia / ib are resident node ids (append order, renumbered by
+ * drop_oldest): the adapter numbers the anchor window's `block` ids as resident node ids and passes the renumbered window
+ * to osb_anchor_set_window after a drop.  The tail is not stored; the next call brings its own.
+ *   Numbering: the chain plan is built from the resident factors alone (on the host, cached by topology); tail rows never
+ *   join a path.  A tail row enters the chain preconditioner as a coupling when its two internal ids are consecutive and
+ *   linked, otherwise through its diagonal blocks -- as osb_solver_solve would place it under that plan.  The index
+ *   tables of (resident, tail) are built on the device in a fixed number of launches, deterministically.
+ *   max_tail picks the launch shape: it is osb_solver_solve's for (n, m + max_tail), and the solve reads m + k from the
+ *   device.  A call is bit-identical to osb_solver_solve of the concatenated list whenever both pick the same shape and
+ *   the same plan.  Size max_tail to the window, not to max_measurements: on the fp32 cluster path, m + max_tail <= 25 600
+ *   keeps the Jacobians in shared memory and <= 12 288 keeps the chain fast path.
+ *   Poses stay on the device: the call starts from a device copy of the resident poses and writes the solution back to it.
+ *   The first host-side solver call afterwards (graph_get_poses, graph_set_poses, graph_add_nodes, graph_drop_oldest,
+ *   solve_resident, solve, last_summary, ...) synchronises once and refreshes the host copy.  When the call was captured,
+ *   every host-side call re-reads what the last replay left, so the caller synchronises a replay before such a call;
+ *   this lasts until a host-side change of the poses or the graph.  Host-side pose changes are uploaded by the next
+ *   device call.
+ *   Refused on the device: a tail row with an unknown type, a node id outside [0, n), ia == ib, or *count_dev < 0
+ *   (OSB_ERR_INVALID) or > max_tail (OSB_ERR_CAPACITY): nothing is solved, poses and graph stay unchanged, and
+ *   osb_solver_last_summary returns the code.  Refused at once, with nothing enqueued: null pointers, max_tail < 0
+ *   (OSB_ERR_INVALID), m + max_tail > max_factors (OSB_ERR_CAPACITY), an empty resident graph (OSB_ERR_INVALID).
+ *   Stream capture: the call needs no host work when the topology and the poses have not changed on the host since the
+ *   previous device call, no factor is waiting to be uploaded and the options and max_tail are the previous call's.  Such
+ *   a call on the cluster path can be captured.  Under capture, a call that would need host work or would run on the
+ *   cooperative path returns OSB_ERR_INVALID before it enqueues anything.
+ *   Everything runs on `stream` (a cudaStream_t; consecutive device calls of a handle on one stream), after the handle's
+ *   host-side calls, which end in a synchronisation.  Six launches per call.
+ *   Memory: the first call acquires the device pose copy, the resident plan's tables and the per-call scratch (about
+ *   60 n + 36 m + 8 n ceil(m / 256) bytes at the handle's capacity n nodes, m factors); later calls acquire nothing. */
+osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev, const int32_t* ia_dev,
+                                         const int32_t* ib_dev, const double* payload_dev, const uint8_t* huber_dev,
+                                         const int32_t* count_dev, const osb_solve_options* opt, void* stream);
+/* synchronises with the last osb_solver_solve_resident_dev call -> its status; on OSB_OK its summary (n_residuals =
+ * resident + tail; solve_ms from CUDA events, 0 when the call was captured) */
+osb_status osb_solver_last_summary(osb_solver* h, osb_solve_summary* summary);
 /* profiling aid: SM-clock cycles block 0 spent in the phases of the LAST solve, summed over its CG iterations:
  * out[0] factor phase, [1] barrier after it, [2] node phase 1, [3] reduction 1, [4] node phase 2, [5] reduction 2,
  * [6] number of CG iterations, [7] whole kernel; [8] CTAs, [9] 1 = one thread-block cluster (hardware barrier) /

@@ -341,6 +341,23 @@ class ResidentPoseGraph {
     for (size_t i = 0; i < ptr_.size(); ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
     return s;
   }
+  // The resident window plus this solve's loop and detection rows where osb_anchor_compact_factors_dev left them (device
+  // pointers, *count_dev rows whose ia / ib are this graph's node ids, i.e. the anchor window's `block` ids; see
+  // osb_solver_solve_resident_dev).  Sends what was added, solves on `stream`, then waits for the solve and writes the
+  // poses back to the caller's double[4] blocks.
+  osb_solve_summary solve_with_device_factors(int max_tail, const int32_t* type_dev, const int32_t* ia_dev,
+                                              const int32_t* ib_dev, const double* payload_dev, const uint8_t* huber_dev,
+                                              const int32_t* count_dev, void* stream, const osb_solve_options* opt = nullptr) {
+    flush();
+    check(osb_solver_solve_resident_dev(solver_, max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev, count_dev, opt,
+                                        stream), "osb_solver_solve_resident_dev");
+    osb_solve_summary s{};
+    check(osb_solver_last_summary(solver_, &s), "osb_solver_last_summary");
+    std::vector<double> poses(4 * ptr_.size());
+    check(osb_solver_graph_get_poses(solver_, 0, (int)ptr_.size(), poses.data()), "osb_solver_graph_get_poses");
+    for (size_t i = 0; i < ptr_.size(); ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
+    return s;
+  }
 
  private:
   void flush() {                                     // send what was added since the last solve

@@ -220,6 +220,10 @@ struct SolverDev {
   int ctas;                // CTAs per solve (the cluster size on the cluster path)
   int first_trial;
   long long tstride;
+  // device tail (osb_solver_solve_resident_dev, graph_solve_kernel<T, false, true>): [0] status of the call's tables
+  // (non-zero: refused, nothing runs), [1] m = resident factors + tail, [2] fpc = ceil(m / ctas).  m and fpc above are
+  // then the bounds the launch shape was picked for.
+  const int32_t* dev_word;
 };
 
 // trial t's copy of a per-trial state pointer lies t * tstride bytes past trial 0's.  It is recomputed at every use from
@@ -555,9 +559,15 @@ __device__ __forceinline__ void factor_apply(const JStore<T>& J, int li, const T
   }
 }
 
-template <typename T, bool MT>
+// DT: one solve whose factor list ends in a device-side tail (osb_solver_solve_resident_dev).  The factor count and the
+// CTA blocks come from P.dev_word, and a refused call leaves on every CTA before the first barrier.
+template <typename T, bool MT, bool DT = false>
 __global__ void __launch_bounds__(GS_THREADS, 1)
 graph_solve_kernel(SolverDev P) {
+  if (DT) {
+    if (__ldcg(P.dev_word) != 0) return;
+    P.m = __ldcg(P.dev_word + 1); P.fpc = __ldcg(P.dev_word + 2);
+  }
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* smem_j = reinterpret_cast<T*>(smem_raw);
@@ -1061,6 +1071,203 @@ __global__ void multistart_select_kernel(int n_trials, int n, const osb_solve_su
   for (int i = lane; i < 4 * n; i += 32) res->poses()[i] = src[i];
 }
 
+// ---- device tail (osb_solver_solve_resident_dev) ---------------------------------------------------------------------
+// Each call's tables are those upload_graph builds for (resident factors, then the k tail rows) under the resident plan,
+// built on the device in four launches whatever k is.  A node's contribution slots are its base slots, then its tail rows
+// in row order; its chain couplings likewise.  The rank of a tail row among the earlier rows that touch the same node is
+// the rank inside its chunk of TL_ROWS rows (a compare over the chunk in shared memory) plus the node's count in the
+// earlier chunks (a scan down each node's column of per-chunk counts): no atomics, so every table is the same on every run.
+constexpr int TL_ROWS = 256;             // tail rows per CTA of tail_rank_kernel (2 slot keys each: one thread per key)
+
+struct TailDev {
+  int n, m_base, max_tail, ctas, chunks;
+  const int32_t* count;                                              // the caller's k
+  const int32_t *type, *ia, *ib; const double* payload; const uint8_t* huber;   // the caller's tail rows (node ids)
+  // the resident plan: caller's id -> internal id and back, and the base-only tables of upload_graph
+  const int32_t *inv, *order, *b_ia, *b_ib, *b_ptr, *b_slot_a, *b_slot_b, *b_es_ptr, *b_es_slot;
+  const uint8_t *b_fixed, *b_link;
+  // scratch
+  int32_t *key_s, *rank_s;       // [2 max_tail] internal node of slot 2j (node a) / 2j+1 (node b) of row j, -1: none
+  int32_t *key_e, *rank_e;       // [max_tail] the later node of a chain coupling, -1: not a coupling
+  int32_t *hist_s, *hist_e;      // [chunks][n] per-chunk counts, then (tail_scan_kernel) the earlier chunks' counts
+  int32_t *cnt_s, *cnt_e;        // [n] the node's tail slots / couplings, then (tail_ptr_kernel) their exclusive prefix
+  int32_t* flag;                 // [chunks][2] refused row seen, tail residuals
+  int32_t* word;                 // [0] status, [1] m, [2] fpc, [3] tail residuals
+  // the solve's tables (the handle's one-shot buffers) and poses
+  int32_t *ia_o, *ib_o, *ptr_o, *slot_a_o, *slot_b_o, *es_ptr_o, *es_slot_o, *type_o;
+  double* payload_o;
+  uint8_t *huber_o, *fixed_o, *link_o;
+  double* poses;                 // [n][4] the resident poses, caller's order
+  double *x0, *x_out;            // the solve's start and result, internal order
+};
+
+// k, or -1 when *count is outside [0, max_tail]
+__device__ __forceinline__ int tail_count(const TailDev& D) {
+  const int c = __ldcg(D.count);
+  return (c < 0 || c > D.max_tail) ? -1 : c;
+}
+
+// one CTA per chunk of TL_ROWS rows: validate, map to internal ids, rank each key inside the chunk, per-chunk counts
+__global__ void __launch_bounds__(2 * TL_ROWS) tail_rank_kernel(TailDev D) {
+  __shared__ int ks[2 * TL_ROWS], ke[TL_ROWS];
+  const int c = blockIdx.x, t = threadIdx.x, k = max(0, tail_count(D));
+  const int j = c * TL_ROWS + (t >> 1), side = t & 1;
+  int key = -1, ekey = -1, nr = 0;
+  bool bad = false;
+  if (j < k) {
+    const int ty = D.type[j], a = D.ia[j], b = D.ib[j];
+    bad = ty < 0 || ty > 2 || a < 0 || a >= D.n || b < 0 || b >= D.n || a == b;
+    if (!bad) {
+      const int A = D.inv[a], B = D.inv[b], hi = max(A, B);
+      key = side ? B : A;
+      if (side == 0) {
+        if (abs(A - B) == 1 && D.b_link[hi]) ekey = hi;
+        nr = ty == OSB_FACTOR_DISTANCE ? 1 : ty == OSB_FACTOR_RELPOSE ? 4
+             : (((int)D.payload[(size_t)j * OSB_PAYLOAD_LEN + 10] & 1) ? 3 : 2);
+      }
+    }
+  }
+  ks[t] = key;
+  if (side == 0) ke[t >> 1] = ekey;
+  for (int v = t; v < D.n; v += blockDim.x) { D.hist_s[(size_t)c * D.n + v] = 0; D.hist_e[(size_t)c * D.n + v] = 0; }
+  const int any_bad = __syncthreads_or(bad);
+  // tail residuals of the chunk: sum of nr in 1..4 as four block counts
+  const int n1 = __syncthreads_count(nr >= 1), n2 = __syncthreads_count(nr >= 2), n3 = __syncthreads_count(nr >= 3),
+            n4 = __syncthreads_count(nr >= 4);
+  if (t == 0) { D.flag[2 * c] = any_bad; D.flag[2 * c + 1] = n1 + n2 + n3 + n4; }
+  if (key >= 0) {
+    int r = 0;
+    bool last = true;
+    for (int u = 0; u < 2 * TL_ROWS; ++u)
+      if (ks[u] == key) { if (u < t) ++r; else if (u > t) last = false; }
+    D.rank_s[2 * j + side] = r;
+    if (last) D.hist_s[(size_t)c * D.n + key] = r + 1;
+  }
+  if (side == 0 && j < D.max_tail) D.key_e[j] = ekey;
+  if (ekey >= 0) {
+    const int me = t >> 1;
+    int r = 0;
+    bool last = true;
+    for (int u = 0; u < TL_ROWS; ++u)
+      if (ke[u] == ekey) { if (u < me) ++r; else if (u > me) last = false; }
+    D.rank_e[j] = r;
+    if (last) D.hist_e[(size_t)c * D.n + ekey] = r + 1;
+  }
+}
+
+// one thread per node: the exclusive scan of its per-chunk counts down the chunks, and its tail totals
+__global__ void tail_scan_kernel(TailDev D) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= D.n) return;
+  int rs = 0, re = 0;
+  for (int c = 0; c < D.chunks; ++c) {
+    int32_t* hs = D.hist_s + (size_t)c * D.n + v;
+    int32_t* he = D.hist_e + (size_t)c * D.n + v;
+    const int a = *hs, b = *he;
+    *hs = rs; *he = re;
+    rs += a; re += b;
+  }
+  D.cnt_s[v] = rs; D.cnt_e[v] = re;
+}
+
+// exclusive scan of v over the 1024 threads of the block; *total = the sum (sh: 32 ints)
+__device__ __forceinline__ int block_excl_scan(int v, int* sh, int* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+  if (lane == 31) sh[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    int s = sh[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
+    sh[lane] = s;
+  }
+  __syncthreads();
+  const int r = x - v + (w > 0 ? sh[w - 1] : 0);
+  *total = sh[31];
+  __syncthreads();
+  return r;
+}
+
+// one CTA of 1024 threads: the call's status and m, then the CSR pointers of the slots and of the chain couplings
+__global__ void __launch_bounds__(1024) tail_ptr_kernel(TailDev D) {
+  __shared__ int sh[32];
+  __shared__ int status;
+  const int kc = tail_count(D);
+  int bad = 0, nres = 0;
+  for (int c = threadIdx.x; c < D.chunks; c += blockDim.x) { bad |= D.flag[2 * c]; nres += D.flag[2 * c + 1]; }
+  bad = __syncthreads_or(bad);
+  int nres_total = 0;
+  block_excl_scan(nres, sh, &nres_total);
+  if (threadIdx.x == 0) {
+    const int c = __ldcg(D.count);
+    status = kc < 0 ? (c < 0 ? OSB_ERR_INVALID : OSB_ERR_CAPACITY) : bad ? OSB_ERR_INVALID : OSB_OK;
+    const int m = D.m_base + max(kc, 0);
+    D.word[0] = status; D.word[1] = m; D.word[2] = (m + D.ctas - 1) / D.ctas; D.word[3] = nres_total;
+  }
+  __syncthreads();
+  if (status != OSB_OK) return;
+  int carry_s = 0, carry_e = 0;
+  for (int v0 = 0; v0 < D.n; v0 += blockDim.x) {
+    const int v = v0 + threadIdx.x;
+    int ts = 0, te = 0;
+    const int xs = block_excl_scan(v < D.n ? D.cnt_s[v] : 0, sh, &ts);
+    const int xe = block_excl_scan(v < D.n ? D.cnt_e[v] : 0, sh, &te);
+    if (v < D.n) {
+      D.cnt_s[v] = carry_s + xs; D.cnt_e[v] = carry_e + xe;
+      D.ptr_o[v] = D.b_ptr[v] + carry_s + xs; D.es_ptr_o[v] = D.b_es_ptr[v] + carry_e + xe;
+    }
+    carry_s += ts; carry_e += te;
+  }
+  if (threadIdx.x == 0) { D.ptr_o[D.n] = D.b_ptr[D.n] + carry_s; D.es_ptr_o[D.n] = D.b_es_ptr[D.n] + carry_e; }
+}
+
+// one thread per factor of (resident, tail) and per node: the factor tables, the tail rows behind the resident factor
+// arrays, the node tables and the starting poses in internal order
+__global__ void tail_tables_kernel(TailDev D) {
+  if (__ldcg(D.word) != OSB_OK) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int m = __ldcg(D.word + 1);
+  if (i < D.m_base) {
+    const int a = D.b_ia[i], b = D.b_ib[i], e = D.b_es_slot[i];
+    D.ia_o[i] = a; D.ib_o[i] = b;
+    D.slot_a_o[i] = D.b_slot_a[i] + D.cnt_s[a];
+    D.slot_b_o[i] = D.b_slot_b[i] + D.cnt_s[b];
+    D.es_slot_o[i] = e < 0 ? -1 : e + 2 * D.cnt_e[max(a, b)];
+  } else if (i < m) {
+    const int j = i - D.m_base, c = j / TL_ROWS;
+    const int A = D.inv[D.ia[j]], B = D.inv[D.ib[j]];
+    D.ia_o[i] = A; D.ib_o[i] = B;
+    D.slot_a_o[i] = D.ptr_o[A] + (D.b_ptr[A + 1] - D.b_ptr[A]) + D.hist_s[(size_t)c * D.n + A] + D.rank_s[2 * j];
+    D.slot_b_o[i] = D.ptr_o[B] + (D.b_ptr[B + 1] - D.b_ptr[B]) + D.hist_s[(size_t)c * D.n + B] + D.rank_s[2 * j + 1];
+    const int hi = D.key_e[j];
+    D.es_slot_o[i] = hi < 0 ? -1
+        : 2 * (D.es_ptr_o[hi] + (D.b_es_ptr[hi + 1] - D.b_es_ptr[hi]) + D.hist_e[(size_t)c * D.n + hi] + D.rank_e[j]) +
+          (A == hi ? 1 : 0);
+    D.type_o[i] = D.type[j]; D.huber_o[i] = D.huber[j];
+    for (int q = 0; q < OSB_PAYLOAD_LEN; ++q)
+      D.payload_o[(size_t)i * OSB_PAYLOAD_LEN + q] = D.payload[(size_t)j * OSB_PAYLOAD_LEN + q];
+  }
+  if (i < D.n) {
+    D.fixed_o[i] = D.b_fixed[i]; D.link_o[i] = D.b_link[i];
+    const int src = D.order[i];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) D.x0[4 * i + q] = D.poses[4 * src + q];
+  }
+}
+
+// the solution back into the resident poses (caller's order); a refused call leaves them as they were
+__global__ void tail_poses_out_kernel(TailDev D) {
+  if (__ldcg(D.word) != OSB_OK) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.n) return;
+  const int dst = D.order[i];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) D.poses[4 * dst + q] = __ldcg(D.x_out + 4 * i + q);
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -1071,6 +1278,7 @@ struct SolveShape {
   bool f32;              // fp32 inner (PCG) arithmetic
   const void* kern;      // one solve per launch
   const void* kern_multi;  // several clusters per launch, one trial each (same resources, same arithmetic)
+  const void* kern_dt;     // one solve whose factor count is read on the device (osb_solver_solve_resident_dev)
   int cluster;           // 1: one thread-block cluster per solve (hardware barrier); 0: one cooperative grid per launch
   int ctas, fpc, chain, jsmem;
   size_t smem;           // dynamic shared memory per CTA
@@ -1138,7 +1346,26 @@ struct osb_solver {
   unsigned long long g_topo_version = 1, cached_topo = 0;
   std::vector<int32_t> cached_order;
   int cached_nres = 0;
+  // device tail (osb_solver_solve_resident_dev).  The resident plan's base-only tables live in d_tail (acquired by the
+  // first device call, carved by tail_layout) beside the call's scratch, so a one-shot solve never overwrites them.
+  char* d_tail = nullptr;
+  TailDev tail = {};                // d_tail's pointers
+  double* d_rposes = nullptr;       // the resident poses on the device, caller's order
+  osb_solve_summary* d_tsummary = nullptr;
+  cudaEvent_t ev_done = nullptr;
+  unsigned long long tail_topo = 0; // topology the base tables were built for
+  std::vector<int32_t> tail_order;
+  int tail_nres = 0;                // residuals of the resident factors
+  bool rposes_current = false;      // d_rposes holds g_poses (false: the next device call uploads them)
+  long long tail_shape_key = -1;    // (n, m + max_tail, precision, preconditioner) of tail_shape
+  SolveShape tail_shape = {};
+  // the last device call: pending until a host-side call synchronises with it and refreshes g_poses from d_rposes
+  bool dev_pending = false, dev_captured = false, dev_called = false;
+  osb_status dev_status = OSB_OK;
+  osb_solve_summary dev_summary = {};
 };
+
+static osb_status finish_device_call(osb_solver* h);
 
 extern "C" void osb_solve_default_options(osb_solve_options* o) {
   if (!o) return;
@@ -1165,7 +1392,9 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
   OSB_TRY(h->res.event(&h->ev1));
   h->cluster_ok = true;
   for (const void* k : {(const void*)graph_solve_kernel<float, false>, (const void*)graph_solve_kernel<double, false>,
-                        (const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>}) {
+                        (const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>,
+                        (const void*)graph_solve_kernel<float, false, true>,
+                        (const void*)graph_solve_kernel<double, false, true>}) {
     OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
     h->cluster_ok = h->cluster_ok && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
   }
@@ -1288,6 +1517,55 @@ static osb_status validate_graph(int n_nodes, int n_factors, const int32_t* type
   return OSB_OK;
 }
 
+// The index tables of one factor list under a chain plan: internal ids, the CSR of contribution slots, the chain
+// couplings, the fixed flags in internal order and the residual count.
+struct GraphTables {
+  std::vector<int32_t> ia, ib, ptr, slot_a, slot_b, es_ptr, es_slot;
+  std::vector<uint8_t> fixed;
+  int n_res = 0;
+};
+
+static void build_tables(int n_nodes, const uint8_t* fixed, int n_factors, const int32_t* type, const int32_t* ia,
+                         const int32_t* ib, const double* payload, const ChainPlan& plan, GraphTables& t) {
+  const size_t n = n_nodes, m = n_factors;
+  std::vector<int32_t>& ia_p = t.ia; std::vector<int32_t>& ib_p = t.ib;
+  ia_p.resize(m); ib_p.resize(m);
+  std::vector<uint8_t>& fixed_p = t.fixed;
+  fixed_p.resize(n);
+  for (size_t f = 0; f < m; ++f) { ia_p[f] = plan.inv[ia[f]]; ib_p[f] = plan.inv[ib[f]]; }
+  for (size_t i = 0; i < n; ++i) fixed_p[i] = fixed[plan.order[i]];
+  // chain couplings: factor f couples node hi with hi-1 when its two nodes are consecutive and linked
+  std::vector<int32_t>& es_ptr = t.es_ptr; std::vector<int32_t>& es_slot = t.es_slot;
+  es_ptr.assign(n + 1, 0); es_slot.assign(m, -1);
+  for (size_t f = 0; f < m; ++f) {
+    const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
+    if (std::abs(a - b) == 1 && plan.link[hi]) es_ptr[hi + 1]++;
+  }
+  for (size_t i = 0; i < n; ++i) es_ptr[i + 1] += es_ptr[i];
+  {
+    std::vector<int32_t> fill(es_ptr.begin(), es_ptr.end() - 1);
+    for (size_t f = 0; f < m; ++f) {
+      const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
+      if (std::abs(a - b) == 1 && plan.link[hi]) es_slot[f] = 2 * (fill[hi]++) + (a == hi ? 1 : 0);
+    }
+  }
+  // CSR of contribution slots: node n owns slots [ptr[n], ptr[n+1]); factors in index order within a node, so the
+  // gather order -- and therefore every floating-point sum -- is fixed.
+  std::vector<int32_t>& ptr = t.ptr; std::vector<int32_t>& slot_a = t.slot_a; std::vector<int32_t>& slot_b = t.slot_b;
+  ptr.assign(n + 1, 0); slot_a.resize(m); slot_b.resize(m);
+  for (size_t f = 0; f < m; ++f) { ptr[ia_p[f] + 1]++; ptr[ib_p[f] + 1]++; }
+  for (size_t i = 0; i < n; ++i) ptr[i + 1] += ptr[i];
+  {
+    std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
+    for (size_t f = 0; f < m; ++f) { slot_a[f] = fill[ia_p[f]]++; slot_b[f] = fill[ib_p[f]]++; }
+  }
+  int& n_res = t.n_res;
+  n_res = 0;
+  for (size_t f = 0; f < m; ++f)
+    n_res += type[f] == OSB_FACTOR_DISTANCE ? 1 : type[f] == OSB_FACTOR_RELPOSE ? 4
+             : (((int)payload[f * OSB_PAYLOAD_LEN + 10] & 1) ? 3 : 2);
+}
+
 // Upload the graph of one solve and the caller's poses: the chain plan, the internal numbering and the index tables
 // (unless the resident graph's topology is unchanged), the factor arrays when upload_static (the resident entry point has
 // already appended them), then the poses in internal order into x0 through the pinned staging.  The caller holds h->mu.
@@ -1303,37 +1581,12 @@ static osb_status upload_graph(osb_solver* h, int n_nodes, const double* poses, 
   if (!reuse) {
     ChainPlan plan;
     build_chain_plan(n_nodes, fixed, n_factors, type, ia, ib, payload, plan);
-    std::vector<int32_t> ia_p(m), ib_p(m);
-    std::vector<uint8_t> fixed_p(n);
-    for (size_t f = 0; f < m; ++f) { ia_p[f] = plan.inv[ia[f]]; ib_p[f] = plan.inv[ib[f]]; }
-    for (size_t i = 0; i < n; ++i) fixed_p[i] = fixed[plan.order[i]];
-    // chain couplings: factor f couples node hi with hi-1 when its two nodes are consecutive and linked
-    std::vector<int32_t> es_ptr(n + 1, 0), es_slot(m, -1);
-    for (size_t f = 0; f < m; ++f) {
-      const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
-      if (std::abs(a - b) == 1 && plan.link[hi]) es_ptr[hi + 1]++;
-    }
-    for (size_t i = 0; i < n; ++i) es_ptr[i + 1] += es_ptr[i];
-    {
-      std::vector<int32_t> fill(es_ptr.begin(), es_ptr.end() - 1);
-      for (size_t f = 0; f < m; ++f) {
-        const int a = ia_p[f], b = ib_p[f], hi = std::max(a, b);
-        if (std::abs(a - b) == 1 && plan.link[hi]) es_slot[f] = 2 * (fill[hi]++) + (a == hi ? 1 : 0);
-      }
-    }
-    // CSR of contribution slots: node n owns slots [ptr[n], ptr[n+1]); factors in index order within a node, so the
-    // gather order -- and therefore every floating-point sum -- is fixed.
-    std::vector<int32_t> ptr(n + 1, 0), slot_a(m), slot_b(m);
-    for (size_t f = 0; f < m; ++f) { ptr[ia_p[f] + 1]++; ptr[ib_p[f] + 1]++; }
-    for (size_t i = 0; i < n; ++i) ptr[i + 1] += ptr[i];
-    {
-      std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
-      for (size_t f = 0; f < m; ++f) { slot_a[f] = fill[ia_p[f]]++; slot_b[f] = fill[ib_p[f]]++; }
-    }
-    int n_res = 0;
-    for (size_t f = 0; f < m; ++f)
-      n_res += type[f] == OSB_FACTOR_DISTANCE ? 1 : type[f] == OSB_FACTOR_RELPOSE ? 4
-               : (((int)payload[f * OSB_PAYLOAD_LEN + 10] & 1) ? 3 : 2);
+    GraphTables t;
+    build_tables(n_nodes, fixed, n_factors, type, ia, ib, payload, plan, t);
+    const std::vector<int32_t> &ia_p = t.ia, &ib_p = t.ib, &ptr = t.ptr, &slot_a = t.slot_a, &slot_b = t.slot_b;
+    const std::vector<int32_t> &es_ptr = t.es_ptr, &es_slot = t.es_slot;
+    const std::vector<uint8_t>& fixed_p = t.fixed;
+    const int n_res = t.n_res;
     OSB_CUDA(cudaMemcpyAsync(h->d_fixed, fixed_p.data(), n, cudaMemcpyHostToDevice, st));
     if (upload_static) {
       OSB_CUDA(cudaMemcpyAsync(h->d_huber, huber, m, cudaMemcpyHostToDevice, st));
@@ -1367,6 +1620,7 @@ static osb_status solve_shape(const osb_solver* h, int n_nodes, int n_factors, c
   const size_t tsz = s.f32 ? sizeof(float) : sizeof(double);
   s.kern = s.f32 ? (const void*)graph_solve_kernel<float, false> : (const void*)graph_solve_kernel<double, false>;
   s.kern_multi = s.f32 ? (const void*)graph_solve_kernel<float, true> : (const void*)graph_solve_kernel<double, true>;
+  s.kern_dt = s.f32 ? (const void*)graph_solve_kernel<float, false, true> : (const void*)graph_solve_kernel<double, false, true>;
   s.chain = 0;
   // ONE thread-block cluster (hardware barrier, ~0.2 us) when the factor list fits 16 CTAs with their Jacobians in
   // shared memory; otherwise a cooperative grid (software grid barrier).
@@ -1417,21 +1671,24 @@ static SolverDev graph_dev(const osb_solver* h, int n_nodes, int n_factors, cons
 
 // n_trials solves of one shape, P bound at trial 0 = the start of the arena, trial t's block tstride bytes further.
 // Cluster path: ONE launch of n_trials clusters (clusters do not wait for each other, so the grid may exceed what is
-// resident).  Cooperative path: one grid per trial, in order on the stream.
-static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s, int n_trials, long long tstride) {
+// resident).  Cooperative path: one grid per trial, in order on the stream.  dt: the one solve of
+// osb_solver_solve_resident_dev, on the caller's stream `st`.
+static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s, int n_trials, long long tstride,
+                                cudaStream_t st, bool dt = false) {
   P.fpc = s.fpc; P.use_cluster = s.cluster; P.j_in_smem = s.jsmem; P.use_chain = s.chain;
   P.ctas = s.ctas; P.first_trial = 0; P.tstride = tstride;
   h->last_shape = s;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
-  cfg.blockDim = dim3(GS_THREADS); cfg.stream = h->stream; cfg.attrs = attr; cfg.numAttrs = 1;
+  cfg.blockDim = dim3(GS_THREADS); cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
   cfg.dynamicSmemBytes = s.smem;
+  const void* single = dt ? s.kern_dt : s.kern;
   if (s.cluster) {
     cfg.gridDim = dim3(n_trials * s.ctas);
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = s.ctas; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     void* kargs[1] = {&P};
-    OSB_CUDA(cudaLaunchKernelExC(&cfg, n_trials > 1 ? s.kern_multi : s.kern, kargs));
+    OSB_CUDA(cudaLaunchKernelExC(&cfg, n_trials > 1 ? s.kern_multi : single, kargs));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return OSB_OK;
   }
@@ -1442,8 +1699,9 @@ static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s,
     SolverDev Q = P;
     Q.first_trial = t;
     trial_layout(Q, h->d_arena + t * tstride, P.n, P.m, s);
+    if (dt) Q.summary = P.summary;
     void* kargs[1] = {&Q};
-    OSB_CUDA(cudaLaunchKernelExC(&cfg, s.kern, kargs));
+    OSB_CUDA(cudaLaunchKernelExC(&cfg, single, kargs));
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
   return OSB_OK;
@@ -1488,7 +1746,7 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
     OSB_CHECK_LAUNCH();
   }
   OSB_CUDA(cudaEventRecord(h->ev0, st));
-  s = launch_solves(h, P, shape, K, (long long)tstride);
+  s = launch_solves(h, P, shape, K, (long long)tstride, st);
   if (s != OSB_OK) return s;
   OSB_CUDA(cudaEventRecord(h->ev1, st));
   SolveResults* r = h->h_res;
@@ -1530,6 +1788,7 @@ extern "C" osb_status osb_solver_solve(osb_solver* h, int n_nodes, double* poses
   if (s != OSB_OK) return s;
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   h->g_static_valid = false;              // the device factor arrays now hold this graph, not the resident one
   h->cached_topo = 0;                     // ... and so do the index tables
   return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, opt, nullptr, nullptr,
@@ -1558,6 +1817,7 @@ extern "C" osb_status osb_solver_solve_multistart(osb_solver* h, int n_nodes, do
   if (s != OSB_OK) return s;
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   h->g_static_valid = false;              // as osb_solver_solve: the device factor arrays and tables now hold this graph
   h->cached_topo = 0;
   return solver_run(h, n_nodes, poses, fixed, n_factors, type, ia, ib, payload, huber, true, 0, opt, ms, init_mask,
@@ -1575,10 +1835,12 @@ extern "C" osb_status osb_solver_graph_clear(osb_solver* h) {
   OSB_REQUIRE(h != nullptr, "null handle");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   h->g_poses.clear(); h->g_payload.clear(); h->g_fixed.clear(); h->g_huber.clear();
   h->g_type.clear(); h->g_ia.clear(); h->g_ib.clear();
   h->g_uploaded = 0; h->g_static_valid = true;
   ++h->g_topo_version;
+  h->rposes_current = false; h->dev_pending = false;
   return OSB_OK;
 }
 
@@ -1587,12 +1849,14 @@ extern "C" osb_status osb_solver_graph_add_nodes(osb_solver* h, int n, const dou
   OSB_REQUIRE(h != nullptr && n > 0 && poses != nullptr, "bad argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   const size_t have = h->g_fixed.size();
   if (have + (size_t)n > (size_t)h->max_nodes) { set_error("osb_solver_graph_add_nodes", "node capacity exceeded"); return OSB_ERR_CAPACITY; }
   if (first_id) *first_id = (int32_t)have;
   h->g_poses.insert(h->g_poses.end(), poses, poses + 4 * (size_t)n);
   for (int i = 0; i < n; ++i) h->g_fixed.push_back(fixed ? fixed[i] : 0);
   ++h->g_topo_version;
+  h->rposes_current = false; h->dev_pending = false;
   return OSB_OK;
 }
 
@@ -1601,6 +1865,7 @@ extern "C" osb_status osb_solver_graph_add_factors(osb_solver* h, int m, const i
   OSB_REQUIRE(h != nullptr && m > 0 && type && ia && ib && payload && huber, "bad argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   const size_t have = h->g_type.size();
   if (have + (size_t)m > (size_t)h->max_factors) { set_error("osb_solver_graph_add_factors", "factor capacity exceeded"); return OSB_ERR_CAPACITY; }
   osb_status s = validate_graph((int)h->g_fixed.size(), m, type, ia, ib);
@@ -1618,6 +1883,7 @@ extern "C" osb_status osb_solver_graph_set_fixed(osb_solver* h, int node, int fi
   OSB_REQUIRE(h != nullptr, "null handle");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   OSB_REQUIRE(node >= 0 && (size_t)node < h->g_fixed.size(), "node out of range");
   h->g_fixed[node] = fixed ? 1 : 0;
   ++h->g_topo_version;
@@ -1628,8 +1894,10 @@ extern "C" osb_status osb_solver_graph_set_poses(osb_solver* h, int first, int n
   OSB_REQUIRE(h != nullptr && poses != nullptr, "bad argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   OSB_REQUIRE(first >= 0 && n >= 0 && (size_t)(first + n) <= h->g_fixed.size(), "node range out of bounds");
   std::copy(poses, poses + 4 * (size_t)n, h->g_poses.begin() + 4 * (size_t)first);
+  h->rposes_current = false; h->dev_pending = false;
   return OSB_OK;
 }
 
@@ -1637,6 +1905,7 @@ extern "C" osb_status osb_solver_graph_get_poses(osb_solver* h, int first, int n
   OSB_REQUIRE(h != nullptr && poses != nullptr, "bad argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));          // a device call's poses reach g_poses first
   OSB_REQUIRE(first >= 0 && n >= 0 && (size_t)(first + n) <= h->g_fixed.size(), "node range out of bounds");
   std::copy(h->g_poses.begin() + 4 * (size_t)first, h->g_poses.begin() + 4 * (size_t)(first + n), poses);
   return OSB_OK;
@@ -1646,6 +1915,7 @@ extern "C" osb_status osb_solver_graph_size(osb_solver* h, int32_t* n_nodes, int
   OSB_REQUIRE(h != nullptr, "null handle");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   if (n_nodes) *n_nodes = (int32_t)h->g_fixed.size();
   if (n_factors) *n_factors = (int32_t)h->g_type.size();
   return OSB_OK;
@@ -1657,6 +1927,7 @@ extern "C" osb_status osb_solver_graph_drop_oldest(osb_solver* h, int n_nodes) {
   OSB_REQUIRE(h != nullptr && n_nodes >= 0, "bad argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   OSB_REQUIRE((size_t)n_nodes <= h->g_fixed.size(), "cannot drop more nodes than the graph holds");
   if (n_nodes == 0) return OSB_OK;
   h->g_poses.erase(h->g_poses.begin(), h->g_poses.begin() + 4 * (size_t)n_nodes);
@@ -1673,15 +1944,73 @@ extern "C" osb_status osb_solver_graph_drop_oldest(osb_solver* h, int n_nodes) {
   h->g_type.resize(w); h->g_ia.resize(w); h->g_ib.resize(w); h->g_huber.resize(w); h->g_payload.resize(w * OSB_PAYLOAD_LEN);
   h->g_uploaded = 0;                       // factor positions moved: re-send on the next solve
   ++h->g_topo_version;
+  h->rposes_current = false; h->dev_pending = false;
   return OSB_OK;
 }
+
+static osb_status flush_resident_factors(osb_solver* h);
 
 extern "C" osb_status osb_solver_solve_resident(osb_solver* h, const osb_solve_options* opt, osb_solve_summary* summary) {
   OSB_REQUIRE(h != nullptr && summary != nullptr, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   const size_t n = h->g_fixed.size(), m = h->g_type.size();
   OSB_REQUIRE(n > 0 && m > 0, "the resident graph is empty");
+  OSB_TRY(flush_resident_factors(h));
+  h->rposes_current = false;               // this solve writes g_poses
+  h->dev_pending = false;
+  return solver_run(h, (int)n, h->g_poses.data(), h->g_fixed.data(), (int)m, h->g_type.data(), h->g_ia.data(),
+                    h->g_ib.data(), h->g_payload.data(), h->g_huber.data(), false, h->g_topo_version, opt, nullptr,
+                    nullptr, summary);
+}
+
+// ---- device tail (osb_solver_solve_resident_dev) -----------------------------------------------------------------
+// Carve the device-tail buffers from `base` (nullptr: size only) for a handle of n nodes and m factors.
+static size_t tail_layout(TailDev& D, char* base, size_t n, size_t m) {
+  const size_t chunks = std::max<size_t>(1, (m + TL_ROWS - 1) / TL_ROWS);
+  size_t at = 0;
+  auto take = [&](auto*& p, size_t count) {
+    using Q = std::remove_const_t<std::remove_pointer_t<std::remove_reference_t<decltype(p)>>>;
+    p = reinterpret_cast<Q*>(reinterpret_cast<uintptr_t>(base) + at);
+    at += (count * sizeof(Q) + 255) & ~(size_t)255;
+  };
+  take(D.inv, n); take(D.order, n); take(D.b_ia, m); take(D.b_ib, m); take(D.b_ptr, n + 1); take(D.b_slot_a, m);
+  take(D.b_slot_b, m); take(D.b_es_ptr, n + 1); take(D.b_es_slot, m); take(D.b_fixed, n); take(D.b_link, n);
+  take(D.key_s, 2 * m); take(D.rank_s, 2 * m); take(D.key_e, m); take(D.rank_e, m);
+  take(D.hist_s, chunks * n); take(D.hist_e, chunks * n); take(D.cnt_s, n); take(D.cnt_e, n);
+  take(D.flag, 2 * chunks); take(D.word, 4);
+  return at;
+}
+
+// The first host-side call after a device call waits for it and refreshes the host mirror of the poses, the call's status
+// and its summary.  A captured call stays pending: every host-side call re-reads what the last replay left (the caller
+// has synchronised it), until a host-side change of the poses or the graph takes over.  The caller holds h->mu.
+static osb_status finish_device_call(osb_solver* h) {
+  if (!h->dev_pending) return OSB_OK;
+  if (!h->dev_captured) h->dev_pending = false;
+  if (!h->dev_captured) OSB_CUDA(cudaEventSynchronize(h->ev_done));
+  int32_t word[4];
+  osb_solve_summary sm;
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaMemcpyAsync(word, h->tail.word, sizeof(word), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaMemcpyAsync(&sm, h->d_tsummary, sizeof(sm), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaMemcpyAsync(h->g_poses.data(), h->d_rposes, h->g_poses.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  h->dev_status = (osb_status)word[0];
+  if (h->dev_status == OSB_OK) {
+    float msec = 0.f;
+    if (!h->dev_captured) OSB_CUDA(cudaEventElapsedTime(&msec, h->ev0, h->ev1));
+    sm.solve_ms = msec;
+    sm.n_residuals = h->tail_nres + word[3];
+    h->dev_summary = sm;
+  }
+  return OSB_OK;
+}
+
+// the resident factors added since the last solve -> device (all of them after a one-shot call overwrote the arrays)
+static osb_status flush_resident_factors(osb_solver* h) {
+  const size_t m = h->g_type.size();
   if (!h->g_static_valid) { h->g_uploaded = 0; h->g_static_valid = true; h->cached_topo = 0; }
   if (h->g_uploaded < m) {                 // only the factors added since the last solve cross PCIe
     const size_t f0 = h->g_uploaded, k = m - f0;
@@ -1692,15 +2021,140 @@ extern "C" osb_status osb_solver_solve_resident(osb_solver* h, const osb_solve_o
                              k * OSB_PAYLOAD_LEN * sizeof(double), cudaMemcpyHostToDevice, st));
     h->g_uploaded = m;
   }
-  return solver_run(h, (int)n, h->g_poses.data(), h->g_fixed.data(), (int)m, h->g_type.data(), h->g_ia.data(),
-                    h->g_ib.data(), h->g_payload.data(), h->g_huber.data(), false, h->g_topo_version, opt, nullptr,
-                    nullptr, summary);
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev,
+                                                    const int32_t* ia_dev, const int32_t* ib_dev, const double* payload_dev,
+                                                    const uint8_t* huber_dev, const int32_t* count_dev,
+                                                    const osb_solve_options* opt, void* stream) {
+  OSB_REQUIRE(h && type_dev && ia_dev && ib_dev && payload_dev && huber_dev && count_dev, "null argument");
+  OSB_REQUIRE(max_tail >= 0, "max_tail must be >= 0");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  OSB_CUDA(cudaStreamIsCapturing(st, &cap));
+  const bool capturing = cap != cudaStreamCaptureStatusNone;
+  const size_t n = h->g_fixed.size(), m_base = h->g_type.size();
+  OSB_REQUIRE(n > 0 && m_base > 0, "the resident graph is empty");
+  if (m_base + (size_t)max_tail > (size_t)h->max_factors) {
+    set_error("osb_solver_solve_resident_dev", "resident factors + max_tail exceed the solver capacity");
+    return OSB_ERR_CAPACITY;
+  }
+  osb_solve_options o;
+  if (opt) o = *opt; else osb_solve_default_options(&o);
+  const int m_bound = (int)m_base + max_tail;
+  // the launch shape is solve_shape's for (n, m + max_tail); cached so that a captured call makes no occupancy query
+  const bool f32 = o.inner_precision == OSB_INNER_FP32 || (o.inner_precision == OSB_INNER_AUTO && o.pcg_tolerance >= 1e-4);
+  const long long shape_key = (((long long)n * (h->max_factors + 1LL) + m_bound) * 2 + (f32 ? 1 : 0)) * 2 +
+                              (o.preconditioner == OSB_PRECOND_BLOCK_JACOBI ? 1 : 0);
+  const bool host_work = h->d_tail == nullptr || h->tail_topo != h->g_topo_version || !h->g_static_valid ||
+                         h->g_uploaded < m_base || !h->rposes_current || shape_key != h->tail_shape_key;
+  if (capturing && (host_work || !h->tail_shape.cluster)) {
+    set_error("osb_solver_solve_resident_dev", capturing && !host_work
+              ? "the cooperative path cannot be captured"
+              : "a captured call cannot do host work: run the call once outside the capture after the graph changed");
+    return OSB_ERR_INVALID;
+  }
+  if (host_work) {
+    if (h->d_tail == nullptr) {                // everything a device call needs, once per handle
+      TailDev D = {};
+      OSB_TRY(h->res.alloc(&h->d_tail, tail_layout(D, nullptr, h->max_nodes, h->max_factors)));
+      OSB_TRY(h->res.alloc(&h->d_rposes, 4 * (size_t)h->max_nodes));
+      OSB_TRY(h->res.alloc(&h->d_tsummary, 1));
+      OSB_TRY(h->res.event(&h->ev_done));
+      tail_layout(h->tail, h->d_tail, h->max_nodes, h->max_factors);
+    }
+    OSB_TRY(flush_resident_factors(h));
+    cudaStream_t hs = h->stream;
+    GraphTables t;
+    ChainPlan plan;
+    if (h->tail_topo != h->g_topo_version) {   // the resident plan and its base-only tables
+      build_chain_plan((int)n, h->g_fixed.data(), (int)m_base, h->g_type.data(), h->g_ia.data(), h->g_ib.data(),
+                       h->g_payload.data(), plan);
+      build_tables((int)n, h->g_fixed.data(), (int)m_base, h->g_type.data(), h->g_ia.data(), h->g_ib.data(),
+                   h->g_payload.data(), plan, t);
+      const TailDev& D = h->tail;
+      const size_t i4 = sizeof(int32_t);
+      OSB_CUDA(cudaMemcpyAsync((void*)D.inv, plan.inv.data(), n * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.order, plan.order.data(), n * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_ia, t.ia.data(), m_base * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_ib, t.ib.data(), m_base * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_ptr, t.ptr.data(), (n + 1) * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_slot_a, t.slot_a.data(), m_base * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_slot_b, t.slot_b.data(), m_base * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_es_ptr, t.es_ptr.data(), (n + 1) * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_es_slot, t.es_slot.data(), m_base * i4, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_fixed, t.fixed.data(), n, cudaMemcpyHostToDevice, hs));
+      OSB_CUDA(cudaMemcpyAsync((void*)D.b_link, plan.link.data(), n, cudaMemcpyHostToDevice, hs));
+      h->tail_order = plan.order;
+      h->tail_nres = t.n_res;
+      h->tail_topo = h->g_topo_version;
+    }
+    if (!h->rposes_current) {
+      OSB_CUDA(cudaMemcpyAsync(h->d_rposes, h->g_poses.data(), 4 * n * sizeof(double), cudaMemcpyHostToDevice, hs));
+      h->rposes_current = true;
+    }
+    if (shape_key != h->tail_shape_key) {
+      OSB_TRY(solve_shape(h, (int)n, m_bound, o, h->tail_shape));
+      h->tail_shape_key = shape_key;
+    }
+    OSB_CUDA(cudaStreamSynchronize(hs));       // the staging vectors above die here; the caller's stream comes after
+  }
+  const SolveShape& shape = h->tail_shape;
+  SolverDev P = graph_dev(h, (int)n, m_bound, o);
+  trial_layout(P, h->d_arena, n, m_bound, shape);
+  P.summary = h->d_tsummary;
+  P.dev_word = h->tail.word;
+  TailDev D = h->tail;
+  D.n = (int)n; D.m_base = (int)m_base; D.max_tail = max_tail; D.ctas = shape.ctas;
+  D.chunks = std::max(1, cdiv(max_tail, TL_ROWS));
+  D.count = count_dev; D.type = type_dev; D.ia = ia_dev; D.ib = ib_dev; D.payload = payload_dev; D.huber = huber_dev;
+  D.ia_o = h->d_ia; D.ib_o = h->d_ib; D.ptr_o = h->d_ptr; D.slot_a_o = h->d_slot_a; D.slot_b_o = h->d_slot_b;
+  D.es_ptr_o = h->d_es_ptr; D.es_slot_o = h->d_es_slot; D.type_o = h->d_type; D.payload_o = h->d_payload;
+  D.huber_o = h->d_huber; D.fixed_o = h->d_fixed; D.link_o = h->d_link;
+  D.poses = h->d_rposes; D.x0 = P.x[0]; D.x_out = P.poses_out;
+  h->cached_topo = 0;                          // the one-shot index tables now hold this call's list
+  OSB_LAUNCH(tail_rank_kernel, D.chunks, 2 * TL_ROWS, 0, st, D);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(tail_scan_kernel, cdiv((int)n, 256), 256, 0, st, D);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(tail_ptr_kernel, 1, 1024, 0, st, D);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(tail_tables_kernel, cdiv(std::max(m_bound, (int)n), 256), 256, 0, st, D);
+  OSB_CHECK_LAUNCH();
+  if (!capturing) OSB_CUDA(cudaEventRecord(h->ev0, st));
+  OSB_TRY(launch_solves(h, P, shape, 1, 0, st, true));
+  if (!capturing) OSB_CUDA(cudaEventRecord(h->ev1, st));
+  OSB_LAUNCH(tail_poses_out_kernel, cdiv((int)n, 256), 256, 0, st, D);
+  OSB_CHECK_LAUNCH();
+  if (!capturing) OSB_CUDA(cudaEventRecord(h->ev_done, st));
+  h->dev_pending = true; h->dev_captured = capturing; h->dev_called = true;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_solver_last_summary(osb_solver* h, osb_solve_summary* summary) {
+  OSB_REQUIRE(h != nullptr && summary != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
+  OSB_REQUIRE(h->dev_called, "no osb_solver_solve_resident_dev call on this handle");
+  if (h->dev_status != OSB_OK) {
+    set_error("osb_solver_last_summary", h->dev_status == OSB_ERR_CAPACITY
+              ? "the device call was refused: *count_dev > max_tail"
+              : "the device call was refused: a tail row has an unknown type or a bad node id, or *count_dev < 0");
+    return h->dev_status;
+  }
+  *summary = h->dev_summary;
+  return OSB_OK;
 }
 
 extern "C" osb_status osb_solver_phase_cycles(osb_solver* h, double* out12) {
   OSB_REQUIRE(h != nullptr && out12 != nullptr, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   long long c[8];
   OSB_CUDA(cudaMemcpy(c, h->d_dbg, sizeof(c), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 8; ++i) out12[i] = (double)c[i];
@@ -1714,6 +2168,7 @@ extern "C" osb_status osb_solver_chain_cycles(osb_solver* h, double* out128) {
   OSB_REQUIRE(h != nullptr && out128 != nullptr, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   long long c[128];
   OSB_CUDA(cudaMemcpy(c, h->d_dbg + 8, sizeof(c), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 128; ++i) out128[i] = (double)c[i];
@@ -1730,6 +2185,7 @@ extern "C" osb_status osb_solver_linearize(osb_solver* h, int n_nodes, const dou
   if (s != OSB_OK) return s;
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
   h->g_static_valid = false;              // as osb_solver_solve: the device factor arrays and tables now hold this graph
   h->cached_topo = 0;
   const size_t n = n_nodes, m = n_factors;

@@ -347,6 +347,22 @@ class PoseGraphSolver(_Handle):
         _l.check(self._lib.osb_solver_solve_resident(self._h, C.byref(opt), C.byref(summ)))
         return summ
 
+    def solve_resident_dev(self, max_tail: int, type_ptr: int, ia_ptr: int, ib_ptr: int, payload_ptr: int,
+                           huber_ptr: int, count_ptr: int, stream: int, options: _l.SolveOptions | None = None):
+        """solve the resident graph plus *count_ptr tail rows read on the device (compact_anchored_factors' arrays), on
+        `stream` without synchronising; the poses stay on the device until a host-side call (see last_summary)"""
+        opt = options if options is not None else self.default_options()
+        _l.check(self._lib.osb_solver_solve_resident_dev(self._h, int(max_tail), C.c_void_p(type_ptr), C.c_void_p(ia_ptr),
+                                                         C.c_void_p(ib_ptr), C.c_void_p(payload_ptr),
+                                                         C.c_void_p(huber_ptr), C.c_void_p(count_ptr), C.byref(opt),
+                                                         C.c_void_p(stream)))
+
+    def last_summary(self) -> _l.SolveSummary:
+        """synchronises with the last solve_resident_dev call -> its summary (raises its refusal code)"""
+        summ = _l.SolveSummary()
+        _l.check(self._lib.osb_solver_last_summary(self._h, C.byref(summ)))
+        return summ
+
     def phase_cycles(self) -> dict:
         c = np.zeros(12, np.float64)
         _l.check(self._lib.osb_solver_phase_cycles(self._h, _l.ptr(c)))

@@ -230,6 +230,8 @@ _SIG = {
     "osb_solver_graph_size": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "osb_solver_graph_drop_oldest": (C.c_int, [_P, C.c_int]),
     "osb_solver_solve_resident": (C.c_int, [_P, _P, _P]),
+    "osb_solver_solve_resident_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "osb_solver_last_summary": (C.c_int, [_P, _P]),
     "osb_solver_phase_cycles": (C.c_int, [_P, _P]),
     "osb_solver_chain_cycles": (C.c_int, [_P, _P]),
     "osb_solver_chain_plan": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
