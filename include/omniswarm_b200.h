@@ -99,6 +99,12 @@ osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int n);
 #define OSB_PRECISION_SPLIT_FP16 0
 #define OSB_PRECISION_FP16 1
 osb_status osb_superpoint_set_precision(osb_superpoint* h, int precision);
+/* Geometry of the blanked band (tests only; no device needed): for images of height x width whose rows >= zero_row are
+ * zero, the front-end's SuperPoint skips the trunk's (conv1a .. conv4b) tiles whose output is the layer's constant.
+ * out [68] int32: for each trunk layer l, out[8l .. 8l+3] = its constant output pixels (after the pool) and
+ * out[8l+4 .. 8l+7] = its constant 8 x 16 output tiles (before the pool), each as y0, y1, x0, x1 of [y0, y1) x [x0, x1);
+ * out[64 .. 67] = the conv1a pixels that no computed conv1b tile reads.  An empty set has y0 >= y1 or x0 >= x1. */
+osb_status osb_superpoint_band_geometry(int height, int width, int zero_row, int32_t* out);
 
 /* Convolution parity hooks (tests only): ONE layer of the tensor-core path, run by the same host functions and kernels
  * as the SuperPoint / NetVLAD networks, on caller-supplied operands.  Weights and biases are HOST fp32, OIHW; activation

@@ -125,7 +125,48 @@ struct UmmaArgs {
   int n_split;             // a layer wider than the kernel's N runs as n_split work items per tile (N channels each)
   int epi;                 // 0: bias/act/pool + store; 1: detector head -- softmax over 65 logits, drop the dustbin,
                            //    8x8 pixel shuffle straight into the heat map `out_f32` ([B][8H][8W])
+  TileRect band;           // BAND kernels: these tiles of every image are stored as the constant band_hi / band_lo
+  const __half* band_hi;   // [out_c] each
+  const __half* band_lo;
 };
+
+// BAND kernels: the launch's work items are the tiles outside the band, compacted in tile order; image b's items follow
+// image b - 1's.  Producer and consumers map an item to its tile here.
+__device__ __forceinline__ int band_tile(int item, int tiles_x, int tiles_y, const UmmaArgs& P) {
+  const int bh = P.band.y1 - P.band.y0, bw = P.band.x1 - P.band.x0, m = tiles_x - bw;   // m: computed tiles per band row
+  const int per = tiles_x * tiles_y - bh * bw;
+  const int b = item / per;
+  int k = item - b * per, t;
+  const int head = P.band.y0 * tiles_x;
+  if (k < head) {
+    t = k;
+  } else if ((k -= head) < bh * m) {
+    const int row = k / m, c = k - row * m;
+    t = (P.band.y0 + row) * tiles_x + (c < P.band.x0 ? c : c + bw);
+  } else {
+    t = P.band.y1 * tiles_x + (k - bh * m);
+  }
+  return b * tiles_x * tiles_y + t;
+}
+
+// BAND kernels: the band's outputs (after the pool, if any), 8 channels of one pixel per 16-byte store of each plane.  The
+// CTAs of the launch share the work; thread t of the CTA's nt filling threads.
+template <bool FP16>
+__device__ void band_fill(const UmmaArgs& P, int t, int nt) {
+  const int sh = P.pool ? 1 : 0;
+  const int Ho = P.H >> sh, Wo = P.W >> sh;
+  const int y0 = (P.band.y0 * UM_TH) >> sh, x0 = (P.band.x0 * UM_TW) >> sh;
+  const int bh = ((P.band.y1 - P.band.y0) * UM_TH) >> sh, bw = ((P.band.x1 - P.band.x0) * UM_TW) >> sh;
+  const int c8 = P.out_c / 8, total = P.B * bh * bw * c8;              // < 2^31: checked on the host
+  const uint4* chi = reinterpret_cast<const uint4*>(P.band_hi);
+  const uint4* clo = reinterpret_cast<const uint4*>(P.band_lo);
+  for (int e = blockIdx.x * nt + t; e < total; e += gridDim.x * nt) {
+    const int c = e % c8, p = e / c8, x = p % bw, y = (p / bw) % bh, b = p / (bw * bh);
+    const size_t o = (((size_t)b * Ho + y0 + y) * Wo + x0 + x) * P.out_cstride + P.n_off + 8 * c;
+    *reinterpret_cast<uint4*>(P.out_hi + o) = __ldg(chi + c);
+    if constexpr (!FP16) *reinterpret_cast<uint4*>(P.out_lo + o) = __ldg(clo + c);
+  }
+}
 
 // 4 x 4 transpose of 32-bit words across the four lanes of a quad (t4 = lane % 4): on return v[k] is the word v[t4] of
 // quad lane k.  Round r takes word (t4 - r) % 4 from lane (t4 + r) % 4; all indices stay compile-time after unrolling.
@@ -545,7 +586,9 @@ __device__ __forceinline__ void tr_epilogue(const float (&acc)[64], const float 
   }
 }
 
-template <bool FP16 = false>
+// BAND: the tiles of P.band are not computed: the items are the other tiles (band_tile), and producer warps 1-3, idle
+// otherwise, store the band's constant (band_fill) while the MMAs run.
+template <bool FP16 = false, bool BAND = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
@@ -562,7 +605,8 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 
   const int lane = threadIdx.x & 31;
   const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
-  const int n_tiles = P.B * tiles_x * tiles_y;
+  const int n_tiles = P.B * (tiles_x * tiles_y - (BAND ? (P.band.y1 - P.band.y0) * (P.band.x1 - P.band.x0) : 0));
+  auto tile_of = [&](int item) { return BAND ? band_tile(item, tiles_x, tiles_y, P) : item; };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < AS; ++s) { mbar_init(a_full(0, s), 1); mbar_init(a_full(1, s), 1); mbar_init(a_empty(s), 1); }
@@ -586,9 +630,11 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    if constexpr (BAND) if (pt >= 32) band_fill<FP16>(P, pt - 32, 96);
     if (pt < 32 && elect_one()) {
       int as = 0; uint32_t aph = 0;
-      for (int i = 0, tile = blockIdx.x; tile < n_tiles; ++i, tile += gridDim.x) {
+      for (int i = 0, item = blockIdx.x; item < n_tiles; ++i, item += gridDim.x) {
+        const int tile = tile_of(item);
         const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
         const int x0 = tx * UM_TW, y0 = ty * UM_TH;
         for (int kx = 0; kx < 3; ++kx) {
@@ -611,7 +657,8 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     for (int t = 0; t < 9; ++t) mbar_wait(w_full(t), 0);
     const float bias[2] = {__ldg(P.bias + P.n_off + 16 * w + r), __ldg(P.bias + P.n_off + 16 * w + 8 + r)};
     uint32_t fph = 0;                                        // bit s: parity of this warpgroup's next box in slot s
-    for (int i = g, tile = blockIdx.x + g * gridDim.x; tile < n_tiles; i += 2, tile += 2 * gridDim.x) {
+    for (int i = g, item = blockIdx.x + g * gridDim.x; item < n_tiles; i += 2, item += 2 * gridDim.x) {
+      const int tile = tile_of(item);
       // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo.  fp16: main only
       float acc[64], cross[FP16 ? 1 : 64];
 #pragma unroll
@@ -672,7 +719,8 @@ conv_res64_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 // Skew: warpgroup 1 starts once warpgroup 0 has issued the MMAs of its first box.  From then on the two run a box apart,
 // so that each one's epilogue overlaps the other's MMAs instead of leaving the tensor pipe idle.
 // FP16: one wgmma W_hi*X_hi per K step on hi-only boxes and W_hi-only half slots; tm_a_lo / tm_w_lo are not used.
-template <bool SPLIT, bool FP16 = false>
+// BAND (not with SPLIT): the tiles of P.band are not computed (conv_res64_kernel); producer warp 3 stores their constant.
+template <bool SPLIT, bool FP16 = false, bool BAND = false>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_stream_t_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                      const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, UmmaArgs P) {
@@ -690,8 +738,11 @@ conv_stream_t_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_c
   const int lane = threadIdx.x & 31;
   const int tiles_x = (P.W + UM_TW - 1) / UM_TW, tiles_y = (P.H + UM_TH - 1) / UM_TH;
   // work item = (tile, 128-channel block): items of one tile are adjacent, so concurrent CTAs share its activations in L2
+  static_assert(!(SPLIT && BAND), "a band is not taken by the layers of more than 128 channels");
   const int n_split = SPLIT ? P.n_split : 1;          // compile-time 1 for ordinary layers: no div / mod per item
-  const int n_items = P.B * tiles_x * tiles_y * n_split;
+  const int n_items =
+      P.B * (tiles_x * tiles_y - (BAND ? (P.band.y1 - P.band.y0) * (P.band.x1 - P.band.x0) : 0)) * n_split;
+  auto tile_of = [&](int item) { return SPLIT ? item / n_split : BAND ? band_tile(item, tiles_x, tiles_y, P) : item; };
   const int halo = P.ks / 2;
   const uint32_t a_box_bytes = (uint32_t)(UM_TH + 2 * halo) * UM_ROW;   // bytes of one A plane box
 
@@ -707,11 +758,12 @@ conv_stream_t_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_c
     const int pw = (threadIdx.x - UM_CONSUMERS) >> 5;      // producer warp: 0 A boxes, 1 + g weight rows of warpgroup g
     setmaxnreg_dec<UM_PRODUCER_REGS>();
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    if constexpr (BAND) if (pw == 3) band_fill<FP16>(P, lane, 32);
     if (pw < 3 && elect_one()) {
       const int g = pw - 1;
       int s = 0; uint32_t ph = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
+        const int tile = tile_of(item), n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
         const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
         for (int kx = 0; kx < P.ks; ++kx) {
           for (int cs = 0; cs < P.cin_slabs; ++cs) {
@@ -757,7 +809,7 @@ conv_stream_t_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_c
     int as = 0; uint32_t aph = 0;
     int ws = 0; uint32_t wph = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int tile = SPLIT ? item / n_split : item, n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
+      const int tile = tile_of(item), n_off = SPLIT ? P.n_off + (item % n_split) * 128 : P.n_off;
       const int c_abs = n_off + 64 * g;
       const float bias[2] = {__ldg(P.bias + c_abs + 16 * w + r), __ldg(P.bias + c_abs + 16 * w + 8 + r)};
       // disjoint fragments (64 registers each): main = hi*hi, cross = lo*hi + hi*lo.  fp16: main only
@@ -838,15 +890,17 @@ __device__ __forceinline__ void split_store8(__half* hi, __half* lo, const float
 // once per CTA in shared memory and slide down the column through registers (3 broadcast LDS per pixel instead of one
 // LDS per FMA pair), and the 8 threads of a pixel write its 128-byte channel vector as eight adjacent 16-byte chunks --
 // a warp stores 4 pixels x 128 B contiguously per plane, no staging of the output.  The plane scale (a power of two) is
-// folded into weights and bias, and the 9 taps (ky-major) accumulate onto the bias.
+// folded into weights and bias, and the 9 taps (ky-major) accumulate onto the bias.  The pixels of `skip` (those no
+// computed tile of the next layer reads) are neither computed nor written.
 constexpr int CF_TW = 32, CF_TH = 8;
 template <bool FP16 = false>
 __global__ void __launch_bounds__(256)
 conv_first_split_kernel(const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ lut,
                         const uint8_t* __restrict__ img, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                        int H, int W, float out_scale) {
+                        int H, int W, float out_scale, TileRect skip) {
   __shared__ float sin_[CF_TH + 2][CF_TW + 2];
   const int tid = threadIdx.x, b = blockIdx.z, x0 = blockIdx.x * CF_TW, y0 = blockIdx.y * CF_TH;
+  if (y0 >= skip.y0 && y0 + CF_TH <= skip.y1 && x0 >= skip.x0 && x0 + CF_TW <= skip.x1) return;   // the whole block
   const uint8_t* ib = img + (size_t)b * H * W;
   for (int e = tid; e < (CF_TH + 2) * (CF_TW + 2); e += 256) {
     const int r = e / (CF_TW + 2), c = e % (CF_TW + 2);
@@ -881,7 +935,7 @@ conv_first_split_kernel(const float* __restrict__ w, const float* __restrict__ b
 #pragma unroll
     for (int k = 0; k < 3; ++k) in[2][k] = sin_[r + 2][px + k];
     const int y = y0 + r;
-    if (y < H && x < W) {
+    if (y < H && x < W && !(y >= skip.y0 && y < skip.y1 && x >= skip.x0 && x < skip.x1)) {
       uint32_t h[4], l[4];
 #pragma unroll
       for (int j2 = 0; j2 < 4; ++j2) {
@@ -1006,9 +1060,12 @@ static osb_status launch_persistent(int smem_bytes, const CUtensorMap& a_hi, con
                                     const CUtensorMap& w_hi, const CUtensorMap& w_lo, const UmmaArgs& P, cudaStream_t st,
                                     int max_ctas) {
   OSB_SMEM_OPT_IN(kernel, smem_bytes);
-  const int tiles = P.B * cdiv(P.W, UM_TW) * cdiv(P.H, UM_TH) * P.n_split;
+  // work items: the tiles outside the band.  Every CTA must get one: conv_stream_t_kernel's warpgroup 1 waits for
+  // warpgroup 0 to start its first item
+  const int band_tiles = (P.band.y1 - P.band.y0) * (P.band.x1 - P.band.x0);
+  const int tiles = P.B * (cdiv(P.W, UM_TW) * cdiv(P.H, UM_TH) - (P.band.empty() ? 0 : band_tiles)) * P.n_split;
   // persistent CTAs, one per SM; `max_ctas` leaves SMs free for a kernel running beside this one on another stream
-  const int grid = std::min(tiles, persistent_ctas(max_ctas));
+  const int grid = std::max(1, std::min(tiles, persistent_ctas(max_ctas)));
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   cfg.gridDim = dim3(grid); cfg.blockDim = dim3(UM_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
@@ -1027,14 +1084,46 @@ static osb_status launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, 
                                                       max_ctas);
 }
 
-template <bool SPLIT, bool FP16>
+template <bool SPLIT, bool FP16, bool BAND = false>
 static osb_status launch_stream_t(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const UmmaLayer& L, const UmmaArgs& P,
                                   cudaStream_t st, int max_ctas) {
-  return launch_persistent<conv_stream_t_kernel<SPLIT, FP16>>(StreamTCfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo,
-                                                              P, st, max_ctas);
+  return launch_persistent<conv_stream_t_kernel<SPLIT, FP16, BAND>>(StreamTCfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi,
+                                                                    L.tm_lo, P, st, max_ctas);
 }
 
 static bool precision_fp16(int precision) { return precision == OSB_PRECISION_FP16; }
+
+void band_geometry(int H, int W, int r0, const BandLayer* layers, int n, TileRect* px, TileRect* tiles,
+                   TileRect* first_skip) {
+  // the constant input of the first layer: the zero rows
+  TileRect in;
+  if (r0 >= 0 && r0 < H) in = TileRect{r0, H, 0, W};
+  int h = H, w = W;
+  for (int l = 0; l < n; ++l) {
+    const int halo = layers[l].ks / 2;
+    // outputs whose window lies in the image and in the constant input
+    TileRect o{std::max(in.y0 + halo, halo), std::min(in.y1 - halo, h - halo), std::max(in.x0 + halo, halo),
+               std::min(in.x1 - halo, w - halo)};
+    if (in.empty() || o.empty()) o = TileRect{};
+    TileRect t{cdiv(o.y0, UM_TH), o.y1 / UM_TH, cdiv(o.x0, UM_TW), o.x1 / UM_TW};     // tiles inside o (never ragged)
+    tiles[l] = (o.empty() || t.empty()) ? TileRect{} : t;
+    if (layers[l].pool) {
+      // a pooled pixel is constant when its whole 2 x 2 window is
+      o = TileRect{cdiv(o.y0, 2), o.y1 / 2, cdiv(o.x0, 2), o.x1 / 2};
+      if (o.empty()) o = TileRect{};
+      h /= 2; w /= 2;
+    }
+    px[l] = in = o;
+  }
+  // a computed tile of the second layer reads its rows and columns plus the halo
+  *first_skip = TileRect{};
+  if (n > 1 && !tiles[1].empty()) {
+    const int halo = layers[1].ks / 2;
+    const TileRect& t = tiles[1];
+    const TileRect s{t.y0 * UM_TH + halo, t.y1 * UM_TH - halo, t.x0 * UM_TW + halo, t.x1 * UM_TW - halo};
+    if (!s.empty()) *first_skip = s;
+  }
+}
 
 // the arguments that follow from the layer and its input; the caller adds the output and the epilogue
 static UmmaArgs umma_args(const UmmaLayer& L, int B, int H, int W, float act_scale) {
@@ -1047,14 +1136,24 @@ static UmmaArgs umma_args(const UmmaLayer& L, int B, int H, int W, float act_sca
 template <bool FP16>
 static osb_status umma_conv_launch(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, UmmaArgs& P,
                                    cudaStream_t st, int max_ctas) {
+  const bool band = !P.band.empty();
+  const bool res64 = L.n_pad == 64 && L.ks == 3 && L.cin == UM_KC;
+  // conv_umma_kernel and the split layers have no band form
+  OSB_REQUIRE(!band || res64 || L.n_pad == 128, "a constant band needs a 64 -> 64 3x3 or a 128-channel layer");
   switch (L.n_pad) {
     case 64:
-      if (L.ks == 3 && L.cin == UM_KC)            // weights resident, transposed GEMM
+      if (res64) {                                // weights resident, transposed GEMM
+        if (band)
+          return launch_persistent<conv_res64_kernel<FP16, true>>(R64Cfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo,
+                                                                  P, st, max_ctas);
         return launch_persistent<conv_res64_kernel<FP16>>(R64Cfg<FP16>::SMEM_BYTES, a_hi, a_lo, L.tm_hi, L.tm_lo, P, st,
                                                           max_ctas);
+      }
       return launch_umma<64, FP16>(a_hi, a_lo, L, P, st, max_ctas);
     case 80: return launch_umma<80, FP16>(a_hi, a_lo, L, P, st, max_ctas);
-    case 128: return launch_stream_t<false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
+    case 128:
+      if (band) return launch_stream_t<false, FP16, true>(a_hi, a_lo, L, P, st, max_ctas);
+      return launch_stream_t<false, FP16>(a_hi, a_lo, L, P, st, max_ctas);
     case 256:                                     // 2 / 4 items of 128 channels per tile (a 256-wide accumulator pair
     case 512:                                     // would not fit a warpgroup's registers)
       P.n_split = L.n_pad / 128;
@@ -1066,12 +1165,21 @@ static osb_status umma_conv_launch(const UmmaLayer& L, const CUtensorMap& a_hi, 
 
 osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                              float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
-                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas, int precision) {
+                             float out_scale, int relu, int pool, cudaStream_t st, int max_ctas, int precision,
+                             const ConvBand* band) {
   OSB_REQUIRE(!pool || (H % 2 == 0 && W % 2 == 0), "fused max-pool needs even H and W");
   OSB_REQUIRE(out_c % 16 == 0 && out_c <= L.n_pad && out_cstride % 8 == 0, "tensor-core conv: bad output channel layout");
   UmmaArgs P = umma_args(L, B, H, W, act_scale);
   P.out_hi = out_hi; P.out_lo = out_lo; P.out_f32 = out_f32; P.out_c = out_c; P.out_cstride = out_cstride;
   P.out_scale = out_scale; P.relu = relu; P.pool = pool;
+  if (band && !band->tiles.empty()) {
+    const TileRect& t = band->tiles;
+    OSB_REQUIRE(out_hi && !out_f32 && band->hi && (band->lo || precision_fp16(precision)),
+                "a constant band is stored into split planes");
+    OSB_REQUIRE(t.y0 >= 0 && t.x0 >= 0 && t.y1 * UM_TH <= H && t.x1 * UM_TW <= W, "band tiles outside the image");
+    OSB_REQUIRE((int64_t)B * t.y1 * UM_TH * t.x1 * UM_TW * (out_c / 8) < INT32_MAX, "band too large");
+    P.band = t; P.band_hi = band->hi; P.band_lo = band->lo;
+  }
   return precision_fp16(precision) ? umma_conv_launch<true>(L, a_hi, a_lo, P, st, max_ctas)
                                    : umma_conv_launch<false>(L, a_hi, a_lo, P, st, max_ctas);
 }
@@ -1214,10 +1322,10 @@ osb_status umma_dwconv_forward(const float* w_tap_c, const float* bias, const fl
 
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
                               __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st,
-                              int precision) {
+                              int precision, TileRect skip) {
   dim3 grid(cdiv(W, CF_TW), cdiv(H, CF_TH), B);
   const auto kernel = precision_fp16(precision) ? conv_first_split_kernel<true> : conv_first_split_kernel<false>;
-  OSB_LAUNCH(kernel, grid, 256, 0, st, w_tap_cout, bias, lut, img, out_hi, out_lo, H, W, out_scale);
+  OSB_LAUNCH(kernel, grid, 256, 0, st, w_tap_cout, bias, lut, img, out_hi, out_lo, H, W, out_scale, skip);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

@@ -20,6 +20,28 @@ struct UmmaLayer {
   CUtensorMap tm_hi, tm_lo;           // boxes of 64 rows (80 for the 80-row detector head)
 };
 
+// Blanked band: when every image of a batch is zero from row r0 down, an output pixel whose receptive field lies in the
+// zero rows and touches no padding has the same value everywhere: the layer's constant.  A tile whose 8 x 16 outputs are
+// all such pixels is not computed; it receives the constant as plain stores.
+struct TileRect {                     // [y0, y1) x [x0, x1)
+  int y0 = 0, y1 = 0, x0 = 0, x1 = 0;
+  bool empty() const { return y0 >= y1 || x0 >= x1; }
+};
+struct BandLayer { int ks, pool; };   // a layer of a chain: kernel size, fused 2x2 max-pool of its output
+// The chain's first layer reads the H x W images, each later one the previous one's output.  For every layer: px[l], its
+// output pixels (after the pool) that equal the layer's constant, and tiles[l], its 8 x 16 output tiles (before the pool)
+// that are constant throughout.  first_skip: the first layer's output pixels that only constant tiles of the second read.
+// A pixel counts as constant only when its whole window lies inside the image and inside the constant input (the zero
+// rows for the first layer), so padding never enters; ragged tiles never qualify.
+void band_geometry(int H, int W, int r0, const BandLayer* layers, int n, TileRect* px, TileRect* tiles,
+                   TileRect* first_skip);
+// the constant tiles of one launch and the layer's constant output (out_c channels per plane; lo unused in plain fp16)
+struct ConvBand {
+  TileRect tiles;
+  const __half* hi = nullptr;
+  const __half* lo = nullptr;
+};
+
 // the weight planes and bias belong to `res`
 osb_status umma_layer_upload(Resources& res, UmmaLayer* L, const float* w_oihw, const float* bias, int cin, int cout,
                              int ks, float w_scale);
@@ -30,16 +52,18 @@ osb_status umma_act_maps(CUtensorMap* hi, CUtensorMap* lo, __half* p_hi, __half*
 // output either as split fp16 planes (out_hi/out_lo, scaled by out_scale) or as fp32.
 // precision (these four functions): OSB_PRECISION_SPLIT_FP16 (default) reads and writes both planes, OSB_PRECISION_FP16
 // only the hi planes (one MMA per K step; out_lo and the lo input planes are not touched).  The weights are the same.
+// band (optional): tiles of every image that are stored as its constant instead of computed; only the 64 -> 64 3x3 and the
+// 128-channel layers take one, with split planes as output.
 osb_status umma_conv_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                              float act_scale, __half* out_hi, __half* out_lo, float* out_f32, int out_c, int out_cstride,
                              float out_scale, int relu, int pool, cudaStream_t st, int max_ctas = 0,
-                             int precision = OSB_PRECISION_SPLIT_FP16);
+                             int precision = OSB_PRECISION_SPLIT_FP16, const ConvBand* band = nullptr);
 osb_status umma_conv_softmax_forward(const UmmaLayer& L, const CUtensorMap& a_hi, const CUtensorMap& a_lo, int B, int H, int W,
                                      float act_scale, float* semi, cudaStream_t st, int max_ctas = 0,
                                      int precision = OSB_PRECISION_SPLIT_FP16);
 osb_status umma_first_forward(const float* w_tap_cout, const float* bias, const float* lut, const uint8_t* img,
                               __half* out_hi, __half* out_lo, int B, int H, int W, float out_scale, cudaStream_t st,
-                              int precision = OSB_PRECISION_SPLIT_FP16);
+                              int precision = OSB_PRECISION_SPLIT_FP16, TileRect skip = {});   // skip: pixels not written
 osb_status umma_make_tmap(CUtensorMap* tm, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
 // depthwise 3x3 + bias + ReLU6, fp32 NHWC in, split fp16 planes out (feeds a pointwise tensor-core conv).  Stride 1 runs

@@ -14,6 +14,55 @@ static const int SP_KS[12] = {3, 3, 3, 3, 3, 3, 3, 3, 3, 1, 3, 1};
 // power-of-two scales of the split-fp16 planes (exact): activations (post-ReLU, O(1)) x 16, weights (O(0.05)) x 1024
 constexpr float SP_ACT_SCALE = 16.f;
 constexpr float SP_W_SCALE = 1024.f;
+// the trunk conv1a .. conv4b as the chain of band_geometry (trunk layer i is layer i above); the layers after it read
+// conv4b's output, which no geometry the front-end runs leaves a constant tile in
+constexpr int SP_TRUNK = 8;
+static const BandLayer SP_TRUNK_LAYERS[SP_TRUNK] = {{3, 0}, {3, 1}, {3, 0}, {3, 1}, {3, 0}, {3, 1}, {3, 0}, {3, 0}};
+constexpr int SP_BAND_C = 128;         // channel stride of band_c (the widest trunk layer)
+
+static void sp_band_geometry(int H, int W, int zero_row, TileRect* px, TileRect* tiles, TileRect* first_skip) {
+  band_geometry(H, W, zero_row, SP_TRUNK_LAYERS, SP_TRUNK, px, tiles, first_skip);
+}
+
+static size_t band_offset(int prec, int layer, int plane) {
+  const int p = prec == OSB_PRECISION_FP16 ? 1 : 0;
+  return ((size_t)(p * SP_TRUNK + layer) * 2 + plane) * SP_BAND_C;
+}
+
+const __half* SuperPoint::band_const(int prec, int layer, int plane) const {
+  return band_c + band_offset(prec, layer, plane);
+}
+
+// Every trunk layer's constant from its own kernel: a zero image (one, of the handle's size) through conv1a .. conv4b with
+// nothing skipped, and the output pixel of each layer read off inside its constant region (band_geometry with zero_row
+// 0).  Interior pixels run the same K order, accumulators and epilogue wherever they sit, so the pixel is bit-exact for
+// every constant tile of that layer.
+osb_status SuperPoint::band_init() {
+  if (!use_umma || band_c) return OSB_OK;
+  TileRect px[SP_TRUNK], tiles[SP_TRUNK], skip;
+  sp_band_geometry(H, W, 0, px, tiles, &skip);
+  __half* c = nullptr;
+  OSB_TRY(res.alloc(&c, (size_t)2 * SP_TRUNK * 2 * SP_BAND_C));
+  OSB_CUDA(cudaMemsetAsync(d_img, 0, (size_t)H * W, stream));
+  for (const int prec : {OSB_PRECISION_SPLIT_FP16, OSB_PRECISION_FP16}) {
+    OSB_TRY(umma_first_forward(w1a, b1a, lut, d_img, in_hi[1], in_lo[1], 1, H, W, SP_ACT_SCALE, stream, prec));
+    int h = H, w = W;
+    for (int i = 1; i < SP_TRUNK; ++i) {
+      const int pool = SP_TRUNK_LAYERS[i].pool;
+      OSB_TRY(umma_conv_forward(UL[i], tmA[i], tmB[i], 1, h, w, SP_ACT_SCALE, in_hi[i + 1], in_lo[i + 1], nullptr,
+                                SP_COUT[i], SP_COUT[i], SP_ACT_SCALE, 1, pool, stream, 0, prec));
+      if (pool) { h /= 2; w /= 2; }
+      if (px[i].empty()) continue;                   // then no geometry of this size has a constant tile here
+      const size_t at = ((size_t)px[i].y0 * w + px[i].x0) * SP_COUT[i], bytes = SP_COUT[i] * sizeof(__half);
+      OSB_CUDA(cudaMemcpyAsync(c + band_offset(prec, i, 0), in_hi[i + 1] + at, bytes, cudaMemcpyDeviceToDevice, stream));
+      if (prec == OSB_PRECISION_SPLIT_FP16)
+        OSB_CUDA(cudaMemcpyAsync(c + band_offset(prec, i, 1), in_lo[i + 1] + at, bytes, cudaMemcpyDeviceToDevice, stream));
+    }
+  }
+  OSB_CUDA(cudaStreamSynchronize(stream));
+  band_c = c;
+  return OSB_OK;
+}
 
 size_t sp_expected_weights() {
   size_t n = 0;
@@ -117,17 +166,25 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
 
 // tensor-core network: every activation is a pair of fp16 planes (hi, lo) scaled by SP_ACT_SCALE; the planes of a
 // layer's output live in the ping-pong buffer the next layer's TMA descriptors point at.
-osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp) {
+osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp, int zero_row) {
   const float SA = SP_ACT_SCALE;
   n_lev = 0;
   mark(st);
+  // blanked band: the trunk's constant tiles are stored, not computed, and conv1a skips the pixels only they would read
+  TileRect band_px[SP_TRUNK], band_tiles[SP_TRUNK], first_skip;
+  const bool banded = zero_row >= 0 && band_c;
+  if (banded) sp_band_geometry(H, W, zero_row, band_px, band_tiles, &first_skip);
   // conv layer i at resolution h x w; its output (optionally 2x2 max-pooled in the epilogue) becomes the input planes
   // of layer `out_layer`
   auto conv = [&](int i, int h, int w, int out_layer, int pool) {
+    ConvBand band;
+    if (banded && i < SP_TRUNK)
+      band = ConvBand{band_tiles[i], band_const(precision, i, 0), band_const(precision, i, 1)};
     return umma_conv_forward(UL[i], tmA[i], tmB[i], B, h, w, SA, in_hi[out_layer], in_lo[out_layer], nullptr,
-                             SP_COUT[i], SP_COUT[i], SA, 1, pool, st, 0, precision);
+                             SP_COUT[i], SP_COUT[i], SA, 1, pool, st, 0, precision, &band);
   };
-  OSB_TRY(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st, precision));   // conv1a -> A
+  OSB_TRY(umma_first_forward(w1a, b1a, lut, img_dev, in_hi[1], in_lo[1], B, H, W, SA, st, precision,
+                             banded ? first_skip : TileRect{}));                               // conv1a -> A
   mark(st);
   OSB_TRY(conv(1, H, W, 2, 1));                                                               // conv1b + pool     -> B
   mark(st);
@@ -177,8 +234,8 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
 }
 
 // the network: u8 images (device) -> d_semi, d_desc
-osb_status SuperPoint::network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp) {
-  if (use_umma) return network_umma(img_dev, B, st, kp);
+osb_status SuperPoint::network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp, int zero_row) {
+  if (use_umma) return network_umma(img_dev, B, st, kp, zero_row);
   OSB_TRY(conv_first_forward(w1a, b1a, lut, img_dev, actA, B, H, W, 64, 1, ACT_RELU, st));  // conv1a
   OSB_TRY(conv_forward(L[1], actA, actB, B, H, W, 64, ACT_RELU, st));                        // conv1b
   OSB_TRY(maxpool2x2_forward(actB, actA, B, H, W, 64, st));
@@ -331,6 +388,17 @@ extern "C" osb_status osb_superpoint_layer_ms(osb_superpoint* h, float* ms, int 
     float t = 0.f;
     if (cudaEventElapsedTime(&t, sp.lev[i], sp.lev[i + 1]) == cudaSuccess) ms[i] = t; else cudaGetLastError();
   }
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_superpoint_band_geometry(int height, int width, int zero_row, int32_t* out) {
+  OSB_REQUIRE(out != nullptr, "null out");
+  OSB_REQUIRE(height > 0 && width > 0 && height % 8 == 0 && width % 8 == 0, "width/height must be multiples of 8");
+  TileRect px[SP_TRUNK], tiles[SP_TRUNK], skip;
+  sp_band_geometry(height, width, zero_row, px, tiles, &skip);
+  auto put = [&](int32_t* o, const TileRect& r) { o[0] = r.y0; o[1] = r.y1; o[2] = r.x0; o[3] = r.x1; };
+  for (int l = 0; l < SP_TRUNK; ++l) { put(out + 8 * l, px[l]); put(out + 8 * l + 4, tiles[l]); }
+  put(out + 8 * SP_TRUNK, skip);
   return OSB_OK;
 }
 

@@ -40,6 +40,12 @@ struct SuperPoint {
   UmmaLayer UL[12];
   CUtensorMap tmA[12], tmB[12];     // [layer] -> (hi, lo) descriptors of that layer's INPUT planes
   __half *in_hi[12] = {}, *in_lo[12] = {};
+  // blanked band (network's zero_row): per precision and trunk layer (conv1a .. conv4b), the hi and lo planes of the
+  // layer's constant output, 128 channels apart.  Null until band_init; while it is null, network ignores zero_row.
+  __half* band_c = nullptr;
+  const __half* band_const(int prec, int layer, int plane) const;
+  // computes band_c with each layer's own kernel on a zero image (both precisions); synchronizes `stream`
+  osb_status band_init();
   // per-layer timing (debug / bench): ev[i] is recorded after launch i of the network when `layer_prof` is set
   bool layer_prof = false;
   cudaEvent_t lev[20] = {};
@@ -56,8 +62,10 @@ struct SuperPoint {
   cudaEvent_t ev_semi = nullptr, ev_kp = nullptr;
   bool overlap_kp = true;
   bool fused_softmax = true;       // detector-head softmax + pixel shuffle in convPb's epilogue (OSB_SP_FUSED_SOFTMAX=0: two kernels)
-  osb_status network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp = nullptr);
-  osb_status network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp);
+  // zero_row >= 0: rows zero_row .. H - 1 of every image are zero, so the tensor-core trunk skips the tiles whose output is
+  // the layer's constant (after band_init; DESIGN.md section 3)
+  osb_status network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp = nullptr, int zero_row = -1);
+  osb_status network_umma(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp, int zero_row);
   osb_status keypoints(int B, const KpJob& kp, cudaStream_t st);
   osb_status descriptors(int B, const KpJob& kp, float* out, cudaStream_t st);
   // network + keypoints + descriptors (what inference() is)

@@ -126,6 +126,15 @@ class SuperPoint(_Handle):
         _l.check(self._lib.osb_superpoint_read(self._h, code, image, _l.ptr(out), out.size))
         return out
 
+    @staticmethod
+    def band_geometry(height: int, width: int, zero_row: int) -> dict:
+        """the blanked band of images zero from row `zero_row` down (osb_superpoint_band_geometry): 'px' and 'tiles' [8, 4]
+        per trunk layer conv1a .. conv4b, 'first_skip' [4]; every rectangle as y0, y1, x0, x1 of [y0, y1) x [x0, x1)"""
+        out = np.zeros(68, np.int32)
+        _l.check(_l.load().osb_superpoint_band_geometry(height, width, zero_row, _l.ptr(out)))
+        r = out[:64].reshape(8, 2, 4)
+        return {"px": r[:, 0].copy(), "tiles": r[:, 1].copy(), "first_skip": out[64:].copy()}
+
 
 class NetVLAD(_Handle):
     """`inference(image) -> [4096] f32` (mobilenetvlad_tensorrt.cpp:4-15)."""

@@ -174,6 +174,7 @@ _SIG = {
     "osb_superpoint_set_profiling": (C.c_int, [_P, C.c_int]),
     "osb_superpoint_layer_ms": (C.c_int, [_P, _P, C.c_int]),
     "osb_superpoint_set_precision": (C.c_int, [_P, C.c_int]),
+    "osb_superpoint_band_geometry": (C.c_int, [C.c_int, C.c_int, C.c_int, _P]),
     "osb_conv_layer_parity": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int, C.c_int, C.c_int,
                                         C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                         C.c_float, _P]),
