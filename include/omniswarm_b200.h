@@ -573,6 +573,30 @@ osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const int64_t* fra
 osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out, int32_t* n_out);
 osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
                               void* stream);
+/* osb_anchor_add_measurements_dev(): add_new_loop_connection / add_new_detection (swarm_localization_solver.cpp:558-588) for
+ *   rows [0, *count_dev) of a DEVICE buffer, e.g. what osb_frontend_loop_measurements wrote, on `stream` without
+ *   synchronising.  A LOOP row is dropped when sqrt((x*x + y*y) + z*z) of its relative_pose, in fp64 without fused
+ *   multiply-adds, is > (double)loop_outlier_distance_threshold (a float, as the reference's parameter); detections are not
+ *   gated.  The kept rows are stored as osb_anchor_add_measurements stores them, in row order.  A dropped loop has used up
+ *   its id, so the ids in the store may have gaps, as in the reference.  One launch (a one-CTA block scan that validates,
+ *   gates, appends and updates the counts, which then live on the device).
+ *   Refused on the device, leaving the store unchanged: an unknown type or a drone id outside 0..max_drones-1
+ *   (OSB_ERR_INVALID), *count_dev outside [0, max_n] (OSB_ERR_INVALID), more kept rows than max_measurements leaves room for
+ *   (OSB_ERR_CAPACITY); osb_anchor_status() reports it.  Null pointers and max_n < 0 return OSB_ERR_INVALID at once, with
+ *   nothing enqueued.  The first call acquires 8 bytes of device counts, a mapped pinned feedback word and an event.
+ *   While an append may not have run, the host keeps a bound of the row count: the count the last executed append reported
+ *   plus the max_n of every append enqueued after it, capped at max_measurements.  run_dev launches over that bound, reads
+ *   the true counts on the device, writes rows past them as OSB_ANCHOR_VOID (skip = 1, every other field zero: PCM and the
+ *   factor compaction pass over them) and returns the bound as *n_out.  Every synchronising call (run, size,
+ *   add_measurements, push_odometry, set_window, status) first waits for the last device append, after which the counts are
+ *   exact and run returns exactly n_loops + n_detections rows.  A handle that never calls add_measurements_dev behaves as
+ *   if it did not exist.
+ * osb_anchor_status(): waits for the last device append and writes its status to *last (OSB_OK when none ran); returns the
+ *   same value. */
+#define OSB_ANCHOR_VOID 6
+osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_measurement* m_dev, const int32_t* count_dev, int max_n,
+                                           float loop_outlier_distance_threshold, void* stream);
+osb_status osb_anchor_status(osb_anchor* h, osb_status* last);
 
 /* ------------------------------------------------------------------------------------------------------------
  * The solve's chain from re-anchoring to factor rows on the device: run_dev -> reject_anchored -> compact_factors_dev, all
@@ -972,6 +996,35 @@ osb_status osb_frontend_set_loop_params(osb_frontend* h, const osb_loop_params* 
 osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev, const osb_loop_result* results_dev,
                                      int n, const osb_loop_candidate* cand /*HOST [n]*/, osb_loop_edge_result* out_dev,
                                      void* stream);
+/* Loop edges -> the back-end's measurement rows on the device -- the success branch of compute_loop that builds the
+ *   LoopEdge (loop_detector.cpp:787-829), for a whole round.  results_dev, edges_dev, cand and n are what the preceding
+ *   osb_frontend_compute_loop received or wrote; stamps [n] (HOST) are the two keyframes' stamps of each candidate.
+ * Only candidates with status == OSB_LOOP_ACCEPTED give a row, in candidate order (the reference handles a round one keyframe
+ *   at a time); *count_dev = the number of rows (a deterministic in-block scan, no atomics).  Row k (out_dev[k]):
+ *   id = self_id * 100000000 + loop_count, in int64 (the reference computes it in int, which overflows for self_id >= 22);
+ *   type OSB_MEAS_LOOP; id_a / id_b = the edge's drone_id_a / drone_id_b (old / new); relative_pose = the edge's;
+ *   stamp_a / self_pose_a the old keyframe's and stamp_b / self_pose_b the new one's, routed by results[i].swapped as
+ *   compute_loop routes them (swapped == 1: old = the query record, from stamp_query_ns / pose_query);
+ *   cov = diag(loop_cov_pos x3, loop_cov_ang x3), translation block first.
+ * Counters, on the device: loop_count (the next id's suffix) grows by one per row; for every row
+ *   inter_drone_loop_count[new][old] and [old][new] grow by one each (an intra-drone loop adds 2 to its cell, :826-827).
+ *   The pair counts are kept for drone ids 0..255; a row with a drone id outside that range is emitted all the same.
+ *   osb_frontend_db_reset leaves both counters as they are (the reference never resets them).
+ * 0 <= n <= 64; one launch, no host synchronisation; the host arrays travel as kernel parameters.  The first call acquires
+ *   the counters (8 bytes + 256 KB and an event); no later call allocates.  Calls on one handle must be ordered (one stream,
+ *   or joined by the caller).
+ * osb_frontend_loop_counts(): waits for the last loop_measurements call and reads loop_count and, unless pair_counts is
+ *   NULL, inter_drone_loop_count [256][256] row-major ([new][old]); zeros before the first call. */
+typedef struct {
+  int64_t stamp_query_ns;          /* stamp of records[i] */
+  int64_t stamp_hit_ns;            /* stamp of the hit keyframe (results[i].hit_msg_id) */
+} osb_loop_stamps;
+osb_status osb_frontend_loop_measurements(osb_frontend* h, const osb_loop_result* results_dev,
+                                          const osb_loop_edge_result* edges_dev, int n,
+                                          const osb_loop_candidate* cand /*HOST [n]*/, const osb_loop_stamps* stamps /*HOST [n]*/,
+                                          double loop_cov_pos, double loop_cov_ang, osb_measurement* out_dev /*[n]*/,
+                                          int32_t* count_dev, void* stream);
+osb_status osb_frontend_loop_counts(osb_frontend* h, int64_t* loop_count, int32_t* pair_counts /*[256][256] or NULL*/);
 /* ------------------------------------------------------------------------------------------------------------
  * Swarm-wide keyframe exchange -- replaces LoopNet::broadcast_fisheye_desc / image_desc_callback
  *   (swarm_loop/src/loop_net.cpp:20-120,142-172; called from swarm_loop/src/swarm_loop.cpp:167): the LCM UDP multicast of

@@ -8,6 +8,8 @@
 //   ceres::Solve in solve_once (swarm_localization/src/swarm_localization_solver.cpp:1695-1712) -> osb::FlatPoseGraph
 //   find_available_loops_detections (swarm_localization_solver.cpp:1594-1666)    -> osb_anchor_* + add_anchored_factors
 //                                                                                   (or add_compacted_factors)
+//   on_loop_connection -> add_new_loop_connection (loop_detector.cpp:787-829, swarm_localization_solver.cpp:558-588)
+//                                                                                -> osb::hand_loops_to_anchor
 //
 // The cv::Mat / cv::Point2f / cv::DMatch overloads are compiled when OSB_WITH_OPENCV is defined (the reference build
 // has OpenCV; this repository's container does not, so tests/cpp/adapter_smoke.cpp exercises the raw-pointer forms).
@@ -270,6 +272,22 @@ inline int add_anchored_factors(FlatPoseGraph& graph, const osb_anchor_result* r
     ++added;
   }
   return added;
+}
+
+// LoopDetector::on_loop_connection feeding SwarmLocalizationSolver::add_new_loop_connection, on the device: the accepted
+// loop edges of the compute_loop call that took (results_dev, cand, n) and wrote edges_dev become LoopEdge rows
+// (osb_frontend_loop_measurements) and pass the solver's distance gate into the anchor's store
+// (osb_anchor_add_measurements_dev), stream-ordered, no host copy and no synchronisation.  meas_dev [n] and count_dev
+// are the caller's device scratch; the next osb_anchor_run_dev on any stream sees the rows.
+inline void hand_loops_to_anchor(osb_frontend* fe, osb_anchor* anchor, const osb_loop_result* results_dev,
+                                 const osb_loop_edge_result* edges_dev, int n, const osb_loop_candidate* cand,
+                                 const osb_loop_stamps* stamps, double loop_cov_pos, double loop_cov_ang,
+                                 float loop_outlier_distance_threshold, osb_measurement* meas_dev, int32_t* count_dev,
+                                 void* stream) {
+  check(osb_frontend_loop_measurements(fe, results_dev, edges_dev, n, cand, stamps, loop_cov_pos, loop_cov_ang, meas_dev,
+                                       count_dev, stream), "osb_frontend_loop_measurements");
+  check(osb_anchor_add_measurements_dev(anchor, meas_dev, count_dev, n, loop_outlier_distance_threshold, stream),
+        "osb_anchor_add_measurements_dev");
 }
 
 // The same factors from osb_anchor_compact_factors_dev's SoA after its one copy to the host: count rows of type / ia / ib /

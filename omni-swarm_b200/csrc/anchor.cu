@@ -31,6 +31,9 @@ struct AnchorView {
   const int32_t* loop_slot;        // all_loops[i] = meas[loop_slot[i]]
   const int32_t* det_slot;         // all_detections_6d[i] = meas[det_slot[i]]
   int n_loops, n_total;
+  const int32_t* counts;           // [2] loops, detections on the device while a device append may be in flight (then
+                                   // n_loops / n_total are unused), else null
+  int n_bound;                     // rows written: n_total, or the host's bound of it; rows n_total.. are OSB_ANCHOR_VOID
   const int64_t* traj_stamp;       // [max_drones][max_samples]
   const double* traj_pose;         // [max_drones][max_samples][7]
   const double* traj_len;          // [max_drones][max_samples]
@@ -121,11 +124,25 @@ anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
   __shared__ double s_out[ANCHOR_WARPS][RESULT_WORDS];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * ANCHOR_WARPS + w;
-  if (i >= v.n_total) return;                                      // warp-uniform
-  const int slot = i < v.n_loops ? v.loop_slot[i] : v.det_slot[i - v.n_loops];
+  if (i >= v.n_bound) return;                                      // warp-uniform
+  const int n_loops = v.counts ? v.counts[0] : v.n_loops;
+  const int n_total = v.counts ? n_loops + v.counts[1] : v.n_total;
+  for (int k = lane; k < RESULT_WORDS; k += 32) s_out[w][k] = 0.0;
+  if (i >= n_total) {                                              // past the true count: a VOID row, skipped downstream
+    __syncwarp();
+    if (lane == 0) {
+      osb_anchor_result& r = *reinterpret_cast<osb_anchor_result*>(s_out[w]);
+      r.status = OSB_ANCHOR_VOID;
+      r.skip = 1;
+    }
+    __syncwarp();
+    double* dst = reinterpret_cast<double*>(out + i);
+    for (int j = lane; j < RESULT_WORDS; j += 32) dst[j] = s_out[w][j];
+    return;
+  }
+  const int slot = i < n_loops ? v.loop_slot[i] : v.det_slot[i - n_loops];
   const double* src = reinterpret_cast<const double*>(v.meas + slot);
   for (int k = lane; k < MEAS_WORDS; k += 32) s_meas[w][k] = src[k];
-  for (int k = lane; k < RESULT_WORDS; k += 32) s_out[w][k] = 0.0;
   __syncwarp();
   const osb_measurement& m = *reinterpret_cast<const osb_measurement*>(s_meas[w]);
   osb_anchor_result& r = *reinterpret_cast<osb_anchor_result*>(s_out[w]);
@@ -268,6 +285,108 @@ anchor_compact_kernel(const osb_anchor_result* __restrict__ rows, int n, const u
   if (threadIdx.x == 0) *count = out_base;
 }
 
+// Row-count feedback of the device append, written into mapped pinned host memory as the front-end's FeFeedback is: the last
+// append that has run reports the true counts, its status and how much had been charged to the host's bound when it was
+// enqueued, so bound = count + what was charged since.  seq_begin / seq_end make a torn read detectable.
+struct AnchorFeedback {
+  volatile long long seq_begin;
+  volatile long long n_loops, n_dets, charged, status;
+  volatile long long seq_end;
+};
+
+// add_new_loop_connection / add_new_detection for rows [0, *count) of a device buffer (solver.cpp:558-588): one CTA.
+// Pass 1 validates every row and counts what the distance gate keeps; a refused call writes nothing but the feedback.
+// Pass 2 appends tile by tile: a block scan of (kept loop, kept detection) per thread gives each row its arrival slot and
+// its place in the loop or detection list, in row order (no atomics).
+constexpr int APPEND_THREADS = 256;
+
+// exclusive block scan over APPEND_THREADS threads; *total = the block's sum.  Ends with a barrier, so it can be called again.
+__device__ __forceinline__ int append_block_scan(int v, int* total) {
+  __shared__ int s_warp[APPEND_THREADS / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  if (lane == 31) s_warp[wid] = inc;
+  __syncthreads();
+  int base = 0, sum = 0;
+#pragma unroll
+  for (int w = 0; w < APPEND_THREADS / 32; ++w) { if (w < wid) base += s_warp[w]; sum += s_warp[w]; }
+  __syncthreads();
+  *total = sum;
+  return base + inc - v;
+}
+
+// the reference's gate: relative_pose.pos().norm() > loop_outlier_distance_threshold drops a loop; detections pass
+__device__ __forceinline__ bool append_keeps(const osb_measurement& r, float thres) {
+  if (r.type != OSB_MEAS_LOOP) return true;
+  const double* p = r.relative_pose;
+  const double d = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(p[0], p[0]), __dmul_rn(p[1], p[1])), __dmul_rn(p[2], p[2])));
+  return !(d > (double)thres);
+}
+
+__global__ void __launch_bounds__(APPEND_THREADS)
+anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __restrict__ count_dev, int max_n, float thres,
+                     int max_drones, int max_meas, osb_measurement* __restrict__ meas, int32_t* __restrict__ loop_slot,
+                     int32_t* __restrict__ det_slot, int32_t* __restrict__ counts, AnchorFeedback* __restrict__ fb,
+                     long long seq, long long charged) {
+  __shared__ int s_bad;
+  const int tid = threadIdx.x;
+  const int n = *count_dev;
+  const int have_l = counts[0], have_d = counts[1];               // thread 0 rewrites them after the last barrier
+  if (tid == 0) s_bad = 0;
+  __syncthreads();
+  int status = (n < 0 || n > max_n) ? OSB_ERR_INVALID : OSB_OK;
+  int kept = 0;
+  if (status == OSB_OK)
+#pragma unroll 1
+    for (int i = tid; i < n; i += APPEND_THREADS) {
+      const osb_measurement& r = m[i];
+      const bool ok = (r.type == OSB_MEAS_LOOP || r.type == OSB_MEAS_DET4D || r.type == OSB_MEAS_DET6D) &&
+                      r.id_a >= 0 && r.id_a < max_drones && r.id_b >= 0 && r.id_b < max_drones;
+      if (!ok) s_bad = 1;
+      else kept += append_keeps(r, thres);
+    }
+  int total;
+  append_block_scan(kept, &total);                                 // its barriers also publish s_bad
+  if (status == OSB_OK && s_bad) status = OSB_ERR_INVALID;
+  if (status == OSB_OK && (long long)have_l + have_d + total > max_meas) status = OSB_ERR_CAPACITY;
+  int nl = 0, nd = 0;                                              // kept loops / detections of the tiles before
+  if (status == OSB_OK)
+#pragma unroll 1
+    for (int base = 0; base < n; base += APPEND_THREADS) {
+      const int i = base + tid;
+      const bool kept_i = i < n && append_keeps(m[i], thres);
+      const int loop = kept_i && m[i].type == OSB_MEAS_LOOP, det = kept_i && m[i].type != OSB_MEAS_LOOP;
+      int tile;
+      const int ex = append_block_scan(loop | (det << 16), &tile);   // a tile's counts fit 16 bits each
+      if (loop | det) {
+        const int el = ex & 0xffff, ed = ex >> 16;
+        const int slot = have_l + have_d + nl + nd + el + ed;     // arrival order
+        const double* src = reinterpret_cast<const double*>(m + i);
+        double* dst = reinterpret_cast<double*>(meas + slot);
+        for (int k = 0; k < MEAS_WORDS; ++k) dst[k] = src[k];
+        if (loop) loop_slot[have_l + nl + el] = slot;
+        else det_slot[have_d + nd + ed] = slot;
+      }
+      nl += tile & 0xffff;
+      nd += tile >> 16;
+    }
+  if (tid != 0) return;
+  if (status == OSB_OK) { counts[0] = have_l + nl; counts[1] = have_d + nd; }
+  fb->seq_begin = seq;
+  __threadfence_system();
+  fb->n_loops = status == OSB_OK ? have_l + nl : have_l;
+  fb->n_dets = status == OSB_OK ? have_d + nd : have_d;
+  fb->charged = charged;
+  fb->status = status;
+  __threadfence_system();
+  fb->seq_end = seq;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -295,6 +414,17 @@ struct osb_anchor {
   int32_t *d_win_frame = nullptr, *d_win_block = nullptr;
   double* d_win_pose = nullptr;
   osb_anchor_result* d_out = nullptr;
+  // device appends (osb_anchor_add_measurements_dev), acquired by the first one: the counts on the device, their feedback
+  // (mapped pinned memory + its device alias) and an event recorded after every append
+  int32_t* d_counts = nullptr;                    // [2] loops, detections
+  AnchorFeedback* fb_host = nullptr;
+  AnchorFeedback* fb_dev = nullptr;
+  cudaEvent_t last_append = nullptr;
+  bool append_pending = false;                    // an append may not have run: n_loops / n_dets are stale, `upper` bounds them
+  long long append_seq = 0, fb_min_seq = 1;       // feedback older than fb_min_seq carries nothing new
+  long long charged = 0;                          // max_n summed over every device append
+  long long upper = 0;                            // bound of n_loops + n_dets while append_pending
+  osb_status last_status = OSB_OK;                // the last device append's, once synchronised
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -316,6 +446,32 @@ osb_status anchor_wait_last_run(osb_anchor* h) {
 }
 
 bool drone_ok(const osb_anchor* h, int32_t d) { return d >= 0 && d < h->p.max_drones; }
+
+// wait for the last device append and take its exact counts and status (every synchronising call starts with this)
+osb_status anchor_settle(osb_anchor* h) {
+  if (!h->append_pending) return OSB_OK;
+  OSB_CUDA(cudaEventSynchronize(h->last_append));
+  const AnchorFeedback* fb = h->fb_host;
+  h->n_loops = (int)fb->n_loops;
+  h->n_dets = (int)fb->n_dets;
+  h->last_status = (osb_status)fb->status;
+  h->upper = h->n_loops + h->n_dets;
+  h->append_pending = false;
+  h->fb_min_seq = h->append_seq + 1;
+  return OSB_OK;
+}
+
+// lower the bound with what the most recent append that has RUN reported (no synchronisation)
+void anchor_tighten(osb_anchor* h) {
+  const AnchorFeedback* fb = h->fb_host;
+  const long long e = fb->seq_end;
+  std::atomic_thread_fence(std::memory_order_acquire);
+  const long long nl = fb->n_loops, nd = fb->n_dets, ch = fb->charged;
+  std::atomic_thread_fence(std::memory_order_acquire);
+  const long long b = fb->seq_begin;
+  if (b != e || e < h->fb_min_seq) return;
+  h->upper = std::min(h->upper, nl + nd + (h->charged - ch));
+}
 
 }  // namespace
 
@@ -378,6 +534,7 @@ extern "C" osb_status osb_anchor_push_odometry(osb_anchor* h, int32_t drone, int
   OSB_REQUIRE(h != nullptr && n >= 0 && (n == 0 || (stamps_ns && poses)), "null argument or negative count");
   OSB_REQUIRE(drone_ok(h, drone), "drone id outside 0..max_drones-1");
   std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(anchor_settle(h));
   const int have = h->traj_n[drone];
   for (int i = 0; i < n; ++i) {
     const int64_t prev = i > 0 ? stamps_ns[i - 1] : h->last_stamp[drone];
@@ -426,6 +583,7 @@ extern "C" osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const os
     OSB_REQUIRE(drone_ok(h, m[i].id_a) && drone_ok(h, m[i].id_b), "drone id outside 0..max_drones-1");
   }
   std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(anchor_settle(h));
   const int have = h->n_loops + h->n_dets;
   if ((long long)have + n > h->p.max_measurements) {
     set_error(__func__, "the handle would exceed max_measurements");
@@ -450,6 +608,9 @@ extern "C" osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const os
   if (n > new_loops)
     OSB_CUDA(cudaMemcpyAsync(h->d_det_slot + h->n_dets, slot.data() + new_loops, (size_t)(n - new_loops) * sizeof(int32_t),
                              cudaMemcpyHostToDevice, st));
+  const int32_t counts[2] = {h->n_loops + new_loops, h->n_dets + n - new_loops};
+  if (h->d_counts)                                                 // device appends continue from here
+    OSB_CUDA(cudaMemcpyAsync(h->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   h->n_loops += new_loops;
   h->n_dets += n - new_loops;
@@ -459,6 +620,7 @@ extern "C" osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const os
 extern "C" osb_status osb_anchor_size(osb_anchor* h, int32_t* n_loops, int32_t* n_detections) {
   OSB_REQUIRE(h != nullptr && n_loops != nullptr && n_detections != nullptr, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(anchor_settle(h));
   *n_loops = h->n_loops;
   *n_detections = h->n_dets;
   return OSB_OK;
@@ -475,6 +637,7 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
     OSB_REQUIRE(n_entries == 0 || entries != nullptr, "null entries");
   }
   std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(anchor_settle(h));
   if (n_entries > h->p.max_window_entries) {
     set_error(__func__, "the window would exceed max_window_entries");
     return OSB_ERR_CAPACITY;
@@ -548,9 +711,17 @@ osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_ancho
   v.huber = h->p.huber;
   for (int d = 0; d < h->p.max_drones; ++d)
     if (yaw_observable[d]) v.yaw_obs[d >> 6] |= 1ull << (d & 63);
-  *n_out = v.n_total;
-  if (v.n_total == 0) return OSB_OK;
-  OSB_LAUNCH(anchor_kernel, cdiv(v.n_total, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
+  v.counts = nullptr;
+  v.n_bound = v.n_total;
+  if (h->append_pending) {                      // the counts are the device's; the grid covers the host's bound of them
+    anchor_tighten(h);
+    OSB_CUDA(cudaStreamWaitEvent(st, h->last_append, 0));
+    v.counts = h->d_counts;
+    v.n_bound = (int)h->upper;
+  }
+  *n_out = v.n_bound;
+  if (v.n_bound == 0) return OSB_OK;
+  OSB_LAUNCH(anchor_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(cudaEventRecord(h->last_run, st));
   return OSB_OK;
@@ -581,6 +752,7 @@ extern "C" osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* ro
 extern "C" osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out, int32_t* n_out) {
   OSB_REQUIRE(h != nullptr && yaw_observable != nullptr && n_out != nullptr, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(anchor_settle(h));                                       // exact counts: run writes no VOID row
   OSB_REQUIRE(out != nullptr || h->n_loops + h->n_dets == 0, "null output");
   DeviceGuard dg(h->device);
   OSB_TRY(anchor_launch(h, yaw_observable, h->d_out, n_out, h->stream));
@@ -588,4 +760,61 @@ extern "C" osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observabl
     OSB_CUDA(cudaMemcpyAsync(out, h->d_out, (size_t)*n_out * sizeof(osb_anchor_result), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   return OSB_OK;
+}
+
+namespace {
+
+// the first device append acquires the device counts (seeded with the host's exact ones), the feedback and the event
+osb_status anchor_dev_init(osb_anchor* h) {
+  if (h->d_counts) return OSB_OK;
+  Resources& R = h->res;
+  OSB_TRY(R.alloc(&h->d_counts, 2));
+  OSB_TRY(R.host_alloc(&h->fb_host, 1, cudaHostAllocMapped));
+  memset((void*)h->fb_host, 0, sizeof(AnchorFeedback));
+  OSB_CUDA(cudaHostGetDevicePointer((void**)&h->fb_dev, (void*)h->fb_host, 0));
+  OSB_TRY(R.event(&h->last_append, cudaEventDisableTiming));
+  const int32_t counts[2] = {h->n_loops, h->n_dets};
+  OSB_CUDA(cudaMemcpyAsync(h->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  return OSB_OK;
+}
+
+}  // namespace
+
+extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_measurement* m_dev, const int32_t* count_dev,
+                                                      int max_n, float loop_outlier_distance_threshold, void* stream) {
+  OSB_REQUIRE(h != nullptr && m_dev != nullptr && count_dev != nullptr, "null argument");
+  OSB_REQUIRE(max_n >= 0, "negative max_n");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_TRY(anchor_dev_init(h));
+  // the append rewrites the counts a run reads and follows the previous append, whichever streams those ran on
+  OSB_CUDA(cudaStreamWaitEvent(st, h->last_run, 0));
+  if (h->append_pending) {
+    OSB_CUDA(cudaStreamWaitEvent(st, h->last_append, 0));
+    anchor_tighten(h);
+  } else {
+    h->upper = h->n_loops + h->n_dets;
+  }
+  const long long seq = h->append_seq + 1, charged = h->charged + max_n;
+  OSB_LAUNCH(anchor_append_kernel, 1, APPEND_THREADS, 0, st, m_dev, count_dev, max_n, loop_outlier_distance_threshold,
+             h->p.max_drones, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb_dev, seq,
+             charged);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(cudaEventRecord(h->last_append, st));
+  h->append_seq = seq;
+  h->charged = charged;
+  h->upper = std::min<long long>(h->upper + max_n, h->p.max_measurements);
+  h->append_pending = true;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_status(osb_anchor* h, osb_status* last) {
+  OSB_REQUIRE(h != nullptr && last != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(anchor_settle(h));
+  *last = h->last_status;
+  return h->last_status;
 }

@@ -663,6 +663,51 @@ lc_finalise_kernel(const uint8_t* __restrict__ mask, const osb_pnp_result* __res
   for (int k = 0; k < 4; ++k) o->relative_pose[3 + k] = dp.q[k];
 }
 
+// ---- loop edges -> the back-end's measurement rows: the success branch of compute_loop (loop_detector.cpp:787-829) for a
+// whole round, candidate c on thread c of one 256-thread CTA ------------------------------------------------------------
+constexpr long long LM_MAX_LOOP_ID = 100000000ll;        // MAX_LOOP_ID (loop_detector.cpp:9)
+constexpr int LM_PAIR_DRONES = 256;                      // inter_drone_loop_count is kept for drone ids 0..255
+
+struct LoopMeasBatch {         // the host's poses and stamps of the candidates, passed as kernel parameters (8 KB)
+  double pose_query[LC_MAX][7];
+  double pose_hit[LC_MAX][7];
+  int64_t stamp_query[LC_MAX];
+  int64_t stamp_hit[LC_MAX];
+};
+
+__global__ void __launch_bounds__(256)
+lm_emit_kernel(const osb_loop_result* __restrict__ results, const osb_loop_edge_result* __restrict__ edges, int n,
+               const __grid_constant__ LoopMeasBatch b, int self_id, double cov_pos, double cov_ang,
+               osb_measurement* __restrict__ out, int32_t* __restrict__ count, long long* __restrict__ loop_count,
+               int32_t* __restrict__ pair_counts) {
+  const int c = threadIdx.x;
+  const long long first = *loop_count;                     // read by every thread before fe_block_compact's barrier
+  const bool keep = c < n && edges[c].status == OSB_LOOP_ACCEPTED;
+  int total;
+  const int pos = fe_block_compact(keep, &total);          // candidate order = the reference's one-keyframe-at-a-time order
+  if (c == 0) { *count = total; *loop_count = first + total; }
+  if (!keep) return;
+  const osb_loop_edge_result& e = edges[c];
+  const bool swapped = results[c].swapped != 0;            // compute_loop's roles: swapped -> old = the query record
+  osb_measurement& m = out[pos];
+  m.id = (long long)self_id * LM_MAX_LOOP_ID + first + pos;   // :811, in int64 (DESIGN §5)
+  m.type = OSB_MEAS_LOOP;
+  m.id_a = e.drone_id_a;
+  m.id_b = e.drone_id_b;
+  m.reserved = 0;
+  m.stamp_a = swapped ? b.stamp_query[c] : b.stamp_hit[c];
+  m.stamp_b = swapped ? b.stamp_hit[c] : b.stamp_query[c];
+  const double* pa = swapped ? b.pose_query[c] : b.pose_hit[c];
+  const double* pb = swapped ? b.pose_hit[c] : b.pose_query[c];
+  for (int k = 0; k < 7; ++k) { m.relative_pose[k] = e.relative_pose[k]; m.self_pose_a[k] = pa[k]; m.self_pose_b[k] = pb[k]; }
+  for (int k = 0; k < 36; ++k) m.cov[k] = (k % 7 == 0) ? (k < 21 ? cov_pos : cov_ang) : 0.0;     // pos_cov / ang_cov (:800-808)
+  const int a = e.drone_id_a, nw = e.drone_id_b;           // :824-827: an intra-drone loop adds 2 to its one cell
+  if (a >= 0 && a < LM_PAIR_DRONES && nw >= 0 && nw < LM_PAIR_DRONES) {
+    atomicAdd(&pair_counts[nw * LM_PAIR_DRONES + a], 1);
+    atomicAdd(&pair_counts[a * LM_PAIR_DRONES + nw], 1);
+  }
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -716,6 +761,11 @@ struct osb_frontend {
   osb_pnp_params* d_lc_params = nullptr;
   uint8_t* d_lc_mask = nullptr;                           // [LC_MAX][LC_MAXN]
   osb_pnp_result* d_lc_pnp = nullptr;
+  // osb_frontend_loop_measurements: loop_count and inter_drone_loop_count [256][256] on the device, acquired by its first
+  // call; ev_lm is recorded after every call so that osb_frontend_loop_counts can wait for the last one
+  long long* d_lm_count = nullptr;
+  int32_t* d_lm_pairs = nullptr;
+  cudaEvent_t ev_lm = nullptr;
   int32_t* d_assign = nullptr;   // [max_records][4]
   float* d_load_stage = nullptr;   // [FE_LOAD_ROWS][4096]: osb_frontend_db_load's fp32 -> fp16 staging, acquired by the first
                                    // load into an fp16 store
@@ -1318,6 +1368,60 @@ extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyfr
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(lc_finalise_kernel, n, 256, 0, st, h->d_lc_mask, h->d_lc_pnp, h->d_lc_params, out_dev);
   OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_loop_measurements(osb_frontend* h, const osb_loop_result* results_dev,
+                                                     const osb_loop_edge_result* edges_dev, int n,
+                                                     const osb_loop_candidate* cand, const osb_loop_stamps* stamps,
+                                                     double loop_cov_pos, double loop_cov_ang, osb_measurement* out_dev,
+                                                     int32_t* count_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 0 && n <= LC_MAX, "n must be 0..64");
+  OSB_REQUIRE(out_dev && count_dev && (n == 0 || (results_dev && edges_dev && cand && stamps)), "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!h->d_lm_count) {                                    // the first call acquires the counters, zero
+    Resources& m = h->res;
+    OSB_TRY(m.alloc(&h->d_lm_count, 1));
+    OSB_TRY(m.alloc(&h->d_lm_pairs, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES));
+    OSB_TRY(m.event(&h->ev_lm, cudaEventDisableTiming));
+    OSB_CUDA(cudaMemsetAsync(h->d_lm_count, 0, sizeof(long long), st));
+    OSB_CUDA(cudaMemsetAsync(h->d_lm_pairs, 0, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES * sizeof(int32_t), st));
+  }
+  LoopMeasBatch b;
+  memset(&b, 0, sizeof(b));
+  for (int i = 0; i < n; ++i) {
+    memcpy(b.pose_query[i], cand[i].pose_query, sizeof(b.pose_query[i]));
+    memcpy(b.pose_hit[i], cand[i].pose_hit, sizeof(b.pose_hit[i]));
+    b.stamp_query[i] = stamps[i].stamp_query_ns;
+    b.stamp_hit[i] = stamps[i].stamp_hit_ns;
+  }
+  OSB_LAUNCH(lm_emit_kernel, 1, 256, 0, st, results_dev, edges_dev, n, b, h->cfg.self_id, loop_cov_pos, loop_cov_ang,
+             out_dev, count_dev, h->d_lm_count, h->d_lm_pairs);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(cudaEventRecord(h->ev_lm, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_loop_counts(osb_frontend* h, int64_t* loop_count, int32_t* pair_counts) {
+  OSB_REQUIRE(h != nullptr && loop_count != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  const size_t pair_bytes = (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES * sizeof(int32_t);
+  if (!h->d_lm_count) {                                    // no call yet: both counters are zero
+    *loop_count = 0;
+    if (pair_counts) memset(pair_counts, 0, pair_bytes);
+    return OSB_OK;
+  }
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaStreamWaitEvent(st, h->ev_lm, 0));
+  long long cnt = 0;
+  OSB_CUDA(cudaMemcpyAsync(&cnt, h->d_lm_count, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  if (pair_counts) OSB_CUDA(cudaMemcpyAsync(pair_counts, h->d_lm_pairs, pair_bytes, cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  *loop_count = cnt;
   return OSB_OK;
 }
 

@@ -509,6 +509,35 @@ class KeyframeFrontend(_Handle):
         _l.check(self._lib.osb_frontend_compute_loop(self._h, C.c_void_p(records_dev), C.c_void_p(results_dev), len(cands),
                                                      arr, C.c_void_p(out_dev), C.c_void_p(stream)))
 
+    @staticmethod
+    def loop_stamps(stamps):
+        """[(stamp_query_ns, stamp_hit_ns)] per candidate -> LoopStamps array"""
+        arr = (_l.LoopStamps * len(stamps))()
+        for a, (q, h) in zip(arr, stamps):
+            a.stamp_query_ns, a.stamp_hit_ns = int(q), int(h)
+        return arr
+
+    def loop_measurements(self, results_dev: int, edges_dev: int, cands, stamps, loop_cov_pos: float, loop_cov_ang: float,
+                          out_dev: int, count_dev: int, stream: int):
+        """the LoopEdge of every ACCEPTED candidate of the preceding compute_loop (osb_frontend_loop_measurements): rows of
+        lib.MEASUREMENT_DTYPE at out_dev in candidate order and their number into the int32 at count_dev, on `stream`
+        without synchronising.  cands: the list compute_loop took; stamps: (stamp_query_ns, stamp_hit_ns) per candidate.
+        Either may also be given as the ctypes array loop_candidates / loop_stamps made of it, built once by a caller that
+        repeats the call."""
+        assert len(stamps) == len(cands), "one stamp pair per candidate"
+        arr = cands if isinstance(cands, C.Array) else self.loop_candidates(cands)
+        st = stamps if isinstance(stamps, C.Array) else self.loop_stamps(stamps)
+        _l.check(self._lib.osb_frontend_loop_measurements(self._h, C.c_void_p(results_dev), C.c_void_p(edges_dev),
+                                                          len(cands), arr, st, float(loop_cov_pos), float(loop_cov_ang),
+                                                          C.c_void_p(out_dev), C.c_void_p(count_dev), C.c_void_p(stream)))
+
+    def loop_counts(self):
+        """waits for the last loop_measurements -> (loop_count, inter_drone_loop_count [256, 256] int32, [new][old])"""
+        n = C.c_int64(0)
+        pairs = np.zeros((_l.LOOP_PAIR_DRONES, _l.LOOP_PAIR_DRONES), np.int32)
+        _l.check(self._lib.osb_frontend_loop_counts(self._h, C.byref(n), _l.ptr(pairs)))
+        return n.value, pairs
+
     def finish(self, stream: int):
         _l.check(self._lib.osb_frontend_finish(self._h, C.c_void_p(stream)))
 
@@ -799,6 +828,21 @@ class LoopAnchor(_Handle):
     def add_measurements(self, meas):
         meas = np.ascontiguousarray(meas, _l.MEASUREMENT_DTYPE)
         _l.check(self._lib.osb_anchor_add_measurements(self._h, len(meas), _l.ptr(meas)))
+
+    def add_measurements_dev(self, meas_ptr: int, count_ptr: int, max_n: int, loop_outlier_distance_threshold: float,
+                             stream: int):
+        """add_new_loop_connection / add_new_detection for rows [0, *count_ptr) of lib.MEASUREMENT_DTYPE in device memory
+        (osb_anchor_add_measurements_dev), on `stream` without synchronising; a refused call shows in status()"""
+        _l.check(self._lib.osb_anchor_add_measurements_dev(self._h, C.c_void_p(meas_ptr), C.c_void_p(count_ptr), int(max_n),
+                                                           float(loop_outlier_distance_threshold), C.c_void_p(stream)))
+
+    def status(self) -> int:
+        """waits for the last add_measurements_dev -> its status (lib.OK, lib.ERR_INVALID or lib.ERR_CAPACITY)"""
+        last = C.c_int(0)
+        st = self._lib.osb_anchor_status(self._h, C.byref(last))
+        if st not in (_l.OK, last.value):
+            _l.check(st)
+        return last.value
 
     def size(self) -> tuple[int, int]:
         """-> (loops, detections) held"""

@@ -100,7 +100,7 @@ ANCHOR_RESULT_DTYPE = np.dtype([("id", "<i8"), ("type", "<i4"), ("status", "<i4"
                                 ("dt_err_ns", "<i8"), ("dpos", "<f8"), ("edge", LOOP_EDGE_DTYPE), ("skip", "<i4"),
                                 ("factor_type", "<i4"), ("ia", "<i4"), ("ib", "<i4"), ("huber", "<i4"), ("reserved", "<i4"),
                                 ("payload", "<f8", PAYLOAD_LEN)])
-ANCHOR_OK, ANCHOR_EMPTY_WINDOW, ANCHOR_BEFORE_WINDOW, ANCHOR_NO_FRAME, ANCHOR_NO_TRAJECTORY, ANCHOR_DPOS = range(6)
+ANCHOR_OK, ANCHOR_EMPTY_WINDOW, ANCHOR_BEFORE_WINDOW, ANCHOR_NO_FRAME, ANCHOR_NO_TRAJECTORY, ANCHOR_DPOS, ANCHOR_VOID = range(7)
 
 
 class PnpParams(C.Structure):
@@ -143,6 +143,13 @@ class LoopEdgeResult(C.Structure):
                 ("relative_pose", C.c_double * 7), ("corr_dir_new", C.c_int32 * LOOP_MAXN),
                 ("corr_idx_new", C.c_int32 * LOOP_MAXN), ("corr_dir_old", C.c_int32 * LOOP_MAXN),
                 ("corr_idx_old", C.c_int32 * LOOP_MAXN), ("inlier", C.c_uint8 * LOOP_MAXN)]
+
+
+class LoopStamps(C.Structure):
+    _fields_ = [("stamp_query_ns", C.c_int64), ("stamp_hit_ns", C.c_int64)]
+
+
+LOOP_PAIR_DRONES = 256         # inter_drone_loop_count is kept for drone ids 0..255 (osb_frontend_loop_counts)
 
 
 class FrontendConfig(C.Structure):
@@ -247,6 +254,8 @@ _SIG = {
     "osb_frontend_query_received": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "osb_frontend_set_loop_params": (C.c_int, [_P, C.POINTER(LoopParams)]),
     "osb_frontend_compute_loop": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
+    "osb_frontend_loop_measurements": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P]),
+    "osb_frontend_loop_counts": (C.c_int, [_P, C.POINTER(C.c_int64), _P]),
     "osb_frontend_process": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
     "osb_frontend_finish": (C.c_int, [_P, _P]),
     "osb_frontend_set_profiling": (C.c_int, [_P, C.c_int]),
@@ -289,6 +298,8 @@ _SIG = {
     "osb_anchor_run": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32)]),
     "osb_anchor_run_dev": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32), _P]),
     "osb_anchor_compact_factors_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "osb_anchor_add_measurements_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_float, _P]),
+    "osb_anchor_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
