@@ -8,7 +8,8 @@ Names, argument meaning and error behaviour follow the reference (paths relative
   PoseGraphSolver   <- SwarmLocalizationSolver::solve_once  swarm_localization/src/swarm_localization_solver.cpp:1668
   KeyframeFrontend  <- LoopCam::on_flattened_images + LoopDetector::on_image_recv database work
   LoopAnchor        <- SwarmLocalizationSolver::find_available_loops_detections  swarm_localization_solver.cpp:1594-1666
-All compute happens in libomniswarm_b200.so; these classes only marshal numpy arrays.
+All compute happens in libomniswarm_b200.so; these classes only marshal numpy arrays.  FactorRows and AnchoredChain hold
+the device buffers (torch tensors) that one solve's *_dev calls pass between them.
 """
 from __future__ import annotations
 
@@ -909,6 +910,111 @@ def compact_anchored_factors(rows_ptr: int, n: int, keep_ptr, type_ptr: int, ia_
 def anchored_loop_edges(res: np.ndarray) -> np.ndarray:
     """the re-anchored edges as the packed [n, 60] array PcmState.reject takes"""
     return np.ascontiguousarray(res["edge"]).view(np.float64).reshape(len(res), 60)
+
+
+def anchored_keep(state: PcmState, res: np.ndarray) -> np.ndarray:
+    """the keep mask PcmState.reject_anchored writes, on the host: the OK rows through state.reject, scattered back to
+    one uint8 per row"""
+    ok = res["status"] == _l.ANCHOR_OK
+    keep = np.zeros(len(res), np.uint8)
+    keep[ok] = state.reject(anchored_loop_edges(res[ok]), res["id"][ok])
+    return keep
+
+
+FACTOR_KEYS = ("ftype", "ia", "ib", "payload", "huber")
+
+
+class FactorRows:
+    """cap solver rows in device memory, laid out as compact_anchored_factors writes them and
+    PoseGraphSolver.solve_resident_dev reads them: type / ia / ib int32, payload [cap, PAYLOAD_LEN] float64, huber uint8,
+    and their count in one int32.  Host-side rows are dicts of FACTOR_KEYS arrays, in anchored_factor_rows' order."""
+
+    def __init__(self, cap: int):
+        import torch
+        cap = max(cap, 1)
+        self.type, self.ia, self.ib = (torch.zeros(cap, dtype=torch.int32, device="cuda") for _ in range(3))
+        self.payload = torch.zeros(cap * _l.PAYLOAD_LEN, dtype=torch.float64, device="cuda")
+        self.huber = torch.zeros(cap, dtype=torch.uint8, device="cuda")
+        self.count = torch.zeros(1, dtype=torch.int32, device="cuda")
+
+    def ptrs(self) -> tuple:
+        """the six device pointers, in the order compact_anchored_factors and solve_resident_dev take them"""
+        return tuple(t.data_ptr() for t in (self.type, self.ia, self.ib, self.payload, self.huber, self.count))
+
+    def set(self, rows: dict, count: int | None = None):
+        """copies host rows in on the current stream; count: the count stored (default: the number of rows)"""
+        import torch
+        k = len(rows["ftype"])
+        if k:
+            self.type[:k] = torch.from_numpy(np.asarray(rows["ftype"], np.int32)).cuda()
+            self.ia[:k] = torch.from_numpy(np.asarray(rows["ia"], np.int32)).cuda()
+            self.ib[:k] = torch.from_numpy(np.asarray(rows["ib"], np.int32)).cuda()
+            self.payload[:k * _l.PAYLOAD_LEN] = torch.from_numpy(np.ascontiguousarray(rows["payload"]).reshape(-1)).cuda()
+            self.huber[:k] = torch.from_numpy(np.asarray(rows["huber"], np.uint8)).cuda()
+        self.count.fill_(k if count is None else count)
+
+    def on_host(self, stream=None) -> dict:
+        """waits for `stream` (a torch stream; None: the current one), the stream that wrote the rows -> the first count
+        rows"""
+        import torch
+        with torch.cuda.stream(stream):
+            k = int(self.count.cpu()[0])
+            return {"ftype": self.type[:k].cpu().numpy(), "ia": self.ia[:k].cpu().numpy(), "ib": self.ib[:k].cpu().numpy(),
+                    "payload": self.payload[:k * _l.PAYLOAD_LEN].cpu().numpy().reshape(k, _l.PAYLOAD_LEN),
+                    "huber": self.huber[:k].cpu().numpy()}
+
+    def solve(self, solver: PoseGraphSolver, max_tail: int, options=None, stream=None):
+        """solver.solve_resident_dev with these rows as its tail, on `stream` (a torch stream; None: the current one)"""
+        import torch
+        s = torch.cuda.current_stream() if stream is None else stream
+        solver.solve_resident_dev(max_tail, *self.ptrs(), s.cuda_stream, options)
+
+
+class AnchoredChain:
+    """The device buffers of one solve's chain and the stream it runs on: LoopAnchor.run_dev's rows (cap of them),
+    PcmState.reject_anchored's keep mask and the FactorRows compact_anchored_factors fills.  Each step is one method;
+    calling the chain runs run -> reject -> compact, nothing copied between them."""
+
+    def __init__(self, cap: int, stream=None):
+        import torch
+        self.rows = torch.zeros(cap * _l.ANCHOR_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+        self.keep = torch.zeros(cap, dtype=torch.uint8, device="cuda")
+        self.factors = FactorRows(cap)
+        self.stream = torch.cuda.Stream() if stream is None else stream
+        self.stream.wait_stream(torch.cuda.current_stream())        # the buffers are zeroed on the current stream
+
+    def upload(self, res: np.ndarray):
+        """host rows of lib.ANCHOR_RESULT_DTYPE in place of run's, copied on the current stream, which the chain's stream
+        then waits for (so does everything else written there before)"""
+        import torch
+        self.rows[:len(res) * _l.ANCHOR_RESULT_DTYPE.itemsize].copy_(torch.from_numpy(res.view(np.uint8).copy()))
+        self.stream.wait_stream(torch.cuda.current_stream())
+
+    def run(self, anchor: LoopAnchor, yaw_observable=None) -> int:
+        return anchor.run_dev(self.rows.data_ptr(), self.stream.cuda_stream, yaw_observable)
+
+    def reject(self, state: PcmState, n: int):
+        state.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), self.stream.cuda_stream)
+
+    def compact(self, n: int, keep: bool = True):
+        """the factor rows of the first n rows, with the keep mask or without it"""
+        compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr() if keep else None, *self.factors.ptrs(),
+                                 self.stream.cuda_stream)
+
+    def solve(self, solver: PoseGraphSolver, max_tail: int, options=None):
+        self.factors.solve(solver, max_tail, options, self.stream)
+
+    def keep_on_host(self, n: int) -> np.ndarray:
+        import torch
+        with torch.cuda.stream(self.stream):
+            return self.keep[:n].cpu().numpy()
+
+    def __call__(self, anchor: LoopAnchor, state: PcmState, yaw_observable=None) -> int:
+        """run -> reject -> compact on the chain's stream, without synchronising -> the number of rows"""
+        n = self.run(anchor, yaw_observable)
+        self.reject(state, n)
+        self.compact(n)
+        return n
 
 
 class Swarm(_Handle):

@@ -772,3 +772,44 @@ def anchor_swarm(n_drones: int = 5, n_frames: int = 60, n_meas: int = 400, seed:
     prm = dict(begin_min_loop_dt_s=1000.0, det_dpos_thres=1.0, odom_pos_cov_per_m=1e-3, odom_ang_cov_per_m=2e-4, huber=True)
     return dict(trajs=trajs, window=(frame_stamps, np.array(first, np.int32), entries), meas=meas,
                 max_drones=n_drones + 2, prm=prm)
+
+
+def _quat_yaw(q):
+    """the yaw of a unit quaternion wxyz (the z angle of its ZYX Euler angles)"""
+    w, x, y, z = q
+    return np.arctan2(2.0 * (w * z + x * y), 1.0 - 2.0 * (y * y + z * z))
+
+
+def anchor_window_graph(g: dict) -> dict:
+    """The pose graph of an anchor_swarm window, in the layout osb_solver_solve takes: one block per window pose block at
+    its entries' self pose (x, y, z, yaw), perturbed except the first, fixed one; an odometry factor (RELPOSE, the
+    4-DoF delta) between consecutive blocks of each drone and a UWB distance between the blocks of each frame."""
+    stamps, first, entries = g["window"]
+    rng = np.random.default_rng(1)
+    n = int(entries["block"].max()) + 1
+    truth = np.zeros((n, 4))
+    for e in entries:
+        truth[e["block"]] = np.r_[e["self_pose"][:3], _quat_yaw(e["self_pose"][3:])]
+    ftype, ia, ib, payload, huber, last = [], [], [], [], [], {}
+    for f in range(len(stamps)):
+        fe = entries[first[f]:first[f + 1]]
+        for e in fe:
+            d, b = int(e["drone_id"]), int(e["block"])
+            if d in last and last[d] != b:
+                pl = np.zeros(PAYLOAD_LEN)
+                pl[:4], pl[4:20] = _delta_pose(truth[last[d]], truth[b]), (np.eye(4) * 50.0).reshape(-1)
+                ftype.append(FACTOR_RELPOSE); ia.append(last[d]); ib.append(b); payload.append(pl); huber.append(0)
+            last[d] = b
+        for i in range(len(fe)):
+            for j in range(i + 1, len(fe)):
+                if fe[i]["block"] == fe[j]["block"]:
+                    continue
+                pl = np.zeros(PAYLOAD_LEN)
+                pl[0], pl[1] = np.linalg.norm(truth[fe[i]["block"], :3] - truth[fe[j]["block"], :3]), 10.0
+                ftype.append(FACTOR_DISTANCE); ia.append(int(fe[i]["block"])); ib.append(int(fe[j]["block"]))
+                payload.append(pl); huber.append(1)
+    fixed = np.zeros(n, np.uint8)
+    fixed[int(entries["block"][0])] = 1
+    init = truth + np.c_[rng.normal(0, 0.05, (n, 3)), rng.normal(0, 0.01, n)] * (1 - fixed[:, None])
+    return dict(init=init, fixed=fixed, ftype=np.array(ftype, np.int32), ia=np.array(ia, np.int32),
+                ib=np.array(ib, np.int32), payload=np.array(payload), huber=np.array(huber, np.uint8))

@@ -25,7 +25,6 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
-import torch  # noqa: E402
 
 from gpu_env import smi  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
@@ -33,42 +32,6 @@ from omniswarm_b200 import host, lib, synth  # noqa: E402
 SIZES = (6005, 60050, 600050)
 THRES = 15.0
 NEW_PER_PAIR = 4
-ROW = lib.ANCHOR_RESULT_DTYPE.itemsize
-
-
-def host_chain(a, st, yaw):
-    rows = a.run(yaw)
-    ok = rows["status"] == lib.ANCHOR_OK
-    keep = np.zeros(len(rows), np.uint8)
-    keep[ok] = st.reject(host.anchored_loop_edges(rows[ok]), rows["id"][ok])
-    return keep, host.anchored_factor_rows(rows, keep)
-
-
-class DeviceChain:
-    def __init__(self, cap):
-        self.rows = torch.empty(cap * ROW, dtype=torch.uint8, device="cuda")
-        self.keep = torch.empty(cap, dtype=torch.uint8, device="cuda")
-        self.type = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.ia = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.ib = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.payload = torch.empty(cap * lib.PAYLOAD_LEN, dtype=torch.float64, device="cuda")
-        self.huber = torch.empty(cap, dtype=torch.uint8, device="cuda")
-        self.count = torch.empty(1, dtype=torch.int32, device="cuda")
-        self.stream = torch.cuda.Stream()
-
-    def __call__(self, a, st, yaw):
-        s = self.stream.cuda_stream
-        n = a.run_dev(self.rows.data_ptr(), s, yaw)
-        st.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), s)
-        host.compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr(), self.type.data_ptr(),
-                                      self.ia.data_ptr(), self.ib.data_ptr(), self.payload.data_ptr(),
-                                      self.huber.data_ptr(), self.count.data_ptr(), s)
-        with torch.cuda.stream(self.stream):
-            k = int(self.count.cpu()[0])                             # the solve's one synchronisation ...
-            out = (self.type[:k].cpu().numpy(), self.ia[:k].cpu().numpy(), self.ib[:k].cpu().numpy(),
-                   self.payload[:k * lib.PAYLOAD_LEN].cpu().numpy().reshape(k, lib.PAYLOAD_LEN),
-                   self.huber[:k].cpu().numpy())                     # ... and the copy of the kept rows
-        return n, out
 
 
 def main():
@@ -96,9 +59,9 @@ def main():
         a.add_measurements(base)
         sa, sb = (host.PcmState(0, True, THRES, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"],
                                 max_pairs=15, pair_capacity=4096) for _ in range(2))
-        dev = DeviceChain(cap)
+        dev = host.AnchoredChain(cap)
         first_rows = a.run(yaw)
-        host_chain(a, sa, yaw)                                       # both states store the base ids
+        host.anchored_keep(sa, a.run(yaw))                           # both states store the base ids
         dev(a, sb, yaw)
         a.add_measurements(meas[len(base):])
         # per pair, its OK loops: the grow case re-submits them under new ids
@@ -126,17 +89,21 @@ def main():
                 for form in ((0, 1) if r % 2 == 0 else (1, 0)):
                     t0 = time.perf_counter()
                     if form == 0:
-                        keep_a, fa = host_chain(a, sa, yaw)
+                        rows = a.run(yaw)
+                        keep_a = host.anchored_keep(sa, rows)
+                        fa = host.anchored_factor_rows(rows, keep_a)
                     else:
-                        n, fb = dev(a, sb, yaw)
+                        n = dev(a, sb, yaw)
+                        fb = dev.factors.on_host(dev.stream)         # the solve's one synchronisation, one copy of the rows
                     ms = (time.perf_counter() - t0) * 1e3
                     if r >= args.warmup:
                         (ta if form == 0 else tb).append(ms)
-                same &= dev.keep[:n].cpu().numpy().tobytes() == keep_a.tobytes()
-                same &= all(x.tobytes() == y.tobytes() for x, y in zip(fa, fb))
+                same &= dev.keep_on_host(n).tobytes() == keep_a.tobytes()
+                same &= all(x.tobytes() == y.tobytes() for x, y in zip(fa, fb.values()))
             row[case] = {"host_sequence_ms_wall": float(np.median(ta)), "host_sequence_ms_min": float(np.min(ta)),
                          "device_chain_ms_wall": float(np.median(tb)), "device_chain_ms_min": float(np.min(tb)),
-                         "speedup": float(np.median(ta) / np.median(tb)), "rows": int(n), "factors": int(len(fb[0]))}
+                         "speedup": float(np.median(ta) / np.median(tb)), "rows": int(n),
+                         "factors": int(len(fb["ftype"]))}
         row["identical"] = bool(same and sb.status() == lib.OK)
         out["sizes"].append(row)
         print(json.dumps(row), file=sys.stderr)

@@ -29,77 +29,7 @@ from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 THRES = 15.0
 NEW_PER_PAIR = 4
-ROW = lib.ANCHOR_RESULT_DTYPE.itemsize
-KEYS = ("ftype", "ia", "ib", "payload", "huber")
-
-
-def _yaw(q):
-    w, x, y, z = q
-    return np.arctan2(2 * (w * z + x * y), 1 - 2 * (y * y + z * z))
-
-
-def window_graph(g):
-    """the window's pose blocks (entries' self poses, perturbed) with odometry between consecutive blocks of each drone
-    and UWB distances between the drones of each frame"""
-    stamps, first, entries = g["window"]
-    rng = np.random.default_rng(1)
-    n = int(entries["block"].max()) + 1
-    truth = np.zeros((n, 4))
-    for e in entries:
-        truth[e["block"]] = np.r_[e["self_pose"][:3], _yaw(e["self_pose"][3:])]
-    ftype, ia, ib, payload, huber, last = [], [], [], [], [], {}
-    for f in range(len(stamps)):
-        fe = entries[first[f]:first[f + 1]]
-        for e in fe:
-            d, b = int(e["drone_id"]), int(e["block"])
-            if d in last and last[d] != b:
-                A, B = truth[last[d]], truth[b]
-                c, s = np.cos(A[3]), np.sin(A[3])
-                dx = B[:3] - A[:3]
-                pl = np.zeros(lib.PAYLOAD_LEN)
-                pl[:4] = [c * dx[0] + s * dx[1], -s * dx[0] + c * dx[1], dx[2], B[3] - A[3]]
-                pl[4:20] = (np.eye(4) * 50.0).reshape(-1)
-                ftype.append(1); ia.append(last[d]); ib.append(b); payload.append(pl); huber.append(0)
-            last[d] = b
-        for i in range(len(fe)):
-            for j in range(i + 1, len(fe)):
-                if fe[i]["block"] == fe[j]["block"]:
-                    continue
-                pl = np.zeros(lib.PAYLOAD_LEN)
-                pl[0], pl[1] = np.linalg.norm(truth[fe[i]["block"], :3] - truth[fe[j]["block"], :3]), 10.0
-                ftype.append(0); ia.append(int(fe[i]["block"])); ib.append(int(fe[j]["block"])); payload.append(pl)
-                huber.append(1)
-    fixed = np.zeros(n, np.uint8)
-    fixed[int(entries["block"][0])] = 1
-    init = truth + np.c_[rng.normal(0, 0.05, (n, 3)), rng.normal(0, 0.01, n)] * (1 - fixed[:, None])
-    return dict(init=init, fixed=fixed, ftype=np.array(ftype, np.int32), ia=np.array(ia, np.int32),
-                ib=np.array(ib, np.int32), payload=np.array(payload), huber=np.array(huber, np.uint8))
-
-
-class Chain:
-    def __init__(self, cap):
-        self.rows = torch.empty(cap * ROW, dtype=torch.uint8, device="cuda")
-        self.keep = torch.empty(cap, dtype=torch.uint8, device="cuda")
-        self.type = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.ia = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.ib = torch.empty(cap, dtype=torch.int32, device="cuda")
-        self.payload = torch.empty(cap * lib.PAYLOAD_LEN, dtype=torch.float64, device="cuda")
-        self.huber = torch.empty(cap, dtype=torch.uint8, device="cuda")
-        self.count = torch.empty(1, dtype=torch.int32, device="cuda")
-        self.stream = torch.cuda.Stream()
-
-    def rows_to_soa(self, a, st):
-        s = self.stream.cuda_stream
-        n = a.run_dev(self.rows.data_ptr(), s)
-        st.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), s)
-        host.compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr(), self.type.data_ptr(),
-                                      self.ia.data_ptr(), self.ib.data_ptr(), self.payload.data_ptr(),
-                                      self.huber.data_ptr(), self.count.data_ptr(), s)
-
-    def resident_solve(self, solver, max_tail, o):
-        solver.solve_resident_dev(max_tail, self.type.data_ptr(), self.ia.data_ptr(), self.ib.data_ptr(),
-                                  self.payload.data_ptr(), self.huber.data_ptr(), self.count.data_ptr(),
-                                  self.stream.cuda_stream, o)
+KEYS = host.FACTOR_KEYS
 
 
 def main():
@@ -110,7 +40,7 @@ def main():
     L = lib.load()
     assert L.osb_device_count() > 0, "needs a CUDA device"
     g = synth.anchor_swarm(5, 400, 6005, seed=0, with_orphans=False)
-    base = window_graph(g)
+    base = synth.anchor_window_graph(g)
     n_nodes, m_base = len(base["init"]), len(base["ftype"])
     rounds = args.warmup + args.reps
     cap = len(g["meas"]) + 15 * NEW_PER_PAIR * rounds + 64
@@ -123,7 +53,7 @@ def main():
     states = [host.PcmState(0, True, THRES, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"],
                             max_pairs=15, pair_capacity=4096) for _ in range(3)]
     solvers = [host.PoseGraphSolver(4096, 32768) for _ in range(3)]
-    chains = [Chain(cap) for _ in range(3)]
+    chains = [host.AnchoredChain(cap) for _ in range(3)]
     for s in solvers[1:]:
         s.graph_add_nodes(base["init"], base["fixed"])
         s.graph_add_factors(*(base[k] for k in KEYS))
@@ -136,20 +66,17 @@ def main():
     def path_a():
         nonlocal pose_a
         c = chains[0]
-        c.rows_to_soa(a, states[0])
-        with torch.cuda.stream(c.stream):
-            k = int(c.count.cpu()[0])
-            tail = (c.type[:k].cpu().numpy(), c.ia[:k].cpu().numpy(), c.ib[:k].cpu().numpy(),
-                    c.payload[:k * lib.PAYLOAD_LEN].cpu().numpy().reshape(k, lib.PAYLOAD_LEN), c.huber[:k].cpu().numpy())
-        gg = {key: np.concatenate([base[key], t]) for key, t in zip(KEYS, tail)}
+        c(a, states[0])
+        tail = c.factors.on_host(c.stream)
+        gg = {key: np.concatenate([base[key], tail[key]]) for key in KEYS}
         gg["fixed"] = base["fixed"]
         pose_a, s = solvers[0].solve(gg, o, init=pose_a)
-        return s, k
+        return s, len(tail["ftype"])
 
     def path_b():
         c = chains[1]
-        c.rows_to_soa(a, states[1])
-        c.resident_solve(solvers[1], max_tail, o)
+        c(a, states[1])
+        c.solve(solvers[1], max_tail, o)
         p = solvers[1].graph_get_poses()
         return solvers[1].last_summary(), p
 
@@ -159,13 +86,13 @@ def main():
         nonlocal graph
         c = chains[2]
         if graph is None:                                    # the first solve runs uncaptured, then the chain is captured
-            c.rows_to_soa(a, states[2])
-            c.resident_solve(solvers[2], max_tail, o)
+            c(a, states[2])
+            c.solve(solvers[2], max_tail, o)
             p = solvers[2].graph_get_poses()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph, stream=c.stream, capture_error_mode="global"):
-                c.rows_to_soa(a, states[2])
-                c.resident_solve(solvers[2], max_tail, o)
+                c(a, states[2])
+                c.solve(solvers[2], max_tail, o)
             return None, p
         graph.replay()
         torch.cuda.synchronize()                             # a replay is not a library call: the caller waits for it

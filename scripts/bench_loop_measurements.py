@@ -29,12 +29,11 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from gpu_env import smi  # noqa: E402
-from bench_backend_solve import window_graph  # noqa: E402
 from omniswarm_b200 import host, lib, synth  # noqa: E402
 
 ND, MN = 4, 200
 RB, RS, EB = lib.RECORD_BYTES, lib.RESULT_BYTES, lib.EDGE_BYTES
-MB, ROW = lib.MEASUREMENT_DTYPE.itemsize, lib.ANCHOR_RESULT_DTYPE.itemsize
+MB = lib.MEASUREMENT_DTYPE.itemsize
 SC = synth.LOOP_SCENE
 SELF, MAX_LOOP_ID = 1, 100000000
 COV_POS, COV_ANG, THRES = 0.02, 0.005, 2.0
@@ -72,7 +71,7 @@ def entry_stamps(g, drone):
 
 
 class Backend:
-    """anchor + PCM state + resident solver, and the device buffers of one solve's chain"""
+    """anchor + PCM state + resident solver, and one solve's chain on the current stream"""
 
     def __init__(self, g, base, cap):
         self.a = host.LoopAnchor(g["max_drones"], max(len(v[0]) for v in g["trajs"].values()), cap, len(g["window"][2]),
@@ -88,19 +87,11 @@ class Backend:
         self.solver.graph_add_factors(base["ftype"], base["ia"], base["ib"], base["payload"], base["huber"])
         self.o = self.solver.default_options()
         self.cap = cap
-        self.rows = torch.empty(cap * ROW, dtype=torch.uint8, device="cuda")
-        self.keep = torch.empty(cap, dtype=torch.uint8, device="cuda")
-        self.soa = [torch.empty(cap * w, dtype=dt, device="cuda") for w, dt in
-                    ((1, torch.int32), (1, torch.int32), (1, torch.int32), (lib.PAYLOAD_LEN, torch.float64),
-                     (1, torch.uint8), (1, torch.int32))]
+        self.chain = host.AnchoredChain(cap, torch.cuda.current_stream())
 
-    def solve(self, st):
-        n = self.a.run_dev(self.rows.data_ptr(), st)
-        self.pcm.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), st)
-        host.compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr(), *(t.data_ptr() for t in self.soa), st)
-        t = self.soa
-        self.solver.solve_resident_dev(self.cap, t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(),
-                                       t[4].data_ptr(), t[5].data_ptr(), st, self.o)
+    def solve(self):
+        self.chain(self.a, self.pcm)
+        self.chain.solve(self.solver, self.cap, self.o)
 
     def close(self):
         for h in (self.pcm, self.solver, self.a):
@@ -134,7 +125,7 @@ def main():
     fe.compute_loop(rt.data_ptr(), res_t.data_ptr(), cands, edges_t.data_ptr(), st)
     fe.finish(st)
     g = synth.anchor_swarm(5, 60, 600, seed=0, with_orphans=False)
-    base = window_graph(g)
+    base = synth.anchor_window_graph(g)
     own = entry_stamps(g, SELF)
     stamps = [(int(entry_stamps(g, 2 + r % 3)[(7 * r + 3) % 40]), int(own[(5 * r + 1) % 40])) for r in range(64)]
     calls = a.warmup + a.reps + 1 + a.host_reps
@@ -184,11 +175,11 @@ def main():
                     fe.loop_measurements(res_t.data_ptr(), edges_t.data_ptr(), cands[:n], stamps[:n], COV_POS, COV_ANG,
                                          meas_t.data_ptr(), cnt_t.data_ptr(), st)
                     dev.a.add_measurements_dev(meas_t.data_ptr(), cnt_t.data_ptr(), n, THRES, st)
-                    dev.solve(st)
+                    dev.solve()
                 else:
                     rows, lc_host = host_rows(edges_t, res_t, n, cands, stamps, lc_host)
                     hop.a.add_measurements(rows)
-                    hop.solve(st)
+                    hop.solve()
                 (dev if form == 0 else hop).solver.graph_get_poses()             # synchronises with the solve
                 if r >= 1:
                     tr[form].append((time.perf_counter() - t0) * 1e3)

@@ -1,5 +1,6 @@
 """What the keyframe front-end's GPU tests share: synthetic frames, a front-end of the synthetic networks, device records
-and results, and oracle/loop_ref.compute_loop fed a device query result.  Test modules import it as `frontend_harness`."""
+and results, the loop scene's front-end and own-keyframe query, and oracle/loop_ref.compute_loop fed a device query result.
+Test modules import it as `frontend_harness`."""
 import numpy as np
 import torch
 
@@ -61,6 +62,44 @@ def records(t, n):
 def edges(t, n):
     """the raw bytes of n loop edges"""
     return _split(t, n, EB)
+
+
+# ---- the loop scene (synth.LOOP_SCENE) seen by a stereo front-end with loop parameters ------------------------------
+SC = synth.LOOP_SCENE
+LOOP_COV = np.eye(6) * 0.01
+LOOP_PARAMS = dict(odometry_consistency_threshold=10.0, seed=3)
+LOOP_CONFIG = dict(db_capacity=64, init_mode_product_thres=0.2, match_index_dist=5, geometric_filter=True, ransac_seed=0)
+
+
+def loop_frontend(cameras="stereo", loop_params=True, **kw):
+    """make_frontend(LOOP_CONFIG, **kw) with the scene's cameras ("stereo", "depth", "both" or None) and LOOP_PARAMS"""
+    fe = make_frontend(LOOP_CONFIG, **kw)
+    if cameras in ("stereo", "both"):
+        fe.set_cameras(SC["K"], SC["ext"], SC["ext"], 0.006)
+    if cameras in ("depth", "both"):
+        fe.set_depth_camera(SC["K"], SC["ext"])
+    if loop_params:
+        fe.set_loop_params(**LOOP_PARAMS)
+    return fe
+
+
+def own_query(fe, st, old_rec, new_rec, nonkeyframe=False, ingest_old=True):
+    """ingest the old record, then the new one (own, as on_image_recv does), query the new one -> (rec_t, res_t, result)"""
+    if ingest_old:
+        ot = upload([old_rec])
+        fe.ingest_own(ot.data_ptr(), st)
+    rt = upload([new_rec])
+    fe.ingest_own(rt.data_ptr(), st)
+    res_t = filled(RS)
+    fe.query(rt.data_ptr(), res_t.data_ptr(), st, nonkeyframe=nonkeyframe)
+    fe.finish(st)
+    return rt, res_t, results(res_t, 1)[0]
+
+
+def cand_own(init_mode=False, odom=None):
+    """the candidate of an own query of the new keyframe hitting the old one"""
+    return dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], init_mode=init_mode,
+                odom_rel=SC["delta_true"] if odom is None else odom, cov=LOOP_COV)
 
 
 # ---- the loop-edge oracle --------------------------------------------------------------------------------------------

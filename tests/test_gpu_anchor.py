@@ -5,7 +5,8 @@ import pytest
 import torch
 
 from omniswarm_b200 import host, lib as _l, synth
-from oracle import anchor_ref as ar, pnp_ref as pn, solver_ref as sr
+from oracle import anchor_ref as ar
+from backend_harness import feed, make_anchor, pcm_state
 
 pytestmark = pytest.mark.gpu
 INT_FIELDS = ("id", "type", "status", "frame_a", "frame_b", "node_a", "node_b", "stamp_a", "stamp_b", "dt_err_ns", "skip",
@@ -31,23 +32,6 @@ def check(res, ref):
         close(res["edge"][f], ref["edge"][f])
 
 
-def make(g, max_meas=None, max_entries=None):
-    s = g["trajs"]
-    return host.LoopAnchor(g["max_drones"], max(len(v[0]) for v in s.values()) + 64, max_meas or len(g["meas"]) + 64,
-                           max_entries or len(g["window"][2]) + 64, g["prm"]["det_dpos_thres"],
-                           g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"], g["prm"]["begin_min_loop_dt_s"])
-
-
-def feed(a, g, chunks=3):
-    for d, (st, p) in g["trajs"].items():
-        for c in np.array_split(np.arange(len(st)), chunks):             # only new samples cross PCIe, length continues
-            a.push_odometry(d, st[c], p[c])
-    m = g["meas"]
-    a.add_measurements(m[: len(m) // 3])
-    a.add_measurements(m[len(m) // 3:])
-    a.set_window(*g["window"])
-
-
 def oracle(g, yaw=None, window=None):
     yaw = np.ones(g["max_drones"], np.uint8) if yaw is None else yaw
     return ar.anchor(g["trajs"], window or g["window"], g["meas"], yaw, g["prm"])
@@ -56,7 +40,7 @@ def oracle(g, yaw=None, window=None):
 @pytest.mark.parametrize("seed", [0, 1])
 def test_matches_oracle_on_a_synthetic_swarm(gpu, seed):
     g = synth.anchor_swarm(5, 60, 600, seed=seed)
-    a = make(g)
+    a = make_anchor(g)
     feed(a, g)
     yaw = np.ones(g["max_drones"], np.uint8)
     yaw[2] = 0
@@ -79,7 +63,7 @@ def test_matches_oracle_on_a_synthetic_swarm(gpu, seed):
 
 def test_window_slides_over_several_runs(gpu):
     g = synth.anchor_swarm(4, 50, 400, seed=5)
-    a = make(g, max_meas=2000)
+    a = make_anchor(g, max_meas=2000)
     feed(a, g)
     rng = np.random.default_rng(0)
     stamps, first, entries = g["window"]
@@ -111,8 +95,7 @@ def test_window_slides_over_several_runs(gpu):
 
 def test_capacity_and_invalid_input_leave_the_handle_unchanged(gpu):
     g = synth.anchor_swarm(3, 20, 100, seed=7)
-    a = host.LoopAnchor(g["max_drones"], max(len(v[0]) for v in g["trajs"].values()), 100, len(g["window"][2]),
-                        g["prm"]["det_dpos_thres"], g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"])
+    a = make_anchor(g, 100, len(g["window"][2]), traj_margin=0)
     feed(a, g)
     before = a.run()
     check(before, oracle(g))
@@ -140,7 +123,7 @@ def test_capacity_and_invalid_input_leave_the_handle_unchanged(gpu):
 def test_empty_window_and_resources(gpu):
     live = host.live_resources()
     g = synth.anchor_swarm(3, 10, 50, seed=8)
-    a = make(g)
+    a = make_anchor(g)
     feed(a, g)
     a.set_window(np.zeros(0, np.int64), np.zeros(1, np.int32), np.zeros(0, _l.WINDOW_ENTRY_DTYPE))
     res = a.run()
@@ -150,51 +133,13 @@ def test_empty_window_and_resources(gpu):
     assert host.live_resources() == live
 
 
-def window_graph(g):
-    """the window's pose blocks (x, y, z, yaw of the entries' self poses, perturbed) with odometry factors between
-    consecutive blocks of each drone and UWB distances between the drones of each frame"""
-    stamps, first, entries = g["window"]
-    rng = np.random.default_rng(1)
-    n = int(entries["block"].max()) + 1
-    truth = np.zeros((n, 4))
-    for e in entries:
-        truth[e["block"]] = np.r_[e["self_pose"][:3], pn.quat2eulers(e["self_pose"][3:])[2]]
-    ftype, ia, ib, payload, huber = [], [], [], [], []
-    last = {}
-    for f in range(len(stamps)):
-        fe = entries[first[f]:first[f + 1]]
-        for e in fe:
-            d, b = int(e["drone_id"]), int(e["block"])
-            if d in last and last[d] != b:
-                a0 = truth[last[d]]
-                dp = pn.delta_pose(np.r_[a0[:3], pn.quat_from_rotvec(np.r_[0, 0, a0[3]])],
-                                   np.r_[truth[b][:3], pn.quat_from_rotvec(np.r_[0, 0, truth[b][3]])], True)
-                pl = np.zeros(24)
-                pl[:3], pl[3], pl[4:20] = dp[:3], pn.quat2eulers(dp[3:])[2], (np.eye(4) * 50.0).reshape(-1)
-                ftype.append(sr.FACTOR_RELPOSE); ia.append(last[d]); ib.append(b); payload.append(pl); huber.append(0)
-            last[d] = b
-        for i in range(len(fe)):
-            for j in range(i + 1, len(fe)):
-                if fe[i]["block"] == fe[j]["block"]:
-                    continue
-                pl = np.zeros(24)
-                pl[0], pl[1] = np.linalg.norm(truth[fe[i]["block"], :3] - truth[fe[j]["block"], :3]), 10.0
-                ftype.append(sr.FACTOR_DISTANCE); ia.append(int(fe[i]["block"])); ib.append(int(fe[j]["block"]))
-                payload.append(pl); huber.append(1)
-    fixed = np.zeros(n, np.uint8)
-    fixed[int(entries["block"][0])] = 1
-    init = truth + np.c_[rng.normal(0, 0.05, (n, 3)), rng.normal(0, 0.01, n)] * (1 - fixed[:, None])
-    return dict(init=init, fixed=fixed, ftype=np.array(ftype, np.int32), ia=np.array(ia, np.int32),
-                ib=np.array(ib, np.int32), payload=np.array(payload), huber=np.array(huber, np.uint8))
-
-
 def test_factor_rows_feed_the_solver_as_the_oracles_do(gpu):
     g = synth.anchor_swarm(4, 30, 300, seed=9, with_orphans=False)
-    a = make(g)
+    a = make_anchor(g)
     feed(a, g)
     res = a.run()
     ref = oracle(g)
-    base = window_graph(g)
+    base = synth.anchor_window_graph(g)
     solver = host.PoseGraphSolver(4096, 32768)
     o = solver.default_options()
     o.function_tolerance = 1e-14; o.gradient_tolerance = 1e-11; o.parameter_tolerance = 1e-12
@@ -209,9 +154,7 @@ def test_factor_rows_feed_the_solver_as_the_oracles_do(gpu):
         poses.append(p)
     assert np.abs(poses[0] - poses[1]).max() < 1e-5
     # the re-anchored edges go to the PCM state as they are
-    keep = host.PcmState(0, True, 15.0, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"], max_pairs=16,
-                         pair_capacity=512).reject(host.anchored_loop_edges(res[res["status"] == 0]),
-                                                   res["id"][res["status"] == 0])
+    keep = pcm_state(g, 16, 512).reject(host.anchored_loop_edges(res[res["status"] == 0]), res["id"][res["status"] == 0])
     assert keep.any()
     solver.close()
     a.close()

@@ -10,47 +10,21 @@ import numpy as np
 import pytest
 
 from omniswarm_b200 import synth, host, lib
-from frontend_harness import EB, RB, RS, filled, loop_oracle, upload
+from frontend_harness import (EB, LOOP_COV, LOOP_PARAMS, RB, RS, SC, cand_own, filled, loop_frontend, loop_oracle,
+                              own_query, upload)
 import frontend_harness as fh
 
 pytestmark = pytest.mark.gpu
 
 ND, MN = 4, 200
 QDIR = 1
-SC, NPT = synth.LOOP_SCENE, synth.LOOP_NPT
-COV = np.eye(6) * 0.01
-PARAMS = dict(odometry_consistency_threshold=10.0, seed=3)
-CONFIG = dict(db_capacity=64, init_mode_product_thres=0.2, match_index_dist=5, geometric_filter=True, ransac_seed=0)
+NPT = synth.LOOP_NPT
 record, noisy_g = synth.loop_record, synth.loop_noisy_g
-
-
-def make_frontend(cameras="stereo", loop_params=True, **kw):
-    fe = fh.make_frontend(CONFIG, **kw)
-    if cameras in ("stereo", "both"):
-        fe.set_cameras(SC["K"], SC["ext"], SC["ext"], 0.006)
-    if cameras in ("depth", "both"):
-        fe.set_depth_camera(SC["K"], SC["ext"])
-    if loop_params:
-        fe.set_loop_params(**PARAMS)
-    return fe
 
 
 def oracle(res, query_rec, hit_rec, cand, params=None, K=None):
     return loop_oracle(res, query_rec, hit_rec, cand, SC["K"] if K is None else K, SC["ext"],
-                       dict(PARAMS, **(params or {})), QDIR)
-
-
-def own_query(fe, st, old_rec, new_rec, nonkeyframe=False, ingest_old=True):
-    """ingest the old record, then the new one (own, as on_image_recv does), query the new one -> (rec_t, res_t, result)"""
-    if ingest_old:
-        ot = upload([old_rec])
-        fe.ingest_own(ot.data_ptr(), st)
-    rt = upload([new_rec])
-    fe.ingest_own(rt.data_ptr(), st)
-    res_t = filled(RS)
-    fe.query(rt.data_ptr(), res_t.data_ptr(), st, nonkeyframe=nonkeyframe)
-    fe.finish(st)
-    return rt, res_t, fh.results(res_t, 1)[0]
+                       dict(LOOP_PARAMS, **(params or {})), QDIR)
 
 
 def run_loop(fe, st, rec_ptr, res_ptr, cands):
@@ -94,14 +68,9 @@ def same_pnp(a, b):
     return bytes(a) == bytes(b)
 
 
-def cand_own(init_mode=False, odom=None):
-    return dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], init_mode=init_mode,
-                odom_rel=SC["delta_true"] if odom is None else odom, cov=COV)
-
-
 def test_own_query_local_hit_and_pnp_inputs(gpu):
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=1, g=noisy_g(1))
     rt, res_t, res = own_query(fe, st, old, new)
     assert res.accepted and not res.swapped and res.hit_dir == QDIR and sum(res.geo_valid) == ND
@@ -122,7 +91,7 @@ def test_own_query_local_hit_and_pnp_inputs(gpu):
 def test_own_query_remote_hit_is_swapped(gpu):
     """the own keyframe hits a remote one: new = the remote keyframe, its 3-D landmarks read from the remote store"""
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     remote = record(2, 200, "new", seed=2, g=noisy_g(2))
     t = upload([remote])
     fe.ingest(t.data_ptr(), 1, -1, st)
@@ -143,7 +112,7 @@ def test_received_batch_equals_single_calls(gpu):
     """a round of 10 received keyframes: hits with outliers, a failed homography pair (the 1-3-match quirk), init mode,
     misses; one call for all, each equal to its one-candidate call and to the oracle"""
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     old = record(1, 100, "old")
     ot = upload([old])
     fe.ingest_own(ot.data_ptr(), st)
@@ -154,7 +123,7 @@ def test_received_batch_equals_single_calls(gpu):
         recs.append(record(2 + r % 3, 300 + r, "new", seed=20 + r, g=g, n_outliers=2 + r % 4,
                            few_flags_dir=(r % 4) if r in (1, 6) else None))
         cands.append(dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], init_mode=(r == 2),
-                          odom_rel=rng.normal(size=7), cov=COV))
+                          odom_rel=rng.normal(size=7), cov=LOOP_COV))
     rt = upload(recs)
     res_t = filled(10 * RS)
     fe.query_received(rt.data_ptr(), 10, -1, res_t.data_ptr(), st, init_mode=[c["init_mode"] for c in cands])
@@ -177,9 +146,9 @@ def test_depth_keyframe_camera(gpu):
     """a depth-camera handle lifts the old frame through set_depth_camera's pinhole and extrinsics"""
     st = fh.stream()
     K2 = np.array([80.0, 80.0, 40.0, 30.0])
-    fe = make_frontend(cameras=None, loop_params=False)
+    fe = loop_frontend(cameras=None, loop_params=False)
     fe.set_depth_camera(K2, SC["ext"])
-    fe.set_loop_params(**PARAMS)
+    fe.set_loop_params(**LOOP_PARAMS)
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=3, g=noisy_g(3))
     rt, res_t, res = own_query(fe, st, old, new)
     cand = cand_own()
@@ -190,14 +159,14 @@ def test_depth_keyframe_camera(gpu):
 
 def test_every_status_code(gpu):
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=4, g=noisy_g(4))
     rt, res_t, res = own_query(fe, st, old, new)
     seen = {}
     by_msg = {100: old, 101: new}
 
     def go(params, cand, rec=new, rt_=rt, res_t_=res_t, res_=res):
-        fe.set_loop_params(**dict(PARAMS, **params))
+        fe.set_loop_params(**dict(LOOP_PARAMS, **params))
         raw = run_loop(fe, st, rt_.data_ptr(), res_t_.data_ptr(), [cand])[0]
         e = check(raw, oracle(res_, rec, by_msg.get(res_.hit_msg_id), cand, params))
         seen[e.status] = seen.get(e.status, 0) + 1
@@ -222,7 +191,7 @@ def test_every_status_code(gpu):
     assert go({}, cand_own(), miss, mt, mres_t, mres).status == lib.LOOP_NO_HIT
     fe.close()
     # a row put in with db_load has no keyframe behind it
-    fe = make_frontend()
+    fe = loop_frontend()
     q = record(1, 101, "new", seed=4, g=noisy_g(4))
     fe.db_load(np.stack([np.ctypeslib.as_array(q.global_desc[QDIR])]), synth.local_descriptors(MN, 3)[None],
                np.array([NPT], np.int32))
@@ -239,7 +208,7 @@ def test_every_status_code(gpu):
 def test_arguments_errors_and_resources(gpu):
     st = fh.stream()
     base = host.live_resources()
-    fe = make_frontend()
+    fe = loop_frontend()
     L = fe._lib
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=1, g=noisy_g(1))
     rt, res_t, res = own_query(fe, st, old, new)
@@ -277,16 +246,16 @@ def test_arguments_errors_and_resources(gpu):
         fe.close()
 
     call = lambda fe: lambda: fe.compute_loop(rt.data_ptr(), res_t.data_ptr(), [cand_own()], out.data_ptr(), st)
-    f = make_frontend(loop_params=False); refused(f, call(f))                  # no loop parameters
-    f = make_frontend(cameras=None); refused(f, call(f))                       # no camera
-    f = make_frontend(cameras="both"); refused(f, call(f))                     # two cameras
-    f = make_frontend(geometric_filter=False); refused(f, call(f))             # the reference's USE_FUNDMENTAL path only
-    f = make_frontend(loop_params=False)                                       # after a remote ingest: no 3-D plane
+    f = loop_frontend(loop_params=False); refused(f, call(f))                  # no loop parameters
+    f = loop_frontend(cameras=None); refused(f, call(f))                       # no camera
+    f = loop_frontend(cameras="both"); refused(f, call(f))                     # two cameras
+    f = loop_frontend(geometric_filter=False); refused(f, call(f))             # the reference's USE_FUNDMENTAL path only
+    f = loop_frontend(loop_params=False)                                       # after a remote ingest: no 3-D plane
     t = upload([record(2, 200, "new")])
     f.ingest(t.data_ptr(), 1, -1, st)
     refused(f, lambda: f.set_loop_params())
     # without set_loop_params nothing is allocated
-    f = make_frontend(loop_params=False)
+    f = loop_frontend(loop_params=False)
     live = host.live_resources()
     f.ingest(t.data_ptr(), 1, -1, st)
     f.finish(st)

@@ -10,18 +10,17 @@ import pytest
 import torch
 
 from omniswarm_b200 import host, lib, synth
-from frontend_harness import EB, RS, filled, upload
+from frontend_harness import EB, LOOP_COV, RS, SC, cand_own, filled, loop_frontend, own_query, upload
 import frontend_harness as fh
 import loop_measurements_ref as lm
-from test_gpu_loop_edge import SC, COV, make_frontend, own_query, cand_own, record, noisy_g
-from test_gpu_anchor import make, window_graph
-from test_gpu_solver_device_tail import DeviceChain, resident, options
+from backend_harness import make_anchor, options, pcm_state, resident
 
 pytestmark = pytest.mark.gpu
 
 MB, ROW = lib.MEASUREMENT_DTYPE.itemsize, lib.ANCHOR_RESULT_DTYPE.itemsize
 COV_POS, COV_ANG = 0.02, 0.005
 SELF = fh.FRONTEND["self_id"]
+record, noisy_g = synth.loop_record, synth.loop_noisy_g
 
 
 def edge_dicts(raw):
@@ -67,7 +66,7 @@ def check_round(fe, st, res_t, results, edges_t, raw, cands, stamps, counters):
 
 def test_rows_and_counters_equal_the_oracle(gpu):
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     counters = lm.new_counters()
     assert fe.loop_counts()[0] == 0
     # round 1: an own keyframe hits an own one (intra-drone, unswapped); the second candidate fails the odometry check
@@ -86,7 +85,7 @@ def test_rows_and_counters_equal_the_oracle(gpu):
     for r in range(10):
         g = noisy_g(10 + r) if r % 5 != 4 else synth.descriptor_db(4, 4096, 300 + r)
         recs.append(record(2 + r % 3, 300 + r, "new", seed=20 + r, g=g, n_outliers=2 + r % 4))
-        cands.append(dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], cov=COV))
+        cands.append(dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], cov=LOOP_COV))
     rt = upload(recs)
     res_t = filled(10 * RS)
     fe.query_received(rt.data_ptr(), 10, -1, res_t.data_ptr(), st)
@@ -110,7 +109,7 @@ def test_rows_and_counters_equal_the_oracle(gpu):
     assert n == counters[0] and np.array_equal(pairs, counters[1])
     fe.close()
     # a swapped round, n = 1: the own keyframe hits a remote one, so the query record is the old side
-    fe = make_frontend()
+    fe = loop_frontend()
     remote = record(2, 200, "new", seed=2, g=noisy_g(2))
     t = upload([remote])
     fe.ingest(t.data_ptr(), 1, -1, st)
@@ -144,7 +143,7 @@ def test_device_appends_equal_host_appends(gpu):
     g = synth.anchor_swarm(4, 30, 300, seed=11, with_orphans=False)
     meas = g["meas"]
     thr = float(np.float32(np.median(loop_distances(meas))))
-    a, b = make(g, max_meas=1024), make(g, max_meas=1024)
+    a, b = make_anchor(g, max_meas=1024), make_anchor(g, max_meas=1024)
     for h in (a, b):
         prepare(h, g)
     st = fh.stream()
@@ -164,45 +163,40 @@ def test_device_appends_equal_host_appends(gpu):
         b.add_measurements_dev(buf.data_ptr(), cnt.data_ptr(), len(ch) + 5, thr, st)
         assert host.launch_count() - c0 == 1
     cap = len(meas) + 64
-    rows_a, rows_b = (torch.zeros(cap * ROW, dtype=torch.uint8, device="cuda") for _ in range(2))
-    nb = b.run_dev(rows_b.data_ptr(), st)                     # before anything synchronises: the bound
-    na = a.run_dev(rows_a.data_ptr(), st)
+    ca, cb = (host.AnchoredChain(cap, torch.cuda.current_stream()) for _ in range(2))
+    nb = cb.run(b)                                            # before anything synchronises: the bound
+    na = ca.run(a)
     assert na == sum(a.size()) and na < nb <= na + len(chunks[-1]) + 5
-    ra = rows_a[:na * ROW].cpu().numpy().tobytes()
-    rb = rows_b[:nb * ROW].cpu().numpy().tobytes()
+    ra = ca.rows[:na * ROW].cpu().numpy().tobytes()
+    rb = cb.rows[:nb * ROW].cpu().numpy().tobytes()
     assert rb[:na * ROW] == ra
     void = np.frombuffer(rb[na * ROW:], lib.ANCHOR_RESULT_DTYPE)
     ref = np.zeros(nb - na, lib.ANCHOR_RESULT_DTYPE)
     ref["status"], ref["skip"] = lib.ANCHOR_VOID, 1
     assert void.tobytes() == ref.tobytes()
     # PCM and the factor compaction pass over the VOID rows
-    pa, pb = (host.PcmState(0, True, 15.0, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"], max_pairs=16,
-                            pair_capacity=1024) for _ in range(2))
-    ka, kb = (torch.full((cap,), 9, dtype=torch.uint8, device="cuda") for _ in range(2))
-    pa.reject_anchored(rows_a.data_ptr(), na, ka.data_ptr(), st)
-    pb.reject_anchored(rows_b.data_ptr(), nb, kb.data_ptr(), st)
-    soa = []
-    for rows, n, keep in ((rows_a, na, ka), (rows_b, nb, kb)):
-        t = [torch.zeros(cap * w, dtype=dt, device="cuda") for w, dt in
-             ((1, torch.int32), (1, torch.int32), (1, torch.int32), (lib.PAYLOAD_LEN, torch.float64), (1, torch.uint8),
-              (1, torch.int32))]
-        host.compact_anchored_factors(rows.data_ptr(), n, keep.data_ptr(), *(x.data_ptr() for x in t), st)
-        soa.append(t)
+    pa, pb = (pcm_state(g, 16, 1024) for _ in range(2))
+    for c, h, n in ((ca, pa, na), (cb, pb, nb)):
+        c.keep.fill_(9)
+        c.reject(h, n)
+        c.compact(n)
     torch.cuda.synchronize()
     assert pa.status() == pb.status() == lib.OK
-    assert ka[:na].cpu().numpy().tobytes() == kb[:na].cpu().numpy().tobytes() and not kb[na:nb].cpu().numpy().any()
-    assert ka[:na].cpu().numpy().any()
-    k = int(soa[0][5].cpu()[0])
-    assert k > 0 and int(soa[1][5].cpu()[0]) == k
-    for x, y, w in zip(soa[0][:5], soa[1][:5], (1, 1, 1, lib.PAYLOAD_LEN, 1)):
-        assert x[:k * w].cpu().numpy().tobytes() == y[:k * w].cpu().numpy().tobytes()
+    ka, kb = ca.keep_on_host(na), cb.keep_on_host(nb)
+    assert ka.tobytes() == kb[:na].tobytes() and not kb[na:nb].any()
+    assert ka.any()
+    fa, fb = ca.factors.on_host(), cb.factors.on_host()
+    k = len(fa["ftype"])
+    assert k > 0 and len(fb["ftype"]) == k
+    for key in fa:
+        assert fa[key].tobytes() == fb[key].tobytes()
     for i in range(4):
         for j in range(i, 4):
             assert [x.tobytes() for x in pa.pair(i, j)] == [x.tobytes() for x in pb.pair(i, j)]
     # after a synchronising call the counts are exact: run and size agree with the host-fed handle
     assert b.status() == lib.OK and b.size() == a.size()
     assert b.run().tobytes() == a.run().tobytes()
-    assert b.run_dev(rows_b.data_ptr(), st) == na
+    assert cb.run(b) == na
     # a host append after device appends continues from the device's counts
     extra = synth.anchor_swarm(4, 30, 40, seed=12, with_orphans=False)["meas"]
     extra["id"] += 50_000
@@ -217,8 +211,7 @@ def test_refusals_launches_and_resources(gpu):
     live0 = host.live_resources()
     st = fh.stream()
     g = synth.anchor_swarm(3, 20, 100, seed=7)
-    a = host.LoopAnchor(g["max_drones"], max(len(v[0]) for v in g["trajs"].values()), 96, len(g["window"][2]),
-                        g["prm"]["det_dpos_thres"], g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"])
+    a = make_anchor(g, 96, len(g["window"][2]), traj_margin=0)
     prepare(a, g)
     a.add_measurements(g["meas"][:90])
     assert a.status() == lib.OK                               # no device append yet
@@ -250,7 +243,7 @@ def test_refusals_launches_and_resources(gpu):
     assert a.status() == lib.OK and sum(a.size()) == 96 and host.live_resources() == live1
     a.close()
     # the front-end's call: one launch whatever n, refusals before anything is enqueued, counters acquired once
-    fe = make_frontend()
+    fe = loop_frontend()
     old, new = record(1, 100, "old"), record(1, 101, "new", seed=1, g=noisy_g(1))
     rt, res_t, res = own_query(fe, st, old, new)
     edges_t, _ = compute_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), [cand_own()])
@@ -296,29 +289,28 @@ def entry_stamp(g, drone, frame):
 
 def test_device_round_solves_as_the_host_hop_round(gpu):
     g = synth.anchor_swarm(5, 30, 300, seed=9, with_orphans=False)
-    base = window_graph(g)
+    base = synth.anchor_window_graph(g)
     st = fh.stream()
-    fe = make_frontend()
+    fe = loop_frontend()
     old = record(1, 100, "old")
     ot = upload([old])
     fe.ingest_own(ot.data_ptr(), st)
     n = 6
     recs = [record(2 + r % 3, 300 + r, "new", seed=20 + r, g=noisy_g(10 + r)) for r in range(n)]
-    cands = [dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], cov=COV) for _ in range(n)]
+    cands = [dict(pose_query=SC["pose_new"], pose_hit=SC["pose_old"], cov=LOOP_COV) for _ in range(n)]
     stamps = [(entry_stamp(g, 2 + r % 3, 4 + 3 * r), entry_stamp(g, 1, 2 + 3 * r)) for r in range(n)]
     rt, res_t = upload(recs), filled(n * RS)
     fe.query_received(rt.data_ptr(), n, -1, res_t.data_ptr(), st)
     edges_t, raw = compute_loop(fe, st, rt.data_ptr(), res_t.data_ptr(), cands)
     assert sum(e["status"] == lib.LOOP_ACCEPTED for e in edge_dicts(raw)) >= 3
-    anchors = [make(g, max_meas=1024) for _ in range(2)]
+    anchors = [make_anchor(g, max_meas=1024) for _ in range(2)]
     for h in anchors:
         prepare(h, g)
         h.add_measurements(g["meas"][:200])
-    states = [host.PcmState(0, True, 15.0, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"], max_pairs=32,
-                            pair_capacity=1024) for _ in range(2)]
+    states = [pcm_state(g, 32, 1024) for _ in range(2)]
     solvers = [host.PoseGraphSolver(4096, 32768) for _ in range(2)]
     o = options(solvers[0], "tight")
-    chains = [DeviceChain(2048) for _ in range(2)]
+    chains = [host.AnchoredChain(2048) for _ in range(2)]
     for s in solvers:
         resident(s, base)
     # (B) the device round: loop_measurements -> add_measurements_dev -> run_dev -> reject_anchored -> compact -> solve
@@ -328,16 +320,18 @@ def test_device_round_solves_as_the_host_hop_round(gpu):
     fe.loop_measurements(res_t.data_ptr(), edges_t.data_ptr(), cands, stamps, COV_POS, COV_ANG, meas_t.data_ptr(),
                          cnt_t.data_ptr(), s)
     anchors[1].add_measurements_dev(meas_t.data_ptr(), cnt_t.data_ptr(), n, 2.0, s)
-    chains[1](anchors[1], states[1], solvers[1], 2048, o)
+    chains[1](anchors[1], states[1])
+    chains[1].solve(solvers[1], 2048, o)
     # (A) the host hop: download the edge and query results, build the rows, add them on the host
     results = fh.results(res_t, n)
     rows, _ = lm.loop_measurements(edge_dicts(raw), [r.swapped for r in results], cands, stamps, SELF, COV_POS, COV_ANG,
                                    lm.new_counters())
     anchors[0].add_measurements(lm.add_new_loop_connection(rows, 2.0))
-    chains[0](anchors[0], states[0], solvers[0], 2048, o)
+    chains[0](anchors[0], states[0])
+    chains[0].solve(solvers[0], 2048, o)
     torch.cuda.synchronize()
     assert anchors[1].status() == lib.OK and anchors[1].size() == anchors[0].size()
-    ta, tb = chains[0].rows_on_host(), chains[1].rows_on_host()
+    ta, tb = (c.factors.on_host(c.stream) for c in chains)
     assert len(ta["ftype"]) > 0 and all(ta[k].tobytes() == tb[k].tobytes() for k in ta)
     ok = anchors[0].run()
     assert (ok["status"][ok["type"] == lib.MEAS_LOOP][-len(rows):] == lib.ANCHOR_OK).any()

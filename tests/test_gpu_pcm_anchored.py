@@ -11,9 +11,9 @@ import torch
 
 from omniswarm_b200 import host, lib as _l, synth
 from oracle.pcm_state_ref import PcmStateRef
+from backend_harness import THRES, make_anchor, pcm_state
 
 pytestmark = pytest.mark.gpu
-THRES = 15.0
 DRONES = 5
 PAIRS = [(a, b) for a in range(DRONES + 2) for b in range(DRONES + 2) if a <= b]
 ROW = _l.ANCHOR_RESULT_DTYPE.itemsize
@@ -53,61 +53,6 @@ def solve_rounds(seed=0, rounds=4):
     return g, out
 
 
-def make_anchor(g):
-    return host.LoopAnchor(g["max_drones"], max(len(v[0]) for v in g["trajs"].values()) + 8, 4096, 4096,
-                           g["prm"]["det_dpos_thres"], g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"])
-
-
-def make_state(g, self_id, redundant, max_pairs=len(PAIRS), cap=512):
-    return host.PcmState(self_id, redundant, THRES, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"],
-                         max_pairs=max_pairs, pair_capacity=cap)
-
-
-def host_sequence(st, rows):
-    """the host sequence the device chain replaces: the OK rows through reject, the mask scattered back"""
-    ok = rows["status"] == _l.ANCHOR_OK
-    keep = np.zeros(len(rows), np.uint8)
-    keep[ok] = st.reject(host.anchored_loop_edges(rows[ok]), rows["id"][ok])
-    return keep
-
-
-class Chain:
-    """device buffers of one solve: rows, keep mask and the compacted SoA"""
-
-    def __init__(self, cap_rows):
-        self.rows = torch.zeros(cap_rows * ROW, dtype=torch.uint8, device="cuda")
-        self.keep = torch.zeros(cap_rows, dtype=torch.uint8, device="cuda")
-        self.type = torch.zeros(cap_rows, dtype=torch.int32, device="cuda")
-        self.ia = torch.zeros(cap_rows, dtype=torch.int32, device="cuda")
-        self.ib = torch.zeros(cap_rows, dtype=torch.int32, device="cuda")
-        self.payload = torch.zeros(cap_rows * _l.PAYLOAD_LEN, dtype=torch.float64, device="cuda")
-        self.huber = torch.zeros(cap_rows, dtype=torch.uint8, device="cuda")
-        self.count = torch.zeros(1, dtype=torch.int32, device="cuda")
-        self.stream = torch.cuda.Stream()
-
-    def upload(self, rows):
-        self.rows[:len(rows) * ROW].copy_(torch.from_numpy(rows.view(np.uint8).copy()))
-
-    def reject(self, st, n):
-        self.stream.wait_stream(torch.cuda.current_stream())         # uploads and fills made on the current stream
-        st.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), self.stream.cuda_stream)
-
-    def compact(self, n, keep=True):
-        host.compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr() if keep else None, self.type.data_ptr(),
-                                      self.ia.data_ptr(), self.ib.data_ptr(), self.payload.data_ptr(),
-                                      self.huber.data_ptr(), self.count.data_ptr(), self.stream.cuda_stream)
-
-    def keep_np(self, n):
-        self.stream.synchronize()
-        return self.keep[:n].cpu().numpy()
-
-    def factors(self):
-        self.stream.synchronize()
-        k = int(self.count.cpu()[0])
-        return (self.type[:k].cpu().numpy(), self.ia[:k].cpu().numpy(), self.ib[:k].cpu().numpy(),
-                self.payload[:k * _l.PAYLOAD_LEN].cpu().numpy().reshape(k, _l.PAYLOAD_LEN), self.huber[:k].cpu().numpy())
-
-
 def same_state(a, b, pairs=PAIRS):
     for p in pairs:
         for x, y in zip(a.pair(*p), b.pair(*p)):
@@ -125,28 +70,28 @@ def ref_edges(rows):
 @pytest.mark.parametrize("redundant", [True, False])
 def test_solve_rounds_match_the_host_sequence(gpu, redundant):
     g, rounds = solve_rounds(seed=3)
-    a = make_anchor(g)
+    a = make_anchor(g, 4096, 4096, traj_margin=8)
     for d, (s, p) in g["trajs"].items():
         a.push_odometry(d, s, p)
     yaw = np.ones(g["max_drones"], np.uint8)
     yaw[2] = 0
-    ha, hb = make_state(g, 0, redundant), make_state(g, 0, redundant)
+    ha, hb = (pcm_state(g, len(PAIRS), 512, 0, redundant) for _ in range(2))
     ref = PcmStateRef(0, redundant, THRES, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"])
-    chain = Chain(4096)
+    chain = host.AnchoredChain(4096)
     seen_status, set_on = set(), {}
     for r, (new, win) in enumerate(rounds):
         a.add_measurements(new)
         a.set_window(*win)
-        n = a.run_dev(chain.rows.data_ptr(), chain.stream.cuda_stream, yaw)
+        n = chain.run(a, yaw)
         chain.stream.synchronize()
         rows = np.frombuffer(chain.rows[:n * ROW].cpu().numpy().tobytes(), _l.ANCHOR_RESULT_DTYPE)
-        keep_a = host_sequence(ha, rows)
+        keep_a = host.anchored_keep(ha, rows)
         ok = rows["status"] == _l.ANCHOR_OK
         assert np.array_equal(keep_a[ok], ref.reject(ref_edges(rows[ok]), rows["id"][ok]))
         chain.reject(hb, n)
         chain.compact(n)
-        fb = chain.factors()
-        assert chain.keep_np(n).tobytes() == keep_a.tobytes()
+        fb = chain.factors.on_host(chain.stream).values()
+        assert chain.keep_on_host(n).tobytes() == keep_a.tobytes()
         fa = host.anchored_factor_rows(rows, keep_a)
         assert len(fa[0]) > 0 and all(x.tobytes() == y.tobytes() for x, y in zip(fa, fb))
         same_state(ha, hb)
@@ -172,22 +117,22 @@ def test_solve_rounds_match_the_host_sequence(gpu, redundant):
 
 def test_host_and_anchored_calls_mix_on_one_handle(gpu):
     g, rounds = solve_rounds(seed=5, rounds=5)
-    a = make_anchor(g)
+    a = make_anchor(g, 4096, 4096, traj_margin=8)
     for d, (s, p) in g["trajs"].items():
         a.push_odometry(d, s, p)
-    hh, hm = make_state(g, 1, True), make_state(g, 1, True)
-    chain = Chain(4096)
+    hh, hm = (pcm_state(g, len(PAIRS), 512, 1) for _ in range(2))
+    chain = host.AnchoredChain(4096)
     for r, (new, win) in enumerate(rounds):
         a.add_measurements(new)
         a.set_window(*win)
         rows = a.run()
         chain.upload(rows)
-        keep_h = host_sequence(hh, rows)
+        keep_h = host.anchored_keep(hh, rows)
         if r % 2 == 0:
             chain.reject(hm, len(rows))
-            keep_m = chain.keep_np(len(rows))
+            keep_m = chain.keep_on_host(len(rows))
         else:
-            keep_m = host_sequence(hm, rows)
+            keep_m = host.anchored_keep(hm, rows)
         assert keep_m.tobytes() == keep_h.tobytes(), r
         ok_ids = rows["id"][rows["status"] == _l.ANCHOR_OK]
         for h in (hh, hm):                                           # other drones' sets between the calls
@@ -225,14 +170,14 @@ def test_sizes_across_the_shared_memory_bound_and_to_capacity(gpu):
     idm = np.arange(1300, dtype=np.int64) + (6 << 32)
     ids_s = np.arange(5, dtype=np.int64) + (7 << 32)
     st = host.PcmState(1, True, THRES, 1e-4, 1e-5, max_pairs=3, pair_capacity=4096)
-    chain = Chain(4096 + 1300 + 5)
+    chain = host.AnchoredChain(4096 + 1300 + 5)
     first = pcm_rows(big[:3000] + mid[:1270] + small[:2], np.concatenate([idb[:3000], idm[:1270], ids_s[:2]]))
     chain.upload(first)
     chain.reject(st, len(first))
     rows = pcm_rows(big + mid[:1290] + small, np.concatenate([idb, idm[:1290], ids_s]))
     chain.upload(rows)
     chain.reject(st, len(rows))
-    keep = chain.keep_np(len(rows))
+    keep = chain.keep_on_host(len(rows))
     for (a, b), edges in (((1, 2), big), ((1, 3), mid[:1290]), ((3, 3), small)):
         ids, adj, clique = st.pair(a, b)
         rclique, radj = stateless(edges)
@@ -249,7 +194,7 @@ def test_capacity_is_refused_on_the_device_and_changes_nothing(gpu):
     i12 = np.arange(70, dtype=np.int64) + (3 << 32)
     i13 = np.arange(20, dtype=np.int64) + (4 << 32)
     st = host.PcmState(1, True, THRES, 1e-4, 1e-5, max_pairs=2, pair_capacity=64)
-    chain = Chain(256)
+    chain = host.AnchoredChain(256)
     chain.upload(pcm_rows(e12[:60] + e13[:10], np.concatenate([i12[:60], i13[:10]])))
     chain.reject(st, 70)
     assert st.status() == _l.OK
@@ -260,7 +205,7 @@ def test_capacity_is_refused_on_the_device_and_changes_nothing(gpu):
         chain.keep.fill_(0xAB)
         chain.upload(pcm_rows(edges, ids))
         chain.reject(st, len(ids))
-        assert (chain.keep_np(len(chain.keep)) == 0xAB).all()              # not written
+        assert (chain.keep_on_host(len(chain.keep)) == 0xAB).all()       # not written
         assert st.status() == _l.ERR_CAPACITY
         with pytest.raises(_l.OsbError) as e:                        # the next host-side call reports it once
             st.inliers(1, 2)
@@ -280,17 +225,17 @@ def test_capacity_is_refused_on_the_device_and_changes_nothing(gpu):
 def test_capturable_constant_launches_and_resources(gpu):
     live0 = host.live_resources()
     g, rounds = solve_rounds(seed=7, rounds=3)
-    a = make_anchor(g)
+    a = make_anchor(g, 4096, 4096, traj_margin=8)
     for d, (s, p) in g["trajs"].items():
         a.push_odometry(d, s, p)
-    st, ref = make_state(g, 0, True), make_state(g, 0, True)
-    chain = Chain(4096)
+    st, ref = (pcm_state(g, len(PAIRS), 512) for _ in range(2))
+    chain = host.AnchoredChain(4096)
     launches, live = [], None
     for r, (new, win) in enumerate(rounds[:2]):
         a.add_measurements(new)
         a.set_window(*win)
-        host_sequence(ref, a.run())
-        n = a.run_dev(chain.rows.data_ptr(), chain.stream.cuda_stream)
+        host.anchored_keep(ref, a.run())
+        n = chain.run(a)
         live = host.live_resources()
         n0 = host.launch_count()
         chain.reject(st, n)
@@ -312,20 +257,20 @@ def test_capturable_constant_launches_and_resources(gpu):
     a.add_measurements(new)
     a.set_window(*win)
     rows_now = a.run()
-    keep_ref = host_sequence(ref, rows_now)
+    keep_ref = host.anchored_keep(ref, rows_now)
     graph = torch.cuda.CUDAGraph()
     live = host.live_resources()
     with torch.cuda.graph(graph, stream=chain.stream, capture_error_mode="global"):
-        n = a.run_dev(chain.rows.data_ptr(), chain.stream.cuda_stream)
+        n = chain.run(a)
         chain.reject(st, n)
         chain.compact(n)
     assert host.live_resources() == live
     graph.replay()
     chain.stream.synchronize()
     torch.cuda.synchronize()
-    assert chain.keep_np(n).tobytes() == keep_ref.tobytes()
+    assert chain.keep_on_host(n).tobytes() == keep_ref.tobytes()
     fa = host.anchored_factor_rows(rows_now, keep_ref)
-    assert all(x.tobytes() == y.tobytes() for x, y in zip(fa, chain.factors()))
+    assert all(x.tobytes() == y.tobytes() for x, y in zip(fa, chain.factors.on_host(chain.stream).values()))
     same_state(ref, st)
     del graph
     for h in (st, ref, a):

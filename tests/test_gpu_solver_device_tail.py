@@ -12,64 +12,17 @@ import torch
 
 from omniswarm_b200 import host, lib as _l, synth
 from oracle import solver_ref as sr
-from test_gpu_anchor import window_graph, make, feed
+from backend_harness import KEYS, feed, make_anchor, options, pcm_state, resident
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "omni-swarm_b200", "csrc")
 CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-ROW = _l.ANCHOR_RESULT_DTYPE.itemsize
-KEYS = ("ftype", "ia", "ib", "payload", "huber")
-
-
-def options(solver, kind):
-    o = solver.default_options()
-    if kind in ("tight", "fp64", "jacobi"):
-        o.function_tolerance = 1e-14; o.pcg_tolerance = 1e-8; o.max_pcg_iterations = 2000
-    if kind == "fp64":
-        o.inner_precision = 1                                  # OSB_INNER_FP64
-    if kind == "jacobi":
-        o.preconditioner = 1                                   # OSB_PRECOND_BLOCK_JACOBI
-    return o
 
 
 def concat(base, tail, init):
     g = {k: np.concatenate([base[k], tail[k]]) if len(tail["ftype"]) else base[k].copy() for k in KEYS}
     g["fixed"], g["init"] = base["fixed"], init
     return g
-
-
-def resident(solver, base):
-    solver.graph_clear()
-    solver.graph_add_nodes(base["init"], base["fixed"])
-    solver.graph_add_factors(*(base[k] for k in KEYS))
-
-
-class Tail:
-    """a tail in device memory, laid out as osb_anchor_compact_factors_dev writes it"""
-
-    def __init__(self, cap):
-        cap = max(cap, 1)
-        self.type = torch.zeros(cap, dtype=torch.int32, device="cuda")
-        self.ia = torch.zeros(cap, dtype=torch.int32, device="cuda")
-        self.ib = torch.zeros(cap, dtype=torch.int32, device="cuda")
-        self.payload = torch.zeros(cap * _l.PAYLOAD_LEN, dtype=torch.float64, device="cuda")
-        self.huber = torch.zeros(cap, dtype=torch.uint8, device="cuda")
-        self.count = torch.zeros(1, dtype=torch.int32, device="cuda")
-
-    def set(self, t, count=None):
-        k = len(t["ftype"])
-        if k:
-            self.type[:k] = torch.from_numpy(np.asarray(t["ftype"], np.int32)).cuda()
-            self.ia[:k] = torch.from_numpy(np.asarray(t["ia"], np.int32)).cuda()
-            self.ib[:k] = torch.from_numpy(np.asarray(t["ib"], np.int32)).cuda()
-            self.payload[:k * _l.PAYLOAD_LEN] = torch.from_numpy(np.ascontiguousarray(t["payload"]).reshape(-1)).cuda()
-            self.huber[:k] = torch.from_numpy(np.asarray(t["huber"], np.uint8)).cuda()
-        self.count.fill_(k if count is None else count)
-
-    def solve(self, solver, max_tail, o, stream=None):
-        s = torch.cuda.current_stream() if stream is None else stream
-        solver.solve_resident_dev(max_tail, self.type.data_ptr(), self.ia.data_ptr(), self.ib.data_ptr(),
-                                  self.payload.data_ptr(), self.huber.data_ptr(), self.count.data_ptr(), s.cuda_stream, o)
 
 
 def candidate_rows(base, k, rng, kinds=(0, 1)):
@@ -125,7 +78,7 @@ def shape(solver):
 
 def window():
     g = synth.anchor_swarm(4, 30, 300, seed=9, with_orphans=False)
-    return g, window_graph(g)
+    return g, synth.anchor_window_graph(g)
 
 
 @pytest.mark.gpu
@@ -137,7 +90,7 @@ def test_bit_identical_to_one_shot(gpu, kind, k):
     dev, flat = host.PoseGraphSolver(4096, 32768), host.PoseGraphSolver(4096, 32768)
     o = options(dev, kind)
     resident(dev, base)
-    buf = Tail(64)
+    buf = host.FactorRows(64)
     buf.set(tail)
     buf.solve(dev, k + 3, o)
     poses = dev.graph_get_poses()
@@ -151,35 +104,6 @@ def test_bit_identical_to_one_shot(gpu, kind, k):
     assert s.initial_cost == s1.initial_cost and s.solve_ms > 0.0
     for h in (dev, flat):
         h.close()
-
-
-class DeviceChain:
-    """run_dev -> reject_anchored -> compact_factors_dev -> solve_resident_dev on one stream, nothing copied between"""
-
-    def __init__(self, cap):
-        self.rows = torch.zeros(cap * ROW, dtype=torch.uint8, device="cuda")
-        self.keep = torch.zeros(cap, dtype=torch.uint8, device="cuda")
-        self.tail = Tail(cap)
-        self.stream = torch.cuda.Stream()
-
-    def __call__(self, a, st, solver, max_tail, o):
-        s = self.stream.cuda_stream
-        n = a.run_dev(self.rows.data_ptr(), s)
-        st.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), s)
-        t = self.tail
-        host.compact_anchored_factors(self.rows.data_ptr(), n, self.keep.data_ptr(), t.type.data_ptr(), t.ia.data_ptr(),
-                                      t.ib.data_ptr(), t.payload.data_ptr(), t.huber.data_ptr(), t.count.data_ptr(), s)
-        t.solve(solver, max_tail, o, self.stream)
-        return n
-
-    def rows_on_host(self):
-        """(test only) the tail this call solved, for the one-shot reference"""
-        torch.cuda.synchronize()
-        k = int(self.tail.count.cpu()[0])
-        t = self.tail
-        return {"ftype": t.type[:k].cpu().numpy(), "ia": t.ia[:k].cpu().numpy(), "ib": t.ib[:k].cpu().numpy(),
-                "payload": t.payload[:k * _l.PAYLOAD_LEN].cpu().numpy().reshape(k, _l.PAYLOAD_LEN),
-                "huber": t.huber[:k].cpu().numpy()}
 
 
 def slide(win, base, d):
@@ -205,14 +129,13 @@ def slide(win, base, d):
 @pytest.mark.gpu
 def test_rows_from_the_device_chain(gpu):
     g, base = window()
-    a = make(g, max_meas=4096)
+    a = make_anchor(g, max_meas=4096)
     g0 = dict(g, meas=g["meas"][:200])
     feed(a, g0)
-    st = host.PcmState(0, True, 15.0, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"], max_pairs=32,
-                       pair_capacity=1024)
+    st = pcm_state(g, 32, 1024)
     dev, flat = host.PoseGraphSolver(4096, 32768), host.PoseGraphSolver(4096, 32768)
     resident(dev, base)
-    chain = DeviceChain(4096)
+    chain = host.AnchoredChain(4096)
     o = options(dev, "tight")
     win = g["window"]
     exact = close = 0
@@ -228,10 +151,11 @@ def test_rows_from_the_device_chain(gpu):
             a.set_window(*win)
             base["init"] = start[d:]
         start = dev.graph_get_poses()
-        chain(a, st, dev, 2048, o)
+        chain(a, st)
+        chain.solve(dev, 2048, o)
         poses = dev.graph_get_poses()
         s = dev.last_summary()
-        tail = chain.rows_on_host()
+        tail = chain.factors.on_host(chain.stream)
         assert len(tail["ftype"]) > 0
         gcat = concat(base, tail, start)
         gcat["fixed"] = base["fixed"]
@@ -260,7 +184,7 @@ def test_mixed_with_host_calls(gpu):
     o = options(dev, "tight")
     resident(dev, base)
     resident(twin, base)
-    buf = Tail(64)
+    buf = host.FactorRows(64)
     buf.set(tail)
     buf.solve(dev, 16, o)
     p1 = dev.graph_get_poses()                                 # graph_get_poses after a device call
@@ -296,7 +220,7 @@ def test_refusals(gpu):
     dev, flat = host.PoseGraphSolver(4096, 32768), host.PoseGraphSolver(4096, 32768)
     o = options(dev, "tight")
     resident(dev, base)
-    buf = Tail(64)
+    buf = host.FactorRows(64)
     buf.set(tail)
     buf.solve(dev, 8, o)
     good = dev.graph_get_poses()
@@ -321,8 +245,7 @@ def test_refusals(gpu):
     assert np.array_equal(dev.graph_get_poses(), ref)
     # refused on the host: nothing enqueued
     n0 = host.launch_count()
-    args = [buf.type.data_ptr(), buf.ia.data_ptr(), buf.ib.data_ptr(), buf.payload.data_ptr(), buf.huber.data_ptr(),
-            buf.count.data_ptr()]
+    args = buf.ptrs()
     for i in range(6):
         a2 = list(args)
         a2[i] = 0
@@ -350,7 +273,7 @@ def test_launches_and_memory(gpu):
     resident(dev, base)
     rng = np.random.default_rng(11)
     big = candidate_rows(base, 3000, rng)
-    buf = Tail(3000)
+    buf = host.FactorRows(3000)
     o = options(dev, "default")
     buf.set(big, 1)
     buf.solve(dev, 3000, o)
@@ -384,26 +307,28 @@ def test_capture_of_the_whole_chain(gpu):
     g, base = window()
 
     def setup():
-        a = make(g, max_meas=4096)
+        a = make_anchor(g, max_meas=4096)
         feed(a, g)
-        st = host.PcmState(0, True, 15.0, g["prm"]["odom_pos_cov_per_m"], g["prm"]["odom_ang_cov_per_m"],
-                           max_pairs=32, pair_capacity=1024)
+        st = pcm_state(g, 32, 1024)
         dev = host.PoseGraphSolver(4096, 32768)
         resident(dev, base)
-        return a, st, dev, DeviceChain(4096)
+        return a, st, dev, host.AnchoredChain(4096)
 
     a, st, dev, chain = setup()
     o = options(dev, "default")
     want = []
     for _ in range(3):                                        # the uncaptured sequence: three solves
-        chain(a, st, dev, 2048, o)
+        chain(a, st)
+        chain.solve(dev, 2048, o)
         want.append(dev.graph_get_poses())
     want = want[1:]
     a2, st2, dev2, chain2 = setup()
-    chain2(a2, st2, dev2, 2048, o)                            # warm: the plan, the tables and the poses are on the device
+    chain2(a2, st2)                                           # warm: the plan, the tables and the poses are on the device
+    chain2.solve(dev2, 2048, o)
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph, stream=chain2.stream, capture_error_mode="global"):
-        chain2(a2, st2, dev2, 2048, o)
+        chain2(a2, st2)
+        chain2.solve(dev2, 2048, o)
     for w in want:                                            # every replay's poses reach the host copy
         graph.replay()
         torch.cuda.synchronize()
@@ -414,7 +339,7 @@ def test_capture_of_the_whole_chain(gpu):
     x = torch.zeros(4, device="cuda")
     with torch.cuda.graph(g2, stream=chain2.stream, capture_error_mode="global"):
         with pytest.raises(_l.OsbError) as e:
-            chain2.tail.solve(dev2, 2048, o, chain2.stream)
+            chain2.solve(dev2, 2048, o)
         x += 1
     assert e.value.status == _l.ERR_INVALID
     g2.replay()
@@ -433,7 +358,7 @@ def test_cooperative_path(gpu):
     dev, flat = host.PoseGraphSolver(4096, 32768), host.PoseGraphSolver(4096, 32768)
     o = options(dev, "tight")
     resident(dev, base)
-    buf = Tail(k)
+    buf = host.FactorRows(k)
     buf.set(tail)
     buf.solve(dev, k, o)
     poses = dev.graph_get_poses()
