@@ -68,9 +68,17 @@ struct KeypointScratch {   // per handle, sized for max_batch images
 };
 osb_status sp_keypoints(const float* semi, int B, int H, int W, float thres, int max_num, KeypointScratch& ks,
                         int32_t* n_kpts, float* kpts, float* conf, cudaStream_t st);
-// desc_nhwc [B][Hc][Wc][256]; kpts [B][max_num][2]; out [B][max_num][64]
+// desc_nhwc [B][Hc][Wc][256]; kpts [B][max_num][2]; out [B][max_num][64].  With `slot` ([B][Hc][Wc], sp_cell_gather)
+// desc_nhwc is convDb's output at the listed cells only, [B * seg][256] and not yet L2-normalised: the kernels divide each
+// tap by its row's norm (kept in cell_n [B * seg]), the value l2norm_cells would have stored
 osb_status sp_descriptors(const float* desc_nhwc, int B, int H, int W, const int32_t* n_kpts, const float* kpts,
                           int max_num, const float* pca_compT /*[256][64]*/, const float* pca_mean, float* cnorm, float* out,
+                          cudaStream_t st, const int32_t* slot = nullptr, int seg = 0, float* cell_n = nullptr);
+// sparse descriptor head: the cells the keypoints' bilinear taps read, numbered row-major per image into segments of
+// `seg` rows (slot [B][Hc][Wc], -1 where unsampled), and convDa's input at them: x [B][Hc][Wc][128] split planes ->
+// col [B * seg][1152] (9 taps x 128 channels in conv_stream_t_kernel's K order, zero for padding rows)
+osb_status sp_cell_gather(int B, int H, int W, const int32_t* n_kpts, const float* kpts, int max_num, int seg, int32_t* slot,
+                          const __half* x_hi, const __half* x_lo, __half* col_hi, __half* col_lo, bool fp16,
                           cudaStream_t st);
 // layout helper: [B][C][h][w] -> [B][h][w][C]
 osb_status nchw_to_nhwc(const float* in, float* out, int B, int C, int h, int w, cudaStream_t st);

@@ -870,6 +870,7 @@ extern "C" osb_status osb_frontend_create(osb_frontend** out, const osb_frontend
   OSB_TRY(h->sp.init(sp_weights, n_sp_weights, cfg->width, cfg->height, cfg->sp_thres, mn, pca_comp, pca_mean, 2 * nd));
   h->sp.ks.write_surv = false;       // the survivor plane is only a parity hook of the standalone SuperPoint handle
   if (cfg->zero_bottom_quarter) OSB_TRY(h->sp.band_init());
+  OSB_TRY(h->sp.sparse_init());
   OSB_TRY(h->nv.init(nv_weights, n_nv_weights, cfg->width, cfg->height, nd));
   OSB_TRY(dbstore_alloc(m, h->db[0], cfg->db_capacity, mn));
   OSB_TRY(dbstore_alloc(m, h->db[1], cfg->db_capacity, mn));

@@ -46,16 +46,21 @@ osb_status sp_softmax_shuffle(const float* logits, int cstride, float* semi, int
   return OSB_OK;
 }
 
+// ||p||_2 over C channels, by one warp (every lane gets it); the sparse descriptor head divides by the same value
+__device__ __forceinline__ float cell_norm(const float* p, int C, int lane) {
+  float s = 0.f;
+  for (int c = lane; c < C; c += 32) { const float v = p[c]; s = fmaf(v, v, s); }
+  s = warp_sum(s);
+  return sqrtf(s);
+}
+
 // descriptor head epilogue: desc /= ||desc||_2 over channels (superpoint.ipynb:187-188); one warp per cell
 __global__ void l2norm_cells_kernel(float* __restrict__ x, int64_t cells, int C) {
   const int64_t cell = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (cell >= cells) return;
   float* p = x + (size_t)cell * C;
-  float s = 0.f;
-  for (int c = lane; c < C; c += 32) { const float v = p[c]; s = fmaf(v, v, s); }
-  s = warp_sum(s);
-  const float n = sqrtf(s);
+  const float n = cell_norm(p, C, lane);
   for (int c = lane; c < C; c += 32) p[c] = p[c] / n;
 }
 
@@ -416,30 +421,143 @@ __device__ __forceinline__ Taps bilinear_taps(float kx, float ky, int W, int H, 
   return t;
 }
 
-__device__ __forceinline__ float sample_channel(const float* __restrict__ d, const Taps& t, int Wc, int Hc, int ch) {
+// SLOT: d holds convDb's output at the listed cells only, row slot[y][x] for cell (y, x) of the image (sp_cell_gather), not
+// yet normalised: the value is d / nrm[row - row0], what l2norm_cells stores.  Else d is the image's normalised dense
+// [Hc][Wc][256] map.
+template <bool SLOT = false>
+__device__ __forceinline__ float sample_channel(const float* __restrict__ d, const int32_t* __restrict__ slot,
+                                                const float* nrm, int row0, const Taps& t, int Wc, int Hc, int ch) {
+  auto at = [&](int y, int x) {
+    if constexpr (SLOT) {
+      const int row = slot[y * Wc + x];
+      return d[(size_t)row * 256 + ch] / nrm[row - row0];
+    } else {
+      return d[((size_t)y * Wc + x) * 256 + ch];
+    }
+  };
   float r = 0.f;
   const bool x0 = t.x0 >= 0 && t.x0 < Wc, x1 = t.x0 + 1 >= 0 && t.x0 + 1 < Wc;
   const bool y0 = t.y0 >= 0 && t.y0 < Hc, y1 = t.y0 + 1 >= 0 && t.y0 + 1 < Hc;
-  if (y0 && x0) r = __fadd_rn(r, __fmul_rn(d[((size_t)t.y0 * Wc + t.x0) * 256 + ch], t.nw));
-  if (y0 && x1) r = __fadd_rn(r, __fmul_rn(d[((size_t)t.y0 * Wc + t.x0 + 1) * 256 + ch], t.ne));
-  if (y1 && x0) r = __fadd_rn(r, __fmul_rn(d[((size_t)(t.y0 + 1) * Wc + t.x0) * 256 + ch], t.sw));
-  if (y1 && x1) r = __fadd_rn(r, __fmul_rn(d[((size_t)(t.y0 + 1) * Wc + t.x0 + 1) * 256 + ch], t.se));
+  if (y0 && x0) r = __fadd_rn(r, __fmul_rn(at(t.y0, t.x0), t.nw));
+  if (y0 && x1) r = __fadd_rn(r, __fmul_rn(at(t.y0, t.x0 + 1), t.ne));
+  if (y1 && x0) r = __fadd_rn(r, __fmul_rn(at(t.y0 + 1, t.x0), t.sw));
+  if (y1 && x1) r = __fadd_rn(r, __fmul_rn(at(t.y0 + 1, t.x0 + 1), t.se));
   return r;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// Sparse descriptor head: the cells the selected keypoints sample, and their convDa input as a 1x1 layer's
+// -------------------------------------------------------------------------------------------------------------
+// Grid (image, CL_SPLIT).  Every CTA marks the in-range taps of the image's keypoints (sample_channel's conditions) and
+// numbers them row-major in shared memory: rank r of the image is row b * seg + r, and the image's rows past its cells are
+// padding (-1).  CTA 0 of the image writes slot [b][Hc][Wc] (-1 for an unsampled cell).  Then each CTA gathers its share of
+// the image's rows: convDa's input at the cell as the input of a 1x1 layer of 9 x 128 channels, channel slab
+// (kx * 2 + s) * 3 + ky holding channels 64 s .. 64 s + 63 of the cell's (ky, kx) neighbour in x ([B][Hc][Wc][128] split
+// planes), zero outside the image or for a padding row.  That slab order is conv_stream_t_kernel's K order (kx, slab, ky)
+// of the 3x3 layer.  Work unit = (row, tap, 16-byte chunk of the 128 channels).
+constexpr int CL_THREADS = KP_THREADS;             // block_exclusive_scan's block
+constexpr int CL_SPLIT = 16;
+template <bool FP16>
+__global__ void __launch_bounds__(CL_THREADS)
+sp_cell_gather_kernel(int H, int W, const int32_t* __restrict__ n_kpts, const float* __restrict__ kpts, int max_num, int seg,
+                      int32_t* __restrict__ slot, const __half* __restrict__ x_hi, const __half* __restrict__ x_lo,
+                      __half* __restrict__ col_hi, __half* __restrict__ col_lo) {
+  extern __shared__ int32_t list[];                    // [seg], then the marks [Hc * Wc] as bytes
+  __shared__ int wsum[32], total;
+  const int b = blockIdx.x, tid = threadIdx.x, Hc = H / 8, Wc = W / 8, cells = Hc * Wc;
+  uint8_t* mark = reinterpret_cast<uint8_t*>(list + seg);
+  for (int c = tid; c < cells; c += CL_THREADS) mark[c] = 0;
+  __syncthreads();
+  const int N = n_kpts[b];
+  for (int n = tid; n < N; n += CL_THREADS) {
+    const Taps t = bilinear_taps(kpts[((size_t)b * max_num + n) * 2], kpts[((size_t)b * max_num + n) * 2 + 1], W, H, Wc, Hc);
+    for (int dy = 0; dy < 2; ++dy)
+      for (int dx = 0; dx < 2; ++dx) {
+        const int y = t.y0 + dy, x = t.x0 + dx;
+        if (y >= 0 && y < Hc && x >= 0 && x < Wc) mark[y * Wc + x] = 1;
+      }
+  }
+  __syncthreads();
+  // each thread numbers a contiguous run of cells: its count, a block-wide exclusive scan, then the run
+  const int per = (cells + CL_THREADS - 1) / CL_THREADS, c0 = tid * per, c1 = min(c0 + per, cells);
+  int cnt = 0;
+  for (int c = c0; c < c1; ++c) cnt += mark[c];
+  int rank = block_exclusive_scan(cnt, wsum, &total);
+  const bool writer = blockIdx.y == 0;
+  for (int c = c0; c < c1; ++c) {
+    if (mark[c]) {
+      if (writer) slot[(size_t)b * cells + c] = b * seg + rank;
+      list[rank++] = c;
+    } else if (writer) {
+      slot[(size_t)b * cells + c] = -1;
+    }
+  }
+  for (int r = total + tid; r < seg; r += CL_THREADS) list[r] = -1;
+  __syncthreads();
+  for (int e = blockIdx.y * CL_THREADS + tid; e < seg * 144; e += CL_SPLIT * CL_THREADS) {
+    const int i = e / 144, r = e % 144, tap = r / 16, j = r % 16, ky = tap / 3, kx = tap % 3, s = j / 8;
+    const int c = list[i];
+    uint4 h = make_uint4(0, 0, 0, 0), l = h;
+    if (c >= 0) {
+      const int y = c / Wc + ky - 1, xx = c % Wc + kx - 1;
+      if (y >= 0 && y < Hc && xx >= 0 && xx < Wc) {
+        const size_t src = (((size_t)b * Hc + y) * Wc + xx) * 128 + j * 8;
+        h = *reinterpret_cast<const uint4*>(x_hi + src);
+        if constexpr (!FP16) l = *reinterpret_cast<const uint4*>(x_lo + src);
+      }
+    }
+    const size_t dst = ((size_t)b * seg + i) * 1152 + ((kx * 2 + s) * 3 + ky) * 64 + (j % 8) * 8;
+    *reinterpret_cast<uint4*>(col_hi + dst) = h;
+    if constexpr (!FP16) *reinterpret_cast<uint4*>(col_lo + dst) = l;
+  }
+}
+
+osb_status sp_cell_gather(int B, int H, int W, const int32_t* n_kpts, const float* kpts, int max_num, int seg, int32_t* slot,
+                          const __half* x_hi, const __half* x_lo, __half* col_hi, __half* col_lo, bool fp16,
+                          cudaStream_t st) {
+  const int smem = seg * 4 + (H / 8) * (W / 8);
+  OSB_REQUIRE(smem <= 48 * 1024, "sparse descriptor head: too many cells per image");
+  const dim3 grid(B, CL_SPLIT);
+  if (fp16)
+    OSB_LAUNCH(sp_cell_gather_kernel<true>, grid, CL_THREADS, smem, st, H, W, n_kpts, kpts, max_num, seg, slot, x_hi, x_lo,
+               col_hi, col_lo);
+  else
+    OSB_LAUNCH(sp_cell_gather_kernel<false>, grid, CL_THREADS, smem, st, H, W, n_kpts, kpts, max_num, seg, slot, x_hi, x_lo,
+               col_hi, col_lo);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
 }
 
 // per-channel L2 norm over the keypoints of an image (torch::norm(desc, 2, 1) on [256,N], :214).
 // The kernel is a chain of dependent L2 round trips (keypoint -> 4 taps), so it is spread wide: CTA = (image, 64-channel
 // slab), 1024 threads = 16 keypoint groups x 64 channels; group g sums keypoints g, g+16, ... (two in flight per
 // iteration) and the 16 partial sums are combined in a fixed order.
+// SLOT (here and in sp_desc_pca_kernel): desc holds the listed cells only, found through slot [B][Hc][Wc] (sample_channel)
 constexpr int DN_GROUPS = 16, DN_CH = 64;
+template <bool SLOT = false>
 __global__ void __launch_bounds__(DN_GROUPS * DN_CH)
-sp_desc_norm_kernel(const float* __restrict__ desc, int H, int W, const int32_t* __restrict__ n_kpts,
-                    const float* __restrict__ kpts, int max_num, float* __restrict__ cnorm) {
+sp_desc_norm_kernel(const float* __restrict__ desc, const int32_t* __restrict__ slot, int seg, float* __restrict__ cell_n,
+                    int H, int W, const int32_t* __restrict__ n_kpts, const float* __restrict__ kpts, int max_num,
+                    float* __restrict__ cnorm) {
   __shared__ float part[DN_GROUPS][DN_CH];
+  extern __shared__ float nrm[];                       // SLOT: [seg] the norms of the image's rows
   const int b = blockIdx.x, c = threadIdx.x % DN_CH, g = threadIdx.x / DN_CH;
   const int ch = blockIdx.y * DN_CH + c;
   const int Hc = H / 8, Wc = W / 8;
-  const float* d = desc + (size_t)b * Hc * Wc * 256;
+  const float* d = SLOT ? desc : desc + (size_t)b * Hc * Wc * 256;
+  const int32_t* sl = SLOT ? slot + (size_t)b * Hc * Wc : nullptr;
+  if constexpr (SLOT) {
+    // every row's L2 norm, one warp per row as l2norm_cells; the image's first CTA also keeps them for sp_desc_pca_kernel
+    const int lane = threadIdx.x & 31;
+    for (int r = threadIdx.x >> 5; r < seg; r += DN_GROUPS * DN_CH / 32) {
+      const float n = cell_norm(desc + ((size_t)b * seg + r) * 256, 256, lane);
+      if (lane == 0) {
+        nrm[r] = n;
+        if (blockIdx.y == 0) cell_n[(size_t)b * seg + r] = n;
+      }
+    }
+    __syncthreads();
+  }
   const float* kp = kpts + (size_t)b * max_num * 2;
   const int N = n_kpts[b];
   float s = 0.f;
@@ -447,8 +565,8 @@ sp_desc_norm_kernel(const float* __restrict__ desc, int H, int W, const int32_t*
     const int n2 = n + DN_GROUPS;
     const Taps t0 = bilinear_taps(kp[2 * n], kp[2 * n + 1], W, H, Wc, Hc);
     const Taps t1 = bilinear_taps(kp[2 * min(n2, N - 1)], kp[2 * min(n2, N - 1) + 1], W, H, Wc, Hc);
-    const float v0 = sample_channel(d, t0, Wc, Hc, ch);
-    const float v1 = sample_channel(d, t1, Wc, Hc, ch);
+    const float v0 = sample_channel<SLOT>(d, sl, nrm, b * seg, t0, Wc, Hc, ch);
+    const float v1 = sample_channel<SLOT>(d, sl, nrm, b * seg, t1, Wc, Hc, ch);
     s = fmaf(v0, v0, s);
     if (n2 < N) s = fmaf(v1, v1, s);
   }
@@ -464,8 +582,10 @@ sp_desc_norm_kernel(const float* __restrict__ desc, int H, int W, const int32_t*
 
 // (S^T / cnorm - mean) @ comp^T  (:215-221).  CTA = 8 keypoints of one image, 256 threads.
 constexpr int DP_KP = 8;
+template <bool SLOT = false>
 __global__ void __launch_bounds__(256)
-sp_desc_pca_kernel(const float* __restrict__ desc, int H, int W, const int32_t* __restrict__ n_kpts,
+sp_desc_pca_kernel(const float* __restrict__ desc, const int32_t* __restrict__ slot, const float* __restrict__ cell_n,
+                   int H, int W, const int32_t* __restrict__ n_kpts,
                    const float* __restrict__ kpts, int max_num, const float* __restrict__ cnorm,
                    const float* __restrict__ pca_compT, const float* __restrict__ pca_mean, float* __restrict__ out) {
   __shared__ float sv[DP_KP][256];
@@ -473,7 +593,8 @@ sp_desc_pca_kernel(const float* __restrict__ desc, int H, int W, const int32_t* 
   const int N = n_kpts[b];
   if (n0 >= N) return;
   const int Hc = H / 8, Wc = W / 8;
-  const float* d = desc + (size_t)b * Hc * Wc * 256;
+  const float* d = SLOT ? desc : desc + (size_t)b * Hc * Wc * 256;
+  const int32_t* sl = SLOT ? slot + (size_t)b * Hc * Wc : nullptr;
   const float cn = cnorm[b * 256 + tid], mu = pca_mean[tid];
 #pragma unroll
   for (int i = 0; i < DP_KP; ++i) {                       // unrolled: the 8 x 4 tap loads are independent L2 round trips
@@ -481,7 +602,7 @@ sp_desc_pca_kernel(const float* __restrict__ desc, int H, int W, const int32_t* 
     float v = 0.f;
     if (n < N) {
       const Taps t = bilinear_taps(kpts[((size_t)b * max_num + n) * 2], kpts[((size_t)b * max_num + n) * 2 + 1], W, H, Wc, Hc);
-      v = __fsub_rn(__fdiv_rn(sample_channel(d, t, Wc, Hc, tid), cn), mu);
+      v = __fsub_rn(__fdiv_rn(sample_channel<SLOT>(d, sl, cell_n, 0, t, Wc, Hc, tid), cn), mu);
     }
     sv[i][tid] = v;
   }
@@ -501,11 +622,22 @@ sp_desc_pca_kernel(const float* __restrict__ desc, int H, int W, const int32_t* 
 
 osb_status sp_descriptors(const float* desc_nhwc, int B, int H, int W, const int32_t* n_kpts, const float* kpts,
                           int max_num, const float* pca_compT, const float* pca_mean, float* cnorm, float* out,
-                          cudaStream_t st) {
-  OSB_LAUNCH(sp_desc_norm_kernel, dim3(B, 256 / DN_CH), DN_GROUPS * DN_CH, 0, st, desc_nhwc, H, W, n_kpts, kpts, max_num, cnorm);
-  OSB_CHECK_LAUNCH();
-  dim3 grid(cdiv(max_num, DP_KP), B);
-  OSB_LAUNCH(sp_desc_pca_kernel, grid, 256, 0, st, desc_nhwc, H, W, n_kpts, kpts, max_num, cnorm, pca_compT, pca_mean, out);
+                          cudaStream_t st, const int32_t* slot, int seg, float* cell_n) {
+  const dim3 gn(B, 256 / DN_CH), gp(cdiv(max_num, DP_KP), B);
+  if (slot) {
+    OSB_REQUIRE(seg * 4 <= 48 * 1024 && cell_n, "sparse descriptor head: too many rows per image");
+    OSB_LAUNCH(sp_desc_norm_kernel<true>, gn, DN_GROUPS * DN_CH, seg * 4, st, desc_nhwc, slot, seg, cell_n, H, W, n_kpts,
+               kpts, max_num, cnorm);
+    OSB_CHECK_LAUNCH();
+    OSB_LAUNCH(sp_desc_pca_kernel<true>, gp, 256, 0, st, desc_nhwc, slot, cell_n, H, W, n_kpts, kpts, max_num, cnorm,
+               pca_compT, pca_mean, out);
+  } else {
+    OSB_LAUNCH(sp_desc_norm_kernel<false>, gn, DN_GROUPS * DN_CH, 0, st, desc_nhwc, slot, 0, cell_n, H, W, n_kpts, kpts,
+               max_num, cnorm);
+    OSB_CHECK_LAUNCH();
+    OSB_LAUNCH(sp_desc_pca_kernel<false>, gp, 256, 0, st, desc_nhwc, slot, cell_n, H, W, n_kpts, kpts, max_num, cnorm,
+               pca_compT, pca_mean, out);
+  }
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

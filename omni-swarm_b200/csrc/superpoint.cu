@@ -64,6 +64,38 @@ osb_status SuperPoint::band_init() {
   return OSB_OK;
 }
 
+osb_status SuperPoint::sparse_init() {
+  if (const char* e = getenv("OSB_SP_SPARSE_HEAD")) if (atoi(e) == 0) return OSB_OK;
+  if (!use_umma || sparse_head) return OSB_OK;
+  seg = cdiv(std::min(4 * max_num, Hc * Wc), 128) * 128;
+  const size_t rows = (size_t)max_batch * seg;
+  OSB_TRY(res.alloc(&cell_slot, (size_t)max_batch * Hc * Wc));
+  OSB_TRY(res.alloc(&cell_n, rows));
+  OSB_TRY(res.alloc(&col_hi, rows * 1152));
+  OSB_TRY(res.alloc(&col_lo, rows * 1152));
+  OSB_TRY(res.alloc(&da_hi, rows * 256));
+  OSB_TRY(res.alloc(&da_lo, rows * 256));
+  OSB_TRY(res.alloc(&desc_c, rows * 256));
+  // the rows as images of one 8 x 16 tile (the tensor-core kernels' tile), which a 1x1 layer reads without a halo
+  const int tiles = (int)(rows / 128);
+  OSB_TRY(umma_act_maps(&tm_col[0], &tm_col[1], col_hi, col_lo, tiles, 8, 16, 1152, 1));
+  OSB_TRY(umma_act_maps(&tm_da[0], &tm_da[1], da_hi, da_lo, tiles, 8, 16, 256, 1));
+  sparse_head = true;
+  return OSB_OK;
+}
+
+osb_status SuperPoint::sparse_desc_head(int B, const KpJob& kp, cudaStream_t st) {
+  const float SA = SP_ACT_SCALE;
+  const int tiles = B * seg / 128;
+  OSB_TRY(sp_cell_gather(B, H, W, kp.nk, kp.kpts, max_num, seg, cell_slot, in_hi[10], in_lo[10], col_hi, col_lo,
+                         precision == OSB_PRECISION_FP16, st));
+  OSB_TRY(umma_conv_forward(UDa_col, tm_col[0], tm_col[1], tiles, 8, 16, SA, da_hi, da_lo, nullptr, 256, 256, SA, 1, 0, st,
+                            0, precision));                                                   // convDa
+  // convDb; the L2 norm of each row is taken inside the descriptor kernels (sp_descriptors)
+  return umma_conv_forward(UL[11], tm_da[0], tm_da[1], tiles, 8, 16, SA, nullptr, nullptr, desc_c, 256, 256, 1.f, 0, 0, st,
+                           0, precision);
+}
+
 size_t sp_expected_weights() {
   size_t n = 0;
   for (int i = 0; i < 12; ++i) n += (size_t)SP_COUT[i] * SP_CIN[i] * SP_KS[i] * SP_KS[i] + SP_COUT[i];
@@ -108,6 +140,18 @@ osb_status SuperPoint::init(const float* weights, size_t n_weights, int width, i
     const size_t nw = (size_t)SP_COUT[i] * SP_CIN[i] * SP_KS[i] * SP_KS[i];
     OSB_TRY(conv_layer_upload(res, &L[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i]));
     if (use_umma) OSB_TRY(umma_layer_upload(res, &UL[i], p, p + nw, SP_CIN[i], SP_COUT[i], SP_KS[i], SP_W_SCALE));
+    if (use_umma && i == 10) {
+      // convDa as a 1x1 layer of 9 x 128 inputs: input slab (kx * 2 + s) * 3 + ky is channel slab s of tap (ky, kx), the
+      // 3x3 layer's K order (sp_cell_gather)
+      std::vector<float> wc((size_t)256 * 1152);
+      for (int o = 0; o < 256; ++o)
+        for (int c = 0; c < 128; ++c)
+          for (int t = 0; t < 9; ++t) {
+            const int ky = t / 3, kx = t % 3, slab = (kx * 2 + c / 64) * 3 + ky;
+            wc[(size_t)o * 1152 + slab * 64 + c % 64] = p[((size_t)o * 128 + c) * 9 + t];
+          }
+      OSB_TRY(umma_layer_upload(res, &UDa_col, wc.data(), p + nw, 1152, 256, 1, SP_W_SCALE));
+    }
     p += nw + SP_COUT[i];
   }
   {
@@ -211,6 +255,12 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
     mark(st);
     OSB_TRY(sp_softmax_shuffle(d_logits, 80, d_semi, B, Hc, Wc, st));
   }
+  // sparse head: the keypoints first, then the descriptor head at the cells they sample only
+  sparse_ran = sparse_head && kp && !layer_prof;
+  if (sparse_ran) {
+    OSB_TRY(keypoints(B, *kp, st));
+    return sparse_desc_head(B, *kp, st);
+  }
   // the keypoint kernel (one CTA per image, latency-bound) runs beside the descriptor head, which leaves it B SMs
   const bool fork = kp && overlap_kp && !layer_prof && kp_stream;
   int head_ctas = 0;
@@ -235,6 +285,7 @@ osb_status SuperPoint::network_umma(const uint8_t* img_dev, int B, cudaStream_t 
 
 // the network: u8 images (device) -> d_semi, d_desc
 osb_status SuperPoint::network(const uint8_t* img_dev, int B, cudaStream_t st, const KpJob* kp, int zero_row) {
+  sparse_ran = false;
   if (use_umma) return network_umma(img_dev, B, st, kp, zero_row);
   OSB_TRY(conv_first_forward(w1a, b1a, lut, img_dev, actA, B, H, W, 64, 1, ACT_RELU, st));  // conv1a
   OSB_TRY(conv_forward(L[1], actA, actB, B, H, W, 64, ACT_RELU, st));                        // conv1b
@@ -262,10 +313,14 @@ osb_status SuperPoint::keypoints(int B, const KpJob& kp, cudaStream_t st) {
 }
 
 osb_status SuperPoint::descriptors(int B, const KpJob& kp, float* out, cudaStream_t st) {
+  if (sparse_ran)
+    return sp_descriptors(desc_c, B, H, W, kp.nk, kp.kpts, max_num, pca_compT, pca_mean_d, ks.cnorm, out, st, cell_slot, seg,
+                          cell_n);
   return sp_descriptors(d_desc, B, H, W, kp.nk, kp.kpts, max_num, pca_compT, pca_mean_d, ks.cnorm, out, st);
 }
 
 osb_status SuperPoint::postprocess(int B, int32_t* nk, float* kpts, float* conf, float* out, cudaStream_t st) {
+  sparse_ran = false;                   // the caller's map is in d_desc
   const KpJob kp{nk, kpts, conf};
   osb_status s = keypoints(B, kp, st);
   if (s != OSB_OK) return s;

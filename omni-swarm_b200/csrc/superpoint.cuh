@@ -46,6 +46,19 @@ struct SuperPoint {
   const __half* band_const(int prec, int layer, int plane) const;
   // computes band_c with each layer's own kernel on a zero image (both precisions); synchronizes `stream`
   osb_status band_init();
+  // sparse descriptor head (front-end only, after sparse_init): convDa and convDb at the cells the keypoints' bilinear
+  // taps read (sp_cell_gather), the L2 norm inside the descriptor kernels.  convDa runs as a 1x1 layer (UDa_col: 9 x 128
+  // inputs in the 3x3 layer's K order) over those cells' gathered neighbourhoods, so each computed cell is bit-identical to
+  // the dense map's.  Rows of image b: b * seg .. b * seg + seg - 1, seg a multiple of the 128-cell tile.
+  // OSB_SP_SPARSE_HEAD=0 keeps the dense head.
+  UmmaLayer UDa_col;
+  bool sparse_head = false, sparse_ran = false;      // sparse_ran: the last network() left desc_c + cell_slot, not d_desc
+  int seg = 0;
+  int32_t* cell_slot = nullptr;
+  __half *col_hi = nullptr, *col_lo = nullptr, *da_hi = nullptr, *da_lo = nullptr;
+  float *desc_c = nullptr, *cell_n = nullptr;
+  CUtensorMap tm_col[2], tm_da[2];
+  osb_status sparse_init();
   // per-layer timing (debug / bench): ev[i] is recorded after launch i of the network when `layer_prof` is set
   bool layer_prof = false;
   cudaEvent_t lev[20] = {};
@@ -58,6 +71,7 @@ struct SuperPoint {
   // keypoint extraction needs only the detector head: when a KpJob is passed, the network launches it on `kp_stream`
   // as soon as the heat map exists and runs the descriptor head beside it (on B fewer SMs); `st` re-joins before return
   struct KpJob { int32_t* nk; float* kpts; float* conf; };
+  osb_status sparse_desc_head(int B, const KpJob& kp, cudaStream_t st);
   cudaStream_t kp_stream = nullptr;
   cudaEvent_t ev_semi = nullptr, ev_kp = nullptr;
   bool overlap_kp = true;
