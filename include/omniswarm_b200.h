@@ -590,7 +590,9 @@ osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_
  *   factor compaction pass over them) and returns the bound as *n_out.  Every synchronising call (run, size,
  *   add_measurements, push_odometry, set_window, status) first waits for the last device append, after which the counts are
  *   exact and run returns exactly n_loops + n_detections rows.  A handle that never calls add_measurements_dev behaves as
- *   if it did not exist.
+ *   if it did not exist.  The call can be captured into a CUDA graph (after an uncaptured first call): its waits for the
+ *   handle's last run and append become external event waits, and its own event an external record, so the synchronising
+ *   calls after a replay wait for the replayed append.
  * osb_anchor_status(): waits for the last device append and writes its status to *last (OSB_OK when none ran); returns the
  *   same value. */
 #define OSB_ANCHOR_VOID 6
@@ -1025,6 +1027,88 @@ osb_status osb_frontend_loop_measurements(osb_frontend* h, const osb_loop_result
                                           double loop_cov_pos, double loop_cov_ang, osb_measurement* out_dev /*[n]*/,
                                           int32_t* count_dev, void* stream);
 osb_status osb_frontend_loop_counts(osb_frontend* h, int64_t* loop_count, int32_t* pair_counts /*[256][256] or NULL*/);
+
+/* Keyframe metadata on the device -- the pose_drone and timestamp every FisheyeFrameDescriptor_t carries
+ *   (fisheyeframe_database, loop_detector.cpp:105-111, 150-173) and the ego-motion trajectory built from them (:27), so that
+ *   a round's loop candidates are built without a host read.
+ * osb_keyframe_meta travels beside osb_keyframe_record: one meta per record, same index (72 bytes).
+ * ingest_meta / ingest_own_meta: exactly osb_frontend_ingest / osb_frontend_ingest_own (the same rows, routing, frame slots,
+ *   host bounds and launches), and each meta goes into the frame slot its record took.  A meta whose drone_id or msg_id
+ *   differs from its record's is not stored (that frame has no meta) and the call's status is OSB_ERR_INVALID.  Every own
+ *   keyframe (drone_id == self_id) ingested with a stored meta appends (stamp_ns, pose_drone) to the ego-motion trajectory in
+ *   ingest order; a stamp not after the last sample is not appended (status OSB_ERR_INVALID), nor is a sample beyond
+ *   db_capacity samples (OSB_ERR_CAPACITY).  Frames ingested through ingest / ingest_own and rows of db_load have no meta.
+ *   The first call acquires the meta tables of both stores (a meta and a flag per frame slot, db_capacity x 76 bytes each) and
+ *   the trajectory (db_capacity samples x 72 bytes); osb_frontend_db_reset clears the tables and keeps the trajectory.  Null
+ *   pointers give OSB_ERR_INVALID with nothing enqueued.
+ * osb_frontend_meta_status(): waits for the last ingest and writes the status of the last meta ingest to *last (OSB_OK
+ *   when none ran); returns the same value.
+ * Trajectory: length[k] = the sequential fp64 sum of |p_k - p_(k-1)| (sqrt((dx*dx + dy*dy) + dz*dz), no fused multiply-add);
+ *   a look-up takes the sample nearest to the stamp (ties to the earlier, clamped at both ends), as osb_anchor's.
+ *   relative pose (ts_a, ts_b) = pose(ts_a)^-1 * pose(ts_b); its covariance = |len(ts_b) - len(ts_a)| *
+ *   diag(pos_covariance_per_meter x3, yaw_covariance_per_meter x3).  Only own keyframes enter it (the reference also pushes
+ *   foreign frames, DESIGN.md section 5).
+ * set_candidate_params: inter_drone_init_frames and the covariances of swarm_loop.cpp:227-256. */
+typedef struct {
+  int32_t drone_id;
+  int32_t msg_id;
+  int64_t stamp_ns;
+  double pose_drone[7];            /* x y z, qw qx qy qz */
+} osb_keyframe_meta;
+typedef struct {
+  int32_t inter_drone_init_frames; /* inter_drone_init_frames (50) */
+  int32_t reserved;
+  double pos_covariance_per_meter; /* 0.01 */
+  double yaw_covariance_per_meter; /* 0.003 */
+  double loop_cov_pos;             /* 0.013 */
+  double loop_cov_ang;             /* 2.5e-4 */
+} osb_candidate_params;
+osb_status osb_frontend_ingest_meta(osb_frontend* h, const osb_keyframe_record* records_dev, const osb_keyframe_meta* metas_dev,
+                                    int n_records, int skip, void* stream);
+osb_status osb_frontend_ingest_own_meta(osb_frontend* h, const osb_keyframe_record* record_dev, const osb_keyframe_meta* meta_dev,
+                                        void* stream);
+osb_status osb_frontend_meta_status(osb_frontend* h, osb_status* last);
+osb_status osb_frontend_set_candidate_params(osb_frontend* h, const osb_candidate_params* p);
+/* osb_frontend_init_modes_dev(): init_mode_out_dev[r] (bytes, DEVICE) = the init_mode of on_image_recv (loop_detector.cpp
+ *   :65-72) for records r of a received round: 1 iff drone_id != self_id and inter_drone_loop_count[drone_id][self_id] <
+ *   inter_drone_init_frames, read from the device's counters (osb_frontend_loop_measurements); 0 for r == skip.  Drone ids
+ *   outside 0..255 count 0.  One launch, no synchronisation; 0 <= n_records <= 64; needs set_candidate_params.
+ * osb_frontend_query_received_dev(): osb_frontend_query_received with init_mode a DEVICE byte array [n_records] (or NULL, all
+ *   0) read by the rule kernel; the same launches and results. */
+osb_status osb_frontend_init_modes_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records, int skip,
+                                       uint8_t* init_mode_out_dev, void* stream);
+osb_status osb_frontend_query_received_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records, int skip,
+                                           const uint8_t* init_mode_dev, osb_loop_result* results_dev, void* stream);
+/* osb_frontend_loop_candidates_dev(): the osb_loop_candidate and osb_loop_stamps a host caller of compute_loop /
+ *   loop_measurements writes (INTEGRATION.md 2.5), built on the device for results_dev [n] of query / query_received,
+ *   records_dev [n] and metas_dev [n] (DEVICE), with the stores as they are now.  One launch, one thread per candidate, no
+ *   synchronisation; 0 <= n <= 64 (0 does nothing); needs set_candidate_params.  Acquires the meta tables and the loop
+ *   counters when no earlier call has.
+ *   Query side: metas_dev[i] (pose_query, stamp_query_ns) when its drone_id / msg_id are records[i]'s.  Hit side (accepted
+ *   results): the meta of the hit's frame in the store that holds it (pose_hit, stamp_hit_ns).  A missing side is the
+ *   identity pose and stamp 0.  init_mode: init_mode_dev[i] when init_mode_dev is not NULL, else the rule of
+ *   osb_frontend_init_modes_dev on records[i].drone_id.  Same-drone accepted candidates (drone_id == hit_drone_id):
+ *   odom_rel = the trajectory's relative pose (ts_a, ts_b) with a = the old side, b = the new side (results[i].swapped
+ *   routes them as compute_loop does), odom_edge_cov = its covariance + diag(loop_cov_pos x3, loop_cov_ang x3); other
+ *   candidates: odom_rel identity, odom_edge_cov zero.  Every value is computed in fp64 with each product rounded on its own
+ *   (the order of tests/loop_candidates_ref.py).  reserved = 1 marks an accepted candidate whose query or hit has no meta (or
+ *   a same-drone one with an empty trajectory): compute_loop_dev gives it OSB_LOOP_NO_FRAME; 0 otherwise.
+ * osb_frontend_compute_loop_dev() / osb_frontend_loop_measurements_dev(): osb_frontend_compute_loop /
+ *   osb_frontend_loop_measurements with the candidates (and stamps) read from DEVICE arrays [n], e.g. what
+ *   loop_candidates_dev wrote; the same launches and, for unmarked candidates, the same bytes.  With them a round from
+ *   query_received through osb_anchor_add_measurements_dev enqueues with no host read and can be captured into a CUDA
+ *   graph. */
+osb_status osb_frontend_loop_candidates_dev(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                            const osb_keyframe_meta* metas_dev, const osb_loop_result* results_dev, int n,
+                                            const uint8_t* init_mode_dev, osb_loop_candidate* cand_out_dev,
+                                            osb_loop_stamps* stamps_out_dev, void* stream);
+osb_status osb_frontend_compute_loop_dev(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                         const osb_loop_result* results_dev, int n, const osb_loop_candidate* cand_dev,
+                                         osb_loop_edge_result* out_dev, void* stream);
+osb_status osb_frontend_loop_measurements_dev(osb_frontend* h, const osb_loop_result* results_dev,
+                                              const osb_loop_edge_result* edges_dev, int n, const osb_loop_candidate* cand_dev,
+                                              const osb_loop_stamps* stamps_dev, double loop_cov_pos, double loop_cov_ang,
+                                              osb_measurement* out_dev, int32_t* count_dev, void* stream);
 /* ------------------------------------------------------------------------------------------------------------
  * Swarm-wide keyframe exchange -- replaces LoopNet::broadcast_fisheye_desc / image_desc_callback
  *   (swarm_loop/src/loop_net.cpp:20-120,142-172; called from swarm_loop/src/swarm_loop.cpp:167): the LCM UDP multicast of
@@ -1054,6 +1138,11 @@ osb_status osb_swarm_exchange(osb_swarm* h, const osb_keyframe_record* record_de
 osb_status osb_swarm_exchange_async(osb_swarm* h, const osb_keyframe_record* record_dev, osb_keyframe_record* gathered_dev,
                                     void* stream);
 osb_status osb_swarm_wait(osb_swarm* h, void* stream);
+/* exchange_meta: meta_dev (this drone's osb_keyframe_meta, the one beside its record) -> gathered_dev[world] in rank order:
+ *   one ncclAllGather of world x 72 bytes on `stream` (a device copy at world == 1), no synchronisation.  Pair it with
+ *   osb_swarm_exchange of the record, so that gathered metas and records share their index. */
+osb_status osb_swarm_exchange_meta(osb_swarm* h, const osb_keyframe_meta* meta_dev, osb_keyframe_meta* gathered_dev,
+                                   void* stream);
 int osb_swarm_transport(osb_swarm* h);     /* what exchange_async uses: 1 = peer-to-peer copy engines (CUDA IPC inboxes, stream
                                               stamps; no SM, no NCCL kernel), 0 = ncclAllGather on the side stream */
 int osb_swarm_rank(osb_swarm* h);

@@ -290,6 +290,40 @@ inline void hand_loops_to_anchor(osb_frontend* fe, osb_anchor* anchor, const osb
         "osb_anchor_add_measurements_dev");
 }
 
+// A whole received round on the device, from LoopDetector::on_image_recv to add_new_loop_connection: the init modes from the
+// device's inter_drone_loop_count, query_received, the candidates from the keyframe metadata (records_dev / metas_dev [n],
+// the all-gather outputs of osb_swarm_exchange and osb_swarm_exchange_meta; the keyframes ingested with
+// osb_frontend_ingest_meta), compute_loop, the LoopEdge rows and the anchor's append.  Stream-ordered, no host read and no
+// synchronisation, so the sequence can be captured into a CUDA graph.  The DEVICE scratch: init_dev [n], results_dev [n],
+// cand_dev [n], stamps_dev [n], edges_dev [n], meas_dev [n] and count_dev.
+struct RoundScratch {
+  uint8_t* init_dev;
+  osb_loop_result* results_dev;
+  osb_loop_candidate* cand_dev;
+  osb_loop_stamps* stamps_dev;
+  osb_loop_edge_result* edges_dev;
+  osb_measurement* meas_dev;
+  int32_t* count_dev;
+};
+inline void hand_round_to_anchor_dev(osb_frontend* fe, osb_anchor* anchor, const osb_keyframe_record* records_dev,
+                                     const osb_keyframe_meta* metas_dev, int n, int skip, const RoundScratch& s,
+                                     double loop_cov_pos, double loop_cov_ang, float loop_outlier_distance_threshold,
+                                     void* stream) {
+  if (n == 0) return;
+  check(osb_frontend_init_modes_dev(fe, records_dev, n, skip, s.init_dev, stream), "osb_frontend_init_modes_dev");
+  check(osb_frontend_query_received_dev(fe, records_dev, n, skip, s.init_dev, s.results_dev, stream),
+        "osb_frontend_query_received_dev");
+  check(osb_frontend_loop_candidates_dev(fe, records_dev, metas_dev, s.results_dev, n, s.init_dev, s.cand_dev, s.stamps_dev,
+                                         stream), "osb_frontend_loop_candidates_dev");
+  check(osb_frontend_compute_loop_dev(fe, records_dev, s.results_dev, n, s.cand_dev, s.edges_dev, stream),
+        "osb_frontend_compute_loop_dev");
+  check(osb_frontend_loop_measurements_dev(fe, s.results_dev, s.edges_dev, n, s.cand_dev, s.stamps_dev, loop_cov_pos,
+                                           loop_cov_ang, s.meas_dev, s.count_dev, stream),
+        "osb_frontend_loop_measurements_dev");
+  check(osb_anchor_add_measurements_dev(anchor, s.meas_dev, s.count_dev, n, loop_outlier_distance_threshold, stream),
+        "osb_anchor_add_measurements_dev");
+}
+
 // The same factors from osb_anchor_compact_factors_dev's SoA after its one copy to the host: count rows of type / ia / ib /
 // payload [count][OSB_PAYLOAD_LEN] / huber.  Returns the number of factors added (count).
 inline int add_compacted_factors(FlatPoseGraph& graph, int count, const int32_t* ia, const int32_t* ib, const double* payload,

@@ -74,18 +74,6 @@ __device__ __forceinline__ int anchor_search(const AnchorView& v, int d, int64_t
   return idx == INT_MAX ? -1 : idx;
 }
 
-// DroneTrajectory look-up: the sample nearest to t, ties to the earlier one, clamped to the first / last sample
-__device__ __forceinline__ int nearest_sample(const int64_t* __restrict__ s, int n, int64_t t) {
-  int lo = 0, hi = n;                                              // first k with s[k] >= t
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (s[mid] < t) lo = mid + 1; else hi = mid;
-  }
-  if (lo == 0) return 0;
-  if (lo == n) return n - 1;
-  return (t - s[lo - 1]) <= (s[lo] - t) ? lo - 1 : lo;
-}
-
 // RelativePoseFactor4d::CreateCov6d: S = sqrt|inv(blkdiag(cov[0:3,0:3], cov[5,5]))|, Gauss-Jordan with partial pivoting
 __device__ void sqrt_information_4d(const double* cov, double* S) {
   double A[4][8];
@@ -790,9 +778,9 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
   cudaStream_t st = (cudaStream_t)stream;
   OSB_TRY(anchor_dev_init(h));
   // the append rewrites the counts a run reads and follows the previous append, whichever streams those ran on
-  OSB_CUDA(cudaStreamWaitEvent(st, h->last_run, 0));
+  OSB_CUDA(wait_event_capturable(st, h->last_run));
   if (h->append_pending) {
-    OSB_CUDA(cudaStreamWaitEvent(st, h->last_append, 0));
+    OSB_CUDA(wait_event_capturable(st, h->last_append));
     anchor_tighten(h);
   } else {
     h->upper = h->n_loops + h->n_dets;
@@ -802,7 +790,7 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
              h->p.max_drones, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb_dev, seq,
              charged);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(cudaEventRecord(h->last_append, st));
+  OSB_CUDA(record_event_capturable(h->last_append, st));
   h->append_seq = seq;
   h->charged = charged;
   h->upper = std::min<long long>(h->upper + max_n, h->p.max_measurements);

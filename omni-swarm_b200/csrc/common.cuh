@@ -129,6 +129,25 @@ inline osb_status require_device() {
   return OSB_OK;
 }
 
+// cudaEventRecord for an event the handle's synchronising calls wait on later: inside a stream capture it becomes an
+// external event-record node, so every replay of the graph records the event (a plain record in a capture is only a
+// dependency edge, and the event would stay as the last uncaptured record left it)
+inline cudaError_t record_event_capturable(cudaEvent_t ev, cudaStream_t st) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+  if (e != cudaSuccess) return e;
+  return cs == cudaStreamCaptureStatusActive ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal)
+                                             : cudaEventRecord(ev, st);
+}
+// cudaStreamWaitEvent for such an event: inside a stream capture an external event-wait node, which on every replay waits
+// for the event's latest record (a plain wait on work recorded outside the capture invalidates the capture)
+inline cudaError_t wait_event_capturable(cudaStream_t st, cudaEvent_t ev) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+  if (e != cudaSuccess) return e;
+  return cudaStreamWaitEvent(st, ev, cs == cudaStreamCaptureStatusActive ? cudaEventWaitExternal : 0);
+}
+
 // The one owner of CUDA resources: every device buffer, pinned host buffer, stream and event of a handle (or of one call)
 // is acquired through it, and its destructor releases them all in reverse order of acquisition, on the device it was
 // created on.  An early return therefore frees whatever was acquired so far.  Not copyable: nothing is released twice.

@@ -172,12 +172,62 @@ __global__ void fe_pack_kernel(osb_keyframe_record* __restrict__ rec, int drone_
   }
 }
 
-// add_to_database for a batch of records: phase 1 (one thread) assigns rows in record/direction order
+// keyframe metadata (osb_frontend_ingest_meta): per store a meta and a stored-flag per frame slot, and the ego-motion
+// trajectory of the own keyframes (stamps, poses, sequential lengths) with its sample count and the last call's status
+struct FeMetaDev {
+  int32_t traj_n;
+  int32_t status;
+};
+struct FeMeta {
+  osb_keyframe_meta* meta[2];   // [cap] per store, indexed by frame slot
+  int32_t* ok[2];               // [cap] 1 = the slot's meta is stored
+  int64_t* t_stamp;             // [t_cap]
+  double* t_pose;               // [t_cap][7]
+  double* t_len;                // [t_cap]
+  int t_cap;
+  FeMetaDev* dev;
+};
+
+// a product rounded on its own (__dmul_rn is never contracted into an FMA)
+__device__ __forceinline__ double lc_mul(double a, double b) { return __dmul_rn(a, b); }
+
+// the meta of the record that has just taken frame slot fs of store is_remote; own keyframes also extend the trajectory.
+// Returns the status so far, the first refusal kept.
+__device__ int fe_store_meta(const FeMeta& mt, int is_remote, int fs, const osb_keyframe_record* rec,
+                             const osb_keyframe_meta& m, int status) {
+  const bool ok = m.drone_id == rec->drone_id && m.msg_id == rec->msg_id;
+  mt.ok[is_remote][fs] = ok ? 1 : 0;
+  if (!ok) return status != OSB_OK ? status : OSB_ERR_INVALID;
+  mt.meta[is_remote][fs] = m;
+  if (is_remote) return status;
+  const int n = mt.dev->traj_n;
+  int refused = OSB_OK;
+  if (n > 0 && m.stamp_ns <= mt.t_stamp[n - 1]) refused = OSB_ERR_INVALID;
+  else if (n >= mt.t_cap) refused = OSB_ERR_CAPACITY;
+  if (refused != OSB_OK) return status != OSB_OK ? status : refused;
+  double len = 0.0;                                          // length[k] = length[k-1] + |p_k - p_(k-1)|, in sample order
+  if (n > 0) {
+    const double* q = mt.t_pose + (size_t)(n - 1) * 7;
+    const double dx = m.pose_drone[0] - q[0], dy = m.pose_drone[1] - q[1], dz = m.pose_drone[2] - q[2];
+    len = mt.t_len[n - 1] + sqrt((lc_mul(dx, dx) + lc_mul(dy, dy)) + lc_mul(dz, dz));
+  }
+  mt.t_stamp[n] = m.stamp_ns;
+  for (int k = 0; k < 7; ++k) mt.t_pose[(size_t)n * 7 + k] = m.pose_drone[k];
+  mt.t_len[n] = len;
+  mt.dev->traj_n = n + 1;
+  return status;
+}
+
+// add_to_database for a batch of records: phase 1 (one thread) assigns rows in record/direction order.  META: metas [n]
+// beside the records go into the frame slots the records take (osb_frontend_ingest_meta); the plain ingest passes none.
+template <bool META>
 __global__ void fe_assign_kernel(const osb_keyframe_record* __restrict__ recs, int n_records, int skip, int self_id,
                                  long long cap, const __grid_constant__ FeStores dbs,
                                  int32_t* __restrict__ assign /*[n_records][4]: row | (remote<<30), or -1*/,
-                                 FeFeedback* __restrict__ fb, long long seq, long long charged) {
+                                 FeFeedback* __restrict__ fb, long long seq, long long charged,
+                                 const osb_keyframe_meta* __restrict__ metas, FeMeta mt) {
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  int meta_status = OSB_OK;
   for (int r = 0; r < n_records; ++r) {
     for (int d = 0; d < OSB_MAX_DIRS; ++d) assign[r * OSB_MAX_DIRS + d] = -1;
     if (r == skip) continue;
@@ -189,6 +239,7 @@ __global__ void fe_assign_kernel(const osb_keyframe_record* __restrict__ recs, i
     const int fs = cnt.nframes++;
     db.frame_msg[fs] = rec->msg_id;
     db.frame_drone[fs] = rec->drone_id;
+    if constexpr (META) meta_status = fe_store_meta(mt, is_remote ? 1 : 0, fs, rec, metas[r], meta_status);
     for (int d = 0; d < OSB_MAX_DIRS; ++d) {
       db.frame_rows[fs * OSB_MAX_DIRS + d] = -1;
       if (d >= rec->n_dirs || rec->n_kpts[d] <= 0) continue;         // landmark_num > 0 (loop_detector.cpp:153)
@@ -200,6 +251,7 @@ __global__ void fe_assign_kernel(const osb_keyframe_record* __restrict__ recs, i
     }
     *db.dev = cnt;
   }
+  if constexpr (META) mt.dev->status = meta_status;
   fb->seq_begin = seq;
   __threadfence_system();
   fb->n_local = dbs.db[0].dev->ntotal; fb->n_remote = dbs.db[1].dev->ntotal; fb->charged = charged;
@@ -277,9 +329,11 @@ __device__ int fe_search_rule(const float* scores, const int64_t* ids, int k, in
 // one thread per record (qp.n of them): the acceptance rule of query_from_database / query_fisheyeframe_from_database
 // and the direction pairing of compute_correspond_features (loop_detector.cpp:455-465); fills record r's OSB_MAX_DIRS
 // slots of the matcher's pair table.  The remote top-k (read for own keyframes only) is the remote store's.
+// DEV_INIT: record r's init_mode is init_dev[r] (a device byte array, or null: all 0) instead of bit r of qp.init_mask.
+template <bool DEV_INIT>
 __global__ void fe_query_rule_kernel(QueryParams qp, const osb_keyframe_record* __restrict__ recs,
                                      const __grid_constant__ FeStores dbs, osb_loop_result* __restrict__ results,
-                                     FePairView pairs) {
+                                     FePairView pairs, const uint8_t* __restrict__ init_dev) {
   const int rr = threadIdx.x;
   if (blockIdx.x != 0 || rr >= qp.n) return;
   const osb_keyframe_record* rec = recs + rr;
@@ -289,7 +343,9 @@ __global__ void fe_query_rule_kernel(QueryParams qp, const osb_keyframe_record* 
   // a received batch queries the foreign records only (on_image_recv runs for them, :98-104); the skipped slot is not read
   const bool closed = qp.received && (rr == qp.skip || rec->drone_id == qp.self_id);
   const bool own = !closed && rec->drone_id == qp.self_id;
-  const bool init_mode = (qp.init_mask >> rr) & 1ull;
+  bool init_mode;
+  if constexpr (DEV_INIT) init_mode = init_dev != nullptr && init_dev[rr] != 0;
+  else init_mode = (qp.init_mask >> rr) & 1ull;
   const float* l_scores = qp.l_scores + (size_t)rr * qp.l_stride;
   const int64_t* l_ids = qp.l_ids + (size_t)rr * qp.l_stride;
   const double thres = init_mode ? qp.init_mode_product_thres : qp.inner_product_thres;
@@ -459,10 +515,14 @@ struct LoopCams {              // the old (own) frame's camera: pinhole fx fy cx
 struct LoopCandBatch {         // the host's candidates, passed as kernel parameters (sm_90 takes up to 32 KB of them)
   osb_loop_candidate c[LC_MAX];
 };
+struct LoopCandPtr {           // candidates in device memory (osb_frontend_compute_loop_dev)
+  const osb_loop_candidate* c;
+};
+__device__ __forceinline__ const osb_loop_candidate& lc_cand(const LoopCandBatch& b, int i) { return b.c[i]; }
+__device__ __forceinline__ const osb_loop_candidate& lc_cand(const LoopCandPtr& b, int i) { return b.c[i]; }
 
 // Swarm::Pose algebra in the evaluation order of oracle/pcm_ref.py with every product rounded on its own (__dmul_rn is never
 // contracted into an FMA): the PnP prior and the rotated points are then the bits a numpy host caller computes
-__device__ __forceinline__ double lc_mul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ void lc_cross(const double* a, const double* b, double* o) {
   o[0] = lc_mul(a[1], b[2]) - lc_mul(a[2], b[1]);
   o[1] = lc_mul(a[2], b[0]) - lc_mul(a[0], b[2]);
@@ -506,16 +566,19 @@ __device__ __forceinline__ float2 lc_lift_rotate(float kx, float ky, const doubl
   return make_float2((float)(r[0] / z), (float)(r[1] / z));
 }
 
+// Cands: LoopCandBatch (the host's array as parameters) or LoopCandPtr (a device array, whose reserved != 0 marks a
+// candidate without keyframe metadata: OSB_LOOP_NO_FRAME)
+template <class Cands>
 __global__ void __launch_bounds__(256)
 lc_assemble_kernel(const osb_keyframe_record* __restrict__ recs, const osb_loop_result* __restrict__ results,
-                   const __grid_constant__ FeStores dbs, const __grid_constant__ LoopCandBatch cands,
+                   const __grid_constant__ FeStores dbs, const __grid_constant__ Cands cands,
                    const __grid_constant__ LoopCams cam, const osb_loop_params lp, int query_dir, int max_num,
                    osb_loop_edge_result* __restrict__ out, float* __restrict__ pts3d, float* __restrict__ pts2d,
                    int32_t* __restrict__ n_pts, osb_pnp_params* __restrict__ params) {
   const int c = blockIdx.x, tid = threadIdx.x;
   const osb_keyframe_record* rec = recs + c;
   const osb_loop_result* res = results + c;
-  const osb_loop_candidate& cd = cands.c[c];
+  const osb_loop_candidate& cd = lc_cand(cands, c);
   osb_loop_edge_result* o = out + c;
   const DbView &L = dbs.db[0], &R = dbs.db[1];
   // roles (:113-118): swapped -> the remote hit is "new", this drone's record "old"; the old frame is always our own (:637)
@@ -530,6 +593,8 @@ lc_assemble_kernel(const osb_keyframe_record* __restrict__ recs, const osb_loop_
     fs = hdb.row_frame[hit_remote ? res->hit_id - OSB_REMOTE_MAGIN_NUMBER : res->hit_id];
     // a row put in with db_load has no keyframe behind it; the new side of a swapped edge needs the remote 3-D plane
     if (res->hit_msg_id == -1 || (swapped && R.l3d == nullptr) || hit_remote != swapped) status = OSB_LOOP_NO_FRAME;
+    if constexpr (std::is_same<Cands, LoopCandPtr>::value)
+      if (cd.reserved != 0) status = OSB_LOOP_NO_FRAME;
   }
   if (status == LC_PENDING) {                               // new_frame_desc.landmark_num < MIN_LOOP_NUM (:632)
     int lm = 0;
@@ -674,10 +739,23 @@ struct LoopMeasBatch {         // the host's poses and stamps of the candidates,
   int64_t stamp_query[LC_MAX];
   int64_t stamp_hit[LC_MAX];
 };
+struct LoopMeasPtr {           // the same read from device arrays (osb_frontend_loop_measurements_dev)
+  const osb_loop_candidate* cand;
+  const osb_loop_stamps* stamps;
+};
+__device__ __forceinline__ const double* lm_pose_query(const LoopMeasBatch& b, int c) { return b.pose_query[c]; }
+__device__ __forceinline__ const double* lm_pose_hit(const LoopMeasBatch& b, int c) { return b.pose_hit[c]; }
+__device__ __forceinline__ int64_t lm_stamp_query(const LoopMeasBatch& b, int c) { return b.stamp_query[c]; }
+__device__ __forceinline__ int64_t lm_stamp_hit(const LoopMeasBatch& b, int c) { return b.stamp_hit[c]; }
+__device__ __forceinline__ const double* lm_pose_query(const LoopMeasPtr& b, int c) { return b.cand[c].pose_query; }
+__device__ __forceinline__ const double* lm_pose_hit(const LoopMeasPtr& b, int c) { return b.cand[c].pose_hit; }
+__device__ __forceinline__ int64_t lm_stamp_query(const LoopMeasPtr& b, int c) { return b.stamps[c].stamp_query_ns; }
+__device__ __forceinline__ int64_t lm_stamp_hit(const LoopMeasPtr& b, int c) { return b.stamps[c].stamp_hit_ns; }
 
+template <class Meas>
 __global__ void __launch_bounds__(256)
 lm_emit_kernel(const osb_loop_result* __restrict__ results, const osb_loop_edge_result* __restrict__ edges, int n,
-               const __grid_constant__ LoopMeasBatch b, int self_id, double cov_pos, double cov_ang,
+               const __grid_constant__ Meas b, int self_id, double cov_pos, double cov_ang,
                osb_measurement* __restrict__ out, int32_t* __restrict__ count, long long* __restrict__ loop_count,
                int32_t* __restrict__ pair_counts) {
   const int c = threadIdx.x;
@@ -695,10 +773,10 @@ lm_emit_kernel(const osb_loop_result* __restrict__ results, const osb_loop_edge_
   m.id_a = e.drone_id_a;
   m.id_b = e.drone_id_b;
   m.reserved = 0;
-  m.stamp_a = swapped ? b.stamp_query[c] : b.stamp_hit[c];
-  m.stamp_b = swapped ? b.stamp_hit[c] : b.stamp_query[c];
-  const double* pa = swapped ? b.pose_query[c] : b.pose_hit[c];
-  const double* pb = swapped ? b.pose_hit[c] : b.pose_query[c];
+  m.stamp_a = swapped ? lm_stamp_query(b, c) : lm_stamp_hit(b, c);
+  m.stamp_b = swapped ? lm_stamp_hit(b, c) : lm_stamp_query(b, c);
+  const double* pa = swapped ? lm_pose_query(b, c) : lm_pose_hit(b, c);
+  const double* pb = swapped ? lm_pose_hit(b, c) : lm_pose_query(b, c);
   for (int k = 0; k < 7; ++k) { m.relative_pose[k] = e.relative_pose[k]; m.self_pose_a[k] = pa[k]; m.self_pose_b[k] = pb[k]; }
   for (int k = 0; k < 36; ++k) m.cov[k] = (k % 7 == 0) ? (k < 21 ? cov_pos : cov_ang) : 0.0;     // pos_cov / ang_cov (:800-808)
   const int a = e.drone_id_a, nw = e.drone_id_b;           // :824-827: an intra-drone loop adds 2 to its one cell
@@ -706,6 +784,82 @@ lm_emit_kernel(const osb_loop_result* __restrict__ results, const osb_loop_edge_
     atomicAdd(&pair_counts[nw * LM_PAIR_DRONES + a], 1);
     atomicAdd(&pair_counts[a * LM_PAIR_DRONES + nw], 1);
   }
+}
+
+// ---- a round's loop candidates from the device's keyframe metadata (osb_frontend_loop_candidates_dev) -----------------
+struct CandRule {              // osb_candidate_params and the handle's self_id
+  int self_id, init_frames;
+  double pos_per_m, ang_per_m, loop_pos, loop_ang;
+};
+
+// on_image_recv's init_mode (loop_detector.cpp:65-72) from inter_drone_loop_count [256][256] ([new][old]); ids outside
+// 0..255 count 0
+__device__ __forceinline__ bool fe_init_mode(int drone, int self_id, const int32_t* __restrict__ pairs, int init_frames) {
+  if (drone == self_id) return false;
+  const bool in = drone >= 0 && drone < LM_PAIR_DRONES && self_id >= 0 && self_id < LM_PAIR_DRONES;
+  const int cnt = in ? pairs[drone * LM_PAIR_DRONES + self_id] : 0;
+  return !(cnt >= init_frames);
+}
+
+__global__ void fe_init_modes_kernel(const osb_keyframe_record* __restrict__ recs, int n, int skip, CandRule cr,
+                                     const int32_t* __restrict__ pairs, uint8_t* __restrict__ out) {
+  const int i = threadIdx.x;
+  if (i >= n) return;
+  out[i] = (i != skip && fe_init_mode(recs[i].drone_id, cr.self_id, pairs, cr.init_frames)) ? 1 : 0;
+}
+
+// candidate i on thread i: the query side from metas[i], the hit side from the meta table of the hit's store, init_mode,
+// and for same-drone hits the ego-motion trajectory's relative pose and covariance (check_loop_odometry_consistency,
+// loop_detector.cpp:294-303) in the order of tests/loop_candidates_ref.py
+__global__ void lc_candidates_kernel(const osb_keyframe_record* __restrict__ recs, const osb_keyframe_meta* __restrict__ metas,
+                                     const osb_loop_result* __restrict__ results, int n, const uint8_t* __restrict__ init_dev,
+                                     const __grid_constant__ FeStores dbs, FeMeta mt, const int32_t* __restrict__ pairs,
+                                     CandRule cr, osb_loop_candidate* __restrict__ cand_out,
+                                     osb_loop_stamps* __restrict__ stamps_out) {
+  const int i = threadIdx.x;
+  if (i >= n) return;
+  const osb_keyframe_record* rec = recs + i;
+  const osb_loop_result* res = results + i;
+  const osb_keyframe_meta& mq = metas[i];
+  const bool q_ok = mq.drone_id == rec->drone_id && mq.msg_id == rec->msg_id;
+  const bool accepted = res->accepted != 0;
+  const osb_keyframe_meta* mh = nullptr;
+  if (accepted) {
+    const bool hit_remote = res->hit_id >= OSB_REMOTE_MAGIN_NUMBER;
+    const int fs = dbs.db[hit_remote].row_frame[hit_remote ? res->hit_id - OSB_REMOTE_MAGIN_NUMBER : res->hit_id];
+    if (mt.ok[hit_remote][fs]) mh = mt.meta[hit_remote] + fs;
+  }
+  osb_loop_candidate c;
+  memset(&c, 0, sizeof(c));
+  c.init_mode = (init_dev ? init_dev[i] != 0 : fe_init_mode(rec->drone_id, cr.self_id, pairs, cr.init_frames)) ? 1 : 0;
+  const int64_t sq = q_ok ? mq.stamp_ns : 0, sh = mh ? mh->stamp_ns : 0;
+  for (int k = 0; k < 7; ++k) {
+    const double id = k == 3 ? 1.0 : 0.0;
+    c.pose_query[k] = q_ok ? mq.pose_drone[k] : id;
+    c.pose_hit[k] = mh ? mh->pose_drone[k] : id;
+    c.odom_rel[k] = id;
+  }
+  bool mark = accepted && (!q_ok || mh == nullptr);
+  if (accepted && !mark && rec->drone_id == res->hit_drone_id) {
+    const int tn = mt.dev->traj_n;
+    if (tn == 0) {
+      mark = true;
+    } else {
+      const bool swapped = res->swapped != 0;                 // compute_loop's roles: a = old, b = new
+      const int ka = nearest_sample(mt.t_stamp, tn, swapped ? sq : sh);
+      const int kb = nearest_sample(mt.t_stamp, tn, swapped ? sh : sq);
+      double inv[7];
+      lc_pose_inv(mt.t_pose + (size_t)ka * 7, inv);
+      lc_pose_mul(inv, mt.t_pose + (size_t)kb * 7, c.odom_rel);
+      const double dl = fabs(mt.t_len[kb] - mt.t_len[ka]);
+      for (int k = 0; k < 6; ++k)
+        c.odom_edge_cov[k * 7] = k < 3 ? lc_mul(dl, cr.pos_per_m) + cr.loop_pos : lc_mul(dl, cr.ang_per_m) + cr.loop_ang;
+    }
+  }
+  c.reserved = mark ? 1 : 0;
+  cand_out[i] = c;
+  stamps_out[i].stamp_query_ns = sq;
+  stamps_out[i].stamp_hit_ns = sh;
 }
 
 }  // namespace osb
@@ -766,6 +920,13 @@ struct osb_frontend {
   long long* d_lm_count = nullptr;
   int32_t* d_lm_pairs = nullptr;
   cudaEvent_t ev_lm = nullptr;
+  // keyframe metadata (osb_frontend_ingest_meta): both stores' meta tables and the ego-motion trajectory, acquired by the
+  // first meta ingest (meta_ready); h_meta is the pinned copy osb_frontend_meta_status reads
+  bool meta_ready = false;
+  FeMeta meta{};
+  FeMetaDev* h_meta = nullptr;
+  bool have_cand_params = false;             // osb_frontend_set_candidate_params
+  osb_candidate_params cand_params{};
   int32_t* d_assign = nullptr;   // [max_records][4]
   float* d_load_stage = nullptr;   // [FE_LOAD_ROWS][4096]: osb_frontend_db_load's fp32 -> fp16 staging, acquired by the first
                                    // load into an fp16 store
@@ -1118,8 +1279,9 @@ static void fe_tighten_bounds(osb_frontend* h) {
 
 // side: which store the host CHARGES for the batch (its bounds): 0 = unknown (both), 1 = all records are this drone's own,
 // 2 = all records are foreign.  The kernel always routes by drone_id.
+// metas: one osb_keyframe_meta per record (osb_frontend_ingest_meta; the tables must be acquired), or null
 static osb_status fe_ingest(osb_frontend* h, const osb_keyframe_record* recs, int n_records, int skip, cudaStream_t st,
-                            int side = 0) {
+                            int side = 0, const osb_keyframe_meta* metas = nullptr) {
   OSB_REQUIRE(n_records >= 0 && n_records <= h->max_records, "too many records in one ingest (max 64)");
   if (n_records == 0) return OSB_OK;
   DbStore &L = h->db[0], &R = h->db[1];
@@ -1145,8 +1307,12 @@ static osb_status fe_ingest(osb_frontend* h, const osb_keyframe_record* recs, in
   }
   fe_mark(h, 4, st);
   const FeStores dbs = fe_stores(h);
-  OSB_LAUNCH(fe_assign_kernel, 1, 32, 0, st, recs, n_records, skip, h->cfg.self_id, (long long)L.cap, dbs, h->d_assign,
-             h->fb_dev, h->ingest_seq + 1, h->charged + (long long)n_records * OSB_MAX_DIRS);
+  if (metas)
+    OSB_LAUNCH(fe_assign_kernel<true>, 1, 32, 0, st, recs, n_records, skip, h->cfg.self_id, (long long)L.cap, dbs, h->d_assign,
+               h->fb_dev, h->ingest_seq + 1, h->charged + (long long)n_records * OSB_MAX_DIRS, metas, h->meta);
+  else
+    OSB_LAUNCH(fe_assign_kernel<false>, 1, 32, 0, st, recs, n_records, skip, h->cfg.self_id, (long long)L.cap, dbs, h->d_assign,
+               h->fb_dev, h->ingest_seq + 1, h->charged + (long long)n_records * OSB_MAX_DIRS, nullptr, FeMeta{});
   OSB_CHECK_LAUNCH();
   ++h->ingest_seq;
   h->charged += (long long)n_records * OSB_MAX_DIRS;
@@ -1154,7 +1320,7 @@ static osb_status fe_ingest(osb_frontend* h, const osb_keyframe_record* recs, in
   OSB_CHECK_LAUNCH();
   L.upper += chg_l;
   R.upper += chg_r;
-  OSB_CUDA(cudaEventRecord(h->ev_ingest, st));
+  OSB_CUDA(record_event_capturable(h->ev_ingest, st));
   h->ingest_pending = true;
   fe_mark(h, 5, st);
   return OSB_OK;
@@ -1191,12 +1357,17 @@ static QueryParams fe_query_params(const osb_frontend* h) {
 // direction pairs (loop_detector.cpp:564-567; empty pairs produce n = 0) and, with the geometric filter,
 // loop_detector.cpp:569-598 (3-D-flag filter, homography RANSAC mask, reduceVector) -- each one launch for all records.
 // Record r's results go to res[r]; `m` holds OSB_MAX_DIRS * qp.n slots.
+// dev_init: the records' init_mode flags are the device bytes init_dev (or all 0 when null), not qp.init_mask
 static osb_status fe_rule_match(osb_frontend* h, const QueryParams& qp, const osb_keyframe_record* recs,
-                                osb_loop_result* res, const FeMatchScratch& m, cudaStream_t st) {
+                                osb_loop_result* res, const FeMatchScratch& m, cudaStream_t st, bool dev_init = false,
+                                const uint8_t* init_dev = nullptr) {
   const osb_frontend_config& c = h->cfg;
   const int slots = OSB_MAX_DIRS * qp.n;
   osb_status s;
-  OSB_LAUNCH(fe_query_rule_kernel, 1, 32 * cdiv(qp.n, 32), 0, st, qp, recs, fe_stores(h), res, m.pairs);
+  if (dev_init)
+    OSB_LAUNCH(fe_query_rule_kernel<true>, 1, 32 * cdiv(qp.n, 32), 0, st, qp, recs, fe_stores(h), res, m.pairs, init_dev);
+  else
+    OSB_LAUNCH(fe_query_rule_kernel<false>, 1, 32 * cdiv(qp.n, 32), 0, st, qp, recs, fe_stores(h), res, m.pairs, nullptr);
   OSB_CHECK_LAUNCH();
   s = bf_match_device(slots, c.max_num, OSB_MAX_KPTS, m.pairs.q, m.pairs.nq, m.pairs.t, m.pairs.nt, m.dist,
                       &res->match_new[0][0], &res->match_old[0][0], m.dout, &res->n_matches[0], nullptr, st, OSB_MAX_DIRS,
@@ -1271,7 +1442,8 @@ static osb_status fe_rq_alloc(osb_frontend* h, cudaStream_t st) {
 // only the local store, which the adds of received keyframes never change, so one pass over the local store answers all of
 // them as the reference's one-at-a-time add / query sequence would
 static osb_status fe_query_received(osb_frontend* h, const osb_keyframe_record* recs, int n, int skip,
-                                    unsigned long long init_mask, osb_loop_result* res, cudaStream_t st) {
+                                    unsigned long long init_mask, osb_loop_result* res, cudaStream_t st,
+                                    bool dev_init = false, const uint8_t* init_dev = nullptr) {
   const osb_frontend_config& c = h->cfg;
   DbStore& L = h->db[0];
   osb_status s;
@@ -1288,7 +1460,7 @@ static osb_status fe_query_received(osb_frontend* h, const osb_keyframe_record* 
   qp.init_mask = init_mask;
   qp.l_scores = h->d_rq_scores; qp.l_ids = h->d_rq_ids; qp.l_stride = FE_RQ_K;
   qp.received = 1; qp.skip = skip;
-  return fe_rule_match(h, qp, recs, res, h->rq, st);
+  return fe_rule_match(h, qp, recs, res, h->rq, st, dev_init, init_dev);
 }
 
 extern "C" osb_status osb_frontend_query_received(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records,
@@ -1337,20 +1509,19 @@ static osb_status fe_lc_alloc(osb_frontend* h) {
   return OSB_OK;
 }
 
-extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev,
-                                                const osb_loop_result* results_dev, int n, const osb_loop_candidate* cand,
-                                                osb_loop_edge_result* out_dev, void* stream) {
-  OSB_REQUIRE(h != nullptr, "null handle");
-  OSB_REQUIRE(n >= 1 && n <= LC_MAX, "n must be 1..64");
-  OSB_REQUIRE(records_dev && results_dev && cand && out_dev, "null argument");
-  std::lock_guard<std::mutex> lk(h->mu);
+// the handle's state compute_loop needs (under h->mu)
+static osb_status fe_compute_loop_ready(osb_frontend* h) {
   OSB_REQUIRE(h->have_loop_params, "no loop parameters: call osb_frontend_set_loop_params first");
   OSB_REQUIRE(h->cfg.geometric_filter != 0, "compute_loop needs geometric_filter = 1 (the reference's USE_FUNDMENTAL path)");
   OSB_REQUIRE(h->have_cameras != h->have_depth_camera,
               "compute_loop needs the old frame's camera: exactly one of set_cameras / set_depth_camera");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  OSB_TRY(fe_lc_alloc(h));
+  return fe_lc_alloc(h);
+}
+
+// assemble -> PnP-RANSAC -> finalise for n candidates read from `cands` (LoopCandBatch or LoopCandPtr)
+template <class Cands>
+static osb_status fe_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev, const osb_loop_result* results_dev,
+                                  int n, const Cands& cands, osb_loop_edge_result* out_dev, cudaStream_t st) {
   LoopCams cam{};
   const bool depth = h->have_depth_camera;
   for (int i = 0; i < 4; ++i) cam.K[i] = depth ? h->depth_K[i] : h->K[i];
@@ -1358,10 +1529,7 @@ extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyfr
     for (int i = 0; i < 7; ++i)       // the main camera's extrinsic is the direction's camera_extrinsic (loop_cam.cpp:372)
       cam.ext[d][i] = d < h->cfg.n_dirs ? (depth ? h->depth_ext[d][i] : h->main_down ? h->right_ext[d][i] : h->left_ext[d][i])
                                         : (i == 3 ? 1.0 : 0.0);
-  LoopCandBatch cb;
-  memset(&cb, 0, sizeof(cb));
-  memcpy(cb.c, cand, (size_t)n * sizeof(osb_loop_candidate));
-  OSB_LAUNCH(lc_assemble_kernel, n, 256, 0, st, records_dev, results_dev, fe_stores(h), cb, cam, h->loop_params,
+  OSB_LAUNCH(lc_assemble_kernel<Cands>, n, 256, 0, st, records_dev, results_dev, fe_stores(h), cands, cam, h->loop_params,
              h->cfg.query_dir, h->cfg.max_num, out_dev, h->d_lc_pts3d, h->d_lc_pts2d, h->d_lc_n, h->d_lc_params);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(pnp_ransac_kernel, n, PNP_THREADS, 0, st, h->d_lc_pts3d, h->d_lc_pts2d, h->d_lc_n, LC_MAXN, h->d_lc_params,
@@ -1369,6 +1537,59 @@ extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyfr
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(lc_finalise_kernel, n, 256, 0, st, h->d_lc_mask, h->d_lc_pnp, h->d_lc_params, out_dev);
   OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_compute_loop(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                                const osb_loop_result* results_dev, int n, const osb_loop_candidate* cand,
+                                                osb_loop_edge_result* out_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 1 && n <= LC_MAX, "n must be 1..64");
+  OSB_REQUIRE(records_dev && results_dev && cand && out_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(fe_compute_loop_ready(h));
+  DeviceGuard dg(h->device);
+  LoopCandBatch cb;
+  memset(&cb, 0, sizeof(cb));
+  memcpy(cb.c, cand, (size_t)n * sizeof(osb_loop_candidate));
+  return fe_compute_loop(h, records_dev, results_dev, n, cb, out_dev, (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_frontend_compute_loop_dev(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                                    const osb_loop_result* results_dev, int n,
+                                                    const osb_loop_candidate* cand_dev, osb_loop_edge_result* out_dev,
+                                                    void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 1 && n <= LC_MAX, "n must be 1..64");
+  OSB_REQUIRE(records_dev && results_dev && cand_dev && out_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_TRY(fe_compute_loop_ready(h));
+  DeviceGuard dg(h->device);
+  return fe_compute_loop(h, records_dev, results_dev, n, LoopCandPtr{cand_dev}, out_dev, (cudaStream_t)stream);
+}
+
+// loop_count and inter_drone_loop_count on the device, acquired zero by the first call that needs them
+static osb_status fe_lm_alloc(osb_frontend* h, cudaStream_t st) {
+  if (h->d_lm_count) return OSB_OK;
+  Resources& m = h->res;
+  OSB_TRY(m.alloc(&h->d_lm_count, 1));
+  OSB_TRY(m.alloc(&h->d_lm_pairs, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES));
+  OSB_TRY(m.event(&h->ev_lm, cudaEventDisableTiming));
+  OSB_CUDA(cudaMemsetAsync(h->d_lm_count, 0, sizeof(long long), st));
+  OSB_CUDA(cudaMemsetAsync(h->d_lm_pairs, 0, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES * sizeof(int32_t), st));
+  return OSB_OK;
+}
+
+// the rows of a round from `b` (LoopMeasBatch or LoopMeasPtr)
+template <class Meas>
+static osb_status fe_loop_measurements(osb_frontend* h, const osb_loop_result* results_dev, const osb_loop_edge_result* edges_dev,
+                                       int n, const Meas& b, double loop_cov_pos, double loop_cov_ang, osb_measurement* out_dev,
+                                       int32_t* count_dev, cudaStream_t st) {
+  OSB_TRY(fe_lm_alloc(h, st));
+  OSB_LAUNCH(lm_emit_kernel<Meas>, 1, 256, 0, st, results_dev, edges_dev, n, b, h->cfg.self_id, loop_cov_pos, loop_cov_ang,
+             out_dev, count_dev, h->d_lm_count, h->d_lm_pairs);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->ev_lm, st));
   return OSB_OK;
 }
 
@@ -1382,15 +1603,6 @@ extern "C" osb_status osb_frontend_loop_measurements(osb_frontend* h, const osb_
   OSB_REQUIRE(out_dev && count_dev && (n == 0 || (results_dev && edges_dev && cand && stamps)), "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!h->d_lm_count) {                                    // the first call acquires the counters, zero
-    Resources& m = h->res;
-    OSB_TRY(m.alloc(&h->d_lm_count, 1));
-    OSB_TRY(m.alloc(&h->d_lm_pairs, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES));
-    OSB_TRY(m.event(&h->ev_lm, cudaEventDisableTiming));
-    OSB_CUDA(cudaMemsetAsync(h->d_lm_count, 0, sizeof(long long), st));
-    OSB_CUDA(cudaMemsetAsync(h->d_lm_pairs, 0, (size_t)LM_PAIR_DRONES * LM_PAIR_DRONES * sizeof(int32_t), st));
-  }
   LoopMeasBatch b;
   memset(&b, 0, sizeof(b));
   for (int i = 0; i < n; ++i) {
@@ -1399,11 +1611,22 @@ extern "C" osb_status osb_frontend_loop_measurements(osb_frontend* h, const osb_
     b.stamp_query[i] = stamps[i].stamp_query_ns;
     b.stamp_hit[i] = stamps[i].stamp_hit_ns;
   }
-  OSB_LAUNCH(lm_emit_kernel, 1, 256, 0, st, results_dev, edges_dev, n, b, h->cfg.self_id, loop_cov_pos, loop_cov_ang,
-             out_dev, count_dev, h->d_lm_count, h->d_lm_pairs);
-  OSB_CHECK_LAUNCH();
-  OSB_CUDA(cudaEventRecord(h->ev_lm, st));
-  return OSB_OK;
+  return fe_loop_measurements(h, results_dev, edges_dev, n, b, loop_cov_pos, loop_cov_ang, out_dev, count_dev,
+                              (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_frontend_loop_measurements_dev(osb_frontend* h, const osb_loop_result* results_dev,
+                                                         const osb_loop_edge_result* edges_dev, int n,
+                                                         const osb_loop_candidate* cand_dev, const osb_loop_stamps* stamps_dev,
+                                                         double loop_cov_pos, double loop_cov_ang, osb_measurement* out_dev,
+                                                         int32_t* count_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 0 && n <= LC_MAX, "n must be 0..64");
+  OSB_REQUIRE(out_dev && count_dev && (n == 0 || (results_dev && edges_dev && cand_dev && stamps_dev)), "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  return fe_loop_measurements(h, results_dev, edges_dev, n, LoopMeasPtr{cand_dev, stamps_dev}, loop_cov_pos, loop_cov_ang,
+                              out_dev, count_dev, (cudaStream_t)stream);
 }
 
 extern "C" osb_status osb_frontend_loop_counts(osb_frontend* h, int64_t* loop_count, int32_t* pair_counts) {
@@ -1574,6 +1797,8 @@ extern "C" osb_status osb_frontend_db_reset(osb_frontend* h) {
     OSB_CUDA(cudaMemsetAsync(h->db[i].v.dev, 0, sizeof(DbDev), h->stream));
     OSB_CUDA(cudaMemsetAsync(h->db[i].v.top_ids, 0xFF, FE_KMAX * sizeof(int64_t), h->stream));
     h->db[i].upper = 0;
+    if (h->meta_ready)                                     // the frames' metas go; the trajectory stays
+      OSB_CUDA(cudaMemsetAsync(h->meta.ok[i], 0, (size_t)h->db[i].cap * sizeof(int32_t), h->stream));
   }
   h->fb_min_seq = h->ingest_seq + 1;
   OSB_CUDA(cudaStreamSynchronize(h->stream));
@@ -1655,5 +1880,125 @@ extern "C" osb_status osb_frontend_db_load(osb_frontend* h, int remote, int64_t 
   OSB_CUDA(cudaMemcpyAsync(v.dev, &hd, sizeof(DbDev), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   S.upper = hd.ntotal;
+  return OSB_OK;
+}
+
+// ---- keyframe metadata and a round's loop candidates on the device -----------------------------------------------------
+// both stores' meta tables and the trajectory, acquired zero by the first meta ingest (db_capacity frames / samples each)
+static osb_status fe_meta_alloc(osb_frontend* h, cudaStream_t st) {
+  if (h->meta_ready) return OSB_OK;
+  Resources& m = h->res;
+  FeMeta& mt = h->meta;
+  const size_t cap = (size_t)h->cfg.db_capacity;
+  for (int i = 0; i < 2; ++i) {
+    OSB_TRY(m.alloc(&mt.meta[i], cap));
+    OSB_TRY(m.alloc(&mt.ok[i], cap));
+    OSB_CUDA(cudaMemsetAsync(mt.ok[i], 0, cap * sizeof(int32_t), st));
+  }
+  OSB_TRY(m.alloc(&mt.t_stamp, cap));
+  OSB_TRY(m.alloc(&mt.t_pose, cap * 7));
+  OSB_TRY(m.alloc(&mt.t_len, cap));
+  OSB_TRY(m.alloc(&mt.dev, 1));
+  OSB_TRY(m.host_alloc(&h->h_meta, 1, cudaHostAllocDefault));
+  OSB_CUDA(cudaMemsetAsync(mt.dev, 0, sizeof(FeMetaDev), st));
+  mt.t_cap = (int)cap;
+  h->meta_ready = true;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_ingest_meta(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                               const osb_keyframe_meta* metas_dev, int n_records, int skip, void* stream) {
+  OSB_REQUIRE(h && records_dev && metas_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(fe_meta_alloc(h, (cudaStream_t)stream));
+  return fe_ingest(h, records_dev, n_records, skip, (cudaStream_t)stream, 0, metas_dev);
+}
+
+extern "C" osb_status osb_frontend_ingest_own_meta(osb_frontend* h, const osb_keyframe_record* record_dev,
+                                                   const osb_keyframe_meta* meta_dev, void* stream) {
+  OSB_REQUIRE(h && record_dev && meta_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(fe_meta_alloc(h, (cudaStream_t)stream));
+  return fe_ingest(h, record_dev, 1, -1, (cudaStream_t)stream, 1, meta_dev);
+}
+
+extern "C" osb_status osb_frontend_meta_status(osb_frontend* h, osb_status* last) {
+  OSB_REQUIRE(h && last, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *last = OSB_OK;
+  if (!h->meta_ready) return OSB_OK;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  if (h->ingest_pending) OSB_CUDA(cudaStreamWaitEvent(st, h->ev_ingest, 0));
+  OSB_CUDA(cudaMemcpyAsync(h->h_meta, h->meta.dev, sizeof(FeMetaDev), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  *last = (osb_status)h->h_meta->status;
+  return *last;
+}
+
+extern "C" osb_status osb_frontend_set_candidate_params(osb_frontend* h, const osb_candidate_params* p) {
+  OSB_REQUIRE(h && p, "null argument");
+  OSB_REQUIRE(p->pos_covariance_per_meter >= 0 && p->yaw_covariance_per_meter >= 0 && p->loop_cov_pos >= 0 &&
+              p->loop_cov_ang >= 0, "negative covariance");
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->cand_params = *p;
+  h->have_cand_params = true;
+  return OSB_OK;
+}
+
+static CandRule fe_cand_rule(const osb_frontend* h) {
+  const osb_candidate_params& p = h->cand_params;
+  return CandRule{h->cfg.self_id, p.inter_drone_init_frames, p.pos_covariance_per_meter, p.yaw_covariance_per_meter,
+                  p.loop_cov_pos, p.loop_cov_ang};
+}
+
+extern "C" osb_status osb_frontend_init_modes_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records,
+                                                  int skip, uint8_t* init_mode_out_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n_records >= 0 && n_records <= FE_MAX_RECORDS, "n_records must be 0..64");
+  OSB_REQUIRE(records_dev && init_mode_out_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->have_cand_params, "no candidate parameters: call osb_frontend_set_candidate_params first");
+  if (n_records == 0) return OSB_OK;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_TRY(fe_lm_alloc(h, st));
+  OSB_LAUNCH(fe_init_modes_kernel, 1, FE_MAX_RECORDS, 0, st, records_dev, n_records, skip, fe_cand_rule(h), h->d_lm_pairs,
+             init_mode_out_dev);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_query_received_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records,
+                                                      int skip, const uint8_t* init_mode_dev, osb_loop_result* results_dev,
+                                                      void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n_records >= 0 && n_records <= FE_MAX_RECORDS, "n_records must be 0..64");
+  if (n_records == 0) return OSB_OK;
+  OSB_REQUIRE(records_dev && results_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  return fe_query_received(h, records_dev, n_records, skip, 0ull, results_dev, (cudaStream_t)stream, true, init_mode_dev);
+}
+
+extern "C" osb_status osb_frontend_loop_candidates_dev(osb_frontend* h, const osb_keyframe_record* records_dev,
+                                                       const osb_keyframe_meta* metas_dev, const osb_loop_result* results_dev,
+                                                       int n, const uint8_t* init_mode_dev, osb_loop_candidate* cand_out_dev,
+                                                       osb_loop_stamps* stamps_out_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n >= 0 && n <= LC_MAX, "n must be 0..64");
+  OSB_REQUIRE(n == 0 || (records_dev && metas_dev && results_dev && cand_out_dev && stamps_out_dev), "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->have_cand_params, "no candidate parameters: call osb_frontend_set_candidate_params first");
+  if (n == 0) return OSB_OK;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_TRY(fe_meta_alloc(h, st));                           // a handle without meta ingests: every hit lacks its meta
+  OSB_TRY(fe_lm_alloc(h, st));
+  OSB_LAUNCH(lc_candidates_kernel, 1, LC_MAX, 0, st, records_dev, metas_dev, results_dev, n, init_mode_dev, fe_stores(h),
+             h->meta, h->d_lm_pairs, fe_cand_rule(h), cand_out_dev, stamps_out_dev);
+  OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

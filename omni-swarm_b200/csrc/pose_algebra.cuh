@@ -120,4 +120,16 @@ __device__ __forceinline__ PoseD delta_pose4(const PoseD& a, const PoseD& b) {
   return o;
 }
 
+// DroneTrajectory look-up: the sample nearest to t, ties to the earlier one, clamped to the first / last sample
+__device__ __forceinline__ int nearest_sample(const int64_t* __restrict__ s, int n, int64_t t) {
+  int lo = 0, hi = n;                                              // first k with s[k] >= t
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (s[mid] < t) lo = mid + 1; else hi = mid;
+  }
+  if (lo == 0) return 0;
+  if (lo == n) return n - 1;
+  return (t - s[lo - 1]) <= (s[lo] - t) ? lo - 1 : lo;
+}
+
 }  // namespace osb

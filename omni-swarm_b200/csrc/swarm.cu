@@ -209,13 +209,14 @@ extern "C" osb_status osb_swarm_init(osb_swarm** out, const uint8_t* id, int ran
   return OSB_OK;
 }
 
-static osb_status swarm_gather(osb_swarm* h, const osb_keyframe_record* rec, osb_keyframe_record* gathered, cudaStream_t st) {
+// `bytes` of every rank's src -> gathered[world * bytes] in rank order on st
+static osb_status swarm_gather(osb_swarm* h, const void* src, void* gathered, size_t bytes, cudaStream_t st) {
   if (h->world == 1) {
-    if (gathered != rec) OSB_CUDA(cudaMemcpyAsync(gathered, rec, sizeof(osb_keyframe_record), cudaMemcpyDeviceToDevice, st));
+    if (gathered != src) OSB_CUDA(cudaMemcpyAsync(gathered, src, bytes, cudaMemcpyDeviceToDevice, st));
     return OSB_OK;
   }
   NcclApi* api = nccl_api();
-  OSB_NCCL(api, api->AllGather(rec, gathered, sizeof(osb_keyframe_record), ncclUint8, h->comm, st));
+  OSB_NCCL(api, api->AllGather(src, gathered, bytes, ncclUint8, h->comm, st));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return OSB_OK;
 }
@@ -225,7 +226,15 @@ extern "C" osb_status osb_swarm_exchange(osb_swarm* h, const osb_keyframe_record
   OSB_REQUIRE(h && record_dev && gathered_dev, "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  return swarm_gather(h, record_dev, gathered_dev, (cudaStream_t)stream);
+  return swarm_gather(h, record_dev, gathered_dev, sizeof(osb_keyframe_record), (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_swarm_exchange_meta(osb_swarm* h, const osb_keyframe_meta* meta_dev, osb_keyframe_meta* gathered_dev,
+                                              void* stream) {
+  OSB_REQUIRE(h && meta_dev && gathered_dev, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  return swarm_gather(h, meta_dev, gathered_dev, sizeof(osb_keyframe_meta), (cudaStream_t)stream);
 }
 
 extern "C" osb_status osb_swarm_exchange_async(osb_swarm* h, const osb_keyframe_record* record_dev,
@@ -257,7 +266,7 @@ extern "C" osb_status osb_swarm_exchange_async(osb_swarm* h, const osb_keyframe_
     h->in_flight = true;
     return OSB_OK;
   }
-  osb_status s = swarm_gather(h, record_dev, gathered_dev, h->side);
+  osb_status s = swarm_gather(h, record_dev, gathered_dev, sizeof(osb_keyframe_record), h->side);
   if (s != OSB_OK) return s;
   OSB_CUDA(cudaEventRecord(h->ev_done, h->side));
   h->in_flight = true;

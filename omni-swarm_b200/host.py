@@ -539,6 +539,74 @@ class KeyframeFrontend(_Handle):
         _l.check(self._lib.osb_frontend_loop_counts(self._h, C.byref(n), _l.ptr(pairs)))
         return n.value, pairs
 
+    # ---- keyframe metadata and a round's loop candidates on the device ------------------------------------------
+    @staticmethod
+    def keyframe_metas(metas):
+        """list of (drone_id, msg_id, stamp_ns, pose_drone [7]) -> KeyframeMeta array (upload its bytes beside the records)"""
+        arr = (_l.KeyframeMeta * len(metas))()
+        for a, (drone, msg, stamp, pose) in zip(arr, metas):
+            a.drone_id, a.msg_id, a.stamp_ns = int(drone), int(msg), int(stamp)
+            a.pose_drone[:] = [float(x) for x in pose]
+        return arr
+
+    def ingest_meta(self, records_dev: int, metas_dev: int, n_records: int, skip: int, stream: int):
+        """ingest, and each record's osb_keyframe_meta (metas_dev [n_records]) into the frame slot it takes"""
+        _l.check(self._lib.osb_frontend_ingest_meta(self._h, C.c_void_p(records_dev), C.c_void_p(metas_dev), n_records, skip,
+                                                    C.c_void_p(stream)))
+
+    def ingest_own_meta(self, record_dev: int, meta_dev: int, stream: int):
+        """ingest_own with the keyframe's meta; it also extends the ego-motion trajectory"""
+        _l.check(self._lib.osb_frontend_ingest_own_meta(self._h, C.c_void_p(record_dev), C.c_void_p(meta_dev),
+                                                        C.c_void_p(stream)))
+
+    def meta_status(self) -> int:
+        """waits for the last ingest -> the status of the last meta ingest (lib.OK, lib.ERR_INVALID, lib.ERR_CAPACITY)"""
+        st = C.c_int(0)
+        self._lib.osb_frontend_meta_status(self._h, C.byref(st))
+        return st.value
+
+    def set_candidate_params(self, inter_drone_init_frames=50, pos_covariance_per_meter=0.01, yaw_covariance_per_meter=0.003,
+                             loop_cov_pos=0.013, loop_cov_ang=2.5e-4):
+        """the constants of the device-built candidates (swarm_loop.cpp:227-256 defaults)"""
+        p = _l.CandidateParams(inter_drone_init_frames=inter_drone_init_frames,
+                               pos_covariance_per_meter=pos_covariance_per_meter,
+                               yaw_covariance_per_meter=yaw_covariance_per_meter, loop_cov_pos=loop_cov_pos,
+                               loop_cov_ang=loop_cov_ang)
+        _l.check(self._lib.osb_frontend_set_candidate_params(self._h, C.byref(p)))
+
+    def init_modes_dev(self, records_dev: int, n_records: int, skip: int, out_dev: int, stream: int):
+        """init_mode bytes [n_records] of a received round from the device's inter_drone_loop_count"""
+        _l.check(self._lib.osb_frontend_init_modes_dev(self._h, C.c_void_p(records_dev), n_records, skip, C.c_void_p(out_dev),
+                                                       C.c_void_p(stream)))
+
+    def query_received_dev(self, records_dev: int, n_records: int, skip: int, init_mode_dev, results_dev: int, stream: int):
+        """query_received with init_mode a device byte array [n_records] (or None: all 0)"""
+        _l.check(self._lib.osb_frontend_query_received_dev(self._h, C.c_void_p(records_dev), n_records, skip,
+                                                           None if init_mode_dev is None else C.c_void_p(init_mode_dev),
+                                                           C.c_void_p(results_dev), C.c_void_p(stream)))
+
+    def loop_candidates_dev(self, records_dev: int, metas_dev: int, results_dev: int, n: int, init_mode_dev,
+                            cand_out_dev: int, stamps_out_dev: int, stream: int):
+        """LoopCandidate [n] and LoopStamps [n] of a round's results, built on the device (osb_frontend_loop_candidates_dev)"""
+        _l.check(self._lib.osb_frontend_loop_candidates_dev(self._h, C.c_void_p(records_dev), C.c_void_p(metas_dev),
+                                                            C.c_void_p(results_dev), n,
+                                                            None if init_mode_dev is None else C.c_void_p(init_mode_dev),
+                                                            C.c_void_p(cand_out_dev), C.c_void_p(stamps_out_dev),
+                                                            C.c_void_p(stream)))
+
+    def compute_loop_dev(self, records_dev: int, results_dev: int, n: int, cand_dev: int, out_dev: int, stream: int):
+        """compute_loop with the candidates read from the device array cand_dev [n]"""
+        _l.check(self._lib.osb_frontend_compute_loop_dev(self._h, C.c_void_p(records_dev), C.c_void_p(results_dev), n,
+                                                         C.c_void_p(cand_dev), C.c_void_p(out_dev), C.c_void_p(stream)))
+
+    def loop_measurements_dev(self, results_dev: int, edges_dev: int, n: int, cand_dev: int, stamps_dev: int,
+                              loop_cov_pos: float, loop_cov_ang: float, out_dev: int, count_dev: int, stream: int):
+        """loop_measurements with the candidates and stamps read from device arrays [n]"""
+        _l.check(self._lib.osb_frontend_loop_measurements_dev(self._h, C.c_void_p(results_dev), C.c_void_p(edges_dev), n,
+                                                              C.c_void_p(cand_dev), C.c_void_p(stamps_dev),
+                                                              float(loop_cov_pos), float(loop_cov_ang), C.c_void_p(out_dev),
+                                                              C.c_void_p(count_dev), C.c_void_p(stream)))
+
     def finish(self, stream: int):
         _l.check(self._lib.osb_frontend_finish(self._h, C.c_void_p(stream)))
 
@@ -1052,6 +1120,10 @@ class Swarm(_Handle):
     def wait(self, stream: int):
         """`stream` waits for the last exchange_async (osb_swarm_wait)"""
         _l.check(self._lib.osb_swarm_wait(self._h, C.c_void_p(stream)))
+
+    def exchange_meta(self, meta_dev: int, gathered_dev: int, stream: int):
+        """this drone's KeyframeMeta -> gathered_dev [world] in rank order (osb_swarm_exchange_meta)"""
+        _l.check(self._lib.osb_swarm_exchange_meta(self._h, C.c_void_p(meta_dev), C.c_void_p(gathered_dev), C.c_void_p(stream)))
 
 
 def conv_layer_parity(w, bias, in_hi, in_lo, act_scale: float, *, w_scale: float = 1024.0, relu: int = 0, pool: int = 0,

@@ -152,6 +152,20 @@ class LoopStamps(C.Structure):
 LOOP_PAIR_DRONES = 256         # inter_drone_loop_count is kept for drone ids 0..255 (osb_frontend_loop_counts)
 
 
+class KeyframeMeta(C.Structure):
+    _fields_ = [("drone_id", C.c_int32), ("msg_id", C.c_int32), ("stamp_ns", C.c_int64), ("pose_drone", C.c_double * 7)]
+
+
+class CandidateParams(C.Structure):
+    _fields_ = [("inter_drone_init_frames", C.c_int32), ("reserved", C.c_int32), ("pos_covariance_per_meter", C.c_double),
+                ("yaw_covariance_per_meter", C.c_double), ("loop_cov_pos", C.c_double), ("loop_cov_ang", C.c_double)]
+
+
+META_BYTES = C.sizeof(KeyframeMeta)
+CANDIDATE_BYTES = C.sizeof(LoopCandidate)
+STAMPS_BYTES = C.sizeof(LoopStamps)
+
+
 class FrontendConfig(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_dirs", C.c_int32), ("max_num", C.c_int32),
                 ("sp_thres", C.c_float), ("self_id", C.c_int32), ("db_capacity", C.c_int32),
@@ -256,6 +270,15 @@ _SIG = {
     "osb_frontend_compute_loop": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
     "osb_frontend_loop_measurements": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P]),
     "osb_frontend_loop_counts": (C.c_int, [_P, C.POINTER(C.c_int64), _P]),
+    "osb_frontend_ingest_meta": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P]),
+    "osb_frontend_ingest_own_meta": (C.c_int, [_P, _P, _P, _P]),
+    "osb_frontend_meta_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
+    "osb_frontend_set_candidate_params": (C.c_int, [_P, C.POINTER(CandidateParams)]),
+    "osb_frontend_init_modes_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
+    "osb_frontend_query_received_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "osb_frontend_loop_candidates_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
+    "osb_frontend_compute_loop_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
+    "osb_frontend_loop_measurements_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P]),
     "osb_frontend_process": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P]),
     "osb_frontend_finish": (C.c_int, [_P, _P]),
     "osb_frontend_set_profiling": (C.c_int, [_P, C.c_int]),
@@ -306,6 +329,7 @@ _SIG = {
     "osb_swarm_exchange": (C.c_int, [_P, _P, _P, _P]),
     "osb_swarm_exchange_async": (C.c_int, [_P, _P, _P, _P]),
     "osb_swarm_wait": (C.c_int, [_P, _P]),
+    "osb_swarm_exchange_meta": (C.c_int, [_P, _P, _P, _P]),
     "osb_swarm_rank": (C.c_int, [_P]),
     "osb_swarm_transport": (C.c_int, [_P]),
     "osb_swarm_world": (C.c_int, [_P]),

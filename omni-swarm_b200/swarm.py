@@ -29,6 +29,20 @@ def exchange_records(record: torch.Tensor, gathered: torch.Tensor | None = None,
     return gathered
 
 
+def exchange_metas(meta: torch.Tensor, gathered: torch.Tensor | None = None, group=None) -> torch.Tensor:
+    """meta: uint8 tensor [META_BYTES] (this rank's osb_keyframe_meta, the one beside its record) -> uint8 tensor
+    [world * META_BYTES] in rank order, so that gathered metas and records share their index."""
+    assert meta.dtype == torch.uint8 and meta.numel() == _l.META_BYTES
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    if gathered is None:
+        gathered = torch.empty(world * _l.META_BYTES, dtype=torch.uint8, device=meta.device)
+    if world == 1:
+        gathered.copy_(meta)
+        return gathered
+    dist.all_gather_into_tensor(gathered, meta, group=group)
+    return gathered
+
+
 def record_view(gathered: torch.Tensor, rank: int) -> torch.Tensor:
     return gathered[rank * _l.RECORD_BYTES:(rank + 1) * _l.RECORD_BYTES]
 
