@@ -273,15 +273,6 @@ anchor_compact_kernel(const osb_anchor_result* __restrict__ rows, int n, const u
   if (threadIdx.x == 0) *count = out_base;
 }
 
-// Row-count feedback of the device append, written into mapped pinned host memory as the front-end's FeFeedback is: the last
-// append that has run reports the true counts, its status and how much had been charged to the host's bound when it was
-// enqueued, so bound = count + what was charged since.  seq_begin / seq_end make a torn read detectable.
-struct AnchorFeedback {
-  volatile long long seq_begin;
-  volatile long long n_loops, n_dets, charged, status;
-  volatile long long seq_end;
-};
-
 // add_new_loop_connection / add_new_detection for rows [0, *count) of a device buffer (solver.cpp:558-588): one CTA.
 // Pass 1 validates every row and counts what the distance gate keeps; a refused call writes nothing but the feedback.
 // Pass 2 appends tile by tile: a block scan of (kept loop, kept detection) per thread gives each row its arrival slot and
@@ -319,7 +310,7 @@ __device__ __forceinline__ bool append_keeps(const osb_measurement& r, float thr
 __global__ void __launch_bounds__(APPEND_THREADS)
 anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __restrict__ count_dev, int max_n, float thres,
                      int max_drones, int max_meas, osb_measurement* __restrict__ meas, int32_t* __restrict__ loop_slot,
-                     int32_t* __restrict__ det_slot, int32_t* __restrict__ counts, AnchorFeedback* __restrict__ fb,
+                     int32_t* __restrict__ det_slot, int32_t* __restrict__ counts, CountRecord* __restrict__ fb,
                      long long seq, long long charged) {
   __shared__ int s_bad;
   const int tid = threadIdx.x;
@@ -365,14 +356,7 @@ anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __res
     }
   if (tid != 0) return;
   if (status == OSB_OK) { counts[0] = have_l + nl; counts[1] = have_d + nd; }
-  fb->seq_begin = seq;
-  __threadfence_system();
-  fb->n_loops = status == OSB_OK ? have_l + nl : have_l;
-  fb->n_dets = status == OSB_OK ? have_d + nd : have_d;
-  fb->charged = charged;
-  fb->status = status;
-  __threadfence_system();
-  fb->seq_end = seq;
+  fb->publish(seq, status == OSB_OK ? have_l + nl : have_l, status == OSB_OK ? have_d + nd : have_d, status, charged);
 }
 
 }  // namespace osb
@@ -402,16 +386,11 @@ struct osb_anchor {
   int32_t *d_win_frame = nullptr, *d_win_block = nullptr;
   double* d_win_pose = nullptr;
   osb_anchor_result* d_out = nullptr;
-  // device appends (osb_anchor_add_measurements_dev), acquired by the first one: the counts on the device, their feedback
-  // (mapped pinned memory + its device alias) and an event recorded after every append
+  // device appends (osb_anchor_add_measurements_dev), acquired by the first one: the counts on the device and their feedback
+  // (each append charges its max_n and publishes the loop and detection counts and its status)
   int32_t* d_counts = nullptr;                    // [2] loops, detections
-  AnchorFeedback* fb_host = nullptr;
-  AnchorFeedback* fb_dev = nullptr;
-  cudaEvent_t last_append = nullptr;
-  bool append_pending = false;                    // an append may not have run: n_loops / n_dets are stale, `upper` bounds them
-  long long append_seq = 0, fb_min_seq = 1;       // feedback older than fb_min_seq carries nothing new
-  long long charged = 0;                          // max_n summed over every device append
-  long long upper = 0;                            // bound of n_loops + n_dets while append_pending
+  CountFeedback fb;                               // fb.pending: an append may not have run, n_loops / n_dets are stale
+  long long upper = 0;                            // bound of n_loops + n_dets while fb.pending
   osb_status last_status = OSB_OK;                // the last device append's, once synchronised
   // host record
   int n_loops = 0, n_dets = 0;
@@ -437,28 +416,16 @@ bool drone_ok(const osb_anchor* h, int32_t d) { return d >= 0 && d < h->p.max_dr
 
 // wait for the last device append and take its exact counts and status (every synchronising call starts with this)
 osb_status anchor_settle(osb_anchor* h) {
-  if (!h->append_pending) return OSB_OK;
-  OSB_CUDA(cudaEventSynchronize(h->last_append));
-  const AnchorFeedback* fb = h->fb_host;
-  h->n_loops = (int)fb->n_loops;
-  h->n_dets = (int)fb->n_dets;
-  h->last_status = (osb_status)fb->status;
+  if (!h->fb.pending) return OSB_OK;
+  OSB_CUDA(cudaEventSynchronize(h->fb.ev));
+  const CountRecord* r = h->fb.host;
+  h->n_loops = (int)r->count[0];
+  h->n_dets = (int)r->count[1];
+  h->last_status = (osb_status)r->status;
   h->upper = h->n_loops + h->n_dets;
-  h->append_pending = false;
-  h->fb_min_seq = h->append_seq + 1;
+  h->fb.pending = false;
+  h->fb.exact();
   return OSB_OK;
-}
-
-// lower the bound with what the most recent append that has RUN reported (no synchronisation)
-void anchor_tighten(osb_anchor* h) {
-  const AnchorFeedback* fb = h->fb_host;
-  const long long e = fb->seq_end;
-  std::atomic_thread_fence(std::memory_order_acquire);
-  const long long nl = fb->n_loops, nd = fb->n_dets, ch = fb->charged;
-  std::atomic_thread_fence(std::memory_order_acquire);
-  const long long b = fb->seq_begin;
-  if (b != e || e < h->fb_min_seq) return;
-  h->upper = std::min(h->upper, nl + nd + (h->charged - ch));
 }
 
 }  // namespace
@@ -701,9 +668,10 @@ osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_ancho
     if (yaw_observable[d]) v.yaw_obs[d >> 6] |= 1ull << (d & 63);
   v.counts = nullptr;
   v.n_bound = v.n_total;
-  if (h->append_pending) {                      // the counts are the device's; the grid covers the host's bound of them
-    anchor_tighten(h);
-    OSB_CUDA(cudaStreamWaitEvent(st, h->last_append, 0));
+  if (h->fb.pending) {                          // the counts are the device's; the grid covers the host's bound of them
+    long long n[2], since;                      // lowered by what the last append that has RUN reported
+    if (h->fb.read(n, &since)) h->upper = std::min(h->upper, n[0] + n[1] + since);
+    OSB_CUDA(cudaStreamWaitEvent(st, h->fb.ev, 0));
     v.counts = h->d_counts;
     v.n_bound = (int)h->upper;
   }
@@ -752,15 +720,11 @@ extern "C" osb_status osb_anchor_run(osb_anchor* h, const uint8_t* yaw_observabl
 
 namespace {
 
-// the first device append acquires the device counts (seeded with the host's exact ones), the feedback and the event
+// the first device append acquires the device counts (seeded with the host's exact ones) and the feedback
 osb_status anchor_dev_init(osb_anchor* h) {
   if (h->d_counts) return OSB_OK;
-  Resources& R = h->res;
-  OSB_TRY(R.alloc(&h->d_counts, 2));
-  OSB_TRY(R.host_alloc(&h->fb_host, 1, cudaHostAllocMapped));
-  memset((void*)h->fb_host, 0, sizeof(AnchorFeedback));
-  OSB_CUDA(cudaHostGetDevicePointer((void**)&h->fb_dev, (void*)h->fb_host, 0));
-  OSB_TRY(R.event(&h->last_append, cudaEventDisableTiming));
+  OSB_TRY(h->res.alloc(&h->d_counts, 2));
+  OSB_TRY(h->fb.init(h->res));
   const int32_t counts[2] = {h->n_loops, h->n_dets};
   OSB_CUDA(cudaMemcpyAsync(h->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
@@ -779,22 +743,20 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
   OSB_TRY(anchor_dev_init(h));
   // the append rewrites the counts a run reads and follows the previous append, whichever streams those ran on
   OSB_CUDA(wait_event_capturable(st, h->last_run));
-  if (h->append_pending) {
-    OSB_CUDA(wait_event_capturable(st, h->last_append));
-    anchor_tighten(h);
+  if (h->fb.pending) {
+    OSB_CUDA(wait_event_capturable(st, h->fb.ev));
+    long long n[2], since;
+    if (h->fb.read(n, &since)) h->upper = std::min(h->upper, n[0] + n[1] + since);
   } else {
     h->upper = h->n_loops + h->n_dets;
   }
-  const long long seq = h->append_seq + 1, charged = h->charged + max_n;
+  const long long seq = h->fb.charge(max_n);
   OSB_LAUNCH(anchor_append_kernel, 1, APPEND_THREADS, 0, st, m_dev, count_dev, max_n, loop_outlier_distance_threshold,
-             h->p.max_drones, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb_dev, seq,
-             charged);
+             h->p.max_drones, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb.dev, seq,
+             h->fb.charged);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_append, st));
-  h->append_seq = seq;
-  h->charged = charged;
+  OSB_CUDA(h->fb.record(st));
   h->upper = std::min<long long>(h->upper + max_n, h->p.max_measurements);
-  h->append_pending = true;
   return OSB_OK;
 }
 

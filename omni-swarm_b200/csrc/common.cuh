@@ -225,6 +225,66 @@ class Resources {
   }
 };
 
+// Host upper bound of row counts that live on the device, kept tight without a synchronisation.  The host charges every
+// launch that may add rows with what it may add; the kernel publishes the true counts into mapped pinned memory, tagged with
+// what had been charged when it was enqueued, so the last record that has landed gives bound = count + what was charged
+// since.  seq_begin / seq_end make a torn read detectable, and a record older than min_seq (from before the counts were
+// last made exact on the host) carries nothing new.
+struct CountRecord {
+  volatile long long seq_begin;
+  volatile long long count[2];
+  volatile long long status;
+  volatile long long charged;
+  volatile long long seq_end;
+  // one thread, after the kernel's last write of the counts
+  __device__ __forceinline__ void publish(long long seq, long long n0, long long n1, long long st, long long ch) {
+    seq_begin = seq;
+    __threadfence_system();
+    count[0] = n0; count[1] = n1; status = st; charged = ch;
+    __threadfence_system();
+    seq_end = seq;
+  }
+};
+struct CountFeedback {
+  CountRecord* host = nullptr;                    // mapped pinned memory
+  CountRecord* dev = nullptr;                     // its device alias, what the publishing kernel gets
+  cudaEvent_t ev = nullptr;                       // recorded after the last publishing launch, on ITS stream
+  bool pending = false;                           // that launch may not have run
+  long long seq = 0, min_seq = 1;
+  long long charged = 0;                          // summed over every publishing launch
+
+  osb_status init(Resources& R) {
+    OSB_TRY(R.host_alloc(&host, 1, cudaHostAllocMapped));
+    memset((void*)host, 0, sizeof(CountRecord));
+    OSB_CUDA(cudaHostGetDevicePointer((void**)&dev, (void*)host, 0));
+    return R.event(&ev, cudaEventDisableTiming);
+  }
+  // charges the next publishing launch with n rows -> the sequence number it publishes (with `charged`)
+  long long charge(long long n) {
+    charged += n;
+    return ++seq;
+  }
+  // after the publishing launch and whatever else the waits on `ev` must cover
+  cudaError_t record(cudaStream_t st) {
+    const cudaError_t e = record_event_capturable(ev, st);
+    if (e == cudaSuccess) pending = true;
+    return e;
+  }
+  // the last record that has landed: false when it is torn or older than min_seq
+  bool read(long long n[2], long long* since) const {
+    const long long e = host->seq_end;
+    std::atomic_thread_fence(std::memory_order_acquire);
+    n[0] = host->count[0]; n[1] = host->count[1];
+    const long long ch = host->charged;
+    std::atomic_thread_fence(std::memory_order_acquire);
+    const long long b = host->seq_begin;
+    *since = charged - ch;
+    return b == e && e >= min_seq;
+  }
+  // the host's counts are exact now: no record already enqueued carries anything new
+  void exact() { min_seq = seq + 1; }
+};
+
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -15,23 +15,12 @@
 // swarm_loop/src/tensorrt_generic.cpp:73).
 #include "superpoint.cuh"
 #include "pose_algebra.cuh"
-#include <atomic>
 
 namespace osb {
 
 struct DbDev {                 // device-resident counters of a database (one for own keyframes, one for remote ones)
   int64_t ntotal;              // rows (faiss ntotal)
   int nframes;
-};
-
-// Row-count feedback of the ingest kernel, written into mapped pinned host memory (no copy, no synchronisation): the host's
-// bounds are conservative (every ingested record is charged to BOTH stores because its drone_id is only known on the
-// device); the last ingest that has actually run reports the true counts together with how much had been charged when it
-// was enqueued, so bound = count + what was charged since.  seq_begin / seq_end make a torn read detectable.
-struct FeFeedback {
-  volatile long long seq_begin;
-  volatile long long n_local, n_remote, charged;
-  volatile long long seq_end;
 };
 
 // what the kernels see of one database
@@ -224,7 +213,7 @@ template <bool META>
 __global__ void fe_assign_kernel(const osb_keyframe_record* __restrict__ recs, int n_records, int skip, int self_id,
                                  long long cap, const __grid_constant__ FeStores dbs,
                                  int32_t* __restrict__ assign /*[n_records][4]: row | (remote<<30), or -1*/,
-                                 FeFeedback* __restrict__ fb, long long seq, long long charged,
+                                 CountRecord* __restrict__ fb, long long seq, long long charged,
                                  const osb_keyframe_meta* __restrict__ metas, FeMeta mt) {
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
   int meta_status = OSB_OK;
@@ -252,11 +241,7 @@ __global__ void fe_assign_kernel(const osb_keyframe_record* __restrict__ recs, i
     *db.dev = cnt;
   }
   if constexpr (META) mt.dev->status = meta_status;
-  fb->seq_begin = seq;
-  __threadfence_system();
-  fb->n_local = dbs.db[0].dev->ntotal; fb->n_remote = dbs.db[1].dev->ntotal; fb->charged = charged;
-  __threadfence_system();
-  fb->seq_end = seq;
+  fb->publish(seq, dbs.db[0].dev->ntotal, dbs.db[1].dev->ntotal, 0, charged);
 }
 
 // phase 2: copy global + local descriptors of every assigned (record, direction) into its row
@@ -938,12 +923,9 @@ struct osb_frontend {
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   DbDev* h_cnt = nullptr;                         // pinned [2]: row counters read back without blocking the driver (a copy
                                                   // to pageable memory would hold other host threads' launches until it ran)
-  FeFeedback* fb_host = nullptr;                  // mapped pinned memory + its device alias
-  FeFeedback* fb_dev = nullptr;
-  long long ingest_seq = 0, fb_min_seq = 1;       // feedback older than fb_min_seq predates a load / reset and is ignored
-  long long charged = 0;                          // rows charged to each store by ingests so far
-  cudaEvent_t ev_ingest = nullptr;                // recorded after the last ingest on ITS stream
-  bool ingest_pending = false;
+  // the stores' row counts as the ingests report them: every ingest charges the most rows it could give ONE store (a
+  // record's drone_id, and so its store, is only known on the device) and publishes both ntotal
+  CountFeedback fb;
   bool profiling = false;
   cudaEvent_t ev[9] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool ev_valid[9] = {false, false, false, false, false, false, false, false, false};
@@ -1023,11 +1005,8 @@ extern "C" osb_status osb_frontend_create(osb_frontend** out, const osb_frontend
   OSB_TRY(m.stream(&h->stream2));
   OSB_TRY(m.event(&h->ev_fork, cudaEventDisableTiming));
   OSB_TRY(m.event(&h->ev_join, cudaEventDisableTiming));
-  OSB_TRY(m.event(&h->ev_ingest, cudaEventDisableTiming));
   OSB_TRY(m.host_alloc(&h->h_cnt, 2, cudaHostAllocDefault));
-  OSB_TRY(m.host_alloc(&h->fb_host, 1, cudaHostAllocMapped));
-  memset((void*)h->fb_host, 0, sizeof(FeFeedback));
-  OSB_CUDA(cudaHostGetDevicePointer((void**)&h->fb_dev, (void*)h->fb_host, 0));
+  OSB_TRY(h->fb.init(m));
   OSB_TRY(h->sp.init(sp_weights, n_sp_weights, cfg->width, cfg->height, cfg->sp_thres, mn, pca_comp, pca_mean, 2 * nd));
   h->sp.ks.write_surv = false;       // the survivor plane is only a parity hook of the standalone SuperPoint handle
   if (cfg->zero_bottom_quarter) OSB_TRY(h->sp.band_init());
@@ -1263,20 +1242,6 @@ extern "C" osb_status osb_frontend_extract_depth_dev(osb_frontend* h, const uint
 
 static osb_status fe_refresh_counts(osb_frontend* h, cudaStream_t st);
 
-// lower the host bounds with what the most recent EXECUTED ingest reported (no synchronisation; see FeFeedback)
-static void fe_tighten_bounds(osb_frontend* h) {
-  const FeFeedback* fb = h->fb_host;
-  const long long e = fb->seq_end;
-  std::atomic_thread_fence(std::memory_order_acquire);
-  const long long nl = fb->n_local, nr = fb->n_remote, ch = fb->charged;
-  std::atomic_thread_fence(std::memory_order_acquire);
-  const long long b = fb->seq_begin;
-  if (b != e || e < h->fb_min_seq) return;
-  const long long since = h->charged - ch;
-  h->db[0].upper = std::min<int64_t>(h->db[0].upper, nl + since);
-  h->db[1].upper = std::min<int64_t>(h->db[1].upper, nr + since);
-}
-
 // side: which store the host CHARGES for the batch (its bounds): 0 = unknown (both), 1 = all records are this drone's own,
 // 2 = all records are foreign.  The kernel always routes by drone_id.
 // metas: one osb_keyframe_meta per record (osb_frontend_ingest_meta; the tables must be acquired), or null
@@ -1285,7 +1250,9 @@ static osb_status fe_ingest(osb_frontend* h, const osb_keyframe_record* recs, in
   OSB_REQUIRE(n_records >= 0 && n_records <= h->max_records, "too many records in one ingest (max 64)");
   if (n_records == 0) return OSB_OK;
   DbStore &L = h->db[0], &R = h->db[1];
-  fe_tighten_bounds(h);
+  long long n[2], since;                        // lower the bounds with what the last ingest that has RUN reported
+  if (h->fb.read(n, &since))
+    for (int i = 0; i < 2; ++i) h->db[i].upper = std::min<int64_t>(h->db[i].upper, n[i] + since);
   const int64_t chg_l = side == 2 ? 0 : (int64_t)n_records * OSB_MAX_DIRS, chg_r = side == 1 ? 0 : (int64_t)n_records * OSB_MAX_DIRS;
   if (L.upper + chg_l > L.cap || R.upper + chg_r > R.cap) {
     // the upper bounds are conservative (every record charged to both databases): make them exact, and count which
@@ -1307,21 +1274,19 @@ static osb_status fe_ingest(osb_frontend* h, const osb_keyframe_record* recs, in
   }
   fe_mark(h, 4, st);
   const FeStores dbs = fe_stores(h);
+  const long long seq = h->fb.charge((long long)n_records * OSB_MAX_DIRS);
   if (metas)
     OSB_LAUNCH(fe_assign_kernel<true>, 1, 32, 0, st, recs, n_records, skip, h->cfg.self_id, (long long)L.cap, dbs, h->d_assign,
-               h->fb_dev, h->ingest_seq + 1, h->charged + (long long)n_records * OSB_MAX_DIRS, metas, h->meta);
+               h->fb.dev, seq, h->fb.charged, metas, h->meta);
   else
     OSB_LAUNCH(fe_assign_kernel<false>, 1, 32, 0, st, recs, n_records, skip, h->cfg.self_id, (long long)L.cap, dbs, h->d_assign,
-               h->fb_dev, h->ingest_seq + 1, h->charged + (long long)n_records * OSB_MAX_DIRS, nullptr, FeMeta{});
+               h->fb.dev, seq, h->fb.charged, nullptr, FeMeta{});
   OSB_CHECK_LAUNCH();
-  ++h->ingest_seq;
-  h->charged += (long long)n_records * OSB_MAX_DIRS;
   OSB_LAUNCH(fe_copy_rows_kernel, n_records * OSB_MAX_DIRS, 256, 0, st, recs, h->d_assign, h->cfg.max_num, dbs);
   OSB_CHECK_LAUNCH();
   L.upper += chg_l;
   R.upper += chg_r;
-  OSB_CUDA(record_event_capturable(h->ev_ingest, st));
-  h->ingest_pending = true;
+  OSB_CUDA(h->fb.record(st));
   fe_mark(h, 5, st);
   return OSB_OK;
 }
@@ -1393,7 +1358,9 @@ static osb_status fe_query(osb_frontend* h, const osb_keyframe_record* rec, int 
   QueryParams qp = fe_query_params(h);
   osb_status s;
   fe_mark(h, 5, st);
-  fe_tighten_bounds(h);
+  long long n[2], since;
+  if (h->fb.read(n, &since))
+    for (int i = 0; i < 2; ++i) h->db[i].upper = std::min<int64_t>(h->db[i].upper, n[i] + since);
   // a store that has never received a row needs no scan: its top-k list still holds the -1 labels it was created with
   // (upper is an upper bound of ntotal, so 0 is exact)
   if (R.upper > 0 &&
@@ -1448,7 +1415,9 @@ static osb_status fe_query_received(osb_frontend* h, const osb_keyframe_record* 
   DbStore& L = h->db[0];
   osb_status s;
   if ((s = fe_rq_alloc(h, st)) != OSB_OK) return s;
-  fe_tighten_bounds(h);
+  long long nr[2], since;
+  if (h->fb.read(nr, &since))
+    for (int i = 0; i < 2; ++i) h->db[i].upper = std::min<int64_t>(h->db[i].upper, nr[i] + since);
   // the queried direction's global descriptor of every record -> one contiguous [n][4096] slab
   OSB_CUDA(cudaMemcpy2DAsync(h->d_rq_desc, OSB_DEEP_DESC_SIZE * sizeof(float), &recs->global_desc[c.query_dir][0],
                              sizeof(osb_keyframe_record), OSB_DEEP_DESC_SIZE * sizeof(float), n, cudaMemcpyDeviceToDevice, st));
@@ -1653,13 +1622,13 @@ extern "C" osb_status osb_frontend_loop_counts(osb_frontend* h, int64_t* loop_co
 // (streams are non-blocking): wait for that ingest first, or the bound could be lowered below the true count while the
 // rows are still being appended -- the scan grid is sized from it.
 static osb_status fe_refresh_counts(osb_frontend* h, cudaStream_t st) {
-  if (h->ingest_pending) OSB_CUDA(cudaStreamWaitEvent(st, h->ev_ingest, 0));
+  if (h->fb.pending) OSB_CUDA(cudaStreamWaitEvent(st, h->fb.ev, 0));
   OSB_CUDA(cudaMemcpyAsync(&h->h_cnt[0], h->db[0].v.dev, sizeof(DbDev), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaMemcpyAsync(&h->h_cnt[1], h->db[1].v.dev, sizeof(DbDev), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   h->db[0].upper = h->h_cnt[0].ntotal; h->db[1].upper = h->h_cnt[1].ntotal;
-  h->ingest_pending = false;
-  h->fb_min_seq = h->ingest_seq + 1;            // exact now: older feedback carries nothing new
+  h->fb.pending = false;
+  h->fb.exact();
   return OSB_OK;
 }
 
@@ -1800,7 +1769,7 @@ extern "C" osb_status osb_frontend_db_reset(osb_frontend* h) {
     if (h->meta_ready)                                     // the frames' metas go; the trajectory stays
       OSB_CUDA(cudaMemsetAsync(h->meta.ok[i], 0, (size_t)h->db[i].cap * sizeof(int32_t), h->stream));
   }
-  h->fb_min_seq = h->ingest_seq + 1;
+  h->fb.exact();
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   return OSB_OK;
 }
@@ -1931,7 +1900,7 @@ extern "C" osb_status osb_frontend_meta_status(osb_frontend* h, osb_status* last
   if (!h->meta_ready) return OSB_OK;
   DeviceGuard dg(h->device);
   cudaStream_t st = h->stream;
-  if (h->ingest_pending) OSB_CUDA(cudaStreamWaitEvent(st, h->ev_ingest, 0));
+  if (h->fb.pending) OSB_CUDA(cudaStreamWaitEvent(st, h->fb.ev, 0));
   OSB_CUDA(cudaMemcpyAsync(h->h_meta, h->meta.dev, sizeof(FeMetaDev), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   *last = (osb_status)h->h_meta->status;
