@@ -291,6 +291,41 @@ def evaluate_vec(g: dict, x: np.ndarray, want_jac: bool = True):
     return cost, r, Ja, Jb
 
 
+def _jacobian_layout(g: dict):
+    """-> (free [nf] node ids, col_of [n] (-1: fixed), masks ma / mb [m,4,4] of the free blocks, rows R and columns C of
+    their entries in the [4m, 4 nf] Jacobian: factor f owns rows 4f..4f+3, free node i columns 4 col_of[i]..+3)"""
+    n, m = len(g["fixed"]), len(g["ftype"])
+    free = np.nonzero(g["fixed"] == 0)[0]
+    col_of = -np.ones(n, np.int64); col_of[free] = np.arange(len(free))
+    ia, ib = g["ia"], g["ib"]
+    rows = (np.arange(m)[:, None, None] * 4 + np.arange(4)[None, :, None]) + np.zeros((1, 1, 4), np.int64)
+    ca = (col_of[ia][:, None, None] * 4 + np.arange(4)[None, None, :]) + np.zeros((1, 4, 1), np.int64)
+    cb = (col_of[ib][:, None, None] * 4 + np.arange(4)[None, None, :]) + np.zeros((1, 4, 1), np.int64)
+    ma = np.broadcast_to((col_of[ia] >= 0)[:, None, None], (m, 4, 4))
+    mb = np.broadcast_to((col_of[ib] >= 0)[:, None, None], (m, 4, 4))
+    return free, col_of, ma, mb, np.concatenate([rows[ma], rows[mb]]), np.concatenate([ca[ma], cb[mb]])
+
+
+def lm_system(g: dict, x: np.ndarray, radius: float) -> dict:
+    """The LM step's linear system at poses x, as solve_fast builds it: robustified J (sparse [4m, 4 nf], factor f in
+    rows 4f..4f+3), H = J^T J, grad = J^T r, D = diag(H) clipped to [1e-6, 1e32], the free-node map and the cost.
+    The step solves (H + diag(D) / radius) delta = -grad; delta[4 col_of[i] + k] moves component k of free node i."""
+    import scipy.sparse as sp
+    free, col_of, ma, mb, R, Cc = _jacobian_layout(g)
+    m = len(g["ftype"])
+    cost, r, Ja, Jb = evaluate_vec(g, np.asarray(x, np.float64))
+    J = sp.csr_matrix((np.concatenate([Ja[ma], Jb[mb]]), (R, Cc)), shape=(4 * m, 4 * len(free)))
+    H = (J.T @ J).tocsc()
+    return dict(J=J, H=H, grad=J.T @ r.reshape(-1), D=np.clip(H.diagonal(), 1e-6, 1e32), radius=float(radius),
+                free=free, col_of=col_of, cost=cost)
+
+
+def lm_step(sysm: dict) -> np.ndarray:
+    """the exact step of an lm_system: (H + diag(D) / radius)^-1 (-grad), by the sparse direct solve solve_fast uses"""
+    import scipy.sparse as sp
+    return _spd_solve((sysm["H"] + sp.diags(sysm["D"] / sysm["radius"])).tocsc(), -sysm["grad"])
+
+
 def solve_fast(g: dict, max_iters: int = 200, function_tol: float = 1e-6, gradient_tol: float = 1e-10,
                param_tol: float = 1e-8, num_threads: int | None = None):
     """Same LM as solve(), vectorised; default tolerances = Ceres defaults (the configuration the reference runs,
@@ -298,18 +333,9 @@ def solve_fast(g: dict, max_iters: int = 200, function_tol: float = 1e-6, gradie
     import scipy.sparse as sp
     import scipy.sparse.linalg as spla
     x = g["init"].astype(np.float64).copy()
-    n = x.shape[0]
     m = len(g["ftype"])
-    free = np.nonzero(g["fixed"] == 0)[0]
-    col_of = -np.ones(n, np.int64); col_of[free] = np.arange(len(free))
+    free, col_of, ma, mb, R, Cc = _jacobian_layout(g)
     nv = 4 * len(free)
-    ia, ib = g["ia"], g["ib"]
-    rows = (np.arange(m)[:, None, None] * 4 + np.arange(4)[None, :, None]) + np.zeros((1, 1, 4), np.int64)
-    ca = (col_of[ia][:, None, None] * 4 + np.arange(4)[None, None, :]) + np.zeros((1, 4, 1), np.int64)
-    cb = (col_of[ib][:, None, None] * 4 + np.arange(4)[None, None, :]) + np.zeros((1, 4, 1), np.int64)
-    ma = np.broadcast_to((col_of[ia] >= 0)[:, None, None], (m, 4, 4))
-    mb = np.broadcast_to((col_of[ib] >= 0)[:, None, None], (m, 4, 4))
-    R = np.concatenate([rows[ma], rows[mb]]); Cc = np.concatenate([ca[ma], cb[mb]])
     radius, decrease = 1e4, 2.0
     cost, r, Ja, Jb = evaluate_vec(g, x)
     initial_cost = cost
