@@ -513,7 +513,7 @@ osb_status osb_pcm_state_pair(osb_pcm_state* s, int32_t id_a, int32_t id_b, int3
  *   drone twice in one frame or a malformed frame_first give OSB_ERR_INVALID; exceeding a capacity gives OSB_ERR_CAPACITY.
  *   Either way the handle is unchanged.  Updates wait for the handle's last run on any stream before they overwrite state.
  * Memory: create acquires everything (a stream, an event, the trajectories, measurements, window and run output at their
- *   capacities); nothing is acquired later. */
+ *   capacities); later only the first add_measurements_dev and the first observe_dev acquire theirs (below). */
 #define OSB_MEAS_LOOP 0
 #define OSB_MEAS_DET4D 1
 #define OSB_MEAS_DET6D 2
@@ -599,6 +599,49 @@ osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_
 osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_measurement* m_dev, const int32_t* count_dev, int max_n,
                                            float loop_outlier_distance_threshold, void* stream);
 osb_status osb_anchor_status(osb_anchor* h, osb_status* last);
+/* osb_anchor_observe_dev(): SwarmLocalizationSolver::estimate_observability (swarm_localization_solver.cpp:1336-1427) on the
+ *   device, from the n rows osb_anchor_run_dev wrote (n = its n_out, VOID tail included), on `stream` without
+ *   synchronising.  Goes between run_dev and osb_anchor_compact_factors_dev (before or after osb_pcm_state_reject_anchored,
+ *   which reads only status).  With the window's frame count, the node set and the drones' bounding boxes, and the
+ *   handle's persistent state (pos, enable, solve_master):
+ *   1. E = the unordered pairs (edge.id_a, edge.id_b) of the rows with status == OSB_ANCHOR_OK (loops and detections);
+ *   2. L = {self_id}, or its closure over E when the node set holds more than one drone (loop_observable_set, :1299-1334);
+ *   3. yaw is cleared; 4. more than 3 frames (SINGLE_DRONE_SFS_THRES) and exactly one node: solve_master;
+ *   5. every d in L: to_init if !pos[d]; pos = yaw = enable = 1; solve_master when d != self_id;
+ *   6. self_id's box: xmax - xmin > init_xy_movement && ymax - ymin > init_xy_movement && zmax - zmin > init_z_movement
+ *      (the float thresholds compared as doubles): solve_master, motion; every node with !pos: motion_new, to_init;
+ *      every node: pos = enable = 1;
+ *   7. every node whose box's x or y extent is > 1.0 (THRES_YAW_OBSER_XY): yaw;
+ *   8. every row: skip = !(status == OK && yaw[edge.id_a] && yaw[edge.id_b] && node_a != node_b), written in place; no
+ *      other byte of a row changes.  So the rows become run_dev's with this yaw as its yaw_observable.
+ *   A drone's box covers its vo_available entries of the current window, from max = -1000 and min = +1000 per axis
+ *   (boundingbox_sldwin, :848-878), in fp64; an empty box has extents of -2000.  The node set (all_nodes) is every drone id
+ *   of every set_window entry since create, vo_available or not.  pos and enable start at 0 and only ever become 1, as
+ *   does solve_master; enable[self_id] is always 1 (:640).  set_window derives the frame count, the node set and the
+ *   boxes on the host, so a captured observe sees the window set before each replay.
+ *   Three launches whatever n and the drone count (one pass over the rows sets a drone-pair bit matrix from status,
+ *   edge.id_a and edge.id_b; one CTA runs the closure and steps 3-7; one pass rewrites skip).  The first call acquires the
+ *   state, the bit matrix, the window record and an event, and synchronises; later calls acquire nothing and can be
+ *   captured into a CUDA graph.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n < 0, self_id
+ *   outside 0..max_drones-1.  Each observe waits for the handle's last observe on any stream; the updates (push_odometry,
+ *   add_measurements, set_window) wait for it as they wait for the last run.
+ * osb_anchor_observability(): waits for the last observe and writes its outcome: per drone the node set, yaw, the sticky
+ *   pos and enable and to_init (ids_to_init), 1 or 0 each; solve_master (enable_to_solve_master, sticky), motion (the self
+ *   box test held) and motion_new (it found a node with !pos).  The caller's state machine keeps finish_init and
+ *   system_is_initied_by_motion: motion_new means finish_init = 0 and by_motion = 1; motion && !finish_init means
+ *   by_motion = 1 (:1392-1402).  All zero before the first observe. */
+typedef struct {
+  int32_t self_id;
+  float init_xy_movement, init_z_movement;   /* the reference's float parameters */
+  int32_t reserved;
+} osb_observe_params;
+typedef struct {
+  uint8_t nodes[256], yaw[256], pos[256], enable[256], to_init[256];   /* [drone], 1 or 0; drones >= max_drones are 0 */
+  int32_t solve_master, motion, motion_new, reserved;
+} osb_observability;
+osb_status osb_anchor_observe_dev(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev, int n,
+                                  void* stream);
+osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * The solve's chain from re-anchoring to factor rows on the device: run_dev -> reject_anchored -> compact_factors_dev, all

@@ -359,6 +359,126 @@ anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __res
   fb->publish(seq, status == OSB_OK ? have_l + nl : have_l, status == OSB_OK ? have_d + nd : have_d, status, charged);
 }
 
+// estimate_observability (swarm_localization_solver.cpp:1336-1427) from the rows of this solve: three launches.
+// observe_edges_kernel ORs the drone pair of every OK row into a bit matrix (row d: drone d's neighbours, 256 bits);
+// observe_state_kernel, one CTA, takes the matrix (and clears it for the next call), walks it from self_id a frontier of
+// four 64-bit words at a time, applies the rules to the persistent state and writes the record; observe_skip_kernel
+// rewrites each row's skip from the record's yaw.
+constexpr int OBS_THREADS = 256;                                  // = ANCHOR_MAX_DRONES: thread d owns drone d
+constexpr int OBS_WORDS = ANCHOR_MAX_DRONES / 64;                 // 64-bit words of a drone set
+constexpr int OBS_ROW32 = ANCHOR_MAX_DRONES / 32;                 // 32-bit words of a matrix row
+constexpr double THRES_YAW_OBSER_XY = 1.0;                        // :49
+constexpr int SINGLE_DRONE_SFS_THRES = 3;                         // :62
+
+// what observe takes from the window, derived by set_window on the host
+struct ObserveWindow {
+  double ext[ANCHOR_MAX_DRONES][3];   // boundingbox_sldwin's max - min per axis (-2000 for a drone without an entry)
+  uint64_t nodes[OBS_WORDS];          // all_nodes: every drone of every window since create
+  int32_t n_frames, n_nodes;
+};
+
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_edges_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_drones, unsigned* __restrict__ adj) {
+  __shared__ unsigned s_adj[ANCHOR_MAX_DRONES * OBS_ROW32];
+  volatile unsigned* vs = s_adj;
+  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS) s_adj[k] = 0;
+  __syncthreads();
+  for (int i = blockIdx.x * OBS_THREADS + threadIdx.x; i < n; i += gridDim.x * OBS_THREADS) {
+    if (rows[i].status != OSB_ANCHOR_OK) continue;
+    const int a = rows[i].edge.id_a, b = rows[i].edge.id_b;
+    if ((unsigned)a >= (unsigned)max_drones || (unsigned)b >= (unsigned)max_drones) continue;
+    const int ab = a * OBS_ROW32 + (b >> 5), ba = b * OBS_ROW32 + (a >> 5);
+    const unsigned bit_b = 1u << (b & 31), bit_a = 1u << (a & 31);
+    if (!(vs[ab] & bit_b)) atomicOr(&s_adj[ab], bit_b);          // most rows repeat a pair already set
+    if (!(vs[ba] & bit_a)) atomicOr(&s_adj[ba], bit_a);
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS)
+    if (s_adj[k]) atomicOr(adj + k, s_adj[k]);
+}
+
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
+                     int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs) {
+  __shared__ unsigned long long s_adj[ANCHOR_MAX_DRONES][OBS_WORDS];
+  __shared__ unsigned long long s_seen[OBS_WORDS], s_front[OBS_WORDS], s_next[OBS_WORDS];
+  __shared__ int s_more;
+  const int d = threadIdx.x;
+  for (int k = d; k < max_drones * OBS_WORDS; k += OBS_THREADS) {
+    s_adj[k / OBS_WORDS][k % OBS_WORDS] = adj[k];
+    adj[k] = 0;
+  }
+  if (d < OBS_WORDS) {
+    s_seen[d] = s_front[d] = d == (self_id >> 6) ? 1ull << (self_id & 63) : 0ull;
+    s_next[d] = 0;
+  }
+  __syncthreads();
+  if (win->n_nodes > 1) {                                          // loop_observable_set's BFS, one level per pass
+    for (;;) {
+      if (d < max_drones && ((s_front[d >> 6] >> (d & 63)) & 1ull))
+        for (int w = 0; w < OBS_WORDS; ++w)
+          if (s_adj[d][w]) atomicOr(&s_next[w], s_adj[d][w]);
+      __syncthreads();
+      if (d == 0) {
+        int more = 0;
+        for (int w = 0; w < OBS_WORDS; ++w) {
+          const unsigned long long f = s_next[w] & ~s_seen[w];
+          s_front[w] = f;
+          s_seen[w] |= f;
+          s_next[w] = 0;
+          more |= f != 0;
+        }
+        s_more = more;
+      }
+      __syncthreads();
+      if (!s_more) break;
+    }
+  }
+  const bool live = d < max_drones;
+  const bool node = live && ((win->nodes[d >> 6] >> (d & 63)) & 1ull);
+  const bool in_l = live && ((s_seen[d >> 6] >> (d & 63)) & 1ull);
+  bool pos = live && obs->pos[d], enable = live && obs->enable[d], yaw = false, to_init = false, fresh = false;
+  if (in_l) {                                                      // :1369-1379
+    to_init = !pos;
+    pos = yaw = enable = true;
+  }
+  const double* se = win->ext[self_id];                            // :1381-1403
+  const bool motion = se[0] > (double)xy_thres && se[1] > (double)xy_thres && se[2] > (double)z_thres;
+  if (motion && node) {
+    if (!pos) fresh = to_init = true;
+    pos = enable = true;
+  }
+  if (node && (win->ext[d][0] > THRES_YAW_OBSER_XY || win->ext[d][1] > THRES_YAW_OBSER_XY)) yaw = true;   // :1413-1422
+  if (d == self_id) enable = true;                                 // :640
+  const int other = __syncthreads_or(in_l && d != self_id);
+  const int motion_new = __syncthreads_or(fresh);
+  obs->nodes[d] = node;
+  obs->yaw[d] = yaw;
+  obs->pos[d] = pos;
+  obs->enable[d] = enable;
+  obs->to_init[d] = to_init;
+  if (d == 0) {
+    const bool single = win->n_frames > SINGLE_DRONE_SFS_THRES && win->n_nodes == 1;   // :1364-1367
+    obs->solve_master = obs->solve_master || single || other || motion;
+    obs->motion = motion;
+    obs->motion_new = motion_new;
+    obs->reserved = 0;
+  }
+}
+
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones, const osb_observability* __restrict__ obs) {
+  const int i = blockIdx.x * OBS_THREADS + threadIdx.x;
+  if (i >= n) return;
+  bool use = rows[i].status == OSB_ANCHOR_OK;                      // anchor_kernel's rule (:1066-1073) with this yaw
+  if (use) {
+    const int a = rows[i].edge.id_a, b = rows[i].edge.id_b;
+    use = (unsigned)a < (unsigned)max_drones && (unsigned)b < (unsigned)max_drones && obs->yaw[a] && obs->yaw[b] &&
+          rows[i].node_a != rows[i].node_b;
+  }
+  rows[i].skip = use ? 0 : 1;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -366,6 +486,7 @@ using namespace osb;
 static_assert(sizeof(osb_measurement) == 496, "osb_measurement layout");
 static_assert(sizeof(osb_window_entry) == 80, "osb_window_entry layout");
 static_assert(sizeof(osb_anchor_result) == 760, "osb_anchor_result layout");
+static_assert(sizeof(osb_observability) == 5 * 256 + 16, "osb_observability layout");
 
 struct osb_anchor {
   Resources res;
@@ -392,6 +513,13 @@ struct osb_anchor {
   CountFeedback fb;                               // fb.pending: an append may not have run, n_loops / n_dets are stale
   long long upper = 0;                            // bound of n_loops + n_dets while fb.pending
   osb_status last_status = OSB_OK;                // the last device append's, once synchronised
+  // observe_dev, acquired by the first one: the drone-pair matrix (zero between calls), the window record and the
+  // persistent state, which is also the outcome osb_anchor_observability reads
+  unsigned* d_adj = nullptr;                      // [max_drones][8] 32-bit words
+  ObserveWindow* d_obs_win = nullptr;
+  osb_observability* d_obs = nullptr;
+  cudaEvent_t last_observe = nullptr;             // recorded after every observe, on its stream
+  ObserveWindow obs_win{};                        // the host's, kept by set_window whether or not observe ever ran
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -409,7 +537,32 @@ namespace {
 
 osb_status anchor_wait_last_run(osb_anchor* h) {
   OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_run, 0));
+  if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
   return OSB_OK;
+}
+
+// the window's part of observe: all_nodes grows by every drone of the window; each drone's box spans its vo_available
+// entries, from max = -1000 and min = +1000 per axis (boundingbox_sldwin, swarm_localization_solver.cpp:848-878)
+void observe_window(ObserveWindow& w, int max_drones, int n_frames, int n_entries, const osb_window_entry* entries) {
+  double lo[ANCHOR_MAX_DRONES][3], hi[ANCHOR_MAX_DRONES][3];
+  for (int d = 0; d < max_drones; ++d)
+    for (int j = 0; j < 3; ++j) { hi[d][j] = -1000.0; lo[d][j] = 1000.0; }
+  for (int e = 0; e < n_entries; ++e) {
+    const int d = entries[e].drone_id;
+    w.nodes[d >> 6] |= 1ull << (d & 63);
+    if (!entries[e].vo_available) continue;
+    for (int j = 0; j < 3; ++j) {
+      const double x = entries[e].self_pose[j];
+      if (x > hi[d][j]) hi[d][j] = x;
+      if (x < lo[d][j]) lo[d][j] = x;
+    }
+  }
+  for (int d = 0; d < max_drones; ++d)
+    for (int j = 0; j < 3; ++j) w.ext[d][j] = hi[d][j] - lo[d][j];
+  int n_nodes = 0;
+  for (int k = 0; k < OBS_WORDS; ++k) n_nodes += __builtin_popcountll(w.nodes[k]);
+  w.n_frames = n_frames;
+  w.n_nodes = n_nodes;
 }
 
 bool drone_ok(const osb_anchor* h, int32_t d) { return d >= 0 && d < h->p.max_drones; }
@@ -475,6 +628,7 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
   h->h_win_pose.resize(E * 7);
   h->h_len.reserve(S);
   h->h_slot.reserve(M);
+  observe_window(h->obs_win, p->max_drones, 0, 0, nullptr);
   *out = h.release();
   return OSB_OK;
 }
@@ -621,9 +775,12 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
       std::copy(entries[e].self_pose, entries[e].self_pose + 7, h->h_win_pose.begin() + (size_t)k * 7);
     }
   const int n_vo = first[D];
+  observe_window(h->obs_win, D, n_frames, n_entries, entries);
   OSB_TRY(anchor_wait_last_run(h));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemcpyAsync(h->d_drone_first, first.data(), (size_t)(D + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (h->d_obs_win)
+    OSB_CUDA(cudaMemcpyAsync(h->d_obs_win, &h->obs_win, sizeof(ObserveWindow), cudaMemcpyHostToDevice, st));
   if (n_vo > 0) {
     OSB_CUDA(cudaMemcpyAsync(h->d_win_stamp, h->h_win_stamp.data(), (size_t)n_vo * sizeof(int64_t), cudaMemcpyHostToDevice, st));
     OSB_CUDA(cudaMemcpyAsync(h->d_win_frame, h->h_win_frame.data(), (size_t)n_vo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -767,4 +924,62 @@ extern "C" osb_status osb_anchor_status(osb_anchor* h, osb_status* last) {
   OSB_TRY(anchor_settle(h));
   *last = h->last_status;
   return h->last_status;
+}
+
+namespace {
+
+// the first observe acquires the matrix (zeroed), the window record (the host's), the state (zeroed) and the event
+osb_status observe_init(osb_anchor* h) {
+  if (h->d_obs) return OSB_OK;
+  const size_t D = (size_t)h->p.max_drones;
+  OSB_TRY(h->res.alloc(&h->d_adj, D * OBS_ROW32));
+  OSB_TRY(h->res.alloc(&h->d_obs_win, 1));
+  OSB_TRY(h->res.event(&h->last_observe, cudaEventDisableTiming));
+  osb_observability* obs = nullptr;
+  OSB_TRY(h->res.alloc(&obs, 1));
+  OSB_CUDA(cudaMemsetAsync(h->d_adj, 0, D * OBS_ROW32 * sizeof(unsigned), h->stream));
+  OSB_CUDA(cudaMemsetAsync(obs, 0, sizeof(osb_observability), h->stream));
+  OSB_CUDA(cudaMemcpyAsync(h->d_obs_win, &h->obs_win, sizeof(ObserveWindow), cudaMemcpyHostToDevice, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  h->d_obs = obs;                                                  // set last: a failed first call is tried again
+  return OSB_OK;
+}
+
+}  // namespace
+
+extern "C" osb_status osb_anchor_observe_dev(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev, int n,
+                                             void* stream) {
+  OSB_REQUIRE(h != nullptr && p != nullptr && rows_dev != nullptr, "null argument");
+  OSB_REQUIRE(n >= 0, "negative row count");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(observe_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = h->p.max_drones;
+  const int blocks = cdiv(std::max(n, 1), OBS_THREADS);
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // the state and the matrix are the last observe's
+  OSB_LAUNCH(observe_edges_kernel, std::min(blocks, 4 * num_sms()), OBS_THREADS, 0, st, rows_dev, n, D, h->d_adj);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(observe_state_kernel, 1, OBS_THREADS, 0, st, reinterpret_cast<unsigned long long*>(h->d_adj), h->d_obs_win, D,
+             p->self_id, p->init_xy_movement, p->init_z_movement, h->d_obs);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(observe_skip_kernel, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_observe, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out) {
+  OSB_REQUIRE(h != nullptr && out != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (!h->d_obs) {
+    memset(out, 0, sizeof(*out));
+    return OSB_OK;
+  }
+  DeviceGuard dg(h->device);
+  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
+  OSB_CUDA(cudaMemcpyAsync(out, h->d_obs, sizeof(*out), cudaMemcpyDeviceToHost, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  return OSB_OK;
 }

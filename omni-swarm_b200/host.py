@@ -951,6 +951,24 @@ class LoopAnchor(_Handle):
         _l.check(self._lib.osb_anchor_run_dev(self._h, _l.ptr(y), C.c_void_p(out_ptr), C.byref(n), C.c_void_p(stream)))
         return n.value
 
+    def observe_dev(self, rows_ptr: int, n: int, stream: int, self_id: int, init_xy_movement: float,
+                    init_z_movement: float):
+        """estimate_observability on the device (osb_anchor_observe_dev) from the n rows run_dev wrote at rows_ptr: updates
+        the handle's observability state and rewrites each row's skip with this solve's yaw-observable drones, on `stream`
+        without synchronising"""
+        p = _l.ObserveParams(int(self_id), float(init_xy_movement), float(init_z_movement), 0)
+        _l.check(self._lib.osb_anchor_observe_dev(self._h, C.byref(p), C.c_void_p(rows_ptr), int(n), C.c_void_p(stream)))
+
+    def observability(self) -> dict:
+        """waits for the last observe_dev -> its outcome: bool arrays [max_drones] nodes, yaw, pos, enable, to_init and
+        the flags solve_master, motion, motion_new"""
+        o = _l.Observability()
+        _l.check(self._lib.osb_anchor_observability(self._h, C.byref(o)))
+        out = {k: np.frombuffer(bytes(getattr(o, k)), np.uint8)[:self.max_drones].astype(bool)
+               for k in ("nodes", "yaw", "pos", "enable", "to_init")}
+        out.update(solve_master=bool(o.solve_master), motion=bool(o.motion), motion_new=bool(o.motion_new))
+        return out
+
 
 def anchored_factor_rows(res: np.ndarray, keep=None):
     """the solver rows of the results with skip == 0 (and keep[i], e.g. the PCM keep mask) -> (ftype, ia, ib, payload,
@@ -1060,6 +1078,10 @@ class AnchoredChain:
 
     def run(self, anchor: LoopAnchor, yaw_observable=None) -> int:
         return anchor.run_dev(self.rows.data_ptr(), self.stream.cuda_stream, yaw_observable)
+
+    def observe(self, anchor: LoopAnchor, n: int, self_id: int, init_xy_movement: float, init_z_movement: float):
+        """the observability of the first n rows, their skip rewritten in place (LoopAnchor.observe_dev)"""
+        anchor.observe_dev(self.rows.data_ptr(), n, self.stream.cuda_stream, self_id, init_xy_movement, init_z_movement)
 
     def reject(self, state: PcmState, n: int):
         state.reject_anchored(self.rows.data_ptr(), n, self.keep.data_ptr(), self.stream.cuda_stream)

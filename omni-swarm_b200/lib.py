@@ -86,6 +86,20 @@ class AnchorParams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class ObserveParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("init_xy_movement", C.c_float), ("init_z_movement", C.c_float),
+                ("reserved", C.c_int32)]
+
+
+OBS_DRONES = 256                         # per-drone bytes of osb_observability
+
+
+class Observability(C.Structure):
+    _fields_ = [("nodes", C.c_uint8 * OBS_DRONES), ("yaw", C.c_uint8 * OBS_DRONES), ("pos", C.c_uint8 * OBS_DRONES),
+                ("enable", C.c_uint8 * OBS_DRONES), ("to_init", C.c_uint8 * OBS_DRONES), ("solve_master", C.c_int32),
+                ("motion", C.c_int32), ("motion_new", C.c_int32), ("reserved", C.c_int32)]
+
+
 MEAS_LOOP, MEAS_DET4D, MEAS_DET6D = 0, 1, 2
 # numpy views of osb_measurement, osb_window_entry, osb_loop_edge and osb_anchor_result (include/omniswarm_b200.h)
 MEASUREMENT_DTYPE = np.dtype([("id", "<i8"), ("type", "<i4"), ("id_a", "<i4"), ("id_b", "<i4"), ("reserved", "<i4"),
@@ -323,6 +337,8 @@ _SIG = {
     "osb_anchor_compact_factors_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "osb_anchor_add_measurements_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_float, _P]),
     "osb_anchor_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
+    "osb_anchor_observe_dev": (C.c_int, [_P, C.POINTER(ObserveParams), _P, C.c_int, _P]),
+    "osb_anchor_observability": (C.c_int, [_P, C.POINTER(Observability)]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
