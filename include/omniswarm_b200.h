@@ -386,8 +386,43 @@ osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail, const int3
                                          const int32_t* ib_dev, const double* payload_dev, const uint8_t* huber_dev,
                                          const int32_t* count_dev, const osb_solve_options* opt, void* stream);
 /* synchronises with the last osb_solver_solve_resident_dev call -> its status; on OSB_OK its summary (n_residuals =
- * resident + tail; solve_ms from CUDA events, 0 when the call was captured) */
+ * resident + tail; solve_ms from CUDA events, 0 when the call was captured).  After an
+ * osb_solver_solve_multistart_resident_dev call it returns OSB_ERR_INVALID: osb_solver_last_multistart reads that call. */
 osb_status osb_solver_last_summary(osb_solver* h, osb_solve_summary* summary);
+/* Random-restart initialisation on the device chain -- solve_with_multiple_init (swarm_localization_solver.cpp:781-845)
+ * of the resident window plus a device tail, the branch solve() takes at start-up, when a drone appears and after a solve
+ * whose equv_cost exceeds acpt_cost (:880-960).  Takes osb_solver_solve_resident_dev's arguments, plus:
+ *   init_mask_dev [n] (caller's node ids, device): the nodes to scatter, e.g. what osb_anchor_init_mask_dev wrote;
+ *   init_yaw_dev [n] (device) or NULL: a scattered node's yaw (the odometry yaw of random_init_pose, :212); NULL keeps
+ *   the node's yaw; ms: as osb_solver_solve_multistart.
+ *   Rule: osb_solver_solve_multistart of the concatenated list (resident factors, then the *count_dev tail rows) under the
+ *   resident plan, started from the resident device poses: the same draws keyed (seed, trial, caller's node id,
+ *   component), the same ranking (equv, strict < against acpt_cost, first of equal minima), with n_residuals (for
+ *   normalise) = resident + tail residuals counted on the device.  A trial's arithmetic is osb_solver_solve_resident_dev's
+ *   from its starting poses, so every trial, equv and the choice are bit-identical to osb_solver_solve_multistart of the
+ *   concatenated list whenever both pick the same shape and plan.  The chosen trial's poses go into the resident device
+ *   pose copy; with no trial accepted (chosen = -1) that copy is left as it was (osb_solver_solve_multistart's documented
+ *   deviation, not the reference's "last trial's poses").  The host copy is refreshed as after osb_solver_solve_resident_dev.
+ *   Launches: the shape is osb_solver_solve's for (n, m + max_tail); the four tail-table launches (built once, shared by
+ *   the trials), one scatter, the trials, one selection: 7 launches on the cluster path (all trials in one launch, one
+ *   cluster each), 6 + n_trials on the cooperative path (the trials in turn, each keeping its own summary).
+ *   Refused on the device as osb_solver_solve_resident_dev (every trial leaves before its first barrier): chosen = -1, poses
+ *   and graph unchanged, osb_solver_last_multistart returns the code.  Refused at once with nothing enqueued: its refusals,
+ *   a null init_mask_dev or ms, and osb_solver_solve_multistart's checks of ms (n_trials outside 1 ... 256, normalise with
+ *   window_size < 1, rand_xy / rand_z negative or not finite, acpt_cost NaN).
+ *   Memory: the first call acquires what osb_solver_solve_resident_dev's first call does; the arena grows to n_trials solves
+ *   as in osb_solver_solve_multistart.  Growing it is host work: under stream capture a call that would need it returns
+ *   OSB_ERR_INVALID with nothing enqueued.  Otherwise capture follows osb_solver_solve_resident_dev's rules. */
+osb_status osb_solver_solve_multistart_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev,
+                                                    const int32_t* ia_dev, const int32_t* ib_dev, const double* payload_dev,
+                                                    const uint8_t* huber_dev, const int32_t* count_dev,
+                                                    const uint8_t* init_mask_dev, const double* init_yaw_dev,
+                                                    const osb_solve_options* opt, const osb_multistart_options* ms,
+                                                    void* stream);
+/* synchronises with the last osb_solver_solve_multistart_resident_dev call -> its status; on OSB_OK every trial's summary
+ * [n_trials] (n_residuals = resident + tail; solve_ms = the device time of all trials from CUDA events, 0 when the call was
+ * captured), equv [n_trials] and chosen (-1: none accepted).  OSB_ERR_INVALID when the last device call was a single solve. */
+osb_status osb_solver_last_multistart(osb_solver* h, osb_solve_summary* summaries, double* equv, int32_t* chosen);
 /* profiling aid: SM-clock cycles block 0 spent in the phases of the LAST solve, summed over its CG iterations:
  * out[0] factor phase, [1] barrier after it, [2] node phase 1, [3] reduction 1, [4] node phase 2, [5] reduction 2,
  * [6] number of CG iterations, [7] whole kernel; [8] CTAs, [9] 1 = one thread-block cluster (hardware barrier) /
@@ -642,6 +677,22 @@ typedef struct {
 osb_status osb_anchor_observe_dev(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev, int n,
                                   void* stream);
 osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out);
+/* osb_anchor_init_mask_dev(): random_init_pose's choice of blocks (swarm_localization_solver.cpp:204-216) from the window
+ *   and the record the last osb_anchor_observe_dev wrote, on the device: mask_dev[b] = 1 iff block b belongs to a window
+ *   entry of a drone d with to_init[d] and d != self_id, and yaw_dev[b] = the yaw of that entry's self_pose (NodeFrame::yaw(),
+ *   the odometry yaw; quaternion -> yaw as the re-anchoring computes it, oracle/anchor_ref.py).  Every window entry counts,
+ *   vo_available or not (add_as_keyframe gives each node frame an est_poses block, :517-540).  A block shared by several
+ *   frames takes its latest frame's pose (the reference writes the shared block once per frame, in stamp order).  Every
+ *   other element of [0, n_nodes) gets mask 0 and yaw 0.  The output feeds osb_solver_solve_multistart_resident_dev.
+ *   set_window derives each block's drone and pose on the host; the first call acquires the device copy (at
+ *   max_window_entries blocks, or the window's largest block id + 1 if more) and synchronises, and set_window keeps it
+ *   current after that.  to_init is read on the device, so a captured call follows both the window set before each replay
+ *   and that replay's observe.  (A set_window whose block ids outgrow the copy replaces it: capture again after it.)
+ *   One launch on `stream`, ordered after the handle's last observe on any stream; the next observe and set_window are
+ *   ordered after it.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n_nodes < 1, a window block
+ *   outside 0 .. n_nodes-1, self_id outside 0..max_drones-1, or no observe_dev since create. */
+osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, int n_nodes, uint8_t* mask_dev, double* yaw_dev,
+                                    void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * The solve's chain from re-anchoring to factor rows on the device: run_dev -> reject_anchored -> compact_factors_dev, all

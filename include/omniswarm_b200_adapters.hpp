@@ -410,6 +410,31 @@ class ResidentPoseGraph {
     for (size_t i = 0; i < ptr_.size(); ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
     return s;
   }
+  // solve_with_multiple_init (:781-845) on the device chain: the resident window plus this solve's rows (as
+  // solve_with_device_factors), ms.n_trials restarts of the blocks init_mask_dev marks (e.g. osb_anchor_init_mask_dev's
+  // output after the solve's osb_anchor_observe_dev), with their yaw from init_yaw_dev (or kept, when null).  Sends what was
+  // added, solves on `stream`, waits, and writes the poses back to the caller's double[4] blocks only when a trial got
+  // below ms.acpt_cost; returns that (cost_updated, :844) and sets cost_now to the accepted trial's equv_cost.
+  bool solve_with_multiple_init_dev(int max_tail, const int32_t* type_dev, const int32_t* ia_dev, const int32_t* ib_dev,
+                                    const double* payload_dev, const uint8_t* huber_dev, const int32_t* count_dev,
+                                    const uint8_t* init_mask_dev, const double* init_yaw_dev,
+                                    const osb_multistart_options& ms, void* stream, const osb_solve_options* opt = nullptr) {
+    flush();
+    check(osb_solver_solve_multistart_resident_dev(solver_, max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev,
+                                                   count_dev, init_mask_dev, init_yaw_dev, opt, &ms, stream),
+          "osb_solver_solve_multistart_resident_dev");
+    std::vector<osb_solve_summary> summaries(ms.n_trials);
+    std::vector<double> equv(ms.n_trials);
+    int32_t chosen = -1;
+    check(osb_solver_last_multistart(solver_, summaries.data(), equv.data(), &chosen), "osb_solver_last_multistart");
+    if (chosen < 0) return false;
+    std::vector<double> poses(4 * ptr_.size());
+    check(osb_solver_graph_get_poses(solver_, 0, (int)ptr_.size(), poses.data()), "osb_solver_graph_get_poses");
+    for (size_t i = 0; i < ptr_.size(); ++i) for (int j = 0; j < 4; ++j) ptr_[i][j] = poses[4 * i + j];
+    cost_now = equv[chosen];
+    return true;
+  }
+  double cost_now = 0.0;             // equv_cost of the trial solve_with_multiple_init_dev accepted last (:809)
 
  private:
   void flush() {                                     // send what was added since the last solve

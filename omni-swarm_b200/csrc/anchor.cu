@@ -479,6 +479,20 @@ observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones,
   rows[i].skip = use ? 0 : 1;
 }
 
+// random_init_pose's choice of blocks (swarm_localization_solver.cpp:204-216) from the last observe's to_init: thread b
+// masks block b iff its drone is to be initialised and is not self_id, and gives it the odometry yaw of its latest frame
+__global__ void init_mask_kernel(const int32_t* __restrict__ blk_drone, const double* __restrict__ blk_q,
+                                 const int32_t* __restrict__ n_blk, int n_nodes, int self_id,
+                                 const osb_observability* __restrict__ obs, uint8_t* __restrict__ mask,
+                                 double* __restrict__ yaw) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n_nodes) return;
+  const int d = b < *n_blk ? blk_drone[b] : -1;
+  const bool m = d >= 0 && d != self_id && obs->to_init[d];
+  mask[b] = m ? 1 : 0;
+  yaw[b] = m ? quat_yaw(blk_q + 4 * (size_t)b) : 0.0;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -520,6 +534,14 @@ struct osb_anchor {
   osb_observability* d_obs = nullptr;
   cudaEvent_t last_observe = nullptr;             // recorded after every observe, on its stream
   ObserveWindow obs_win{};                        // the host's, kept by set_window whether or not observe ever ran
+  // init_mask_dev: every window block's drone (-1: no entry) and its latest frame's self_pose quaternion, derived by
+  // set_window on the host; the first init_mask_dev acquires the device copy (and its length), set_window keeps it current
+  std::vector<int32_t> blk_drone;
+  std::vector<double> blk_q;                      // [block][4] qw qx qy qz
+  bool blk_negative = false;                      // a window entry with block < 0
+  int32_t* d_blk_drone = nullptr;                 // [blk_cap], then the table's length
+  double* d_blk_q = nullptr;
+  size_t blk_cap = 0;
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -578,6 +600,31 @@ osb_status anchor_settle(osb_anchor* h) {
   h->upper = h->n_loops + h->n_dets;
   h->fb.pending = false;
   h->fb.exact();
+  return OSB_OK;
+}
+
+// the block table to the device: acquired at max_window_entries blocks (or the window's, if more), replaced by a larger one
+// only when the window's block ids outgrow it.  The handle's stream is idle: the callers have waited for the last run and
+// observe and synchronised.
+osb_status upload_blocks(osb_anchor* h) {
+  const size_t n_blk = h->blk_drone.size();
+  if (!h->d_blk_drone || n_blk > h->blk_cap) {
+    const size_t cap = std::max(n_blk, (size_t)h->p.max_window_entries);
+    int32_t* drone = nullptr;
+    double* q = nullptr;
+    OSB_TRY(h->res.alloc(&drone, cap + 1));
+    OSB_TRY(h->res.alloc(&q, 4 * cap));
+    if (h->d_blk_drone) { h->res.release(h->d_blk_drone); h->res.release(h->d_blk_q); }
+    h->d_blk_drone = drone; h->d_blk_q = q; h->blk_cap = cap;
+  }
+  const int32_t len = (int32_t)n_blk;
+  cudaStream_t st = h->stream;
+  if (n_blk > 0) {
+    OSB_CUDA(cudaMemcpyAsync(h->d_blk_drone, h->blk_drone.data(), n_blk * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_blk_q, h->blk_q.data(), 4 * n_blk * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
+  OSB_CUDA(cudaMemcpyAsync(h->d_blk_drone + h->blk_cap, &len, sizeof(len), cudaMemcpyHostToDevice, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
 }
 
@@ -776,6 +823,21 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
     }
   const int n_vo = first[D];
   observe_window(h->obs_win, D, n_frames, n_entries, entries);
+  // every entry, vo_available or not; frames in order, so a shared block keeps its latest frame's pose
+  int n_blk = 0;
+  h->blk_negative = false;
+  for (int e = 0; e < n_entries; ++e) {
+    h->blk_negative = h->blk_negative || entries[e].block < 0;
+    n_blk = std::max(n_blk, entries[e].block + 1);
+  }
+  h->blk_drone.assign(n_blk, -1);
+  h->blk_q.assign(4 * (size_t)n_blk, 0.0);
+  for (int e = 0; e < n_entries; ++e) {
+    const int b = entries[e].block;
+    if (b < 0) continue;
+    h->blk_drone[b] = entries[e].drone_id;
+    std::copy(entries[e].self_pose + 3, entries[e].self_pose + 7, h->blk_q.begin() + 4 * (size_t)b);
+  }
   OSB_TRY(anchor_wait_last_run(h));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemcpyAsync(h->d_drone_first, first.data(), (size_t)(D + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -788,6 +850,7 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
     OSB_CUDA(cudaMemcpyAsync(h->d_win_pose, h->h_win_pose.data(), (size_t)n_vo * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
   }
   OSB_CUDA(cudaStreamSynchronize(st));
+  if (h->d_blk_drone) OSB_TRY(upload_blocks(h));
   h->n_frames = n_frames;
   h->frame0_stamp = n_frames > 0 ? frame_stamps_ns[0] : 0;
   return OSB_OK;
@@ -981,5 +1044,27 @@ extern "C" osb_status osb_anchor_observability(osb_anchor* h, osb_observability*
   OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
   OSB_CUDA(cudaMemcpyAsync(out, h->d_obs, sizeof(*out), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, int n_nodes, uint8_t* mask_dev,
+                                               double* yaw_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr && mask_dev != nullptr && yaw_dev != nullptr, "null argument");
+  OSB_REQUIRE(n_nodes >= 1, "n_nodes must be >= 1");
+  OSB_REQUIRE(drone_ok(h, self_id), "self_id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->d_obs != nullptr, "no osb_anchor_observe_dev call on this handle: to_init is not set");
+  OSB_REQUIRE(!h->blk_negative && h->blk_drone.size() <= (size_t)n_nodes, "a window block outside 0..n_nodes-1");
+  DeviceGuard dg(h->device);
+  if (!h->d_blk_drone) {                                          // the first call acquires the table
+    OSB_TRY(anchor_wait_last_run(h));
+    OSB_TRY(upload_blocks(h));
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // to_init is the last observe's
+  OSB_LAUNCH(init_mask_kernel, cdiv(n_nodes, 256), 256, 0, st, h->d_blk_drone, h->d_blk_q, h->d_blk_drone + h->blk_cap,
+             n_nodes, self_id, h->d_obs, mask_dev, yaw_dev);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
   return OSB_OK;
 }

@@ -220,7 +220,8 @@ struct SolverDev {
   int ctas;                // CTAs per solve (the cluster size on the cluster path)
   int first_trial;
   long long tstride;
-  // device tail (osb_solver_solve_resident_dev, graph_solve_kernel<T, false, true>): [0] status of the call's tables
+  // device tail (osb_solver_solve_resident_dev, graph_solve_kernel<T, false, true>; with several trials,
+  // osb_solver_solve_multistart_resident_dev, graph_solve_kernel<T, true, true>): [0] status of the call's tables
   // (non-zero: refused, nothing runs), [1] m = resident factors + tail, [2] fpc = ceil(m / ctas).  m and fpc above are
   // then the bounds the launch shape was picked for.
   const int32_t* dev_word;
@@ -559,8 +560,9 @@ __device__ __forceinline__ void factor_apply(const JStore<T>& J, int li, const T
   }
 }
 
-// DT: one solve whose factor list ends in a device-side tail (osb_solver_solve_resident_dev).  The factor count and the
-// CTA blocks come from P.dev_word, and a refused call leaves on every CTA before the first barrier.
+// DT: a solve whose factor list ends in a device-side tail (osb_solver_solve_resident_dev; with MT, every trial of
+// osb_solver_solve_multistart_resident_dev).  The factor count and the CTA blocks come from P.dev_word, and a refused call
+// leaves on every CTA before the first barrier.
 template <typename T, bool MT, bool DT = false>
 __global__ void __launch_bounds__(GS_THREADS, 1)
 graph_solve_kernel(SolverDev P) {
@@ -1034,6 +1036,31 @@ __global__ void multistart_init_kernel(int n, int n_trials, const uint8_t* __res
   }
 }
 
+// The same scatter on the device chain (osb_solver_solve_multistart_resident_dev), a sibling so that the kernel above keeps
+// its code: the mask read from the caller's device buffer and, with yaw != nullptr, a scattered node's yaw set to
+// yaw[node] in every trial (the odometry yaw of random_init_pose, :212; trial 0 then writes the whole pose, still
+// race-free).  Nothing is written when the call's tail was refused (status: the tail tables' word).
+__global__ void multistart_init_dev_kernel(int n, int n_trials, const int32_t* __restrict__ status,
+                                           const uint8_t* __restrict__ fixed, const int32_t* __restrict__ order,
+                                           const uint8_t* __restrict__ mask, const double* __restrict__ yaw, uint64_t seed,
+                                           double rand_xy, double rand_z, double* x0, long long tstride) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * n_trials || __ldcg(status) != OSB_OK) return;
+  const int t = (int)(idx / n), i = (int)(idx - (long long)t * n);
+  const int node = order[i];
+  double* dst = reinterpret_cast<double*>(reinterpret_cast<char*>(x0) + t * tstride) + 4 * (size_t)i;
+  const double* src = x0 + 4 * (size_t)i;
+  if (mask[node] && !fixed[i]) {
+    dst[0] = multistart_draw(seed, t, node, 0, rand_xy);
+    dst[1] = multistart_draw(seed, t, node, 1, rand_xy);
+    dst[2] = multistart_draw(seed, t, node, 2, rand_z);
+    if (yaw != nullptr) dst[3] = yaw[node];
+    else if (t > 0) dst[3] = src[3];
+  } else if (t > 0) {
+    for (int k = 0; k < 4; ++k) dst[k] = src[k];
+  }
+}
+
 // What a call brings back to the host, followed by the poses [n][4] in internal order.  The selection kernel fills one
 // on the device and one copy moves it into the handle's pinned mirror; a single solve stages its poses (in and out) and
 // its summary in that mirror.
@@ -1048,27 +1075,58 @@ struct SolveResults {
 // One warp.  equv_cost of every trial (solver.cpp:1721-1725), the acceptance walk of solve_with_multiple_init
 // (:783-831: best starts at acpt_cost, strictly lower wins, so the first of equal minima is kept and a NaN never is),
 // then the chosen trial's poses.  summary0 / out0: trial 0's summary and output poses, trial t's lie t * tstride further.
+__device__ __forceinline__ int multistart_rank(int n_trials, const osb_solve_summary* __restrict__ summary0,
+                                               long long tstride, int normalise, int n_res, int window, double acpt_cost,
+                                               SolveResults* __restrict__ res) {
+  int c = -1;
+  double best = acpt_cost;
+  for (int t = 0; t < n_trials; ++t) {
+    const osb_solve_summary sm =
+        *reinterpret_cast<const osb_solve_summary*>(reinterpret_cast<const char*>(summary0) + t * tstride);
+    const double e = normalise ? sqrt(sm.final_cost) / (double)n_res / (double)window : sm.final_cost;
+    res->equv[t] = e;
+    res->summaries[t] = sm;
+    if (e < best) { best = e; c = t; }
+  }
+  res->chosen = c;
+  return c;
+}
+
 __global__ void multistart_select_kernel(int n_trials, int n, const osb_solve_summary* __restrict__ summary0,
                                          const double* __restrict__ out0, long long tstride, int normalise, int n_res,
                                          int window, double acpt_cost, SolveResults* __restrict__ res) {
   const int lane = threadIdx.x;
   int c = -1;
-  if (lane == 0) {
-    double best = acpt_cost;
-    for (int t = 0; t < n_trials; ++t) {
-      const osb_solve_summary sm =
-          *reinterpret_cast<const osb_solve_summary*>(reinterpret_cast<const char*>(summary0) + t * tstride);
-      const double e = normalise ? sqrt(sm.final_cost) / (double)n_res / (double)window : sm.final_cost;
-      res->equv[t] = e;
-      res->summaries[t] = sm;
-      if (e < best) { best = e; c = t; }
-    }
-    res->chosen = c;
-  }
+  if (lane == 0) c = multistart_rank(n_trials, summary0, tstride, normalise, n_res, window, acpt_cost, res);
   c = __shfl_sync(0xffffffffu, c, 0);
   if (c < 0) return;
   const double* src = reinterpret_cast<const double*>(reinterpret_cast<const char*>(out0) + c * tstride);
   for (int i = lane; i < 4 * n; i += 32) res->poses()[i] = src[i];
+}
+
+// The selection on the device chain (osb_solver_solve_multistart_resident_dev), one CTA: n_res = the resident residuals
+// (base_res) + the tail's (word[3]), and the chosen trial's poses go into the resident pose copy in caller order (order:
+// internal -> caller).  A refused tail (word[0] != OSB_OK) ran no trial: chosen = -1, nothing else written.
+__global__ void __launch_bounds__(256)
+multistart_select_dev_kernel(int n_trials, int n, const osb_solve_summary* __restrict__ summary0,
+                             const double* __restrict__ out0, long long tstride, int normalise,
+                             const int32_t* __restrict__ word, int base_res, int window, double acpt_cost,
+                             SolveResults* __restrict__ res, const int32_t* __restrict__ order, double* __restrict__ rposes) {
+  __shared__ int chosen;
+  if (threadIdx.x == 0) {
+    chosen = __ldcg(word) != OSB_OK ? -1
+             : multistart_rank(n_trials, summary0, tstride, normalise, base_res + __ldcg(word + 3), window, acpt_cost, res);
+    if (chosen < 0) res->chosen = -1;
+  }
+  __syncthreads();
+  const int c = chosen;
+  if (c < 0) return;
+  const double* src = reinterpret_cast<const double*>(reinterpret_cast<const char*>(out0) + c * tstride);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int dst = order[i];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) rposes[4 * dst + q] = __ldcg(src + 4 * i + q);
+  }
 }
 
 // ---- device tail (osb_solver_solve_resident_dev) ---------------------------------------------------------------------
@@ -1279,6 +1337,8 @@ struct SolveShape {
   const void* kern;      // one solve per launch
   const void* kern_multi;  // several clusters per launch, one trial each (same resources, same arithmetic)
   const void* kern_dt;     // one solve whose factor count is read on the device (osb_solver_solve_resident_dev)
+  const void* kern_multi_dt;  // both: one trial per cluster, the factor count read on the device
+                              // (osb_solver_solve_multistart_resident_dev)
   int cluster;           // 1: one thread-block cluster per solve (hardware barrier); 0: one cooperative grid per launch
   int ctas, fpc, chain, jsmem;
   size_t smem;           // dynamic shared memory per CTA
@@ -1363,6 +1423,12 @@ struct osb_solver {
   bool dev_pending = false, dev_captured = false, dev_called = false;
   osb_status dev_status = OSB_OK;
   osb_solve_summary dev_summary = {};
+  // ... when it was osb_solver_solve_multistart_resident_dev: its n_trials (0: a single solve) and, once refreshed, what
+  // osb_solver_last_multistart returns
+  int dev_trials = 0;
+  std::vector<osb_solve_summary> dev_ms_summaries;
+  std::vector<double> dev_ms_equv;
+  int32_t dev_ms_chosen = -1;
 };
 
 static osb_status finish_device_call(osb_solver* h);
@@ -1394,7 +1460,9 @@ extern "C" osb_status osb_solver_create(osb_solver** out, int max_nodes, int max
   for (const void* k : {(const void*)graph_solve_kernel<float, false>, (const void*)graph_solve_kernel<double, false>,
                         (const void*)graph_solve_kernel<float, true>, (const void*)graph_solve_kernel<double, true>,
                         (const void*)graph_solve_kernel<float, false, true>,
-                        (const void*)graph_solve_kernel<double, false, true>}) {
+                        (const void*)graph_solve_kernel<double, false, true>,
+                        (const void*)graph_solve_kernel<float, true, true>,
+                        (const void*)graph_solve_kernel<double, true, true>}) {
     OSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_DYN_MAX));
     h->cluster_ok = h->cluster_ok && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
   }
@@ -1621,6 +1689,7 @@ static osb_status solve_shape(const osb_solver* h, int n_nodes, int n_factors, c
   s.kern = s.f32 ? (const void*)graph_solve_kernel<float, false> : (const void*)graph_solve_kernel<double, false>;
   s.kern_multi = s.f32 ? (const void*)graph_solve_kernel<float, true> : (const void*)graph_solve_kernel<double, true>;
   s.kern_dt = s.f32 ? (const void*)graph_solve_kernel<float, false, true> : (const void*)graph_solve_kernel<double, false, true>;
+  s.kern_multi_dt = s.f32 ? (const void*)graph_solve_kernel<float, true, true> : (const void*)graph_solve_kernel<double, true, true>;
   s.chain = 0;
   // ONE thread-block cluster (hardware barrier, ~0.2 us) when the factor list fits 16 CTAs with their Jacobians in
   // shared memory; otherwise a cooperative grid (software grid barrier).
@@ -1671,10 +1740,11 @@ static SolverDev graph_dev(const osb_solver* h, int n_nodes, int n_factors, cons
 
 // n_trials solves of one shape, P bound at trial 0 = the start of the arena, trial t's block tstride bytes further.
 // Cluster path: ONE launch of n_trials clusters (clusters do not wait for each other, so the grid may exceed what is
-// resident).  Cooperative path: one grid per trial, in order on the stream.  dt: the one solve of
-// osb_solver_solve_resident_dev, on the caller's stream `st`.
+// resident).  Cooperative path: one grid per trial, in order on the stream.  dt: the factor count is read on the device
+// (the solves of osb_solver_solve_resident_dev and osb_solver_solve_multistart_resident_dev, on the caller's stream `st`).
+// own_summary: every trial writes P.summary instead of its own block's (the one solve of osb_solver_solve_resident_dev).
 static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s, int n_trials, long long tstride,
-                                cudaStream_t st, bool dt = false) {
+                                cudaStream_t st, bool dt = false, bool own_summary = false) {
   P.fpc = s.fpc; P.use_cluster = s.cluster; P.j_in_smem = s.jsmem; P.use_chain = s.chain;
   P.ctas = s.ctas; P.first_trial = 0; P.tstride = tstride;
   h->last_shape = s;
@@ -1683,12 +1753,13 @@ static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s,
   cfg.blockDim = dim3(GS_THREADS); cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
   cfg.dynamicSmemBytes = s.smem;
   const void* single = dt ? s.kern_dt : s.kern;
+  const void* multi = dt ? s.kern_multi_dt : s.kern_multi;
   if (s.cluster) {
     cfg.gridDim = dim3(n_trials * s.ctas);
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = s.ctas; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     void* kargs[1] = {&P};
-    OSB_CUDA(cudaLaunchKernelExC(&cfg, n_trials > 1 ? s.kern_multi : single, kargs));
+    OSB_CUDA(cudaLaunchKernelExC(&cfg, n_trials > 1 ? multi : single, kargs));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return OSB_OK;
   }
@@ -1699,7 +1770,7 @@ static osb_status launch_solves(osb_solver* h, SolverDev P, const SolveShape& s,
     SolverDev Q = P;
     Q.first_trial = t;
     trial_layout(Q, h->d_arena + t * tstride, P.n, P.m, s);
-    if (dt) Q.summary = P.summary;
+    if (own_summary) Q.summary = P.summary;
     void* kargs[1] = {&Q};
     OSB_CUDA(cudaLaunchKernelExC(&cfg, single, kargs));
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1993,17 +2064,27 @@ static osb_status finish_device_call(osb_solver* h) {
   int32_t word[4];
   osb_solve_summary sm;
   cudaStream_t st = h->stream;
+  const int K = h->dev_trials;
   OSB_CUDA(cudaMemcpyAsync(word, h->tail.word, sizeof(word), cudaMemcpyDeviceToHost, st));
-  OSB_CUDA(cudaMemcpyAsync(&sm, h->d_tsummary, sizeof(sm), cudaMemcpyDeviceToHost, st));
+  if (K > 0) OSB_CUDA(cudaMemcpyAsync(h->h_res, h->d_res, sizeof(SolveResults), cudaMemcpyDeviceToHost, st));
+  else OSB_CUDA(cudaMemcpyAsync(&sm, h->d_tsummary, sizeof(sm), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaMemcpyAsync(h->g_poses.data(), h->d_rposes, h->g_poses.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   h->dev_status = (osb_status)word[0];
   if (h->dev_status == OSB_OK) {
     float msec = 0.f;
     if (!h->dev_captured) OSB_CUDA(cudaEventElapsedTime(&msec, h->ev0, h->ev1));
-    sm.solve_ms = msec;
-    sm.n_residuals = h->tail_nres + word[3];
-    h->dev_summary = sm;
+    if (K > 0) {
+      const SolveResults* r = h->h_res;
+      h->dev_ms_summaries.assign(r->summaries, r->summaries + K);
+      for (osb_solve_summary& t : h->dev_ms_summaries) { t.solve_ms = msec; t.n_residuals = h->tail_nres + word[3]; }
+      h->dev_ms_equv.assign(r->equv, r->equv + K);
+      h->dev_ms_chosen = r->chosen;
+    } else {
+      sm.solve_ms = msec;
+      sm.n_residuals = h->tail_nres + word[3];
+      h->dev_summary = sm;
+    }
   }
   return OSB_OK;
 }
@@ -2024,12 +2105,13 @@ static osb_status flush_resident_factors(osb_solver* h) {
   return OSB_OK;
 }
 
-extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev,
-                                                    const int32_t* ia_dev, const int32_t* ib_dev, const double* payload_dev,
-                                                    const uint8_t* huber_dev, const int32_t* count_dev,
-                                                    const osb_solve_options* opt, void* stream) {
-  OSB_REQUIRE(h && type_dev && ia_dev && ib_dev && payload_dev && huber_dev && count_dev, "null argument");
-  OSB_REQUIRE(max_tail >= 0, "max_tail must be >= 0");
+// One device call on the resident window plus a device tail: the single solve of osb_solver_solve_resident_dev (ms ==
+// nullptr) or the ms->n_trials restarts of osb_solver_solve_multistart_resident_dev.  The arguments are checked.
+static osb_status resident_dev_call(osb_solver* h, int max_tail, const int32_t* type_dev, const int32_t* ia_dev,
+                                    const int32_t* ib_dev, const double* payload_dev, const uint8_t* huber_dev,
+                                    const int32_t* count_dev, const osb_solve_options* opt, void* stream,
+                                    const osb_multistart_options* ms, const uint8_t* mask_dev, const double* yaw_dev) {
+  const char* fn = ms ? "osb_solver_solve_multistart_resident_dev" : "osb_solver_solve_resident_dev";
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   cudaStream_t st = (cudaStream_t)stream;
@@ -2037,9 +2119,9 @@ extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail,
   OSB_CUDA(cudaStreamIsCapturing(st, &cap));
   const bool capturing = cap != cudaStreamCaptureStatusNone;
   const size_t n = h->g_fixed.size(), m_base = h->g_type.size();
-  OSB_REQUIRE(n > 0 && m_base > 0, "the resident graph is empty");
+  if (n == 0 || m_base == 0) { set_error(fn, "the resident graph is empty"); return OSB_ERR_INVALID; }
   if (m_base + (size_t)max_tail > (size_t)h->max_factors) {
-    set_error("osb_solver_solve_resident_dev", "resident factors + max_tail exceed the solver capacity");
+    set_error(fn, "resident factors + max_tail exceed the solver capacity");
     return OSB_ERR_CAPACITY;
   }
   osb_solve_options o;
@@ -2052,7 +2134,7 @@ extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail,
   const bool host_work = h->d_tail == nullptr || h->tail_topo != h->g_topo_version || !h->g_static_valid ||
                          h->g_uploaded < m_base || !h->rposes_current || shape_key != h->tail_shape_key;
   if (capturing && (host_work || !h->tail_shape.cluster)) {
-    set_error("osb_solver_solve_resident_dev", capturing && !host_work
+    set_error(fn, capturing && !host_work
               ? "the cooperative path cannot be captured"
               : "a captured call cannot do host work: run the call once outside the capture after the graph changed");
     return OSB_ERR_INVALID;
@@ -2103,9 +2185,23 @@ extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail,
     OSB_CUDA(cudaStreamSynchronize(hs));       // the staging vectors above die here; the caller's stream comes after
   }
   const SolveShape& shape = h->tail_shape;
+  const int K = ms ? ms->n_trials : 1;
   SolverDev P = graph_dev(h, (int)n, m_bound, o);
+  const size_t tstride = trial_layout(P, nullptr, n, m_bound, shape);
+  if ((size_t)K * tstride > h->arena_bytes) {  // multistart only, as in solver_run
+    if (capturing) {
+      set_error(fn, "growing the arena to n_trials solves is host work: run the call once outside the capture");
+      return OSB_ERR_INVALID;
+    }
+    if (h->dev_pending && !h->dev_captured) OSB_CUDA(cudaEventSynchronize(h->ev_done));   // the last call's arena
+    char* grown = nullptr;
+    OSB_TRY(h->res.alloc(&grown, K * tstride));
+    h->res.release(h->d_arena);
+    h->d_arena = grown;
+    h->arena_bytes = K * tstride;
+  }
   trial_layout(P, h->d_arena, n, m_bound, shape);
-  P.summary = h->d_tsummary;
+  if (!ms) P.summary = h->d_tsummary;
   P.dev_word = h->tail.word;
   TailDev D = h->tail;
   D.n = (int)n; D.m_base = (int)m_base; D.max_tail = max_tail; D.ctas = shape.ctas;
@@ -2124,13 +2220,75 @@ extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail,
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(tail_tables_kernel, cdiv(std::max(m_bound, (int)n), 256), 256, 0, st, D);
   OSB_CHECK_LAUNCH();
+  if (ms) {
+    const long long kn = (long long)K * (long long)n;
+    OSB_LAUNCH(multistart_init_dev_kernel, (unsigned)((kn + 255) / 256), 256, 0, st, (int)n, K, D.word, D.b_fixed, D.order,
+               mask_dev, yaw_dev, ms->seed, ms->rand_xy, ms->rand_z, P.x[0], (long long)tstride);
+    OSB_CHECK_LAUNCH();
+  }
   if (!capturing) OSB_CUDA(cudaEventRecord(h->ev0, st));
-  OSB_TRY(launch_solves(h, P, shape, 1, 0, st, true));
+  OSB_TRY(launch_solves(h, P, shape, K, (long long)tstride, st, true, !ms));
   if (!capturing) OSB_CUDA(cudaEventRecord(h->ev1, st));
-  OSB_LAUNCH(tail_poses_out_kernel, cdiv((int)n, 256), 256, 0, st, D);
+  if (ms) {
+    OSB_LAUNCH(multistart_select_dev_kernel, 1, 256, 0, st, K, (int)n, P.summary, P.poses_out, (long long)tstride,
+               ms->normalise ? 1 : 0, D.word, h->tail_nres, ms->window_size, ms->acpt_cost, h->d_res, D.order, D.poses);
+  } else {
+    OSB_LAUNCH(tail_poses_out_kernel, cdiv((int)n, 256), 256, 0, st, D);
+  }
   OSB_CHECK_LAUNCH();
   if (!capturing) OSB_CUDA(cudaEventRecord(h->ev_done, st));
   h->dev_pending = true; h->dev_captured = capturing; h->dev_called = true;
+  h->dev_trials = ms ? K : 0;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_solver_solve_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev,
+                                                    const int32_t* ia_dev, const int32_t* ib_dev, const double* payload_dev,
+                                                    const uint8_t* huber_dev, const int32_t* count_dev,
+                                                    const osb_solve_options* opt, void* stream) {
+  OSB_REQUIRE(h && type_dev && ia_dev && ib_dev && payload_dev && huber_dev && count_dev, "null argument");
+  OSB_REQUIRE(max_tail >= 0, "max_tail must be >= 0");
+  return resident_dev_call(h, max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev, count_dev, opt, stream, nullptr,
+                           nullptr, nullptr);
+}
+
+// ---- random-restart initialisation on the device chain: solve_with_multiple_init (solver.cpp:781-845) of the resident
+// window plus the device tail, the trials started from the resident device poses with the caller's device mask
+extern "C" osb_status osb_solver_solve_multistart_resident_dev(osb_solver* h, int max_tail, const int32_t* type_dev,
+                                                               const int32_t* ia_dev, const int32_t* ib_dev,
+                                                               const double* payload_dev, const uint8_t* huber_dev,
+                                                               const int32_t* count_dev, const uint8_t* init_mask_dev,
+                                                               const double* init_yaw_dev, const osb_solve_options* opt,
+                                                               const osb_multistart_options* ms, void* stream) {
+  OSB_REQUIRE(h && type_dev && ia_dev && ib_dev && payload_dev && huber_dev && count_dev && init_mask_dev && ms,
+              "null argument");
+  OSB_REQUIRE(max_tail >= 0, "max_tail must be >= 0");
+  OSB_REQUIRE(ms->n_trials >= 1 && ms->n_trials <= MS_MAX_TRIALS, "n_trials must be 1 ... 256");
+  OSB_REQUIRE(!ms->normalise || ms->window_size >= 1, "window_size must be >= 1 when normalise is set");
+  OSB_REQUIRE(std::isfinite(ms->rand_xy) && ms->rand_xy >= 0.0 && std::isfinite(ms->rand_z) && ms->rand_z >= 0.0,
+              "rand_xy and rand_z must be finite and >= 0");
+  OSB_REQUIRE(!std::isnan(ms->acpt_cost), "acpt_cost is NaN");
+  return resident_dev_call(h, max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev, count_dev, opt, stream, ms,
+                           init_mask_dev, init_yaw_dev);
+}
+
+extern "C" osb_status osb_solver_last_multistart(osb_solver* h, osb_solve_summary* summaries, double* equv,
+                                                 int32_t* chosen) {
+  OSB_REQUIRE(h != nullptr && summaries != nullptr && equv != nullptr && chosen != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(finish_device_call(h));
+  OSB_REQUIRE(h->dev_called && h->dev_trials > 0,
+              "the last device call was not osb_solver_solve_multistart_resident_dev (osb_solver_last_summary reads it)");
+  if (h->dev_status != OSB_OK) {
+    set_error("osb_solver_last_multistart", h->dev_status == OSB_ERR_CAPACITY
+              ? "the device call was refused: *count_dev > max_tail"
+              : "the device call was refused: a tail row has an unknown type or a bad node id, or *count_dev < 0");
+    return h->dev_status;
+  }
+  std::copy(h->dev_ms_summaries.begin(), h->dev_ms_summaries.end(), summaries);
+  std::copy(h->dev_ms_equv.begin(), h->dev_ms_equv.end(), equv);
+  *chosen = h->dev_ms_chosen;
   return OSB_OK;
 }
 
@@ -2140,6 +2298,8 @@ extern "C" osb_status osb_solver_last_summary(osb_solver* h, osb_solve_summary* 
   DeviceGuard dg(h->device);
   OSB_TRY(finish_device_call(h));
   OSB_REQUIRE(h->dev_called, "no osb_solver_solve_resident_dev call on this handle");
+  OSB_REQUIRE(h->dev_trials == 0,
+              "the last device call was osb_solver_solve_multistart_resident_dev: osb_solver_last_multistart reads it");
   if (h->dev_status != OSB_OK) {
     set_error("osb_solver_last_summary", h->dev_status == OSB_ERR_CAPACITY
               ? "the device call was refused: *count_dev > max_tail"

@@ -373,6 +373,33 @@ class PoseGraphSolver(_Handle):
         _l.check(self._lib.osb_solver_last_summary(self._h, C.byref(summ)))
         return summ
 
+    def solve_multistart_resident_dev(self, max_tail: int, type_ptr: int, ia_ptr: int, ib_ptr: int, payload_ptr: int,
+                                      huber_ptr: int, count_ptr: int, mask_ptr: int, yaw_ptr, stream: int, n_trials: int,
+                                      seed: int, window_size: int, acpt_cost: float, normalise: bool = True,
+                                      options: _l.SolveOptions | None = None, rand_xy: float = 5.0, rand_z: float = 1.0):
+        """solve_multistart of the resident graph plus *count_ptr tail rows read on the device, started from the resident
+        device poses, the nodes of the uint8 device mask at mask_ptr scattered (yaw from the float64 device array at
+        yaw_ptr, or kept when it is None), on `stream` without synchronising; the chosen poses stay on the device until a
+        host-side call (see last_multistart)"""
+        opt = options if options is not None else self.default_options()
+        ms = _l.MultistartOptions(n_trials=int(n_trials), normalise=int(normalise), window_size=int(window_size),
+                                  seed=int(seed), rand_xy=rand_xy, rand_z=rand_z, acpt_cost=acpt_cost)
+        _l.check(self._lib.osb_solver_solve_multistart_resident_dev(
+            self._h, int(max_tail), C.c_void_p(type_ptr), C.c_void_p(ia_ptr), C.c_void_p(ib_ptr), C.c_void_p(payload_ptr),
+            C.c_void_p(huber_ptr), C.c_void_p(count_ptr), C.c_void_p(mask_ptr),
+            None if yaw_ptr is None else C.c_void_p(yaw_ptr), C.byref(opt), C.byref(ms), C.c_void_p(stream)))
+        self._ms_trials = int(n_trials)
+
+    def last_multistart(self):
+        """synchronises with the last solve_multistart_resident_dev call -> (chosen, summaries, equv), as
+        solve_multistart returns them (raises its refusal code)"""
+        k = max(1, getattr(self, "_ms_trials", 1))
+        summ = (_l.SolveSummary * k)()
+        equv = np.zeros(k, np.float64)
+        chosen = C.c_int32(-2)
+        _l.check(self._lib.osb_solver_last_multistart(self._h, C.cast(summ, C.c_void_p), _l.ptr(equv), C.byref(chosen)))
+        return int(chosen.value), list(summ), equv
+
     def phase_cycles(self) -> dict:
         c = np.zeros(12, np.float64)
         _l.check(self._lib.osb_solver_phase_cycles(self._h, _l.ptr(c)))
@@ -959,6 +986,12 @@ class LoopAnchor(_Handle):
         p = _l.ObserveParams(int(self_id), float(init_xy_movement), float(init_z_movement), 0)
         _l.check(self._lib.osb_anchor_observe_dev(self._h, C.byref(p), C.c_void_p(rows_ptr), int(n), C.c_void_p(stream)))
 
+    def init_mask_dev(self, self_id: int, n_nodes: int, mask_ptr: int, yaw_ptr: int, stream: int):
+        """random_init_pose's blocks from the window and the last observe_dev's to_init (osb_anchor_init_mask_dev): uint8
+        mask [n_nodes] at mask_ptr and float64 odometry yaw [n_nodes] at yaw_ptr, on `stream` without synchronising"""
+        _l.check(self._lib.osb_anchor_init_mask_dev(self._h, int(self_id), int(n_nodes), C.c_void_p(mask_ptr),
+                                                    C.c_void_p(yaw_ptr), C.c_void_p(stream)))
+
     def observability(self) -> dict:
         """waits for the last observe_dev -> its outcome: bool arrays [max_drones] nodes, yaw, pos, enable, to_init and
         the flags solve_master, motion, motion_new"""
@@ -1066,6 +1099,7 @@ class AnchoredChain:
         self.rows = torch.zeros(cap * _l.ANCHOR_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
         self.keep = torch.zeros(cap, dtype=torch.uint8, device="cuda")
         self.factors = FactorRows(cap)
+        self.mask = self.yaw = None                                  # init_mask's buffers, acquired by its first call
         self.stream = torch.cuda.Stream() if stream is None else stream
         self.stream.wait_stream(torch.cuda.current_stream())        # the buffers are zeroed on the current stream
 
@@ -1093,6 +1127,24 @@ class AnchoredChain:
 
     def solve(self, solver: PoseGraphSolver, max_tail: int, options=None):
         self.factors.solve(solver, max_tail, options, self.stream)
+
+    def init_mask(self, anchor: LoopAnchor, self_id: int, n_nodes: int):
+        """the init branch's mask and yaw of n_nodes blocks into the chain's buffers (LoopAnchor.init_mask_dev), after
+        observe; the buffers are (re)acquired on the current stream when n_nodes outgrows them"""
+        import torch
+        if self.mask is None or self.mask.numel() < n_nodes:
+            self.mask = torch.zeros(n_nodes, dtype=torch.uint8, device="cuda")
+            self.yaw = torch.zeros(n_nodes, dtype=torch.float64, device="cuda")
+            self.stream.wait_stream(torch.cuda.current_stream())
+        anchor.init_mask_dev(self_id, n_nodes, self.mask.data_ptr(), self.yaw.data_ptr(), self.stream.cuda_stream)
+
+    def init_solve(self, solver: PoseGraphSolver, max_tail: int, n_trials: int, seed: int, window_size: int,
+                   acpt_cost: float, normalise: bool = True, options=None):
+        """the init branch's last step: solver.solve_multistart_resident_dev with the chain's rows as its tail and
+        init_mask's mask and yaw, on the chain's stream"""
+        solver.solve_multistart_resident_dev(max_tail, *self.factors.ptrs(), self.mask.data_ptr(), self.yaw.data_ptr(),
+                                             self.stream.cuda_stream, n_trials, seed, window_size, acpt_cost, normalise,
+                                             options)
 
     def keep_on_host(self, n: int) -> np.ndarray:
         import torch

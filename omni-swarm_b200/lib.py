@@ -268,6 +268,9 @@ _SIG = {
     "osb_solver_solve_resident": (C.c_int, [_P, _P, _P]),
     "osb_solver_solve_resident_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "osb_solver_last_summary": (C.c_int, [_P, _P]),
+    "osb_solver_solve_multistart_resident_dev": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                           C.POINTER(SolveOptions), C.POINTER(MultistartOptions), _P]),
+    "osb_solver_last_multistart": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32)]),
     "osb_solver_phase_cycles": (C.c_int, [_P, _P]),
     "osb_solver_chain_cycles": (C.c_int, [_P, _P]),
     "osb_solver_chain_plan": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
@@ -339,6 +342,7 @@ _SIG = {
     "osb_anchor_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "osb_anchor_observe_dev": (C.c_int, [_P, C.POINTER(ObserveParams), _P, C.c_int, _P]),
     "osb_anchor_observability": (C.c_int, [_P, C.POINTER(Observability)]),
+    "osb_anchor_init_mask_dev": (C.c_int, [_P, C.c_int32, C.c_int, _P, _P, _P]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
