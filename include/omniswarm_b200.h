@@ -693,6 +693,80 @@ osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out);
  *   outside 0 .. n_nodes-1, self_id outside 0..max_drones-1, or no observe_dev since create. */
 osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, int n_nodes, uint8_t* mask_dev, double* yaw_dev,
                                     void* stream);
+/* osb_anchor_sync_dev(): SwarmLocalizationSolver::sync_est_poses (swarm_localization_solver.cpp:962-1057) on the device,
+ *   after the solver's last device call (osb_solver_solve_resident_dev or osb_solver_solve_multistart_resident_dev), on
+ *   `stream` without synchronising.  It is ordered after that call on any stream, also inside a CUDA graph.
+ *   Applied only if solve() would accept that call (:925, :947-951), decided on the device:
+ *     a single solve when its status is OK and !(equv > acpt_cost), equv = normalise ? sqrt(final_cost) / n_residuals /
+ *     window_size : final_cost, n_residuals = the resident factors' residuals + the device tail's;
+ *     a multistart when it chose a trial (chosen >= 0); the sync is then an init sync (is_init_solve).
+ *   A sync not applied changes no output and no state.  An applied sync, with the window set last and the solved poses
+ *   (x y z yaw) of its blocks:
+ *   keyframe path of drone d: one sample per window entry of d, in frame order, vo_available or not; stamp = the entry's
+ *     FRAME stamp; pose = Pose(block pose, yaw) with att = att * (AngleAxis(-yaw(ego), Z) * att(ego)), ego = d's odometry
+ *     at the frame stamp (nearest sample, as the re-anchoring looks it up).  Every path is rebuilt: a drone without a window
+ *     entry has none.  A quaternion of yaw y is quat_from_rotvec(0, 0, y), as everywhere in the back-end;
+ *   full path (full_path != 0) of every drone with a keyframe path: odometry samples i = 0, 10, 20, ... (FULL_PATH_STEP);
+ *     the keyframe sample nearest to the odometry stamp, the earlier one on ties (the reference's forward walk, bounded at
+ *     the last sample); pose = kf_pose * DeltaPose(vo_ref, ego_i, 4-DoF), then att = att * att_no_yaw(ego at the
+ *     keyframe's stamp), vo_ref = that keyframe entry's self_pose; stamp = the odometry stamp.  full_path == 0: no drone
+ *     has one (the reference clears full_trajs);
+ *   prediction record (est_poses_tsid_saved / last_saved_est_kf_ts, read by osb_anchor_predict): per drone, the last
+ *     pushed frame holding it, with its solved block pose and its entry's self_pose.  An init sync pushes every window
+ *     frame in order; a steady sync pushes the last frame that has entries.  A record whose frame is still in the window
+ *     is rewritten in place (the reference rewrites est_poses_tsid_saved of every window frame); once its frame has left,
+ *     it is frozen.  This equals the reference's reverse scan of last_saved_est_kf_ts as long as a frame stamp keeps the
+ *     drones it was first pushed with (a SwarmFrame does).
+ *   Refused on the device with every output and all state unchanged: a window drone without odometry (the reference
+ *   throws from ego_motion_trajs.at()) -- osb_anchor_sync_result reports OSB_ERR_INVALID.
+ *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer; self_id outside 0..max_drones-1; normalise
+ *   with window_size < 1; a NaN acpt_cost; the two handles on different devices; no solver device call since its last
+ *   host-side pose or graph change; a window block < 0 or >= the solver's node count.
+ *   Work: 3 launches whatever the window, the drone count or the trajectory lengths (one CTA decides, writes the record
+ *   and the path counts; one pass over the window entries writes the keyframe paths; a fixed grid-stride pass over
+ *   max_drones x ceil(max_traj_samples / 10) writes the full paths).  The trajectory counts and the window are read on the
+ *   device, so a captured sync follows push_odometry and set_window made between replays.
+ *   Memory: the first call acquires 136 E + 4 (D + 1) bytes of window table and keyframe paths, 64 D S10 + 4 D bytes of
+ *   full paths, 104 D bytes of records, about 1 KB of window counts and outcome, and an event (E = max_window_entries,
+ *   D = max_drones, S10 = ceil(max_traj_samples / 10); 6.5 MB for 5 drones, 2e5 samples and 2048 entries), and
+ *   synchronises; set_window keeps the table current after that.
+ *   Later calls acquire nothing and can be captured.  Each sync is ordered after the handle's last sync on any stream;
+ *   push_odometry and set_window wait for it as they wait for the last run.
+ *   self_id is checked only: the sync does not depend on it (the reference's does not either). */
+typedef struct {
+  int32_t self_id, full_path;
+  int32_t normalise, window_size;   /* the equv_cost rule of osb_multistart_options */
+  double acpt_cost;
+} osb_sync_params;
+osb_status osb_anchor_sync_dev(osb_anchor* h, osb_solver* s, const osb_sync_params* p, void* stream);
+/* osb_anchor_sync_result(): waits for the last sync -> *applied (1: applied, 0: not accepted, refused, or none ran) and
+ *   *last (OSB_OK, or OSB_ERR_INVALID for a window drone without odometry); returns OSB_OK. */
+osb_status osb_anchor_sync_result(osb_anchor* h, int32_t* applied, osb_status* last);
+/* osb_anchor_paths(): waits for the last sync and copies drone's keyframe path (full == 0) or full path (full != 0):
+ *   *n = its sample count, -1 when the drone has none (also before the first applied sync); min(*n, cap) samples of
+ *   stamps [ns] and poses7 [x y z qw qx qy qz] are written. */
+osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, int64_t* stamps, double* poses7, int cap, int32_t* n);
+/* osb_anchor_predict(): PredictSwarm / PredictNode / NodeCooridnateOffset (swarm_localization_solver.cpp:673-765) for one
+ *   frame of n drones (distinct ids, vo_poses7 [n][7] their odometry now), from the prediction record of the last applied
+ *   sync.  With the drone's record (saved block pose P4, its frame's self_pose vo):
+ *     node_pose = Pose(P4, yaw) * DeltaPose(set_yaw_only(vo), vo_now, 6-DoF), valid iff the drone is enabled in the last
+ *       observe (osb_anchor_observability; self_id always is);
+ *     base_pose = set_yaw_only(Pose(P4, yaw)) * set_yaw_only(vo)^-1.
+ *   A drone without a record (no applied sync pushed a frame holding it), or finish_init == 0, gives neither.  One launch,
+ *   then a synchronisation (no launch before the first sync or with finish_init == 0); the record never leaves the
+ *   device.  Refused (OSB_ERR_INVALID): a null pointer, n outside 0..max_drones, a drone id or self_id outside
+ *   0..max_drones-1.  The first call that launches acquires 188 D bytes of query and result buffers. */
+typedef struct {
+  int32_t self_id, finish_init;
+} osb_predict_params;
+typedef struct {
+  int32_t node_valid, reserved0;
+  double node_pose[7];
+  int32_t base_valid, reserved1;
+  double base_pose[7];
+} osb_predict_result;
+osb_status osb_anchor_predict(osb_anchor* h, const osb_predict_params* p, int n, const int32_t* drones,
+                              const double* vo_poses7, osb_predict_result* out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * The solve's chain from re-anchoring to factor rows on the device: run_dev -> reject_anchored -> compact_factors_dev, all

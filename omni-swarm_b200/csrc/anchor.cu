@@ -14,6 +14,7 @@
 // DroneTrajectory / NodeFrame / LoopEdge arithmetic is defined in oracle/anchor_ref.py (swarm_msgs is not in the tree).
 // Built with -fmad=false (Makefile) so every product is rounded as the oracle rounds it.
 #include <climits>
+#include <cmath>
 
 #include "common.cuh"
 #include "pose_algebra.cuh"
@@ -493,6 +494,176 @@ __global__ void init_mask_kernel(const int32_t* __restrict__ blk_drone, const do
   yaw[b] = m ? quat_yaw(blk_q + 4 * (size_t)b) : 0.0;
 }
 
+// sync_est_poses (swarm_localization_solver.cpp:962-1057) and PredictSwarm (:673-765): three launches per sync.
+// sync_gate_kernel (one CTA, thread d = drone d) decides whether the solver's last device call is accepted and the window
+// has odometry for every drone, then writes the path counts and the prediction record; sync_kf_kernel writes one keyframe
+// path sample per window entry; sync_full_kernel strides over every (drone, 10th odometry sample) of the capacities.
+constexpr int SYNC_THREADS = 256;                                  // = ANCHOR_MAX_DRONES
+constexpr int FULL_PATH_STEP = 10;                                 // :66
+
+// what sync reads of the window, derived by set_window on the host: every entry, vo_available or not, ordered by
+// (drone, frame) -- drone d's are [first[d], first[d+1]) -- and the stamp a steady sync pushes
+struct SyncWindow {
+  int32_t first[ANCHOR_MAX_DRONES + 1];
+  int32_t n_frames, reserved;
+  int64_t push_stamp;                 // the last frame that has entries (the reference's last_ts)
+};
+struct SyncRecord {                   // est_poses_tsid_saved[ts][d] of the last pushed frame ts holding d
+  int64_t stamp;
+  int32_t valid, reserved;
+  double saved[4];                    // the solved block pose, x y z yaw
+  double vo[7];                       // the entry's self_pose (all_sf[ts].id2nodeframe[d].pose())
+};
+struct SyncOutcome { int32_t applied, status; };
+
+struct SyncView {
+  const SyncWindow* win;
+  const int64_t* w_stamp;             // [E] the entry's frame stamp
+  const int32_t *w_drone, *w_block;   // [E]
+  const double* w_pose;               // [E][7] self_pose
+  int max_entries, max_drones, max_samples, max_full;
+  const int64_t* traj_stamp;
+  const double* traj_pose;
+  const int32_t* traj_n;
+  // the solver's last device call
+  const double* poses;
+  const int32_t* word;
+  const osb_solve_summary* summary;
+  const int32_t* chosen;
+  int trials, base_res, normalise, window_size, full_path;
+  double acpt_cost;
+  // outputs
+  SyncOutcome* outcome;
+  SyncRecord* rec;
+  int32_t* kf_first;                  // [D + 1] the paths' (snapshot of win->first)
+  int64_t* kf_stamp;                  // [E]
+  double* kf_pose;                    // [E][7]
+  int32_t* full_n;                    // [D], -1: none
+  int64_t* full_stamp;                // [D][max_full]
+  double* full_pose;                  // [D][max_full][7]
+};
+
+__device__ __forceinline__ PoseD pose_from4(const double* p) {   // Pose(double[4], true)
+  PoseD o;
+  o.t[0] = p[0]; o.t[1] = p[1]; o.t[2] = p[2];
+  const double rv[3] = {0.0, 0.0, p[3]};
+  quat_from_rotvec(rv, o.q);
+  return o;
+}
+// AngleAxis(-yaw(ego), Z) * att(ego)
+__device__ __forceinline__ void att_no_yaw(const PoseD& ego, double* q) {
+  double qy[4];
+  const double rv[3] = {0.0, 0.0, -quat_yaw(ego.q)};
+  quat_from_rotvec(rv, qy);
+  q_mul(qy, ego.q, q);
+}
+__device__ __forceinline__ PoseD ego_at(const SyncView& v, int d, int64_t t) {
+  const size_t base = (size_t)d * v.max_samples;
+  return load_pose(v.traj_pose + (base + nearest_sample(v.traj_stamp + base, v.traj_n[d], t)) * 7);
+}
+
+__global__ void __launch_bounds__(SYNC_THREADS) sync_gate_kernel(const SyncView v) {
+  __shared__ int s_ok;
+  const int d = threadIdx.x;
+  const SyncWindow& w = *v.win;
+  if (d == 0) {
+    bool ok;
+    if (v.trials > 0) {
+      ok = __ldcg(v.chosen) >= 0;                                  // solve_with_multiple_init's finish_init
+    } else {
+      const double c = __ldcg(&v.summary->final_cost);
+      const int n_res = v.base_res + __ldcg(v.word + 3);
+      const double e = v.normalise ? sqrt(c) / (double)n_res / (double)v.window_size : c;
+      ok = __ldcg(v.word) == OSB_OK && !(e > v.acpt_cost);         // :947-951
+    }
+    s_ok = ok;
+  }
+  const bool live = d < v.max_drones;
+  const int lo = live ? w.first[d] : 0, hi = live ? w.first[d + 1] : 0;
+  __syncthreads();
+  const bool accepted = s_ok != 0;
+  const bool no_odom = __syncthreads_or(accepted && hi > lo && v.traj_n[d] == 0);
+  if (d == 0) {
+    v.outcome->applied = accepted && !no_odom;
+    v.outcome->status = no_odom ? OSB_ERR_INVALID : OSB_OK;
+  }
+  if (!accepted || no_odom || !live) return;
+  v.kf_first[d] = lo;
+  if (d == v.max_drones - 1) v.kf_first[d + 1] = hi;
+  v.full_n[d] = (v.full_path && hi > lo) ? (v.traj_n[d] + FULL_PATH_STEP - 1) / FULL_PATH_STEP : -1;
+  SyncRecord& r = v.rec[d];
+  int k = -1;
+  if (hi > lo && (v.trials > 0 || v.win->push_stamp == v.w_stamp[hi - 1])) {
+    k = hi - 1;                                                    // a pushed frame holds d: the last of them
+  } else if (r.valid) {
+    for (int j = lo; j < hi; ++j)                                  // its frame is still in the window: rewritten
+      if (v.w_stamp[j] == r.stamp) { k = j; break; }
+  }
+  if (k < 0) return;
+  r.stamp = v.w_stamp[k];
+  r.valid = 1;
+  const double* p = v.poses + 4 * (size_t)v.w_block[k];
+  for (int j = 0; j < 4; ++j) r.saved[j] = p[j];
+  for (int j = 0; j < 7; ++j) r.vo[j] = v.w_pose[(size_t)k * 7 + j];
+}
+
+__global__ void sync_kf_kernel(const SyncView v) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= v.max_entries || !v.outcome->applied || k >= v.win->first[v.max_drones]) return;
+  const int d = v.w_drone[k];
+  const int64_t t = v.w_stamp[k];
+  PoseD p = pose_from4(v.poses + 4 * (size_t)v.w_block[k]);
+  double q[4], qa[4];
+  att_no_yaw(ego_at(v, d, t), qa);
+  q_mul(p.q, qa, q);
+  for (int j = 0; j < 4; ++j) p.q[j] = q[j];
+  v.kf_stamp[k] = t;
+  store_pose(v.kf_pose + (size_t)k * 7, p);
+}
+
+__global__ void sync_full_kernel(const SyncView v) {
+  if (!v.outcome->applied) return;
+  const long long total = (long long)v.max_drones * v.max_full;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int d = (int)(i / v.max_full), j = (int)(i % v.max_full);
+    if (j >= v.full_n[d]) continue;
+    const int lo = v.kf_first[d], hi = v.kf_first[d + 1];
+    const size_t s = (size_t)d * v.max_samples + (size_t)j * FULL_PATH_STEP;
+    const int64_t ts_vo = v.traj_stamp[s];
+    const int k = lo + nearest_sample(v.kf_stamp + lo, hi - lo, ts_vo);   // the walk of :1034-1040
+    PoseD p = pose_mul(load_pose(v.kf_pose + (size_t)k * 7),
+                       delta_pose4(load_pose(v.w_pose + (size_t)k * 7), load_pose(v.traj_pose + s * 7)));
+    double q[4], qa[4];
+    att_no_yaw(ego_at(v, d, v.kf_stamp[k]), qa);
+    q_mul(p.q, qa, q);
+    for (int c = 0; c < 4; ++c) p.q[c] = q[c];
+    const size_t o = (size_t)d * v.max_full + j;
+    v.full_stamp[o] = ts_vo;
+    store_pose(v.full_pose + o * 7, p);
+  }
+}
+
+__global__ void predict_kernel(int n, const int32_t* __restrict__ drones, const double* __restrict__ vo_now,
+                               const SyncRecord* __restrict__ rec, const osb_observability* __restrict__ obs, int self_id,
+                               osb_predict_result* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int d = drones[i];
+  const SyncRecord& r = rec[d];
+  osb_predict_result o = {};
+  if (r.valid) {
+    const PoseD est = pose_from4(r.saved), vo = load_pose(r.vo);
+    const PoseD vo4 = pose_yaw_only(vo);
+    if (d == self_id || (obs != nullptr && obs->enable[d])) {      // :676-678
+      o.node_valid = 1;
+      store_pose(o.node_pose, pose_mul(est, pose_mul(pose_inv(vo4), load_pose(vo_now + (size_t)i * 7))));   // :691
+    }
+    o.base_valid = 1;
+    store_pose(o.base_pose, pose_mul(pose_yaw_only(est), pose_inv(vo4)));                                   // :708-715
+  }
+  out[i] = o;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -501,6 +672,8 @@ static_assert(sizeof(osb_measurement) == 496, "osb_measurement layout");
 static_assert(sizeof(osb_window_entry) == 80, "osb_window_entry layout");
 static_assert(sizeof(osb_anchor_result) == 760, "osb_anchor_result layout");
 static_assert(sizeof(osb_observability) == 5 * 256 + 16, "osb_observability layout");
+static_assert(sizeof(osb_predict_result) == 128, "osb_predict_result layout");
+static_assert(sizeof(osb_sync_params) == 24, "osb_sync_params layout");
 
 struct osb_anchor {
   Resources res;
@@ -542,6 +715,27 @@ struct osb_anchor {
   int32_t* d_blk_drone = nullptr;                 // [blk_cap], then the table's length
   double* d_blk_q = nullptr;
   size_t blk_cap = 0;
+  // sync_dev, acquired by the first one: the window table (set_window keeps it current after that), the paths, the
+  // prediction record, the outcome, and the event recorded after every sync; predict's query and result buffers
+  SyncWindow sync_win{};                          // the host's, kept by set_window whether or not a sync ever ran
+  std::vector<int64_t> sw_stamp;
+  std::vector<int32_t> sw_drone, sw_block;
+  std::vector<double> sw_pose;
+  int sw_max_block = -1;                          // the window's largest block id (-1: none)
+  SyncWindow* d_sync_win = nullptr;
+  int64_t* d_sw_stamp = nullptr;
+  int32_t *d_sw_drone = nullptr, *d_sw_block = nullptr;
+  double* d_sw_pose = nullptr;
+  SyncOutcome* d_outcome = nullptr;
+  SyncRecord* d_rec = nullptr;
+  int32_t *d_kf_first = nullptr, *d_full_n = nullptr;
+  int64_t *d_kf_stamp = nullptr, *d_full_stamp = nullptr;
+  double *d_kf_pose = nullptr, *d_full_pose = nullptr;
+  int max_full = 0;                               // ceil(max_traj_samples / 10)
+  cudaEvent_t last_sync = nullptr;
+  int32_t* d_pred_drone = nullptr;
+  double* d_pred_vo = nullptr;
+  osb_predict_result* d_pred_out = nullptr;
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -560,6 +754,48 @@ namespace {
 osb_status anchor_wait_last_run(osb_anchor* h) {
   OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_run, 0));
   if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
+  if (h->last_sync) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_sync, 0));
+  return OSB_OK;
+}
+
+// the window's part of sync: every entry ordered by (drone, frame), with its frame's stamp (a counting sort by drone)
+void sync_window(osb_anchor* h, int n_frames, const int64_t* frame_stamps, const int32_t* frame_first,
+                 const osb_window_entry* entries) {
+  const int D = h->p.max_drones, n = n_frames == 0 ? 0 : frame_first[n_frames];
+  SyncWindow& w = h->sync_win;
+  std::fill(w.first, w.first + ANCHOR_MAX_DRONES + 1, 0);
+  for (int e = 0; e < n; ++e) ++w.first[entries[e].drone_id + 1];
+  for (int d = 0; d < D; ++d) w.first[d + 1] += w.first[d];
+  for (int d = D + 1; d <= ANCHOR_MAX_DRONES; ++d) w.first[d] = w.first[D];
+  w.n_frames = n_frames;
+  w.push_stamp = 0;
+  h->sw_stamp.resize(n); h->sw_drone.resize(n); h->sw_block.resize(n); h->sw_pose.resize((size_t)n * 7);
+  std::vector<int32_t> fill(w.first, w.first + D);
+  h->sw_max_block = -1;
+  for (int f = 0; f < n_frames; ++f) {
+    if (frame_first[f + 1] > frame_first[f]) w.push_stamp = frame_stamps[f];
+    for (int e = frame_first[f]; e < frame_first[f + 1]; ++e) {
+      const int k = fill[entries[e].drone_id]++;
+      h->sw_stamp[k] = frame_stamps[f];
+      h->sw_drone[k] = entries[e].drone_id;
+      h->sw_block[k] = entries[e].block;
+      std::copy(entries[e].self_pose, entries[e].self_pose + 7, h->sw_pose.begin() + (size_t)k * 7);
+      h->sw_max_block = std::max(h->sw_max_block, entries[e].block);
+    }
+  }
+}
+
+// the sync's window table to the device, on the handle's stream (the caller synchronises)
+osb_status upload_sync_window(osb_anchor* h) {
+  cudaStream_t st = h->stream;
+  const size_t n = h->sw_stamp.size();
+  OSB_CUDA(cudaMemcpyAsync(h->d_sync_win, &h->sync_win, sizeof(SyncWindow), cudaMemcpyHostToDevice, st));
+  if (n > 0) {
+    OSB_CUDA(cudaMemcpyAsync(h->d_sw_stamp, h->sw_stamp.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_sw_drone, h->sw_drone.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_sw_block, h->sw_block.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_sw_pose, h->sw_pose.data(), n * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
   return OSB_OK;
 }
 
@@ -676,6 +912,7 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
   h->h_len.reserve(S);
   h->h_slot.reserve(M);
   observe_window(h->obs_win, p->max_drones, 0, 0, nullptr);
+  sync_window(h.get(), 0, nullptr, nullptr, nullptr);
   *out = h.release();
   return OSB_OK;
 }
@@ -849,6 +1086,8 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
     OSB_CUDA(cudaMemcpyAsync(h->d_win_block, h->h_win_block.data(), (size_t)n_vo * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     OSB_CUDA(cudaMemcpyAsync(h->d_win_pose, h->h_win_pose.data(), (size_t)n_vo * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
   }
+  sync_window(h, n_frames, frame_stamps_ns, frame_first, entries);
+  if (h->d_sync_win) OSB_TRY(upload_sync_window(h));
   OSB_CUDA(cudaStreamSynchronize(st));
   if (h->d_blk_drone) OSB_TRY(upload_blocks(h));
   h->n_frames = n_frames;
@@ -899,7 +1138,7 @@ osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_ancho
   if (v.n_bound == 0) return OSB_OK;
   OSB_LAUNCH(anchor_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(cudaEventRecord(h->last_run, st));
+  OSB_CUDA(record_event_capturable(h->last_run, st));             // captured: the updates after a replay wait for it
   return OSB_OK;
 }
 
@@ -1066,5 +1305,164 @@ extern "C" osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, i
              n_nodes, self_id, h->d_obs, mask_dev, yaw_dev);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
+  return OSB_OK;
+}
+
+namespace {
+
+// the first sync acquires the window table (the host's), the paths (no drone has one), the records (none valid), the
+// outcome (nothing applied) and the event
+osb_status sync_init(osb_anchor* h) {
+  if (h->d_outcome) return OSB_OK;
+  const size_t D = (size_t)h->p.max_drones, E = (size_t)h->p.max_window_entries;
+  h->max_full = (int)cdiv64(h->p.max_traj_samples, FULL_PATH_STEP);
+  const size_t F = D * (size_t)h->max_full;
+  Resources& R = h->res;
+  OSB_TRY(R.alloc(&h->d_sync_win, 1));
+  OSB_TRY(R.alloc(&h->d_sw_stamp, E));
+  OSB_TRY(R.alloc(&h->d_sw_drone, E));
+  OSB_TRY(R.alloc(&h->d_sw_block, E));
+  OSB_TRY(R.alloc(&h->d_sw_pose, E * 7));
+  OSB_TRY(R.alloc(&h->d_kf_first, D + 1));
+  OSB_TRY(R.alloc(&h->d_kf_stamp, E));
+  OSB_TRY(R.alloc(&h->d_kf_pose, E * 7));
+  OSB_TRY(R.alloc(&h->d_full_n, D));
+  OSB_TRY(R.alloc(&h->d_full_stamp, F));
+  OSB_TRY(R.alloc(&h->d_full_pose, F * 7));
+  OSB_TRY(R.alloc(&h->d_rec, D));
+  OSB_TRY(R.event(&h->last_sync, cudaEventDisableTiming));
+  SyncOutcome* outcome = nullptr;
+  OSB_TRY(R.alloc(&outcome, 1));
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaMemsetAsync(h->d_kf_first, 0, (D + 1) * sizeof(int32_t), st));
+  OSB_CUDA(cudaMemsetAsync(h->d_full_n, 0xff, D * sizeof(int32_t), st));
+  OSB_CUDA(cudaMemsetAsync(h->d_rec, 0, D * sizeof(SyncRecord), st));
+  OSB_CUDA(cudaMemsetAsync(outcome, 0, sizeof(SyncOutcome), st));
+  OSB_TRY(upload_sync_window(h));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  h->d_outcome = outcome;                                          // set last: a failed first call is tried again
+  return OSB_OK;
+}
+
+}  // namespace
+
+extern "C" osb_status osb_anchor_sync_dev(osb_anchor* h, osb_solver* s, const osb_sync_params* p, void* stream) {
+  OSB_REQUIRE(h != nullptr && s != nullptr && p != nullptr, "null argument");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  OSB_REQUIRE(!p->normalise || p->window_size >= 1, "window_size must be >= 1 when normalise is set");
+  OSB_REQUIRE(!std::isnan(p->acpt_cost), "acpt_cost is NaN");
+  SolverDeviceCall c{};
+  OSB_TRY(solver_device_call(s, &c));
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(c.device == h->device, "the anchor and the solver are on different devices");
+  OSB_REQUIRE(!h->blk_negative && h->sw_max_block < c.n_nodes, "a window block outside 0 .. the solver's node count - 1");
+  DeviceGuard dg(h->device);
+  OSB_TRY(sync_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  SyncView v{};
+  v.win = h->d_sync_win;
+  v.w_stamp = h->d_sw_stamp; v.w_drone = h->d_sw_drone; v.w_block = h->d_sw_block; v.w_pose = h->d_sw_pose;
+  v.max_entries = h->p.max_window_entries; v.max_drones = h->p.max_drones; v.max_samples = h->p.max_traj_samples;
+  v.max_full = h->max_full;
+  v.traj_stamp = h->d_traj_stamp; v.traj_pose = h->d_traj_pose; v.traj_n = h->d_traj_n;
+  v.poses = c.poses; v.word = c.word; v.summary = c.summary; v.chosen = c.chosen;
+  v.trials = c.trials; v.base_res = c.base_res;
+  v.normalise = p->normalise ? 1 : 0; v.window_size = p->window_size; v.full_path = p->full_path ? 1 : 0;
+  v.acpt_cost = p->acpt_cost;
+  v.outcome = h->d_outcome; v.rec = h->d_rec;
+  v.kf_first = h->d_kf_first; v.kf_stamp = h->d_kf_stamp; v.kf_pose = h->d_kf_pose;
+  v.full_n = h->d_full_n; v.full_stamp = h->d_full_stamp; v.full_pose = h->d_full_pose;
+  OSB_CUDA(wait_event_capturable(st, c.done));                    // the solved poses and the call's outcome
+  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the record and the paths are the last sync's
+  OSB_LAUNCH(sync_gate_kernel, 1, SYNC_THREADS, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(sync_kf_kernel, cdiv(v.max_entries, 256), 256, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  const long long work = (long long)v.max_drones * v.max_full;
+  OSB_LAUNCH(sync_full_kernel, (int)std::min<long long>(cdiv64(work, 256), 8LL * num_sms()), 256, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_sync, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_sync_result(osb_anchor* h, int32_t* applied, osb_status* last) {
+  OSB_REQUIRE(h != nullptr && applied != nullptr && last != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *applied = 0;
+  *last = OSB_OK;
+  if (!h->d_outcome) return OSB_OK;
+  DeviceGuard dg(h->device);
+  SyncOutcome o;
+  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_sync, 0));
+  OSB_CUDA(cudaMemcpyAsync(&o, h->d_outcome, sizeof(o), cudaMemcpyDeviceToHost, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  *applied = o.applied;
+  *last = (osb_status)o.status;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, int64_t* stamps, double* poses7, int cap,
+                                       int32_t* n) {
+  OSB_REQUIRE(h != nullptr && n != nullptr && cap >= 0 && (cap == 0 || (stamps && poses7)), "null argument or negative cap");
+  OSB_REQUIRE(drone_ok(h, drone), "drone id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *n = -1;
+  if (!h->d_outcome) return OSB_OK;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
+  int32_t cnt[2];
+  const int64_t* src_stamp;
+  const double* src_pose;
+  if (full) {
+    OSB_CUDA(cudaMemcpyAsync(cnt, h->d_full_n + drone, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaStreamSynchronize(st));
+    const size_t o = (size_t)drone * h->max_full;
+    src_stamp = h->d_full_stamp + o;
+    src_pose = h->d_full_pose + o * 7;
+  } else {
+    OSB_CUDA(cudaMemcpyAsync(cnt, h->d_kf_first + drone, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaStreamSynchronize(st));
+    src_stamp = h->d_kf_stamp + cnt[0];
+    src_pose = h->d_kf_pose + (size_t)cnt[0] * 7;
+    cnt[0] = cnt[1] > cnt[0] ? cnt[1] - cnt[0] : -1;
+  }
+  *n = cnt[0];
+  const int k = std::min(cnt[0], cap);
+  if (k > 0) {
+    OSB_CUDA(cudaMemcpyAsync(stamps, src_stamp, (size_t)k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaMemcpyAsync(poses7, src_pose, (size_t)k * 7 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaStreamSynchronize(st));
+  }
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_predict(osb_anchor* h, const osb_predict_params* p, int n, const int32_t* drones,
+                                         const double* vo_poses7, osb_predict_result* out) {
+  OSB_REQUIRE(h != nullptr && p != nullptr, "null argument");
+  OSB_REQUIRE(n >= 0 && n <= h->p.max_drones, "n outside 0..max_drones");
+  OSB_REQUIRE(n == 0 || (drones && vo_poses7 && out), "null argument");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  for (int i = 0; i < n; ++i) OSB_REQUIRE(drone_ok(h, drones[i]), "drone id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (n > 0) memset(out, 0, (size_t)n * sizeof(osb_predict_result));
+  if (n == 0 || !p->finish_init || !h->d_outcome) return OSB_OK;   // :738-741; no sync: no record
+  DeviceGuard dg(h->device);
+  const size_t D = (size_t)h->p.max_drones;
+  if (!h->d_pred_out) {
+    OSB_TRY(h->res.alloc(&h->d_pred_drone, D));
+    OSB_TRY(h->res.alloc(&h->d_pred_vo, D * 7));
+    OSB_TRY(h->res.alloc(&h->d_pred_out, D));
+  }
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
+  if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(st, h->last_observe, 0));
+  OSB_CUDA(cudaMemcpyAsync(h->d_pred_drone, drones, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  OSB_CUDA(cudaMemcpyAsync(h->d_pred_vo, vo_poses7, (size_t)n * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+  OSB_LAUNCH(predict_kernel, cdiv(n, 128), 128, 0, st, n, h->d_pred_drone, h->d_pred_vo, h->d_rec, h->d_obs, p->self_id,
+             h->d_pred_out);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(cudaMemcpyAsync(out, h->d_pred_out, (size_t)n * sizeof(osb_predict_result), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
   return OSB_OK;
 }

@@ -288,6 +288,22 @@ struct CountFeedback {
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// What osb_anchor_sync_dev reads of a pose-graph solver's last device call (graph.cu; not part of the C ABI).  The
+// pointers are device memory that the call's launches write; `done` is recorded after them, also inside a capture.
+struct SolverDeviceCall {
+  int device;
+  int n_nodes;                            // the resident graph's node count
+  int trials;                             // 0: osb_solver_solve_resident_dev, else the multistart's n_trials
+  int base_res;                           // residuals of the resident factors (the tail's are word[3])
+  const double* poses;                    // [n_nodes][4] x y z yaw, caller's node order
+  const int32_t* word;                    // [0] status, [3] the tail's residuals
+  const osb_solve_summary* summary;       // the single solve's
+  const int32_t* chosen;                  // the multistart's chosen trial (-1: none)
+  cudaEvent_t done;
+};
+// OSB_ERR_INVALID (error text set) when the solver made no device call since its last host-side pose or graph change
+osb_status solver_device_call(osb_solver* h, SolverDeviceCall* out);
+
 // ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------

@@ -1421,6 +1421,7 @@ struct osb_solver {
   SolveShape tail_shape = {};
   // the last device call: pending until a host-side call synchronises with it and refreshes g_poses from d_rposes
   bool dev_pending = false, dev_captured = false, dev_called = false;
+  bool dev_fresh = false;           // a device call since the last host-side pose or graph change (osb_anchor_sync_dev)
   osb_status dev_status = OSB_OK;
   osb_solve_summary dev_summary = {};
   // ... when it was osb_solver_solve_multistart_resident_dev: its n_trials (0: a single solve) and, once refreshed, what
@@ -1790,6 +1791,7 @@ static osb_status solver_run(osb_solver* h, int n_nodes, double* poses, const ui
                              osb_solve_summary* summaries, double* equv = nullptr, int32_t* chosen = nullptr) {
   osb_solve_options o;
   if (opt) o = *opt; else osb_solve_default_options(&o);
+  h->dev_fresh = false;                        // the one-shot results overwrite the multistart's
   const int K = ms ? ms->n_trials : 1;
   const size_t n = n_nodes;
   cudaStream_t st = h->stream;
@@ -1911,7 +1913,7 @@ extern "C" osb_status osb_solver_graph_clear(osb_solver* h) {
   h->g_type.clear(); h->g_ia.clear(); h->g_ib.clear();
   h->g_uploaded = 0; h->g_static_valid = true;
   ++h->g_topo_version;
-  h->rposes_current = false; h->dev_pending = false;
+  h->rposes_current = false; h->dev_pending = false; h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -1927,7 +1929,7 @@ extern "C" osb_status osb_solver_graph_add_nodes(osb_solver* h, int n, const dou
   h->g_poses.insert(h->g_poses.end(), poses, poses + 4 * (size_t)n);
   for (int i = 0; i < n; ++i) h->g_fixed.push_back(fixed ? fixed[i] : 0);
   ++h->g_topo_version;
-  h->rposes_current = false; h->dev_pending = false;
+  h->rposes_current = false; h->dev_pending = false; h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -1947,6 +1949,7 @@ extern "C" osb_status osb_solver_graph_add_factors(osb_solver* h, int m, const i
   h->g_huber.insert(h->g_huber.end(), huber, huber + m);
   h->g_payload.insert(h->g_payload.end(), payload, payload + (size_t)m * OSB_PAYLOAD_LEN);
   ++h->g_topo_version;
+  h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -1958,6 +1961,7 @@ extern "C" osb_status osb_solver_graph_set_fixed(osb_solver* h, int node, int fi
   OSB_REQUIRE(node >= 0 && (size_t)node < h->g_fixed.size(), "node out of range");
   h->g_fixed[node] = fixed ? 1 : 0;
   ++h->g_topo_version;
+  h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -1968,7 +1972,7 @@ extern "C" osb_status osb_solver_graph_set_poses(osb_solver* h, int first, int n
   OSB_TRY(finish_device_call(h));
   OSB_REQUIRE(first >= 0 && n >= 0 && (size_t)(first + n) <= h->g_fixed.size(), "node range out of bounds");
   std::copy(poses, poses + 4 * (size_t)n, h->g_poses.begin() + 4 * (size_t)first);
-  h->rposes_current = false; h->dev_pending = false;
+  h->rposes_current = false; h->dev_pending = false; h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -2015,7 +2019,7 @@ extern "C" osb_status osb_solver_graph_drop_oldest(osb_solver* h, int n_nodes) {
   h->g_type.resize(w); h->g_ia.resize(w); h->g_ib.resize(w); h->g_huber.resize(w); h->g_payload.resize(w * OSB_PAYLOAD_LEN);
   h->g_uploaded = 0;                       // factor positions moved: re-send on the next solve
   ++h->g_topo_version;
-  h->rposes_current = false; h->dev_pending = false;
+  h->rposes_current = false; h->dev_pending = false; h->dev_fresh = false;
   return OSB_OK;
 }
 
@@ -2030,7 +2034,7 @@ extern "C" osb_status osb_solver_solve_resident(osb_solver* h, const osb_solve_o
   OSB_REQUIRE(n > 0 && m > 0, "the resident graph is empty");
   OSB_TRY(flush_resident_factors(h));
   h->rposes_current = false;               // this solve writes g_poses
-  h->dev_pending = false;
+  h->dev_pending = false; h->dev_fresh = false;
   return solver_run(h, (int)n, h->g_poses.data(), h->g_fixed.data(), (int)m, h->g_type.data(), h->g_ia.data(),
                     h->g_ib.data(), h->g_payload.data(), h->g_huber.data(), false, h->g_topo_version, opt, nullptr,
                     nullptr, summary);
@@ -2114,6 +2118,7 @@ static osb_status resident_dev_call(osb_solver* h, int max_tail, const int32_t* 
   const char* fn = ms ? "osb_solver_solve_multistart_resident_dev" : "osb_solver_solve_resident_dev";
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
+  h->dev_fresh = false;                        // until this call has enqueued everything
   cudaStream_t st = (cudaStream_t)stream;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   OSB_CUDA(cudaStreamIsCapturing(st, &cap));
@@ -2236,9 +2241,27 @@ static osb_status resident_dev_call(osb_solver* h, int max_tail, const int32_t* 
     OSB_LAUNCH(tail_poses_out_kernel, cdiv((int)n, 256), 256, 0, st, D);
   }
   OSB_CHECK_LAUNCH();
-  if (!capturing) OSB_CUDA(cudaEventRecord(h->ev_done, st));
-  h->dev_pending = true; h->dev_captured = capturing; h->dev_called = true;
+  OSB_CUDA(record_event_capturable(h->ev_done, st));   // captured: an external record, which osb_anchor_sync_dev waits on
+  h->dev_pending = true; h->dev_captured = capturing; h->dev_called = true; h->dev_fresh = true;
   h->dev_trials = ms ? K : 0;
+  return OSB_OK;
+}
+
+osb_status osb::solver_device_call(osb_solver* h, SolverDeviceCall* out) {
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (!h->dev_fresh) {
+    set_error("osb_anchor_sync_dev", "the solver made no device call since its last host-side pose or graph change");
+    return OSB_ERR_INVALID;
+  }
+  out->device = h->device;
+  out->n_nodes = (int)h->g_fixed.size();
+  out->trials = h->dev_trials;
+  out->base_res = h->tail_nres;
+  out->poses = h->d_rposes;
+  out->word = h->tail.word;
+  out->summary = h->d_tsummary;
+  out->chosen = &h->d_res->chosen;
+  out->done = h->ev_done;
   return OSB_OK;
 }
 

@@ -992,6 +992,44 @@ class LoopAnchor(_Handle):
         _l.check(self._lib.osb_anchor_init_mask_dev(self._h, int(self_id), int(n_nodes), C.c_void_p(mask_ptr),
                                                     C.c_void_p(yaw_ptr), C.c_void_p(stream)))
 
+    def sync_dev(self, solver: PoseGraphSolver, stream: int, self_id: int, acpt_cost: float, window_size: int,
+                 normalise: bool = True, full_path: bool = False):
+        """sync_est_poses on the device (osb_anchor_sync_dev): the keyframe paths, the full paths (full_path) and the
+        prediction record from the solver's last device call, applied only if solve() would accept that call, on
+        `stream` without synchronising"""
+        p = _l.SyncParams(int(self_id), int(bool(full_path)), int(bool(normalise)), int(window_size), float(acpt_cost))
+        _l.check(self._lib.osb_anchor_sync_dev(self._h, solver._h, C.byref(p), C.c_void_p(stream)))
+
+    def sync_result(self) -> tuple[bool, int]:
+        """waits for the last sync_dev -> (applied, status): status lib.ERR_INVALID for a window drone without odometry"""
+        applied, last = C.c_int32(0), C.c_int(0)
+        _l.check(self._lib.osb_anchor_sync_result(self._h, C.byref(applied), C.byref(last)))
+        return bool(applied.value), last.value
+
+    def paths(self, drone: int, full: bool = False):
+        """waits for the last sync_dev -> drone's keyframe path (or full path) as (stamps int64 [n], poses [n, 7]), or
+        None when the drone has none"""
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_anchor_paths(self._h, int(full), int(drone), None, None, 0, C.byref(n)))
+        if n.value < 0:
+            return None
+        stamps = np.zeros(n.value, np.int64)
+        poses = np.zeros((n.value, 7), np.float64)
+        _l.check(self._lib.osb_anchor_paths(self._h, int(full), int(drone), _l.ptr(stamps), _l.ptr(poses), n.value,
+                                            C.byref(n)))
+        return stamps, poses
+
+    def predict(self, drones, vo_poses, self_id: int, finish_init: bool = True) -> dict:
+        """PredictSwarm for one frame (osb_anchor_predict): drones [n], their odometry poses [n, 7] now -> {drone:
+        (node_pose [7] or None, base_pose [7] or None)}"""
+        d = np.ascontiguousarray(drones, np.int32)
+        vo = np.ascontiguousarray(vo_poses, np.float64).reshape(len(d), 7)
+        out = (_l.PredictResult * max(1, len(d)))()
+        p = _l.PredictParams(int(self_id), int(bool(finish_init)))
+        _l.check(self._lib.osb_anchor_predict(self._h, C.byref(p), len(d), _l.ptr(d), _l.ptr(vo), C.cast(out, C.c_void_p)))
+        return {int(d[i]): (np.array(out[i].node_pose) if out[i].node_valid else None,
+                            np.array(out[i].base_pose) if out[i].base_valid else None) for i in range(len(d))}
+
     def observability(self) -> dict:
         """waits for the last observe_dev -> its outcome: bool arrays [max_drones] nodes, yaw, pos, enable, to_init and
         the flags solve_master, motion, motion_new"""

@@ -94,6 +94,20 @@ class ObserveParams(C.Structure):
 OBS_DRONES = 256                         # per-drone bytes of osb_observability
 
 
+class SyncParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("full_path", C.c_int32), ("normalise", C.c_int32), ("window_size", C.c_int32),
+                ("acpt_cost", C.c_double)]
+
+
+class PredictParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("finish_init", C.c_int32)]
+
+
+class PredictResult(C.Structure):
+    _fields_ = [("node_valid", C.c_int32), ("reserved0", C.c_int32), ("node_pose", C.c_double * 7),
+                ("base_valid", C.c_int32), ("reserved1", C.c_int32), ("base_pose", C.c_double * 7)]
+
+
 class Observability(C.Structure):
     _fields_ = [("nodes", C.c_uint8 * OBS_DRONES), ("yaw", C.c_uint8 * OBS_DRONES), ("pos", C.c_uint8 * OBS_DRONES),
                 ("enable", C.c_uint8 * OBS_DRONES), ("to_init", C.c_uint8 * OBS_DRONES), ("solve_master", C.c_int32),
@@ -343,6 +357,10 @@ _SIG = {
     "osb_anchor_observe_dev": (C.c_int, [_P, C.POINTER(ObserveParams), _P, C.c_int, _P]),
     "osb_anchor_observability": (C.c_int, [_P, C.POINTER(Observability)]),
     "osb_anchor_init_mask_dev": (C.c_int, [_P, C.c_int32, C.c_int, _P, _P, _P]),
+    "osb_anchor_sync_dev": (C.c_int, [_P, _P, C.POINTER(SyncParams), _P]),
+    "osb_anchor_sync_result": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int)]),
+    "osb_anchor_paths": (C.c_int, [_P, C.c_int, C.c_int32, _P, _P, C.c_int, C.POINTER(C.c_int32)]),
+    "osb_anchor_predict": (C.c_int, [_P, C.POINTER(PredictParams), C.c_int, _P, _P, _P]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
