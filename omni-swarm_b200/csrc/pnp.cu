@@ -315,7 +315,9 @@ pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts
     rperr = sqrt((eo[0] - en[0]) * (eo[0] - en[0]) + (eo[1] - en[1]) * (eo[1] - en[1]) + (eo[2] - en[2]) * (eo[2] - en[2]));
   }
   res->rperr = rperr;
-  const double dist = sqrt(dp.t[0] * dp.t[0] + dp.t[1] * dp.t[1] + dp.t[2] * dp.t[2]);
+  // rounded step by step, as oracle/pnp_ref.loop_distance: a contracted sum would make the distance check depend on which
+  // fma order the compiler picks, not on the returned dp alone
+  const double dist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dp.t[0], dp.t[0]), __dmul_rn(dp.t[1], dp.t[1])), __dmul_rn(dp.t[2], dp.t[2])));
   res->verified = (rperr <= prm.rperr_thres && best_cnt >= prm.min_loop_num && fabs(yaw) < prm.accept_loop_yaw_rad &&
                    dist < prm.max_loop_dis) ? 1 : 0;                        // pnp_result_verify (:317-336)
   res->odometry_consistent = 1; res->md = 0.0;

@@ -158,6 +158,155 @@ def pnp_ransac(X, uv, prior, iterations=100, thresh=3.0, seed=0):
     return dict(success=True, pose=pose, mask=best_mask.astype(np.uint8), n_inliers=best, winner=best_h)
 
 
+# ---- the same RANSAC vectorised over hypotheses and points --------------------------------------------------------
+# pnp_ransac's arithmetic, operation by operation, on a leading batch axis: every hypothesis runs the same fixed LM
+# schedule with its own lambda, and a hypothesis whose damped system is not positive definite rejects that step alone.
+def _q_rot_b(q, v):
+    u = q[..., 1:]
+    c = np.cross(u, v)
+    return v + 2.0 * (q[..., :1] * c + np.cross(u, c))
+
+
+def _q_mul_b(a, b):
+    aw, ax, ay, az = (a[..., i] for i in range(4))
+    bw, bx, by, bz = (b[..., i] for i in range(4))
+    return np.stack([aw * bw - ax * bx - ay * by - az * bz,
+                     aw * bx + ax * bw + ay * bz - az * by,
+                     aw * by - ax * bz + ay * bw + az * bx,
+                     aw * bz + ax * by - ay * bx + az * bw], -1)
+
+
+def _reproj_sq_b(P, X, uv):
+    """P [B,7], X [B|1,m,3], uv [B|1,m,2] -> squared reprojection errors [B,m]"""
+    Y = _q_rot_b(P[:, None, 3:], X) + P[:, None, :3]
+    du = Y[..., 0] / Y[..., 2] - uv[..., 0]
+    dv = Y[..., 1] / Y[..., 2] - uv[..., 1]
+    return du * du + dv * dv
+
+
+def _normal_eq_b(P, X, uv):
+    """_normal_eq of B poses over their own m points; m = 4 accumulates point by point as _normal_eq does"""
+    Y = _q_rot_b(P[:, None, 3:], X)
+    p = Y + P[:, None, :3]
+    iz = 1.0 / p[..., 2]
+    r0, r1 = p[..., 0] * iz - uv[..., 0], p[..., 1] * iz - uv[..., 1]
+    zero = np.zeros_like(iz)
+    a = np.stack([iz, zero, -p[..., 0] * iz * iz], -1)
+    b = np.stack([zero, iz, -p[..., 1] * iz * iz], -1)
+    J0 = np.concatenate([np.cross(Y, a), a], -1)
+    J1 = np.concatenate([np.cross(Y, b), b], -1)
+    Ak = J0[..., :, None] * J0[..., None, :] + J1[..., :, None] * J1[..., None, :]
+    gk = J0 * r0[..., None] + J1 * r1[..., None]
+    ck = r0 * r0 + r1 * r1
+    m = X.shape[1]
+    if m <= 4:
+        A = np.zeros((len(P), 6, 6)); g = np.zeros((len(P), 6)); cost = np.zeros(len(P))
+        for k in range(m):
+            A += Ak[:, k]; g += gk[:, k]; cost += ck[:, k]
+        return A, g, cost
+    return Ak.sum(1), gk.sum(1), ck.sum(1)
+
+
+def _solve6_b(A, b):
+    """_solve6 of B systems -> (x [B,6], ok [B]); ok is False where _solve6 returns None or x is not finite"""
+    B = len(A)
+    L = np.zeros((B, 6, 6))
+    ok = np.ones(B, bool)
+    for j in range(6):
+        s = A[:, j, j] - np.vecdot(L[:, j, :j], L[:, j, :j])
+        ok &= s > 0
+        L[:, j, j] = np.sqrt(np.where(ok, s, 1.0))
+        for i in range(j + 1, 6):
+            L[:, i, j] = (A[:, i, j] - np.vecdot(L[:, i, :j], L[:, j, :j])) / L[:, j, j]
+    y = np.zeros((B, 6))
+    for i in range(6):
+        y[:, i] = (b[:, i] - np.vecdot(L[:, i, :i], y[:, :i])) / L[:, i, i]
+    x = np.zeros((B, 6))
+    for i in range(5, -1, -1):
+        x[:, i] = (y[:, i] - np.vecdot(L[:, i + 1:, i], x[:, i + 1:])) / L[:, i, i]
+    return x, ok & np.all(np.isfinite(x), 1)
+
+
+def _quat_from_rotvec_b(rv):
+    a = np.sqrt(rv[:, 0] * rv[:, 0] + rv[:, 1] * rv[:, 1] + rv[:, 2] * rv[:, 2])
+    small = a < 1e-12
+    ha = np.where(small, 1.0, a)
+    s = np.sin(0.5 * ha) / ha
+    q = np.where(small[:, None], np.concatenate([np.ones((len(rv), 1)), 0.5 * rv], 1),
+                 np.concatenate([np.cos(0.5 * ha)[:, None], s[:, None] * rv], 1))
+    return q / np.sqrt(np.vecdot(q, q))[:, None]
+
+
+def lm_pose_batched(P0, X, uv, iters):
+    """lm_pose of B poses P0 [B,7], each over its own points X [B,m,3], uv [B,m,2]"""
+    P = np.array(P0, np.float64)
+    B = len(P)
+    lam = np.full(B, 1e-3)
+    A, g, cost = _normal_eq_b(P, X, uv)
+    r = np.arange(6)
+    for _ in range(iters):
+        D = np.zeros_like(A)
+        D[:, r, r] = A[:, r, r]
+        Ad = A + lam[:, None, None] * D + 1e-12 * np.eye(6)
+        d, ok = _solve6_b(Ad, -g)
+        d = np.where(ok[:, None], d, 0.0)
+        dq = _quat_from_rotvec_b(d[:, :3])
+        cand = np.concatenate([_q_rot_b(dq, P[:, :3]) + d[:, 3:], _q_mul_b(dq, P[:, 3:])], 1)
+        cand[:, 3:] /= np.sqrt(np.vecdot(cand[:, 3:], cand[:, 3:]))[:, None]
+        c = _reproj_sq_b(cand, X, uv).sum(1)
+        ok &= np.isfinite(c) & (c < cost)
+        if ok.any():
+            P[ok] = cand[ok]
+            A[ok], g[ok], cost[ok] = _normal_eq_b(P[ok], X[ok], uv[ok])
+        lam = np.where(ok, np.maximum(lam * 0.1, 1e-9), np.minimum(lam * 10.0, 1e6))
+    return P
+
+
+def pnp_ransac_batched(X, uv, prior, iterations=100, thresh=3.0, seed=0):
+    """pnp_ransac with every hypothesis fitted and scored at once; the same result, plus
+    margin = min over hypotheses and points of |e - thresh^2| / thresh^2 (finite errors only; inf if there are none): how
+    far the data keep every inlier decision from the threshold, i.e. how much rounding an implementation may differ by
+    without changing a mask.  ties counts the finite errors exactly at thresh^2 and margin_untied is the margin without
+    them: data built from exactly representable values can put errors on the threshold in every implementation."""
+    X = np.asarray(X, np.float64); uv = np.asarray(uv, np.float64)
+    prior = np.asarray(prior, np.float64)
+    n = len(X)
+    out = dict(success=False, pose=prior, mask=np.zeros(n, np.uint8), n_inliers=0, winner=-1, margin=np.inf,
+               margin_untied=np.inf, ties=0)
+    if n < 4:
+        return out
+    t2 = float(thresh) * float(thresh)
+    hs, idx = [], []
+    for h in range(iterations):
+        s = draw4(seed, h, n)
+        if s is not None:
+            hs.append(h); idx.append(s)
+    if not hs:
+        return out
+    idx = np.asarray(idx)
+    with np.errstate(all="ignore"):
+        P = lm_pose_batched(np.broadcast_to(prior, (len(hs), 7)), X[idx], uv[idx], HYP_ITERS)
+        e = _reproj_sq_b(P, X[None], uv[None])
+        fin = np.isfinite(e)
+        if fin.any():
+            rel = np.abs(e[fin] - t2) / t2
+            out["margin"] = float(rel.min())
+            out["ties"] = int((rel == 0).sum())
+            out["margin_untied"] = float(rel[rel > 0].min()) if (rel > 0).any() else np.inf
+        inl = e <= t2                                    # NaN compares false
+        cnt = inl.sum(1)
+        w = int(np.argmax(cnt))                          # first best
+        best = int(cnt[w])
+        out["winner"] = hs[w]
+        out["n_inliers"] = best
+        if best < 4:
+            return out
+        m = inl[w]
+        pose = lm_pose_batched(P[w:w + 1], X[None, m], uv[None, m], REFINE_ITERS)[0]
+    out.update(success=True, pose=pose, mask=m.astype(np.uint8))
+    return out
+
+
 # ---- what compute_relative_pose does with the PnP result (:396-407) -------------------------------------------------
 def delta_pose(a, b, yaw_only):
     """Swarm::Pose::DeltaPose(a, b, use_yaw_only): 6-DoF a^-1 b, or the 4-DoF form of swarm_localization_factors.hpp:139-149"""
@@ -197,12 +346,28 @@ def loop_from_pnp(res, prm):
     yaw = quat2eulers(dp[3:])[2]
     out["dp"] = np.array([dp[0], dp[1], dp[2], yaw])
     out["rperr"] = rp_error(p_drone_old_in_new, prm["drone_pose_old"], prm["drone_pose_now"])
-    ok = out["rperr"] <= prm["rperr_thres"]                            # :323-326 (fails when rperr > RPERR_THRES)
-    ok = ok and res["n_inliers"] >= prm["min_loop_num"] and abs(yaw) < prm["accept_loop_yaw_rad"] \
-        and float(np.linalg.norm(dp[:3])) < prm["max_loop_dis"]       # :328-332
-    out["verified"] = bool(ok)
+    out["verified"] = verify(out["rperr"], res["n_inliers"], yaw, loop_distance(dp), prm)
     if prm.get("same_drone"):                                          # :294-315
         d = delta_pose(dp if prm["is_4dof"] else dp, prm["odom_rel"], False)
         out["md"] = pr.cholesky_smd(pr.log_map(d), np.asarray(prm["cov"], np.float64))
-        out["odometry_consistent"] = bool(not out["md"] > prm["odometry_consistency_threshold"])
+        out["odometry_consistent"] = odometry_consistent(out["md"], prm)
     return out
+
+
+def loop_distance(dp):
+    """|DP_old_to_new.pos()|, summed and rounded in this order (the kernel's order too), so that the distance check is
+    reproducible from a returned (x, y, z)"""
+    return float(np.sqrt((dp[0] * dp[0] + dp[1] * dp[1]) + dp[2] * dp[2]))
+
+
+def verify(rperr, n_inliers, yaw, dist, prm):
+    """pnp_result_verify (:317-336): fails when rperr > RPERR_THRES (:323-326), too few inliers, |yaw| too large or the
+    loop too long (:328-332)"""
+    return bool(rperr <= prm["rperr_thres"] and n_inliers >= prm["min_loop_num"] and abs(yaw) < prm["accept_loop_yaw_rad"]
+                and dist < prm["max_loop_dis"])
+
+
+def odometry_consistent(md, prm):
+    """check_loop_odometry_consistency (:294-315): inconsistent when the squared Mahalanobis distance exceeds the threshold
+    (an infinite one, from a covariance that is not positive definite, always does)"""
+    return bool(not md > prm["odometry_consistency_threshold"])
