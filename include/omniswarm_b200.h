@@ -567,6 +567,8 @@ typedef struct {
   double det_dpos_thres;
   double odom_pos_cov_per_m, odom_ang_cov_per_m;
   int32_t huber;                 /* 1 = HuberLoss(1.0) on every row (0 = debug_no_rejection) */
+  int32_t max_keyframes;         /* keyframes the distance store holds (osb_anchor_add_keyframe_dev); 0: no store */
+  int32_t max_keyframe_distances;/* distances of one keyframe, all its nodes together */
   int32_t reserved;
 } osb_anchor_params;
 typedef struct {                 /* a Swarm::LoopEdge (LOOP) or DroneDetection (DET4D / DET6D) */
@@ -806,6 +808,98 @@ osb_status osb_pcm_state_status(osb_pcm_state* s, osb_status* last);
 osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int n, const uint8_t* keep_dev,
                                           int32_t* type, int32_t* ia, int32_t* ib, double* payload, uint8_t* huber,
                                           int32_t* count_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * The UWB half of add_new_swarm_frame and of every solve, on the device.
+ * osb_anchor_add_keyframe_dev(): add_as_keyframe (swarm_localization_solver.cpp:517-540) for one keyframe the caller has
+ *   accepted (judge_is_key_frame, the block assignment, the odometry factors and set_window stay with the caller).  nodes
+ *   [n_nodes] in ascending drone id (SwarmFrame::id2nodeframe's order), each followed in `dists` by its n_distances
+ *   (peer, metres) pairs in ascending peer id (NodeFrame::dis_map's order).  On `stream`, without synchronising:
+ *   a. each node with new_block writes its block's initial pose (x y z yaw) into the solver's resident device poses:
+ *      a static node, or a dynamic one with prev_block < 0 that is not self_id before finish_init: the odometry position
+ *        plus a draw in [-5, 5) per axis (RAND_INIT_XY), the odometry yaw (:300-305, :329-335);
+ *      self_id before finish_init: the odometry pose (:306-310);
+ *      otherwise: Pose(prev block, yaw) * DeltaPose(prev_pose, pose, 4-DoF) (Predict_By_VO, :279-298).
+ *      A node with new_block == 0 writes nothing (the not-moving merge of :291-294, a static node's first block).  The
+ *      draw replaces rand(): splitmix64 of (seed, splitmix64(stamp) ^ (drone << 2 | axis)), as the multistart draws;
+ *   b. outlier_distance of each distance to a peer of this keyframe with vo_available (outlier_rejection_frame, :408-515):
+ *      before finish_init: |asin((z_peer - z) / d)| > elevation_threshold || !enable_distance, z the odometry heights;
+ *      after it: |d - |p_peer - p|| > outlier_threshold || d < minimum_distance || |asin((z_peer - z) / d)| >
+ *        elevation_threshold || !enable_distance, p the estimated positions of this keyframe (step a's and the resident
+ *        poses of reused blocks); a node absent from the previous keyframe is skipped, and the first node (in id order)
+ *        without vo_available there ends the walk -- its flags and those of every later node are not written (the
+ *        reference's `return`).  A NaN asin (|dz| > d) compares false.  The float thresholds are compared as doubles;
+ *        debug_no_rejection sets both thresholds to 1e8f and minimum_distance to -1 (:89-96);
+ *   c. stores the keyframe (its nodes, distances and flags: 1 outlier, 0 not, -1 not written) in the handle's ring of
+ *      max_keyframes slots, keyed by stamp; the oldest slot is overwritten.  A call whose slot holds a
+ *      keyframe of the window set last, and a set_window with a frame (holding entries) whose keyframe has left the ring,
+ *      are refused with OSB_ERR_CAPACITY: max_keyframes must cover the window.
+ *   One launch.  The inputs go through a pinned staging ring of 4 slots: a call waits (on the host) only for the call 4
+ *   before it.  Ordered after the solver's last device call and the handle's last keyframe, observe and
+ *   distance_factors_dev, on any stream.  The solver's host mirror is stale afterwards: its next host-side call waits
+ *   for this write and refreshes it, and its next device call starts from the written poses.
+ *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, max_keyframes == 0, n_nodes outside
+ *   1..max_drones, nodes not in ascending drone id, a drone or peer id outside 0..max_drones-1, peers not ascending, a
+ *   block or a used prev_block outside 0 .. the solver's node count - 1, a stamp already stored, the handles on different
+ *   devices; more distances than max_keyframe_distances gives OSB_ERR_CAPACITY.  The solver's next device call, on any
+ *   stream, waits for the write.  The first call acquires the store
+ *   (max_keyframes x (16 + 156 max_drones + 17 max_keyframe_distances) bytes and a frame table of 20 max_window_entries
+ *   bytes, sized once), the staging
+ *   ring and events, and synchronises.
+ * osb_anchor_keyframe_flags(): waits for the last keyframe and copies the stored flags of the keyframe at stamp_ns, in
+ *   `dists` order: *n = their count, -1 when the stamp is not stored; min(*n, cap) are written. */
+typedef struct {                 /* one NodeFrame of a keyframe, 152 bytes */
+  int32_t drone_id;
+  int32_t block;                 /* the pose block the caller assigned (est_poses_idts[id][ts]) */
+  int32_t new_block;             /* 1: a new block, its initial pose is written; 0: a reused block */
+  int32_t prev_block;            /* new dynamic block: the block of the drone's latest keyframe, -1 when it has none */
+  int32_t vo_available, is_static, frame_available, dists_available;
+  int32_t n_distances;           /* this node's pairs in the call's dists, following the previous nodes' */
+  int32_t reserved;
+  double pose[7];                /* odometry x y z qw qx qy qz */
+  double prev_pose[7];           /* the odometry at the drone's latest keyframe (read when prev_block is) */
+} osb_keyframe_node;
+typedef struct {
+  int32_t peer, reserved;
+  double distance;               /* metres */
+} osb_keyframe_distance;
+typedef struct {
+  int32_t self_id, finish_init, enable_distance, debug_no_rejection;
+  float outlier_threshold;       /* distance_measurement_outlier_threshold */
+  float elevation_threshold;     /* distance_measurement_outlier_elevation_threshold */
+  float minimum_distance;
+  int32_t reserved;
+  uint64_t seed;
+} osb_keyframe_params;
+osb_status osb_anchor_add_keyframe_dev(osb_anchor* h, osb_solver* s, int64_t stamp_ns, int n_nodes,
+                                       const osb_keyframe_node* nodes, int n_distances, const osb_keyframe_distance* dists,
+                                       const osb_keyframe_params* p, void* stream);
+osb_status osb_anchor_keyframe_flags(osb_anchor* h, int64_t stamp_ns, int8_t* flags, int cap, int32_t* n);
+/* osb_anchor_distance_factors_dev(): setup_problem_with_sferror (swarm_localization_solver.cpp:1102-1154) of every window
+ *   frame, appended to the SoA osb_anchor_compact_factors_dev wrote, at row *count_dev.  Goes between compact_factors_dev
+ *   and the resident solve (steady or multistart).  For each frame of the window set last whose stamp is stored, each
+ *   stored node a that has a window entry in that frame, and each of its distances to a peer b: one OSB_FACTOR_DISTANCE
+ *   row iff enable_distance && frame_available && dists_available (of a) && b < a && b has a window entry in the frame &&
+ *   the distance is not flagged an outlier (an unwritten flag is not) && (a == self_id || enable[a] of the last
+ *   osb_anchor_observe_dev).  Rows in frame order, then a, then b ascending; ia / ib = the window entries' blocks of a
+ *   and b; payload [d, 1 / sqrt((double)distance_measurement_cov), 0 ...] (the float parameter widened, then the fp64
+ *   square root and division); huber = !debug_no_rejection.  NodeFrame::distance_available (swarm_msgs, not in the
+ *   reference tree) is taken as "has a distance to b that is not flagged"; cutting_edges enables every distance
+ *   (:1225-1297).  A count that would pass max_tail (the buffers' rows) writes -1 to *count_dev and no row past max_tail,
+ *   so the solve refuses the tail; *count_dev < 0 on entry is left as it is.
+ *   One launch of one CTA (a block scan per frame: deterministic, no atomics).  Ordered after the handle's last observe and
+ *   keyframe on any stream; set_window and the next observe come after it.  Everything is read on the device, so the
+ *   call can be captured into a CUDA graph: a replay's rows follow that replay's observe and the window set before it.
+ *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, max_tail < 0, self_id outside
+ *   0..max_drones-1, max_keyframes == 0, or no observe_dev since create.  The first call acquires what the first
+ *   add_keyframe_dev does. */
+typedef struct {
+  int32_t self_id, enable_distance, debug_no_rejection;
+  float distance_measurement_cov;
+} osb_distance_params;
+osb_status osb_anchor_distance_factors_dev(osb_anchor* h, const osb_distance_params* p, int32_t* type, int32_t* ia,
+                                           int32_t* ib, double* payload, uint8_t* huber, int32_t* count_dev, int max_tail,
+                                           void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Geometric filter of the loop matcher (SURVEY.md 8f-1, first half) -- the inlier mask of

@@ -664,6 +664,231 @@ __global__ void predict_kernel(int n, const int32_t* __restrict__ drones, const 
   out[i] = o;
 }
 
+// add_as_keyframe's values (swarm_localization_solver.cpp:272-339, :408-515): one CTA, thread i owns node i for the
+// initial poses, then the threads stride over the keyframe's distances for the flags and the store.
+constexpr int KF_THREADS = 256;                                    // = ANCHOR_MAX_DRONES
+constexpr double RAND_INIT_XY = 5.0;                               // :51
+constexpr int KF_STAGING = 4;                                      // pinned input slots
+
+struct KeyframeView {
+  const osb_keyframe_node* nodes;     // the call's inputs (mapped pinned staging)
+  const osb_keyframe_distance* dists;
+  int n_nodes, n_dists, max_drones, max_dists;
+  int64_t stamp;
+  int self_id, finish_init, enable_distance;
+  double thr, elev, min_d;            // the float parameters, widened
+  uint64_t seed;
+  double* poses;                      // the solver's resident poses, [block][4]
+  int slot, prev_slot;                // the store slot written and the last keyframe's (-1: none)
+  int64_t* st_stamp;                  // [K]
+  int32_t* st_n;                      // [K] node count, -1: empty
+  osb_keyframe_node* st_node;         // [K][max_drones]
+  int32_t* st_first;                  // [K][max_drones + 1] distance offsets
+  osb_keyframe_distance* st_dist;     // [K][max_dists]
+  int8_t* st_flag;                    // [K][max_dists]
+};
+
+__device__ __forceinline__ double kf_draw(uint64_t seed, int64_t stamp, int drone, int comp) {
+  return counter_draw(seed, splitmix64((uint64_t)stamp) ^ (((uint64_t)(uint32_t)drone << 2) | (uint64_t)comp), RAND_INIT_XY);
+}
+__device__ __forceinline__ void store_pose4(double* dst, const double* t, double yaw) {   // to_vector_xyzyaw
+  dst[0] = t[0]; dst[1] = t[1]; dst[2] = t[2]; dst[3] = yaw;
+}
+// the node whose distances hold index k: the last i with first[i] <= k
+__device__ __forceinline__ int kf_owner(const int* first, int n, int k) {
+  int lo = 0, hi = n;                                              // first[lo] <= k < first[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (first[mid] <= k) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(KF_THREADS) keyframe_kernel(const KeyframeView v) {
+  __shared__ int s_node[ANCHOR_MAX_DRONES];                        // drone -> its node here, -1
+  __shared__ int s_last[ANCHOR_MAX_DRONES];                        // drone in the last keyframe: -1 absent, 0 no VO, 1 VO
+  __shared__ int s_first[ANCHOR_MAX_DRONES + 1];
+  __shared__ int s_stop;                                           // the node whose `return` ends the flag walk
+  const int t = threadIdx.x;
+  s_node[t] = -1;
+  s_last[t] = -1;
+  if (t == 0) {
+    s_stop = INT_MAX;
+    int acc = 0;
+    for (int i = 0; i < v.n_nodes; ++i) { s_first[i] = acc; acc += v.nodes[i].n_distances; }
+    s_first[v.n_nodes] = acc;
+  }
+  __syncthreads();
+  const bool mine = t < v.n_nodes;
+  if (v.prev_slot >= 0 && t < v.st_n[v.prev_slot]) {               // read before the slot is written: with one slot
+    const osb_keyframe_node& pn = v.st_node[(size_t)v.prev_slot * v.max_drones + t];   // the two are the same
+    s_last[pn.drone_id] = pn.vo_available ? 1 : 0;
+  }
+  __syncthreads();
+  osb_keyframe_node nd{};
+  if (mine) {
+    nd = v.nodes[t];
+    s_node[nd.drone_id] = t;
+    v.st_node[(size_t)v.slot * v.max_drones + t] = nd;
+  }
+  if (mine && nd.new_block) {                                      // a. the new block's initial pose
+    const PoseD vo = load_pose(nd.pose);
+    double* dst = v.poses + 4 * (size_t)nd.block;
+    const bool dynamic_predict = !nd.is_static && (nd.drone_id != v.self_id || v.finish_init) && nd.prev_block >= 0;
+    const bool self_vo = !nd.is_static && nd.drone_id == v.self_id && !v.finish_init;
+    if (dynamic_predict) {                                         // :279-298
+      const PoseD est_last = pose_from4(v.poses + 4 * (size_t)nd.prev_block);
+      const PoseD p = pose_mul(est_last, delta_pose4(load_pose(nd.prev_pose), vo));
+      store_pose4(dst, p.t, quat_yaw(p.q));
+    } else if (self_vo) {                                          // :306-310
+      store_pose4(dst, vo.t, quat_yaw(vo.q));
+    } else {                                                       // :300-305, :329-335
+      double p[3];
+      for (int c = 0; c < 3; ++c) p[c] = __dadd_rn(vo.t[c], kf_draw(v.seed, v.stamp, nd.drone_id, c));
+      store_pose4(dst, p, quat_yaw(vo.q));
+    }
+  }
+  __syncthreads();                                                 // s_last is complete, the new poses are visible
+  if (mine && v.finish_init && s_last[nd.drone_id] == 0) atomicMin(&s_stop, t);
+  for (int i = t; i <= v.n_nodes; i += KF_THREADS) v.st_first[(size_t)v.slot * (v.max_drones + 1) + i] = s_first[i];
+  __syncthreads();
+  for (int k = t; k < v.n_dists; k += KF_THREADS) {                // b. and c.
+    const int i = kf_owner(s_first, v.n_nodes, k);
+    const osb_keyframe_node* here = v.st_node + (size_t)v.slot * v.max_drones;   // written above, read from the device
+    const osb_keyframe_node& a = here[i];
+    const osb_keyframe_distance dk = v.dists[k];
+    const int jn = s_node[dk.peer];
+    int flag = -1;
+    if (jn >= 0 && here[jn].vo_available) {
+      const osb_keyframe_node& b = here[jn];
+      const double dis = dk.distance;
+      if (!v.finish_init) {                                        // :427-438
+        const double dh = __dadd_rn(b.pose[2], -a.pose[2]);
+        flag = (fabs(asin(dh / dis)) > v.elev || !v.enable_distance) ? 1 : 0;
+      } else if (i < s_stop && s_last[a.drone_id] == 1) {          // :454-460, then :489-507
+        const double* pa = v.poses + 4 * (size_t)a.block;
+        const double* pb = v.poses + 4 * (size_t)b.block;
+        const double dx = __dadd_rn(pb[0], -pa[0]), dy = __dadd_rn(pb[1], -pa[1]), dz = __dadd_rn(pb[2], -pa[2]);
+        const double est = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+        flag = (fabs(__dadd_rn(dis, -est)) > v.thr || dis < v.min_d || fabs(asin(dz / dis)) > v.elev ||
+                !v.enable_distance) ? 1 : 0;
+      }
+    }
+    const size_t o = (size_t)v.slot * v.max_dists + k;
+    v.st_dist[o] = dk;
+    v.st_flag[o] = (int8_t)flag;
+  }
+  if (t == 0) {
+    v.st_stamp[v.slot] = v.stamp;
+    v.st_n[v.slot] = v.n_nodes;
+  }
+}
+
+// setup_problem_with_sferror of every window frame (:1102-1154): one CTA walks the frames in order; per frame a block
+// scan over the stored distances gives each kept one its row, in (a, b) order (no atomics).
+constexpr int DF_THREADS = 1024, DF_WARPS = DF_THREADS / 32;
+
+struct DistanceView {
+  const int64_t* w_stamp;             // the window: frame stamps, frame_first, each entry's drone and block
+  const int32_t *w_first, *w_drone, *w_block, *w_n;
+  const int64_t* st_stamp;
+  const int32_t* st_n;
+  const osb_keyframe_node* st_node;
+  const int32_t* st_first;
+  const osb_keyframe_distance* st_dist;
+  const int8_t* st_flag;
+  int slots, max_drones, max_dists;
+  const osb_observability* obs;
+  int self_id, enable_distance, huber;
+  double sqrt_inf;
+  int32_t *type, *ia, *ib;
+  double* payload;
+  uint8_t* hub;
+  int32_t* count;
+  int max_tail;
+};
+
+__global__ void __launch_bounds__(DF_THREADS) distance_factors_kernel(const DistanceView v) {
+  __shared__ int s_blk[ANCHOR_MAX_DRONES];                         // drone -> its block in the frame, -1
+  __shared__ int s_first[ANCHOR_MAX_DRONES + 1];
+  __shared__ int s_warp[DF_WARPS];
+  __shared__ int s_slot;
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const int base = *v.count;
+  __syncthreads();                                                 // every thread has read it before thread 0 rewrites it
+  if (base < 0) return;                                            // the tail is refused already
+  const int nf = *v.w_n;
+  int out = base;
+  for (int f = 0; f < nf; ++f) {
+    if (t < ANCHOR_MAX_DRONES) s_blk[t] = -1;
+    if (t == 0) s_slot = -1;
+    __syncthreads();
+    const int64_t ts = v.w_stamp[f];
+    for (int s = t; s < v.slots; s += DF_THREADS)                  // stamps are unique among the stored keyframes
+      if (v.st_n[s] >= 0 && v.st_stamp[s] == ts) s_slot = s;
+    for (int e = v.w_first[f] + t; e < v.w_first[f + 1]; e += DF_THREADS) s_blk[v.w_drone[e]] = v.w_block[e];
+    __syncthreads();
+    const int slot = s_slot;
+    const int nn = slot >= 0 ? v.st_n[slot] : 0;
+    if (slot >= 0)
+      for (int i = t; i <= nn; i += DF_THREADS) s_first[i] = v.st_first[(size_t)slot * (v.max_drones + 1) + i];
+    __syncthreads();
+    const int nd = slot >= 0 ? s_first[nn] : 0;
+    for (int k0 = 0; k0 < nd; k0 += DF_THREADS) {
+      const int k = k0 + t;
+      bool sel = false;
+      int ba = 0, bb = 0;
+      double dis = 0.0;
+      if (k < nd) {
+        const osb_keyframe_node& a = v.st_node[(size_t)slot * v.max_drones + kf_owner(s_first, nn, k)];
+        const size_t o = (size_t)slot * v.max_dists + k;
+        const int ida = a.drone_id, idb = v.st_dist[o].peer;
+        dis = v.st_dist[o].distance;
+        sel = v.enable_distance && a.frame_available && a.dists_available && idb < ida && v.st_flag[o] != 1 &&
+              (ida == v.self_id || v.obs->enable[ida]);
+        if (sel) {
+          ba = s_blk[ida];
+          bb = s_blk[idb];
+          sel = ba >= 0 && bb >= 0;
+        }
+      }
+      int inc = sel ? 1 : 0;                                       // block scan of the kept distances
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += u;
+      }
+      if (lane == 31) s_warp[wid] = inc;
+      __syncthreads();
+      if (wid == 0) {
+        int w = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int u = __shfl_up_sync(0xffffffffu, w, o);
+          if (lane >= o) w += u;
+        }
+        s_warp[lane] = w;
+      }
+      __syncthreads();
+      const int row = out + (wid > 0 ? s_warp[wid - 1] : 0) + inc - (sel ? 1 : 0);
+      const int total = s_warp[DF_WARPS - 1];
+      if (sel && row < v.max_tail) {
+        v.type[row] = OSB_FACTOR_DISTANCE;
+        v.ia[row] = ba;
+        v.ib[row] = bb;
+        v.hub[row] = (uint8_t)v.huber;
+        double* pl = v.payload + (size_t)row * OSB_PAYLOAD_LEN;
+        pl[0] = dis;
+        pl[1] = v.sqrt_inf;
+        for (int j = 2; j < OSB_PAYLOAD_LEN; ++j) pl[j] = 0.0;
+      }
+      out += total;
+      __syncthreads();                                             // s_warp is rewritten by the next tile
+    }
+  }
+  if (t == 0) *v.count = out > v.max_tail ? -1 : out;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -736,6 +961,26 @@ struct osb_anchor {
   int32_t* d_pred_drone = nullptr;
   double* d_pred_vo = nullptr;
   osb_predict_result* d_pred_out = nullptr;
+  // the keyframe store (osb_anchor_add_keyframe_dev / distance_factors_dev), acquired by the first of them: a ring of
+  // max_keyframes slots, the window's frame table (set_window keeps it current after that), the pinned staging ring
+  int64_t* d_st_stamp = nullptr;
+  int32_t *d_st_n = nullptr, *d_st_first = nullptr;
+  osb_keyframe_node* d_st_node = nullptr;
+  osb_keyframe_distance* d_st_dist = nullptr;
+  int8_t* d_st_flag = nullptr;
+  std::vector<int64_t> st_stamp;                  // the host's record of the ring: each slot's stamp
+  std::vector<int32_t> st_count;                  // ... its distance count, -1: empty
+  long long kf_seq = 0;                           // keyframes added
+  int kf_last_slot = -1;
+  cudaEvent_t last_keyframe = nullptr;
+  char* kf_stage[KF_STAGING] = {};                // pinned, mapped: nodes [max_drones] then dists [max_dists]
+  char* kf_stage_dev[KF_STAGING] = {};
+  cudaEvent_t kf_stage_ev[KF_STAGING] = {};
+  std::vector<int64_t> kw_stamp;                  // the window's frames (set_window), host side
+  std::vector<int32_t> kw_first, kw_drone, kw_block;
+  int64_t* d_kw_stamp = nullptr;
+  int32_t *d_kw_first = nullptr, *d_kw_drone = nullptr, *d_kw_block = nullptr, *d_kw_n = nullptr;
+  int64_t kf_evicted = INT64_MIN;                 // the largest stamp whose slot a later keyframe took
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -755,6 +1000,23 @@ osb_status anchor_wait_last_run(osb_anchor* h) {
   OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_run, 0));
   if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
   if (h->last_sync) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_sync, 0));
+  if (h->last_keyframe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_keyframe, 0));
+  return OSB_OK;
+}
+
+// the window's frame table of distance_factors_dev to the device, on the handle's stream (the caller synchronises)
+osb_status upload_kf_window(osb_anchor* h) {
+  const size_t nf = h->kw_stamp.size();           // <= max_window_entries: set_window keeps the frames with entries
+  cudaStream_t st = h->stream;
+  const int32_t n = (int32_t)nf;
+  const size_t ne = h->kw_drone.size();
+  OSB_CUDA(cudaMemcpyAsync(h->d_kw_n, &n, sizeof(n), cudaMemcpyHostToDevice, st));
+  OSB_CUDA(cudaMemcpyAsync(h->d_kw_first, h->kw_first.data(), (nf + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (nf > 0) OSB_CUDA(cudaMemcpyAsync(h->d_kw_stamp, h->kw_stamp.data(), nf * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  if (ne > 0) {
+    OSB_CUDA(cudaMemcpyAsync(h->d_kw_drone, h->kw_drone.data(), ne * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OSB_CUDA(cudaMemcpyAsync(h->d_kw_block, h->kw_block.data(), ne * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
   return OSB_OK;
 }
 
@@ -872,6 +1134,8 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
   OSB_REQUIRE(p->max_traj_samples > 0 && p->max_measurements > 0 && p->max_window_entries > 0, "capacities must be positive");
   OSB_REQUIRE((long long)p->max_drones * p->max_traj_samples < (1ll << 31), "max_drones x max_traj_samples too large");
   OSB_REQUIRE(p->begin_min_loop_dt_s >= 0.0 && p->begin_min_loop_dt_s < 9.0e9, "begin_min_loop_dt_s out of range");
+  OSB_REQUIRE(p->max_keyframes >= 0 && (p->max_keyframes == 0 || p->max_keyframe_distances > 0),
+              "max_keyframes must be >= 0, and max_keyframe_distances positive when it is not");
   OSB_TRY(require_device());
   std::unique_ptr<osb_anchor> h(new osb_anchor());
   h->device = current_device();
@@ -913,6 +1177,7 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
   h->h_slot.reserve(M);
   observe_window(h->obs_win, p->max_drones, 0, 0, nullptr);
   sync_window(h.get(), 0, nullptr, nullptr, nullptr);
+  h->kw_first.assign(1, 0);
   *out = h.release();
   return OSB_OK;
 }
@@ -1040,6 +1305,16 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
       OSB_REQUIRE(drone_ok(h, entries[a].drone_id), "drone id outside 0..max_drones-1");
       for (int b = frame_first[f]; b < a; ++b) OSB_REQUIRE(entries[b].drone_id != entries[a].drone_id, "a drone twice in one frame");
     }
+  if (h->d_kw_n)                                                   // a keyframe whose slot was taken has no rows left
+    for (int f = 0; f < n_frames; ++f) {
+      if (frame_first[f + 1] == frame_first[f] || frame_stamps_ns[f] > h->kf_evicted) continue;
+      bool stored = false;
+      for (int k = 0; k < h->p.max_keyframes && !stored; ++k) stored = h->st_count[k] >= 0 && h->st_stamp[k] == frame_stamps_ns[f];
+      if (!stored) {
+        set_error(__func__, "a window frame's keyframe has left the store: max_keyframes does not cover the window");
+        return OSB_ERR_CAPACITY;
+      }
+    }
   DeviceGuard dg(h->device);
   // per-drone index of the vo_available entries in frame order (a counting sort by drone)
   const int D = h->p.max_drones;
@@ -1088,6 +1363,14 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
   }
   sync_window(h, n_frames, frame_stamps_ns, frame_first, entries);
   if (h->d_sync_win) OSB_TRY(upload_sync_window(h));
+  h->kw_stamp.clear();                                             // the frames that hold entries: no other has rows
+  h->kw_first.assign(1, 0);
+  for (int f = 0; f < n_frames; ++f)
+    if (frame_first[f + 1] > frame_first[f]) { h->kw_stamp.push_back(frame_stamps_ns[f]); h->kw_first.push_back(frame_first[f + 1]); }
+  h->kw_drone.resize(n_entries);
+  h->kw_block.resize(n_entries);
+  for (int e = 0; e < n_entries; ++e) { h->kw_drone[e] = entries[e].drone_id; h->kw_block[e] = entries[e].block; }
+  if (h->d_kw_n) OSB_TRY(upload_kf_window(h));
   OSB_CUDA(cudaStreamSynchronize(st));
   if (h->d_blk_drone) OSB_TRY(upload_blocks(h));
   h->n_frames = n_frames;
@@ -1464,5 +1747,188 @@ extern "C" osb_status osb_anchor_predict(osb_anchor* h, const osb_predict_params
   OSB_CHECK_LAUNCH();
   OSB_CUDA(cudaMemcpyAsync(out, h->d_pred_out, (size_t)n * sizeof(osb_predict_result), cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
+}
+
+namespace {
+
+// the first keyframe or distance_factors_dev call acquires the store (every slot empty), the window's frame table (the
+// host's), the staging ring and the events
+osb_status kf_init(osb_anchor* h) {
+  if (h->d_kw_n) return OSB_OK;
+  const size_t K = (size_t)h->p.max_keyframes, D = (size_t)h->p.max_drones, M = (size_t)h->p.max_keyframe_distances;
+  const size_t E = (size_t)h->p.max_window_entries;
+  Resources& R = h->res;
+  OSB_TRY(R.alloc(&h->d_st_stamp, K));
+  OSB_TRY(R.alloc(&h->d_st_n, K));
+  OSB_TRY(R.alloc(&h->d_st_node, K * D));
+  OSB_TRY(R.alloc(&h->d_st_first, K * (D + 1)));
+  OSB_TRY(R.alloc(&h->d_st_dist, K * M));
+  OSB_TRY(R.alloc(&h->d_st_flag, K * M));
+  OSB_TRY(R.alloc(&h->d_kw_drone, E));
+  OSB_TRY(R.alloc(&h->d_kw_stamp, E));
+  OSB_TRY(R.alloc(&h->d_kw_first, E + 1));
+  OSB_TRY(R.alloc(&h->d_kw_block, E));
+  OSB_TRY(R.event(&h->last_keyframe, cudaEventDisableTiming));
+  const size_t stage = D * sizeof(osb_keyframe_node) + M * sizeof(osb_keyframe_distance);
+  for (int k = 0; k < KF_STAGING; ++k) {
+    OSB_TRY(R.host_alloc(&h->kf_stage[k], stage, cudaHostAllocMapped));
+    OSB_CUDA(cudaHostGetDevicePointer((void**)&h->kf_stage_dev[k], h->kf_stage[k], 0));
+    OSB_TRY(R.event(&h->kf_stage_ev[k], cudaEventDisableTiming));
+  }
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaMemsetAsync(h->d_st_n, 0xff, K * sizeof(int32_t), st));
+  int32_t* n = nullptr;
+  OSB_TRY(R.alloc(&n, 1));
+  h->d_kw_n = n;
+  const osb_status s = upload_kf_window(h);
+  if (s != OSB_OK) { h->d_kw_n = nullptr; return s; }
+  for (int k = 0; k < KF_STAGING; ++k) OSB_CUDA(cudaEventRecord(h->kf_stage_ev[k], st));
+  OSB_CUDA(cudaEventRecord(h->last_keyframe, st));
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { h->d_kw_n = nullptr; OSB_CUDA(e); }      // a failed first call is tried again
+  h->st_stamp.assign(K, 0);
+  h->st_count.assign(K, -1);
+  return OSB_OK;
+}
+
+}  // namespace
+
+extern "C" osb_status osb_anchor_add_keyframe_dev(osb_anchor* h, osb_solver* s, int64_t stamp_ns, int n_nodes,
+                                                  const osb_keyframe_node* nodes, int n_distances,
+                                                  const osb_keyframe_distance* dists, const osb_keyframe_params* p,
+                                                  void* stream) {
+  OSB_REQUIRE(h != nullptr && s != nullptr && p != nullptr && nodes != nullptr, "null argument");
+  OSB_REQUIRE(n_distances >= 0 && (n_distances == 0 || dists != nullptr), "null dists or negative count");
+  OSB_REQUIRE(h->p.max_keyframes > 0, "the handle was created with max_keyframes == 0");
+  OSB_REQUIRE(n_nodes >= 1 && n_nodes <= h->p.max_drones, "n_nodes outside 1..max_drones");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  long long total = 0;
+  for (int i = 0; i < n_nodes; ++i) {
+    OSB_REQUIRE(drone_ok(h, nodes[i].drone_id), "drone id outside 0..max_drones-1");
+    OSB_REQUIRE(i == 0 || nodes[i].drone_id > nodes[i - 1].drone_id, "nodes must be in ascending drone id");
+    OSB_REQUIRE(nodes[i].n_distances >= 0 && nodes[i].n_distances <= h->p.max_drones, "n_distances outside 0..max_drones");
+    total += nodes[i].n_distances;
+  }
+  OSB_REQUIRE(total == n_distances, "the nodes' n_distances do not sum to n_distances");
+  for (int i = 0, k = 0; i < n_nodes; ++i)
+    for (int j = 0; j < nodes[i].n_distances; ++j, ++k) {
+      OSB_REQUIRE(drone_ok(h, dists[k].peer), "peer id outside 0..max_drones-1");
+      OSB_REQUIRE(j == 0 || dists[k].peer > dists[k - 1].peer, "a node's peers must be in ascending id");
+    }
+  if (n_distances > h->p.max_keyframe_distances) {
+    set_error(__func__, "the keyframe has more distances than max_keyframe_distances");
+    return OSB_ERR_CAPACITY;
+  }
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(kf_init(h));
+  for (int k = 0; k < h->p.max_keyframes; ++k)
+    OSB_REQUIRE(h->st_count[k] < 0 || h->st_stamp[k] != stamp_ns, "a keyframe with this stamp is already stored");
+  cudaStream_t st = (cudaStream_t)stream;
+  SolverPoseWrite w{};
+  {
+    int solver_dev = 0;
+    const int n_blocks = solver_node_count(s, &solver_dev);   // checked before anything is enqueued
+    OSB_REQUIRE(solver_dev == h->device, "the anchor and the solver are on different devices");
+    for (int i = 0; i < n_nodes; ++i) {
+      const osb_keyframe_node& nd = nodes[i];
+      OSB_REQUIRE(nd.block >= 0 && nd.block < n_blocks, "a block outside 0 .. the solver's node count - 1");
+      const bool uses_prev = nd.new_block && !nd.is_static && (nd.drone_id != p->self_id || p->finish_init);
+      OSB_REQUIRE(!uses_prev || (nd.prev_block >= -1 && nd.prev_block < n_blocks),
+                  "a prev_block outside -1 .. the solver's node count - 1");
+    }
+  }
+  const int slot = (int)(h->kf_seq % h->p.max_keyframes), stage = (int)(h->kf_seq % KF_STAGING);
+  if (h->st_count[slot] >= 0)
+    for (const int64_t ts : h->kw_stamp)
+      if (ts == h->st_stamp[slot]) {
+        set_error(__func__, "the oldest stored keyframe is still in the window: max_keyframes does not cover it");
+        return OSB_ERR_CAPACITY;
+      }
+  OSB_TRY(solver_pose_write(s, st, &w));
+  OSB_CUDA(cudaEventSynchronize(h->kf_stage_ev[stage]));           // the call KF_STAGING before has read its inputs
+  const size_t D = (size_t)h->p.max_drones;
+  memcpy(h->kf_stage[stage], nodes, (size_t)n_nodes * sizeof(osb_keyframe_node));
+  char* dist_stage = h->kf_stage[stage] + D * sizeof(osb_keyframe_node);
+  if (n_distances > 0) memcpy(dist_stage, dists, (size_t)n_distances * sizeof(osb_keyframe_distance));
+  KeyframeView v{};
+  v.nodes = reinterpret_cast<const osb_keyframe_node*>(h->kf_stage_dev[stage]);
+  v.dists = reinterpret_cast<const osb_keyframe_distance*>(h->kf_stage_dev[stage] + D * sizeof(osb_keyframe_node));
+  v.n_nodes = n_nodes; v.n_dists = n_distances; v.max_drones = h->p.max_drones; v.max_dists = h->p.max_keyframe_distances;
+  v.stamp = stamp_ns;
+  v.self_id = p->self_id; v.finish_init = p->finish_init ? 1 : 0; v.enable_distance = p->enable_distance ? 1 : 0;
+  const bool no_rej = p->debug_no_rejection != 0;                  // :89-96
+  v.thr = (double)(no_rej ? 1e8f : p->outlier_threshold);
+  v.elev = (double)(no_rej ? 1e8f : p->elevation_threshold);
+  v.min_d = (double)(no_rej ? -1.0f : p->minimum_distance);
+  v.seed = p->seed;
+  v.poses = w.poses;
+  v.slot = slot; v.prev_slot = h->kf_last_slot;
+  v.st_stamp = h->d_st_stamp; v.st_n = h->d_st_n; v.st_node = h->d_st_node; v.st_first = h->d_st_first;
+  v.st_dist = h->d_st_dist; v.st_flag = h->d_st_flag;
+  OSB_CUDA(wait_event_capturable(st, h->last_keyframe));          // the store is the last keyframe's ...
+  if (h->last_observe) OSB_CUDA(wait_event_capturable(st, h->last_observe));   // ... and distance_factors_dev reads it
+  OSB_LAUNCH(keyframe_kernel, 1, KF_THREADS, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(w.written, st));
+  OSB_CUDA(record_event_capturable(h->kf_stage_ev[stage], st));
+  OSB_CUDA(record_event_capturable(h->last_keyframe, st));
+  if (h->st_count[slot] >= 0) h->kf_evicted = std::max(h->kf_evicted, h->st_stamp[slot]);
+  h->st_stamp[slot] = stamp_ns;
+  h->st_count[slot] = n_distances;
+  h->kf_last_slot = slot;
+  ++h->kf_seq;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_keyframe_flags(osb_anchor* h, int64_t stamp_ns, int8_t* flags, int cap, int32_t* n) {
+  OSB_REQUIRE(h != nullptr && n != nullptr && cap >= 0 && (cap == 0 || flags != nullptr), "null argument or negative cap");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *n = -1;
+  if (!h->d_kw_n) return OSB_OK;
+  int slot = -1;
+  for (int k = 0; k < h->p.max_keyframes; ++k)
+    if (h->st_count[k] >= 0 && h->st_stamp[k] == stamp_ns) slot = k;
+  if (slot < 0) return OSB_OK;
+  *n = h->st_count[slot];
+  const int m = std::min(*n, cap);
+  if (m == 0) return OSB_OK;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaStreamWaitEvent(st, h->last_keyframe, 0));
+  OSB_CUDA(cudaMemcpyAsync(flags, h->d_st_flag + (size_t)slot * h->p.max_keyframe_distances, (size_t)m,
+                           cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_distance_factors_dev(osb_anchor* h, const osb_distance_params* p, int32_t* type,
+                                                      int32_t* ia, int32_t* ib, double* payload, uint8_t* huber,
+                                                      int32_t* count_dev, int max_tail, void* stream) {
+  OSB_REQUIRE(h != nullptr && p != nullptr && type && ia && ib && payload && huber && count_dev, "null argument");
+  OSB_REQUIRE(max_tail >= 0, "max_tail must be >= 0");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  OSB_REQUIRE(h->p.max_keyframes > 0, "the handle was created with max_keyframes == 0");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->d_obs != nullptr, "no osb_anchor_observe_dev call on this handle: enable is not set");
+  DeviceGuard dg(h->device);
+  OSB_TRY(kf_init(h));
+  DistanceView v{};
+  v.w_stamp = h->d_kw_stamp; v.w_first = h->d_kw_first; v.w_drone = h->d_kw_drone; v.w_block = h->d_kw_block;
+  v.w_n = h->d_kw_n;
+  v.st_stamp = h->d_st_stamp; v.st_n = h->d_st_n; v.st_node = h->d_st_node; v.st_first = h->d_st_first;
+  v.st_dist = h->d_st_dist; v.st_flag = h->d_st_flag;
+  v.slots = h->p.max_keyframes; v.max_drones = h->p.max_drones; v.max_dists = h->p.max_keyframe_distances;
+  v.obs = h->d_obs;
+  v.self_id = p->self_id; v.enable_distance = p->enable_distance ? 1 : 0; v.huber = p->debug_no_rejection ? 0 : 1;
+  v.sqrt_inf = 1.0 / sqrt((double)p->distance_measurement_cov);
+  v.type = type; v.ia = ia; v.ib = ib; v.payload = payload; v.hub = huber; v.count = count_dev; v.max_tail = max_tail;
+  cudaStream_t st = (cudaStream_t)stream;
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // enable is the last observe's
+  OSB_CUDA(wait_event_capturable(st, h->last_keyframe));          // the store is the last keyframe's
+  OSB_LAUNCH(distance_factors_kernel, 1, DF_THREADS, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
   return OSB_OK;
 }

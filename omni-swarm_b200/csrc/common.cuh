@@ -304,9 +304,36 @@ struct SolverDeviceCall {
 // OSB_ERR_INVALID (error text set) when the solver made no device call since its last host-side pose or graph change
 osb_status solver_device_call(osb_solver* h, SolverDeviceCall* out);
 
+// A write into the solver's resident device poses from another handle's kernel (osb_anchor_add_keyframe_dev; graph.cu,
+// not part of the C ABI).  solver_pose_write makes the device copy current (uploading the host mirror when the last
+// change was host-side), orders `st` after the solver's last device call and marks the host mirror stale; the caller
+// launches its write on `st` and then records `written` there.  The next host-side call of the solver waits for that
+// event and refreshes its mirror from the device; the next device call starts from the device values.
+struct SolverPoseWrite {
+  int device;
+  int n_nodes;                            // the resident graph's node count
+  double* poses;                          // [n_nodes][4] x y z yaw, caller's node order
+  cudaEvent_t written;
+};
+osb_status solver_pose_write(osb_solver* h, cudaStream_t st, SolverPoseWrite* out);
+int solver_node_count(osb_solver* h, int* device);   // the resident graph's node count and the solver's device, without
+                                                   // waiting for a device call
+
 // ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------
+// Counter-based draws: a value depends only on (seed, key), not on the launch shape or the other draws.  No FMA, so numpy
+// restates it bit for bit (oracle/multistart_ref.py).
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ double counter_draw(uint64_t seed, uint64_t key, double r) {   // [-r, r)
+  const double u = (double)(splitmix64(seed ^ splitmix64(key)) >> 11) * 0x1p-53;          // [0, 1)
+  return __dadd_rn(__dmul_rn(2.0 * r, u), -r);
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

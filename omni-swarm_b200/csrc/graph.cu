@@ -999,18 +999,11 @@ __global__ void graph_linearize_kernel(int m, const double* __restrict__ poses, 
 }
 
 // ---- random-restart initialisation (osb_solver_solve_multistart) ----------------------------------------------------
-// Counter-based draws: a value depends only on (seed, trial, caller's node id, component), not on the launch shape, the
-// chain plan or the other nodes.  No FMA anywhere, so numpy restates it bit for bit (oracle/multistart_ref.py).
-__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
+// A draw depends only on (seed, trial, caller's node id, component), not on the launch shape, the chain plan or the other
+// nodes (common.cuh's counter_draw).
 __device__ __forceinline__ double multistart_draw(uint64_t seed, int trial, int node, int comp, double r) {
   const uint64_t key = ((uint64_t)trial << 34) | ((uint64_t)(uint32_t)node << 2) | (uint64_t)comp;
-  const double u = (double)(splitmix64(seed ^ splitmix64(key)) >> 11) * 0x1p-53;   // [0, 1)
-  return __dadd_rn(__dmul_rn(2.0 * r, u), -r);                                      // [-r, r)
+  return counter_draw(seed, key, r);
 }
 
 // trial t's starting poses, internal order: random_init_pose (solver.cpp:204-216) on the masked free nodes -- x, y in
@@ -1430,6 +1423,10 @@ struct osb_solver {
   std::vector<osb_solve_summary> dev_ms_summaries;
   std::vector<double> dev_ms_equv;
   int32_t dev_ms_chosen = -1;
+  // a write into d_rposes by another handle (solver_pose_write): g_poses is stale until a host-side call waits for
+  // ev_write and copies d_rposes back
+  bool pose_written = false;
+  cudaEvent_t ev_write = nullptr;
 };
 
 static osb_status finish_device_call(osb_solver* h);
@@ -2060,8 +2057,20 @@ static size_t tail_layout(TailDev& D, char* base, size_t n, size_t m) {
 
 // The first host-side call after a device call waits for it and refreshes the host mirror of the poses, the call's status
 // and its summary.  A captured call stays pending: every host-side call re-reads what the last replay left (the caller
-// has synchronised it), until a host-side change of the poses or the graph takes over.  The caller holds h->mu.
+// has synchronised it), until a host-side change of the poses or the graph takes over.  A pose write by another handle
+// came after that call (solver_pose_write orders it so): its values reach g_poses last.  The caller holds h->mu.
+static osb_status finish_solve_call(osb_solver* h);
 static osb_status finish_device_call(osb_solver* h) {
+  OSB_TRY(finish_solve_call(h));
+  if (!h->pose_written) return OSB_OK;
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaStreamWaitEvent(st, h->ev_write, 0));
+  OSB_CUDA(cudaMemcpyAsync(h->g_poses.data(), h->d_rposes, h->g_poses.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  h->pose_written = false;
+  return OSB_OK;
+}
+static osb_status finish_solve_call(osb_solver* h) {
   if (!h->dev_pending) return OSB_OK;
   if (!h->dev_captured) h->dev_pending = false;
   if (!h->dev_captured) OSB_CUDA(cudaEventSynchronize(h->ev_done));
@@ -2148,7 +2157,7 @@ static osb_status resident_dev_call(osb_solver* h, int max_tail, const int32_t* 
     if (h->d_tail == nullptr) {                // everything a device call needs, once per handle
       TailDev D = {};
       OSB_TRY(h->res.alloc(&h->d_tail, tail_layout(D, nullptr, h->max_nodes, h->max_factors)));
-      OSB_TRY(h->res.alloc(&h->d_rposes, 4 * (size_t)h->max_nodes));
+      if (!h->d_rposes) OSB_TRY(h->res.alloc(&h->d_rposes, 4 * (size_t)h->max_nodes));   // or solver_pose_write's
       OSB_TRY(h->res.alloc(&h->d_tsummary, 1));
       OSB_TRY(h->res.event(&h->ev_done));
       tail_layout(h->tail, h->d_tail, h->max_nodes, h->max_factors);
@@ -2217,6 +2226,7 @@ static osb_status resident_dev_call(osb_solver* h, int max_tail, const int32_t* 
   D.huber_o = h->d_huber; D.fixed_o = h->d_fixed; D.link_o = h->d_link;
   D.poses = h->d_rposes; D.x0 = P.x[0]; D.x_out = P.poses_out;
   h->cached_topo = 0;                          // the one-shot index tables now hold this call's list
+  if (h->ev_write) OSB_CUDA(wait_event_capturable(st, h->ev_write));   // the last solver_pose_write, on any stream
   OSB_LAUNCH(tail_rank_kernel, D.chunks, 2 * TL_ROWS, 0, st, D);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(tail_scan_kernel, cdiv((int)n, 256), 256, 0, st, D);
@@ -2262,6 +2272,34 @@ osb_status osb::solver_device_call(osb_solver* h, SolverDeviceCall* out) {
   out->summary = h->d_tsummary;
   out->chosen = &h->d_res->chosen;
   out->done = h->ev_done;
+  return OSB_OK;
+}
+
+int osb::solver_node_count(osb_solver* h, int* device) {
+  std::lock_guard<std::mutex> lk(h->mu);
+  *device = h->device;
+  return (int)h->g_fixed.size();
+}
+
+osb_status osb::solver_pose_write(osb_solver* h, cudaStream_t st, SolverPoseWrite* out) {
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  const size_t n = h->g_fixed.size();
+  if (n == 0) { set_error("osb_anchor_add_keyframe_dev", "the solver's resident graph is empty"); return OSB_ERR_INVALID; }
+  if (!h->d_rposes) OSB_TRY(h->res.alloc(&h->d_rposes, 4 * (size_t)h->max_nodes));
+  if (!h->ev_write) OSB_TRY(h->res.event(&h->ev_write, cudaEventDisableTiming));
+  if (h->dev_called) OSB_CUDA(wait_event_capturable(st, h->ev_done));   // the last device call's poses come first
+  if (!h->rposes_current) {                    // the last change was host-side: the mirror goes up first
+    cudaStream_t hs = h->stream;
+    OSB_CUDA(cudaMemcpyAsync(h->d_rposes, h->g_poses.data(), 4 * n * sizeof(double), cudaMemcpyHostToDevice, hs));
+    OSB_CUDA(cudaStreamSynchronize(hs));       // the solver's own stream: the caller's is not waited for
+    h->rposes_current = true;
+  }
+  h->pose_written = true;
+  out->device = h->device;
+  out->n_nodes = (int)n;
+  out->poses = h->d_rposes;
+  out->written = h->ev_write;
   return OSB_OK;
 }
 

@@ -906,13 +906,17 @@ class LoopAnchor(_Handle):
 
     def __init__(self, max_drones: int, max_traj_samples: int, max_measurements: int, max_window_entries: int,
                  det_dpos_thres: float, odom_pos_cov_per_m: float, odom_ang_cov_per_m: float,
-                 begin_min_loop_dt_s: float = 1000.0, huber: bool = True):
+                 begin_min_loop_dt_s: float = 1000.0, huber: bool = True, max_keyframes: int = 256,
+                 max_keyframe_distances: int | None = None):
         self._lib = _l.load()
         self._h = C.c_void_p()
         self.max_drones = int(max_drones)
+        if max_keyframe_distances is None:                 # every ordered drone pair, up to 4096
+            max_keyframe_distances = min(self.max_drones * self.max_drones, 4096)
         p = _l.AnchorParams(self.max_drones, int(max_traj_samples), int(max_measurements), int(max_window_entries),
                             float(begin_min_loop_dt_s), float(det_dpos_thres), float(odom_pos_cov_per_m),
-                            float(odom_ang_cov_per_m), int(bool(huber)), 0)
+                            float(odom_ang_cov_per_m), int(bool(huber)), int(max_keyframes),
+                            int(max_keyframe_distances), 0)
         _l.check(self._lib.osb_anchor_create(C.byref(self._h), C.byref(p)))
 
     def push_odometry(self, drone: int, stamps_ns, poses):
@@ -1029,6 +1033,47 @@ class LoopAnchor(_Handle):
         _l.check(self._lib.osb_anchor_predict(self._h, C.byref(p), len(d), _l.ptr(d), _l.ptr(vo), C.cast(out, C.c_void_p)))
         return {int(d[i]): (np.array(out[i].node_pose) if out[i].node_valid else None,
                             np.array(out[i].base_pose) if out[i].base_valid else None) for i in range(len(d))}
+
+    def add_keyframe_dev(self, solver: PoseGraphSolver, stamp_ns: int, nodes, dists, stream: int, self_id: int,
+                         finish_init: bool, enable_distance: bool = True, outlier_threshold: float = 0.3,
+                         elevation_threshold: float = 0.5, minimum_distance: float = 0.2,
+                         debug_no_rejection: bool = False, seed: int = 0):
+        """add_as_keyframe on the device (osb_anchor_add_keyframe_dev): nodes [n] of lib.KEYFRAME_NODE_DTYPE in
+        ascending drone id, dists of lib.KEYFRAME_DISTANCE_DTYPE (each node's n_distances in turn, ascending peer).  Writes
+        the new blocks' initial poses into the solver's resident device poses, flags the distances and stores the
+        keyframe, on `stream` without synchronising"""
+        nodes = np.ascontiguousarray(nodes, _l.KEYFRAME_NODE_DTYPE)
+        dists = np.ascontiguousarray(dists, _l.KEYFRAME_DISTANCE_DTYPE)
+        p = _l.KeyframeParams(int(self_id), int(bool(finish_init)), int(bool(enable_distance)),
+                              int(bool(debug_no_rejection)), float(outlier_threshold), float(elevation_threshold),
+                              float(minimum_distance), 0, int(seed) & (2 ** 64 - 1))
+        _l.check(self._lib.osb_anchor_add_keyframe_dev(self._h, solver._h, int(stamp_ns), len(nodes), _l.ptr(nodes),
+                                                       len(dists), _l.ptr(dists) if len(dists) else None, C.byref(p),
+                                                       C.c_void_p(stream)))
+
+    def keyframe_flags(self, stamp_ns: int):
+        """waits for the last add_keyframe_dev -> the stored keyframe's outlier flags (int8: 1, 0, -1 not written) in
+        its dists order, or None when the stamp is not stored"""
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_anchor_keyframe_flags(self._h, int(stamp_ns), None, 0, C.byref(n)))
+        if n.value < 0:
+            return None
+        out = np.zeros(n.value, np.int8)
+        _l.check(self._lib.osb_anchor_keyframe_flags(self._h, int(stamp_ns), _l.ptr(out) if n.value else None, n.value,
+                                                     C.byref(n)))
+        return out
+
+    def distance_factors_dev(self, rows: "FactorRows", max_tail: int, stream: int, self_id: int,
+                             enable_distance: bool = True, debug_no_rejection: bool = False,
+                             distance_measurement_cov: float = 0.2):
+        """setup_problem_with_sferror on the device (osb_anchor_distance_factors_dev): the window's distance rows
+        appended to `rows` at its count, on `stream` without synchronising; a count past max_tail becomes -1"""
+        p = _l.DistanceParams(int(self_id), int(bool(enable_distance)), int(bool(debug_no_rejection)),
+                              float(distance_measurement_cov))
+        ty, ia, ib, pl, hu, cnt = rows.ptrs()
+        _l.check(self._lib.osb_anchor_distance_factors_dev(self._h, C.byref(p), C.c_void_p(ty), C.c_void_p(ia),
+                                                           C.c_void_p(ib), C.c_void_p(pl), C.c_void_p(hu),
+                                                           C.c_void_p(cnt), int(max_tail), C.c_void_p(stream)))
 
     def observability(self) -> dict:
         """waits for the last observe_dev -> its outcome: bool arrays [max_drones] nodes, yaw, pos, enable, to_init and
@@ -1183,6 +1228,10 @@ class AnchoredChain:
         solver.solve_multistart_resident_dev(max_tail, *self.factors.ptrs(), self.mask.data_ptr(), self.yaw.data_ptr(),
                                              self.stream.cuda_stream, n_trials, seed, window_size, acpt_cost, normalise,
                                              options)
+
+    def distances(self, anchor: LoopAnchor, max_tail: int, self_id: int, **kw):
+        """the window's distance rows appended to the chain's rows (LoopAnchor.distance_factors_dev), after compact"""
+        anchor.distance_factors_dev(self.factors, max_tail, self.stream.cuda_stream, self_id, **kw)
 
     def keep_on_host(self, n: int) -> np.ndarray:
         import torch

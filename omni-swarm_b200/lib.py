@@ -83,7 +83,7 @@ class AnchorParams(C.Structure):
     _fields_ = [("max_drones", C.c_int32), ("max_traj_samples", C.c_int32), ("max_measurements", C.c_int32),
                 ("max_window_entries", C.c_int32), ("begin_min_loop_dt_s", C.c_double), ("det_dpos_thres", C.c_double),
                 ("odom_pos_cov_per_m", C.c_double), ("odom_ang_cov_per_m", C.c_double), ("huber", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("max_keyframes", C.c_int32), ("max_keyframe_distances", C.c_int32), ("reserved", C.c_int32)]
 
 
 class ObserveParams(C.Structure):
@@ -92,6 +92,25 @@ class ObserveParams(C.Structure):
 
 
 OBS_DRONES = 256                         # per-drone bytes of osb_observability
+
+
+class KeyframeParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("finish_init", C.c_int32), ("enable_distance", C.c_int32),
+                ("debug_no_rejection", C.c_int32), ("outlier_threshold", C.c_float), ("elevation_threshold", C.c_float),
+                ("minimum_distance", C.c_float), ("reserved", C.c_int32), ("seed", C.c_uint64)]
+
+
+class DistanceParams(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("enable_distance", C.c_int32), ("debug_no_rejection", C.c_int32),
+                ("distance_measurement_cov", C.c_float)]
+
+
+# numpy views of osb_keyframe_node and osb_keyframe_distance (include/omniswarm_b200.h)
+KEYFRAME_NODE_DTYPE = np.dtype([("drone_id", "<i4"), ("block", "<i4"), ("new_block", "<i4"), ("prev_block", "<i4"),
+                                ("vo_available", "<i4"), ("is_static", "<i4"), ("frame_available", "<i4"),
+                                ("dists_available", "<i4"), ("n_distances", "<i4"), ("reserved", "<i4"),
+                                ("pose", "<f8", 7), ("prev_pose", "<f8", 7)])
+KEYFRAME_DISTANCE_DTYPE = np.dtype([("peer", "<i4"), ("reserved", "<i4"), ("distance", "<f8")])
 
 
 class SyncParams(C.Structure):
@@ -361,6 +380,9 @@ _SIG = {
     "osb_anchor_sync_result": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int)]),
     "osb_anchor_paths": (C.c_int, [_P, C.c_int, C.c_int32, _P, _P, C.c_int, C.POINTER(C.c_int32)]),
     "osb_anchor_predict": (C.c_int, [_P, C.POINTER(PredictParams), C.c_int, _P, _P, _P]),
+    "osb_anchor_add_keyframe_dev": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, C.c_int, _P, C.POINTER(KeyframeParams), _P]),
+    "osb_anchor_keyframe_flags": (C.c_int, [_P, C.c_int64, _P, C.c_int, C.POINTER(C.c_int32)]),
+    "osb_anchor_distance_factors_dev": (C.c_int, [_P, C.POINTER(DistanceParams), _P, _P, _P, _P, _P, _P, C.c_int, _P]),
     "osb_swarm_unique_id": (C.c_int, [_P]),
     "osb_swarm_init": (C.c_int, [C.POINTER(_P), _P, C.c_int, C.c_int]),
     "osb_swarm_destroy": (C.c_int, [_P]),
