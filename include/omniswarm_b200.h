@@ -1360,6 +1360,28 @@ osb_status osb_frontend_query_received_dev(osb_frontend* h, const osb_keyframe_r
  *   loop_candidates_dev wrote; the same launches and, for unmarked candidates, the same bytes.  With them a round from
  *   query_received through osb_anchor_add_measurements_dev enqueues with no host read and can be captured into a CUDA
  *   graph. */
+/* osb_frontend_receive_dev(): out_dev[r] = records_dev[r] as this drone's on_image_recv sees it after LoopNet's delivery
+ *   (loop_net.cpp:20-93 sends the directions with landmark_num > 0 and of them only the landmarks with landmarks_flag > 0;
+ *   :142-166, :230-262 rebuild the frame; loop_detector.cpp:36-65 gate it).  Pass out_dev, unchanged and with the metas at
+ *   their indices, to every later call of the round: ingest{,_meta}, init_modes_dev, query_received{,_dev},
+ *   loop_candidates_dev, compute_loop{,_dev}, loop_measurements{,_dev}.
+ *   Records r == skip and records with drone_id == self_id are copied byte for byte.  A foreign record, per direction
+ *   d < n_dirs: the landmarks i < n_kpts[d] with landmarks_flag[d][i] > 0, c_d of them in increasing i, move (kpts,
+ *   local_desc, landmarks_3d, landmarks_flag, stereo_match) to slots 0 .. c_d-1; slots from c_d on are zero, stereo_match -1;
+ *   n_kpts[d] = c_d, n_kpts_down[d] = 0 (no down image travels); global_desc[d] is kept when c_d > 0 and zero otherwise (a
+ *   null image: ingest adds no row for it, and the query gate closes on it).  Directions d >= n_dirs come out as null images.
+ *   The foreign record is dropped (on_image_recv's order) when (a) the local + remote store rows at this point of `stream`
+ *   are 0, (b) fewer than min_direction_loop directions have c_d > 0, or (c) sum c_d < min_loop_num (set_loop_params).  A
+ *   dropped record keeps drone_id, msg_id and n_dirs, so its meta still pairs with it; every other field is zero, so ingest
+ *   adds no row for it and query_received gives it the gate-closed result.
+ *   Gate (a) is exact for a whole round: a dropped frame adds no row, so no frame of the round changes database_size() for
+ *   another.  The caller orders its own keyframe's ingest before or after the call as its callbacks order them in the
+ *   reference (the own keyframe is on_image_recv'd before or after the received ones).
+ *   0 <= n_records <= 64 (0 does nothing); both buffers 16-byte aligned; OSB_ERR_INVALID with nothing enqueued for a null
+ *   pointer, out_dev overlapping records_dev, or a handle without set_loop_params.  One launch, no allocation, no host
+ *   synchronisation: the call can be captured into a CUDA graph. */
+osb_status osb_frontend_receive_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records, int skip,
+                                    osb_keyframe_record* out_dev, void* stream);
 osb_status osb_frontend_loop_candidates_dev(osb_frontend* h, const osb_keyframe_record* records_dev,
                                             const osb_keyframe_meta* metas_dev, const osb_loop_result* results_dev, int n,
                                             const uint8_t* init_mode_dev, osb_loop_candidate* cand_out_dev,

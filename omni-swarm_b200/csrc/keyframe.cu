@@ -793,6 +793,104 @@ __global__ void fe_init_modes_kernel(const osb_keyframe_record* __restrict__ rec
   out[i] = (i != skip && fe_init_mode(recs[i].drone_id, cr.self_id, pairs, cr.init_frames)) ? 1 : 0;
 }
 
+// osb_frontend_receive_dev: a received record as LoopNet delivers it and on_image_recv keeps it (loop_net.cpp:20-93,
+// :142-166, :230-262; loop_detector.cpp:36-65).  One CTA of FE_RECV_THREADS per (record, direction).  Every CTA counts the
+// flagged landmarks of all directions of its record, so it evaluates the frame gates itself; its own direction's flagged
+// landmarks get their slots from a ballot prefix (stable, no atomics).  Records r == skip and own records are copied as they are.
+constexpr int FE_RECV_THREADS = 256;
+static_assert(FE_RECV_THREADS >= OSB_MAX_KPTS && FE_RECV_THREADS == 256, "one thread per landmark; fe_block_compact's 8 warps");
+static_assert(sizeof(osb_keyframe_record) % 16 == 0 && offsetof(osb_keyframe_record, global_desc) % 16 == 0 &&
+                  offsetof(osb_keyframe_record, local_desc) % 16 == 0 && offsetof(osb_keyframe_record, kpts) % 16 == 0 &&
+                  offsetof(osb_keyframe_record, stereo_match) % 16 == 0 &&
+                  offsetof(osb_keyframe_record, landmarks_3d) % 16 == 0 &&
+                  offsetof(osb_keyframe_record, landmarks_flag) % 16 == 0,
+              "the record's planes move as float4");
+
+// n float4 from s to d (both 16-byte aligned)
+__device__ __forceinline__ void fe_copy16(void* __restrict__ d, const void* __restrict__ s, int n) {
+  const float4* a = static_cast<const float4*>(s);
+  float4* b = static_cast<float4*>(d);
+#pragma unroll 4
+  for (int i = threadIdx.x; i < n; i += FE_RECV_THREADS) b[i] = a[i];
+}
+
+__device__ __forceinline__ void fe_zero16(void* __restrict__ d, int n) {
+  float4* b = static_cast<float4*>(d);
+  const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = threadIdx.x; i < n; i += FE_RECV_THREADS) b[i] = z;
+}
+
+template <class T>
+constexpr int fe_f4(const T&) { return (int)(sizeof(T) / 16); }
+
+__global__ void __launch_bounds__(FE_RECV_THREADS)
+fe_receive_kernel(const osb_keyframe_record* __restrict__ in, osb_keyframe_record* __restrict__ out, int skip, int self_id,
+                  int min_direction_loop, int min_loop_num, const DbDev* __restrict__ local_cnt,
+                  const DbDev* __restrict__ remote_cnt) {
+  const int r = blockIdx.x / OSB_MAX_DIRS, d = blockIdx.x % OSB_MAX_DIRS;
+  const int tid = threadIdx.x;
+  const osb_keyframe_record* src = in + r;
+  osb_keyframe_record* dst = out + r;
+  const int drone = src->drone_id;
+  if (r == skip || drone == self_id) {                       // not received: byte for byte
+    if (d == 0 && tid < 3) reinterpret_cast<float4*>(dst)[tid] = reinterpret_cast<const float4*>(src)[tid];
+    fe_copy16(dst->global_desc[d], src->global_desc[d], fe_f4(src->global_desc[d]));
+    fe_copy16(dst->local_desc[d], src->local_desc[d], fe_f4(src->local_desc[d]));
+    fe_copy16(dst->kpts[d], src->kpts[d], fe_f4(src->kpts[d]));
+    fe_copy16(dst->stereo_match[d], src->stereo_match[d], fe_f4(src->stereo_match[d]));
+    fe_copy16(dst->landmarks_3d[d], src->landmarks_3d[d], fe_f4(src->landmarks_3d[d]));
+    fe_copy16(dst->landmarks_flag[d], src->landmarks_flag[d], fe_f4(src->landmarks_flag[d]));
+    return;
+  }
+  // flagged landmarks of every direction: header feature_num = landmark_num after scan_recv_packets (loop_net.cpp:43-48)
+  __shared__ int cnt[OSB_MAX_DIRS];
+  __shared__ int16_t from[OSB_MAX_KPTS];                     // slot -> landmark index of this CTA's direction
+  const int nd = min(max(src->n_dirs, 0), OSB_MAX_DIRS);
+  for (int dd = 0; dd < OSB_MAX_DIRS; ++dd) {
+    const int n = dd < nd ? min(max(src->n_kpts[dd], 0), OSB_MAX_KPTS) : 0;
+    const bool keep = tid < n && src->landmarks_flag[dd][tid] > 0;
+    int total;
+    const int pos = fe_block_compact(keep, &total);
+    if (dd == d && keep) from[pos] = (int16_t)tid;
+    if (tid == 0) cnt[dd] = total;
+    __syncthreads();                                         // fe_block_compact's warp counts are reused next pass
+  }
+  int dirs = 0, sum = 0;
+  for (int dd = 0; dd < OSB_MAX_DIRS; ++dd) { dirs += cnt[dd] > 0 ? 1 : 0; sum += cnt[dd]; }
+  // on_image_recv's gates (loop_detector.cpp:36-38, :53-63, :65): database_size() is local + remote rows at this point
+  const bool dropped = local_cnt->ntotal + remote_cnt->ntotal == 0 || dirs < min_direction_loop || sum < min_loop_num;
+  const int c = dropped ? 0 : cnt[d];
+  if (d == 0 && tid == 0) {
+    dst->drone_id = drone; dst->msg_id = src->msg_id; dst->n_dirs = src->n_dirs;
+    dst->reserved = dropped ? 0 : src->reserved;
+  }
+  if (tid == 0) { dst->n_kpts[d] = c; dst->n_kpts_down[d] = 0; }   // no down image travels
+  if (c > 0) fe_copy16(dst->global_desc[d], src->global_desc[d], fe_f4(src->global_desc[d]));
+  else fe_zero16(dst->global_desc[d], fe_f4(dst->global_desc[d]));   // a null image (generate_null_img_desc)
+  // local descriptors: 16 float4 per landmark, slot s from landmark from[s]
+  {
+    constexpr int R4 = OSB_FEATURE_DESC_SIZE / 4;
+    const float4* a = reinterpret_cast<const float4*>(src->local_desc[d]);
+    float4* b = reinterpret_cast<float4*>(dst->local_desc[d]);
+#pragma unroll 4
+    for (int i = tid; i < OSB_MAX_KPTS * R4; i += FE_RECV_THREADS) {
+      const int s = i / R4, k = i % R4;
+      b[i] = s < c ? a[from[s] * R4 + k] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+  if (tid < OSB_MAX_KPTS) {
+    const int s = tid;
+    const bool ok = s < c;
+    const int j = ok ? from[s] : 0;
+    dst->kpts[d][s][0] = ok ? src->kpts[d][j][0] : 0.f;
+    dst->kpts[d][s][1] = ok ? src->kpts[d][j][1] : 0.f;
+    dst->stereo_match[d][s] = ok ? src->stereo_match[d][j] : (dropped ? 0 : -1);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) dst->landmarks_3d[d][s][k] = ok ? src->landmarks_3d[d][j][k] : 0.f;
+    dst->landmarks_flag[d][s] = ok ? src->landmarks_flag[d][j] : 0;
+  }
+}
+
 // candidate i on thread i: the query side from metas[i], the hit side from the meta table of the hit's store, init_mode,
 // and for same-drone hits the ego-motion trajectory's relative pose and covariance (check_loop_odometry_consistency,
 // loop_detector.cpp:294-303) in the order of tests/loop_candidates_ref.py
@@ -1936,6 +2034,24 @@ extern "C" osb_status osb_frontend_init_modes_dev(osb_frontend* h, const osb_key
   OSB_TRY(fe_lm_alloc(h, st));
   OSB_LAUNCH(fe_init_modes_kernel, 1, FE_MAX_RECORDS, 0, st, records_dev, n_records, skip, fe_cand_rule(h), h->d_lm_pairs,
              init_mode_out_dev);
+  OSB_CHECK_LAUNCH();
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_frontend_receive_dev(osb_frontend* h, const osb_keyframe_record* records_dev, int n_records,
+                                               int skip, osb_keyframe_record* out_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null handle");
+  OSB_REQUIRE(n_records >= 0 && n_records <= FE_MAX_RECORDS, "n_records must be 0..64");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->have_loop_params, "no loop parameters: call osb_frontend_set_loop_params first");
+  if (n_records == 0) return OSB_OK;
+  OSB_REQUIRE(records_dev && out_dev, "null argument");
+  const uintptr_t a = (uintptr_t)records_dev, b = (uintptr_t)out_dev, len = (uintptr_t)n_records * sizeof(osb_keyframe_record);
+  OSB_REQUIRE(a + len <= b || b + len <= a, "out_dev overlaps records_dev");
+  OSB_REQUIRE(a % 16 == 0 && b % 16 == 0, "records_dev and out_dev must be 16-byte aligned");
+  DeviceGuard dg(h->device);
+  OSB_LAUNCH(fe_receive_kernel, n_records * OSB_MAX_DIRS, FE_RECV_THREADS, 0, (cudaStream_t)stream, records_dev, out_dev, skip,
+             h->cfg.self_id, h->loop_params.min_direction_loop, h->loop_params.min_loop_num, h->db[0].v.dev, h->db[1].v.dev);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
 }

@@ -606,6 +606,13 @@ class KeyframeFrontend(_Handle):
         _l.check(self._lib.osb_frontend_init_modes_dev(self._h, C.c_void_p(records_dev), n_records, skip, C.c_void_p(out_dev),
                                                        C.c_void_p(stream)))
 
+    def receive_dev(self, records_dev: int, n_records: int, skip: int, out_dev: int, stream: int):
+        """the received records as LoopNet delivers them and on_image_recv keeps them (osb_frontend_receive_dev): foreign
+        records [n_records] -> their flagged landmarks only, gated frames zeroed, at out_dev; pass out_dev to the rest of
+        the round"""
+        _l.check(self._lib.osb_frontend_receive_dev(self._h, C.c_void_p(records_dev), n_records, skip, C.c_void_p(out_dev),
+                                                    C.c_void_p(stream)))
+
     def query_received_dev(self, records_dev: int, n_records: int, skip: int, init_mode_dev, results_dev: int, stream: int):
         """query_received with init_mode a device byte array [n_records] (or None: all 0)"""
         _l.check(self._lib.osb_frontend_query_received_dev(self._h, C.c_void_p(records_dev), n_records, skip,

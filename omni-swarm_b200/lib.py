@@ -326,6 +326,7 @@ _SIG = {
     "osb_frontend_set_candidate_params": (C.c_int, [_P, C.POINTER(CandidateParams)]),
     "osb_frontend_init_modes_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "osb_frontend_query_received_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "osb_frontend_receive_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "osb_frontend_loop_candidates_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
     "osb_frontend_compute_loop_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
     "osb_frontend_loop_measurements_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_double, C.c_double, _P, _P, _P]),
