@@ -35,15 +35,21 @@ def triangulate_point(pose0, pose1, p0, p1):
     return p, float(err)
 
 
-def stereo_lift(kp_up, kp_down, stereo_match, K, pose_up, pose_down, triangle_thres):
-    """-> (pts3d [n_up,3] f32, flag_up [n_up] u8, flag_down [n_down] u8); K = (fx, fy, cx, cy)"""
+def stereo_lift(kp_up, kp_down, stereo_match, K, pose_up, pose_down, triangle_thres, accept_min_3d_pts=0):
+    """-> (pts3d [n_up,3] f32, flag_up [n_up] u8, flag_down [n_down] u8); K = (fx, fy, cx, cy).
+
+    An image with n_up <= accept_min_3d_pts keypoints is not lifted at all (:385-391).  A match index outside
+    [0, n_down) means "no stereo partner": the reference's indices come from its own matcher and never leave the range, the
+    device kernel skips them, and so does this statement."""
     fx, fy, cx, cy = K
     n_up, n_down = len(kp_up), len(kp_down)
     pts = np.zeros((n_up, 3), np.float32); fu = np.zeros(n_up, np.uint8); fd = np.zeros(n_down, np.uint8)
+    if n_up <= accept_min_3d_pts:
+        return pts, fu, fd
     Ru = rot(pose_up[3:])
     for i in range(n_up):
         j = int(stereo_match[i])
-        if j < 0:
+        if j < 0 or j >= n_down:
             continue
         a = np.array([(kp_up[i][0] - cx) / fx, (kp_up[i][1] - cy) / fy], np.float64)
         b = np.array([(kp_down[j][0] - cx) / fx, (kp_down[j][1] - cy) / fy], np.float64)
@@ -55,12 +61,14 @@ def stereo_lift(kp_up, kp_down, stereo_match, K, pose_up, pose_down, triangle_th
     return pts, fu, fd
 
 
-def depth_lift(kp, depth_mm, K, pose_cam, near, far):
-    """-> (pts3d [n,3] f32, flag [n] u8)"""
+def depth_lift(kp, depth_mm, K, pose_cam, near, far, accept_min_3d_pts=0):
+    """-> (pts3d [n,3] f32, flag [n] u8); nothing is lifted when n <= accept_min_3d_pts (:267)"""
     fx, fy, cx, cy = K
     H, W = depth_mm.shape
     n = len(kp)
     pts = np.zeros((n, 3), np.float32); fl = np.zeros(n, np.uint8)
+    if n <= accept_min_3d_pts:
+        return pts, fl
     for i in range(n):
         x, y = float(kp[i][0]), float(kp[i][1])
         if x < 0 or x > W or y < 0 or y > H:                          # :282 (the reference hard-codes 640 x 480)
