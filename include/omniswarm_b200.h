@@ -748,6 +748,72 @@ osb_status osb_anchor_sync_result(osb_anchor* h, int32_t* applied, osb_status* l
  *   *n = its sample count, -1 when the drone has none (also before the first applied sync); min(*n, cap) samples of
  *   stamps [ns] and poses7 [x y z qw qx qy qz] are written. */
 osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, int64_t* stamps, double* poses7, int cap, int32_t* n);
+/* osb_anchor_record_loops_dev(): the loop map of SwarmLocalOutlierRejection::OutlierRejectionLoopEdges
+ *   (swarm_outlier_rejection.cpp:106-120), which every solve makes whether or not PCM processes a pair, from the n rows
+ *   osb_anchor_run_dev wrote (n = its n_out, VOID tail included), on `stream` without synchronising.  Goes after run_dev,
+ *   once per solve.  Every row with status == OSB_ANCHOR_OK (loops and detections) whose id is not yet recorded:
+ *     all_loop_map[id] = (id, edge.id_a, edge.id_b, stamp_a, stamp_b, edge.rel_pose) -- the re-anchored edge as first
+ *       seen (stamp_a / stamp_b are the anchor node frames' stamps, loc_ret.ts_a / ts_b); when one call holds an id more
+ *       than once, the first row in row order wins.  A recorded id keeps its values for good;
+ *     all_loops_set_by_pair[a][b] and [b][a] gain the id.  Only the smallest id of a pair is kept (the `.begin()` that
+ *       init_pose_by_loops reads); ids are only added, so it only moves down.
+ *   Nothing depends on the order of atomics: a 32-bit atomicMin on the row index picks each id's first row, a second
+ *   launch writes the winners, and a pair's minimum is a 64-bit atomicMin.  An id of INT64_MAX is recorded but never a
+ *   pair's minimum.  Two launches whatever n.  The first call acquires 96 (H + 1) + 8 D^2 bytes (H = the power of two
+ *   >= 2 max_measurements, D = max_drones) and an event, and synchronises; a handle that never makes it holds none of
+ *   this.  Later calls acquire nothing and can be captured.  Each call is ordered after the handle's last record_loops
+ *   and init_by_loops on any stream.  The map holds at most H distinct ids (the rows of one handle have at most
+ *   max_measurements); past that the map is full and osb_anchor_init_by_loops_result reports OSB_ERR_CAPACITY.
+ *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null handle or rows pointer with n > 0, n < 0.
+ * osb_anchor_init_by_loops_dev(): SwarmLocalizationSolver::init_pose_by_loops (swarm_localization_solver.cpp:218-269),
+ *   the start of the single init trial before the swarm is initialised by motion, on the device, on `stream` without
+ *   synchronising.  It reads the last observe's to_init, the PCM state's inlier sets (good_loops_set), the loop map, the
+ *   keyframe paths and estimated drones of the last applied sync, the trajectories and the window, and writes the
+ *   solver's resident pose copy.  For each drone _id with to_init, ascending:
+ *     the candidate pairs are _id's inlier sets when the PCM state holds any set of a pair of _id (a PCM result or a
+ *       set_inliers set, empty ones included), else _id's pairs of the loop map -- the whole map is replaced;
+ *     pairs go by ascending id2 = the other drone; a pair is skipped when its set is empty or id2 is not estimated; each
+ *       later pair overwrites the earlier one, so the largest qualifying id2 decides;
+ *     the loop is all_loop_map[smallest id of the set]; when its id_a != id2 it is inverted (drones and stamps swapped,
+ *       relative pose inverted);
+ *     pose0, t0: id2's keyframe path sample nearest to the loop's stamp_a if id2 has a path; else, for id2 == self_id,
+ *       its odometry sample nearest to stamp_a; else identity and t0 = stamp_a;
+ *     every window entry of _id, vo_available or not: block pose = to_xyzyaw(pose0 * odoma * rel * odomb), odoma = id2's
+ *       relative odometry from t0 to stamp_a, odomb = id2's relative odometry from stamp_b to the entry's FRAME stamp
+ *       (both on id2's trajectory, as the reference computes them); relative pose = pose(t1)^-1 pose(t2) of the nearest
+ *       samples, 6-DoF.  A block shared by frames takes its latest frame's value.
+ *   Estimated drones: every drone that had a window entry at an applied osb_anchor_sync_dev, and self_id while the window
+ *   holds an entry of it (it has a keyframe).  self_id is placed like any other drone when to_init holds it.  Blocks
+ *   belong to one drone (as add_as_keyframe gives them out).  Keyframes outside the window are not written: the solver
+ *   holds only the window.
+ *   Refused on the device with every pose unchanged, reported by osb_anchor_init_by_loops_result: a qualifying pair whose
+ *   smallest id is not in the loop map, or a qualifying id2 without odometry while the window has entries or its start
+ *   needs it (the reference throws from all_loop_map.at() / ego_motion_trajs.at()) -- OSB_ERR_INVALID; a full loop map --
+ *   OSB_ERR_CAPACITY.
+ *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, self_id outside 0..max_drones-1, the handles
+ *   on different devices, no observe_dev since create, a PCM state without a device copy (no reject_anchored call yet), a
+ *   window block < 0 or >= the solver's node count.
+ *   One launch (one CTA: thread d decides drone d, then the threads stride over the window entries).  The first call
+ *   acquires the loop map (as record_loops_dev) and the sync's paths (as sync_dev) if they are not there yet, and
+ *   synchronises; later calls acquire nothing and can be captured, reading to_init, the PCM directory, the map, the paths
+ *   and the trajectories on the device.  Ordered after the handle's last observe, sync and record_loops and the solver's
+ *   last device call on any stream; the next of those, set_window and push_odometry are ordered after it.
+ * osb_anchor_init_by_loops_result(): waits for the last init_by_loops -> *last (OSB_OK when none ran); returns OSB_OK.
+ * osb_anchor_loop_map(): waits for the last record_loops and sync -> *n = the number of recorded ids, min(*n, cap)
+ *   records ascending by id; pair_min [max_drones][max_drones] (or null): each ordered pair's smallest id, INT64_MAX for
+ *   none; estimated [max_drones] (or null): 1 for every drone that had a window entry at an applied sync.  All empty
+ *   before the first call that acquires them. */
+typedef struct {
+  int64_t id;
+  int32_t id_a, id_b;
+  int64_t stamp_a, stamp_b;
+  double rel_pose[7];
+} osb_loop_record;
+osb_status osb_anchor_record_loops_dev(osb_anchor* h, const osb_anchor_result* rows_dev, int n, void* stream);
+osb_status osb_anchor_init_by_loops_dev(osb_anchor* h, osb_pcm_state* pcm, osb_solver* s, int32_t self_id, void* stream);
+osb_status osb_anchor_init_by_loops_result(osb_anchor* h, osb_status* last);
+osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, int cap, int32_t* n, int64_t* pair_min,
+                               uint8_t* estimated);
 /* osb_anchor_predict(): PredictSwarm / PredictNode / NodeCooridnateOffset (swarm_localization_solver.cpp:673-765) for one
  *   frame of n drones (distinct ids, vo_poses7 [n][7] their odometry now), from the prediction record of the last applied
  *   sync.  With the drone's record (saved block pose P4, its frame's self_pose vo):

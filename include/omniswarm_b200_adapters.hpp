@@ -434,6 +434,23 @@ class ResidentPoseGraph {
     cost_now = equv[chosen];
     return true;
   }
+  // The same before the swarm is initialised by motion (:786-806): one trial that starts from init_pose_by_loops
+  // (:218-269) instead of random poses.  osb_anchor_init_by_loops_dev places the blocks of the last observe's to_init
+  // drones on the device, from the loop map that osb_anchor_record_loops_dev keeps after each run_dev, the PCM state's
+  // inlier sets (pcm: its good_loops_set) and the last applied sync's keyframe paths; then one trial with no block
+  // scattered (zero_mask_dev: n_nodes zero bytes on the device).  Nothing between run_dev and this solve reads the host.
+  // Sends what was added first, so the window's blocks exist in the solver; returns whether the trial was accepted.
+  bool solve_with_loops_init_dev(osb_anchor* anchor, osb_pcm_state* pcm, int32_t self_id, int max_tail,
+                                 const int32_t* type_dev, const int32_t* ia_dev, const int32_t* ib_dev,
+                                 const double* payload_dev, const uint8_t* huber_dev, const int32_t* count_dev,
+                                 const uint8_t* zero_mask_dev, osb_multistart_options ms, void* stream,
+                                 const osb_solve_options* opt = nullptr) {
+    flush();
+    check(osb_anchor_init_by_loops_dev(anchor, pcm, solver_, self_id, stream), "osb_anchor_init_by_loops_dev");
+    ms.n_trials = 1;                                 // solve_with_multiple_init's max_number = 1 (:790-792)
+    return solve_with_multiple_init_dev(max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev, count_dev,
+                                        zero_mask_dev, nullptr, ms, stream, opt);
+  }
   double cost_now = 0.0;             // equv_cost of the trial solve_with_multiple_init_dev accepted last (:809)
 
  private:

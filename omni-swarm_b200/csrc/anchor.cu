@@ -510,7 +510,8 @@ struct SyncWindow {
 };
 struct SyncRecord {                   // est_poses_tsid_saved[ts][d] of the last pushed frame ts holding d
   int64_t stamp;
-  int32_t valid, reserved;
+  int32_t valid;
+  int32_t estimated;                  // d had a window entry at an applied sync (estimated_nodes, :996-997); sticky
   double saved[4];                    // the solved block pose, x y z yaw
   double vo[7];                       // the entry's self_pose (all_sf[ts].id2nodeframe[d].pose())
 };
@@ -592,6 +593,7 @@ __global__ void __launch_bounds__(SYNC_THREADS) sync_gate_kernel(const SyncView 
   if (d == v.max_drones - 1) v.kf_first[d + 1] = hi;
   v.full_n[d] = (v.full_path && hi > lo) ? (v.traj_n[d] + FULL_PATH_STEP - 1) / FULL_PATH_STEP : -1;
   SyncRecord& r = v.rec[d];
+  if (hi > lo) r.estimated = 1;
   int k = -1;
   if (hi > lo && (v.trials > 0 || v.win->push_stamp == v.w_stamp[hi - 1])) {
     k = hi - 1;                                                    // a pushed frame holds d: the last of them
@@ -889,6 +891,212 @@ __global__ void __launch_bounds__(DF_THREADS) distance_factors_kernel(const Dist
   if (t == 0) *v.count = out > v.max_tail ? -1 : out;
 }
 
+// The loop map of OutlierRejectionLoopEdges (swarm_outlier_rejection.cpp:106-120): all_loop_map as open addressing over
+// H + 1 records (a power of two H, linear probing, empty key -1; the id -1 itself lives in record H) and
+// all_loops_set_by_pair as each ordered pair's smallest id.  Two launches per call: record_claim_kernel inserts the key of
+// every OK row whose id is not recorded yet, takes the smallest row index of each such id by atomicMin and lowers its
+// pairs' minima; record_write_kernel lets each id's first row write the record.  Only record_write_kernel sets
+// `recorded`, and only the winner reads its own, so no outcome depends on the order of atomics.
+constexpr int LM_THREADS = 256;
+constexpr int64_t LM_EMPTY = -1;
+constexpr unsigned long long LM_NONE = ~0ull;                     // a pair without an id (the id INT64_MAX maps to it)
+struct LoopRec {
+  osb_loop_record r;                  // r.id is the key
+  uint32_t claim;                     // the smallest row of this call that holds the id, UINT32_MAX: none
+  uint32_t recorded;                  // 1: the values are written
+};
+// order-preserving map of an int64 id onto the unsigned pair minima
+__device__ __forceinline__ unsigned long long lm_order(int64_t id) { return (unsigned long long)id ^ (1ull << 63); }
+
+__device__ __forceinline__ int lm_find(const LoopRec* t, int H, int64_t id) {
+  if (id == LM_EMPTY) return H;
+  unsigned long long h = splitmix64((uint64_t)id) & (unsigned long long)(H - 1);
+  for (int p = 0; p < H; ++p, h = (h + 1) & (unsigned long long)(H - 1)) {
+    const int64_t k = *(volatile const int64_t*)&t[h].r.id;
+    if (k == id) return (int)h;
+    if (k == LM_EMPTY) return -1;
+  }
+  return -1;
+}
+__device__ __forceinline__ int lm_insert(LoopRec* t, int H, int64_t id) {   // -> the id's record, -1: the table is full
+  if (id == LM_EMPTY) return H;
+  unsigned long long h = splitmix64((uint64_t)id) & (unsigned long long)(H - 1);
+  for (int p = 0; p < H; ++p, h = (h + 1) & (unsigned long long)(H - 1)) {
+    unsigned long long* k = reinterpret_cast<unsigned long long*>(&t[h].r.id);
+    unsigned long long cur = *(volatile unsigned long long*)k;
+    if (cur == (unsigned long long)LM_EMPTY) cur = atomicCAS(k, (unsigned long long)LM_EMPTY, (unsigned long long)id);
+    if (cur == (unsigned long long)LM_EMPTY || cur == (unsigned long long)id) return (int)h;
+  }
+  return -1;
+}
+
+struct LoopMapView {
+  LoopRec* tab;                       // [H + 1]
+  unsigned long long* pair;           // [D][D] lm_order(smallest id), LM_NONE
+  int32_t* meta;                      // [0] the map overflowed (sticky), [1] the last init_by_loops' status
+  int H, max_drones;
+};
+
+__global__ void __launch_bounds__(LM_THREADS)
+record_claim_kernel(const osb_anchor_result* __restrict__ rows, int n, const LoopMapView v) {
+  for (int i = blockIdx.x * LM_THREADS + threadIdx.x; i < n; i += gridDim.x * LM_THREADS) {
+    if (rows[i].status != OSB_ANCHOR_OK) continue;
+    const int64_t id = rows[i].id;
+    const int s = lm_insert(v.tab, v.H, id);
+    if (s < 0) { v.meta[0] = 1; continue; }
+    if (v.tab[s].recorded == 1u) continue;                         // only record_write_kernel writes it
+    atomicMin(&v.tab[s].claim, (uint32_t)i);
+    const int a = rows[i].edge.id_a, b = rows[i].edge.id_b;
+    if ((unsigned)a >= (unsigned)v.max_drones || (unsigned)b >= (unsigned)v.max_drones) continue;
+    atomicMin(v.pair + (size_t)a * v.max_drones + b, lm_order(id));
+    atomicMin(v.pair + (size_t)b * v.max_drones + a, lm_order(id));
+  }
+}
+
+__global__ void __launch_bounds__(LM_THREADS)
+record_write_kernel(const osb_anchor_result* __restrict__ rows, int n, const LoopMapView v) {
+  for (int i = blockIdx.x * LM_THREADS + threadIdx.x; i < n; i += gridDim.x * LM_THREADS) {
+    if (rows[i].status != OSB_ANCHOR_OK) continue;
+    const int s = lm_find(v.tab, v.H, rows[i].id);
+    if (s < 0 || v.tab[s].recorded == 1u || v.tab[s].claim != (uint32_t)i) continue;
+    osb_loop_record& r = v.tab[s].r;
+    r.id_a = rows[i].edge.id_a;
+    r.id_b = rows[i].edge.id_b;
+    r.stamp_a = rows[i].stamp_a;
+    r.stamp_b = rows[i].stamp_b;
+    for (int j = 0; j < 7; ++j) r.rel_pose[j] = rows[i].edge.rel_pose[j];
+    v.tab[s].recorded = 1u;
+  }
+}
+
+// init_pose_by_loops (swarm_localization_solver.cpp:218-269): one CTA, thread d decides drone d -- its id2, its loop and
+// the prefix pose0 * odoma * rel -- then every thread strides over the window entries (ordered by drone, frame) and writes
+// prefix * odomb into the entry's block.  A refusal anywhere leaves every pose as it was.
+constexpr int IBL_THREADS = 256;                                   // = ANCHOR_MAX_DRONES
+
+struct InitLoopsView {
+  const osb_observability* obs;
+  const PcmDir* dir;
+  const int32_t* n_dir;
+  LoopMapView lm;
+  const SyncWindow* win;              // every window entry by (drone, frame): frame stamp and block
+  const int64_t* w_stamp;
+  const int32_t* w_block;
+  const int32_t* kf_first;            // the keyframe paths of the last applied sync
+  const int64_t* kf_stamp;
+  const double* kf_pose;
+  const SyncRecord* rec;              // rec[d].estimated
+  const int64_t* traj_stamp;
+  const double* traj_pose;
+  const int32_t* traj_n;
+  int max_samples, max_drones, self_id;
+  double* poses;                      // the solver's resident poses, [block][4]
+};
+
+__device__ __forceinline__ PoseD ibl_ego(const InitLoopsView& v, int d, int64_t t, int64_t* t_out) {
+  const size_t base = (size_t)d * v.max_samples;
+  const int k = nearest_sample(v.traj_stamp + base, v.traj_n[d], t);
+  if (t_out) *t_out = v.traj_stamp[base + k];
+  return load_pose(v.traj_pose + (base + k) * 7);
+}
+// get_relative_pose_by_appro_ts(t1, t2) = pose(t1)^-1 pose(t2), nearest samples
+__device__ __forceinline__ PoseD ibl_rel(const InitLoopsView& v, int d, int64_t t1, int64_t t2) {
+  return pose_mul(pose_inv(ibl_ego(v, d, t1, nullptr)), ibl_ego(v, d, t2, nullptr));
+}
+
+__global__ void __launch_bounds__(IBL_THREADS) init_by_loops_kernel(const InitLoopsView v) {
+  __shared__ double s_pre[ANCHOR_MAX_DRONES][7];
+  __shared__ int64_t s_tb[ANCHOR_MAX_DRONES];
+  __shared__ int s_id2[ANCHOR_MAX_DRONES];
+  const int d = threadIdx.x;
+  const int D = v.max_drones;
+  const SyncWindow& w = *v.win;
+  const int n_ent = w.first[D];
+  const bool self_kf = w.first[v.self_id + 1] > w.first[v.self_id];
+  int id2 = -1, status = v.lm.meta[0] ? OSB_ERR_CAPACITY : OSB_OK;
+  int64_t lid = 0;
+  if (d < D && v.obs->to_init[d] && status == OSB_OK) {
+    const int nd = *v.n_dir;
+    bool good = false;                                             // good_loops_set.find(_id) (:221-224)
+    for (int e = 0; e < nd && !good; ++e) {
+      const int64_t key = v.dir[e].key;
+      good = v.dir[e].gn >= 0 && ((int)(key >> 32) == d || (int)(uint32_t)key == d);
+    }
+    const int n_cand = good ? nd : D;
+    for (int c = 0; c < n_cand; ++c) {                             // each qualifying pair in turn (:225-232)
+      int j;
+      int64_t id;
+      if (good) {
+        const PcmDir& e = v.dir[c];
+        const int lo = (int)(e.key >> 32), hi = (int)(uint32_t)e.key;
+        if (e.gn <= 0 || (lo != d && hi != d)) continue;
+        j = lo == d ? hi : lo;
+        id = e.gptr[0];
+      } else {
+        j = c;
+        const unsigned long long m = v.lm.pair[(size_t)d * D + c];
+        if (m == LM_NONE) continue;
+        id = (int64_t)(m ^ (1ull << 63));
+      }
+      if ((unsigned)j >= (unsigned)D || !(v.rec[j].estimated || (j == v.self_id && self_kf))) continue;
+      const int s = lm_find(v.lm.tab, v.lm.H, id);                  // all_loop_map.at() and ego_motion_trajs.at()
+      const bool has_path = v.kf_first[j + 1] > v.kf_first[j];
+      if (s < 0 || v.lm.tab[s].recorded != 1u ||
+          (v.traj_n[j] == 0 && (n_ent > 0 || (j == v.self_id && !has_path)))) {
+        status = OSB_ERR_INVALID;
+        break;
+      }
+      if (j > id2) { id2 = j; lid = id; }                           // the last pair in ascending id2 order wins
+    }
+  }
+  const int bad = __syncthreads_or(status != OSB_OK);
+  if (bad) {
+    const int first_bad = __syncthreads_or(status == OSB_ERR_CAPACITY);
+    if (d == 0) v.lm.meta[1] = first_bad ? OSB_ERR_CAPACITY : OSB_ERR_INVALID;
+    return;
+  }
+  if (d < ANCHOR_MAX_DRONES) s_id2[d] = -1;
+  if (id2 >= 0 && v.traj_n[id2] > 0) {                             // init_pose_by_loop (:236-268)
+    const osb_loop_record& r = v.lm.tab[lm_find(v.lm.tab, v.lm.H, lid)].r;
+    int64_t ta = r.stamp_a, tb = r.stamp_b;
+    PoseD rel = load_pose(r.rel_pose);
+    if (r.id_a != id2) {                                           // invert_loop
+      ta = r.stamp_b;
+      tb = r.stamp_a;
+      rel = pose_inv(rel);
+    }
+    int64_t t0 = ta;
+    PoseD pose0;
+    pose0.t[0] = pose0.t[1] = pose0.t[2] = 0.0;
+    pose0.q[0] = 1.0; pose0.q[1] = pose0.q[2] = pose0.q[3] = 0.0;
+    const int lo = v.kf_first[id2], hi = v.kf_first[id2 + 1];
+    if (hi > lo) {
+      const int k = lo + nearest_sample(v.kf_stamp + lo, hi - lo, t0);
+      t0 = v.kf_stamp[k];
+      pose0 = load_pose(v.kf_pose + (size_t)k * 7);
+    } else if (id2 == v.self_id) {
+      pose0 = ibl_ego(v, id2, ta, &t0);
+    }
+    const PoseD pre = pose_mul(pose_mul(pose0, ibl_rel(v, id2, t0, ta)), rel);
+    store_pose(s_pre[d], pre);
+    s_tb[d] = tb;
+    s_id2[d] = id2;
+  }
+  __syncthreads();
+  for (int k = d; k < n_ent; k += IBL_THREADS) {
+    const int dr = kf_owner(w.first, D, k);                        // the entry's drone: the last d with first[d] <= k
+    const int j2 = s_id2[dr];
+    if (j2 < 0) continue;
+    const int blk = v.w_block[k];
+    bool later = false;                                            // a later frame of the drone shares the block
+    for (int k2 = k + 1; k2 < w.first[dr + 1] && !later; ++k2) later = v.w_block[k2] == blk;
+    if (later) continue;
+    const PoseD p = pose_mul(load_pose(s_pre[dr]), ibl_rel(v, j2, s_tb[dr], v.w_stamp[k]));
+    store_pose4(v.poses + 4 * (size_t)blk, p.t, quat_yaw(p.q));
+  }
+  if (d == 0) v.lm.meta[1] = OSB_OK;
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -898,6 +1106,7 @@ static_assert(sizeof(osb_window_entry) == 80, "osb_window_entry layout");
 static_assert(sizeof(osb_anchor_result) == 760, "osb_anchor_result layout");
 static_assert(sizeof(osb_observability) == 5 * 256 + 16, "osb_observability layout");
 static_assert(sizeof(osb_predict_result) == 128, "osb_predict_result layout");
+static_assert(sizeof(osb_loop_record) == 88, "osb_loop_record layout");
 static_assert(sizeof(osb_sync_params) == 24, "osb_sync_params layout");
 
 struct osb_anchor {
@@ -981,6 +1190,13 @@ struct osb_anchor {
   int64_t* d_kw_stamp = nullptr;
   int32_t *d_kw_first = nullptr, *d_kw_drone = nullptr, *d_kw_block = nullptr, *d_kw_n = nullptr;
   int64_t kf_evicted = INT64_MIN;                 // the largest stamp whose slot a later keyframe took
+  // the loop map (record_loops_dev, init_by_loops_dev), acquired by the first of them: H + 1 records, the pair minima,
+  // the overflow flag and init_by_loops' status, and the event recorded after every call that reads or writes them
+  LoopRec* d_lm = nullptr;
+  unsigned long long* d_lm_pair = nullptr;
+  int32_t* d_lm_meta = nullptr;
+  int lm_H = 0;
+  cudaEvent_t last_loops = nullptr;
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -1930,5 +2146,146 @@ extern "C" osb_status osb_anchor_distance_factors_dev(osb_anchor* h, const osb_d
   OSB_LAUNCH(distance_factors_kernel, 1, DF_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
+  return OSB_OK;
+}
+
+namespace {
+
+// the first record_loops_dev or init_by_loops_dev acquires the map (no id recorded, no pair, no overflow) and its event
+osb_status loops_init(osb_anchor* h) {
+  if (h->d_lm_meta) return OSB_OK;
+  int H = 1;
+  while (H < 2 * h->p.max_measurements) H <<= 1;
+  const size_t D = (size_t)h->p.max_drones;
+  Resources& R = h->res;
+  OSB_TRY(R.alloc(&h->d_lm, (size_t)H + 1));
+  OSB_TRY(R.alloc(&h->d_lm_pair, D * D));
+  OSB_TRY(R.event(&h->last_loops, cudaEventDisableTiming));
+  int32_t* meta = nullptr;
+  OSB_TRY(R.alloc(&meta, 2));
+  cudaStream_t st = h->stream;
+  OSB_CUDA(cudaMemsetAsync(h->d_lm, 0xff, ((size_t)H + 1) * sizeof(LoopRec), st));   // key -1, claim none, not recorded
+  OSB_CUDA(cudaMemsetAsync(h->d_lm_pair, 0xff, D * D * sizeof(unsigned long long), st));
+  OSB_CUDA(cudaMemsetAsync(meta, 0, 2 * sizeof(int32_t), st));
+  OSB_CUDA(cudaEventRecord(h->last_loops, st));
+  OSB_CUDA(cudaStreamSynchronize(st));
+  h->lm_H = H;
+  h->d_lm_meta = meta;                                             // set last: a failed first call is tried again
+  return OSB_OK;
+}
+
+LoopMapView loop_map_view(const osb_anchor* h) {
+  return LoopMapView{h->d_lm, h->d_lm_pair, h->d_lm_meta, h->lm_H, h->p.max_drones};
+}
+
+}  // namespace
+
+extern "C" osb_status osb_anchor_record_loops_dev(osb_anchor* h, const osb_anchor_result* rows_dev, int n, void* stream) {
+  OSB_REQUIRE(h != nullptr && n >= 0 && (n == 0 || rows_dev != nullptr), "null argument or negative count");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(loops_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  const LoopMapView v = loop_map_view(h);
+  const int blocks = std::min(cdiv(std::max(n, 1), LM_THREADS), 4 * num_sms());
+  OSB_CUDA(wait_event_capturable(st, h->last_loops));             // the map is the last record's and init's
+  OSB_LAUNCH(record_claim_kernel, blocks, LM_THREADS, 0, st, rows_dev, n, v);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(record_write_kernel, blocks, LM_THREADS, 0, st, rows_dev, n, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_loops, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_init_by_loops_dev(osb_anchor* h, osb_pcm_state* pcm, osb_solver* s, int32_t self_id,
+                                                   void* stream) {
+  OSB_REQUIRE(h != nullptr && pcm != nullptr && s != nullptr, "null argument");
+  OSB_REQUIRE(drone_ok(h, self_id), "self_id outside 0..max_drones-1");
+  PcmDeviceDir pd{};
+  OSB_TRY(pcm_device_dir(pcm, &pd));
+  int solver_dev = 0;
+  const int n_blocks = solver_node_count(s, &solver_dev);
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(pd.device == h->device && solver_dev == h->device, "the handles are on different devices");
+  OSB_REQUIRE(h->d_obs != nullptr, "no osb_anchor_observe_dev call on this handle: to_init is not set");
+  OSB_REQUIRE(!h->blk_negative && h->sw_max_block < n_blocks, "a window block outside 0 .. the solver's node count - 1");
+  DeviceGuard dg(h->device);
+  OSB_TRY(loops_init(h));
+  OSB_TRY(sync_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  SolverPoseWrite w{};
+  OSB_TRY(solver_pose_write(s, st, &w));
+  InitLoopsView v{};
+  v.obs = h->d_obs;
+  v.dir = pd.dir;
+  v.n_dir = pd.n_dir;
+  v.lm = loop_map_view(h);
+  v.win = h->d_sync_win; v.w_stamp = h->d_sw_stamp; v.w_block = h->d_sw_block;
+  v.kf_first = h->d_kf_first; v.kf_stamp = h->d_kf_stamp; v.kf_pose = h->d_kf_pose;
+  v.rec = h->d_rec;
+  v.traj_stamp = h->d_traj_stamp; v.traj_pose = h->d_traj_pose; v.traj_n = h->d_traj_n;
+  v.max_samples = h->p.max_traj_samples; v.max_drones = h->p.max_drones; v.self_id = self_id;
+  v.poses = w.poses;
+  if (pd.done) OSB_CUDA(wait_event_capturable(st, pd.done));     // the inlier sets of the last anchored PCM call
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // to_init
+  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the paths and the estimated flags
+  OSB_CUDA(wait_event_capturable(st, h->last_loops));             // the map
+  OSB_LAUNCH(init_by_loops_kernel, 1, IBL_THREADS, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(w.written, st));
+  OSB_CUDA(record_event_capturable(h->last_observe, st));         // the next observe, sync and record come after it
+  OSB_CUDA(record_event_capturable(h->last_sync, st));
+  OSB_CUDA(record_event_capturable(h->last_loops, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_init_by_loops_result(osb_anchor* h, osb_status* last) {
+  OSB_REQUIRE(h != nullptr && last != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *last = OSB_OK;
+  if (!h->d_lm_meta) return OSB_OK;
+  DeviceGuard dg(h->device);
+  int32_t st = 0;
+  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_loops, 0));
+  OSB_CUDA(cudaMemcpyAsync(&st, h->d_lm_meta + 1, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  *last = (osb_status)st;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, int cap, int32_t* n, int64_t* pair_min,
+                                          uint8_t* estimated) {
+  OSB_REQUIRE(h != nullptr && n != nullptr && cap >= 0 && (cap == 0 || out != nullptr), "null argument or negative cap");
+  std::lock_guard<std::mutex> lk(h->mu);
+  const size_t D = (size_t)h->p.max_drones;
+  *n = 0;
+  if (pair_min) std::fill(pair_min, pair_min + D * D, INT64_MAX);
+  if (estimated) memset(estimated, 0, D);
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  if (h->d_lm_meta) {
+    std::vector<LoopRec> tab((size_t)h->lm_H + 1);
+    std::vector<unsigned long long> pair(D * D);
+    OSB_CUDA(cudaStreamWaitEvent(st, h->last_loops, 0));
+    OSB_CUDA(cudaMemcpyAsync(tab.data(), h->d_lm, tab.size() * sizeof(LoopRec), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaMemcpyAsync(pair.data(), h->d_lm_pair, D * D * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaStreamSynchronize(st));
+    std::vector<osb_loop_record> recs;
+    for (const LoopRec& r : tab)
+      if (r.recorded == 1u) recs.push_back(r.r);
+    std::sort(recs.begin(), recs.end(), [](const osb_loop_record& a, const osb_loop_record& b) { return a.id < b.id; });
+    *n = (int32_t)recs.size();
+    std::copy(recs.begin(), recs.begin() + std::min((size_t)cap, recs.size()), out);
+    if (pair_min)
+      for (size_t k = 0; k < D * D; ++k)
+        if (pair[k] != LM_NONE) pair_min[k] = (int64_t)(pair[k] ^ (1ull << 63));
+  }
+  if (estimated && h->d_rec) {
+    std::vector<SyncRecord> rec(D);
+    OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
+    OSB_CUDA(cudaMemcpyAsync(rec.data(), h->d_rec, D * sizeof(SyncRecord), cudaMemcpyDeviceToHost, st));
+    OSB_CUDA(cudaStreamSynchronize(st));
+    for (size_t d = 0; d < D; ++d) estimated[d] = rec[d].estimated ? 1 : 0;
+  }
   return OSB_OK;
 }

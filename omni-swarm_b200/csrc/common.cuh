@@ -319,6 +319,27 @@ osb_status solver_pose_write(osb_solver* h, cudaStream_t st, SolverPoseWrite* ou
 int solver_node_count(osb_solver* h, int* device);   // the resident graph's node count and the solver's device, without
                                                    // waiting for a device call
 
+// good_loops_set of one unordered drone pair in a PCM state's device copy (pcm.cu): a pair with a slot, or one that
+// set_inliers named.  Pair keys are (lo << 32) | hi.
+struct PcmDir {
+  int64_t key;
+  int64_t* gptr;               // ascending ids [gn] (duplicates allowed)
+  int32_t slot;                // -1: the pair has no loops
+  int32_t gn;                  // -1: the pair has no set
+  int32_t gcap, reserved;
+};
+// What osb_anchor_init_by_loops_dev reads of a PCM state (pcm.cu; not part of the C ABI): the directory of its device copy,
+// which the state's anchored calls and host-side changes keep current, and the number of entries in use, read on the
+// device.  `done` is recorded after the last anchored call made outside a capture (null otherwise).  OSB_ERR_INVALID
+// (error text set) when the state has no device copy yet.
+struct PcmDeviceDir {
+  int device;
+  const PcmDir* dir;
+  const int32_t* n_dir;
+  cudaEvent_t done;
+};
+osb_status pcm_device_dir(osb_pcm_state* s, PcmDeviceDir* out);
+
 // ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------

@@ -346,13 +346,6 @@ struct PcmSlot {               // a pair's device storage (one allocation)
   int32_t* clique;             // [1 + cap]: size, then the indices in maxCliqueHeu order
   int64_t* good;               // [cap]: the inlier ids of the last clique, ascending
 };
-struct PcmDir {                // good_loops_set of one unordered pair (a pair with a slot, or one set_inliers named)
-  int64_t key;
-  int64_t* gptr;               // ascending ids [gn] (duplicates allowed)
-  int32_t slot;                // -1: the pair has no loops
-  int32_t gn;                  // -1: the pair has no set
-  int32_t gcap, reserved;
-};
 
 struct PcmRows {               // the anchored call's rows and the routing rule
   const osb_anchor_result* rows;
@@ -1174,6 +1167,19 @@ extern "C" osb_status osb_pcm_state_reject_anchored(osb_pcm_state* s, const osb_
   s->ev_valid = cs == cudaStreamCaptureStatusNone;
   if (s->ev_valid) OSB_CUDA(cudaEventRecord(s->ev, st));
   s->dev_ahead = true;
+  return OSB_OK;
+}
+
+osb_status osb::pcm_device_dir(osb_pcm_state* s, PcmDeviceDir* out) {
+  std::lock_guard<std::mutex> lk(s->mu);
+  if (!s->dev) {
+    set_error("osb_anchor_init_by_loops_dev", "the PCM state has no device copy yet: no reject_anchored call on it");
+    return OSB_ERR_INVALID;
+  }
+  out->device = s->device;
+  out->dir = s->d_dir;
+  out->n_dir = &s->d_meta->n_dir;
+  out->done = s->ev_valid ? s->ev : nullptr;
   return OSB_OK;
 }
 

@@ -1030,6 +1030,37 @@ class LoopAnchor(_Handle):
                                             C.byref(n)))
         return stamps, poses
 
+    def record_loops_dev(self, rows_ptr: int, n: int, stream: int):
+        """the loop map of OutlierRejectionLoopEdges (osb_anchor_record_loops_dev) from the n rows run_dev wrote at
+        rows_ptr: every OK row's id the first time it is seen, and each drone pair's smallest id, on `stream` without
+        synchronising"""
+        _l.check(self._lib.osb_anchor_record_loops_dev(self._h, C.c_void_p(rows_ptr), int(n), C.c_void_p(stream)))
+
+    def init_by_loops_dev(self, pcm: "PcmState", solver: PoseGraphSolver, self_id: int, stream: int):
+        """init_pose_by_loops on the device (osb_anchor_init_by_loops_dev): the window blocks of the last observe's
+        to_init drones placed from their loops to estimated drones, written into the solver's resident poses on `stream`
+        without synchronising; a refusal shows in init_by_loops_result()"""
+        _l.check(self._lib.osb_anchor_init_by_loops_dev(self._h, pcm._h, solver._h, int(self_id), C.c_void_p(stream)))
+
+    def init_by_loops_result(self) -> int:
+        """waits for the last init_by_loops_dev -> its status (lib.OK, lib.ERR_INVALID or lib.ERR_CAPACITY)"""
+        last = C.c_int(0)
+        _l.check(self._lib.osb_anchor_init_by_loops_result(self._h, C.byref(last)))
+        return last.value
+
+    def loop_map(self) -> dict:
+        """waits for the last record_loops_dev and sync_dev -> dict(records: lib.LOOP_RECORD_DTYPE [n] ascending by id,
+        pair_min: int64 [max_drones, max_drones] (INT64_MAX: no id), estimated: bool [max_drones])"""
+        D = self.max_drones
+        n = C.c_int32(0)
+        pair = np.zeros((D, D), np.int64)
+        est = np.zeros(D, np.uint8)
+        _l.check(self._lib.osb_anchor_loop_map(self._h, None, 0, C.byref(n), _l.ptr(pair), _l.ptr(est)))
+        recs = np.zeros(n.value, _l.LOOP_RECORD_DTYPE)
+        if n.value:
+            _l.check(self._lib.osb_anchor_loop_map(self._h, _l.ptr(recs), n.value, C.byref(n), None, None))
+        return dict(records=recs, pair_min=pair, estimated=est.astype(bool))
+
     def predict(self, drones, vo_poses, self_id: int, finish_init: bool = True) -> dict:
         """PredictSwarm for one frame (osb_anchor_predict): drones [n], their odometry poses [n, 7] now -> {drone:
         (node_pose [7] or None, base_pose [7] or None)}"""
@@ -1235,6 +1266,23 @@ class AnchoredChain:
         solver.solve_multistart_resident_dev(max_tail, *self.factors.ptrs(), self.mask.data_ptr(), self.yaw.data_ptr(),
                                              self.stream.cuda_stream, n_trials, seed, window_size, acpt_cost, normalise,
                                              options)
+
+    def record_loops(self, anchor: LoopAnchor, n: int):
+        """the loop map from the first n rows (LoopAnchor.record_loops_dev), after run"""
+        anchor.record_loops_dev(self.rows.data_ptr(), n, self.stream.cuda_stream)
+
+    def init_by_loops(self, anchor: LoopAnchor, state: PcmState, solver: PoseGraphSolver, self_id: int, n_nodes: int):
+        """the pre-motion init branch's start (LoopAnchor.init_by_loops_dev), after reject and observe; the chain's mask
+        and yaw become n_nodes zeros (no block scattered), acquired on the current stream when n_nodes outgrows them"""
+        import torch
+        if self.mask is None or self.mask.numel() < n_nodes:
+            self.mask = torch.zeros(n_nodes, dtype=torch.uint8, device="cuda")
+            self.yaw = torch.zeros(n_nodes, dtype=torch.float64, device="cuda")
+            self.stream.wait_stream(torch.cuda.current_stream())
+        else:
+            with torch.cuda.stream(self.stream):
+                self.mask.zero_()
+        anchor.init_by_loops_dev(state, solver, self_id, self.stream.cuda_stream)
 
     def distances(self, anchor: LoopAnchor, max_tail: int, self_id: int, **kw):
         """the window's distance rows appended to the chain's rows (LoopAnchor.distance_factors_dev), after compact"""

@@ -147,6 +147,8 @@ ANCHOR_RESULT_DTYPE = np.dtype([("id", "<i8"), ("type", "<i4"), ("status", "<i4"
                                 ("dt_err_ns", "<i8"), ("dpos", "<f8"), ("edge", LOOP_EDGE_DTYPE), ("skip", "<i4"),
                                 ("factor_type", "<i4"), ("ia", "<i4"), ("ib", "<i4"), ("huber", "<i4"), ("reserved", "<i4"),
                                 ("payload", "<f8", PAYLOAD_LEN)])
+LOOP_RECORD_DTYPE = np.dtype([("id", "<i8"), ("id_a", "<i4"), ("id_b", "<i4"), ("stamp_a", "<i8"), ("stamp_b", "<i8"),
+                              ("rel_pose", "<f8", 7)])                  # osb_loop_record
 ANCHOR_OK, ANCHOR_EMPTY_WINDOW, ANCHOR_BEFORE_WINDOW, ANCHOR_NO_FRAME, ANCHOR_NO_TRAJECTORY, ANCHOR_DPOS, ANCHOR_VOID = range(7)
 
 
@@ -380,6 +382,10 @@ _SIG = {
     "osb_anchor_sync_dev": (C.c_int, [_P, _P, C.POINTER(SyncParams), _P]),
     "osb_anchor_sync_result": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int)]),
     "osb_anchor_paths": (C.c_int, [_P, C.c_int, C.c_int32, _P, _P, C.c_int, C.POINTER(C.c_int32)]),
+    "osb_anchor_record_loops_dev": (C.c_int, [_P, _P, C.c_int, _P]),
+    "osb_anchor_init_by_loops_dev": (C.c_int, [_P, _P, _P, C.c_int32, _P]),
+    "osb_anchor_init_by_loops_result": (C.c_int, [_P, C.POINTER(C.c_int)]),
+    "osb_anchor_loop_map": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int32), _P, _P]),
     "osb_anchor_predict": (C.c_int, [_P, C.POINTER(PredictParams), C.c_int, _P, _P, _P]),
     "osb_anchor_add_keyframe_dev": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, C.c_int, _P, C.POINTER(KeyframeParams), _P]),
     "osb_anchor_keyframe_flags": (C.c_int, [_P, C.c_int64, _P, C.c_int, C.POINTER(C.c_int32)]),
