@@ -814,6 +814,76 @@ osb_status osb_anchor_init_by_loops_dev(osb_anchor* h, osb_pcm_state* pcm, osb_s
 osb_status osb_anchor_init_by_loops_result(osb_anchor* h, osb_status* last);
 osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, int cap, int32_t* n, int64_t* pair_min,
                                uint8_t* estimated);
+/* Data association of anonymous detections (LocalizationDAInit, localization_DA_init.cpp, called at
+ *   swarm_localization_solver.cpp:893-916).  Opt-in: a handle that never calls osb_anchor_set_data_association behaves as
+ *   before, byte for byte.
+ * osb_anchor_set_data_association(): enables data association with the given parameters (a later call replaces them).
+ *   From then on add_measurements and add_measurements_dev also accept DET4D / DET6D rows whose id_b >= anon_min (an
+ *   anonymous target; the reference's MAX_DRONE_ID = 1000); id_a must still be a drone id and loops keep both ids in
+ *   0..max_drones-1.  Anonymous rows re-anchor as OSB_ANCHOR_NO_FRAME (find_node_frame_for_measurement_2drones finds no
+ *   frame of their target).  The first call acquires 280 bytes of device result and synchronises.  Refused
+ *   (OSB_ERR_INVALID): a null pointer, anon_min < max_drones, max_nodes < 1, a NaN accept_thres.
+ * osb_anchor_data_association_dev(): the DA branch of solve() on the device, on `stream` without synchronising.  One launch
+ *   of one CTA.  It runs when all of these hold on the device (else it changes nothing and reports applied = 0, OSB_OK):
+ *   the last observe's node set holds a drone with enable == 0 (has_node_not_inited), holds more than one drone, and the
+ *   store holds a detection (DET4D or DET6D: add_new_detection pushes both kinds to all_detections_6d).  Then, over the
+ *   store in order, the trajectories and the keyframe paths of the last applied osb_anchor_sync_dev:
+ *     unidentified = the id_b >= anon_min of the detections whose id_a has odometry; per such id the detector and the
+ *       covariance of its LAST such detection, and the FIRST detection of its SMALLEST detector (estimate_path);
+ *     no unidentified id, or self_id without odometry: nothing happens;
+ *     t0 = the largest first odometry stamp; est[self_id] = self's odometry at t0; then every drone with a keyframe path,
+ *       ascending: est[d] = path(d) at t0 (stamp t1) * odom_d(t1)^-1 odom_d(t0) (nearest samples, ties to the earlier);
+ *     the reference's DFS, literally (DESIGN.md section 7b): at each level the remaining ids ascending, skipping one whose
+ *       detector has no estimate; each drone with odometry other than the detector is tried, ascending; for a candidate
+ *       c > 0 the pose est[smallest detector] * odom(t0, ts_a) * relative_pose * odom_c(ts_b, t0) must pass
+ *       smd(log(est[c]^-1 pose), cov) < accept_thres when c has an estimate, and becomes est[c]; drone 0 is guessed but
+ *       never estimated; a leaf succeeds iff accept_thres > 0 and est covers every drone with odometry; the first
+ *       success of a level is kept, every candidate of that level is still searched, and a level whose id finds none
+ *       goes on to the next id.
+ *   On success every detection with id_b >= anon_min gets id_b = its guess, in place (anyoumos_det_mapper stays empty,
+ *   as in the reference) and the word osb_anchor_data_association_word points to becomes 1; else it becomes 0.
+ *   Refused on the device with no row renamed (applied = 0), reported by osb_anchor_data_association_result:
+ *   OSB_ERR_INVALID where the reference throws (a keyframe-path drone without odometry; estimate_path of a smallest
+ *   detector without an estimate; a leaf whose detectors or guessed drones lack an estimate, verify's at(); a success while
+ *   an anonymous row's id is not unidentified, guess.at()); OSB_ERR_CAPACITY for more than 32 unidentified ids or more DFS
+ *   calls than max_nodes.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null handle, self_id outside
+ *   0..max_drones-1, no set_data_association or no observe_dev since create.  The first call acquires the device counts
+ *   (as add_measurements_dev) and the sync's paths (as sync_dev) if they are not there yet, and synchronises; later calls
+ *   acquire nothing and can be captured.  Ordered after the handle's last run, append, observe and sync on any stream;
+ *   the next run_dev_if, append, update (push_odometry, add_measurements, set_window), observe and sync are ordered after
+ *   it.  A run_dev on another stream is not: order it after the data association on the caller's side.
+ *   The branch, as solve() runs it: run_dev -> observe_dev -> record_loops_dev -> reject_anchored -> data_association_dev
+ *   -> run_dev_if -> observe_dev_if -> record_loops_dev -> reject_anchored -> ...  (estimate_observability runs the loop
+ *   map and PCM each time; when nothing was applied the second pair sees the same rows and changes nothing).
+ *   max_nodes: the search runs on one thread (about 4-10 us a DFS call on an H100), and a search that does not resolve
+ *   uses its whole budget, so the budget bounds the branch's latency; 4096 is the bindings' default.
+ * osb_anchor_data_association_result(): waits for the last data_association_dev -> *applied (1: rows renamed), *status
+ *   (OSB_OK, or the refusal), *n = the unidentified ids of an applied call and min(*n, cap) (anonymous id, drone) pairs,
+ *   ascending by anonymous id.  All zero before the first call.
+ * osb_anchor_data_association_word(): the device address of the applied word (an int32, 0 before the first call), for
+ *   osb_anchor_run_dev_if / osb_anchor_observe_dev_if.  OSB_ERR_INVALID before set_data_association.
+ * osb_anchor_run_dev_if() / osb_anchor_observe_dev_if(): run_dev and observe_dev with the same launches, predicated on
+ *   *pred_dev read on the device: 0 writes nothing (rows, state and record keep every byte), else the call is run_dev's /
+ *   observe_dev's, except that observe_dev_if keeps a motion_new the record already holds (motion_new |= this call's), so
+ *   the record reflects both observe calls of one solve.  run_dev_if returns the same *n_out as run_dev. */
+typedef struct {
+  float accept_thres;            /* DA_accept_thres (3.345f), compared as a double */
+  int32_t anon_min;              /* MAX_DRONE_ID (1000): detection targets at or above it are anonymous */
+  int32_t max_nodes;             /* search budget: DFS calls per data_association_dev */
+  int32_t reserved;
+} osb_da_params;
+typedef struct {
+  int32_t anon_id, drone_id;
+} osb_da_guess;
+osb_status osb_anchor_set_data_association(osb_anchor* h, const osb_da_params* p);
+osb_status osb_anchor_data_association_dev(osb_anchor* h, int32_t self_id, void* stream);
+osb_status osb_anchor_data_association_result(osb_anchor* h, int32_t* applied, osb_status* status, osb_da_guess* guess,
+                                              int cap, int32_t* n);
+osb_status osb_anchor_data_association_word(osb_anchor* h, const int32_t** applied_dev);
+osb_status osb_anchor_run_dev_if(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
+                                 const int32_t* pred_dev, void* stream);
+osb_status osb_anchor_observe_dev_if(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev, int n,
+                                     const int32_t* pred_dev, void* stream);
 /* osb_anchor_predict(): PredictSwarm / PredictNode / NodeCooridnateOffset (swarm_localization_solver.cpp:673-765) for one
  *   frame of n drones (distinct ids, vo_poses7 [n][7] their odometry now), from the prediction record of the last applied
  *   sync.  With the drone's record (saved block pose P4, its frame's self_pose vo):

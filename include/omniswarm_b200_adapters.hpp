@@ -451,6 +451,22 @@ class ResidentPoseGraph {
     return solve_with_multiple_init_dev(max_tail, type_dev, ia_dev, ib_dev, payload_dev, huber_dev, count_dev,
                                         zero_mask_dev, nullptr, ms, stream, opt);
   }
+  // solve()'s data association (:893-916) after the first run -> observe -> record_loops -> reject_anchored, on the
+  // device (record_loops_dev and reject_anchored follow it again, as the second estimate_observability runs them): the
+  // search and
+  // the renaming (osb_anchor_data_association_dev), then estimate_observability again on the renamed store, predicated
+  // on the search's applied word (run_dev_if, observe_dev_if), so the launches do not depend on the outcome and the
+  // branch can be captured.  rows_dev holds the first run_dev's n rows and gets the second's; returns its row count.
+  static int32_t try_data_association_dev(osb_anchor* anchor, const osb_observe_params* obs_params,
+                                          const uint8_t* yaw_observable, osb_anchor_result* rows_dev, void* stream) {
+    check(osb_anchor_data_association_dev(anchor, obs_params->self_id, stream), "osb_anchor_data_association_dev");
+    const int32_t* applied = nullptr;
+    check(osb_anchor_data_association_word(anchor, &applied), "osb_anchor_data_association_word");
+    int32_t n = 0;
+    check(osb_anchor_run_dev_if(anchor, yaw_observable, rows_dev, &n, applied, stream), "osb_anchor_run_dev_if");
+    check(osb_anchor_observe_dev_if(anchor, obs_params, rows_dev, n, applied, stream), "osb_anchor_observe_dev_if");
+    return n;
+  }
   double cost_now = 0.0;             // equv_cost of the trial solve_with_multiple_init_dev accepted last (:809)
 
  private:

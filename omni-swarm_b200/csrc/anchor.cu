@@ -107,8 +107,7 @@ __device__ __forceinline__ void store_pose(double* dst, const PoseD& p) {
   dst[0] = p.t[0]; dst[1] = p.t[1]; dst[2] = p.t[2]; dst[3] = p.q[0]; dst[4] = p.q[1]; dst[5] = p.q[2]; dst[6] = p.q[3];
 }
 
-__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
-anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
+__device__ __forceinline__ void anchor_rows(const AnchorView& v, osb_anchor_result* __restrict__ out) {
   __shared__ double s_meas[ANCHOR_WARPS][MEAS_WORDS];
   __shared__ double s_out[ANCHOR_WARPS][RESULT_WORDS];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -215,6 +214,18 @@ anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
   for (int j = lane; j < RESULT_WORDS; j += 32) dst[j] = s_out[w][j];
 }
 
+__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
+anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
+  anchor_rows(v, out);
+}
+
+// the same, predicated on a device word (osb_anchor_run_dev_if): 0 writes nothing
+__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
+anchor_if_kernel(const AnchorView v, osb_anchor_result* __restrict__ out, const int32_t* __restrict__ pred) {
+  if (*pred == 0) return;
+  anchor_rows(v, out);
+}
+
 // setup_problem_with_loops_and_detections on the device: the rows with skip == 0 (and keep[i]) become the solver's SoA in
 // row order.  One CTA streams the rows in tiles of COMPACT_THREADS x COMPACT_ROWS; thread t owns COMPACT_ROWS consecutive
 // rows of a tile and a block scan of the per-thread counts gives each kept row its output index (no atomics, so the order
@@ -310,7 +321,7 @@ __device__ __forceinline__ bool append_keeps(const osb_measurement& r, float thr
 
 __global__ void __launch_bounds__(APPEND_THREADS)
 anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __restrict__ count_dev, int max_n, float thres,
-                     int max_drones, int max_meas, osb_measurement* __restrict__ meas, int32_t* __restrict__ loop_slot,
+                     int max_drones, int anon_min, int max_meas, osb_measurement* __restrict__ meas, int32_t* __restrict__ loop_slot,
                      int32_t* __restrict__ det_slot, int32_t* __restrict__ counts, CountRecord* __restrict__ fb,
                      long long seq, long long charged) {
   __shared__ int s_bad;
@@ -326,7 +337,9 @@ anchor_append_kernel(const osb_measurement* __restrict__ m, const int32_t* __res
     for (int i = tid; i < n; i += APPEND_THREADS) {
       const osb_measurement& r = m[i];
       const bool ok = (r.type == OSB_MEAS_LOOP || r.type == OSB_MEAS_DET4D || r.type == OSB_MEAS_DET6D) &&
-                      r.id_a >= 0 && r.id_a < max_drones && r.id_b >= 0 && r.id_b < max_drones;
+                      r.id_a >= 0 && r.id_a < max_drones && r.id_b >= 0 &&
+                      (r.id_b < max_drones || (r.type != OSB_MEAS_LOOP && anon_min > 0 && r.id_b >= anon_min));
+                                                                                                  // anon_min 0: no DA
       if (!ok) s_bad = 1;
       else kept += append_keeps(r, thres);
     }
@@ -398,9 +411,10 @@ observe_edges_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_
     if (s_adj[k]) atomicOr(adj + k, s_adj[k]);
 }
 
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
-                     int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs) {
+// keep_new: motion_new |= the record's (the second observe of a solve, observe_dev_if)
+__device__ __forceinline__ void observe_state(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win,
+                                              int max_drones, int self_id, float xy_thres, float z_thres,
+                                              osb_observability* __restrict__ obs, bool keep_new) {
   __shared__ unsigned long long s_adj[ANCHOR_MAX_DRONES][OBS_WORDS];
   __shared__ unsigned long long s_seen[OBS_WORDS], s_front[OBS_WORDS], s_next[OBS_WORDS];
   __shared__ int s_more;
@@ -462,13 +476,18 @@ observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* 
     const bool single = win->n_frames > SINGLE_DRONE_SFS_THRES && win->n_nodes == 1;   // :1364-1367
     obs->solve_master = obs->solve_master || single || other || motion;
     obs->motion = motion;
-    obs->motion_new = motion_new;
+    obs->motion_new = motion_new || (keep_new && obs->motion_new);
     obs->reserved = 0;
   }
 }
-
 __global__ void __launch_bounds__(OBS_THREADS)
-observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones, const osb_observability* __restrict__ obs) {
+observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
+                     int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs) {
+  observe_state(adj, win, max_drones, self_id, xy_thres, z_thres, obs, false);
+}
+
+__device__ __forceinline__ void observe_skip(osb_anchor_result* __restrict__ rows, int n, int max_drones,
+                                             const osb_observability* __restrict__ obs) {
   const int i = blockIdx.x * OBS_THREADS + threadIdx.x;
   if (i >= n) return;
   bool use = rows[i].status == OSB_ANCHOR_OK;                      // anchor_kernel's rule (:1066-1073) with this yaw
@@ -478,6 +497,48 @@ observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones,
           rows[i].node_a != rows[i].node_b;
   }
   rows[i].skip = use ? 0 : 1;
+}
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones, const osb_observability* __restrict__ obs) {
+  observe_skip(rows, n, max_drones, obs);
+}
+
+// observe_dev_if: the three launches above, predicated on a device word (0 writes nothing)
+// a copy of observe_edges_kernel's body: sharing it through an inline function changes that kernel's register
+// allocation, and the unpredicated kernels keep their code
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_edges_if_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_drones, unsigned* __restrict__ adj,
+                        const int32_t* __restrict__ pred) {
+  if (*pred == 0) return;
+  __shared__ unsigned s_adj[ANCHOR_MAX_DRONES * OBS_ROW32];
+  volatile unsigned* vs = s_adj;
+  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS) s_adj[k] = 0;
+  __syncthreads();
+  for (int i = blockIdx.x * OBS_THREADS + threadIdx.x; i < n; i += gridDim.x * OBS_THREADS) {
+    if (rows[i].status != OSB_ANCHOR_OK) continue;
+    const int a = rows[i].edge.id_a, b = rows[i].edge.id_b;
+    if ((unsigned)a >= (unsigned)max_drones || (unsigned)b >= (unsigned)max_drones) continue;
+    const int ab = a * OBS_ROW32 + (b >> 5), ba = b * OBS_ROW32 + (a >> 5);
+    const unsigned bit_b = 1u << (b & 31), bit_a = 1u << (a & 31);
+    if (!(vs[ab] & bit_b)) atomicOr(&s_adj[ab], bit_b);          // most rows repeat a pair already set
+    if (!(vs[ba] & bit_a)) atomicOr(&s_adj[ba], bit_a);
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS)
+    if (s_adj[k]) atomicOr(adj + k, s_adj[k]);
+}
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_state_if_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
+                        int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs,
+                        const int32_t* __restrict__ pred) {
+  if (*pred == 0) return;
+  observe_state(adj, win, max_drones, self_id, xy_thres, z_thres, obs, true);
+}
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_skip_if_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones,
+                       const osb_observability* __restrict__ obs, const int32_t* __restrict__ pred) {
+  if (*pred == 0) return;
+  observe_skip(rows, n, max_drones, obs);
 }
 
 // random_init_pose's choice of blocks (swarm_localization_solver.cpp:204-216) from the last observe's to_init: thread b
@@ -1097,6 +1158,260 @@ __global__ void __launch_bounds__(IBL_THREADS) init_by_loops_kernel(const InitLo
   if (d == 0) v.lm.meta[1] = OSB_OK;
 }
 
+// LocalizationDAInit::try_data_association (localization_DA_init.cpp:29-90) and its DFS (:153-272) for the call site at
+// swarm_localization_solver.cpp:893-916.  One CTA: the threads gather the unidentified ids (ascending, by repeated block
+// minima, so the order is the reference's std::set and no result depends on atomics' order), their detections and the
+// starting estimates; thread 0 then walks the DFS with an explicit stack in the reference's order, and on success the
+// threads rename the store's anonymous rows.
+constexpr int DA_THREADS = 256;                                    // = ANCHOR_MAX_DRONES
+constexpr int DA_MAX_IDS = 32;
+constexpr int DA_WORDS = ANCHOR_MAX_DRONES / 64;
+
+struct DaResult {                     // the device record data_association_result reads; applied is the predicate word
+  int32_t applied, status, n, reserved;
+  int64_t nodes;                      // DFS calls of the last search
+  int32_t anon[DA_MAX_IDS], guess[DA_MAX_IDS];
+};
+
+struct DaView {
+  const osb_observability* obs;
+  const osb_measurement* meas;
+  const int32_t* det_slot;
+  const int32_t* counts;              // [2] loops, detections
+  const int64_t* traj_stamp;
+  const double* traj_pose;
+  const int32_t* traj_n;
+  const int32_t* kf_first;
+  const int64_t* kf_stamp;
+  const double* kf_pose;
+  int max_samples, max_drones, self_id, anon_min, max_nodes;
+  double thres;
+  DaResult* res;
+  osb_measurement* meas_w;            // = meas: the rows renamed in place
+};
+
+__device__ __forceinline__ PoseD da_ego(const DaView& v, int d, int64_t t, int64_t* t_out) {
+  const size_t base = (size_t)d * v.max_samples;
+  const int k = nearest_sample(v.traj_stamp + base, v.traj_n[d], t);
+  if (t_out) *t_out = v.traj_stamp[base + k];
+  return load_pose(v.traj_pose + (base + k) * 7);
+}
+__device__ __forceinline__ PoseD da_rel(const DaView& v, int d, int64_t t1, int64_t t2) {   // pose(t1)^-1 pose(t2)
+  return pose_mul(pose_inv(da_ego(v, d, t1, nullptr)), da_ego(v, d, t2, nullptr));
+}
+__device__ __forceinline__ bool bit_of(const unsigned long long* m, int d) { return (m[d >> 6] >> (d & 63)) & 1ull; }
+__device__ __forceinline__ int da_index(const int* ids, int n, int id) {   // the unidentified id's index, -1: none
+  for (int k = 0; k < n; ++k)
+    if (ids[k] == id) return k;
+  return -1;
+}
+
+__global__ void __launch_bounds__(DA_THREADS) data_association_kernel(const DaView v) {
+  __shared__ double s_est[ANCHOR_MAX_DRONES][7];
+  __shared__ unsigned long long s_has[DA_WORDS], s_avail[DA_WORDS], s_need[DA_WORDS];
+  __shared__ int s_ids[DA_MAX_IDS + 1], s_n, s_min;
+  __shared__ int s_last[DA_MAX_IDS], s_det_min[DA_MAX_IDS], s_first[DA_MAX_IDS];
+  __shared__ int s_guess[DA_MAX_IDS];
+  __shared__ unsigned long long s_t0;
+  __shared__ int s_orphan, s_status, s_ok;
+  const int t = threadIdx.x;
+  const int D = v.max_drones;
+  DaResult& R = *v.res;
+  if (t == 0) { R.applied = 0; R.status = OSB_OK; R.n = 0; R.nodes = 0; }
+  // the gate (:893-900): a node not enabled, more than one node, a detection in the store
+  const bool node = t < D && v.obs->nodes[t];
+  const int not_inited = __syncthreads_or(node && !v.obs->enable[t]);
+  const int n_nodes = __syncthreads_count(node);
+  const int n_det = v.counts[1];
+  if (!not_inited || n_nodes <= 1 || n_det <= 0) return;
+  // unidentified, ascending: repeated block minima of the anonymous ids above the last one found
+  if (t == 0) s_n = 0;
+  if (t < DA_WORDS) { s_has[t] = s_avail[t] = s_need[t] = 0ull; }
+  if (t < DA_MAX_IDS) { s_last[t] = -1; s_det_min[t] = INT_MAX; s_first[t] = INT_MAX; }
+  if (t == 0) { s_t0 = 0ull; s_orphan = 0; s_status = OSB_OK; s_ok = 0; }
+  __syncthreads();
+  for (int prev = INT_MIN;;) {
+    if (t == 0) s_min = INT_MAX;
+    __syncthreads();
+    int mine = INT_MAX;
+    for (int i = t; i < n_det; i += DA_THREADS) {
+      const osb_measurement& m = v.meas[v.det_slot[i]];
+      if (m.id_b >= v.anon_min && m.id_b > prev && v.traj_n[m.id_a] > 0 && m.id_b < mine) mine = m.id_b;
+    }
+    if (mine != INT_MAX) atomicMin(&s_min, mine);
+    __syncthreads();
+    const int found = s_min;
+    __syncthreads();
+    if (found == INT_MAX) break;
+    if (t == 0) s_ids[s_n] = found;
+    if (t == 0) ++s_n;
+    __syncthreads();
+    if (s_n > DA_MAX_IDS) break;
+    prev = found;
+  }
+  const int n_u = s_n;
+  if (n_u == 0) return;                                            // :46-48
+  // per id: its last detection (raw_dets, uniden_detector), its detectors, the first row of its smallest detector
+  for (int i = t; i < n_det; i += DA_THREADS) {
+    const osb_measurement& m = v.meas[v.det_slot[i]];
+    if (m.id_b < v.anon_min) continue;
+    const int k = da_index(s_ids, min(n_u, DA_MAX_IDS), m.id_b);
+    if (k < 0) { s_orphan = 1; continue; }                          // no detector with odometry: guess.at() throws
+    if (v.traj_n[m.id_a] == 0) continue;
+    atomicMax(&s_last[k], i);
+    atomicMin(&s_det_min[k], m.id_a);
+    atomicOr(&s_need[m.id_a >> 6], 1ull << (m.id_a & 63));        // verify() reads every detector's estimate
+  }
+  __syncthreads();
+  for (int i = t; i < n_det; i += DA_THREADS) {
+    const osb_measurement& m = v.meas[v.det_slot[i]];
+    if (m.id_b < v.anon_min) continue;
+    const int k = da_index(s_ids, min(n_u, DA_MAX_IDS), m.id_b);
+    if (k >= 0 && m.id_a == s_det_min[k]) atomicMin(&s_first[k], i);
+  }
+  // available_nodes and t0 = the largest first odometry stamp (:56-65)
+  const bool avail = t < D && v.traj_n[t] > 0;
+  if (avail) {
+    atomicOr(&s_avail[t >> 6], 1ull << (t & 63));
+    atomicMax(&s_t0, (unsigned long long)v.traj_stamp[(size_t)t * v.max_samples] ^ (1ull << 63));
+  }
+  __syncthreads();
+  if (!bit_of(s_avail, v.self_id)) return;                         // :53-55
+  const int64_t t0 = (int64_t)(s_t0 ^ (1ull << 63));
+  // est_poses_t0 (:67-76): self from its odometry, then every drone with a keyframe path (self overwritten)
+  if (t == v.self_id) {
+    store_pose(s_est[t], da_ego(v, t, t0, nullptr));
+    atomicOr(&s_has[t >> 6], 1ull << (t & 63));
+  }
+  __syncthreads();
+  bool bad = false;
+  if (t < D && v.kf_first[t + 1] > v.kf_first[t]) {
+    if (!avail) {
+      bad = true;                                                  // ego_motions.at() throws
+    } else {
+      const int lo = v.kf_first[t], hi = v.kf_first[t + 1];
+      const int k = lo + nearest_sample(v.kf_stamp + lo, hi - lo, t0);
+      store_pose(s_est[t], pose_mul(load_pose(v.kf_pose + (size_t)k * 7), da_rel(v, t, v.kf_stamp[k], t0)));
+      atomicOr(&s_has[t >> 6], 1ull << (t & 63));
+    }
+  }
+  if (__syncthreads_or(bad)) {
+    if (t == 0) R.status = OSB_ERR_INVALID;
+    return;
+  }
+  if (n_u > DA_MAX_IDS) {
+    if (t == 0) R.status = OSB_ERR_CAPACITY;
+    return;
+  }
+  if (t == 0) {
+    // the DFS with an explicit stack; frame l holds the remaining ids, the id and candidate it is at, whether a candidate
+    // of that id succeeded, and what its candidate changed in est (to undo on return)
+    uint32_t rem[DA_MAX_IDS + 1];
+    int u_at[DA_MAX_IDS + 1], c_at[DA_MAX_IDS + 1], g[DA_MAX_IDS + 1];
+    bool found[DA_MAX_IDS + 1], had[DA_MAX_IDS + 1];
+    double old[DA_MAX_IDS + 1][7];
+    int lvl = 0, status = OSB_OK;
+    long long nodes = 0;
+    bool recorded = false, ret = false;
+    rem[0] = n_u == 32 ? 0xffffffffu : ((1u << n_u) - 1u);
+    enum { ENTER, NEXT_U, NEXT_C, RETURN } step = ENTER;
+    for (;;) {
+      if (step == ENTER) {
+        if (++nodes > v.max_nodes) { status = OSB_ERR_CAPACITY; break; }
+        if (rem[lvl] == 0u) {                                      // a leaf (:166-181)
+          unsigned long long need[DA_WORDS];
+          for (int w = 0; w < DA_WORDS; ++w) need[w] = s_need[w];
+          for (int l = 0; l < lvl; ++l) need[g[l] >> 6] |= 1ull << (g[l] & 63);
+          bool miss = false, all = true;
+          for (int w = 0; w < DA_WORDS; ++w) {
+            miss = miss || (need[w] & ~s_has[w]) != 0ull;          // verify()'s est_pathes.at() throws
+            all = all && s_has[w] == s_avail[w];
+          }
+          if (miss) { status = OSB_ERR_INVALID; break; }
+          ret = v.thres > 0.0 && all;                              // verify() is 0: cost in [0, thres) iff thres > 0
+          if (ret && !recorded) {
+            for (int l = 0; l < lvl; ++l) s_guess[u_at[l]] = g[l];
+            recorded = true;
+          }
+          step = RETURN;
+          continue;
+        }
+        u_at[lvl] = -1;
+        step = NEXT_U;
+        continue;
+      }
+      if (step == RETURN) {
+        if (lvl == 0) break;
+        --lvl;
+        const int c = c_at[lvl];
+        if (c > 0) {                                               // undo this candidate's est entry
+          if (had[lvl]) for (int j = 0; j < 7; ++j) s_est[c][j] = old[lvl][j];
+          else s_has[c >> 6] &= ~(1ull << (c & 63));
+        }
+        found[lvl] = found[lvl] || ret;
+        step = NEXT_C;
+        continue;
+      }
+      if (step == NEXT_U) {                                        // the next id whose detector has an estimate
+        int u = u_at[lvl] + 1;
+        while (u < n_u && (!((rem[lvl] >> u) & 1u) || !bit_of(s_has, v.meas[v.det_slot[s_last[u]]].id_a))) ++u;
+        if (u >= n_u) { ret = false; step = RETURN; continue; }
+        u_at[lvl] = u;
+        c_at[lvl] = -1;
+        found[lvl] = false;
+        step = NEXT_C;
+        continue;
+      }
+      // NEXT_C: the next candidate drone of id u_at[lvl]
+      const int u = u_at[lvl];
+      const osb_measurement& last = v.meas[v.det_slot[s_last[u]]];
+      int c = c_at[lvl] + 1;
+      while (c < D && (!bit_of(s_avail, c) || c == last.id_a)) ++c;
+      if (c >= D) {
+        if (found[lvl]) { ret = true; step = RETURN; }             // the first success of this id is kept (:259-263)
+        else step = NEXT_U;                                        // on to the next id
+        continue;
+      }
+      c_at[lvl] = c;
+      had[lvl] = false;
+      if (c > 0) {                                                 // estimate_path (:277-289) and the Mahalanobis gate
+        const osb_measurement& e = v.meas[v.det_slot[s_first[u]]];
+        if (!bit_of(s_has, e.id_a)) { status = OSB_ERR_INVALID; break; }   // est_poses_t0.at(edge.id_a)
+        const PoseD pose = pose_mul(pose_mul(pose_mul(load_pose(s_est[e.id_a]), da_rel(v, e.id_a, t0, e.stamp_a)),
+                                             load_pose(e.relative_pose)), da_rel(v, c, e.stamp_b, t0));
+        had[lvl] = bit_of(s_has, c);
+        if (had[lvl]) {
+          double lg[6];
+          pose_log(pose_mul(pose_inv(load_pose(s_est[c])), pose), lg);
+          if (!(smd6(lg, last.cov) < v.thres)) { c_at[lvl] = c; continue; }   // skip the candidate (step stays NEXT_C)
+          for (int j = 0; j < 7; ++j) old[lvl][j] = s_est[c][j];
+        }
+        store_pose(s_est[c], pose);
+        s_has[c >> 6] |= 1ull << (c & 63);
+      }
+      g[lvl] = c;
+      rem[lvl + 1] = rem[lvl] & ~(1u << u);
+      ++lvl;
+      step = ENTER;
+    }
+    R.nodes = nodes;
+    if (status == OSB_OK && ret && s_orphan) status = OSB_ERR_INVALID;   // guess.at() of a row left out of the search
+    s_status = status;
+    s_ok = status == OSB_OK && ret;
+  }
+  __syncthreads();
+  if (!s_ok) {
+    if (t == 0) R.status = s_status;
+    return;
+  }
+  for (int i = t; i < n_det; i += DA_THREADS) {                    // :84-88, in place
+    osb_measurement& m = v.meas_w[v.det_slot[i]];
+    if (m.id_b >= v.anon_min) m.id_b = s_guess[da_index(s_ids, n_u, m.id_b)];
+  }
+  if (t < n_u) { R.anon[t] = s_ids[t]; R.guess[t] = s_guess[t]; }
+  if (t == 0) { R.n = n_u; R.applied = 1; }
+}
+
 }  // namespace osb
 
 using namespace osb;
@@ -1197,6 +1512,12 @@ struct osb_anchor {
   int32_t* d_lm_meta = nullptr;
   int lm_H = 0;
   cudaEvent_t last_loops = nullptr;
+  // data association (set_data_association, data_association_dev): 0 until the setter, and then >= max_drones >= 1;
+  // 0 makes no id_b anonymous
+  int32_t da_anon_min = 0;
+  osb_da_params da{};
+  DaResult* d_da = nullptr;                       // acquired by the setter
+  cudaEvent_t last_da = nullptr;
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -1451,12 +1772,13 @@ extern "C" osb_status osb_anchor_push_odometry(osb_anchor* h, int32_t drone, int
 
 extern "C" osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const osb_measurement* m) {
   OSB_REQUIRE(h != nullptr && n >= 0 && (n == 0 || m), "null argument or negative count");
+  std::lock_guard<std::mutex> lk(h->mu);
   for (int i = 0; i < n; ++i) {
     OSB_REQUIRE(m[i].type == OSB_MEAS_LOOP || m[i].type == OSB_MEAS_DET4D || m[i].type == OSB_MEAS_DET6D,
                 "unknown measurement type");
-    OSB_REQUIRE(drone_ok(h, m[i].id_a) && drone_ok(h, m[i].id_b), "drone id outside 0..max_drones-1");
+    const bool anon = m[i].type != OSB_MEAS_LOOP && h->da_anon_min > 0 && m[i].id_b >= h->da_anon_min;
+    OSB_REQUIRE(drone_ok(h, m[i].id_a) && (drone_ok(h, m[i].id_b) || anon), "drone id outside 0..max_drones-1");
   }
-  std::lock_guard<std::mutex> lk(h->mu);
   OSB_TRY(anchor_settle(h));
   const int have = h->n_loops + h->n_dets;
   if ((long long)have + n > h->p.max_measurements) {
@@ -1596,8 +1918,9 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
 
 namespace {
 
+// pred: null for run / run_dev, the device word of run_dev_if
 osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
-                         cudaStream_t st) {
+                         cudaStream_t st, const int32_t* pred = nullptr) {
   AnchorView v{};
   v.meas = h->d_meas;
   v.loop_slot = h->d_loop_slot;
@@ -1629,13 +1952,14 @@ osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_ancho
   if (h->fb.pending) {                          // the counts are the device's; the grid covers the host's bound of them
     long long n[2], since;                      // lowered by what the last append that has RUN reported
     if (h->fb.read(n, &since)) h->upper = std::min(h->upper, n[0] + n[1] + since);
-    OSB_CUDA(cudaStreamWaitEvent(st, h->fb.ev, 0));
+    OSB_CUDA(wait_event_capturable(st, h->fb.ev));                // captured after a captured append: an external wait
     v.counts = h->d_counts;
     v.n_bound = (int)h->upper;
   }
   *n_out = v.n_bound;
   if (v.n_bound == 0) return OSB_OK;
-  OSB_LAUNCH(anchor_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
+  if (pred) OSB_LAUNCH(anchor_if_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev, pred);
+  else OSB_LAUNCH(anchor_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(h->last_run, st));             // captured: the updates after a replay wait for it
   return OSB_OK;
@@ -1649,6 +1973,17 @@ extern "C" osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_obser
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
   return anchor_launch(h, yaw_observable, out_dev, n_out, (cudaStream_t)stream);
+}
+
+extern "C" osb_status osb_anchor_run_dev_if(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev,
+                                            int32_t* n_out, const int32_t* pred_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr && yaw_observable != nullptr && out_dev != nullptr && n_out != nullptr && pred_dev != nullptr,
+              "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h->last_da) OSB_CUDA(wait_event_capturable(st, h->last_da));   // the word of the handle's own data association
+  return anchor_launch(h, yaw_observable, out_dev, n_out, st, pred_dev);
 }
 
 extern "C" osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int n, const uint8_t* keep_dev,
@@ -1710,7 +2045,7 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
   }
   const long long seq = h->fb.charge(max_n);
   OSB_LAUNCH(anchor_append_kernel, 1, APPEND_THREADS, 0, st, m_dev, count_dev, max_n, loop_outlier_distance_threshold,
-             h->p.max_drones, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb.dev, seq,
+             h->p.max_drones, h->da_anon_min, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb.dev, seq,
              h->fb.charged);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(h->fb.record(st));
@@ -1766,6 +2101,31 @@ extern "C" osb_status osb_anchor_observe_dev(osb_anchor* h, const osb_observe_pa
              p->self_id, p->init_xy_movement, p->init_z_movement, h->d_obs);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(observe_skip_kernel, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_observe, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_observe_dev_if(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev,
+                                                int n, const int32_t* pred_dev, void* stream) {
+  OSB_REQUIRE(h != nullptr && p != nullptr && rows_dev != nullptr && pred_dev != nullptr, "null argument");
+  OSB_REQUIRE(n >= 0, "negative row count");
+  OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  OSB_TRY(observe_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = h->p.max_drones;
+  const int blocks = cdiv(std::max(n, 1), OBS_THREADS);
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));
+  if (h->last_da) OSB_CUDA(wait_event_capturable(st, h->last_da));
+  OSB_LAUNCH(observe_edges_if_kernel, std::min(blocks, 4 * num_sms()), OBS_THREADS, 0, st, rows_dev, n, D, h->d_adj,
+             pred_dev);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(observe_state_if_kernel, 1, OBS_THREADS, 0, st, reinterpret_cast<unsigned long long*>(h->d_adj),
+             h->d_obs_win, D, p->self_id, p->init_xy_movement, p->init_z_movement, h->d_obs, pred_dev);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(observe_skip_if_kernel, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs, pred_dev);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(h->last_observe, st));
   return OSB_OK;
@@ -2287,5 +2647,90 @@ extern "C" osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, i
     OSB_CUDA(cudaStreamSynchronize(st));
     for (size_t d = 0; d < D; ++d) estimated[d] = rec[d].estimated ? 1 : 0;
   }
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_set_data_association(osb_anchor* h, const osb_da_params* p) {
+  OSB_REQUIRE(h != nullptr && p != nullptr, "null argument");
+  OSB_REQUIRE(p->anon_min >= h->p.max_drones, "anon_min must be >= max_drones: an anonymous id is no drone id");
+  OSB_REQUIRE(p->max_nodes >= 1, "max_nodes must be >= 1");
+  OSB_REQUIRE(!std::isnan(p->accept_thres), "accept_thres is NaN");
+  std::lock_guard<std::mutex> lk(h->mu);
+  DeviceGuard dg(h->device);
+  if (!h->d_da) {                                                  // the first call acquires the result and its event
+    OSB_TRY(h->res.event(&h->last_da, cudaEventDisableTiming));
+    DaResult* r = nullptr;
+    OSB_TRY(h->res.alloc(&r, 1));
+    OSB_CUDA(cudaMemsetAsync(r, 0, sizeof(DaResult), h->stream));
+    OSB_CUDA(cudaEventRecord(h->last_da, h->stream));
+    OSB_CUDA(cudaStreamSynchronize(h->stream));
+    h->d_da = r;
+  }
+  h->da = *p;
+  h->da_anon_min = p->anon_min;
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_data_association_dev(osb_anchor* h, int32_t self_id, void* stream) {
+  OSB_REQUIRE(h != nullptr, "null argument");
+  OSB_REQUIRE(drone_ok(h, self_id), "self_id outside 0..max_drones-1");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->d_da != nullptr, "no osb_anchor_set_data_association call on this handle");
+  OSB_REQUIRE(h->d_obs != nullptr, "no osb_anchor_observe_dev call on this handle: the node set is not known");
+  DeviceGuard dg(h->device);
+  OSB_TRY(anchor_dev_init(h));
+  OSB_TRY(sync_init(h));
+  cudaStream_t st = (cudaStream_t)stream;
+  DaView v{};
+  v.obs = h->d_obs;
+  v.meas = h->d_meas; v.meas_w = h->d_meas;
+  v.det_slot = h->d_det_slot;
+  v.counts = h->d_counts;
+  v.traj_stamp = h->d_traj_stamp; v.traj_pose = h->d_traj_pose; v.traj_n = h->d_traj_n;
+  v.kf_first = h->d_kf_first; v.kf_stamp = h->d_kf_stamp; v.kf_pose = h->d_kf_pose;
+  v.max_samples = h->p.max_traj_samples; v.max_drones = h->p.max_drones; v.self_id = self_id;
+  v.anon_min = h->da.anon_min; v.max_nodes = h->da.max_nodes;
+  v.thres = (double)h->da.accept_thres;
+  v.res = h->d_da;
+  OSB_CUDA(wait_event_capturable(st, h->last_run));               // the store: no run reads a row while it is renamed
+  if (h->fb.pending) OSB_CUDA(wait_event_capturable(st, h->fb.ev));   // ... and the device appends have written it
+  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // the node set and enable
+  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the keyframe paths
+  OSB_CUDA(wait_event_capturable(st, h->last_da));
+  OSB_LAUNCH(data_association_kernel, 1, DA_THREADS, 0, st, v);
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(record_event_capturable(h->last_run, st));             // the next run, append and update come after it
+  OSB_CUDA(record_event_capturable(h->last_observe, st));
+  OSB_CUDA(record_event_capturable(h->last_sync, st));
+  OSB_CUDA(record_event_capturable(h->last_da, st));
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_data_association_result(osb_anchor* h, int32_t* applied, osb_status* status,
+                                                         osb_da_guess* guess, int cap, int32_t* n) {
+  OSB_REQUIRE(h != nullptr && applied != nullptr && status != nullptr && n != nullptr && cap >= 0 &&
+              (cap == 0 || guess != nullptr), "null argument or negative cap");
+  std::lock_guard<std::mutex> lk(h->mu);
+  *applied = 0;
+  *status = OSB_OK;
+  *n = 0;
+  if (!h->d_da) return OSB_OK;
+  DeviceGuard dg(h->device);
+  DaResult r{};
+  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_da, 0));
+  OSB_CUDA(cudaMemcpyAsync(&r, h->d_da, sizeof(r), cudaMemcpyDeviceToHost, h->stream));
+  OSB_CUDA(cudaStreamSynchronize(h->stream));
+  *applied = r.applied;
+  *status = (osb_status)r.status;
+  *n = r.applied ? r.n : 0;
+  for (int k = 0; k < std::min(cap, (int)*n); ++k) guess[k] = osb_da_guess{r.anon[k], r.guess[k]};
+  return OSB_OK;
+}
+
+extern "C" osb_status osb_anchor_data_association_word(osb_anchor* h, const int32_t** applied_dev) {
+  OSB_REQUIRE(h != nullptr && applied_dev != nullptr, "null argument");
+  std::lock_guard<std::mutex> lk(h->mu);
+  OSB_REQUIRE(h->d_da != nullptr, "no osb_anchor_set_data_association call on this handle");
+  *applied_dev = &h->d_da->applied;
   return OSB_OK;
 }

@@ -1061,6 +1061,47 @@ class LoopAnchor(_Handle):
             _l.check(self._lib.osb_anchor_loop_map(self._h, _l.ptr(recs), n.value, C.byref(n), None, None))
         return dict(records=recs, pair_min=pair, estimated=est.astype(bool))
 
+    def set_data_association(self, accept_thres: float = 3.345, anon_min: int = 1000, max_nodes: int = 4096):
+        """enables data association (osb_anchor_set_data_association): detections with id_b >= anon_min are accepted
+        as anonymous; accept_thres is the reference's float DA_accept_thres; max_nodes bounds each search's DFS calls
+        (one thread, about 4-10 us a call on an H100: 4096 calls bound a search that does not resolve to tens of ms)"""
+        p = _l.DaParams(float(accept_thres), int(anon_min), int(max_nodes), 0)
+        _l.check(self._lib.osb_anchor_set_data_association(self._h, C.byref(p)))
+
+    def data_association_dev(self, self_id: int, stream: int):
+        """LocalizationDAInit on the device (osb_anchor_data_association_dev): on success the store's anonymous detections
+        are renamed in place, on `stream` without synchronising; the outcome shows in data_association_result()"""
+        _l.check(self._lib.osb_anchor_data_association_dev(self._h, int(self_id), C.c_void_p(stream)))
+
+    def data_association_result(self) -> tuple[bool, int, dict]:
+        """waits for the last data_association_dev -> (applied, status, {anonymous id: drone} of an applied call)"""
+        applied, status, n = C.c_int32(0), C.c_int(0), C.c_int32(0)
+        pairs = np.zeros((32, 2), np.int32)
+        _l.check(self._lib.osb_anchor_data_association_result(self._h, C.byref(applied), C.byref(status), _l.ptr(pairs),
+                                                              32, C.byref(n)))
+        return bool(applied.value), status.value, {int(a): int(d) for a, d in pairs[:n.value]}
+
+    def data_association_word(self) -> int:
+        """the device address of the applied word that run_dev_if / observe_dev_if read"""
+        w = C.c_void_p()
+        _l.check(self._lib.osb_anchor_data_association_word(self._h, C.byref(w)))
+        return int(w.value)
+
+    def run_dev_if(self, out_ptr: int, pred_ptr: int, stream: int, yaw_observable=None) -> int:
+        """run_dev predicated on the int32 at pred_ptr, read on the device (0 writes nothing) -> the row count"""
+        y = self._yaw(yaw_observable)
+        n = C.c_int32(0)
+        _l.check(self._lib.osb_anchor_run_dev_if(self._h, _l.ptr(y), C.c_void_p(out_ptr), C.byref(n), C.c_void_p(pred_ptr),
+                                                 C.c_void_p(stream)))
+        return n.value
+
+    def observe_dev_if(self, rows_ptr: int, n: int, pred_ptr: int, stream: int, self_id: int, init_xy_movement: float,
+                       init_z_movement: float):
+        """observe_dev predicated on the int32 at pred_ptr (0 writes nothing); a motion_new the record holds is kept"""
+        p = _l.ObserveParams(int(self_id), float(init_xy_movement), float(init_z_movement), 0)
+        _l.check(self._lib.osb_anchor_observe_dev_if(self._h, C.byref(p), C.c_void_p(rows_ptr), int(n), C.c_void_p(pred_ptr),
+                                                     C.c_void_p(stream)))
+
     def predict(self, drones, vo_poses, self_id: int, finish_init: bool = True) -> dict:
         """PredictSwarm for one frame (osb_anchor_predict): drones [n], their odometry poses [n, 7] now -> {drone:
         (node_pose [7] or None, base_pose [7] or None)}"""
@@ -1283,6 +1324,18 @@ class AnchoredChain:
             with torch.cuda.stream(self.stream):
                 self.mask.zero_()
         anchor.init_by_loops_dev(state, solver, self_id, self.stream.cuda_stream)
+
+    def data_association(self, anchor: LoopAnchor, self_id: int, init_xy_movement: float, init_z_movement: float) -> int:
+        """the DA branch (solve(), :893-916) after the first run -> observe -> record_loops -> reject:
+        LoopAnchor.data_association_dev, then run and observe again predicated on its applied word, the same launches
+        whatever the outcome -> the row count.  record_loops and reject follow it again, as the reference's second
+        estimate_observability runs them (with nothing applied they see the same rows and change nothing)"""
+        anchor.data_association_dev(self_id, self.stream.cuda_stream)
+        w = anchor.data_association_word()
+        n2 = anchor.run_dev_if(self.rows.data_ptr(), w, self.stream.cuda_stream)
+        anchor.observe_dev_if(self.rows.data_ptr(), n2, w, self.stream.cuda_stream, self_id, init_xy_movement,
+                              init_z_movement)
+        return n2
 
     def distances(self, anchor: LoopAnchor, max_tail: int, self_id: int, **kw):
         """the window's distance rows appended to the chain's rows (LoopAnchor.distance_factors_dev), after compact"""

@@ -113,6 +113,10 @@ KEYFRAME_NODE_DTYPE = np.dtype([("drone_id", "<i4"), ("block", "<i4"), ("new_blo
 KEYFRAME_DISTANCE_DTYPE = np.dtype([("peer", "<i4"), ("reserved", "<i4"), ("distance", "<f8")])
 
 
+class DaParams(C.Structure):
+    _fields_ = [("accept_thres", C.c_float), ("anon_min", C.c_int32), ("max_nodes", C.c_int32), ("reserved", C.c_int32)]
+
+
 class SyncParams(C.Structure):
     _fields_ = [("self_id", C.c_int32), ("full_path", C.c_int32), ("normalise", C.c_int32), ("window_size", C.c_int32),
                 ("acpt_cost", C.c_double)]
@@ -386,6 +390,13 @@ _SIG = {
     "osb_anchor_init_by_loops_dev": (C.c_int, [_P, _P, _P, C.c_int32, _P]),
     "osb_anchor_init_by_loops_result": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "osb_anchor_loop_map": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int32), _P, _P]),
+    "osb_anchor_set_data_association": (C.c_int, [_P, C.POINTER(DaParams)]),
+    "osb_anchor_data_association_dev": (C.c_int, [_P, C.c_int32, _P]),
+    "osb_anchor_data_association_result": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int), _P, C.c_int,
+                                                     C.POINTER(C.c_int32)]),
+    "osb_anchor_data_association_word": (C.c_int, [_P, C.POINTER(C.c_void_p)]),
+    "osb_anchor_run_dev_if": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32), _P, _P]),
+    "osb_anchor_observe_dev_if": (C.c_int, [_P, C.POINTER(ObserveParams), _P, C.c_int, _P, _P]),
     "osb_anchor_predict": (C.c_int, [_P, C.POINTER(PredictParams), C.c_int, _P, _P, _P]),
     "osb_anchor_add_keyframe_dev": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, C.c_int, _P, C.POINTER(KeyframeParams), _P]),
     "osb_anchor_keyframe_flags": (C.c_int, [_P, C.c_int64, _P, C.c_int, C.POINTER(C.c_int32)]),
