@@ -855,8 +855,12 @@ osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, int cap, int
  *   The branch, as solve() runs it: run_dev -> observe_dev -> record_loops_dev -> reject_anchored -> data_association_dev
  *   -> run_dev_if -> observe_dev_if -> record_loops_dev -> reject_anchored -> ...  (estimate_observability runs the loop
  *   map and PCM each time; when nothing was applied the second pair sees the same rows and changes nothing).
- *   max_nodes: the search runs on one thread (about 4-10 us a DFS call on an H100), and a search that does not resolve
- *   uses its whole budget, so the budget bounds the branch's latency; 4096 is the bindings' default.
+ *   max_nodes: the search runs on one thread and a search that does not resolve uses its whole budget.  The budget counts
+ *   DFS calls, not gate evaluations: one call can gate up to n_u x (D - 1) candidates (8160 at 32 ids and 256 drones), so
+ *   a search is bounded by max_nodes x n_u x (D - 1) gates, about 7.5 us each on an H100 80GB HBM3 at 700 W (measured).
+ *   At 32 ids and 256 drones that bounds a call by about 61 ms and the bindings' default of 4096 calls by about 250 s
+ *   (a measured worst case took about 50 ms a call).  Size max_nodes from the gate bound where latency matters
+ *   (DESIGN.md section 5).
  * osb_anchor_data_association_result(): waits for the last data_association_dev -> *applied (1: rows renamed), *status
  *   (OSB_OK, or the refusal), *n = the unidentified ids of an applied call and min(*n, cap) (anonymous id, drone) pairs,
  *   ascending by anonymous id.  All zero before the first call.

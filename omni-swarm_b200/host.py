@@ -1063,8 +1063,11 @@ class LoopAnchor(_Handle):
 
     def set_data_association(self, accept_thres: float = 3.345, anon_min: int = 1000, max_nodes: int = 4096):
         """enables data association (osb_anchor_set_data_association): detections with id_b >= anon_min are accepted
-        as anonymous; accept_thres is the reference's float DA_accept_thres; max_nodes bounds each search's DFS calls
-        (one thread, about 4-10 us a call on an H100: 4096 calls bound a search that does not resolve to tens of ms)"""
+        as anonymous; accept_thres is the reference's float DA_accept_thres; max_nodes bounds each search's DFS calls,
+        not its gate evaluations: a call can gate up to n_u x (max_drones - 1) candidates, so a search does up to
+        max_nodes x n_u x (max_drones - 1) of them, on one thread at about 7.5 us each (measured on an H100 80GB HBM3
+        at 700 W).  At 32 ids and 256 drones that bounds a call by about 61 ms and 4096 calls by about 250 s (a measured
+        worst case took about 50 ms a call)"""
         p = _l.DaParams(float(accept_thres), int(anon_min), int(max_nodes), 0)
         _l.check(self._lib.osb_anchor_set_data_association(self._h, C.byref(p)))
 

@@ -71,7 +71,7 @@ class DAInit:
         self.anon_min, self.max_nodes = anon_min, max_nodes
         self.available_nodes = sorted(self.ego)
         self.drone_dets_pair, self.drone_dets_by_pair, self.uniden_detector = {}, {}, {}
-        self.nodes = 0
+        self.nodes = self.gates = 0                                 # DFS calls and Mahalanobis gate evaluations
 
     def ego_at(self, d) -> ar.Trajectory:
         if d not in self.ego:
@@ -161,10 +161,11 @@ class DAInit:
                 new_est = dict(est)
                 if new_id > 0:
                     pose = self.estimate_path(u, new_guess, new_est, t0)
-                    if new_id not in new_est or mahalanobis(new_est[new_id], pose, cov) < self.accept_thres:
-                        new_est[new_id] = pose
-                    else:
-                        continue
+                    if new_id in new_est:
+                        self.gates += 1
+                        if not mahalanobis(new_est[new_id], pose, cov) < self.accept_thres:
+                            continue
+                    new_est[new_id] = pose
                 ok, c = self.dfs(new_est, new_guess, unidentified - {u}, raw, t0)
                 if ok and c < best_cost:
                     best_cost, best_guess, best_est = c, new_guess, new_est
@@ -175,22 +176,32 @@ class DAInit:
         return False, -1
 
 
-def da_literal(self_id, trajs, kf, dets, accept_thres, anon_min=1000, max_nodes=1 << 20):
-    """-> (applied, status, guess, id_b after the call) with status 'ok' / 'invalid' / 'capacity'"""
+def da_literal(self_id, trajs, kf, dets, accept_thres, anon_min=1000, max_nodes=1 << 20, stats=None):
+    """-> (applied, status, guess, id_b after the call) with status 'ok' / 'invalid' / 'capacity'; stats (a dict) gets
+    the search's DFS calls ("nodes") and Mahalanobis gate evaluations ("gates")"""
     ids = [int(r["id_b"]) for r in dets]
+    lit = DAInit(self_id, trajs, kf, dets, accept_thres, anon_min, max_nodes)
     try:
-        ok, guess, out = DAInit(self_id, trajs, kf, dets, accept_thres, anon_min, max_nodes).try_data_association()
+        ok, guess, out = lit.try_data_association()
     except Refused:
-        return False, "invalid", {}, ids
+        ok, guess, out, status = False, {}, ids, "invalid"
     except Capacity:
-        return False, "capacity", {}, ids
-    return ok, "ok", guess, out
+        ok, guess, out, status = False, {}, ids, "capacity"
+    else:
+        status = "ok"
+    if stats is not None:
+        stats.update(nodes=min(lit.nodes, max_nodes), gates=lit.gates)
+    return ok, status, guess, out
 
 
 # ---- the same over the device's representation ------------------------------------------------------------------
-def da_vec(self_id, trajs: dict, kf: dict, dets, accept_thres, anon_min=1000, max_nodes=1 << 20, max_drones=256):
-    """the kernel's walk: detection rows in store order, est as [D, 7] with a mask, the DFS as an explicit stack"""
+def da_vec(self_id, trajs: dict, kf: dict, dets, accept_thres, anon_min=1000, max_nodes=1 << 20, max_drones=256,
+           stats=None):
+    """the kernel's walk: detection rows in store order, est as [D, 7] with a mask, the DFS as an explicit stack; stats
+    (a dict) gets the DFS calls ("nodes", at most max_nodes) and Mahalanobis gate evaluations ("gates")"""
     D = max_drones
+    count = stats if stats is not None else {}
+    count.update(nodes=0, gates=0)
     thres = float(np.float32(accept_thres))
     id_a = np.asarray(dets["id_a"], np.int64)
     id_b = np.asarray(dets["id_b"], np.int64)
@@ -240,6 +251,7 @@ def da_vec(self_id, trajs: dict, kf: dict, dets, accept_thres, anon_min=1000, ma
             nodes += 1
             if nodes > max_nodes:
                 return False, "capacity", {}, id_b.tolist()
+            count["nodes"] = nodes
             if rem[lvl] == 0:
                 want = need.copy()
                 want[g[:lvl]] = True
@@ -297,6 +309,7 @@ def da_vec(self_id, trajs: dict, kf: dict, dets, accept_thres, anon_min=1000, ma
             had[lvl] = bool(has[c])
             if had[lvl]:
                 cov = np.asarray(dets[last[u]]["cov"], np.float64).reshape(6, 6)
+                count["gates"] += 1
                 if not mahalanobis(est[c], pose, cov) < thres:
                     continue
                 old[lvl] = est[c].copy()
