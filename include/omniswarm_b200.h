@@ -471,6 +471,17 @@ osb_status osb_pcm(const osb_loop_edge* edges, int n, double pcm_thres, double o
 osb_status osb_pcm_dev(const osb_loop_edge* edges_dev, int n, double pcm_thres, double odom_pos_cov_per_m,
                        double odom_ang_cov_per_m, int32_t* clique_dev, int32_t* clique_size_dev, uint8_t* adj_dev,
                        double* smd_dev, void* stream);
+/* Clique parity hook (tests only): pcm_max_clique_kernel on caller-given adjacency bit matrices, launched as each of its
+ *   callers launches it.  Graph g has n[g] vertices (1..slot_rows); its row i is bits[(g * slot_rows + i) * stride ..] with
+ *   bit j of word j / 32 set iff i and j are adjacent (symmetric, zero diagonal, bits past n[g] zero); stride >= the words
+ *   of a slot_rows-bit row.  out [n_graphs][1 + slot_rows]: the clique size, then its vertices in maxCliqueHeu's order.
+ *   form 0: one graph in one CTA, as osb_pcm_dev (pass stride = ceil(n / 32));
+ *   form 1: one CTA per graph from a host job list, with the shared memory of the largest in-smem graph, as
+ *           osb_pcm_state_reject;
+ *   form 2: n_ctas >= n_graphs CTAs with 200 KiB of shared memory and the job count read from the device, so the CTAs past
+ *           it exit, as osb_pcm_state_reject_anchored. */
+osb_status osb_pcm_clique_parity(int form, const uint32_t* bits, int n_graphs, const int32_t* n, int slot_rows, int stride,
+                                 int n_ctas, int32_t* out);
 /* Persistent PCM state -- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges (swarm_outlier_rejection.cpp:98-167, 173-297)
  *   with the state it keeps between solves: the consistency graph and the loops of every drone pair stay on the device, a
  *   call checks only its new loops (O(new x L) pair checks, not O(L^2)) and reruns maxCliqueHeu on the pairs that gained any.

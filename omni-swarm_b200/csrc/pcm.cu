@@ -31,6 +31,14 @@ namespace osb {
 
 constexpr int PCM_MAX_N = 4096;
 constexpr int PCM_MAX_W = PCM_MAX_N / 32;
+constexpr size_t PCM_CLIQUE_SMEM = 200 * 1024;       // the clique kernel's opt-in: a bit matrix of n <= 1280 fits
+
+// shared memory the clique kernel copies the bit matrix of an n-loop pair into: n x ceil(n/32) words when that fits in
+// PCM_CLIQUE_SMEM, else 0 (the kernel then reads the rows from global memory)
+__host__ __device__ inline size_t pcm_clique_smem(int n) {
+  const size_t need = (size_t)n * ((n + 31) / 32) * 4;
+  return need <= PCM_CLIQUE_SMEM ? need : 0;
+}
 
 // squared Mahalanobis consistency error of (e1 = the LATER loop, e2 = the earlier one); +inf for another drone pair
 __device__ double pcm_pair_smd(const osb_loop_edge* __restrict__ e1, const osb_loop_edge* __restrict__ e2, double pos_cov,
@@ -188,7 +196,7 @@ pcm_max_clique_kernel(const PcmPairJob* __restrict__ jobs, PcmPairJob one, int s
   clique_size += (size_t)blockIdx.x * out_step;
   const int n = job.n, W = (n + 31) / 32;
   const int lane = threadIdx.x;
-  const bool in_smem = (size_t)n * W * 4 <= 200 * 1024;
+  const bool in_smem = pcm_clique_smem(n) > 0;
   if (in_smem)
     for (int i = lane; i < n * W; i += 32) s_rows[i] = bits[(size_t)(i / W) * stride + i % W];
   __syncwarp();
@@ -277,14 +285,19 @@ osb_status pcm_device(const osb_loop_edge* edges_dev, int n, double thres, doubl
   const int W = (n + 31) / 32;
   OSB_LAUNCH(pcm_consistency_kernel, cdiv(n * W, 128), 128, 0, st, edges_dev, n, W, thres, pos_cov, ang_cov, bits, smd_dev);
   OSB_CHECK_LAUNCH();
-  const size_t need = (size_t)n * W * 4;
-  const size_t smem = need <= 200 * 1024 ? need : 0;
-  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, 200 * 1024);
+  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, PCM_CLIQUE_SMEM);
   const PcmPairJob one{nullptr, bits, deg, inter, 0, n, 0, 0};
-  OSB_LAUNCH(pcm_max_clique_kernel, 1, 32, smem, st, nullptr, one, W, clique_dev, size_dev, 0, adj_dev,
+  OSB_LAUNCH(pcm_max_clique_kernel, 1, 32, pcm_clique_smem(n), st, nullptr, one, W, clique_dev, size_dev, 0, adj_dev,
              (const int32_t*)nullptr);
   OSB_CHECK_LAUNCH();
   return OSB_OK;
+}
+
+// dynamic shared memory of a clique launch over a host-built job list: the largest in-smem job's bit matrix
+size_t pcm_jobs_clique_smem(const PcmPairJob* jobs, int k) {
+  size_t smem = 0;
+  for (int b = 0; b < k; ++b) smem = std::max(smem, pcm_clique_smem(jobs[b].n));
+  return smem;
 }
 
 // Incremental consistency of every pair that gained loops, in one launch.  Job k owns the work items
@@ -699,6 +712,50 @@ extern "C" osb_status osb_pcm(const osb_loop_edge* edges, int n, double pcm_thre
   return OSB_OK;
 }
 
+// Test-only parity hook: pcm_max_clique_kernel on caller-given bit matrices, in the launch form of each of its callers.
+extern "C" osb_status osb_pcm_clique_parity(int form, const uint32_t* bits, int n_graphs, const int32_t* n, int slot_rows,
+                                            int stride, int n_ctas, int32_t* out) {
+  OSB_REQUIRE(bits && n && out, "null argument");
+  OSB_REQUIRE(form >= 0 && form <= 2, "form must be 0 (one pair), 1 (host job list) or 2 (device job count)");
+  OSB_REQUIRE(n_graphs >= 1 && (form != 0 || n_graphs == 1), "form 0 takes one graph, the others at least one");
+  OSB_REQUIRE(slot_rows >= 1 && slot_rows <= PCM_MAX_N, "slot_rows must be in 1..4096");
+  OSB_REQUIRE(stride >= (slot_rows + 31) / 32 && stride <= PCM_MAX_W, "stride must hold a row of slot_rows bits");
+  OSB_REQUIRE(form != 2 || n_ctas >= n_graphs, "form 2 launches at least one CTA per graph");
+  for (int g = 0; g < n_graphs; ++g) OSB_REQUIRE(n[g] >= 1 && n[g] <= slot_rows, "every n must be in 1..slot_rows");
+  OSB_TRY(require_device());
+  Resources res;
+  const size_t slot_words = (size_t)slot_rows * stride, out_step = 1 + (size_t)slot_rows;
+  uint32_t* d_bits = nullptr;
+  int32_t *d_scratch = nullptr, *d_out = nullptr, *d_n_jobs = nullptr;
+  OSB_TRY(res.upload(&d_bits, bits, (size_t)n_graphs * slot_words));
+  OSB_TRY(res.alloc(&d_scratch, (size_t)n_graphs * 2 * slot_rows));
+  OSB_TRY(res.alloc(&d_out, (size_t)n_graphs * out_step));
+  std::vector<PcmPairJob> jobs(n_graphs);
+  for (int g = 0; g < n_graphs; ++g) {
+    int32_t* deg = d_scratch + (size_t)g * 2 * slot_rows;
+    jobs[g] = PcmPairJob{nullptr, d_bits + g * slot_words, deg, deg + slot_rows, 0, n[g], 0, 0};
+  }
+  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, PCM_CLIQUE_SMEM);
+  if (form == 0) {                                                  // osb_pcm_dev
+    OSB_LAUNCH(pcm_max_clique_kernel, 1, 32, pcm_clique_smem(n[0]), nullptr, nullptr, jobs[0], stride, d_out + 1, d_out,
+               0, (uint8_t*)nullptr, (const int32_t*)nullptr);
+  } else {
+    PcmPairJob* d_jobs = nullptr;
+    OSB_TRY(res.upload(&d_jobs, jobs.data(), jobs.size()));
+    if (form == 1) {                                                // osb_pcm_state_reject
+      OSB_LAUNCH(pcm_max_clique_kernel, n_graphs, 32, pcm_jobs_clique_smem(jobs.data(), n_graphs), nullptr, d_jobs,
+                 PcmPairJob{}, stride, d_out + 1, d_out, (int)out_step, (uint8_t*)nullptr, (const int32_t*)nullptr);
+    } else {                                                        // osb_pcm_state_reject_anchored
+      OSB_TRY(res.upload(&d_n_jobs, &n_graphs, 1));
+      OSB_LAUNCH(pcm_max_clique_kernel, n_ctas, 32, PCM_CLIQUE_SMEM, nullptr, d_jobs, PcmPairJob{}, stride, d_out + 1,
+                 d_out, (int)out_step, (uint8_t*)nullptr, (const int32_t*)d_n_jobs);
+    }
+  }
+  OSB_CHECK_LAUNCH();
+  OSB_CUDA(cudaMemcpy(out, d_out, (size_t)n_graphs * out_step * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return OSB_OK;
+}
+
 // =============================================================================================================
 // C ABI: osb_pcm_state -- SwarmLocalOutlierRejection's persistent PCM state (swarm_outlier_rejection.cpp:37-56, 98-297)
 // =============================================================================================================
@@ -998,7 +1055,6 @@ osb_status pcm_state_grow(osb_pcm_state* s, const std::map<std::pair<int32_t, in
   int64_t* staged_ids = (int64_t*)(s->h_stage + s->jobs_bytes + s->edges_bytes);
   int k = 0, n_staged = 0;
   long long items = 0;
-  size_t smem = 0;
   std::vector<int> changed;
   for (const auto& kv : fresh) {
     const int pi = s->index[kv.first];
@@ -1013,8 +1069,6 @@ osb_status pcm_state_grow(osb_pcm_state* s, const std::map<std::pair<int32_t, in
       staged[n_staged++] = edges[i];
     }
     items += (long long)m * (W - (m >> 5)) + (long long)(n - m) * W;
-    const size_t need = (size_t)n * W * 4;
-    if (need <= 200 * 1024) smem = std::max(smem, need);
     changed.push_back(pi);
     OSB_REQUIRE(items < (1ll << 31), "too many pair checks in one call");
   }
@@ -1030,9 +1084,9 @@ osb_status pcm_state_grow(osb_pcm_state* s, const std::map<std::pair<int32_t, in
   OSB_LAUNCH(pcm_grow_kernel, cdiv((int)items, 128), 128, 0, st, d_jobs, k, (int)items, (const PcmMeta*)nullptr, f, seen,
              s->stride, s->p.pcm_thres, s->p.odom_pos_cov_per_m, s->p.odom_ang_cov_per_m);
   OSB_CHECK_LAUNCH();
-  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, 200 * 1024);
+  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, PCM_CLIQUE_SMEM);
   const int out_step = 1 + s->p.pair_capacity;
-  OSB_LAUNCH(pcm_max_clique_kernel, k, 32, smem, st, d_jobs, PcmPairJob{}, s->stride, s->d_out + 1, s->d_out, out_step,
+  OSB_LAUNCH(pcm_max_clique_kernel, k, 32, pcm_jobs_clique_smem(jobs, k), st, d_jobs, PcmPairJob{}, s->stride, s->d_out + 1, s->d_out, out_step,
              (uint8_t*)nullptr, (const int32_t*)nullptr);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, (size_t)k * out_step * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1152,9 +1206,9 @@ extern "C" osb_status osb_pcm_state_reject_anchored(osb_pcm_state* s, const osb_
   OSB_LAUNCH(pcm_grow_kernel, 4 * s->G, 128, 0, st, s->d_jobs, 0, 0, s->d_meta, f, seen, s->stride, s->p.pcm_thres,
              s->p.odom_pos_cov_per_m, s->p.odom_ang_cov_per_m);
   OSB_CHECK_LAUNCH();
-  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, 200 * 1024);
+  OSB_SMEM_OPT_IN(pcm_max_clique_kernel, PCM_CLIQUE_SMEM);
   const int out_step = 1 + s->p.pair_capacity;
-  OSB_LAUNCH(pcm_max_clique_kernel, s->p.max_pairs, 32, 200 * 1024, st, s->d_jobs, PcmPairJob{}, s->stride, s->d_out + 1,
+  OSB_LAUNCH(pcm_max_clique_kernel, s->p.max_pairs, 32, PCM_CLIQUE_SMEM, st, s->d_jobs, PcmPairJob{}, s->stride, s->d_out + 1,
              s->d_out, out_step, (uint8_t*)nullptr, (const int32_t*)&s->d_meta->n_jobs);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(pcm_anchored_finish_kernel, s->p.max_pairs, PCM_FINISH_THREADS, 0, st, s->d_jobs, s->d_meta, s->d_out,

@@ -361,6 +361,7 @@ _SIG = {
     "osb_pnp_ransac_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "osb_pcm": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P]),
     "osb_pcm_dev": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P, _P]),
+    "osb_pcm_clique_parity": (C.c_int, [C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
     "osb_pcm_state_create": (C.c_int, [C.POINTER(_P), C.POINTER(PcmStateParams)]),
     "osb_pcm_state_destroy": (C.c_int, [_P]),
     "osb_pcm_state_reject": (C.c_int, [_P, _P, _P, C.c_int, _P]),

@@ -26,6 +26,8 @@ Third-party arithmetic that is ABSENT from the reference tree (HKUST-Swarm/swarm
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 
 
@@ -177,3 +179,146 @@ def max_clique_exact(adj):
         if all(adj[a, b] for k, a in enumerate(vs) for b in vs[k + 1:]):
             best = len(vs)
     return best
+
+
+# ---- the same arithmetic over arrays of pairs (a full 4096 x 4096 matrix, not a sample) ------------------------------
+# A pose is a tuple of 7 arrays (tx ty tz qw qx qy qz); every expression is the scalar one above, term for term.
+def _cross_v(a, b):
+    return (a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0])
+
+
+def _q_mul_v(a, b):
+    aw, ax, ay, az = a
+    bw, bx, by, bz = b
+    return (aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+            aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw)
+
+
+def _q_rot_v(q, v):
+    u = q[1:]
+    c = _cross_v(u, v)
+    d = _cross_v(u, c)
+    return tuple(v[k] + 2.0 * (q[0] * c[k] + d[k]) for k in range(3))
+
+
+def _pose_mul_v(a, b):
+    r = _q_rot_v(a[3:], b[:3])
+    return tuple(a[k] + r[k] for k in range(3)) + _q_mul_v(a[3:], b[3:])
+
+
+def _pose_inv_v(a):
+    qc = (a[3], -a[4], -a[5], -a[6])
+    r = _q_rot_v(qc, a[:3])
+    return (-r[0], -r[1], -r[2]) + qc
+
+
+def _log_map_v(p):
+    neg = p[3] < 0
+    q = tuple(np.where(neg, -x, x) for x in p[3:])
+    n = np.sqrt(q[1] * q[1] + q[2] * q[2] + q[3] * q[3])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        k = np.where(n < 1e-12, 2.0, 2.0 * np.arctan2(n, q[0]) / n)
+    return p[:3] + (k * q[1], k * q[2], k * q[3])
+
+
+def edge_arrays(edges):
+    """edge dicts -> dict of arrays (ids [n], rel / odom_a / odom_b [n, 7], cov [n, 6, 6], len_a / len_b [n])"""
+    return dict(id_a=np.array([e["id_a"] for e in edges], np.int64), id_b=np.array([e["id_b"] for e in edges], np.int64),
+                rel=np.array([e["rel"] for e in edges], np.float64).reshape(-1, 7),
+                cov=np.array([np.asarray(e["cov"], np.float64).reshape(6, 6) for e in edges]).reshape(-1, 6, 6),
+                odom_a=np.array([e["odom_a"] for e in edges], np.float64).reshape(-1, 7),
+                odom_b=np.array([e["odom_b"] for e in edges], np.float64).reshape(-1, 7),
+                len_a=np.array([e["len_a"] for e in edges], np.float64),
+                len_b=np.array([e["len_b"] for e in edges], np.float64))
+
+
+def pair_smd_batched(E, I, J, pos_cov_per_m, ang_cov_per_m, terms=False):
+    """pair_smd(edges[I[k]], edges[J[k]]) for every k (edge1 = I, the later loop), E = edge_arrays(edges): +inf for
+    another drone pair or a C that is not positive definite.  The same operations in the same order as pair_smd and
+    cholesky_smd, each one elementwise numpy operation.  With terms, also the quantities a forward-error bound of the
+    pair needs (tests/pcm_edges_ref.py)."""
+    ia, ib, ja, jb = E["id_a"][I], E["id_b"][I], E["id_a"][J], E["id_b"][J]
+    srp = np.where((ia == ja) & (ib == jb), 1, np.where((ia == jb) & (ib == ja), 2, 0))
+    two = srp == 2
+    pose = lambda a, idx: tuple(a[idx, k] for k in range(7))                      # noqa: E731
+    rel2 = pose(E["rel"], J)
+    inv2 = _pose_inv_v(rel2)
+    p2 = tuple(np.where(two, x, y) for x, y in zip(inv2, rel2))
+    oa2, ob2 = pose(E["odom_a"], J), pose(E["odom_b"], J)
+    a2 = tuple(np.where(two, x, y) for x, y in zip(ob2, oa2))
+    b2 = tuple(np.where(two, x, y) for x, y in zip(oa2, ob2))
+    la2 = np.where(two, E["len_b"][J], E["len_a"][J])
+    lb2 = np.where(two, E["len_a"][J], E["len_b"][J])
+    oa1, ob1, rel1 = pose(E["odom_a"], I), pose(E["odom_b"], I), pose(E["rel"], I)
+    odom_a = _pose_mul_v(_pose_inv_v(oa1), a2)
+    odom_b = _pose_mul_v(_pose_inv_v(ob1), b2)
+    dl = np.abs(la2 - E["len_a"][I]) + np.abs(lb2 - E["len_b"][I])
+    err = _pose_mul_v(_pose_mul_v(_pose_mul_v(odom_a, p2), _pose_inv_v(odom_b)), _pose_inv_v(rel1))
+    v = _log_map_v(err)
+    covI, covJ = E["cov"].reshape(-1, 36)[I], E["cov"].reshape(-1, 36)[J]
+    per_m = [pos_cov_per_m] * 3 + [ang_cov_per_m] * 3
+    C = [[covI[:, 6 * i + j] + covJ[:, 6 * i + j] + (np.diag(per_m)[i, j] * dl if i == j else 0.0) for j in range(6)]
+         for i in range(6)]
+    ok = srp > 0
+    L = [[None] * 6 for _ in range(6)]
+    y = [None] * 6
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for j in range(6):
+            s = C[j][j]
+            for k in range(j):
+                s = s - L[j][k] * L[j][k]
+            ok &= s > 0
+            L[j][j] = np.sqrt(np.where(ok, s, 1.0))
+            for i in range(j + 1, 6):
+                c = C[i][j]
+                for k in range(j):
+                    c = c - L[i][k] * L[j][k]
+                L[i][j] = c / L[j][j]
+        smd = 0.0
+        for i in range(6):
+            c = v[i]
+            for k in range(i):
+                c = c - L[i][k] * y[k]
+            y[i] = c / L[i][i]
+            smd = smd + y[i] * y[i]
+    smd = np.where(ok, smd, np.inf)
+    if not terms:
+        return smd
+    tn = lambda p: np.sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2])                   # noqa: E731
+    return smd, dict(T=tn(oa1) + tn(ob1) + tn(rel1) + tn(a2) + tn(b2) + tn(p2),
+                     Lsum=np.abs(E["len_a"][I]) + np.abs(E["len_b"][I]) + np.abs(la2) + np.abs(lb2), dl=dl,
+                     covF=np.linalg.norm(covI, axis=1) + np.linalg.norm(covJ, axis=1),
+                     C=np.stack([np.stack(np.broadcast_arrays(*row), -1) for row in C], -2),
+                     rv=np.sqrt(v[3] * v[3] + v[4] * v[4] + v[5] * v[5]), srp=srp)
+
+
+def consistency_matrix_batched(edges, pcm_thres, pos_cov_per_m, ang_cov_per_m, pairs_per_chunk=1 << 18, workers=None):
+    """consistency_matrix over arrays, a chunk of rows at a time (chunks on `workers` threads: numpy releases the GIL in
+    its elementwise loops): the same adjacency and smd matrices"""
+    from concurrent.futures import ThreadPoolExecutor
+    n = len(edges)
+    E = edge_arrays(edges)
+    adj = np.zeros((n, n), np.uint8)
+    smd = np.full((n, n), np.inf)
+    chunks, i0 = [], 1
+    while i0 < n:
+        i1 = i0 + 1
+        while i1 < n and (i1 * (i1 - 1) - i0 * (i0 - 1)) // 2 < pairs_per_chunk:
+            i1 += 1
+        chunks.append((i0, i1))
+        i0 = i1
+
+    def run(c):
+        i0, i1 = c
+        I, J = np.nonzero(np.tril(np.ones((i1 - i0, i1), bool), i0 - 1))
+        I += i0
+        s = pair_smd_batched(E, I, J, pos_cov_per_m, ang_cov_per_m)
+        smd[I, J] = s
+        smd[J, I] = s
+        a = (s < pcm_thres).astype(np.uint8)
+        adj[I, J] = a
+        adj[J, I] = a
+
+    with ThreadPoolExecutor(workers or min(16, os.cpu_count() or 1)) as ex:
+        list(ex.map(run, chunks))
+    return adj, smd

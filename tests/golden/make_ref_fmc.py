@@ -6,9 +6,13 @@ vertex, for
     (regenerated there from the same seed), and
   * the consistency graphs of tests/test_gpu_pcm.py (oracle/pcm_ref.py's consistency matrix of the seeded loop edges),
 
-so that both tests keep comparing with the reference where the reference tree is absent.
+so that both tests keep comparing with the reference where the reference tree is absent; and, in
+tests/golden/ref_fmc_edges.npz, its clique for each graph of tests/pcm_edges_ref.graph_families() (regenerated there from
+its seed; only the names and the cliques are stored), which tests/test_gpu_pcm_edges.py runs through every launch form of
+the clique kernel.
 
-    python tests/golden/make_ref_fmc.py        (needs the reference tree to build the library; writes tests/golden/ref_fmc.npz)
+    python tests/golden/make_ref_fmc.py        (needs the reference tree to build the library; writes both files)
+    python tests/golden/make_ref_fmc.py edges  (writes tests/golden/ref_fmc_edges.npz only)
 """
 import os
 import sys
@@ -60,9 +64,22 @@ def _row(i):
     return i, [(j, pr.pair_smd(_EDGES[i], _EDGES[j], POS, ANG)) for j in range(i)]
 
 
+def edge_families():
+    """tests/golden/ref_fmc_edges.npz: the library's clique of every graph of pcm_edges_ref.graph_families()"""
+    sys.path.insert(0, os.path.dirname(HERE))
+    import pcm_edges_ref
+    fams = pcm_edges_ref.graph_families()
+    verts, offs = pack([fmc_ref.max_clique_heu(a)[0] for _, a in fams])
+    np.savez_compressed(os.path.join(HERE, "ref_fmc_edges.npz"), names=np.array([nm for nm, _ in fams]), verts=verts,
+                        offs=offs)
+
+
 def main():
     global _EDGES
     assert fmc_ref.build(), "oracle/_ref/libfmc_ref.so could not be built (is the reference tree present?)"
+    edge_families()
+    if sys.argv[1:] == ["edges"]:
+        return
     out = {}
     pin = [fmc_ref.max_clique_heu(a) for a in pin_graphs()]
     out["pin_verts"], out["pin_offs"] = pack([c for c, _ in pin])

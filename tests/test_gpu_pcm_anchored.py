@@ -12,6 +12,8 @@ import torch
 from omniswarm_b200 import host, lib as _l, synth
 from oracle.pcm_state_ref import PcmStateRef
 from backend_harness import THRES, make_anchor, pcm_state
+from oracle import pcm_ref as pr
+import pcm_edges_ref as R
 
 pytestmark = pytest.mark.gpu
 DRONES = 5
@@ -95,6 +97,14 @@ def test_solve_rounds_match_the_host_sequence(gpu, redundant):
         fa = host.anchored_factor_rows(rows, keep_a)
         assert len(fa[0]) > 0 and all(x.tobytes() == y.tobytes() for x, y in zip(fa, fb))
         same_state(ha, hb)
+        for key, p in ref.pairs.items():                             # correlated covariances: against float64
+            smd, bnd = R.bound_matrix(p["edges"], ref.pos, ref.ang)
+            fin = np.isfinite(smd)
+            assert np.all(np.abs(smd[fin] - THRES) > 2 * bnd[fin]), "a pair within the bound of the threshold"
+            _, adj_d, clique_d = hb.pair(*key)
+            radj, _ = pr.consistency_matrix_batched(p["edges"], THRES, ref.pos, ref.ang)
+            assert np.array_equal(adj_d, radj) and np.array_equal(adj_d, p["adj"])
+            assert clique_d.tolist() == p["clique"]
         if r == 1:                                                   # other drones' sets, replaced when their pair grows
             for p in PAIRS:
                 if 0 not in p:
