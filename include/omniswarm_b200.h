@@ -557,9 +557,31 @@ osb_status osb_pcm_state_pair(osb_pcm_state* s, int32_t id_a, int32_t id_b, int3
  *   yaw_observable [max_drones] is read during the call.  Every run is one kernel launch (none when there is no measurement).
  * Errors: a drone id outside 0..max_drones-1, a null pointer, a stamp not after the drone's last one, an unknown type, a
  *   drone twice in one frame or a malformed frame_first give OSB_ERR_INVALID; exceeding a capacity gives OSB_ERR_CAPACITY.
- *   Either way the handle is unchanged.  Updates wait for the handle's last run on any stream before they overwrite state.
- * Memory: create acquires everything (a stream, an event, the trajectories, measurements, window and run output at their
- *   capacities); later only the first add_measurements_dev and the first observe_dev acquire theirs (below). */
+ *   Either way the handle is unchanged.
+ * Ordering: the handle's device state is in six parts.  A device call waits for the last call that touched (read or
+ *   wrote) each part it touches, on any stream, and then becomes that part's last toucher; so the calls that touch one
+ *   part run in the order they were made, whatever streams they are on, also inside a CUDA graph (there the waits and
+ *   records are external event nodes).  Reads and writes count alike: two runs on different streams do not overlap.
+ *     STORE      measurements, loop and detection slots, device counts: run, run_dev, run_dev_if, add_measurements_dev,
+ *                data_association_dev
+ *     OBSERVE    drone-pair matrix, observe window record, osb_observability record: observe_dev, observe_dev_if,
+ *                init_mask_dev, distance_factors_dev, init_by_loops_dev, data_association_dev
+ *     SYNC       sync window table, keyframe and full paths, prediction records, outcome: sync_dev, init_by_loops_dev,
+ *                data_association_dev
+ *     KEYFRAMES  keyframe ring and its frame table: add_keyframe_dev, distance_factors_dev
+ *     LOOPS      loop map, pair minima, overflow flag and init_by_loops' status: record_loops_dev, init_by_loops_dev
+ *     DA         data association result, the applied word included: data_association_dev, run_dev_if, observe_dev_if
+ *   The synchronising readers (observability, sync_result, paths, predict, keyframe_flags, init_by_loops_result,
+ *   loop_map, data_association_result) wait for the parts they read.  The updates (push_odometry, add_measurements,
+ *   set_window) alone write the trajectories, the window and init_mask's block table, and wait for every part first.
+ *   Work of another handle (the solver's last device call, the PCM state's last anchored call) is waited for where a call
+ *   below says so.
+ * Memory: create acquires a stream, six events, and the trajectories, measurements, window and run output at their
+ *   capacities.  The first call that needs the rest acquires it (each call below gives the sizes): the device counts
+ *   (add_measurements_dev, data_association_dev), the observe state (observe_dev, observe_dev_if), the block table
+ *   (init_mask_dev), the sync's window table, paths and records (sync_dev, init_by_loops_dev, data_association_dev),
+ *   predict's buffers (predict), the keyframe store (add_keyframe_dev, distance_factors_dev), the loop map
+ *   (record_loops_dev, init_by_loops_dev) and the data association result (set_data_association). */
 #define OSB_MEAS_LOOP 0
 #define OSB_MEAS_DET4D 1
 #define OSB_MEAS_DET6D 2
@@ -638,9 +660,8 @@ osb_status osb_anchor_run_dev(osb_anchor* h, const uint8_t* yaw_observable, osb_
  *   factor compaction pass over them) and returns the bound as *n_out.  Every synchronising call (run, size,
  *   add_measurements, push_odometry, set_window, status) first waits for the last device append, after which the counts are
  *   exact and run returns exactly n_loops + n_detections rows.  A handle that never calls add_measurements_dev behaves as
- *   if it did not exist.  The call can be captured into a CUDA graph (after an uncaptured first call): its waits for the
- *   handle's last run and append become external event waits, and its own event an external record, so the synchronising
- *   calls after a replay wait for the replayed append.
+ *   if it did not exist.  The call can be captured into a CUDA graph (after an uncaptured first call): its event waits
+ *   and records are external event nodes, so the synchronising calls after a replay wait for the replayed append.
  * osb_anchor_status(): waits for the last device append and writes its status to *last (OSB_OK when none ran); returns the
  *   same value. */
 #define OSB_ANCHOR_VOID 6
@@ -669,10 +690,9 @@ osb_status osb_anchor_status(osb_anchor* h, osb_status* last);
  *   boxes on the host, so a captured observe sees the window set before each replay.
  *   Three launches whatever n and the drone count (one pass over the rows sets a drone-pair bit matrix from status,
  *   edge.id_a and edge.id_b; one CTA runs the closure and steps 3-7; one pass rewrites skip).  The first call acquires the
- *   state, the bit matrix, the window record and an event, and synchronises; later calls acquire nothing and can be
- *   captured into a CUDA graph.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n < 0, self_id
- *   outside 0..max_drones-1.  Each observe waits for the handle's last observe on any stream; the updates (push_odometry,
- *   add_measurements, set_window) wait for it as they wait for the last run.
+ *   state, the bit matrix and the window record, and synchronises; later calls acquire nothing and can be captured into a
+ *   CUDA graph.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n < 0, self_id outside
+ *   0..max_drones-1.
  * osb_anchor_observability(): waits for the last observe and writes its outcome: per drone the node set, yaw, the sticky
  *   pos and enable and to_init (ids_to_init), 1 or 0 each; solve_master (enable_to_solve_master, sticky), motion (the self
  *   box test held) and motion_new (it found a node with !pos).  The caller's state machine keeps finish_init and
@@ -701,9 +721,8 @@ osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out);
  *   max_window_entries blocks, or the window's largest block id + 1 if more) and synchronises, and set_window keeps it
  *   current after that.  to_init is read on the device, so a captured call follows both the window set before each replay
  *   and that replay's observe.  (A set_window whose block ids outgrow the copy replaces it: capture again after it.)
- *   One launch on `stream`, ordered after the handle's last observe on any stream; the next observe and set_window are
- *   ordered after it.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n_nodes < 1, a window block
- *   outside 0 .. n_nodes-1, self_id outside 0..max_drones-1, or no observe_dev since create. */
+ *   One launch on `stream`.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, n_nodes < 1, a
+ *   window block outside 0 .. n_nodes-1, self_id outside 0..max_drones-1, or no observe_dev since create. */
 osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, int n_nodes, uint8_t* mask_dev, double* yaw_dev,
                                     void* stream);
 /* osb_anchor_sync_dev(): SwarmLocalizationSolver::sync_est_poses (swarm_localization_solver.cpp:962-1057) on the device,
@@ -740,11 +759,10 @@ osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, int n_nodes,
  *   max_drones x ceil(max_traj_samples / 10) writes the full paths).  The trajectory counts and the window are read on the
  *   device, so a captured sync follows push_odometry and set_window made between replays.
  *   Memory: the first call acquires 136 E + 4 (D + 1) bytes of window table and keyframe paths, 64 D S10 + 4 D bytes of
- *   full paths, 104 D bytes of records, about 1 KB of window counts and outcome, and an event (E = max_window_entries,
+ *   full paths, 104 D bytes of records and about 1 KB of window counts and outcome (E = max_window_entries,
  *   D = max_drones, S10 = ceil(max_traj_samples / 10); 6.5 MB for 5 drones, 2e5 samples and 2048 entries), and
  *   synchronises; set_window keeps the table current after that.
- *   Later calls acquire nothing and can be captured.  Each sync is ordered after the handle's last sync on any stream;
- *   push_odometry and set_window wait for it as they wait for the last run.
+ *   Later calls acquire nothing and can be captured.
  *   self_id is checked only: the sync does not depend on it (the reference's does not either). */
 typedef struct {
   int32_t self_id, full_path;
@@ -771,9 +789,8 @@ osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, int64_t* sta
  *   Nothing depends on the order of atomics: a 32-bit atomicMin on the row index picks each id's first row, a second
  *   launch writes the winners, and a pair's minimum is a 64-bit atomicMin.  An id of INT64_MAX is recorded but never a
  *   pair's minimum.  Two launches whatever n.  The first call acquires 96 (H + 1) + 8 D^2 bytes (H = the power of two
- *   >= 2 max_measurements, D = max_drones) and an event, and synchronises; a handle that never makes it holds none of
- *   this.  Later calls acquire nothing and can be captured.  Each call is ordered after the handle's last record_loops
- *   and init_by_loops on any stream.  The map holds at most H distinct ids (the rows of one handle have at most
+ *   >= 2 max_measurements, D = max_drones) and synchronises; a handle that never makes it holds none of this.  Later
+ *   calls acquire nothing and can be captured.  The map holds at most H distinct ids (the rows of one handle have at most
  *   max_measurements); past that the map is full and osb_anchor_init_by_loops_result reports OSB_ERR_CAPACITY.
  *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null handle or rows pointer with n > 0, n < 0.
  * osb_anchor_init_by_loops_dev(): SwarmLocalizationSolver::init_pose_by_loops (swarm_localization_solver.cpp:218-269),
@@ -807,8 +824,8 @@ osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, int64_t* sta
  *   One launch (one CTA: thread d decides drone d, then the threads stride over the window entries).  The first call
  *   acquires the loop map (as record_loops_dev) and the sync's paths (as sync_dev) if they are not there yet, and
  *   synchronises; later calls acquire nothing and can be captured, reading to_init, the PCM directory, the map, the paths
- *   and the trajectories on the device.  Ordered after the handle's last observe, sync and record_loops and the solver's
- *   last device call on any stream; the next of those, set_window and push_odometry are ordered after it.
+ *   and the trajectories on the device.  Ordered after the solver's last device call and the PCM state's last anchored
+ *   call on any stream.
  * osb_anchor_init_by_loops_result(): waits for the last init_by_loops -> *last (OSB_OK when none ran); returns OSB_OK.
  * osb_anchor_loop_map(): waits for the last record_loops and sync -> *n = the number of recorded ids, min(*n, cap)
  *   records ascending by id; pair_min [max_drones][max_drones] (or null): each ordered pair's smallest id, INT64_MAX for
@@ -860,9 +877,7 @@ osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, int cap, int
  *   calls than max_nodes.  Refused at once with nothing enqueued (OSB_ERR_INVALID): a null handle, self_id outside
  *   0..max_drones-1, no set_data_association or no observe_dev since create.  The first call acquires the device counts
  *   (as add_measurements_dev) and the sync's paths (as sync_dev) if they are not there yet, and synchronises; later calls
- *   acquire nothing and can be captured.  Ordered after the handle's last run, append, observe and sync on any stream;
- *   the next run_dev_if, append, update (push_odometry, add_measurements, set_window), observe and sync are ordered after
- *   it.  A run_dev on another stream is not: order it after the data association on the caller's side.
+ *   acquire nothing and can be captured.
  *   The branch, as solve() runs it: run_dev -> observe_dev -> record_loops_dev -> reject_anchored -> data_association_dev
  *   -> run_dev_if -> observe_dev_if -> record_loops_dev -> reject_anchored -> ...  (estimate_observability runs the loop
  *   map and PCM each time; when nothing was applied the second pair sees the same rows and changes nothing).
@@ -986,9 +1001,9 @@ osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int
  *      keyframe of the window set last, and a set_window with a frame (holding entries) whose keyframe has left the ring,
  *      are refused with OSB_ERR_CAPACITY: max_keyframes must cover the window.
  *   One launch.  The inputs go through a pinned staging ring of 4 slots: a call waits (on the host) only for the call 4
- *   before it.  Ordered after the solver's last device call and the handle's last keyframe, observe and
- *   distance_factors_dev, on any stream.  The solver's host mirror is stale afterwards: its next host-side call waits
- *   for this write and refreshes it, and its next device call starts from the written poses.
+ *   before it.  Ordered after the solver's last device call on any stream.  The solver's host mirror is stale afterwards:
+ *   its next host-side call waits for this write and refreshes it, and its next device call starts from the written
+ *   poses.
  *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, max_keyframes == 0, n_nodes outside
  *   1..max_drones, nodes not in ascending drone id, a drone or peer id outside 0..max_drones-1, peers not ascending, a
  *   block or a used prev_block outside 0 .. the solver's node count - 1, a stamp already stored, the handles on different
@@ -996,7 +1011,7 @@ osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int
  *   stream, waits for the write.  The first call acquires the store
  *   (max_keyframes x (16 + 156 max_drones + 17 max_keyframe_distances) bytes and a frame table of 20 max_window_entries
  *   bytes, sized once), the staging
- *   ring and events, and synchronises.
+ *   ring and its events, and synchronises.
  * osb_anchor_keyframe_flags(): waits for the last keyframe and copies the stored flags of the keyframe at stamp_ns, in
  *   `dists` order: *n = their count, -1 when the stamp is not stored; min(*n, cap) are written. */
 typedef struct {                 /* one NodeFrame of a keyframe, 152 bytes */
@@ -1038,8 +1053,7 @@ osb_status osb_anchor_keyframe_flags(osb_anchor* h, int64_t stamp_ns, int8_t* fl
  *   reference tree) is taken as "has a distance to b that is not flagged"; cutting_edges enables every distance
  *   (:1225-1297).  A count that would pass max_tail (the buffers' rows) writes -1 to *count_dev and no row past max_tail,
  *   so the solve refuses the tail; *count_dev < 0 on entry is left as it is.
- *   One launch of one CTA (a block scan per frame: deterministic, no atomics).  Ordered after the handle's last observe and
- *   keyframe on any stream; set_window and the next observe come after it.  Everything is read on the device, so the
+ *   One launch of one CTA (a block scan per frame: deterministic, no atomics).  Everything is read on the device, so the
  *   call can be captured into a CUDA graph: a replay's rows follow that replay's observe and the window set before it.
  *   Refused at once with nothing enqueued (OSB_ERR_INVALID): a null pointer, max_tail < 0, self_id outside
  *   0..max_drones-1, max_keyframes == 0, or no observe_dev since create.  The first call acquires what the first

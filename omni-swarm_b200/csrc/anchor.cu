@@ -107,7 +107,13 @@ __device__ __forceinline__ void store_pose(double* dst, const PoseD& p) {
   dst[0] = p.t[0]; dst[1] = p.t[1]; dst[2] = p.t[2]; dst[3] = p.q[0]; dst[4] = p.q[1]; dst[5] = p.q[2]; dst[6] = p.q[3];
 }
 
-__device__ __forceinline__ void anchor_rows(const AnchorView& v, osb_anchor_result* __restrict__ out) {
+// PRED (osb_anchor_run_dev_if): predicated on a device word, 0 writes nothing
+template <bool PRED>
+__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
+anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out, const int32_t* __restrict__ pred) {
+  if constexpr (PRED) {
+    if (*pred == 0) return;
+  }
   __shared__ double s_meas[ANCHOR_WARPS][MEAS_WORDS];
   __shared__ double s_out[ANCHOR_WARPS][RESULT_WORDS];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -212,18 +218,6 @@ __device__ __forceinline__ void anchor_rows(const AnchorView& v, osb_anchor_resu
   __syncwarp();
   double* dst = reinterpret_cast<double*>(out + i);
   for (int j = lane; j < RESULT_WORDS; j += 32) dst[j] = s_out[w][j];
-}
-
-__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
-anchor_kernel(const AnchorView v, osb_anchor_result* __restrict__ out) {
-  anchor_rows(v, out);
-}
-
-// the same, predicated on a device word (osb_anchor_run_dev_if): 0 writes nothing
-__global__ void __launch_bounds__(ANCHOR_WARPS * 32)
-anchor_if_kernel(const AnchorView v, osb_anchor_result* __restrict__ out, const int32_t* __restrict__ pred) {
-  if (*pred == 0) return;
-  anchor_rows(v, out);
 }
 
 // setup_problem_with_loops_and_detections on the device: the rows with skip == 0 (and keep[i]) become the solver's SoA in
@@ -391,8 +385,14 @@ struct ObserveWindow {
   int32_t n_frames, n_nodes;
 };
 
+// observe_dev's three launches; the PRED instantiations (observe_dev_if) are predicated on a device word, 0 writes nothing
+template <bool PRED>
 __global__ void __launch_bounds__(OBS_THREADS)
-observe_edges_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_drones, unsigned* __restrict__ adj) {
+observe_edges_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_drones, unsigned* __restrict__ adj,
+                     const int32_t* __restrict__ pred) {
+  if constexpr (PRED) {
+    if (*pred == 0) return;
+  }
   __shared__ unsigned s_adj[ANCHOR_MAX_DRONES * OBS_ROW32];
   volatile unsigned* vs = s_adj;
   for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS) s_adj[k] = 0;
@@ -411,10 +411,15 @@ observe_edges_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_
     if (s_adj[k]) atomicOr(adj + k, s_adj[k]);
 }
 
-// keep_new: motion_new |= the record's (the second observe of a solve, observe_dev_if)
-__device__ __forceinline__ void observe_state(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win,
-                                              int max_drones, int self_id, float xy_thres, float z_thres,
-                                              osb_observability* __restrict__ obs, bool keep_new) {
+// PRED keeps motion_new: motion_new |= the record's (the second observe of a solve)
+template <bool PRED>
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
+                     int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs,
+                     const int32_t* __restrict__ pred) {
+  if constexpr (PRED) {
+    if (*pred == 0) return;
+  }
   __shared__ unsigned long long s_adj[ANCHOR_MAX_DRONES][OBS_WORDS];
   __shared__ unsigned long long s_seen[OBS_WORDS], s_front[OBS_WORDS], s_next[OBS_WORDS];
   __shared__ int s_more;
@@ -476,18 +481,18 @@ __device__ __forceinline__ void observe_state(unsigned long long* __restrict__ a
     const bool single = win->n_frames > SINGLE_DRONE_SFS_THRES && win->n_nodes == 1;   // :1364-1367
     obs->solve_master = obs->solve_master || single || other || motion;
     obs->motion = motion;
-    obs->motion_new = motion_new || (keep_new && obs->motion_new);
+    obs->motion_new = motion_new || (PRED && obs->motion_new);
     obs->reserved = 0;
   }
 }
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_state_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
-                     int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs) {
-  observe_state(adj, win, max_drones, self_id, xy_thres, z_thres, obs, false);
-}
 
-__device__ __forceinline__ void observe_skip(osb_anchor_result* __restrict__ rows, int n, int max_drones,
-                                             const osb_observability* __restrict__ obs) {
+template <bool PRED>
+__global__ void __launch_bounds__(OBS_THREADS)
+observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones, const osb_observability* __restrict__ obs,
+                    const int32_t* __restrict__ pred) {
+  if constexpr (PRED) {
+    if (*pred == 0) return;
+  }
   const int i = blockIdx.x * OBS_THREADS + threadIdx.x;
   if (i >= n) return;
   bool use = rows[i].status == OSB_ANCHOR_OK;                      // anchor_kernel's rule (:1066-1073) with this yaw
@@ -497,48 +502,6 @@ __device__ __forceinline__ void observe_skip(osb_anchor_result* __restrict__ row
           rows[i].node_a != rows[i].node_b;
   }
   rows[i].skip = use ? 0 : 1;
-}
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_skip_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones, const osb_observability* __restrict__ obs) {
-  observe_skip(rows, n, max_drones, obs);
-}
-
-// observe_dev_if: the three launches above, predicated on a device word (0 writes nothing)
-// a copy of observe_edges_kernel's body: sharing it through an inline function changes that kernel's register
-// allocation, and the unpredicated kernels keep their code
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_edges_if_kernel(const osb_anchor_result* __restrict__ rows, int n, int max_drones, unsigned* __restrict__ adj,
-                        const int32_t* __restrict__ pred) {
-  if (*pred == 0) return;
-  __shared__ unsigned s_adj[ANCHOR_MAX_DRONES * OBS_ROW32];
-  volatile unsigned* vs = s_adj;
-  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS) s_adj[k] = 0;
-  __syncthreads();
-  for (int i = blockIdx.x * OBS_THREADS + threadIdx.x; i < n; i += gridDim.x * OBS_THREADS) {
-    if (rows[i].status != OSB_ANCHOR_OK) continue;
-    const int a = rows[i].edge.id_a, b = rows[i].edge.id_b;
-    if ((unsigned)a >= (unsigned)max_drones || (unsigned)b >= (unsigned)max_drones) continue;
-    const int ab = a * OBS_ROW32 + (b >> 5), ba = b * OBS_ROW32 + (a >> 5);
-    const unsigned bit_b = 1u << (b & 31), bit_a = 1u << (a & 31);
-    if (!(vs[ab] & bit_b)) atomicOr(&s_adj[ab], bit_b);          // most rows repeat a pair already set
-    if (!(vs[ba] & bit_a)) atomicOr(&s_adj[ba], bit_a);
-  }
-  __syncthreads();
-  for (int k = threadIdx.x; k < max_drones * OBS_ROW32; k += OBS_THREADS)
-    if (s_adj[k]) atomicOr(adj + k, s_adj[k]);
-}
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_state_if_kernel(unsigned long long* __restrict__ adj, const ObserveWindow* __restrict__ win, int max_drones,
-                        int self_id, float xy_thres, float z_thres, osb_observability* __restrict__ obs,
-                        const int32_t* __restrict__ pred) {
-  if (*pred == 0) return;
-  observe_state(adj, win, max_drones, self_id, xy_thres, z_thres, obs, true);
-}
-__global__ void __launch_bounds__(OBS_THREADS)
-observe_skip_if_kernel(osb_anchor_result* __restrict__ rows, int n, int max_drones,
-                       const osb_observability* __restrict__ obs, const int32_t* __restrict__ pred) {
-  if (*pred == 0) return;
-  observe_skip(rows, n, max_drones, obs);
 }
 
 // random_init_pose's choice of blocks (swarm_localization_solver.cpp:204-216) from the last observe's to_init: thread b
@@ -1424,13 +1387,28 @@ static_assert(sizeof(osb_predict_result) == 128, "osb_predict_result layout");
 static_assert(sizeof(osb_loop_record) == 88, "osb_loop_record layout");
 static_assert(sizeof(osb_sync_params) == 24, "osb_sync_params layout");
 
+// The parts of a handle's device state, one bit each.  A device call waits for the last call that touched (read or wrote)
+// each part it touches, on any stream, and then becomes that part's last toucher: the touchers of a part form one chain,
+// so one event per part orders them.  The trajectories, the run's window and init_mask's block table are written only by
+// the synchronising updates (push_odometry, add_measurements, set_window), which wait for every part.
+enum AnchorPart : unsigned {
+  STORE = 1u << 0,        // measurements, loop and detection slots, device counts
+  OBSERVE = 1u << 1,      // drone-pair matrix, observe window record, osb_observability record
+  SYNC = 1u << 2,         // sync window table, keyframe and full paths, prediction records, outcome
+  KEYFRAMES = 1u << 3,    // keyframe ring and its frame table
+  LOOPS = 1u << 4,        // loop map, pair minima, meta words
+  DA = 1u << 5,           // data association result, the applied word included
+};
+constexpr int ANCHOR_PARTS = 6;
+constexpr unsigned ALL_PARTS = (1u << ANCHOR_PARTS) - 1;
+
 struct osb_anchor {
   Resources res;
   int device = 0;
   osb_anchor_params p{};
   int64_t begin_dt_ns = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t last_run = nullptr;     // recorded after every run: updates wait for it before they overwrite state
+  cudaEvent_t last[ANCHOR_PARTS] = {};   // [k]: recorded after the last call that touched part 1 << k, on its stream
   std::mutex mu;
   // device state
   osb_measurement* d_meas = nullptr;
@@ -1454,7 +1432,6 @@ struct osb_anchor {
   unsigned* d_adj = nullptr;                      // [max_drones][8] 32-bit words
   ObserveWindow* d_obs_win = nullptr;
   osb_observability* d_obs = nullptr;
-  cudaEvent_t last_observe = nullptr;             // recorded after every observe, on its stream
   ObserveWindow obs_win{};                        // the host's, kept by set_window whether or not observe ever ran
   // init_mask_dev: every window block's drone (-1: no entry) and its latest frame's self_pose quaternion, derived by
   // set_window on the host; the first init_mask_dev acquires the device copy (and its length), set_window keeps it current
@@ -1465,7 +1442,7 @@ struct osb_anchor {
   double* d_blk_q = nullptr;
   size_t blk_cap = 0;
   // sync_dev, acquired by the first one: the window table (set_window keeps it current after that), the paths, the
-  // prediction record, the outcome, and the event recorded after every sync; predict's query and result buffers
+  // prediction record and the outcome; predict's query and result buffers
   SyncWindow sync_win{};                          // the host's, kept by set_window whether or not a sync ever ran
   std::vector<int64_t> sw_stamp;
   std::vector<int32_t> sw_drone, sw_block;
@@ -1481,7 +1458,6 @@ struct osb_anchor {
   int64_t *d_kf_stamp = nullptr, *d_full_stamp = nullptr;
   double *d_kf_pose = nullptr, *d_full_pose = nullptr;
   int max_full = 0;                               // ceil(max_traj_samples / 10)
-  cudaEvent_t last_sync = nullptr;
   int32_t* d_pred_drone = nullptr;
   double* d_pred_vo = nullptr;
   osb_predict_result* d_pred_out = nullptr;
@@ -1496,7 +1472,6 @@ struct osb_anchor {
   std::vector<int32_t> st_count;                  // ... its distance count, -1: empty
   long long kf_seq = 0;                           // keyframes added
   int kf_last_slot = -1;
-  cudaEvent_t last_keyframe = nullptr;
   char* kf_stage[KF_STAGING] = {};                // pinned, mapped: nodes [max_drones] then dists [max_dists]
   char* kf_stage_dev[KF_STAGING] = {};
   cudaEvent_t kf_stage_ev[KF_STAGING] = {};
@@ -1506,18 +1481,16 @@ struct osb_anchor {
   int32_t *d_kw_first = nullptr, *d_kw_drone = nullptr, *d_kw_block = nullptr, *d_kw_n = nullptr;
   int64_t kf_evicted = INT64_MIN;                 // the largest stamp whose slot a later keyframe took
   // the loop map (record_loops_dev, init_by_loops_dev), acquired by the first of them: H + 1 records, the pair minima,
-  // the overflow flag and init_by_loops' status, and the event recorded after every call that reads or writes them
+  // the overflow flag and init_by_loops' status
   LoopRec* d_lm = nullptr;
   unsigned long long* d_lm_pair = nullptr;
   int32_t* d_lm_meta = nullptr;
   int lm_H = 0;
-  cudaEvent_t last_loops = nullptr;
   // data association (set_data_association, data_association_dev): 0 until the setter, and then >= max_drones >= 1;
   // 0 makes no id_b anonymous
   int32_t da_anon_min = 0;
   osb_da_params da{};
   DaResult* d_da = nullptr;                       // acquired by the setter
-  cudaEvent_t last_da = nullptr;
   // host record
   int n_loops = 0, n_dets = 0;
   std::vector<int32_t> traj_n;
@@ -1533,11 +1506,18 @@ struct osb_anchor {
 
 namespace {
 
-osb_status anchor_wait_last_run(osb_anchor* h) {
-  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_run, 0));
-  if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
-  if (h->last_sync) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_sync, 0));
-  if (h->last_keyframe) OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_keyframe, 0));
+// orders `st` after the last toucher of each part in `parts` (an external wait inside a capture)
+osb_status anchor_wait(osb_anchor* h, unsigned parts, cudaStream_t st) {
+  for (int k = 0; k < ANCHOR_PARTS; ++k)
+    if (parts & (1u << k)) OSB_CUDA(wait_event_capturable(st, h->last[k]));
+  return OSB_OK;
+}
+
+// makes the work enqueued on `st` so far the last toucher of each part in `parts` (an external record inside a capture,
+// so the calls after a replay wait for the replayed work)
+osb_status anchor_record(osb_anchor* h, unsigned parts, cudaStream_t st) {
+  for (int k = 0; k < ANCHOR_PARTS; ++k)
+    if (parts & (1u << k)) OSB_CUDA(record_event_capturable(h->last[k], st));
   return OSB_OK;
 }
 
@@ -1639,8 +1619,8 @@ osb_status anchor_settle(osb_anchor* h) {
 }
 
 // the block table to the device: acquired at max_window_entries blocks (or the window's, if more), replaced by a larger one
-// only when the window's block ids outgrow it.  The handle's stream is idle: the callers have waited for the last run and
-// observe and synchronised.
+// only when the window's block ids outgrow it.  The handle's stream is idle: the callers have waited for every part and
+// synchronised.
 osb_status upload_blocks(osb_anchor* h) {
   const size_t n_blk = h->blk_drone.size();
   if (!h->d_blk_drone || n_blk > h->blk_cap) {
@@ -1683,7 +1663,7 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
                E = (size_t)p->max_window_entries;
   Resources& R = h->res;
   OSB_TRY(R.stream(&h->stream));
-  OSB_TRY(R.event(&h->last_run, cudaEventDisableTiming));
+  for (cudaEvent_t& e : h->last) OSB_TRY(R.event(&e, cudaEventDisableTiming));
   OSB_TRY(R.alloc(&h->d_meas, M));
   OSB_TRY(R.alloc(&h->d_loop_slot, M));
   OSB_TRY(R.alloc(&h->d_det_slot, M));
@@ -1699,7 +1679,7 @@ extern "C" osb_status osb_anchor_create(osb_anchor** out, const osb_anchor_param
   OSB_TRY(R.alloc(&h->d_out, M));
   OSB_CUDA(cudaMemsetAsync(h->d_traj_n, 0, D * sizeof(int32_t), h->stream));
   OSB_CUDA(cudaMemsetAsync(h->d_drone_first, 0, (D + 1) * sizeof(int32_t), h->stream));
-  OSB_CUDA(cudaEventRecord(h->last_run, h->stream));
+  OSB_TRY(anchor_record(h.get(), ALL_PARTS, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   h->traj_n.assign(D, 0);
   h->last_stamp.assign(D, 0);
@@ -1756,7 +1736,7 @@ extern "C" osb_status osb_anchor_push_odometry(osb_anchor* h, int32_t drone, int
   }
   const size_t base = (size_t)drone * h->p.max_traj_samples + have;
   const int32_t new_n = have + n;
-  OSB_TRY(anchor_wait_last_run(h));
+  OSB_TRY(anchor_wait(h, ALL_PARTS, h->stream));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemcpyAsync(h->d_traj_stamp + base, stamps_ns, (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_traj_pose + base * 7, poses, (size_t)n * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -1795,7 +1775,7 @@ extern "C" osb_status osb_anchor_add_measurements(osb_anchor* h, int n, const os
   const int new_loops = (int)slot.size();
   for (int i = 0; i < n; ++i)
     if (m[i].type != OSB_MEAS_LOOP) slot.push_back(have + i);
-  OSB_TRY(anchor_wait_last_run(h));
+  OSB_TRY(anchor_wait(h, ALL_PARTS, h->stream));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemcpyAsync(h->d_meas + have, m, (size_t)n * sizeof(osb_measurement), cudaMemcpyHostToDevice, st));
   if (new_loops > 0)
@@ -1888,7 +1868,7 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
     h->blk_drone[b] = entries[e].drone_id;
     std::copy(entries[e].self_pose + 3, entries[e].self_pose + 7, h->blk_q.begin() + 4 * (size_t)b);
   }
-  OSB_TRY(anchor_wait_last_run(h));
+  OSB_TRY(anchor_wait(h, ALL_PARTS, h->stream));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemcpyAsync(h->d_drone_first, first.data(), (size_t)(D + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   if (h->d_obs_win)
@@ -1918,7 +1898,7 @@ extern "C" osb_status osb_anchor_set_window(osb_anchor* h, int n_frames, const i
 
 namespace {
 
-// pred: null for run / run_dev, the device word of run_dev_if
+// pred: null for run / run_dev, the device word of run_dev_if, which also touches DA
 osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_anchor_result* out_dev, int32_t* n_out,
                          cudaStream_t st, const int32_t* pred = nullptr) {
   AnchorView v{};
@@ -1952,17 +1932,17 @@ osb_status anchor_launch(osb_anchor* h, const uint8_t* yaw_observable, osb_ancho
   if (h->fb.pending) {                          // the counts are the device's; the grid covers the host's bound of them
     long long n[2], since;                      // lowered by what the last append that has RUN reported
     if (h->fb.read(n, &since)) h->upper = std::min(h->upper, n[0] + n[1] + since);
-    OSB_CUDA(wait_event_capturable(st, h->fb.ev));                // captured after a captured append: an external wait
     v.counts = h->d_counts;
     v.n_bound = (int)h->upper;
   }
   *n_out = v.n_bound;
   if (v.n_bound == 0) return OSB_OK;
-  if (pred) OSB_LAUNCH(anchor_if_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev, pred);
-  else OSB_LAUNCH(anchor_kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev);
+  const unsigned parts = pred ? STORE | DA : STORE;
+  const auto kernel = pred ? anchor_kernel<true> : anchor_kernel<false>;
+  OSB_TRY(anchor_wait(h, parts, st));
+  OSB_LAUNCH(kernel, cdiv(v.n_bound, ANCHOR_WARPS), ANCHOR_WARPS * 32, 0, st, v, out_dev, pred);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_run, st));             // captured: the updates after a replay wait for it
-  return OSB_OK;
+  return anchor_record(h, parts, st);
 }
 
 }  // namespace
@@ -1981,9 +1961,7 @@ extern "C" osb_status osb_anchor_run_dev_if(osb_anchor* h, const uint8_t* yaw_ob
               "null argument");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (h->last_da) OSB_CUDA(wait_event_capturable(st, h->last_da));   // the word of the handle's own data association
-  return anchor_launch(h, yaw_observable, out_dev, n_out, st, pred_dev);
+  return anchor_launch(h, yaw_observable, out_dev, n_out, (cudaStream_t)stream, pred_dev);
 }
 
 extern "C" osb_status osb_anchor_compact_factors_dev(const osb_anchor_result* rows_dev, int n, const uint8_t* keep_dev,
@@ -2034,10 +2012,8 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
   DeviceGuard dg(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   OSB_TRY(anchor_dev_init(h));
-  // the append rewrites the counts a run reads and follows the previous append, whichever streams those ran on
-  OSB_CUDA(wait_event_capturable(st, h->last_run));
+  OSB_TRY(anchor_wait(h, STORE, st));
   if (h->fb.pending) {
-    OSB_CUDA(wait_event_capturable(st, h->fb.ev));
     long long n[2], since;
     if (h->fb.read(n, &since)) h->upper = std::min(h->upper, n[0] + n[1] + since);
   } else {
@@ -2048,6 +2024,7 @@ extern "C" osb_status osb_anchor_add_measurements_dev(osb_anchor* h, const osb_m
              h->p.max_drones, h->da_anon_min, h->p.max_measurements, h->d_meas, h->d_loop_slot, h->d_det_slot, h->d_counts, h->fb.dev, seq,
              h->fb.charged);
   OSB_CHECK_LAUNCH();
+  OSB_TRY(anchor_record(h, STORE, st));
   OSB_CUDA(h->fb.record(st));
   h->upper = std::min<long long>(h->upper + max_n, h->p.max_measurements);
   return OSB_OK;
@@ -2064,13 +2041,12 @@ extern "C" osb_status osb_anchor_status(osb_anchor* h, osb_status* last) {
 
 namespace {
 
-// the first observe acquires the matrix (zeroed), the window record (the host's), the state (zeroed) and the event
+// the first observe acquires the matrix (zeroed), the window record (the host's) and the state (zeroed)
 osb_status observe_init(osb_anchor* h) {
   if (h->d_obs) return OSB_OK;
   const size_t D = (size_t)h->p.max_drones;
   OSB_TRY(h->res.alloc(&h->d_adj, D * OBS_ROW32));
   OSB_TRY(h->res.alloc(&h->d_obs_win, 1));
-  OSB_TRY(h->res.event(&h->last_observe, cudaEventDisableTiming));
   osb_observability* obs = nullptr;
   OSB_TRY(h->res.alloc(&obs, 1));
   OSB_CUDA(cudaMemsetAsync(h->d_adj, 0, D * OBS_ROW32 * sizeof(unsigned), h->stream));
@@ -2079,6 +2055,27 @@ osb_status observe_init(osb_anchor* h) {
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   h->d_obs = obs;                                                  // set last: a failed first call is tried again
   return OSB_OK;
+}
+
+// pred: null for observe_dev, the device word of observe_dev_if, which also touches DA
+osb_status observe_launch(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev, int n, cudaStream_t st,
+                          const int32_t* pred = nullptr) {
+  OSB_TRY(observe_init(h));
+  const int D = h->p.max_drones;
+  const int blocks = cdiv(std::max(n, 1), OBS_THREADS);
+  const unsigned parts = pred ? OBSERVE | DA : OBSERVE;
+  const auto edges = pred ? observe_edges_kernel<true> : observe_edges_kernel<false>;
+  const auto state = pred ? observe_state_kernel<true> : observe_state_kernel<false>;
+  const auto skip = pred ? observe_skip_kernel<true> : observe_skip_kernel<false>;
+  OSB_TRY(anchor_wait(h, parts, st));
+  OSB_LAUNCH(edges, std::min(blocks, 4 * num_sms()), OBS_THREADS, 0, st, rows_dev, n, D, h->d_adj, pred);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(state, 1, OBS_THREADS, 0, st, reinterpret_cast<unsigned long long*>(h->d_adj), h->d_obs_win, D, p->self_id,
+             p->init_xy_movement, p->init_z_movement, h->d_obs, pred);
+  OSB_CHECK_LAUNCH();
+  OSB_LAUNCH(skip, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs, pred);
+  OSB_CHECK_LAUNCH();
+  return anchor_record(h, parts, st);
 }
 
 }  // namespace
@@ -2090,20 +2087,7 @@ extern "C" osb_status osb_anchor_observe_dev(osb_anchor* h, const osb_observe_pa
   OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  OSB_TRY(observe_init(h));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = h->p.max_drones;
-  const int blocks = cdiv(std::max(n, 1), OBS_THREADS);
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // the state and the matrix are the last observe's
-  OSB_LAUNCH(observe_edges_kernel, std::min(blocks, 4 * num_sms()), OBS_THREADS, 0, st, rows_dev, n, D, h->d_adj);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(observe_state_kernel, 1, OBS_THREADS, 0, st, reinterpret_cast<unsigned long long*>(h->d_adj), h->d_obs_win, D,
-             p->self_id, p->init_xy_movement, p->init_z_movement, h->d_obs);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(observe_skip_kernel, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs);
-  OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_observe, st));
-  return OSB_OK;
+  return observe_launch(h, p, rows_dev, n, (cudaStream_t)stream);
 }
 
 extern "C" osb_status osb_anchor_observe_dev_if(osb_anchor* h, const osb_observe_params* p, osb_anchor_result* rows_dev,
@@ -2113,22 +2097,7 @@ extern "C" osb_status osb_anchor_observe_dev_if(osb_anchor* h, const osb_observe
   OSB_REQUIRE(drone_ok(h, p->self_id), "self_id outside 0..max_drones-1");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  OSB_TRY(observe_init(h));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = h->p.max_drones;
-  const int blocks = cdiv(std::max(n, 1), OBS_THREADS);
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));
-  if (h->last_da) OSB_CUDA(wait_event_capturable(st, h->last_da));
-  OSB_LAUNCH(observe_edges_if_kernel, std::min(blocks, 4 * num_sms()), OBS_THREADS, 0, st, rows_dev, n, D, h->d_adj,
-             pred_dev);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(observe_state_if_kernel, 1, OBS_THREADS, 0, st, reinterpret_cast<unsigned long long*>(h->d_adj),
-             h->d_obs_win, D, p->self_id, p->init_xy_movement, p->init_z_movement, h->d_obs, pred_dev);
-  OSB_CHECK_LAUNCH();
-  OSB_LAUNCH(observe_skip_if_kernel, blocks, OBS_THREADS, 0, st, rows_dev, n, D, h->d_obs, pred_dev);
-  OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_observe, st));
-  return OSB_OK;
+  return observe_launch(h, p, rows_dev, n, (cudaStream_t)stream, pred_dev);
 }
 
 extern "C" osb_status osb_anchor_observability(osb_anchor* h, osb_observability* out) {
@@ -2139,7 +2108,7 @@ extern "C" osb_status osb_anchor_observability(osb_anchor* h, osb_observability*
     return OSB_OK;
   }
   DeviceGuard dg(h->device);
-  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_observe, 0));
+  OSB_TRY(anchor_wait(h, OBSERVE, h->stream));
   OSB_CUDA(cudaMemcpyAsync(out, h->d_obs, sizeof(*out), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   return OSB_OK;
@@ -2155,22 +2124,21 @@ extern "C" osb_status osb_anchor_init_mask_dev(osb_anchor* h, int32_t self_id, i
   OSB_REQUIRE(!h->blk_negative && h->blk_drone.size() <= (size_t)n_nodes, "a window block outside 0..n_nodes-1");
   DeviceGuard dg(h->device);
   if (!h->d_blk_drone) {                                          // the first call acquires the table
-    OSB_TRY(anchor_wait_last_run(h));
+    OSB_TRY(anchor_wait(h, ALL_PARTS, h->stream));
     OSB_TRY(upload_blocks(h));
   }
   cudaStream_t st = (cudaStream_t)stream;
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // to_init is the last observe's
+  OSB_TRY(anchor_wait(h, OBSERVE, st));
   OSB_LAUNCH(init_mask_kernel, cdiv(n_nodes, 256), 256, 0, st, h->d_blk_drone, h->d_blk_q, h->d_blk_drone + h->blk_cap,
              n_nodes, self_id, h->d_obs, mask_dev, yaw_dev);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
-  return OSB_OK;
+  return anchor_record(h, OBSERVE, st);
 }
 
 namespace {
 
-// the first sync acquires the window table (the host's), the paths (no drone has one), the records (none valid), the
-// outcome (nothing applied) and the event
+// the first sync acquires the window table (the host's), the paths (no drone has one), the records (none valid) and the
+// outcome (nothing applied)
 osb_status sync_init(osb_anchor* h) {
   if (h->d_outcome) return OSB_OK;
   const size_t D = (size_t)h->p.max_drones, E = (size_t)h->p.max_window_entries;
@@ -2189,7 +2157,6 @@ osb_status sync_init(osb_anchor* h) {
   OSB_TRY(R.alloc(&h->d_full_stamp, F));
   OSB_TRY(R.alloc(&h->d_full_pose, F * 7));
   OSB_TRY(R.alloc(&h->d_rec, D));
-  OSB_TRY(R.event(&h->last_sync, cudaEventDisableTiming));
   SyncOutcome* outcome = nullptr;
   OSB_TRY(R.alloc(&outcome, 1));
   cudaStream_t st = h->stream;
@@ -2232,7 +2199,7 @@ extern "C" osb_status osb_anchor_sync_dev(osb_anchor* h, osb_solver* s, const os
   v.kf_first = h->d_kf_first; v.kf_stamp = h->d_kf_stamp; v.kf_pose = h->d_kf_pose;
   v.full_n = h->d_full_n; v.full_stamp = h->d_full_stamp; v.full_pose = h->d_full_pose;
   OSB_CUDA(wait_event_capturable(st, c.done));                    // the solved poses and the call's outcome
-  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the record and the paths are the last sync's
+  OSB_TRY(anchor_wait(h, SYNC, st));
   OSB_LAUNCH(sync_gate_kernel, 1, SYNC_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(sync_kf_kernel, cdiv(v.max_entries, 256), 256, 0, st, v);
@@ -2240,8 +2207,7 @@ extern "C" osb_status osb_anchor_sync_dev(osb_anchor* h, osb_solver* s, const os
   const long long work = (long long)v.max_drones * v.max_full;
   OSB_LAUNCH(sync_full_kernel, (int)std::min<long long>(cdiv64(work, 256), 8LL * num_sms()), 256, 0, st, v);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_sync, st));
-  return OSB_OK;
+  return anchor_record(h, SYNC, st);
 }
 
 extern "C" osb_status osb_anchor_sync_result(osb_anchor* h, int32_t* applied, osb_status* last) {
@@ -2252,7 +2218,7 @@ extern "C" osb_status osb_anchor_sync_result(osb_anchor* h, int32_t* applied, os
   if (!h->d_outcome) return OSB_OK;
   DeviceGuard dg(h->device);
   SyncOutcome o;
-  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_sync, 0));
+  OSB_TRY(anchor_wait(h, SYNC, h->stream));
   OSB_CUDA(cudaMemcpyAsync(&o, h->d_outcome, sizeof(o), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   *applied = o.applied;
@@ -2269,7 +2235,7 @@ extern "C" osb_status osb_anchor_paths(osb_anchor* h, int full, int32_t drone, i
   if (!h->d_outcome) return OSB_OK;
   DeviceGuard dg(h->device);
   cudaStream_t st = h->stream;
-  OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
+  OSB_TRY(anchor_wait(h, SYNC, st));
   int32_t cnt[2];
   const int64_t* src_stamp;
   const double* src_pose;
@@ -2314,8 +2280,7 @@ extern "C" osb_status osb_anchor_predict(osb_anchor* h, const osb_predict_params
     OSB_TRY(h->res.alloc(&h->d_pred_out, D));
   }
   cudaStream_t st = h->stream;
-  OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
-  if (h->last_observe) OSB_CUDA(cudaStreamWaitEvent(st, h->last_observe, 0));
+  OSB_TRY(anchor_wait(h, SYNC | OBSERVE, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_pred_drone, drones, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   OSB_CUDA(cudaMemcpyAsync(h->d_pred_vo, vo_poses7, (size_t)n * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
   OSB_LAUNCH(predict_kernel, cdiv(n, 128), 128, 0, st, n, h->d_pred_drone, h->d_pred_vo, h->d_rec, h->d_obs, p->self_id,
@@ -2329,7 +2294,7 @@ extern "C" osb_status osb_anchor_predict(osb_anchor* h, const osb_predict_params
 namespace {
 
 // the first keyframe or distance_factors_dev call acquires the store (every slot empty), the window's frame table (the
-// host's), the staging ring and the events
+// host's) and the staging ring with its events
 osb_status kf_init(osb_anchor* h) {
   if (h->d_kw_n) return OSB_OK;
   const size_t K = (size_t)h->p.max_keyframes, D = (size_t)h->p.max_drones, M = (size_t)h->p.max_keyframe_distances;
@@ -2345,7 +2310,6 @@ osb_status kf_init(osb_anchor* h) {
   OSB_TRY(R.alloc(&h->d_kw_stamp, E));
   OSB_TRY(R.alloc(&h->d_kw_first, E + 1));
   OSB_TRY(R.alloc(&h->d_kw_block, E));
-  OSB_TRY(R.event(&h->last_keyframe, cudaEventDisableTiming));
   const size_t stage = D * sizeof(osb_keyframe_node) + M * sizeof(osb_keyframe_distance);
   for (int k = 0; k < KF_STAGING; ++k) {
     OSB_TRY(R.host_alloc(&h->kf_stage[k], stage, cudaHostAllocMapped));
@@ -2360,7 +2324,6 @@ osb_status kf_init(osb_anchor* h) {
   const osb_status s = upload_kf_window(h);
   if (s != OSB_OK) { h->d_kw_n = nullptr; return s; }
   for (int k = 0; k < KF_STAGING; ++k) OSB_CUDA(cudaEventRecord(h->kf_stage_ev[k], st));
-  OSB_CUDA(cudaEventRecord(h->last_keyframe, st));
   cudaError_t e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) { h->d_kw_n = nullptr; OSB_CUDA(e); }      // a failed first call is tried again
   h->st_stamp.assign(K, 0);
@@ -2443,13 +2406,12 @@ extern "C" osb_status osb_anchor_add_keyframe_dev(osb_anchor* h, osb_solver* s, 
   v.slot = slot; v.prev_slot = h->kf_last_slot;
   v.st_stamp = h->d_st_stamp; v.st_n = h->d_st_n; v.st_node = h->d_st_node; v.st_first = h->d_st_first;
   v.st_dist = h->d_st_dist; v.st_flag = h->d_st_flag;
-  OSB_CUDA(wait_event_capturable(st, h->last_keyframe));          // the store is the last keyframe's ...
-  if (h->last_observe) OSB_CUDA(wait_event_capturable(st, h->last_observe));   // ... and distance_factors_dev reads it
+  OSB_TRY(anchor_wait(h, KEYFRAMES, st));
   OSB_LAUNCH(keyframe_kernel, 1, KF_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(w.written, st));
   OSB_CUDA(record_event_capturable(h->kf_stage_ev[stage], st));
-  OSB_CUDA(record_event_capturable(h->last_keyframe, st));
+  OSB_TRY(anchor_record(h, KEYFRAMES, st));
   if (h->st_count[slot] >= 0) h->kf_evicted = std::max(h->kf_evicted, h->st_stamp[slot]);
   h->st_stamp[slot] = stamp_ns;
   h->st_count[slot] = n_distances;
@@ -2472,7 +2434,7 @@ extern "C" osb_status osb_anchor_keyframe_flags(osb_anchor* h, int64_t stamp_ns,
   if (m == 0) return OSB_OK;
   DeviceGuard dg(h->device);
   cudaStream_t st = h->stream;
-  OSB_CUDA(cudaStreamWaitEvent(st, h->last_keyframe, 0));
+  OSB_TRY(anchor_wait(h, KEYFRAMES, st));
   OSB_CUDA(cudaMemcpyAsync(flags, h->d_st_flag + (size_t)slot * h->p.max_keyframe_distances, (size_t)m,
                            cudaMemcpyDeviceToHost, st));
   OSB_CUDA(cudaStreamSynchronize(st));
@@ -2501,17 +2463,15 @@ extern "C" osb_status osb_anchor_distance_factors_dev(osb_anchor* h, const osb_d
   v.sqrt_inf = 1.0 / sqrt((double)p->distance_measurement_cov);
   v.type = type; v.ia = ia; v.ib = ib; v.payload = payload; v.hub = huber; v.count = count_dev; v.max_tail = max_tail;
   cudaStream_t st = (cudaStream_t)stream;
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // enable is the last observe's
-  OSB_CUDA(wait_event_capturable(st, h->last_keyframe));          // the store is the last keyframe's
+  OSB_TRY(anchor_wait(h, OBSERVE | KEYFRAMES, st));
   OSB_LAUNCH(distance_factors_kernel, 1, DF_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_observe, st));         // set_window and the next observe come after it
-  return OSB_OK;
+  return anchor_record(h, OBSERVE | KEYFRAMES, st);
 }
 
 namespace {
 
-// the first record_loops_dev or init_by_loops_dev acquires the map (no id recorded, no pair, no overflow) and its event
+// the first record_loops_dev or init_by_loops_dev acquires the map (no id recorded, no pair, no overflow)
 osb_status loops_init(osb_anchor* h) {
   if (h->d_lm_meta) return OSB_OK;
   int H = 1;
@@ -2520,14 +2480,12 @@ osb_status loops_init(osb_anchor* h) {
   Resources& R = h->res;
   OSB_TRY(R.alloc(&h->d_lm, (size_t)H + 1));
   OSB_TRY(R.alloc(&h->d_lm_pair, D * D));
-  OSB_TRY(R.event(&h->last_loops, cudaEventDisableTiming));
   int32_t* meta = nullptr;
   OSB_TRY(R.alloc(&meta, 2));
   cudaStream_t st = h->stream;
   OSB_CUDA(cudaMemsetAsync(h->d_lm, 0xff, ((size_t)H + 1) * sizeof(LoopRec), st));   // key -1, claim none, not recorded
   OSB_CUDA(cudaMemsetAsync(h->d_lm_pair, 0xff, D * D * sizeof(unsigned long long), st));
   OSB_CUDA(cudaMemsetAsync(meta, 0, 2 * sizeof(int32_t), st));
-  OSB_CUDA(cudaEventRecord(h->last_loops, st));
   OSB_CUDA(cudaStreamSynchronize(st));
   h->lm_H = H;
   h->d_lm_meta = meta;                                             // set last: a failed first call is tried again
@@ -2548,13 +2506,12 @@ extern "C" osb_status osb_anchor_record_loops_dev(osb_anchor* h, const osb_ancho
   cudaStream_t st = (cudaStream_t)stream;
   const LoopMapView v = loop_map_view(h);
   const int blocks = std::min(cdiv(std::max(n, 1), LM_THREADS), 4 * num_sms());
-  OSB_CUDA(wait_event_capturable(st, h->last_loops));             // the map is the last record's and init's
+  OSB_TRY(anchor_wait(h, LOOPS, st));
   OSB_LAUNCH(record_claim_kernel, blocks, LM_THREADS, 0, st, rows_dev, n, v);
   OSB_CHECK_LAUNCH();
   OSB_LAUNCH(record_write_kernel, blocks, LM_THREADS, 0, st, rows_dev, n, v);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_loops, st));
-  return OSB_OK;
+  return anchor_record(h, LOOPS, st);
 }
 
 extern "C" osb_status osb_anchor_init_by_loops_dev(osb_anchor* h, osb_pcm_state* pcm, osb_solver* s, int32_t self_id,
@@ -2587,16 +2544,11 @@ extern "C" osb_status osb_anchor_init_by_loops_dev(osb_anchor* h, osb_pcm_state*
   v.max_samples = h->p.max_traj_samples; v.max_drones = h->p.max_drones; v.self_id = self_id;
   v.poses = w.poses;
   if (pd.done) OSB_CUDA(wait_event_capturable(st, pd.done));     // the inlier sets of the last anchored PCM call
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // to_init
-  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the paths and the estimated flags
-  OSB_CUDA(wait_event_capturable(st, h->last_loops));             // the map
+  OSB_TRY(anchor_wait(h, OBSERVE | SYNC | LOOPS, st));
   OSB_LAUNCH(init_by_loops_kernel, 1, IBL_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
   OSB_CUDA(record_event_capturable(w.written, st));
-  OSB_CUDA(record_event_capturable(h->last_observe, st));         // the next observe, sync and record come after it
-  OSB_CUDA(record_event_capturable(h->last_sync, st));
-  OSB_CUDA(record_event_capturable(h->last_loops, st));
-  return OSB_OK;
+  return anchor_record(h, OBSERVE | SYNC | LOOPS, st);
 }
 
 extern "C" osb_status osb_anchor_init_by_loops_result(osb_anchor* h, osb_status* last) {
@@ -2606,7 +2558,7 @@ extern "C" osb_status osb_anchor_init_by_loops_result(osb_anchor* h, osb_status*
   if (!h->d_lm_meta) return OSB_OK;
   DeviceGuard dg(h->device);
   int32_t st = 0;
-  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_loops, 0));
+  OSB_TRY(anchor_wait(h, LOOPS, h->stream));
   OSB_CUDA(cudaMemcpyAsync(&st, h->d_lm_meta + 1, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   *last = (osb_status)st;
@@ -2623,10 +2575,10 @@ extern "C" osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, i
   if (estimated) memset(estimated, 0, D);
   DeviceGuard dg(h->device);
   cudaStream_t st = h->stream;
+  OSB_TRY(anchor_wait(h, LOOPS | SYNC, st));
   if (h->d_lm_meta) {
     std::vector<LoopRec> tab((size_t)h->lm_H + 1);
     std::vector<unsigned long long> pair(D * D);
-    OSB_CUDA(cudaStreamWaitEvent(st, h->last_loops, 0));
     OSB_CUDA(cudaMemcpyAsync(tab.data(), h->d_lm, tab.size() * sizeof(LoopRec), cudaMemcpyDeviceToHost, st));
     OSB_CUDA(cudaMemcpyAsync(pair.data(), h->d_lm_pair, D * D * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     OSB_CUDA(cudaStreamSynchronize(st));
@@ -2642,7 +2594,6 @@ extern "C" osb_status osb_anchor_loop_map(osb_anchor* h, osb_loop_record* out, i
   }
   if (estimated && h->d_rec) {
     std::vector<SyncRecord> rec(D);
-    OSB_CUDA(cudaStreamWaitEvent(st, h->last_sync, 0));
     OSB_CUDA(cudaMemcpyAsync(rec.data(), h->d_rec, D * sizeof(SyncRecord), cudaMemcpyDeviceToHost, st));
     OSB_CUDA(cudaStreamSynchronize(st));
     for (size_t d = 0; d < D; ++d) estimated[d] = rec[d].estimated ? 1 : 0;
@@ -2657,12 +2608,10 @@ extern "C" osb_status osb_anchor_set_data_association(osb_anchor* h, const osb_d
   OSB_REQUIRE(!std::isnan(p->accept_thres), "accept_thres is NaN");
   std::lock_guard<std::mutex> lk(h->mu);
   DeviceGuard dg(h->device);
-  if (!h->d_da) {                                                  // the first call acquires the result and its event
-    OSB_TRY(h->res.event(&h->last_da, cudaEventDisableTiming));
+  if (!h->d_da) {                                                  // the first call acquires the result
     DaResult* r = nullptr;
     OSB_TRY(h->res.alloc(&r, 1));
     OSB_CUDA(cudaMemsetAsync(r, 0, sizeof(DaResult), h->stream));
-    OSB_CUDA(cudaEventRecord(h->last_da, h->stream));
     OSB_CUDA(cudaStreamSynchronize(h->stream));
     h->d_da = r;
   }
@@ -2692,18 +2641,10 @@ extern "C" osb_status osb_anchor_data_association_dev(osb_anchor* h, int32_t sel
   v.anon_min = h->da.anon_min; v.max_nodes = h->da.max_nodes;
   v.thres = (double)h->da.accept_thres;
   v.res = h->d_da;
-  OSB_CUDA(wait_event_capturable(st, h->last_run));               // the store: no run reads a row while it is renamed
-  if (h->fb.pending) OSB_CUDA(wait_event_capturable(st, h->fb.ev));   // ... and the device appends have written it
-  OSB_CUDA(wait_event_capturable(st, h->last_observe));           // the node set and enable
-  OSB_CUDA(wait_event_capturable(st, h->last_sync));              // the keyframe paths
-  OSB_CUDA(wait_event_capturable(st, h->last_da));
+  OSB_TRY(anchor_wait(h, STORE | OBSERVE | SYNC | DA, st));
   OSB_LAUNCH(data_association_kernel, 1, DA_THREADS, 0, st, v);
   OSB_CHECK_LAUNCH();
-  OSB_CUDA(record_event_capturable(h->last_run, st));             // the next run, append and update come after it
-  OSB_CUDA(record_event_capturable(h->last_observe, st));
-  OSB_CUDA(record_event_capturable(h->last_sync, st));
-  OSB_CUDA(record_event_capturable(h->last_da, st));
-  return OSB_OK;
+  return anchor_record(h, STORE | OBSERVE | SYNC | DA, st);
 }
 
 extern "C" osb_status osb_anchor_data_association_result(osb_anchor* h, int32_t* applied, osb_status* status,
@@ -2717,7 +2658,7 @@ extern "C" osb_status osb_anchor_data_association_result(osb_anchor* h, int32_t*
   if (!h->d_da) return OSB_OK;
   DeviceGuard dg(h->device);
   DaResult r{};
-  OSB_CUDA(cudaStreamWaitEvent(h->stream, h->last_da, 0));
+  OSB_TRY(anchor_wait(h, DA, h->stream));
   OSB_CUDA(cudaMemcpyAsync(&r, h->d_da, sizeof(r), cudaMemcpyDeviceToHost, h->stream));
   OSB_CUDA(cudaStreamSynchronize(h->stream));
   *applied = r.applied;
